@@ -1,19 +1,23 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json metric: concurrent audio streams x frames / second on N B200s.
+"""bench.py -- BASELINE.json metric: concurrent audio streams x frames / second on N H100s.
 
 A "step" is one pass of the hot path (frontend + MixedNet, `mww_predict_clip`) over one batch of
 synthetic 16 kHz int16 audio: 65 536 streams x 3 s (= 300 ten-ms frames, 100 model steps per stream)
 per GPU -- BASELINE.json configs[1].  Streams are independent, so N GPUs run N shards of 65 536
 streams each with no data-path collective (weak scaling; configs[4] = 8 x 65 536 = 524 288 streams).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--model f32|int8]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--model f32|int8] [--dump-outputs DIR]
 
 One JSON line on stdout (rank 0).  Keys beyond the driver contract:
-  roofline      dominant kernel (K1 spectral) achieved algorithmic GB/s vs MEASURED_PEAKS.json
+  roofline      dominant kernel (K1 spectral) achieved algorithmic GB/s vs MEASURED_PEAKS.json (else the H100 data sheet)
   kernels       per-kernel-class device ms/step from CUDA events recorded by the library on the launch stream
   cpu_baseline  the CPU oracle (the reference's own native dependencies are not installable: "port") on the
                 box's host cores, bounded sample
   e2e           same metric through mww_predict_clip_host with pinned HOST buffers (H2D + D2H inside the timed region)
+
+Every timed leg runs --steps steps (after its own warm-up calls); a live-mode step is 3 s of audio fed as 100 calls of 30 ms.
+--dump-outputs DIR writes what the timed path returned in its last timed step (the probabilities [streams, steps]) as
+DIR/probs.npy, float32; the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 
 from __future__ import annotations
@@ -37,6 +41,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 STREAMS_PER_GPU = 65536
 SAMPLES_PER_STEP = 48000          # 3 s -> 300 frames / stream / step
 FRAMES_PER_STEP = SAMPLES_PER_STEP // 160
+DUMP_BYTES = 64 << 20            # --dump-outputs budget: larger outputs keep a fixed, seeded sample of their rows
 K1_ALG_BYTES_PER_FRAME = 320      # 160 new int16 samples per 10 ms frame: the only mandatory HBM traffic of K1 (DESIGN.md)
 METRIC = "streams_x_frames_per_sec"
 UNIT = "frames/s"
@@ -63,6 +68,8 @@ def parse_args():
                     help="skip the legs for the other BASELINE.json configurations (the other model dtype in clip mode, live 30 ms steps "
                          "for both dtypes, feature extractor only)")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's outputs of its last timed step to DIR/<name>.npy (float32, at most 64 MB in all)")
     return ap.parse_args()
 
 
@@ -77,13 +84,26 @@ def config_dict(args, world):
                     % (args.streams, FRAMES_PER_STEP, "int8 (TFLite semantics)" if args.model == "int8" else "fp32"),
         "streams_per_gpu": args.streams, "streams_total": args.streams * world, "frames_per_stream_per_step": FRAMES_PER_STEP,
         "samples_per_stream_per_step": SAMPLES_PER_STEP, "parallelism": "independent stream shards x%d, no collective" % world,
-        "l2": "inputs %.1f GB per GPU per step >> 126 MB L2 (no flush needed)" % (args.streams * SAMPLES_PER_STEP * 2 / 1e9),
+        "l2": "inputs %.1f GB per GPU per step >> 50 MB L2 (no flush needed)" % (args.streams * SAMPLES_PER_STEP * 2 / 1e9),
         "weights": "synthetic okay_nabu seed 0 (tests/golden)",
     }
 
 
 # --------------------------------------------------------------------------------------------
 # CPU oracle legs
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """arrays (name -> float array, rows first) -> out_dir/<name>.npy as float32; an array over its share of DUMP_BYTES keeps the
+    rows of a fixed seeded sample, in order, so that two runs dump the same rows"""
+    os.makedirs(out_dir, exist_ok=True)
+    share = (DUMP_BYTES - 4096 * len(arrays)) // max(len(arrays), 1)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        if a.nbytes > share:
+            keep = max(share // max(a[0].nbytes, 1), 1)
+            a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
 
 def cpu_sample(n_streams: int) -> np.ndarray:
     from microwakeword_b200.synth_audio import synth_audio
@@ -249,29 +269,10 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not a measured peak)"
 
 
-def ncu_traffic():
-    """dram bytes per K1 launch from the committed ncu --set full capture summary, if present."""
-    p = os.path.join(ROOT, "profiles", "k1_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
-
-
-def issue_roofline(tipf, frames_per_launch, kernel_ms, clock_info):
-    sm_hz = ((clock_info or {}).get("sm_mhz") or 1965.0) * 1e6
-    peak_issue = 148 * 4 * 32 * sm_hz            # 4 schedulers/SM x 1 warp-instruction/clk x 32 threads
-    ach = tipf * frames_per_launch / (kernel_ms / 1e3)
-    return {"thread_instr_per_frame": tipf, "achieved_thread_instr_per_s": ach, "peak_thread_instr_per_s": peak_issue,
-            "frac": ach / peak_issue, "source": "instructions per frame from the committed ncu capture; duration live from CUDA events"}
-
-
-def k1_roofline(prof, S, steps, clock_info):
+def k1_roofline(prof, S, steps):
     """HBM roofline of the dominant kernel (the spectral frontend kernel) from the library's own CUDA events."""
     peak, peak_src = measured_peaks()
     k1_ms, k1_n = prof["k1_spectral"]
@@ -280,18 +281,11 @@ def k1_roofline(prof, S, steps, clock_info):
     frames_per_launch = S * FRAMES_PER_STEP * steps / k1_n
     per_launch_ms = k1_ms / k1_n
     achieved = K1_ALG_BYTES_PER_FRAME * frames_per_launch / (per_launch_ms / 1e3) / 1e9
-    tr = ncu_traffic()
-    roof = {"bound": "hbm", "kernel": (tr or {}).get("kernel", "k1_spectral_kernel"), "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "peak_source": peak_src, "traffic": ((tr or {}).get("dram_bytes_per_unit") or 0) * frames_per_launch or None,
-            "traffic_source": (tr or {}).get("source"),
-            "alg_bytes_per_frame": K1_ALG_BYTES_PER_FRAME, "frames_per_launch": frames_per_launch,
+    return {"bound": "hbm", "kernel": "k1_spectral_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+            "peak_source": peak_src, "alg_bytes_per_frame": K1_ALG_BYTES_PER_FRAME, "frames_per_launch": frames_per_launch,
             "share_of_step": k1_ms / max(sum(v[0] for v in prof.values()), 1e-9),
-            "note": "the frontend kernel is integer-ALU bound by construction (~30k thread-instructions per 320-byte frame, ncu): the HBM "
-                    "fraction is low because the kernel is instruction-issue bound; see `issue`, DESIGN.md and profiles/"}
-    tipf = (tr or {}).get("thread_instr_per_unit")
-    if tipf:
-        roof["issue"] = issue_roofline(tipf, frames_per_launch, per_launch_ms, clock_info)
-    return roof
+            "note": "the frontend kernel is integer-ALU bound by construction: the HBM fraction is low because the kernel is "
+                    "instruction-issue bound (DESIGN.md)"}
 
 
 def run_gpu(args):
@@ -354,8 +348,14 @@ def run_gpu(args):
     barrier()
     l0 = eng.launch_count
     eng.profile(True)
-    ms_resident = timed(lambda: eng.predict_clip(audio, out=probs), args.steps)
+    last = {}
+
+    def resident_step():
+        last["probs"] = eng.predict_clip(audio, out=probs)
+    ms_resident = timed(resident_step, args.steps)
     launches = (eng.launch_count - l0)
+    if args.dump_outputs and world == 1:
+        dump_outputs(args.dump_outputs, {"probs": last["probs"].cpu().numpy()})
     prof = eng.profile_read()
     eng.profile(False)
     checksum = float(probs[:, :100].double().sum().item())
@@ -389,8 +389,8 @@ def run_gpu(args):
         pull_only()
         pull_ms = timed(pull_only, 2)
         del stage
-        # the ingest rank's share of the streams: equal by default.  (Measured at N = 8, staged mode: equal shares 54.9 ms, the
-        # ingest rank feeding only 63.7 ms -- all 8 S streams then cross its NVLink instead of 7 S; DESIGN.md section 5.)
+        # the ingest rank's share of the streams: equal by default (a share of 0 sends all N S streams over the ingest rank's
+        # NVLink instead of (N - 1) S)
         src_share = 1.0 if args.ingest_share is None else float(args.ingest_share)
         why = "equal shares (default)" if args.ingest_share is None else "--ingest-share"
         egress_bound = pull_ms > ms_resident
@@ -413,6 +413,8 @@ def run_gpu(args):
             ingest_step()
         l0 = count_launches()
         ms_per_step = timed(ingest_step, args.steps)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"probs": gathered.cpu().numpy()})
         lt = torch.tensor([count_launches() - l0], dtype=torch.int64, device=device)
         dist.all_reduce(lt, op=dist.ReduceOp.MAX)
         launches = int(lt.item())                      # per rank (the ingest rank launches nothing when its share is 0)
@@ -508,7 +510,7 @@ def run_gpu(args):
 
     clock_info = clocks.stop() if clocks else None
     value = frames_per_step_all / (ms_per_step / 1e3)
-    roof = k1_roofline(prof, S, args.steps, clock_info)
+    roof = k1_roofline(prof, S, args.steps)
 
     # ---- e2e through the host-buffer C-ABI call (pinned buffers on this GPU's NUMA node) ----
     e2e = None
@@ -520,7 +522,7 @@ def run_gpu(args):
         eng.reset()
         for _ in range(2):
             eng.predict_clip_host(ha, out=hp)
-        e2e_steps = max(2, min(args.steps, 4))
+        e2e_steps = args.steps
         t0 = time.perf_counter()
         e2e_ms = timed(lambda: eng.predict_clip_host(ha, out=hp), e2e_steps)
         wall_ms = (time.perf_counter() - t0) * 1e3
@@ -533,15 +535,9 @@ def run_gpu(args):
         del ha, hp
 
     # ---- the other single-GPU configurations of BASELINE.json, each with its own roofline (rank-local, every rank runs them) ----
-    def live_traffic(kind, n_streams):
-        """DRAM bytes per launch of the fp32 live NN kernel, from the committed ncu --set full capture (per stream-step x streams)"""
-        path = os.path.join(ROOT, "profiles", "live_traffic.json")
-        if kind != "f32" or not os.path.exists(path):
-            return None
-        return json.load(open(path))["dram_bytes_per_unit"] * n_streams
-
     def live_leg(kind, n_live=480):
-        """live mode: step() calls with `n_live` new samples per stream; the ring state round-trips HBM on every call"""
+        """live mode: step() calls with `n_live` new samples per stream; the ring state round-trips HBM on every call.  A timed step
+        is the step's 3 s of audio fed as `calls` such calls"""
         le = eng if kind == args.model else StreamEngine(model_blob(kind), n_streams=S, device=local_rank)
         calls = max(SAMPLES_PER_STEP // n_live, 1)
         le.reset()
@@ -554,7 +550,8 @@ def run_gpu(args):
             le.predict_clip(chunks[state["i"] % len(chunks)], out=probs)
             state["i"] += 1
         le.profile(True)
-        live_ms = timed(one, calls)
+        n_calls = calls * args.steps
+        live_ms = timed(one, n_calls)
         lp = le.profile_read()
         le.profile(False)
         frames = S * world * (n_live // 160)
@@ -566,11 +563,11 @@ def run_gpu(args):
         peak, peak_src = measured_peaks()
         nn_gbs = S * step_bytes / (nn_ms / 1e3) / 1e9 if nn_ms else None
         out = {"workload": "configs[1]/[2] streams stepped live: %d calls of %d new samples (one model step) for %d streams, %s" % (calls, n_live, S, kind),
-               "samples_per_call": n_live, "calls": calls, "value": frames / (live_ms / 1e3), "unit": UNIT, "ms_per_call": live_ms,
-               "kernels_ms_per_call": {k: v[0] / calls for k, v in lp.items()},
+               "samples_per_call": n_live, "calls": calls, "steps": args.steps, "value": frames / (live_ms / 1e3), "unit": UNIT, "ms_per_call": live_ms,
+               "kernels_ms_per_call": {k: v[0] / n_calls for k, v in lp.items()},
                "roofline": {"bound": "hbm", "kernel": "nn_f32_live3_kernel" if kind == "f32" else "nn_i8_live_kernel", "achieved": nn_gbs, "peak": peak,
                             "unit": "GB/s", "frac": nn_gbs / peak if nn_gbs else None, "peak_source": peak_src,
-                            "alg_bytes_per_stream_step": step_bytes, "kernel_ms": nn_ms, "traffic": live_traffic(kind, S)},
+                            "alg_bytes_per_stream_step": step_bytes, "kernel_ms": nn_ms},
                "realtime_streams_capacity": S * world * (n_live / 16.0) / live_ms}
         if le is not eng:
             le.close()
@@ -581,13 +578,13 @@ def run_gpu(args):
         for _ in range(3):
             ce.predict_clip(audio, out=probs)
         ce.profile(True)
-        steps = max(3, min(args.steps, 5))
+        steps = args.steps
         ms = timed(lambda: ce.predict_clip(audio, out=probs), steps)
         cp = ce.profile_read()
         ce.profile(False)
         out = {"workload": "configs[2]: %d streams x %d frames per step, okay_nabu mixednet %s, clip mode" % (S, FRAMES_PER_STEP, kind),
                "dtype": kind, "value": S * FRAMES_PER_STEP * world / (ms / 1e3), "unit": UNIT, "ms_per_step": ms, "steps": steps,
-               "kernels": {k: {"ms_per_step": v[0] / steps} for k, v in cp.items()}, "roofline": k1_roofline(cp, S, steps, clock_info)}
+               "kernels": {k: {"ms_per_step": v[0] / steps} for k, v in cp.items()}, "roofline": k1_roofline(cp, S, steps)}
         ce.close()
         return out
 
@@ -595,7 +592,6 @@ def run_gpu(args):
         """BASELINE.json configs[3]: the feature extractor alone on 1 M 30 ms windows (streaming and stateless)"""
         feat = {}
         peak, peak_src = measured_peaks()
-        tr = ncu_traffic() or {}
         for name, fs, fn in (("streaming_4096x256", 4096, 160 * 256 + 320), ("stateless_1048576x480", 1 << 20, 480)):
             fe = StreamEngine(None, n_streams=fs, device=local_rank)
             fa = synth_audio_device(torch, fs, fn, 99 + rank, device)
@@ -607,15 +603,14 @@ def run_gpu(args):
                 fe.features(fa, out=fo)
             for _ in range(3):
                 one()
-            f_ms = timed(one, 10)
+            f_ms = timed(one, args.steps)
             windows = fs * n_fr * world
             alg = (fn * 2 + n_fr * 80) / n_fr
             gbs = fs * (fn * 2 + n_fr * 80) / (f_ms / 1e3) / 1e9
             feat[name] = {"windows": windows, "ms": f_ms, "windows_per_s": windows / (f_ms / 1e3), "alg_bytes_per_window": alg,
+                          "steps": args.steps,
                           "roofline": {"bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak, "peak_source": peak_src,
-                                       "traffic": None,
-                                       "issue": issue_roofline(tr["thread_instr_per_unit"], fs * n_fr, f_ms, clock_info) if tr.get("thread_instr_per_unit") else None,
-                                       "note": "integer-ALU bound like the clip frontend: the issue-slot fraction is the binding one"}}
+                                       "note": "integer-ALU bound like the clip frontend: the HBM fraction is low by construction"}}
             fe.close()
             del fa, fo
         return feat

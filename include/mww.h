@@ -1,6 +1,6 @@
 /*
  * include/mww.h -- C-ABI of libmww_b200.so: the drop-in boundary for microWakeWord's streaming
- * inference hot path on B200 (sm_100a).
+ * inference hot path on H100 (sm_90a).
  *
  * The reference crosses into native code at three places, all un-vendored third-party libraries
  * (SURVEY.md 2.1); each entry point below names the reference call site it replaces:
@@ -219,8 +219,8 @@ int mww_ipc_free(void *d_ptr, int device);
 /* Pinned host memory placed on the NUMA node the GPU hangs off (/sys/bus/pci/devices/<bdf>/numa_node): the calling
  * thread is moved to that node's CPUs (and MPOL_PREFERRED set, where the container allows it) for the duration of the
  * cudaHostAlloc, then put back.  On a two-socket 8-GPU box the default placement puts every rank's buffer on the node
- * the process happened to start on and the GPUs of the other socket copy across the inter-socket link (measured in
- * r01: host->device rate per GPU fell from 54 to 40 GB/s with 8 ranks).  *numa_node_out (optional) = the node, -1 when
+ * the process happened to start on and the GPUs of the other socket copy across the inter-socket link, which lowers
+ * every such rank's host->device rate.  *numa_node_out (optional) = the node, -1 when
  * the topology cannot be read (then this is a plain cudaHostAlloc).  mww_bind_host_thread moves the CALLING thread to
  * the GPU's node for good (a rank calls it once, before anything else allocates). */
 int mww_host_alloc(size_t bytes, int device, void **h_ptr, int *numa_node_out);

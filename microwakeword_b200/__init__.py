@@ -1,4 +1,4 @@
-"""microwakeword_b200 -- B200-native (sm_100a) streaming inference for microWakeWord.
+"""microwakeword_b200 -- H100-native (sm_90a) streaming inference for microWakeWord.
 
 Host side mirrors the reference's Python surface (`inference.Model`,
 `audio.audio_utils.generate_features_for_clip`); the arithmetic lives in libmww_b200.so

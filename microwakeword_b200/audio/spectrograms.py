@@ -4,7 +4,7 @@ non-overlapping segments or slid into overlapping copies, ready for ``RaggedMmap
 
 What changes is only WHERE the features are computed: the reference runs one clip at a time through the native frontend
 (:84-86, its slowest offline step); here clips are pulled from the clip generator in batches and every batch -- clips of
-different lengths -- goes through ONE launch of the B200 frontend (audio_utils.generate_features_for_clips).  Clip retrieval
+different lengths -- goes through ONE launch of the GPU frontend (audio_utils.generate_features_for_clips).  Clip retrieval
 (`Clips`) and augmentation (`Augmentation`) are training-data preparation and stay whatever object the caller passes
 (SURVEY.md section 2: out of scope); only their generator surface is used.
 """

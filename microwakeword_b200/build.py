@@ -1,4 +1,4 @@
-"""Build libmww_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo
+"""Build libmww_b200.so in-tree with nvcc for sm_90a (no JIT cache: the .so travels with the repo
 snapshot to the GPU box).  `python -m microwakeword_b200.build` or `__graft_entry__.build()`."""
 
 from __future__ import annotations
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmww_b200.so")
 SOURCES = ["mww_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_detect.cu", "mww_tables.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
 
 

@@ -56,7 +56,7 @@ const int32_t kOkayNabuArch[30] = {32, 5, 3, 40, 4, 17, 64, 1, 5, 0, 0, 0, 64, 2
 }  // namespace
 
 struct mww_handle {
-    int device = 0, n_streams = 0, sm_count = 148;
+    int device = 0, n_streams = 0, sm_count = 132;
     bool quantized = false;
     bool has_nn = true;
     std::string err;
@@ -66,7 +66,7 @@ struct mww_handle {
     // weights
     uint8_t *d_weights = nullptr;
     NnWeightsF32 W;
-    TcWeights TW{};                 // fp32 okay_nabu: pre-split weights for the tcgen05 clip kernel (mww_nn_tc.cu)
+    TcWeights TW{};                 // fp32 okay_nabu: pre-split weights for the wgmma clip kernel (mww_nn_tc.cu)
     bool no_tc = false;             // MWW_NO_TC: keep the mma.sync clip kernel (A/B measurements)
     int live_variant = 3;           // MWW_LIVE_VARIANT: 3 = bulk-copy stages (default), 2 = warp-specialised with register loads, 1 = r01 kernel
     NnWeightsI8 Wq;
@@ -318,7 +318,7 @@ int run_nn_tile(mww_t *h, int first, int n, const void *d_rows, int row_type, lo
     }
     if (!h->no_tc && row_type == MWW_ROWS_U16 && (h->n_pend + n_rows) / 3 >= kTcMinSteps && reinterpret_cast<uintptr_t>(d_rows) % 16 == 0 &&
         (rows_stream_stride_rows * kNumChannels * 2) % 16 == 0) {
-        // long calls on raw frontend rows: time is the M = 128 dimension of tcgen05.mma (mww_nn_tc.cu)
+        // long calls on raw frontend rows: time is the M dimension of wgmma (mww_nn_tc.cu)
         CU(h, launch_nn_f32_tc(h->W, h->TW, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
                                static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend,
                                static_cast<const uint16_t *>(d_rows), rows_stream_stride_rows * kNumChannels, n_rows, d_probs, probs_stride, n,

@@ -1,4 +1,4 @@
-// mww_common.h -- shared macros / small integer helpers for the B200 streaming-inference kernels.
+// mww_common.h -- shared macros / small integer helpers for the H100 streaming-inference kernels.
 //
 // Every arithmetic helper is __host__ __device__ so that tests/host_emul can execute the *same*
 // phase functions the kernels run, thread by thread, on the CPU (there is no GPU in the authoring

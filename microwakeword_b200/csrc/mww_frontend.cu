@@ -1,4 +1,4 @@
-// mww_frontend.cu -- sm_100a kernels of the batched micro-frontend (see mww_frontend_dev.cuh for the
+// mww_frontend.cu -- sm_90a kernels of the batched micro-frontend (see mww_frontend_dev.cuh for the
 // phase decomposition and the reference citations).
 #include <cuda_runtime.h>
 #include <stdlib.h>
@@ -32,7 +32,7 @@ __device__ __forceinline__ void k1_load_audio_async(int tid, K1Smem &sm, int buf
 }
 
 // vectorised variant of k1_packed_load_audio (same alignment conditions): 8 samples per 16-byte copy instead of one
-// 2-byte load + an integer division per sample (the scalar loop cost ~30 % of the packed kernel's instructions)
+// 2-byte load + an integer division per sample
 __device__ __forceinline__ void k1_packed_load_audio_async(int tid, K1Smem &sm, const int16_t *carry, int used, const int16_t *audio,
                                                            long long audio_stride, int n_samples, long long s0, int n_streams, int spc, int fps) {
     const int span8 = (fps + 2) * (kHop / 8), used8 = used / 8, n8 = n_samples / 8;
@@ -50,7 +50,7 @@ __device__ __forceinline__ void k1_packed_load_audio_async(int tid, K1Smem &sm, 
 // K1: grid = (streams, group_chunks); 256 threads; 16 frames of one stream per iteration.
 // kFuseK2 (grid.y == 1: the CTA walks all of its stream's groups in order): the temporal chain -- noise estimate, PCAN, log --
 // runs from shared memory right behind the filterbank and the kernel writes the uint16 feature rows itself; no V round trip
-// through HBM (148 + 169 B per frame in r01), no K2 launch, no scratch buffer.
+// through HBM, no K2 launch, no scratch buffer.
 // kOcc = CTAs per SM the kernel is compiled for: 3 keeps the per-lane FFT twiddles in registers (80 registers), 4 reads them
 // from shared memory (64 registers).
 template <bool kFuseK2, int kOcc>

@@ -3,7 +3,7 @@
 // Replaces the per-frame arithmetic that pymicro_features.MicroFrontend.ProcessSamples performs
 // when called from microwakeword/audio/audio_utils.py:57-62 (algorithm: SURVEY.md Appendix B).
 //
-// Work decomposition (B200-first, not a translation of the scalar C library):
+// Work decomposition (GPU-first, not a translation of the scalar C library):
 //   * kernel K1 "spectral": every 10 ms frame is independent up to the filterbank sqrt, so a CTA of
 //     256 threads processes 16 frames of one stream at a time, 16 lanes per frame:
 //       P0  coalesced int16 loads of the 18-hop audio span into shared memory
@@ -62,7 +62,7 @@ struct K1Lane {
 };
 
 // The same constants read from shared memory where they are used (15 conflict-free LDS per group) instead of living in 30
-// registers: the clip kernel then fits 64 registers = 4 CTAs per SM (r02: 24 -> 32 resident warps on an issue-bound kernel).
+// registers: the clip kernel then fits 64 registers = 4 CTAs per SM (more resident warps for an issue-bound kernel).
 struct K1LaneShared { const uint32_t *row; };   // &sm.lane_tw[b][0]: [0..3) stage 3, [3 + 3j + q] stage 4
 
 // ---------------------------------------------------------------------------------------------
@@ -138,8 +138,8 @@ MWW_HD uint32_t isqrt64_round(uint64_t x) {
 // real root (s < 2^24), and the library's "round up iff remainder > root" is round-to-nearest of sqrt x, which never
 // ties and never comes closer than 2^-27 to a half-integer (sqrt(n^2 - n) = n - 1/2 - 1/(8n) ...), so
 // trunc(s + 0.5) is exact.  ~22 instructions (MUFU.RSQ64H + 10 FP64 ops) instead of ~70 integer ones; the FP64
-// pipe is otherwise idle in K1 (K1 23.7 -> 22.0 ms per step).  Measured and rejected: a branch-free variant (hand-written
-// RSQ64H seed + two Newton steps + an exact integer check, all of a lane's roots in one block) -- 22.9 ms: the extra
+// pipe is otherwise idle in K1.  Rejected: a branch-free variant (hand-written
+// RSQ64H seed + two Newton steps + an exact integer check, all of a lane's roots in one block) -- the extra
 // instructions cost more than the slow-path branch of sqrt() and the serial FP64 chains.  x >= 2^48 -- only reachable through the library's int32 view of an energy of
 // exactly 2^31 -- takes the integer routine above.
 MWW_HD uint32_t isqrt64_round_fast(uint64_t x) {

@@ -1,4 +1,4 @@
-// mww_nn.cu -- sm_100a kernel + launcher for the fp32 streaming MixedNet in clip formulation
+// mww_nn.cu -- sm_90a kernel + launcher for the fp32 streaming MixedNet in clip formulation
 // (phase functions and reference citations: mww_nn_dev.cuh).
 #include <cuda_runtime.h>
 #include <cstdlib>

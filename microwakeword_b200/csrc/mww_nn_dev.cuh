@@ -6,7 +6,7 @@
 // with folded BatchNorm + ReLU, 17-row ring, Flatten, Dense(1), sigmoid) with the ring semantics of
 // microwakeword/layers/stream.py:581-595.
 //
-// B200-first design: every conv in the graph is a causal 'valid' FIR along time, so a whole chunk of
+// Hopper-first design: every conv in the graph is a causal 'valid' FIR along time, so a whole chunk of
 // TT model steps of one stream is evaluated layer by layer as small dense problems whose M dimension
 // is TIME (README.md:27-28 equivalence; the ring state supplies the k-1 rows of history).  The ring
 // buffers live in shared memory for the entire clip and touch HBM once per call, instead of the
@@ -100,7 +100,7 @@ MWW_HD void nn_load_state_l(int tid, float *sm, const float *state) {
     constexpr NnLayerGeom g = kGeom[L];
     const float *src = state + kStateOff[L + 1];
     // 4-byte cp.async (LDGSTS): the ~15 transposing copies a thread issues are all in flight at once instead of one
-    // load -> store round trip after the other (this phase held 9 % of the kernel's stall samples, all long-scoreboard)
+    // load -> store round trip after the other
     for (int e = tid; e < g.ring * g.cin; e += kNnThreads) {
         const int r = e / g.cin, c = e - r * g.cin;
         float *dst = sm + g.off + c * g.ld + (g.hp - g.ring) + r;
@@ -124,8 +124,7 @@ MWW_HD void nn_load_features(int tid, float *sm, const NnInput &in, int step0, i
     const int n_q = 3 * n + 2, U = n + 1;          // plane column u = q / 3 <= n
     // one thread handles 8 consecutive features of one row: a single 16-byte load on the uint16 fast path.
     // thread -> (8-feature group, plane j, u) with u FASTEST: consecutive lanes store consecutive words of a plane row
-    // (row-major thread order put the 32 lanes of a store on 2-3 banks: 93 % of this phase's wavefronts were
-    // conflict replays, ncu).  The 16-byte global loads of neighbouring lanes are then 3 rows apart and meet in L1.
+    // (row-major thread order puts the 32 lanes of a store on 2-3 banks).  The 16-byte global loads of neighbouring lanes are then 3 rows apart and meet in L1.
     for (int e = tid; e < 15 * U; e += kNnThreads) {
         const int u = e % U, jf = e / U, j = jf % 3, f0 = 8 * (jf / 3);
         const int q = 3 * u + j;

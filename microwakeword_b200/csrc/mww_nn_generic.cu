@@ -1,4 +1,4 @@
-// mww_nn_generic.cu -- sm_100a kernels + launchers of the run-time-geometry MixedNet (phase functions, rationale and
+// mww_nn_generic.cu -- sm_90a kernels + launchers of the run-time-geometry MixedNet (phase functions, rationale and
 // reference citations: mww_nn_generic.cuh).  One CTA = one stream, stepped like the reference's interpreter loop
 // (microwakeword/inference.py:109-123) with every ring resident in shared memory for the whole call.
 #include <cuda_runtime.h>
@@ -148,7 +148,7 @@ cudaError_t launch_gen_fill_state_i8(const GenArch &A, const GenWeightsI8 &W, in
                                      cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
     const long long total = (long long)n * ((long long)A.state_elems + (long long)A.pend_cap * kNumChannels);
-    const unsigned blocks = (unsigned)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const unsigned blocks = (unsigned)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     gen_fill_state_i8_kernel<<<blocks, 256, 0, st>>>(A, W, state, pend, ids, n, n_streams);
     return cudaGetLastError();
 }

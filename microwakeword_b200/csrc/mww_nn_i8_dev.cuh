@@ -33,7 +33,7 @@ struct NnWeightsI8 {
     const int32_t *pw_bf[4];  // [64]  bias - zp_d  * sum_k w
     // input quantisation of a uint16 feature as a table: qlut[u] = nnq_quantize(u * kFeatureScale, in_scale, zp[0]) for every
     // u (64 KB, built by mww_create / the host emulation with that very expression, so exact by construction).  nullptr: compute.
-    // r02 profile of the clip kernel: the float division + conversions of this step were 14 % of its instructions.
+    // The table replaces a float division and conversions per feature.
     const int8_t *qlut = nullptr;
 };
 
@@ -150,7 +150,7 @@ MWW_HD void nnq_load_weights(int tid, int32_t *sm, const NnWeightsI8 &W) {
 // One thread handles 8 consecutive features of one row: a single 8 / 16 / 2 x 16-byte load (int8 / uint16 / float32
 // rows), eight quantisations (Model.quantize_input_data, inference.py:127-147) and one 8-byte store per im2col copy.
 // The first version walked single elements -- one dependent 2-byte load, a division and two byte stores each -- and
-// held 47 % of this kernel's stall samples (profiles/r01_nn_i8_stalls.txt).
+// stalled the kernel on those dependent loads.
 struct alignas(8) NnQ8 { uint32_t lo, hi; };
 MWW_HD NnQ8 nnq_row_octet(const NnInputI8 &in, const NnWeightsI8 &W, int vr, int f0) {
     if (vr < 0) return *reinterpret_cast<const NnQ8 *>(in.ring0 + (2 + vr) * kNumChannels + f0);

@@ -1,4 +1,4 @@
-// mww_nn_i8_live.cu -- sm_100a kernel + launcher of the int8 live-step MixedNet (phase functions and rationale:
+// mww_nn_i8_live.cu -- sm_90a kernel + launcher of the int8 live-step MixedNet (phase functions and rationale:
 // mww_nn_i8_live.cuh).
 #include <cuda_runtime.h>
 
@@ -26,25 +26,18 @@ nn_i8_live_kernel(NnWeightsI8 W, int8_t *__restrict__ state, int8_t *__restrict_
         const long long s0 = (long long)g * kLiveStreams;
         const int n_valid = min(kLiveStreams, n_streams - (int)s0);
         uint32_t keep[4][kLqKeep];
-        // rings are requested from L2 two to three stages before their register loads (mww_nn_live.cuh, "L2 prefetch")
-        live_prefetch_rings<1, 2>(tid, state, s0, n_valid);
         livq_build_a(tid, smb, in, W, s0, n_valid, keep);
         __syncthreads();
-        live_prefetch_rings<3, 3>(tid, state, s0, n_valid);
         livq_write_tail(tid, state, pend, s0, n_valid, keep);
         livq_first_conv_mma(tid, smb, W);
         __syncthreads();
         livq_depthwise<0>(tid, smb, W, state, s0, n_valid, heads.h[0]); __syncthreads();
         livq_pointwise_mma<0>(tid, smb, W); __syncthreads();
         livq_depthwise<1>(tid, smb, W, state, s0, n_valid, heads.h[1]); __syncthreads();
-        live_prefetch_rings<4, 4>(tid, state, s0, n_valid);
         livq_pointwise_mma<1>(tid, smb, W); __syncthreads();
         livq_depthwise<2>(tid, smb, W, state, s0, n_valid, heads.h[2]); __syncthreads();
-        live_prefetch_rings<5, 5>(tid, state, s0, n_valid);
         livq_pointwise_mma<2>(tid, smb, W); __syncthreads();
         livq_depthwise<3>(tid, smb, W, state, s0, n_valid, heads.h[3]); __syncthreads();
-        live_prefetch_next_window(tid, state, pend, rows, rows_stream_stride_bytes, row_type == 1 ? 480u : (row_type == 0 ? 240u : 120u),
-                                  (long long)(g + gridDim.x) * kLiveStreams, n_streams);
         livq_pointwise_mma<3>(tid, smb, W); __syncthreads();
         livq_head_partial(tid, smb, W, state, s0, n_valid, heads.h[4]);
         __syncthreads();

@@ -1,4 +1,4 @@
-// mww_nn_int8.cu -- sm_100a kernel + launcher for the int8-quantised streaming MixedNet
+// mww_nn_int8.cu -- sm_90a kernel + launcher for the int8-quantised streaming MixedNet
 // (phase functions and reference citations: mww_nn_i8_dev.cuh).
 #include <cuda_runtime.h>
 
@@ -87,7 +87,7 @@ cudaError_t launch_nn_i8(const NnWeightsI8 &W, int8_t *state, int8_t *pend, int 
 cudaError_t launch_fill_state_i8(const NnWeightsI8 &W, int8_t *state, int8_t *pend, const int32_t *ids, int n, int n_streams, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
     const long long total = (long long)n * (kStateFloats + 2 * kNumChannels);
-    const unsigned blocks = (unsigned)std::min<long long>((total + 255) / 256, 148 * 16);
+    const unsigned blocks = (unsigned)std::min<long long>((total + 255) / 256, 132 * 16);
     fill_state_i8_kernel<<<blocks, 256, 0, st>>>(W, state, pend, ids, n, n_streams);
     return cudaGetLastError();
 }

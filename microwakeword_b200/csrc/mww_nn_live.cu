@@ -1,4 +1,4 @@
-// mww_nn_live.cu -- sm_100a kernel + launcher of the live-step MixedNet (one model step for many streams per
+// mww_nn_live.cu -- sm_90a kernel + launcher of the live-step MixedNet (one model step for many streams per
 // launch; phase functions and rationale: mww_nn_live.cuh).
 #include <cuda_runtime.h>
 
@@ -28,26 +28,18 @@ nn_f32_live_kernel(NnWeightsF32 W, float *__restrict__ state, float *__restrict_
         const long long s0 = (long long)g * kLiveStreams;
         const int n_valid = min(kLiveStreams, n_streams - (int)s0);
         float keep[4][kLiveKeep];
-        // every ring is requested from L2 two to three stages before its register loads (mww_nn_live.cuh, "L2 prefetch");
-        // at most ~9.7 KB per stream are requested-but-unread at any point of the chain
-        live_prefetch_rings<1, 2>(tid, state, s0, n_valid);
         live_build_a(tid, sm, in, s0, n_valid, keep);
         __syncthreads();
-        live_prefetch_rings<3, 3>(tid, state, s0, n_valid);
         live_write_tail(tid, state, pend, s0, n_valid, keep);
         live_first_conv_mma(tid, sm, W.w0, 32);
         __syncthreads();
         live_depthwise<0>(tid, sm, W, state, s0, n_valid, heads.h[0]); __syncthreads();
         live_pointwise_mma<0>(tid, sm, W); __syncthreads();
         live_depthwise<1>(tid, sm, W, state, s0, n_valid, heads.h[1]); __syncthreads();
-        live_prefetch_rings<4, 4>(tid, state, s0, n_valid);
         live_pointwise_mma<1>(tid, sm, W); __syncthreads();
         live_depthwise<2>(tid, sm, W, state, s0, n_valid, heads.h[2]); __syncthreads();
-        live_prefetch_rings<5, 5>(tid, state, s0, n_valid);
         live_pointwise_mma<2>(tid, sm, W); __syncthreads();
         live_depthwise<3>(tid, sm, W, state, s0, n_valid, heads.h[3]); __syncthreads();
-        live_prefetch_next_window(tid, state, pend, rows, rows_stream_stride_bytes, rows_are_f32 ? 480u : 240u,
-                                  (long long)(g + gridDim.x) * kLiveStreams, n_streams);
         live_pointwise_mma<3>(tid, sm, W); __syncthreads();
         live_head_partial(tid, sm, W, state, s0, n_valid, heads.h[4]);
         __syncthreads();
@@ -127,15 +119,15 @@ nn_f32_live2_kernel(NnWeightsF32 W, float *__restrict__ state, float *__restrict
 }
 
 // =====================================================================================================================
-// v3: the ring data arrive by bulk copy (TMA) instead of register loads.  Measured on v2 (MWW_LIVE_MODE): streamers alone
-// 0.235 ms (81 % of HBM), chain alone 0.16-0.23 ms, together 0.39-0.41 ms -- the chain's shared-memory operands and the
-// streamers' global loads queue in the same LSU / L1 miss pipeline.  Here one elected thread issues one
+// v3: the ring data arrive by bulk copy (TMA) instead of register loads.  In v2 the two halves together take much longer than
+// either alone (MWW_LIVE_MODE runs one half): the chain's shared-memory operands and the streamers' global loads queue in the
+// same LSU / L1 miss pipeline.  Here one elected thread issues one
 // cp.async.bulk (global -> shared, 16 384 B = rings 1..5 of one stream, contiguous in the state layout) per stream into a
 // ring of four stages; nine "P" warps (one ring column per thread, its R rotated taps in registers) turn each stage into the
 // stream's 288 partial sums; six warps build the first-conv window one group ahead; the 8 chain warps are v2's.
 // P is single-buffered: a P thread keeps the 32 sums of the NEXT group in registers and writes them once the chain's layer of
 // the current group has read the buffer (one full / empty named-barrier pair per ring) -- the second P buffer of v2 became
-// two more stages (bytes in flight are what an HBM-bound kernel is made of: 2 stages 0.30 ms, 4 stages see DESIGN.md).
+// two more stages (bytes in flight are what an HBM-bound kernel is made of).
 // The sums and their order are v2's (= v1's): the three kernels are bit-identical.
 constexpr int kLive3PThreads = kLive2Cols;                            // 288: one thread per ring column
 constexpr int kLive3AThreads = kLive3WindowThreads;

@@ -80,7 +80,7 @@ MWW_HD float live_row_value(const LiveInput &in, size_t su, unsigned e) {
 constexpr int kLiveKeep = 10;         // per thread and stream: 7 window values + 3 new-pending values
 // Every load below is UNCONDITIONAL on a clamped, always-valid address and the value is selected afterwards: with
 // conditional loads the compiler emitted one branch per element and the 40 loads of a thread serialised into 40
-// dependent DRAM round trips (measured: +11 % kernel time).
+// dependent DRAM round trips.
 template <bool F32ROWS>
 MWW_HD void live_build_a_t(int tid, float *sm, const LiveInput &in, long long s0, int n_valid, float (&keep)[4][kLiveKeep]) {
     const int warp = tid >> 5;
@@ -285,8 +285,7 @@ MWW_HD void live_canonicalise_column(float *state, long long s, int col, const L
 }
 
 // =====================================================================================================================
-// v2: warp-specialised live step (r02).  ncu on the kernel above: issue-active 20 %, 16 resident warps per SM, stall samples
-// spread evenly over every phase -- the whole kernel runs latency-bound because a CTA's ring loads and its layer chain take
+// v2: warp-specialised live step.  The kernel above runs latency-bound: a CTA's ring loads and its layer chain take
 // turns.  The old ring rows do not depend on this step's activations, so
 //     P[column] = bias + sum over the R old rows of tap(row) * x(row)           ("streamers", 16 warps)
 // can be computed for stream group g+1 while the layer chain of group g runs   ("chain", 8 warps)
@@ -301,10 +300,9 @@ constexpr int kLive2PPitch = 33;                              // P[column][strea
 constexpr int kLive2Cols = 32 + 64 * 4;                       // 288 ring columns per stream (blocks 0..3, head)
 constexpr int kLive2PFloats = kLive2Cols * kLive2PPitch;      // one P buffer
 constexpr int kLive2OffP = kLiveSmemFloats;                   // the chain's regions keep their v1 offsets
-// Everything the CHAIN reads besides its own activations lives in shared memory: measured alone the chain takes 0.23 ms and the
-// streamers 0.23 ms, together 0.41 ms -- with the first conv's and block 0's weights, the newest taps and the biases coming from
-// L2 / L1, every dependent global access of the latency-bound chain slowed down 2-3x while the streamers saturated the memory
-// system.  (The streamers' old-row taps moved the other way, to L1-cached global reads, to make room.)
+// Everything the CHAIN reads besides its own activations lives in shared memory: with the first conv's and block 0's weights,
+// the newest taps and the biases coming from L2 / L1, every dependent global access of the latency-bound chain waits behind the
+// streamers, which keep the memory system saturated.  (The streamers' old-row taps moved the other way, to L1-cached global reads, to make room.)
 constexpr int kLive2W0Pitch = 40;                             // first-conv weights [200][40]: pitch = 8 (mod 32) like kWLd
 constexpr int kLive2OffPw0 = kLive2OffP + 2 * kLive2PFloats;
 constexpr int kLive2OffSmall = kLive2OffPw0 + 32 * kWLd;      // newest taps [288], depthwise... 1x1 biases [4][64], head bias
@@ -402,8 +400,8 @@ MWW_HD void live2_stream_group(int st, const NnWeightsF32 &W, const float *state
 
 // chain: first-conv window without per-thread copies kept across the barrier (the new first-conv ring is read back from
 // the A operand, the new pending rows from the caller's rows)
-// NT = threads that share the work (512: the streamers build the window one group ahead of the chain, r02: with the chain
-// loading it itself, 64 % of the chain's stall samples sat in this phase -- its loads queue behind the streamers' in the LSU)
+// NT = threads that share the work (512: the streamers build the window one group ahead of the chain; a chain loading it
+// itself stalls here, its loads queue behind the streamers' in the LSU)
 template <bool F32ROWS, int NT>
 MWW_HD void live2_build_a_t(int tid, float *sm, const LiveInput &in, long long s0, int n_valid) {
     constexpr int QPW = kLiveStreams / (NT / 32);                  // streams per warp
@@ -443,12 +441,12 @@ MWW_HD void live2_build_a(int tid, float *sm, const LiveInput &in, long long s0,
 }
 // v3: the same window in two halves -- the loads of group k + 1 are issued (into registers) right after group k's window went
 // to shared memory, i.e. a whole chain period before they are needed: under the bulk copies' HBM load a round of global
-// loads costs microseconds, and A is free only after the first conv of the previous group (r02 ncu: with two window warps
-// loading on demand the chain spent 33 % of its samples waiting for A).  The same warps also move the call's last n_pend
+// loads costs microseconds, and A is free only after the first conv of the previous group (window warps loading on demand
+// leave the chain waiting for A).  The same warps also move the call's last n_pend
 // rows into the pending-row buffer (v1 / v2: the chain does, with loads on its critical path): a stream's old pending rows
 // are read (they are part of the window) before its new ones are written (a named barrier among the window warps).
 // 192 threads: thread t owns the (stream, element) pairs t, t + 192, ... of the group's 32 x 200 -- 34 values per thread, no
-// spills at the kernel's 80 registers (128 threads x 56 values spilled, and their loads took 87 % of a chain period).
+// spills at the kernel's 80 registers (128 threads x 56 values spill).
 constexpr int kLive3WindowThreads = 192;
 constexpr int kLive3WindowPerThread = (kLiveStreams * 200 + kLive3WindowThreads - 1) / kLive3WindowThreads;     // 34
 template <bool F32ROWS>
@@ -561,44 +559,6 @@ MWW_HD void live2_dw_from_p(int tid, float *sm, float *state, long long s0, int 
 }
 
 #if defined(__CUDACC__)
-// ---- L2 prefetch of ring data one stage ahead (cp.async.bulk.prefetch.L2: no registers, no shared memory, no barrier) ----
-// The layer chain is serial (ring read -> depthwise -> barrier -> MMA -> barrier -> next ring read), so a CTA's ring loads
-// only ever cover one stage and their DRAM latency is exposed once per stage; with two CTAs per SM that left the kernel
-// bound by bytes in flight (DESIGN.md, NN live step).  One thread per stream asks the L2 for the NEXT stage's ring
-// (<= 5.6 KB per stream, contiguous) while the current stage computes; the later register loads hit in L2.  Look-ahead is
-// a single stage on purpose: 32 streams x 5.6 KB x 296 CTAs = 53 MB stays inside the 126 MB L2, a whole group ahead would not.
-// Addresses and sizes are multiples of 16 by construction (ring offsets 320/832/3392/6976/12608 B, stream pitch 16 704 B).
-MWW_D void l2_prefetch(const void *p, unsigned bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
-MWW_D int live_prefetch_slot(int tid) { return (tid & 31) < 4 ? (tid >> 5) * 4 + (tid & 31) : -1; }   // 256 threads -> 32 streams
-// rings FIRST..LAST of the state (0 = first-conv ring, 1..4 = MixConv blocks, 5 = head) of this CTA's stream group;
-// T = float (fp32 model) or int8_t (int8 model: offsets 80/208/848/1744/3152 B, pitch 4 176 B -- still multiples of 16)
-template <int FIRST, int LAST, typename T>
-MWW_D void live_prefetch_rings(int tid, const T *state, long long s0, int n_valid) {
-    constexpr int lo = kStateOff[FIRST], hi = LAST == 5 ? kStateFloats : kStateOff[LAST + 1];
-    static_assert((lo * sizeof(T)) % 16 == 0 && ((hi - lo) * sizeof(T)) % 16 == 0 && (kStateFloats * sizeof(T)) % 16 == 0,
-                  "bulk prefetch granularity");
-    // UBLKPF takes its address from the uniform datapath, so the compiler serialises the active lanes (R2UR loop): four
-    // lanes of each of the 8 warps issue one request each instead of 32 lanes of one warp
-    const int sl = live_prefetch_slot(tid);
-    if (sl >= 0 && sl < n_valid) l2_prefetch(state + (size_t)(s0 + sl) * kStateFloats + lo, (unsigned)((hi - lo) * sizeof(T)));
-}
-// the next group's first-conv window: first-conv ring + block-0 ring (contiguous), pending rows, feature rows
-template <typename T>
-MWW_D void live_prefetch_next_window(int tid, const T *state, const T *pend, const void *rows, long long rows_stream_stride_bytes,
-                                     unsigned row_bytes, long long s0n, int n_streams) {
-    const int sl = live_prefetch_slot(tid);
-    if (sl < 0 || s0n + sl >= n_streams) return;
-    const size_t su = (size_t)(s0n + sl);
-    constexpr unsigned window_bytes = (unsigned)(kStateOff[2] * sizeof(T));        // first-conv ring + block-0 ring
-    static_assert(window_bytes % 16 == 0 && (2 * kNumChannels * sizeof(T)) % 16 == 0, "bulk prefetch granularity");
-    l2_prefetch(state + su * kStateFloats, window_bytes);
-    l2_prefetch(pend + su * (2 * kNumChannels), (unsigned)(2 * kNumChannels * sizeof(T)));
-    const char *rb = static_cast<const char *>(rows) + su * (size_t)rows_stream_stride_bytes;
-    if ((reinterpret_cast<uintptr_t>(rb) & 15) == 0) l2_prefetch(rb, row_bytes & ~15u);
-}
-
 // named barriers of the warp-specialised kernel (barrier 0 is __syncthreads)
 MWW_D void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 MWW_D void bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }

@@ -2,14 +2,14 @@
 // conv (K = 200, mixednet.py:317-331) and the four 1x1 projections (mixednet.py:349-352), 88 % of the
 // 24 800 MACs per model step (SURVEY.md 8d).  Depthwise convs and the 17-tap head stay on CUDA cores.
 //
-// Why warp-level mma (HMMA.1688.F32.TF32) and not tcgen05: the contraction operands are produced by CUDA
-// cores (depthwise output, im2col'ed feature planes) for ONE stream and 36 time steps at a time; a tcgen05
-// tile needs >= 64 rows of smem-resident, descriptor-addressed operands plus a TMEM round trip per layer,
+// Why warp-level mma (HMMA.1688.F32.TF32) and not wgmma: the contraction operands are produced by CUDA
+// cores (depthwise output, im2col'ed feature planes) for ONE stream and 36 time steps at a time; a wgmma
+// tile needs >= 64 rows of smem-resident, descriptor-addressed operands per warpgroup,
 // and the fp32 parity budget (1e-3 on probabilities; plain TF32 measured 2.6e-3) forces the 3xTF32 split
 // (hi/lo operands), which doubles the operand footprint.  With 59 KB of ring buffers per stream that leaves
-// one CTA per SM and exposes ~1 us of async MMA latency per layer.  Register-fragment mma needs no extra
+// one CTA per SM and exposes the async MMA latency once per layer.  Register-fragment mma needs no extra
 // shared memory, and the tensor work is ~80 m16n8k8 issues per model step -- nowhere near any tensor roofline.
-// DESIGN.md section 3 has the numbers.
+// Long calls on raw uint16 rows take the 128-step wgmma kernel instead (mww_nn_tc.cu).
 //
 // 3xTF32: x = hi + lo with hi = x & 0xFFFFE000 (exactly representable in TF32) and lo = x - hi (exact in
 // fp32, <= 13 significant bits; the hardware drops its lowest bits: relative error 2^-22 of x).
@@ -156,7 +156,7 @@ MWW_HD void fc_finish_tile(float *sm, int t0, int n0, int lane, const float (&c)
 
 // block L's 1x1 conv on tensor cores; D[k][t] (pitch kDLd) is A, the staged weights [k][o] (pitch kWLd) are B
 // `n` = model steps in this chunk: an m-tile whose 16 rows all lie beyond n is skipped by its three warps (the last chunk
-// of a 100-step call has 28 steps: two m-tiles instead of three; the MMA phases are tensor-pipe bound, ncu math_pipe_throttle)
+// of a 100-step call has 28 steps: two m-tiles instead of three)
 template <int L>
 MWW_D void nn_pointwise_mma(int tid, float *sm, const NnWeightsF32 &W, int n) {
     constexpr int cin = kGeom[L].cin;
@@ -172,7 +172,7 @@ MWW_D void nn_pointwise_mma(int tid, float *sm, const NnWeightsF32 &W, int n) {
         for (int q = 0; q < 4; ++q) c[i][q] = 0.f;
     // Every warp issues THREE tiles' worth of MMAs: the warps that own only two n-tiles recompute tile 7 into a dead
     // accumulator.  A warp-dependent tile count put each mma.sync behind a branch the compiler cannot prove uniform, and
-    // every one of them was wrapped in WARPSYNC + NOP (20 % of the instructions of this phase, ncu source view).
+    // every one of them was wrapped in WARPSYNC + NOP.
     int nb[3];
 #pragma unroll
     for (int i = 0; i < 3; ++i) nb[i] = 8 * (nt0 + i < 8 ? nt0 + i : 7);

@@ -1,31 +1,29 @@
-// mww_nn_tc.cu -- fp32 streaming MixedNet, clip formulation, on the 5th-generation tensor cores (tcgen05 + TMEM).
+// mww_nn_tc.cu -- fp32 streaming MixedNet, clip formulation, on the Hopper warpgroup tensor cores (wgmma).
 //
 // Same graph and ring semantics as mww_nn_dev.cuh / mww_nn.cu (microwakeword/mixednet.py:307-386, layers/stream.py:581-595,
 // one call = inference.py:109-123 for many steps); what changes is how the dense 88 % of the MACs -- the strided first conv
 // (K = 200) and the four 1x1 projections -- are contracted:
 //
-//   * one CTA owns one stream and a chunk of up to 128 MODEL STEPS: time is the M = 128 dimension of tcgen05.mma;
+//   * one CTA owns one stream and a chunk of up to 128 MODEL STEPS: time is the M dimension; each of the CTA's two warpgroups
+//     contracts 64 of the steps (wgmma M = 64);
 //   * the CUDA cores produce each contraction's A operand (im2col of the feature rows / the depthwise MixConv output) ONCE, already
 //     split for 3xTF32 into a hi and a lo plane, in the layout the tensor core reads: K cut into slots of 32 values = 128 bytes,
 //     a slot = [128 steps][128 B] with the hardware's 128-byte XOR swizzle, so a warp whose lanes are 32 consecutive channels of
 //     one step stores 128 contiguous bytes (no bank conflicts);
 //   * the weights are split and laid out the same way once, at mww_create (build_tc_weights), and stream from L2 into shared memory
 //     with 16-byte cp.async one layer ahead of their use;
-//   * ONE elected thread issues the MMAs (tcgen05.mma.cta_group::1.kind::tf32, A and B through shared-memory matrix descriptors):
-//     per K = 8 step the three 3xTF32 products lo*hi, hi*lo, hi*hi accumulate into the same fp32 TMEM tile [128 lanes x N columns];
-//     tcgen05.commit -> mbarrier tells the CTA when the tile is complete;
-//   * the epilogue reads the accumulator back with tcgen05.ld (a warp owns 32 lanes = 32 steps), adds the folded-BatchNorm bias,
-//     applies ReLU and writes the next layer's activations [channel][time] for the depthwise stage.
+//   * both warpgroups issue wgmma.mma_async.m64nNk8.f32.tf32.tf32 with A and B through shared-memory matrix descriptors: per K = 8
+//     step the three 3xTF32 products lo*hi, hi*lo, hi*hi accumulate into the same fp32 register tile [64 steps x N];
+//   * the epilogue takes the accumulator straight from the registers, adds the folded-BatchNorm bias, applies ReLU and writes the
+//     next layer's activations [channel][time] for the depthwise stage.
 // Depthwise taps, ring buffers, the 17-row head and the sigmoid stay on CUDA cores, in shared memory for the whole call.
 //
-// r02 measurement behind this kernel (tools/probes/tcgen05_pointwise_probe.cu, profiles/r02_tcgen05_probe.txt): produce + contract +
-// epilogue of one 128 x 64 x 64 3xTF32 tile takes 2.75 us per CTA with tcgen05 against 4.02 us with warp-level mma.sync, same result
-// to the last bit of the comparison (max |error| 2.5e-6 against fp64).  The r01 kernel (mww_nn.cu) remains the path for float32 feature
-// rows and for calls shorter than kTcMinSteps steps.
+// The mma.sync kernel (mww_nn.cu) remains the path for float32 feature rows and for calls shorter than kTcMinSteps steps.
 #include <cuda_runtime.h>
 #include <cstdlib>
 #include <cstring>
 
+#include <type_traits>
 #include <vector>
 
 #include "mww_kernels.h"
@@ -42,17 +40,15 @@ constexpr int kLdx = 151;                       // activation buffer pitch [chan
 constexpr int kFeatRows = 3 * kTcM + 2;         // feature rows one chunk's first conv can touch
 
 // ---- shared memory map (bytes): 102.6 KB, TWO CTAs per SM -- a stream's layer chain is strictly serial (produce -> MMA -> epilogue ->
-// next layer), so the only way to keep the SM busy is a second, independent stream; the first version of this kernel (one CTA per SM,
-// both K-slots of A and all weights of two layers resident: 222 KB) measured 14.9 ms per 65 536 x 100 steps against 14.0 ms for the
-// mma.sync kernel.  Every contraction is therefore fed ONE K-slot (32 input channels) at a time:
+// next layer), so the only way to keep the SM busy is a second, independent stream.  Every contraction is therefore fed ONE K-slot
+// (32 input channels) at a time:
 constexpr int kOffA = 0;                        // one K-slot of A: hi plane 16 KB + lo plane 16 KB
 constexpr int kAPlaneBytes = 16384;
 constexpr int kOffB = 32768;                    // two K-slots of B (double buffer): [N <= 64 rows][128 B] hi + lo = 16 KB each
 constexpr int kBSlotBytes = 16384;
 constexpr int kOffX = kOffB + 2 * kBSlotBytes;  // activations [64][kLdx]; the chunk's raw uint16 feature rows alias it during the first conv
 constexpr int kOffSmall = kOffX + 64 * kLdx * 4;   // first-conv ring rows -2, -1 and the pending rows as floats [4][40]
-constexpr int kOffBar = kOffSmall + 4 * kNumChannels * 4;
-constexpr int kTcSmemBytes = kOffBar + 64;
+constexpr int kTcSmemBytes = kOffSmall + 4 * kNumChannels * 4;
 static_assert(2 * (kTcSmemBytes + 1024) <= 232448, "two CTAs per SM");
 static_assert(kFeatRows * kNumChannels * 2 <= 64 * kLdx * 4, "feature rows alias the activation buffer");
 static_assert(kOffA % 1024 == 0 && kOffB % 1024 == 0, "swizzled operand slots need 1024-byte alignment");
@@ -71,52 +67,64 @@ __device__ __forceinline__ void store_split(unsigned char *a_base, int t, int kk
     *reinterpret_cast<float *>(p + kAPlaneBytes) = lo;
 }
 
+// wgmma shared-memory matrix descriptor of a K-major operand with the 128-byte swizzle
 __device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);      // start address
     d |= (uint64_t)1 << 16;                           // leading byte offset (unused: the operand is one swizzle atom wide in K)
     d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset: next group of 8 rows
-    d |= (uint64_t)1 << 46;                           // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                           // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                           // SWIZZLE_128B
     return d;
 }
-// instruction descriptor of kind::tf32: D fp32, A / B tf32 K-major, M = 128, N given
-__device__ __forceinline__ constexpr uint32_t idesc_tf32(int n) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kTcM >> 4) << 24);
+// D[64 x N] (+)= A[64 x 8] B[8 x N], tf32 operands from shared memory, fp32 accumulator in the warpgroup's registers: N / 2 per thread
+template <int N_>
+__device__ __forceinline__ void mma_tf32(float (&d)[32], uint64_t da, uint64_t db, int accumulate);
+template <>
+__device__ __forceinline__ void mma_tf32<32>(float (&d)[32], uint64_t da, uint64_t db, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+                 "%16, %17, p, 1, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+                   "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-                 : "memory");
+template <>
+__device__ __forceinline__ void mma_tf32<64>(float (&d)[32], uint64_t da, uint64_t db, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+                   "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+                   "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+                   "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(accumulate));
 }
-// one K-slot: `ksteps` K = 8 steps (4, or 1 for the tail of the first conv) of the three 3xTF32 products; A slot at a_s (lo plane at
-// +16 KB), B slot at b_s with its lo plane `b_plane` bytes further
-__device__ __forceinline__ void issue_slot(uint32_t tmem_d, uint32_t a_s, uint32_t b_s, uint32_t b_plane, int n, int ksteps, bool clears) {
-    const uint32_t idesc = idesc_tf32(n);
-    for (int ks = 0; ks < ksteps; ++ks) {
+// the accumulator registers are ordered against the asynchronous MMAs: neither side of a fence / wait may be moved across it
+__device__ __forceinline__ void fence_acc(float (&d)[32]) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// one K-slot for this warpgroup's 64 steps: KSTEPS K = 8 steps (4, or 1 for the tail of the first conv) of the three 3xTF32 products;
+// A rows at a_s (lo plane at +16 KB), B slot at b_s with its lo plane `b_plane` bytes further.  Returns with the MMAs complete.
+template <int N_, int KSTEPS>
+__device__ __forceinline__ void issue_slot(float (&d)[32], uint32_t a_s, uint32_t b_s, uint32_t b_plane, bool clears) {
+    fence_acc(d);
+    asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks) {
         const uint32_t a_hi = a_s + (uint32_t)ks * 32, a_lo = a_hi + kAPlaneBytes;
         const uint32_t b_hi = b_s + (uint32_t)ks * 32, b_lo = b_hi + b_plane;
-        mma_tf32(tmem_d, desc_sw128(a_lo), desc_sw128(b_hi), idesc, !(clears && ks == 0));
-        mma_tf32(tmem_d, desc_sw128(a_hi), desc_sw128(b_lo), idesc, 1);
-        mma_tf32(tmem_d, desc_sw128(a_hi), desc_sw128(b_hi), idesc, 1);
+        mma_tf32<N_>(d, desc_sw128(a_lo), desc_sw128(b_hi), !(clears && ks == 0));
+        mma_tf32<N_>(d, desc_sw128(a_hi), desc_sw128(b_lo), 1);
+        mma_tf32<N_>(d, desc_sw128(a_hi), desc_sw128(b_hi), 1);
     }
-}
-__device__ __forceinline__ void commit_to(uint32_t bar_s) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar_s) : "memory");
-}
-__device__ __forceinline__ void wait_bar(uint32_t bar_s, uint32_t &phase) {
-    uint32_t done = 0;
-    while (!done) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(done) : "r"(bar_s), "r"(phase) : "memory");
-    }
-    phase ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+    asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
+    fence_acc(d);
 }
 // everything the generic proxy wrote to shared memory (st.shared, completed cp.async) becomes visible to the tensor core
 __device__ __forceinline__ void publish_operands() {
     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
 }
 __device__ __forceinline__ void cp16(void *smem_dst, const void *gmem_src) {
@@ -125,21 +133,6 @@ __device__ __forceinline__ void cp16(void *smem_dst, const void *gmem_src) {
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N_>
 __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N_) : "memory"); }
-
-// 32 accumulator columns [col0, col0 + 32) of this warp's 32 TMEM lanes
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-                 "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-                   "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-                   "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 // ---- geometry of the five ring-carrying activation tensors (inputs of block 0..3 and of the head): channels, ring rows ----
 __device__ __forceinline__ constexpr int tc_cin(int i) { return i == 0 ? 32 : 64; }
@@ -205,34 +198,27 @@ __device__ __forceinline__ void depthwise_slot(int tid, int n, const float *x, u
     depthwise_k<L, K>(32 * H + (tid & 31), t0, t1, x, a_base, W);
 }
 
-// accumulator [128 steps x N] -> (+ bias) ReLU -> X[o][hist + t] for t < n.  Warp w: TMEM lanes 32 (w % 4) .., columns 32 (w / 4) ..
+// accumulator [128 steps x N] -> (+ bias) ReLU -> X[o][hist + t] for t < n.  wgmma's fragment of warp w of warpgroup g: steps
+// 64 g + 16 (w % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1) in d[4 j + 2 h + e]
 template <int N_, int HIST>
-__device__ __forceinline__ void epilogue(int tid, int n, uint32_t tmem_d, float *x, const float *bias /* nullptr: none */) {
-    const int warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, half = warp >> 2;
-    if (half * 32 >= N_) return;
-    const int t = 32 * q + lane;
-    if (32 * q >= n) return;                                  // warp-uniform: this lane quarter holds no valid step
-    float v[32];
-    tmem_ld32(tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * half), v);
-    if (t < n) {
+__device__ __forceinline__ void epilogue(int tid, int n, const float (&d)[32], float *x, const float *bias /* nullptr: none */) {
+    const int lane = tid & 31;
+    const int t0 = 64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + (lane >> 2);
+    if (t0 - (lane >> 2) >= n) return;                        // warp-uniform: this warp's 16 steps are all beyond the chunk
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-            const float4 b4 = bias ? __ldg(reinterpret_cast<const float4 *>(bias + 32 * half + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
+    for (int j = 0; j < N_ / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        const float2 b2 = bias ? __ldg(reinterpret_cast<const float2 *>(bias + c)) : make_float2(0.f, 0.f);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const float r = v[j + q] + bb[q];
-                x[(32 * half + j + q) * kLdx + HIST + t] = r > 0.f ? r : 0.f;
+        for (int h = 0; h < 2; ++h) {
+            const int t = t0 + 8 * h;
+            if (t < n) {
+                const float r0 = d[4 * j + 2 * h] + b2.x, r1 = d[4 * j + 2 * h + 1] + b2.y;
+                x[c * kLdx + HIST + t] = r0 > 0.f ? r0 : 0.f;
+                x[(c + 1) * kLdx + HIST + t] = r1 > 0.f ? r1 : 0.f;
             }
         }
     }
-}
-
-// one layer's pre-split weights (contiguous in global memory, already in slot layout) -> shared memory, 16 bytes per cp.async
-__device__ __forceinline__ void stage_b(int tid, unsigned char *dst, const unsigned char *src, int bytes) {
-    for (int e = tid * 16; e < bytes; e += kTcThreads * 16) cp16(dst + e, src + e);
-    cp_commit();
 }
 
 }  // namespace
@@ -246,25 +232,10 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
     float *x = reinterpret_cast<float *>(smem + kOffX);
     uint16_t *feat = reinterpret_cast<uint16_t *>(smem + kOffX);          // alias: dead before X's first write of a chunk
     float *small = reinterpret_cast<float *>(smem + kOffSmall);           // [0,80): first-conv ring rows -2, -1; [80,160): pending rows
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + kOffBar);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + kOffBar + 32);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const uint32_t a_s = (uint32_t)__cvta_generic_to_shared(a_base), b_s = (uint32_t)__cvta_generic_to_shared(b_base);
-    const uint32_t bar_s = (uint32_t)__cvta_generic_to_shared(bar);
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"((uint32_t)__cvta_generic_to_shared(tmem_slot)), "r"(64));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-    }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(bar_s));
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_d = *tmem_slot;
-    uint32_t phase = 0;
+    const int tid = threadIdx.x, wg = tid >> 7;
+    // this warpgroup's 64 rows of the A slot (8 KB, a whole number of 1024-byte swizzle atoms)
+    const uint32_t a_s = (uint32_t)__cvta_generic_to_shared(a_base) + (uint32_t)wg * 64 * 128, b_s = (uint32_t)__cvta_generic_to_shared(b_base);
+    float acc[32];
 
     // The 14 K-slots of a chunk, in order: first conv 0..6 (N = 32; the last holds K = 8), block 0 (one slot), blocks 1..3 (two each).
     // Slot i's weights sit in B buffer i % 2 and are fetched while slot i - 1 is produced and contracted.
@@ -282,19 +253,21 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
         }
         cp_commit();                                     // one group per call (possibly empty): wait_group counts stay uniform
     };
-    // after slot i's A operand is in shared memory: its weights have landed -> publish -> one thread issues -> prefetch slot i + 2's weights
-    // once slot i's MMAs are done with buffer i % 2 (the caller waits on the mbarrier before touching A again anyway)
-    auto contract_slot = [&](int i, int n_out, int ksteps, bool clears) {
+    // after slot i's A operand is in shared memory: its weights have landed -> publish -> each warpgroup contracts its 64 steps (a
+    // warpgroup whose steps all lie beyond the chunk skips) -> once both are done with A and B buffer i % 2, prefetch slot i + 2's weights
+    auto contract_slot = [&](auto n_out, auto ksteps, int i, int n, bool clears) {
         cp_wait<1>();                                    // all but the most recent group: slot i's weights are here
         publish_operands();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-            issue_slot(tmem_d, a_s, b_s + (uint32_t)(i & 1) * kBSlotBytes, i < 7 ? 4096u : 8192u, n_out, ksteps, clears);
-            commit_to(bar_s);
-        }
-        wait_bar(bar_s, phase);                          // A and B buffer i % 2 are free again; the accumulator holds slots <= i
+        if (64 * wg < n)
+            issue_slot<decltype(n_out)::value, decltype(ksteps)::value>(acc, a_s, b_s + (uint32_t)(i & 1) * kBSlotBytes, i < 7 ? 4096u : 8192u,
+                                                                         clears);
+        __syncthreads();                                 // A and B buffer i % 2 are free again; the accumulator holds slots <= i
         stage_slot(i + 2);
     };
+    using N32 = std::integral_constant<int, 32>;
+    using N64 = std::integral_constant<int, 64>;
+    using K4 = std::integral_constant<int, 4>;
+    using K1 = std::integral_constant<int, 1>;
 
     const int n_virtual = n_pend + n_rows;
     const int n_steps = n_virtual / 3;
@@ -335,7 +308,7 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
                 if (vr < n_pend) return small[80 + vr * kNumChannels + f];
                 return (float)feat[(vr - n_pend - row_lo) * kNumChannels + f] * kFeatureScale;
             };
-            // ---- first conv: K = 200 as seven K-slots accumulated in TMEM; thread -> (k column tid % 32, steps tid / 32 + 8 i) ----
+            // ---- first conv: K = 200 as seven K-slots accumulated in registers; thread -> (k column tid % 32, steps tid / 32 + 8 i) ----
 #pragma unroll 1
             for (int slot = 0; slot < 7; ++slot) {
                 const int kk = tid & 31, k = 32 * slot + kk;
@@ -350,32 +323,30 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
                     for (; t < n; t += 8) store_split(a_base, t, kk, (float)src[3 * kNumChannels * t] * kFeatureScale);
                     for (; t < t_pad; t += 8) store_split(a_base, t, kk, 0.f);
                 }
-                contract_slot(slot, 32, slot < 6 ? 4 : 1, slot == 0);
+                if (slot < 6) contract_slot(N32{}, K4{}, slot, n, slot == 0);
+                else contract_slot(N32{}, K1{}, slot, n, false);
             }
             // first conv epilogue: ReLU, no bias -> X (block 0's input), its ring history in front.  The feature rows under X are dead.
-            __syncthreads();
             ring_to_x<0>(tid, x, my_state);
-            epilogue<32, 4>(tid, n, tmem_d, x, nullptr);
-            asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
+            epilogue<32, 4>(tid, n, acc, x, nullptr);
             __syncthreads();
             // ---- four MixConv blocks: per K-slot depthwise -> contract; then ring out / next history in / epilogue ----
 #define MWW_TC_BLOCK_END(L)                                                                                                                 \
             x_to_ring<L>(tid, x, my_state, n);                          /* the last R columns of (history ++ outputs): the ring for later */ \
             __syncthreads();                                                                                                                \
             ring_to_x<L + 1>(tid, x, my_state);                                                                                             \
-            epilogue<64, tc_ring(L + 1)>(tid, n, tmem_d, x, W.pw_b[L]);                                                                     \
-            asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");                                                              \
+            epilogue<64, tc_ring(L + 1)>(tid, n, acc, x, W.pw_b[L]);                                                                        \
             __syncthreads();
-            depthwise_slot<0, 0>(tid, n, x, a_base, W); contract_slot(7, 64, 4, true);
+            depthwise_slot<0, 0>(tid, n, x, a_base, W); contract_slot(N64{}, K4{}, 7, n, true);
             MWW_TC_BLOCK_END(0)
-            depthwise_slot<1, 0>(tid, n, x, a_base, W); contract_slot(8, 64, 4, true);
-            depthwise_slot<1, 1>(tid, n, x, a_base, W); contract_slot(9, 64, 4, false);
+            depthwise_slot<1, 0>(tid, n, x, a_base, W); contract_slot(N64{}, K4{}, 8, n, true);
+            depthwise_slot<1, 1>(tid, n, x, a_base, W); contract_slot(N64{}, K4{}, 9, n, false);
             MWW_TC_BLOCK_END(1)
-            depthwise_slot<2, 0>(tid, n, x, a_base, W); contract_slot(10, 64, 4, true);
-            depthwise_slot<2, 1>(tid, n, x, a_base, W); contract_slot(11, 64, 4, false);
+            depthwise_slot<2, 0>(tid, n, x, a_base, W); contract_slot(N64{}, K4{}, 10, n, true);
+            depthwise_slot<2, 1>(tid, n, x, a_base, W); contract_slot(N64{}, K4{}, 11, n, false);
             MWW_TC_BLOCK_END(2)
-            depthwise_slot<3, 0>(tid, n, x, a_base, W); contract_slot(12, 64, 4, true);
-            depthwise_slot<3, 1>(tid, n, x, a_base, W); contract_slot(13, 64, 4, false);
+            depthwise_slot<3, 0>(tid, n, x, a_base, W); contract_slot(N64{}, K4{}, 12, n, true);
+            depthwise_slot<3, 1>(tid, n, x, a_base, W); contract_slot(N64{}, K4{}, 13, n, false);
             MWW_TC_BLOCK_END(3)
 #undef MWW_TC_BLOCK_END
             cp_wait<0>();
@@ -441,9 +412,6 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
             __syncthreads();                                        // `small` is reloaded for the next stream
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_d), "r"(64));
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// mww_nn_tc.h -- launcher of the tcgen05 clip kernel (mww_nn_tc.cu) and the host-side weight preparation it needs.
+// mww_nn_tc.h -- launcher of the wgmma clip kernel (mww_nn_tc.cu) and the host-side weight preparation it needs.
 #pragma once
 
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// mww_nn_tc_prep.h -- the tcgen05 clip kernel's operand layout, shared by the kernel (mww_nn_tc.cu: the CUDA cores write the A
+// mww_nn_tc_prep.h -- the wgmma clip kernel's operand layout, shared by the kernel (mww_nn_tc.cu: the CUDA cores write the A
 // operand with it, mww_create lays the weights out with it) and by the host-side test that reads the operands back the way the tensor
 // core does (tests/host_emul).  No CUDA dependency.
 #pragma once
@@ -13,7 +13,7 @@
 
 namespace mww {
 
-// 128-byte-swizzled K-major slot (tcgen05 shared-memory matrix descriptor with SWIZZLE_128B, stride byte offset 1024): rows of 128
+// 128-byte-swizzled K-major slot (wgmma shared-memory matrix descriptor with SWIZZLE_128B, stride byte offset 1024): rows of 128
 // bytes = 32 fp32 along K; within each group of 8 rows the 16-byte chunk index is XORed with (row & 7).  Byte offset of element
 // (row, kk), kk in [0, 32).
 MWW_HD uint32_t sw128_off(int row, int kk) {

@@ -1,5 +1,5 @@
 // mww_tables.h -- host-built constant tables of the fixed-point micro-frontend, in the packed
-// layouts the sm_100a kernels consume.  Replaces the table construction that
+// layouts the sm_90a kernels consume.  Replaces the table construction that
 // pymicro_features.MicroFrontend() performs when the reference instantiates it at
 // microwakeword/audio/audio_utils.py:52 (window / KissFFT twiddles / mel filterbank weights /
 // PCAN gain LUT / log LUT; algorithm per SURVEY.md Appendix B).
@@ -24,7 +24,7 @@ constexpr int kFbCoefWords = 16 * (30 + 14 + 6);               // 800 int32 = 3 
 // (zero coefficients in front where the true first bin is odd or the start was moved down): the energies are fetched
 // two per 64-bit load, and the start words of the 16 lanes of a slot are chosen (bipartite matching at table-build
 // time, mww_tables.cc) so that (start / 2) mod 16 is a permutation -- no shared-memory bank conflict in the mel
-// accumulation (r01: 34 % of K1's shared-memory wavefronts were conflict replays, all of them in these loads).
+// accumulation (the natural layout puts the lanes of these loads on the same banks).
 constexpr int kEnergyOffset = 1;
 // Trip counts of the balanced filterbank schedule (mww_tables.cc LPT assignment), padded to even so the
 // Q12 coefficients can be fetched two per 32-bit load.  mww_create verifies the table builder agrees.

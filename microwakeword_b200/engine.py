@@ -1,4 +1,4 @@
-"""StreamEngine: many independent audio streams on one B200, behind the C-ABI of include/mww.h.
+"""StreamEngine: many independent audio streams on one H100, behind the C-ABI of include/mww.h.
 
 Host-side mirror of what the reference does one stream at a time:
   * frontend  ...... microwakeword/audio/audio_utils.py:50-64 (ProcessSamples loop)

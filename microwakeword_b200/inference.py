@@ -1,7 +1,7 @@
 """Drop-in for ``microwakeword.inference`` (reference: microwakeword/inference.py:25-170).
 
 Same class, same methods, same argument meaning and return types; the arithmetic runs in the
-sm_100a kernels of libmww_b200.so instead of tf.lite.Interpreter + pymicro_features.
+sm_90a kernels of libmww_b200.so instead of tf.lite.Interpreter + pymicro_features.
 
 Differences that are deliberate and documented (SURVEY.md Appendix D):
   * the model file is an MWW container (microwakeword_b200/model_file.py), not a .tflite flatbuffer --
@@ -25,7 +25,7 @@ from .model_file import FEATURE_SCALE, NUM_FEATURES
 
 class Model:
     """
-    Class for loading and running microwakeword streaming models on a B200
+    Class for loading and running microwakeword streaming models on an H100
 
     Args:
         tflite_model_path (str | bytes): Path to (or bytes of) a streaming ``.tflite`` model (microwakeword_b200/tflite_file.py)

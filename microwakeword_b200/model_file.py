@@ -2,7 +2,7 @@
 
 The reference loads a ``.tflite`` flatbuffer at ``microwakeword/inference.py:36-45``.  No
 TensorFlow / flatbuffers module and no ``.tflite`` file exist in this environment, so the
-B200 build carries its own little-endian tensor container holding exactly what the
+H100 build carries its own little-endian tensor container holding exactly what the
 streaming graph needs (SURVEY.md section 7 step 2):
 
     0   char  magic[8]  = b"MWWB200\\0"

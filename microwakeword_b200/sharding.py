@@ -43,9 +43,9 @@ def partition(n_streams: int, world: int, shares=None):
 
 def ingest_shares(n_streams: int, world: int, src: int = 0, src_share: float = 1.0):
     """Per-rank stream counts when all audio starts on rank `src`: the ingest rank takes `src_share` of an equal share
-    (0 = it only feeds the others), the rest is spread evenly over the other ranks.  Why: one GPU's NVLink egress
-    (about 840 GB/s measured) bounds how fast N - 1 peers can pull; once that bound exceeds a rank's compute time, the ingest
-    GPU's own kernels only slow its peers' reads of its memory (DESIGN.md section 5: total = pull + 0.6 x its compute time)."""
+    (0 = it only feeds the others), the rest is spread evenly over the other ranks.  Why: one GPU's NVLink egress bounds how
+    fast N - 1 peers can pull; once that bound exceeds a rank's compute time, the ingest GPU's own kernels only slow its
+    peers' reads of its memory."""
     if world < 1 or not 0 <= src < world or not 0.0 <= src_share <= 1.0:
         raise ValueError("bad ingest_shares arguments")
     if world == 1:

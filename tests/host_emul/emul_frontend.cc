@@ -1,7 +1,7 @@
 // tests/host_emul/emul_frontend.cc -- TEST INFRASTRUCTURE.
 //
 // Executes the product's frontend PHASE functions (microwakeword_b200/csrc/mww_frontend_dev.cuh --
-// the very code the sm_100a kernels run) on the CPU, thread by thread with barriers modelled as
+// the very code the sm_90a kernels run) on the CPU, thread by thread with barriers modelled as
 // "finish the phase for all 256 threads", so index math / bit-exactness can be validated against
 // the oracle in the GPU-less authoring container.  Never used by the product.
 #include <stdint.h>

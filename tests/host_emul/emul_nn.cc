@@ -492,7 +492,7 @@ extern "C" void emul_feature_qlut(float in_scale, int zp_in, int8_t *out65536) {
     memcpy(out65536, t.data(), t.size());
 }
 
-// ---- tcgen05 clip kernel: operand layout (mww_nn_tc_prep.h) ------------------------------------------------------
+// ---- wgmma clip kernel: operand layout (mww_nn_tc_prep.h) ------------------------------------------------------
 #include "../../microwakeword_b200/csrc/mww_nn_tc_prep.h"
 extern "C" unsigned emul_sw128_off(int row, int kk) { return sw128_off(row, kk); }
 // lays [K][N] weights out like mww_create does; returns the byte count (out may be NULL to query it)

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box).  Every call goes through the C-ABI of
+"""GPU parity tests (run with -m gpu on an H100).  Every call goes through the C-ABI of
 include/mww.h (via microwakeword_b200.engine / .inference) and is compared with the CPU oracle on the
 same seeded inputs and with the committed golden fixtures.
 
@@ -32,13 +32,13 @@ def _dev_u16(a, torch):
     return torch.from_numpy(np.ascontiguousarray(a).view(np.int16)).cuda().view(torch.uint16)
 
 
-def test_library_loaded_and_device_is_blackwell(torch_cuda):
+def test_library_loaded_and_device_is_hopper(torch_cuda):
     from microwakeword_b200 import _lib
     assert os.path.exists(_lib.SO_PATH)
     L = _lib.lib()
     for sym in _lib.EXPORTS:
         assert hasattr(L, sym)
-    assert torch_cuda.cuda.get_device_capability(0)[0] >= 10
+    assert torch_cuda.cuda.get_device_capability(0) == (9, 0)      # the library is built for sm_90a only
 
 
 def test_features_bit_exact_random_and_edge(torch_cuda):
@@ -166,7 +166,7 @@ def test_predict_spectrogram_dtypes_and_quirks(torch_cuda):
     a = np.asarray(m.predict_spectrogram(feats)); m.reset()
     b = np.asarray(m.predict_spectrogram(feats.astype(np.float32) * np.float32(0.0390625))); m.reset()
     c = np.asarray(m.predict_spectrogram(feats.astype(np.float64) * 0.0390625)); m.reset()
-    # 92 rows -> 30 chunks, 2 rows dropped.  uint16 rows take the tcgen05 clip kernel, float rows the mma.sync one: same values up
+    # 92 rows -> 30 chunks, 2 rows dropped.  uint16 rows take the wgmma clip kernel, float rows the mma.sync one: same values up
     # to the order of fp32 additions inside the two tensor-core paths; float32 and float64 rows are the same path, bit for bit
     assert len(a) == 30 and np.abs(a - b).max() <= 2e-6 and np.array_equal(b, c)
     assert m.predict_spectrogram(feats[:2]) == []

@@ -1,4 +1,4 @@
-"""CPU tests of the PRODUCT's kernel logic: the __host__ __device__ phase functions that the sm_100a
+"""CPU tests of the PRODUCT's kernel logic: the __host__ __device__ phase functions that the sm_90a
 kernels execute (microwakeword_b200/csrc/*_dev.cuh) are run thread-by-thread on the host
 (tests/host_emul) and compared with the oracle.  This is what lets index math and bit-exactness be
 iterated without a GPU; the GPU runs of the very same functions are in tests/test_gpu_parity.py."""
@@ -77,10 +77,9 @@ def test_frontend_phases_bit_exact_random_edge_and_adversarial():
 
 
 def test_filterbank_schedule_is_bank_conflict_free_and_complete():
-    """r01's ncu capture put every one of K1's shared-memory bank conflicts (34 % of its wavefronts) on the per-lane
-    energy loads of the mel accumulation.  The table builder now picks even start words whose (word / 2) mod 16 is a
-    permutation over the 16 lanes of a slot, so each 64-bit load of a half-warp (= one frame) covers the 32 banks exactly
-    once -- for the energies and for the int32 coefficient rows; and the shifted / padded spans still reproduce the
+    """The per-lane energy loads of the mel accumulation are where K1's shared-memory bank conflicts would sit.  The
+    table builder picks even start words whose (word / 2) mod 16 is a permutation over the 16 lanes of a slot, so each
+    64-bit load of a half-warp (= one frame) covers the 32 banks exactly once -- for the energies and for the int32 coefficient rows; and the shifted / padded spans still reproduce the
     triangular weights of every channel."""
     slots, coef = emul.fb_schedule()
     t = emul.tables()
@@ -200,8 +199,8 @@ def test_nn_int8_phases_bit_exact():
     assert np.array_equal(np.concatenate(parts, 1)[0], np.load(os.path.join(GOLDEN, "config0_probs_int8.npy")))
 
 
-def test_tcgen05_operand_layout_round_trips_and_is_a_swizzle_bijection():
-    """The tcgen05 clip kernel's shared-memory operand layout (mww_nn_tc_prep.h; GPU parity proves the kernel, this pins the
+def test_wgmma_operand_layout_round_trips_and_is_a_swizzle_bijection():
+    """The wgmma clip kernel's shared-memory operand layout (mww_nn_tc_prep.h; GPU parity proves the kernel, this pins the
     layout on the CPU): within a K-slot [rows][128 B] the swizzle permutes the eight 16-byte chunks of a row by (row & 7) --
     a bijection onto the slot, a row stays 128 contiguous bytes (the conflict-free store the kernel relies on); the weight
     planes read back through the same map give hi + lo == w exactly, hi is a TF32 (13 low mantissa bits clear), |lo| <= 2^-10 |w|,

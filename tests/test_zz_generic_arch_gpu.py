@@ -1,9 +1,6 @@
 """GPU side of the run-time-geometry MixedNet path (microwakeword_b200/csrc/mww_nn_generic.cu): models whose architecture
 differs from the compiled-in okay_nabu one, through the C-ABI (mww_create -> mww_infer_features / mww_predict_clip /
-mww_get_state), against the oracle.  The same phase functions are checked on the CPU in tests/test_generic_arch.py.
-
-This file sorts last on purpose: these kernels were written after the round's GPU budget was spent, so their first run on
-a real B200 is the driver's round-end `pytest -m gpu`; everything measured and profiled this round runs before them."""
+mww_get_state), against the oracle.  The same phase functions are checked on the CPU in tests/test_generic_arch.py."""
 
 import os
 

@@ -6,7 +6,7 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from bench import model_blob, synth_audio_device  # noqa: E402
+from bench import measured_peaks, model_blob, synth_audio_device  # noqa: E402
 from microwakeword_b200.engine import StreamEngine  # noqa: E402
 
 kind = sys.argv[1] if len(sys.argv) > 1 else "f32"
@@ -31,6 +31,7 @@ p = eng.profile_read()
 eb = 4 if kind == "f32" else 1
 step_bytes = 4176 * eb + 368 * eb + 240 + 4
 nn = p["mixednet"][0] / max(p["mixednet"][1], 1)
-print("%s mode=%s variant=%s: call %.4f ms, frontend %.4f, nn %.4f ms = %.0f GB/s (%.3f of 6576.7)" % (
+peak, peak_src = measured_peaks()
+print("%s mode=%s variant=%s: call %.4f ms, frontend %.4f, nn %.4f ms = %.0f GB/s (%.3f of %.0f GB/s, %s)" % (
     kind, os.environ.get("MWW_LIVE_MODE", "0"), os.environ.get("MWW_LIVE_VARIANT", "-"), a.elapsed_time(b) / calls, p["k1_spectral"][0] / calls, nn,
-    S * step_bytes / nn / 1e6, S * step_bytes / nn / 1e6 / 6576.7))
+    S * step_bytes / nn / 1e6, S * step_bytes / nn / 1e6 / peak, peak, peak_src))

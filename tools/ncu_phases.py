@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Attribute a kernel's executed instructions to barrier-delimited segments (phases) from an .ncu-rep source page.
-    python tools/ncu_phases.py gpurun_out/k1_v2.ncu-rep <units_in_launch>"""
+    python tools/ncu_phases.py k1_v2.ncu-rep <units_in_launch>"""
 import collections, csv, subprocess, sys
 rep, units = sys.argv[1], float(sys.argv[2])
 raw = subprocess.run(["ncu", "-i", rep, "--page", "source", "--csv"], capture_output=True, text=True).stdout

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (one kernel launch) into a small text file for profiles/.
+"""Summarise an .ncu-rep (one kernel launch) into a small text file.
 
-    python tools/ncu_summary.py gpurun_out/k1_full.ncu-rep profiles/r01_k1_full.txt [frames_in_launch]
+    python tools/ncu_summary.py k1_full.ncu-rep k1_full.txt [frames_in_launch]
 """
 import csv
 import json

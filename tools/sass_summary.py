@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Per-kernel SASS census of libmww_b200.so (cuobjdump -sass): registers are in the ptxas log, this lists which
-instruction families each kernel actually contains -- tensor-core (HMMA / IMMA / UTC*MMA), asynchronous copies (LDGSTS,
+instruction families each kernel actually contains -- tensor-core (HMMA / IMMA / HGMMA), asynchronous copies (LDGSTS,
 UBLKCP / UBLKPF, UTMALDG), barriers, 64/128-bit shared and global accesses -- so the claims in DESIGN.md can be checked
-against the binary.    python tools/sass_summary.py > profiles/r02_sass_summary.txt"""
+against the binary.    python tools/sass_summary.py"""
 import collections
 import os
 import re
@@ -11,7 +11,7 @@ import sys
 
 so = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "microwakeword_b200", "libmww_b200.so")
 out = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-FAMILIES = ["HMMA", "IMMA", "UTCHMMA", "UTCIMMA", "UTCQMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UBLKPF", "LDGSTS", "LDG", "STG", "LDS", "STS",
+FAMILIES = ["HMMA", "IMMA", "HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "UBLKPF", "LDGSTS", "LDG", "STG", "LDS", "STS",
             "BAR", "SYNCS", "FFMA", "IMAD", "DFMA", "MUFU", "SHFL", "REDUX", "ATOM"]
 kern, counts, total = None, collections.OrderedDict(), {}
 for line in out.splitlines():
@@ -34,7 +34,7 @@ for line in out.splitlines():
                 counts[kern][wide + (".128" if ".128" in op else ".64")] += 1
         if base == "HMMA" or base == "IMMA":
             counts[kern][op] += 1
-print("SASS census of %s (sm_100a)\n" % os.path.basename(so))
+print("SASS census of %s (sm_90a)\n" % os.path.basename(so))
 for k, c in counts.items():
     if total[k] < 50:
         continue
