@@ -9,6 +9,8 @@
 #include <cuda_runtime.h>
 #include <math.h>
 
+#include <algorithm>
+
 #include "../../include/mww.h"
 
 namespace {
@@ -20,16 +22,16 @@ __device__ __forceinline__ float window_mean(const float *p, int window) {
     return __fdiv_rn(s, (float)window);
 }
 
-// one thread per (track, output position)
+// one thread per (track, output position): tracks on grid x (up to 2^31 - 1 of them), positions on grid y and a grid stride
 __global__ void moving_average_kernel(const float *__restrict__ probs, const long long *__restrict__ offsets,
                                       const int *__restrict__ lengths, int n_tracks, int window, float *__restrict__ out,
                                       const long long *__restrict__ out_offsets) {
-    const int trk = blockIdx.y;
+    const int trk = blockIdx.x;
     if (trk >= n_tracks) return;
     const int n = lengths[trk] - window + 1;
     const float *p = probs + offsets[trk];
     float *o = out + out_offsets[trk];
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) o[i] = window_mean(p + i, window);
+    for (int i = blockIdx.y * blockDim.x + threadIdx.x; i < n; i += gridDim.y * blockDim.x) o[i] = window_mean(p + i, window);
 }
 
 // one thread per (track, cutoff): the cooldown chain is sequential in time (test.py:120-135)
@@ -73,7 +75,9 @@ int mww_moving_average(const float *d_probs, const long long *d_offsets, const i
                        float *d_out, const long long *d_out_offsets, void *cu_stream) {
     if (!d_probs || !d_offsets || !d_lengths || !d_out || !d_out_offsets || window < 1 || n_tracks < 0) return MWW_EINVAL;
     if (n_tracks == 0) return MWW_OK;
-    dim3 grid((unsigned)((max_length + 255) / 256 > 0 ? (max_length + 255) / 256 : 1), (unsigned)n_tracks);
+    // grid y is capped at 65 535 by CUDA: longer tracks are covered by the kernel's grid stride
+    const long long chunks = std::min(std::max(((long long)max_length + 255) / 256, 1ll), 65535ll);
+    dim3 grid((unsigned)n_tracks, (unsigned)chunks);
     moving_average_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(cu_stream)>>>(d_probs, d_offsets, d_lengths, n_tracks, window, d_out, d_out_offsets);
     return cudaGetLastError() == cudaSuccess ? MWW_OK : MWW_ECUDA;
 }

@@ -317,31 +317,6 @@ def test_errors_are_loud(torch_cuda):
         eng.features(torch_cuda.zeros((3, 480), dtype=torch_cuda.int16, device="cuda"))
 
 
-def test_full_size_properties(torch_cuda):
-    """BASELINE.json configs[1] scale (65 536 streams), checked through size-independent properties:
-    replicated streams give identical outputs, silence gives the model's fixed silence response,
-    a sample of streams matches the oracle, and chunked == whole."""
-    from microwakeword_b200.engine import StreamEngine
-    torch = torch_cuda
-    S, N = 65536, 4800
-    base = np.concatenate([np.stack([synth_audio(N, 600 + i) for i in range(60)]), edge_case_audio(N)[:4]])   # 64 distinct streams
-    reps = S // base.shape[0]
-    dev = torch.from_numpy(base).cuda().repeat(reps, 1)
-    blob = _blob("okay_nabu_synth_int8.mww")
-    eng = StreamEngine(blob, n_streams=S)
-    got = eng.predict_clip(dev)
-    assert got.shape == (S, 9)
-    g = got.view(reps, base.shape[0], 9)
-    assert bool((g == g[0:1]).all())                      # every replica identical -> no cross-stream leakage
-    _, want = oracle.run_pipeline(blob, base, want_features=False, threads=8)
-    assert np.array_equal(g[0].cpu().numpy(), want)
-    # chunked streaming at full size equals the whole-clip call
-    eng.reset()
-    a = eng.predict_clip(dev[:, :1760].contiguous())
-    b = eng.predict_clip(dev[:, 1760:].contiguous())
-    assert bool((torch.cat([a, b], 1) == got).all())
-
-
 def test_feature_extractor_only_config3(torch_cuda):
     """BASELINE.json configs[3]: 1 M 30 ms windows through the frontend alone, both layouts SURVEY.md 8(d) names --
     4 096 streams x 256 frames with carried state, and 1 048 576 stateless windows of 480 samples (the packed short-call
