@@ -12,6 +12,7 @@
  *   microwakeword/audio/audio_utils.py:69-81   frontend_op.audio_microfrontend(...)          -> mww_features
  *   microwakeword/inference.py:113-119  set_tensor / invoke / get_tensor, once per 30 ms      -> mww_infer_features
  *   microwakeword/inference.py:66-80    predict_clip (features + predict_spectrogram)         -> mww_predict_clip[_host]
+ *   microwakeword/audio/audio_utils.py:47-48   float clip -> int16 (x * 32768, clipped)      -> the *_f32 entry points
  *
  * Conventions
  *   - plain C types only; every d_* pointer is DEVICE memory on the handle's GPU (for PyTorch
@@ -118,6 +119,15 @@ int mww_set_window_step(mww_t *h, int hop_samples);
  * ((buffered + n_samples - 480) / 160 + 1 when that is >= 1, else 0).  Does not touch the NN state. */
 int mww_features(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride,
                  uint16_t *d_feat, int max_rows, int *h_rows_out, void *cu_stream);
+/* Same, with float32 audio (nominally in [-1, 1]) in device memory; audio_stride is in samples.  The
+ * frontend kernels convert each sample as the reference converts float clips (audio_utils.py:47-48):
+ * int16(trunc(clamp(x * 32768, -32768, 32767))) with the product in float32, NaN -> 0.  Results and
+ * state are bit-identical to mww_features on the converted samples, and the window buffer holds int16
+ * either way, so int16 and float32 calls may alternate on one handle.  Any pointer alignment and
+ * pitch work; a 16-byte-aligned buffer whose pitch, n_samples and buffered count are multiples of 8
+ * takes the vector loads. */
+int mww_features_f32(mww_t *h, const float *d_audio, int n_samples, long long audio_stride,
+                     uint16_t *d_feat, int max_rows, int *h_rows_out, void *cu_stream);
 
 /* NN only.  d_rows: [n_streams][n_rows][40] of `row_type`, stream pitch `rows_stride` rows.
  * Rows are appended to the pending rows; every full `input_feature_slices` rows run one model step.
@@ -129,6 +139,10 @@ int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, l
 /* Frontend + NN on device buffers (scratch features stay inside the library). */
 int mww_predict_clip(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride,
                      float *d_probs, int max_probs, int *h_probs_out, void *cu_stream);
+/* Same, with float32 device audio converted inside the frontend kernels (see mww_features_f32):
+ * probabilities and state are bit-identical to mww_predict_clip on the converted samples. */
+int mww_predict_clip_f32(mww_t *h, const float *d_audio, int n_samples, long long audio_stride,
+                         float *d_probs, int max_probs, int *h_probs_out, void *cu_stream);
 
 /* Same, from/to HOST buffers: the library tiles the streams, overlaps the host->device copy of one
  * tile with the kernels of the previous one, and returns when h_probs is complete.  Pinned host

@@ -23,7 +23,7 @@ EXPORTS = (
     "mww_moving_average", "mww_false_accept_counts", "mww_positive_scores", "mww_copy_async",
     "mww_ipc_alloc", "mww_ipc_open", "mww_ipc_close", "mww_ipc_free",
     "mww_predict_clip_remote", "mww_reset_device_ids", "mww_host_alloc", "mww_host_alloc_wc", "mww_host_free", "mww_bind_host_thread",
-    "mww_set_window_step",
+    "mww_set_window_step", "mww_features_f32", "mww_predict_clip_f32",
 )
 
 
@@ -78,6 +78,10 @@ def lib() -> ctypes.CDLL:
     L.mww_infer_features.argtypes = [vp, vp, i32, i32, ll, vp, i32, pi, vp]
     L.mww_predict_clip.restype = i32
     L.mww_predict_clip.argtypes = [vp, vp, i32, ll, vp, i32, pi, vp]
+    L.mww_features_f32.restype = i32
+    L.mww_features_f32.argtypes = [vp, vp, i32, ll, vp, i32, pi, vp]
+    L.mww_predict_clip_f32.restype = i32
+    L.mww_predict_clip_f32.argtypes = [vp, vp, i32, ll, vp, i32, pi, vp]
     L.mww_predict_clip_host.restype = i32
     L.mww_predict_clip_host.argtypes = [vp, vp, i32, ll, vp, i32, pi]
     L.mww_get_state.restype = i32

@@ -191,8 +191,10 @@ int tile_streams(const mww_t *h, int n_frames, bool need_feat) {
     return (int)t;
 }
 
-// frontend for streams [first, first+n): audio tile pointer is already offset to the tile's first stream
-int run_frontend_tile(mww_t *h, int first, int n, const int16_t *d_audio, long long audio_stride, int n_samples,
+// frontend for streams [first, first+n): audio tile pointer is already offset to the tile's first stream.  T = int16_t or
+// float (converted to int16 inside the kernels); everything after the frontend is the same for both.
+template <typename T>
+int run_frontend_tile(mww_t *h, int first, int n, const T *d_audio, long long audio_stride, int n_samples,
                       int n_frames, uint16_t *d_feat, long long feat_stream_stride, cudaStream_t st) {
     if (n_frames <= 0) return MWW_OK;
     if (h->hop != kHop) {
@@ -232,7 +234,8 @@ int run_frontend_tile(mww_t *h, int first, int n, const int16_t *d_audio, long l
     return MWW_OK;
 }
 
-int run_carry_tile(mww_t *h, int first, int n, const int16_t *d_audio, long long audio_stride, int n_samples, int n_frames,
+template <typename T>
+int run_carry_tile(mww_t *h, int first, int n, const T *d_audio, long long audio_stride, int n_samples, int n_frames,
                    cudaStream_t st) {
     const int consumed = n_frames * h->hop;
     const int new_used = h->used + n_samples - consumed;
@@ -621,6 +624,71 @@ void destroy_impl(mww_t *h) {
     delete h;
 }
 
+// mww_features / mww_features_f32
+template <typename T>
+int features_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
+                  int *h_rows_out, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    ENTER_STATEFUL(h);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    const int n_frames = frames_for(h, n_samples);
+    if (n_frames > max_rows || (n_frames > 0 && !d_feat))
+        return fail(h, MWW_EINVAL, std::string(who) + ": feature buffer too small for the rows this call emits");
+    const int tile = tile_streams(h, n_frames, false);
+    int rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), 0);
+    if (rc) return rc;
+    for (int first = 0; first < h->n_streams; first += tile) {
+        const int n = std::min(tile, h->n_streams - first);
+        rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames,
+                               d_feat + (size_t)first * max_rows * kNumChannels, (long long)max_rows * kNumChannels, st);
+        if (rc) return rc;
+    }
+    if (n_samples > 0) {
+        rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
+        if (rc) return rc;
+    }
+    h->used = h->used + n_samples - n_frames * h->hop;
+    if (h_rows_out) *h_rows_out = n_frames;
+    return MWW_OK;
+}
+
+// mww_predict_clip / mww_predict_clip_f32
+template <typename T>
+int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                      int *h_probs_out, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (!h->has_nn) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
+    ENTER_STATEFUL(h);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    const int n_frames = frames_for(h, n_samples);
+    const int n_steps = (h->n_pend + n_frames) / h->stride;
+    if (n_steps > max_probs || (n_steps > 0 && !d_probs)) return fail(h, MWW_EINVAL, std::string(who) + ": probability buffer too small");
+    const int tile = tile_streams(h, n_frames, true);
+    int rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
+    if (rc) return rc;
+    rc = begin_nn_call(h, n_frames, st);
+    if (rc) return rc;
+    for (int first = 0; first < h->n_streams; first += tile) {
+        const int n = std::min(tile, h->n_streams - first);
+        rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames, h->d_feat,
+                               (long long)n_frames * kNumChannels, st);
+        if (rc) return rc;
+        rc = run_nn_tile(h, first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, d_probs + (size_t)first * max_probs, max_probs, st);
+        if (rc) return rc;
+    }
+    end_nn_call(h, n_frames);
+    if (n_samples > 0) {
+        rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
+        if (rc) return rc;
+    }
+    h->used = h->used + n_samples - n_frames * h->hop;
+    h->n_pend = (h->n_pend + n_frames) % h->stride;
+    if (h_probs_out) *h_probs_out = n_steps;
+    return MWW_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -881,28 +949,20 @@ int mww_reset_frontend(mww_t *h, void *cu_stream) {
 
 int mww_features(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
                  int *h_rows_out, void *cu_stream) {
-    if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, "mww_features: bad audio arguments");
-    ENTER_STATEFUL(h);
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    const int n_frames = frames_for(h, n_samples);
-    if (n_frames > max_rows || (n_frames > 0 && !d_feat)) return fail(h, MWW_EINVAL, "mww_features: feature buffer too small for the rows this call emits");
-    const int tile = tile_streams(h, n_frames, false);
-    int rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), 0);
-    if (rc) return rc;
-    for (int first = 0; first < h->n_streams; first += tile) {
-        const int n = std::min(tile, h->n_streams - first);
-        rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames,
-                               d_feat + (size_t)first * max_rows * kNumChannels, (long long)max_rows * kNumChannels, st);
-        if (rc) return rc;
-    }
-    if (n_samples > 0) {
-        rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
-        if (rc) return rc;
-    }
-    h->used = h->used + n_samples - n_frames * h->hop;
-    if (h_rows_out) *h_rows_out = n_frames;
-    return MWW_OK;
+    return features_impl(h, "mww_features", d_audio, n_samples, audio_stride, d_feat, max_rows, h_rows_out, cu_stream);
+}
+int mww_features_f32(mww_t *h, const float *d_audio, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
+                     int *h_rows_out, void *cu_stream) {
+    return features_impl(h, "mww_features_f32", d_audio, n_samples, audio_stride, d_feat, max_rows, h_rows_out, cu_stream);
+}
+
+int mww_predict_clip(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                     int *h_probs_out, void *cu_stream) {
+    return predict_clip_impl(h, "mww_predict_clip", d_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
+}
+int mww_predict_clip_f32(mww_t *h, const float *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                         int *h_probs_out, void *cu_stream) {
+    return predict_clip_impl(h, "mww_predict_clip_f32", d_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
 }
 
 int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, long long rows_stride, float *d_probs,
@@ -920,40 +980,6 @@ int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, l
     if (rc == MWW_OK) end_nn_call(h, n_rows);
     if (rc) return rc;
     h->n_pend = (h->n_pend + n_rows) % h->stride;
-    if (h_probs_out) *h_probs_out = n_steps;
-    return MWW_OK;
-}
-
-int mww_predict_clip(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
-                     int *h_probs_out, void *cu_stream) {
-    if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, "mww_predict_clip: bad audio arguments");
-    if (!h->has_nn) return fail(h, MWW_EINVAL, "mww_predict_clip: frontend-only handle (created without a model)");
-    ENTER_STATEFUL(h);
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    const int n_frames = frames_for(h, n_samples);
-    const int n_steps = (h->n_pend + n_frames) / h->stride;
-    if (n_steps > max_probs || (n_steps > 0 && !d_probs)) return fail(h, MWW_EINVAL, "mww_predict_clip: probability buffer too small");
-    const int tile = tile_streams(h, n_frames, true);
-    int rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
-    if (rc) return rc;
-    rc = begin_nn_call(h, n_frames, st);
-    if (rc) return rc;
-    for (int first = 0; first < h->n_streams; first += tile) {
-        const int n = std::min(tile, h->n_streams - first);
-        rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames, h->d_feat,
-                               (long long)n_frames * kNumChannels, st);
-        if (rc) return rc;
-        rc = run_nn_tile(h, first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, d_probs + (size_t)first * max_probs, max_probs, st);
-        if (rc) return rc;
-    }
-    end_nn_call(h, n_frames);
-    if (n_samples > 0) {
-        rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
-        if (rc) return rc;
-    }
-    h->used = h->used + n_samples - n_frames * h->hop;
-    h->n_pend = (h->n_pend + n_frames) % h->stride;
     if (h_probs_out) *h_probs_out = n_steps;
     return MWW_OK;
 }

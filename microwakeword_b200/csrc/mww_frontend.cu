@@ -17,23 +17,35 @@ __device__ __forceinline__ void cp_async_commit_and_wait_all() {
     asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
 }
 
+// 8 caller samples -> 16 bytes of int16 staging.  int16 audio: one asynchronous copy.  float32 audio: two float4 loads
+// through registers, converted (pcm16_from_f32) and stored; the copy itself is then synchronous, the rest of the kernel is
+// unchanged.
+__device__ __forceinline__ void stage8(int16_t *dst, const int16_t *src) { cp_async16(dst, src); }
+__device__ __forceinline__ void stage8(int16_t *dst, const float *src) {
+    const float4 a = reinterpret_cast<const float4 *>(src)[0], b = reinterpret_cast<const float4 *>(src)[1];
+    *reinterpret_cast<uint4 *>(dst) = make_uint4(pack16(pcm16_from_f32(a.x), pcm16_from_f32(a.y)), pack16(pcm16_from_f32(a.z), pcm16_from_f32(a.w)),
+                                                 pack16(pcm16_from_f32(b.x), pcm16_from_f32(b.y)), pack16(pcm16_from_f32(b.z), pcm16_from_f32(b.w)));
+}
+
 // vectorised variant of k1_load_audio: valid when `used`, `n_samples` and the row pitch are multiples of 8
 // samples and both base pointers are 16-byte aligned, so no 8-sample vector straddles a source boundary
+template <typename T>
 __device__ __forceinline__ void k1_load_audio_async(int tid, K1Smem &sm, int buf, const int16_t *carry, int used,
-                                                    const int16_t *audio, int n_samples, int f0) {
+                                                    const T *audio, int n_samples, int f0) {
     const int base = kHop * f0;
     for (int v = tid; v < kGroupSamples / 8; v += kK1Threads) {
         const int vi = base + 8 * v;
         int16_t *dst = &sm.audio[buf][8 * v];
         if (vi < used) cp_async16(dst, carry + vi);
-        else if (vi - used < n_samples) cp_async16(dst, audio + (vi - used));
+        else if (vi - used < n_samples) stage8(dst, audio + (vi - used));
         else *reinterpret_cast<uint4 *>(dst) = make_uint4(0, 0, 0, 0);
     }
 }
 
 // vectorised variant of k1_packed_load_audio (same alignment conditions): 8 samples per 16-byte copy instead of one
 // 2-byte load + an integer division per sample
-__device__ __forceinline__ void k1_packed_load_audio_async(int tid, K1Smem &sm, const int16_t *carry, int used, const int16_t *audio,
+template <typename T>
+__device__ __forceinline__ void k1_packed_load_audio_async(int tid, K1Smem &sm, const int16_t *carry, int used, const T *audio,
                                                            long long audio_stride, int n_samples, long long s0, int n_streams, int spc, int fps) {
     const int span8 = (fps + 2) * (kHop / 8), used8 = used / 8, n8 = n_samples / 8;
     int16_t *dst0 = &sm.audio[0][0];
@@ -42,7 +54,7 @@ __device__ __forceinline__ void k1_packed_load_audio_async(int tid, K1Smem &sm, 
         int16_t *dst = dst0 + 8 * i;
         const long long s = s0 + sl;
         if (s < n_streams && v8 < used8) cp_async16(dst, carry + s * kWindow + 8 * v8);
-        else if (s < n_streams && v8 - used8 < n8) cp_async16(dst, audio + s * audio_stride + 8 * (v8 - used8));
+        else if (s < n_streams && v8 - used8 < n8) stage8(dst, audio + s * audio_stride + 8 * (v8 - used8));
         else *reinterpret_cast<uint4 *>(dst) = make_uint4(0, 0, 0, 0);
     }
 }
@@ -53,10 +65,11 @@ __device__ __forceinline__ void k1_packed_load_audio_async(int tid, K1Smem &sm, 
 // through HBM, no K2 launch, no scratch buffer.
 // kOcc = CTAs per SM the kernel is compiled for: 3 keeps the per-lane FFT twiddles in registers (80 registers), 4 reads them
 // from shared memory (64 registers).
-template <bool kFuseK2, int kOcc>
+// T = sample type of the caller's audio (int16_t or float) in this and every kernel below that reads it.
+template <bool kFuseK2, int kOcc, typename T>
 __global__ void __launch_bounds__(kK1Threads, kOcc)
 k1_spectral_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used,
-                   const int16_t *__restrict__ audio, long long audio_stride, int n_samples, int n_frames,
+                   const T *__restrict__ audio, long long audio_stride, int n_samples, int n_frames,
                    int groups_per_block, int vec_ok, uint32_t *__restrict__ vout, uint32_t *__restrict__ estimate,
                    uint16_t *__restrict__ feat, long long feat_stream_stride) {
     extern __shared__ __align__(16) unsigned char k1_smem_raw[];
@@ -73,7 +86,7 @@ k1_spectral_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used
     const int g_begin = blockIdx.y * groups_per_block;
     const int g_end = min(g_begin + groups_per_block, n_groups);
     const int16_t *my_carry = carry + s * kWindow;
-    const int16_t *my_audio = audio + s * audio_stride;
+    const T *my_audio = audio + s * audio_stride;
     uint32_t est = 0;                          // fused: thread ch < 40 carries channel ch's noise estimate across the groups
     if (kFuseK2 && tid < kNumChannels) est = estimate[s * kNumChannels + tid];
     if (g_begin < g_end) {
@@ -118,8 +131,9 @@ k1_spectral_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used
 // Run-time hop variant of the fused clip kernel (any even hop <= 480 samples, i.e. window_step up to 30 ms): one CTA per
 // stream, groups of k1_hop_frames_per_group(hop) frames, single-buffered audio staging.  Used only when the handle's hop is
 // not the 10 ms every shipped model uses; the 10 ms kernels above stay specialised.
+template <typename T>
 __global__ void __launch_bounds__(kK1Threads, 3)
-k1_spectral_hop_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used, const int16_t *__restrict__ audio,
+k1_spectral_hop_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used, const T *__restrict__ audio,
                        long long audio_stride, int n_samples, int n_frames, int hop, uint32_t *__restrict__ estimate,
                        uint16_t *__restrict__ feat, long long feat_stream_stride) {
     extern __shared__ __align__(16) unsigned char k1_smem_raw[];
@@ -132,7 +146,7 @@ k1_spectral_hop_kernel(FrontendParams P, const int16_t *__restrict__ carry, int 
     const int fpg = k1_hop_frames_per_group(hop);
     const int n_groups = (n_frames + fpg - 1) / fpg;
     const int16_t *my_carry = carry + s * kWindow;
-    const int16_t *my_audio = audio + s * audio_stride;
+    const T *my_audio = audio + s * audio_stride;
     uint32_t est = 0;
     if (tid < kNumChannels) est = estimate[s * kNumChannels + tid];
     for (int g = 0; g < n_groups; ++g) {
@@ -159,9 +173,10 @@ k1_spectral_hop_kernel(FrontendParams P, const int16_t *__restrict__ carry, int 
 
 // K1 for short calls (n_frames <= 8, e.g. the three frames of a 30 ms live step): one CTA = `spc` streams x `fps`
 // frames, so the 16 frame slots stay (almost) full instead of serving 3 of 16.
+template <typename T>
 __global__ void __launch_bounds__(kK1Threads, 3)
 k1_spectral_packed_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used,
-                          const int16_t *__restrict__ audio, long long audio_stride, int n_samples, int n_streams, int fps, int spc,
+                          const T *__restrict__ audio, long long audio_stride, int n_samples, int n_streams, int fps, int spc,
                           int vec_ok, uint32_t *__restrict__ vout) {
     extern __shared__ __align__(16) unsigned char k1_smem_raw[];
     K1Smem &sm = *reinterpret_cast<K1Smem *>(k1_smem_raw);
@@ -194,8 +209,9 @@ k1_spectral_packed_kernel(FrontendParams P, const int16_t *__restrict__ carry, i
 // K2 temporal chain (noise reduction -> PCAN -> log) straight from shared memory, then the carry update from the staged
 // audio.  Saves the V round trip through HBM and two launches per live step.  Requires new_used <= 2 hops (the staged
 // span ends 2 hops after the last frame's start) -- the launcher checks.
+template <typename T>
 __global__ void __launch_bounds__(kK1Threads, 3)
-k1k2_packed_kernel(FrontendParams P, int16_t *__restrict__ carry, int used, const int16_t *__restrict__ audio,
+k1k2_packed_kernel(FrontendParams P, int16_t *__restrict__ carry, int used, const T *__restrict__ audio,
                    long long audio_stride, int n_samples, int n_streams, int fps, int spc, int vec_ok, uint32_t *__restrict__ estimate,
                    uint16_t *__restrict__ feat, long long feat_stream_stride, int new_used) {
     extern __shared__ __align__(16) unsigned char k1_smem_raw[];
@@ -283,13 +299,15 @@ k2_temporal_kernel(FrontendParams P, const uint32_t *__restrict__ vin, int n_str
     estimate[idx] = est;
 }
 
-// carry update: keep the samples that did not complete a hop (one CTA of 128 threads per stream)
+// carry update: keep the samples that did not complete a hop (one CTA of 128 threads per stream); float audio is
+// converted, so the carry always holds int16 samples
+template <typename T>
 __global__ void __launch_bounds__(128)
-carry_update_kernel(int16_t *__restrict__ carry, int used, const int16_t *__restrict__ audio, long long audio_stride,
+carry_update_kernel(int16_t *__restrict__ carry, int used, const T *__restrict__ audio, long long audio_stride,
                     int n_samples, int consumed, int new_used) {
     const long long s = blockIdx.x;
     int16_t *c = carry + s * kWindow;
-    const int16_t *a = audio + s * audio_stride;
+    const T *a = audio + s * audio_stride;
     int16_t tmp[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
@@ -297,7 +315,7 @@ carry_update_kernel(int16_t *__restrict__ carry, int used, const int16_t *__rest
         int16_t val = 0;
         if (i < new_used) {
             const int vi = consumed + i;
-            val = vi < used ? c[vi] : a[vi - used];
+            val = vi < used ? c[vi] : pcm16(a[vi - used]);
         }
         tmp[q] = val;
     }
@@ -319,6 +337,13 @@ cudaError_t k1_opt_in(K kernel, bool (&done)[64]) {
     if (!first_launch_on_this_device(done)) return cudaSuccess;
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kK1SmemBytes);
 }
+// the 16-byte loaders (k1_load_audio_async) apply: 8-sample vectors never straddle the carry / audio boundary or a row end,
+// and both sources are 16-byte aligned (8 int16 samples = one cp.async, 8 float samples = two float4 loads)
+template <typename T>
+int audio_vec_ok(const int16_t *carry, int used, const T *audio, long long audio_stride, int n_samples) {
+    return (used % 8 == 0) && (n_samples % 8 == 0) && (audio_stride % 8 == 0) &&
+           (reinterpret_cast<uintptr_t>(audio) % 16 == 0) && (reinterpret_cast<uintptr_t>(carry) % 16 == 0);
+}
 }  // namespace
 
 bool frontend_clip_fuses(int n_streams, int n_frames, int sm_count) {
@@ -327,23 +352,23 @@ bool frontend_clip_fuses(int n_streams, int n_frames, int sm_count) {
     return n_frames > 8 && (long long)n_streams >= (long long)sm_count * 3 * 4;
 }
 
-cudaError_t launch_k1(const FrontendParams &P, const int16_t *carry, int used, const int16_t *audio,
+template <typename T>
+cudaError_t launch_k1(const FrontendParams &P, const int16_t *carry, int used, const T *audio,
                       long long audio_stride, int n_samples, int n_streams, int n_frames, uint32_t *vout, int sm_count,
                       cudaStream_t st) {
     if (n_frames <= 0 || n_streams <= 0) return cudaSuccess;
-    const int vec_ok = (used % 8 == 0) && (n_samples % 8 == 0) && (audio_stride % 8 == 0) &&
-                       (reinterpret_cast<uintptr_t>(audio) % 16 == 0) && (reinterpret_cast<uintptr_t>(carry) % 16 == 0);
+    const int vec_ok = audio_vec_ok(carry, used, audio, audio_stride, n_samples);
     if (n_frames <= 8 && n_streams >= 2) {
         static bool done[64] = {};
-        cudaError_t e = k1_opt_in(k1_spectral_packed_kernel, done);
+        cudaError_t e = k1_opt_in(k1_spectral_packed_kernel<T>, done);
         if (e != cudaSuccess) return e;
         const int spc = k1_packed_streams(n_frames);
         const unsigned grid = (unsigned)((n_streams + spc - 1) / spc);
-        k1_spectral_packed_kernel<<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_streams, n_frames, spc, vec_ok, vout);
+        k1_spectral_packed_kernel<T><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_streams, n_frames, spc, vec_ok, vout);
         return cudaGetLastError();
     }
     static bool done[64] = {};
-    cudaError_t e = k1_opt_in(k1_spectral_kernel<false, 3>, done);
+    cudaError_t e = k1_opt_in(k1_spectral_kernel<false, 3, T>, done);
     if (e != cudaSuccess) return e;
     const int n_groups = (n_frames + kFramesPerGroup - 1) / kFramesPerGroup;
     // enough CTAs to fill the chip a few times over, but keep per-CTA setup amortised when streams abound
@@ -353,41 +378,42 @@ cudaError_t launch_k1(const FrontendParams &P, const int16_t *carry, int used, c
     const int gpb = (n_groups + chunks - 1) / chunks;
     chunks = (n_groups + gpb - 1) / gpb;
     dim3 grid((unsigned)n_streams, (unsigned)chunks);
-    k1_spectral_kernel<false, 3><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, gpb, vec_ok, vout,
-                                                                      nullptr, nullptr, 0);
+    k1_spectral_kernel<false, 3, T><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, gpb, vec_ok, vout,
+                                                                         nullptr, nullptr, 0);
     return cudaGetLastError();
 }
 
-cudaError_t launch_frontend_clip_fused(const FrontendParams &P, const int16_t *carry, int used, const int16_t *audio, long long audio_stride,
+template <typename T>
+cudaError_t launch_frontend_clip_fused(const FrontendParams &P, const int16_t *carry, int used, const T *audio, long long audio_stride,
                                        int n_samples, int n_streams, int n_frames, uint32_t *estimate, uint16_t *feat, long long feat_stream_stride,
                                        cudaStream_t st) {
     if (n_frames <= 0 || n_streams <= 0) return cudaSuccess;
     static bool done3[64] = {}, done4[64] = {};
     static const int occ = getenv("MWW_K1_OCC") ? atoi(getenv("MWW_K1_OCC")) : 4;
-    cudaError_t e = occ == 3 ? k1_opt_in(k1_spectral_kernel<true, 3>, done3) : k1_opt_in(k1_spectral_kernel<true, 4>, done4);
+    cudaError_t e = occ == 3 ? k1_opt_in(k1_spectral_kernel<true, 3, T>, done3) : k1_opt_in(k1_spectral_kernel<true, 4, T>, done4);
     if (e != cudaSuccess) return e;
-    const int vec_ok = (used % 8 == 0) && (n_samples % 8 == 0) && (audio_stride % 8 == 0) &&
-                       (reinterpret_cast<uintptr_t>(audio) % 16 == 0) && (reinterpret_cast<uintptr_t>(carry) % 16 == 0);
+    const int vec_ok = audio_vec_ok(carry, used, audio, audio_stride, n_samples);
     const int n_groups = (n_frames + kFramesPerGroup - 1) / kFramesPerGroup;
     dim3 grid((unsigned)n_streams, 1u);
     if (occ == 3)
-        k1_spectral_kernel<true, 3><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, n_groups, vec_ok,
-                                                                            nullptr, estimate, feat, feat_stream_stride);
+        k1_spectral_kernel<true, 3, T><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, n_groups, vec_ok,
+                                                                               nullptr, estimate, feat, feat_stream_stride);
     else
-        k1_spectral_kernel<true, 4><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, n_groups, vec_ok,
-                                                                            nullptr, estimate, feat, feat_stream_stride);
+        k1_spectral_kernel<true, 4, T><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, n_groups, vec_ok,
+                                                                               nullptr, estimate, feat, feat_stream_stride);
     return cudaGetLastError();
 }
 
-cudaError_t launch_frontend_hop(const FrontendParams &P, const int16_t *carry, int used, const int16_t *audio, long long audio_stride,
+template <typename T>
+cudaError_t launch_frontend_hop(const FrontendParams &P, const int16_t *carry, int used, const T *audio, long long audio_stride,
                                 int n_samples, int n_streams, int n_frames, int hop, uint32_t *estimate, uint16_t *feat,
                                 long long feat_stream_stride, cudaStream_t st) {
     if (n_frames <= 0 || n_streams <= 0) return cudaSuccess;
     static bool done[64] = {};
-    cudaError_t e = k1_opt_in(k1_spectral_hop_kernel, done);
+    cudaError_t e = k1_opt_in(k1_spectral_hop_kernel<T>, done);
     if (e != cudaSuccess) return e;
-    k1_spectral_hop_kernel<<<(unsigned)n_streams, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, hop,
-                                                                                 estimate, feat, feat_stream_stride);
+    k1_spectral_hop_kernel<T><<<(unsigned)n_streams, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_frames, hop,
+                                                                                    estimate, feat, feat_stream_stride);
     return cudaGetLastError();
 }
 
@@ -396,19 +422,19 @@ bool frontend_fusable(int used, int n_samples, int n_frames) {
     return n_frames >= 1 && n_frames <= 8 && new_used >= 0 && new_used <= 2 * kHop;
 }
 
-cudaError_t launch_frontend_fused(const FrontendParams &P, int16_t *carry, int used, const int16_t *audio,
+template <typename T>
+cudaError_t launch_frontend_fused(const FrontendParams &P, int16_t *carry, int used, const T *audio,
                                   long long audio_stride, int n_samples, int n_streams, int n_frames, uint32_t *estimate, uint16_t *feat,
                                   long long feat_stream_stride, cudaStream_t st) {
     if (n_streams <= 0) return cudaSuccess;
     static bool done[64] = {};
-    cudaError_t e = k1_opt_in(k1k2_packed_kernel, done);
+    cudaError_t e = k1_opt_in(k1k2_packed_kernel<T>, done);
     if (e != cudaSuccess) return e;
-    const int vec_ok = (used % 8 == 0) && (n_samples % 8 == 0) && (audio_stride % 8 == 0) &&
-                       (reinterpret_cast<uintptr_t>(audio) % 16 == 0) && (reinterpret_cast<uintptr_t>(carry) % 16 == 0);
+    const int vec_ok = audio_vec_ok(carry, used, audio, audio_stride, n_samples);
     const int spc = k1_packed_streams(n_frames);
     const unsigned grid = (unsigned)((n_streams + spc - 1) / spc);
-    k1k2_packed_kernel<<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_streams, n_frames, spc, vec_ok,
-                                                    estimate, feat, feat_stream_stride, used + n_samples - n_frames * kHop);
+    k1k2_packed_kernel<T><<<grid, kK1Threads, kK1SmemBytes, st>>>(P, carry, used, audio, audio_stride, n_samples, n_streams, n_frames, spc, vec_ok,
+                                                                  estimate, feat, feat_stream_stride, used + n_samples - n_frames * kHop);
     return cudaGetLastError();
 }
 
@@ -421,11 +447,27 @@ cudaError_t launch_k2(const FrontendParams &P, const uint32_t *vin, int n_stream
     return cudaGetLastError();
 }
 
-cudaError_t launch_carry_update(int16_t *carry, int used, const int16_t *audio, long long audio_stride, int n_samples,
+template <typename T>
+cudaError_t launch_carry_update(int16_t *carry, int used, const T *audio, long long audio_stride, int n_samples,
                                 int n_streams, int consumed, int new_used, cudaStream_t st) {
     if (n_streams <= 0) return cudaSuccess;
-    carry_update_kernel<<<(unsigned)n_streams, 128, 0, st>>>(carry, used, audio, audio_stride, n_samples, consumed, new_used);
+    carry_update_kernel<T><<<(unsigned)n_streams, 128, 0, st>>>(carry, used, audio, audio_stride, n_samples, consumed, new_used);
     return cudaGetLastError();
 }
+
+// the two sample types the C-ABI accepts on device (mww_features / mww_predict_clip and their _f32 forms)
+#define MWW_FRONTEND_INSTANTIATE(T)                                                                                            \
+    template cudaError_t launch_k1<T>(const FrontendParams &, const int16_t *, int, const T *, long long, int, int, int, uint32_t *, \
+                                      int, cudaStream_t);                                                                      \
+    template cudaError_t launch_frontend_clip_fused<T>(const FrontendParams &, const int16_t *, int, const T *, long long, int, int, \
+                                                       int, uint32_t *, uint16_t *, long long, cudaStream_t);                 \
+    template cudaError_t launch_frontend_hop<T>(const FrontendParams &, const int16_t *, int, const T *, long long, int, int, int, \
+                                                int, uint32_t *, uint16_t *, long long, cudaStream_t);                        \
+    template cudaError_t launch_frontend_fused<T>(const FrontendParams &, int16_t *, int, const T *, long long, int, int, int,   \
+                                                  uint32_t *, uint16_t *, long long, cudaStream_t);                           \
+    template cudaError_t launch_carry_update<T>(int16_t *, int, const T *, long long, int, int, int, int, cudaStream_t);
+MWW_FRONTEND_INSTANTIATE(int16_t)
+MWW_FRONTEND_INSTANTIATE(float)
+#undef MWW_FRONTEND_INSTANTIATE
 
 }  // namespace mww

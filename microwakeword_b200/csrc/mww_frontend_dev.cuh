@@ -6,7 +6,7 @@
 // Work decomposition (GPU-first, not a translation of the scalar C library):
 //   * kernel K1 "spectral": every 10 ms frame is independent up to the filterbank sqrt, so a CTA of
 //     256 threads processes 16 frames of one stream at a time, 16 lanes per frame:
-//       P0  coalesced int16 loads of the 18-hop audio span into shared memory
+//       P0  coalesced loads of the 18-hop audio span into shared memory (float32 audio is converted to int16 on the way)
 //       P1  Q12 Hann window, packed int16x2, per-lane |max|
 //       P2  input scaling + radix-4 stages 1,2 of the 256-point complex FFT on 16 register-resident
 //           points per lane (bit-exact Q15 roundings of KissFFT FIXED_POINT=16)
@@ -185,15 +185,30 @@ MWW_HD void lane_tw4(const K1Lane &L, int i, int32_t &wr, int32_t &wi) { wr = L.
 MWW_HD void lane_tw3(const K1LaneShared &L, int q, int32_t &wr, int32_t &wi) { const uint32_t w = L.row[q]; wr = unpack_lo(w); wi = unpack_hi(w); }
 MWW_HD void lane_tw4(const K1LaneShared &L, int i, int32_t &wr, int32_t &wi) { const uint32_t w = L.row[3 + i]; wr = unpack_lo(w); wi = unpack_hi(w); }
 
+// ---------------------------------------------------------------------------------------------
+// Caller audio comes as int16 PCM or as float32 in [-1, 1].  A float sample becomes int16 the way the reference converts
+// float clips (audio_utils.py:47-48, np.clip(x * 32768, -32768, 32767).astype(np.int16)): the product in float32 (exact: a
+// power-of-two scale), clamped, truncated toward zero; NaN gives 0, as numpy's cast does on x86-64.  Every kernel converts
+// on load, so shared-memory staging, the window carry and all later phases only ever see int16.
+MWW_HD int16_t pcm16_from_f32(float x) {
+    const float y = x * 32768.0f;
+    if (y != y) return 0;
+    const float c = y < -32768.0f ? -32768.0f : (y > 32767.0f ? 32767.0f : y);
+    return (int16_t)(int32_t)c;
+}
+MWW_HD int16_t pcm16(int16_t v) { return v; }
+MWW_HD int16_t pcm16(float v) { return pcm16_from_f32(v); }
+
 // P0: bring the group's audio span into shared memory.  The stream's sample sequence is
 // carry[0 .. used) followed by audio[0 .. n_samples); group g needs samples [160*f0, 160*f0 + 2880).
-MWW_HD void k1_load_audio(int tid, K1Smem &sm, int buf, const int16_t *carry, int used, const int16_t *audio, int n_samples, int f0) {
+template <typename T>
+MWW_HD void k1_load_audio(int tid, K1Smem &sm, int buf, const int16_t *carry, int used, const T *audio, int n_samples, int f0) {
     const int base = kHop * f0;
     for (int i = tid; i < kGroupSamples; i += kK1Threads) {
         const int vi = base + i;
         int16_t s = 0;
         if (vi < used) s = carry[vi];
-        else if (vi - used < n_samples) s = audio[vi - used];
+        else if (vi - used < n_samples) s = pcm16(audio[vi - used]);
         sm.audio[buf][i] = s;
     }
 }
@@ -205,13 +220,14 @@ MWW_HD int k1_hop_frames_per_group(int hop) {
     const int by_span = (2 * kGroupSamples - kWindow) / hop + 1;
     return by_span < kFramesPerGroup ? by_span : kFramesPerGroup;
 }
-MWW_HD void k1_hop_load_audio(int tid, K1Smem &sm, const int16_t *carry, int used, const int16_t *audio, int n_samples, int base, int span) {
+template <typename T>
+MWW_HD void k1_hop_load_audio(int tid, K1Smem &sm, const int16_t *carry, int used, const T *audio, int n_samples, int base, int span) {
     int16_t *dst = &sm.audio[0][0];
     for (int i = tid; i < span; i += kK1Threads) {
         const int vi = base + i;
         int16_t s = 0;
         if (vi < used) s = carry[vi];
-        else if (vi - used < n_samples) s = audio[vi - used];
+        else if (vi - used < n_samples) s = pcm16(audio[vi - used]);
         dst[i] = s;
     }
 }
@@ -311,7 +327,8 @@ MWW_HD int k1_packed_streams(int fps) {
     const int by_smem = (2 * kGroupSamples) / ((fps + 2) * kHop);
     return by_slots < by_smem ? by_slots : by_smem;
 }
-MWW_HD void k1_packed_load_audio(int tid, K1Smem &sm, const int16_t *carry, int used, const int16_t *audio, long long audio_stride,
+template <typename T>
+MWW_HD void k1_packed_load_audio(int tid, K1Smem &sm, const int16_t *carry, int used, const T *audio, long long audio_stride,
                                  int n_samples, long long s0, int n_streams, int spc, int fps) {
     const int span = (fps + 2) * kHop;
     int16_t *dst = &sm.audio[0][0];
@@ -320,7 +337,7 @@ MWW_HD void k1_packed_load_audio(int tid, K1Smem &sm, const int16_t *carry, int 
         int16_t v = 0;
         if (s0 + sl < n_streams) {
             if (vi < used) v = carry[(s0 + sl) * kWindow + vi];
-            else if (vi - used < n_samples) v = audio[(s0 + sl) * audio_stride + (vi - used)];
+            else if (vi - used < n_samples) v = pcm16(audio[(s0 + sl) * audio_stride + (vi - used)]);
         }
         dst[i] = v;
     }

@@ -18,27 +18,34 @@ inline bool first_launch_on_this_device(bool (&done)[64]) {
     return true;
 }
 
-cudaError_t launch_k1(const FrontendParams &P, const int16_t *carry, int used, const int16_t *audio,
+// Every launcher that reads caller audio is instantiated for T = int16_t (PCM) and T = float (float32 in [-1, 1], converted
+// on load with pcm16_from_f32); the window carry is int16 either way, so calls of both types can follow each other.
+template <typename T>
+cudaError_t launch_k1(const FrontendParams &P, const int16_t *carry, int used, const T *audio,
                       long long audio_stride, int n_samples, int n_streams, int n_frames, uint32_t *vout, int sm_count,
                       cudaStream_t st);
 // long calls with enough streams for one CTA per stream: K1 + the temporal chain in one launch, features written directly
 // (no V scratch).  frontend_clip_fuses() is the predicate the C-ABI layer sizes its scratch with.
 bool frontend_clip_fuses(int n_streams, int n_frames, int sm_count);
-cudaError_t launch_frontend_clip_fused(const FrontendParams &P, const int16_t *carry, int used, const int16_t *audio, long long audio_stride,
+template <typename T>
+cudaError_t launch_frontend_clip_fused(const FrontendParams &P, const int16_t *carry, int used, const T *audio, long long audio_stride,
                                        int n_samples, int n_streams, int n_frames, uint32_t *estimate, uint16_t *feat, long long feat_stream_stride,
                                        cudaStream_t st);
 // any even hop <= 480 samples (window_step != 10 ms): K1 + temporal chain, one CTA per stream, features written directly
-cudaError_t launch_frontend_hop(const FrontendParams &P, const int16_t *carry, int used, const int16_t *audio, long long audio_stride,
+template <typename T>
+cudaError_t launch_frontend_hop(const FrontendParams &P, const int16_t *carry, int used, const T *audio, long long audio_stride,
                                 int n_samples, int n_streams, int n_frames, int hop, uint32_t *estimate, uint16_t *feat,
                                 long long feat_stream_stride, cudaStream_t st);
 // short calls (<= 8 frames per stream, <= 2 hops left over): K1 + K2 + carry update in one launch
 bool frontend_fusable(int used, int n_samples, int n_frames);
-cudaError_t launch_frontend_fused(const FrontendParams &P, int16_t *carry, int used, const int16_t *audio,
+template <typename T>
+cudaError_t launch_frontend_fused(const FrontendParams &P, int16_t *carry, int used, const T *audio,
                                   long long audio_stride, int n_samples, int n_streams, int n_frames, uint32_t *estimate, uint16_t *feat,
                                   long long feat_stream_stride, cudaStream_t st);
 cudaError_t launch_k2(const FrontendParams &P, const uint32_t *vin, int n_streams, int n_frames, uint32_t *estimate,
                       uint16_t *feat, long long feat_stream_stride, cudaStream_t st);
-cudaError_t launch_carry_update(int16_t *carry, int used, const int16_t *audio, long long audio_stride, int n_samples,
+template <typename T>
+cudaError_t launch_carry_update(int16_t *carry, int used, const T *audio, long long audio_stride, int n_samples,
                                 int n_streams, int consumed, int new_used, cudaStream_t st);
 
 }  // namespace mww

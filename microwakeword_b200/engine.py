@@ -132,12 +132,16 @@ class StreamEngine:
         return int(self._L.mww_launch_count(self._h))
 
     def _check_audio(self, audio):
+        """-> (n_samples, row pitch in samples, is_float32).  float32 audio is converted to int16 inside the frontend kernels,
+        exactly as audio_utils.to_int16 converts it on the host; other float dtypes are refused (float64 keeps its exact host
+        conversion: rounding it to float32 first could move a sample across an integer boundary after the x 32768)."""
         torch = _torch()
-        if audio.dtype != torch.int16 or audio.dim() != 2 or audio.shape[0] != self.n_streams or not audio.is_cuda:
-            raise ValueError("audio must be a CUDA int16 tensor of shape [n_streams=%d, n_samples]" % self.n_streams)
+        if (audio.dtype not in (torch.int16, torch.float32) or audio.dim() != 2 or audio.shape[0] != self.n_streams
+                or not audio.is_cuda):
+            raise ValueError("audio must be a CUDA int16 or float32 tensor of shape [n_streams=%d, n_samples]" % self.n_streams)
         if audio.stride(1) != 1 and audio.shape[1] > 1:
             raise ValueError("audio samples must be contiguous along the last dimension")
-        return audio.shape[1], (audio.stride(0) if audio.shape[1] > 0 else 0)
+        return audio.shape[1], (audio.stride(0) if audio.shape[1] > 0 else 0), audio.dtype == torch.float32
 
     # ------------------------------------------------------------------ operations
     def reset(self, stream_ids=None):
@@ -166,9 +170,9 @@ class StreamEngine:
         _lib.check(self._h, self._L.mww_reset_frontend(self._h, self._cu_stream()))
 
     def features(self, audio, out=None):
-        """int16 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer."""
+        """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer."""
         torch = _torch()
-        n, stride = self._check_audio(audio)
+        n, stride, is_f32 = self._check_audio(audio)
         rows = max((self.frontend_buffered + n - WINDOW) // self.hop + 1, 0) if self.frontend_buffered + n >= WINDOW else 0
         if out is None:
             out = torch.empty((self.n_streams, max(rows, 1), NUM_FEATURES), dtype=torch.uint16, device=self._dev())
@@ -176,8 +180,8 @@ class StreamEngine:
               or out.shape[1] < max(rows, 1) or out.shape[2] != NUM_FEATURES):
             raise ValueError("out must be a contiguous CUDA uint16 tensor [n_streams, >= rows, 40]")
         got = ctypes.c_int(0)
-        _lib.check(self._h, self._L.mww_features(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1],
-                                                 ctypes.byref(got), self._cu_stream()))
+        fn = self._L.mww_features_f32 if is_f32 else self._L.mww_features
+        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
     def infer(self, rows):
@@ -196,17 +200,18 @@ class StreamEngine:
         return probs[:, :got.value]
 
     def predict_clip(self, audio, out=None):
-        """int16 CUDA tensor [S, N] -> float32 probabilities [S, steps]; state carries over between calls."""
+        """int16 or float32 CUDA tensor [S, N] -> float32 probabilities [S, steps]; state carries over between calls.  float32
+        samples are converted to int16 inside the frontend kernels (x * 32768, clipped, as audio_utils.to_int16)."""
         torch = _torch()
-        n, stride = self._check_audio(audio)
+        n, stride, is_f32 = self._check_audio(audio)
         buffered = self.frontend_buffered
         rows = (buffered + n - WINDOW) // self.hop + 1 if buffered + n >= WINDOW else 0
         steps = (self.pending_rows + rows) // self.stride
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
         got = ctypes.c_int(0)
-        _lib.check(self._h, self._L.mww_predict_clip(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1],
-                                                     ctypes.byref(got), self._cu_stream()))
+        fn = self._L.mww_predict_clip_f32 if is_f32 else self._L.mww_predict_clip
+        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
     step = predict_clip  # the live "one chunk of new audio per call" surface (north_star step())

@@ -129,7 +129,8 @@ class Model:
 
     # ------------------------------------------------------------------ many-stream extension (north_star step surface)
     def step(self, audio):
-        """Feed new audio for every stream: int16 [batch, n] (numpy or CUDA tensor) -> probabilities [batch, steps].
+        """Feed new audio for every stream: int16 [batch, n] (numpy or CUDA tensor; a CUDA tensor may also be float32 in [-1, 1],
+        converted on the GPU as to_int16 converts it) -> probabilities [batch, steps].
         n is typically 480 (one 30 ms model step); state carries over between calls."""
         torch = _torch()
         if isinstance(audio, np.ndarray):
