@@ -24,14 +24,53 @@ constexpr int kFftSize = 512;
 constexpr int kNcfft = 256;           // complex length of the packed real FFT
 constexpr float kFeatureScale = 0.0390625f;   // inference.py:94
 
-// 1-based index of the highest set bit, 0 for x == 0
-MWW_HD int msb32(uint32_t x) {
+// leading zero bits, 32 for x == 0
+MWW_HD int clz32(uint32_t x) {
 #if defined(__CUDA_ARCH__)
-    return 32 - __clz((int)x);
+    return __clz((int)x);
 #else
-    return x ? 32 - __builtin_clz(x) : 0;
+    return x ? __builtin_clz(x) : 32;
 #endif
 }
+
+// 1-based index of the highest set bit, 0 for x == 0
+MWW_HD int msb32(uint32_t x) { return 32 - clz32(x); }
+
+// The helpers below have a host form and a device intrinsic form.  The CPU tests (tests/test_frontend_scalar_forms.py,
+// tests/test_host_emul.py) run the host forms; the device forms are covered by the GPU parity tests, which compare the
+// kernels' features bit for bit with the oracle.
+
+// x << s for 0 <= s <= 33, zero once s >= 32 (one clamped funnel shift on the device)
+MWW_HD uint32_t shl_clamp32(uint32_t x, int s) {
+#if defined(__CUDA_ARCH__)
+    return __funnelshift_lc(0u, x, (unsigned)s);
+#else
+    return (uint32_t)((uint64_t)x << s);
+#endif
+}
+
+// high word of the signed 32 x 32 -> 64-bit product (IMAD.HI)
+MWW_HD int32_t mulhi_s32(int32_t a, int32_t b) {
+#if defined(__CUDA_ARCH__)
+    return __mulhi(a, b);
+#else
+    return (int32_t)(((int64_t)a * (int64_t)b) >> 32);
+#endif
+}
+
+// per-halfword unsigned maximum of two packed uint16 pairs
+MWW_HD uint32_t vmax_u16x2(uint32_t a, uint32_t b) {
+#if defined(__CUDA_ARCH__)
+    return __vmaxu2(a, b);
+#else
+    const uint32_t lo = (a & 0xFFFFu) > (b & 0xFFFFu) ? (a & 0xFFFFu) : (b & 0xFFFFu);
+    const uint32_t hi = (a >> 16) > (b >> 16) ? (a >> 16) : (b >> 16);
+    return lo | (hi << 16);
+#endif
+}
+
+// two int32 values that one 64-bit shared-memory access moves together
+struct alignas(8) Int2 { int32_t x, y; };
 
 MWW_HD int32_t sext16(int32_t v) { return (int32_t)(int16_t)v; }
 

@@ -130,9 +130,11 @@ k1_spectral_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used
 
 // Run-time hop variant of the fused clip kernel (any even hop <= 480 samples, i.e. window_step up to 30 ms): one CTA per
 // stream, groups of k1_hop_frames_per_group(hop) frames, single-buffered audio staging.  Used only when the handle's hop is
-// not the 10 ms every shipped model uses; the 10 ms kernels above stay specialised.
+// not the 10 ms every shipped model uses; the 10 ms kernels above stay specialised.  72 registers (launched with 256 threads):
+// three CTAs per SM, as the shared memory allows.  nvcc rejects __launch_bounds__ and __maxnreg__ on the same kernel, so the
+// block size is not declared here; launch_frontend_hop is its only launcher and always uses kK1Threads.
 template <typename T>
-__global__ void __launch_bounds__(kK1Threads, 3)
+__global__ void __maxnreg__(72)
 k1_spectral_hop_kernel(FrontendParams P, const int16_t *__restrict__ carry, int used, const T *__restrict__ audio,
                        long long audio_stride, int n_samples, int n_frames, int hop, uint32_t *__restrict__ estimate,
                        uint16_t *__restrict__ feat, long long feat_stream_stride) {

@@ -19,6 +19,8 @@
 // All functions are __host__ __device__: tests/host_emul runs them thread by thread on the CPU.
 #pragma once
 
+#include <stddef.h>
+
 #include "mww_common.h"
 #include "mww_tables.h"
 
@@ -34,25 +36,34 @@ constexpr int kRowWords = 272;   // 256 + 16: two frames of one warp land in dis
 constexpr int kGroupSamples = (kFramesPerGroup + 2) * kHop;   // 2880
 
 
+// The per-lane constants of the FFT phases (window, post-pass and stage-3/4 twiddles) are kept here UNPACKED, one Int2 per
+// value pair: a 64-bit load hands both halves to the multiplies with no PRMT / SHF in between, once per group and lane.
 struct K1Smem {
     uint32_t A[kFramesPerGroup][kRowWords];
     uint32_t B[kFramesPerGroup][kRowWords];
+    Int2 win16[240];                   // window pair p: (w[2p] << 4, w[2p+1] << 4), the scale k1_window_fft1's mulhi_s32 wants
+    Int2 super_tw[128];                // real-FFT post-pass twiddles (re, im)
+    Int2 lane_tw[16][15];              // stage-3 / stage-4 twiddles of lane b (re, im), see K1LaneShared
     int16_t audio[2][kGroupSamples];   // double buffered: group g+1 is prefetched (cp.async) while g is processed
     uint16_t lane_max[kFramesPerGroup][16];
     int32_t shift[kFramesPerGroup];
     int32_t fb_coef[kFbCoefWords];     // span coefficients, [slot][lane][stride] (mww_tables.h)
     int16_t gain_lut[128];             // PCAN / log tables for the temporal chain fused behind the filterbank
     uint16_t log_lut[132];
-    uint32_t lane_tw[16][15];          // stage-3 / stage-4 twiddles of lane b (packed re | im << 16), see K1LaneShared
 };
-// 50.6 KB: above the 48 KB static limit, so the kernels take it as dynamic shared memory (opt-in per kernel and device)
+// 54.2 KB: above the 48 KB static limit, so the kernels take it as dynamic shared memory (opt-in per kernel and device);
+// four CTAs (plus 1 KB reserved each) still fit the H100's 228 KB per SM
 constexpr int kK1SmemBytes = (int)sizeof(K1Smem);
+static_assert(4 * (sizeof(K1Smem) + 1024) <= 228 * 1024, "K1Smem: four CTAs per SM");
+static_assert(offsetof(K1Smem, audio) % 16 == 0 && offsetof(K1Smem, lane_max) % 16 == 0, "K1Smem: 16-byte staging and lane_max rows");
 
 // tables every K1-family kernel keeps in shared memory for its whole lifetime
 MWW_HD void k1_stage_tables(int tid, K1Smem &sm, const FrontendParams &P) {
     for (int i = tid; i < kFbCoefWords; i += kK1Threads) sm.fb_coef[i] = P.fb_coef[i];
     for (int i = tid; i < 128; i += kK1Threads) sm.gain_lut[i] = P.gain_lut[i];
     for (int i = tid; i < 132; i += kK1Threads) sm.log_lut[i] = P.log_lut[i];
+    for (int i = tid; i < 240; i += kK1Threads) { const uint32_t w = P.win_pairs[i]; sm.win16[i] = Int2{unpack_lo(w) << 4, unpack_hi(w) << 4}; }
+    for (int i = tid; i < 128; i += kK1Threads) { const uint32_t w = P.super_tw[i]; sm.super_tw[i] = Int2{unpack_lo(w), unpack_hi(w)}; }
 }
 
 // per-thread constants that do not depend on the frame (kept in registers across groups)
@@ -61,9 +72,9 @@ struct K1Lane {
     int32_t t4r[12], t4i[12];   // stage-4 twiddles tw[k'], tw[2k'], tw[3k'] for k' = 16j + b
 };
 
-// The same constants read from shared memory where they are used (15 conflict-free LDS per group) instead of living in 30
-// registers: the clip kernel then fits 64 registers = 4 CTAs per SM (more resident warps for an issue-bound kernel).
-struct K1LaneShared { const uint32_t *row; };   // &sm.lane_tw[b][0]: [0..3) stage 3, [3 + 3j + q] stage 4
+// The same constants read from shared memory where they are used (15 conflict-free 64-bit LDS per group) instead of living
+// in 30 registers: the clip kernel then fits 64 registers = 4 CTAs per SM (more resident warps for an issue-bound kernel).
+struct K1LaneShared { const Int2 *row; };   // &sm.lane_tw[b][0]: [0..3) stage 3, [3 + 3j + q] stage 4
 
 // ---------------------------------------------------------------------------------------------
 // Q15 primitives of KissFFT FIXED_POINT=16
@@ -142,8 +153,7 @@ MWW_HD uint32_t isqrt64_round(uint64_t x) {
 // RSQ64H seed + two Newton steps + an exact integer check, all of a lane's roots in one block) -- the extra
 // instructions cost more than the slow-path branch of sqrt() and the serial FP64 chains.  x >= 2^48 -- only reachable through the library's int32 view of an energy of
 // exactly 2^31 -- takes the integer routine above.
-MWW_HD uint32_t isqrt64_round_fast(uint64_t x) {
-    if (x >> 48) return isqrt64_round(x);
+MWW_HD uint32_t isqrt64_round_below48(uint64_t x) {   // x < 2^48
 #if defined(__CUDA_ARCH__)
     const uint32_t r = __double2uint_rz(sqrt(__ull2double_rn(x)) + 0.5);
 #else
@@ -152,6 +162,7 @@ MWW_HD uint32_t isqrt64_round_fast(uint64_t x) {
     const uint32_t cap = (x >> 32) == 0 ? 0xFFFFu : 0xFFFFFFFFu;      // the library's 32-bit fast path saturates at 0xFFFF
     return r > cap ? cap : r;
 }
+MWW_HD uint32_t isqrt64_round_fast(uint64_t x) { return (x >> 48) ? isqrt64_round(x) : isqrt64_round_below48(x); }
 
 // ---------------------------------------------------------------------------------------------
 // K1 phases
@@ -177,13 +188,14 @@ MWW_HD void k1_stage_lane_twiddles(int tid, K1Smem &sm, const FrontendParams &P)
         int idx;
         if (e < 3) idx = 4 * b * (e + 1);
         else { const int j = (e - 3) / 3, q = (e - 3) - 3 * j; idx = (16 * j + b) * (q + 1); }
-        sm.lane_tw[b][e] = P.tw[idx];
+        const uint32_t w = P.tw[idx];
+        sm.lane_tw[b][e] = Int2{unpack_lo(w), unpack_hi(w)};
     }
 }
 MWW_HD void lane_tw3(const K1Lane &L, int q, int32_t &wr, int32_t &wi) { wr = L.t3r[q]; wi = L.t3i[q]; }
 MWW_HD void lane_tw4(const K1Lane &L, int i, int32_t &wr, int32_t &wi) { wr = L.t4r[i]; wi = L.t4i[i]; }
-MWW_HD void lane_tw3(const K1LaneShared &L, int q, int32_t &wr, int32_t &wi) { const uint32_t w = L.row[q]; wr = unpack_lo(w); wi = unpack_hi(w); }
-MWW_HD void lane_tw4(const K1LaneShared &L, int i, int32_t &wr, int32_t &wi) { const uint32_t w = L.row[3 + i]; wr = unpack_lo(w); wi = unpack_hi(w); }
+MWW_HD void lane_tw3(const K1LaneShared &L, int q, int32_t &wr, int32_t &wi) { const Int2 w = L.row[q]; wr = w.x; wi = w.y; }
+MWW_HD void lane_tw4(const K1LaneShared &L, int i, int32_t &wr, int32_t &wi) { const Int2 w = L.row[3 + i]; wr = w.x; wi = w.y; }
 
 // ---------------------------------------------------------------------------------------------
 // Caller audio comes as int16 PCM or as float32 in [-1, 1].  A float sample becomes int16 the way the reference converts
@@ -259,9 +271,12 @@ MWW_HD void k1_window_fft1(int tid, K1Smem &sm, int buf, int pair_base, const Fr
             if (j == 15) { xr[b] = 0; xi[b] = 0; continue; }        // samples 480..511 are the zero padding
             const int p = c + 16 * j;
             const uint32_t sw = pairs[p];
-            const uint32_t cw = P.win_pairs[p];
-            const int32_t v0 = (unpack_lo(sw) * unpack_lo(cw)) >> 12;   // |s| <= 32768, c <= 4096: fits int16
-            const int32_t v1 = (unpack_hi(sw) * unpack_hi(cw)) >> 12;
+            const Int2 cw = sm.win16[p];
+            // (s * w) >> 12 as the high word of (s << 16) * (w << 4): the sample stays in its half of the packed word
+            // (s << 16 is exact for int16 s, w <= 4096), and the high word is the floor, like the arithmetic shift.
+            // |s| <= 32768, w <= 4096: fits int16
+            const int32_t v0 = mulhi_s32((int32_t)(sw << 16), cw.x);
+            const int32_t v1 = mulhi_s32((int32_t)(sw & 0xFFFF0000u), cw.y);
             xr[b] = v0; xi[b] = v1;
             if (j == 7) {
                 const int32_t m0 = v0 == -32768 ? 0 : v0, m1 = v1 == -32768 ? 0 : v1;
@@ -277,10 +292,21 @@ MWW_HD void k1_window_fft1(int tid, K1Smem &sm, int buf, int pair_base, const Fr
     if (PART == 2) __syncwarp();
 #endif
     if (PART == 0) return;
-    int32_t mxa = 0;
+    // the 16 lane maxima (each <= 32767) as packed pairs: two 128-bit loads and packed maxima
+    uint32_t m2 = 0;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) { const int32_t v = sm.lane_max[fl][i]; mxa = v > mxa ? v : mxa; }
-    const int shift = 15 - msb32((uint32_t)mxa);
+    for (int h = 0; h < 2; ++h) {
+        uint32_t q[4];
+#if defined(__CUDA_ARCH__)
+        const uint4 v = reinterpret_cast<const uint4 *>(sm.lane_max[fl])[h];
+        q[0] = v.x; q[1] = v.y; q[2] = v.z; q[3] = v.w;
+#else
+        for (int i = 0; i < 4; ++i) q[i] = (uint32_t)sm.lane_max[fl][8 * h + 2 * i] | ((uint32_t)sm.lane_max[fl][8 * h + 2 * i + 1] << 16);
+#endif
+        m2 = vmax_u16x2(m2, vmax_u16x2(vmax_u16x2(q[0], q[1]), vmax_u16x2(q[2], q[3])));
+    }
+    const uint32_t mxa = (m2 & 0xFFFFu) > (m2 >> 16) ? (m2 & 0xFFFFu) : (m2 >> 16);
+    const int shift = 15 - msb32(mxa);
     if (a == 0) sm.shift[fl] = shift;
     // stage 1 (m = 1): unit twiddles; C_MUL by (32767, 0) is the identity on the pre-divided range.
     // The input scaling int16(uint16(v) << shift) is folded into C_FIXDIV's multiplier: v << shift cannot leave
@@ -397,16 +423,19 @@ MWW_HD void k1_real_energy(int tid, K1Smem &sm, const FrontendParams &P) {
         const int k = 1 + 16 * t + l;
         const uint32_t wk = sm.A[fl][k];
         const uint32_t wn = sm.A[fl][kNcfft - k];
-        const uint32_t ws = P.super_tw[k - 1];
+        const Int2 ws = sm.super_tw[k - 1];
         const int32_t pr = fixdiv2(unpack_lo(wk)), pi = fixdiv2(unpack_hi(wk));
         const int32_t nr = fixdiv2(unpack_lo(wn)), ni = fixdiv2(sext16(-unpack_hi(wn)));
         const int32_t f1r = pr + nr, f1i = pi + ni;          // |.| <= 2*16383: no wrap
         const int32_t f2r = pr - nr, f2i = pi - ni;
         int32_t tr, ti;
-        cmul_q15(f2r, f2i, unpack_lo(ws), unpack_hi(ws), tr, ti);
+        cmul_q15(f2r, f2i, ws.x, ws.y, tr, ti);
         tr = sext16(tr); ti = sext16(ti);                    // C_MUL stores into int16
-        const int32_t ar = sext16((f1r + tr) >> 1), ai = sext16((f1i + ti) >> 1);
-        const int32_t br = sext16((f1r - tr) >> 1), bi = sext16((ti - f1i) >> 1);
+        // The library stores these halves as int16, but no wrap can happen: C_FIXDIV(., 2) of an int16 lies in
+        // [-16383, 16383], so |f1| <= 32766, and t is an int16, so f1 +- t lies in [-65534, 65534] and its half in
+        // [-32767, 32767].
+        const int32_t ar = (f1r + tr) >> 1, ai = (f1i + ti) >> 1;
+        const int32_t br = (f1r - tr) >> 1, bi = (ti - f1i) >> 1;
         sm.B[fl][k + kEnergyOffset] = (uint32_t)(ar * ar) + (uint32_t)(ai * ai);
         sm.B[fl][kNcfft - k + kEnergyOffset] = (uint32_t)(br * br) + (uint32_t)(bi * bi);   // for k = 128 this (later) store wins, as in the library
     }
@@ -423,35 +452,54 @@ MWW_HD Pair32 load_pair(const uint32_t *p) {
     return Pair32{p[0], p[1]};
 #endif
 }
+MWW_HD int64_t k1_fb_accumulate(const K1Smem &sm, int fl, const FbSlot &slot, int len) {
+    int64_t acc = 0;
+    const uint32_t *e = &sm.B[fl][slot.word0];
+    const uint32_t *cf = reinterpret_cast<const uint32_t *>(&sm.fb_coef[slot.coef_off]);
+#pragma unroll
+    for (int j = 0; j < len / 2; ++j) {
+        const Pair32 ev = load_pair(e + 2 * j), cv = load_pair(cf + 2 * j);
+        // energy widened as int32, like the library
+        acc = mad_wide_s32((int32_t)ev.x, (int32_t)cv.x, acc);
+        acc = mad_wide_s32((int32_t)ev.y, (int32_t)cv.y, acc);
+    }
+    return acc;
+}
 MWW_HD void k1_filterbank(int tid, K1Smem &sm, const FrontendParams &P, uint32_t *vout_frame /* [40] or nullptr */) {
     const int fl = tid >> 4, l = tid & 15;
     const int sh = sm.shift[fl];
+    // An accumulator >= 2^48 needs the integer square root, and it takes a full-scale energy to make one.  The common path
+    // takes the double root for every channel; if any lane of the warp met such an accumulator, the warp recomputes its
+    // channels with the exact routine.  One vote per frame instead of a branch per channel.
+    bool big = false;
 #pragma unroll
     for (int s = 0; s < kFbSlots; ++s) {
         if (fb_len(s) == 0) continue;
         const FbSlot slot = P.fb_slots[l * kFbSlots + s];
-        int64_t acc = 0;
-        const uint32_t *e = &sm.B[fl][slot.word0];
-        const uint32_t *cf = reinterpret_cast<const uint32_t *>(&sm.fb_coef[slot.coef_off]);
-#pragma unroll
-        for (int j = 0; j < fb_len(s) / 2; ++j) {
-            const Pair32 ev = load_pair(e + 2 * j), cv = load_pair(cf + 2 * j);
-            // energy widened as int32, like the library
-            acc = mad_wide_s32((int32_t)ev.x, (int32_t)cv.x, acc);
-            acc = mad_wide_s32((int32_t)ev.y, (int32_t)cv.y, acc);
-        }
-        if (slot.ch >= 0 && vout_frame) vout_frame[slot.ch] = isqrt64_round_fast((uint64_t)acc) >> sh;
+        const uint64_t acc = (uint64_t)k1_fb_accumulate(sm, fl, slot, fb_len(s));
+        big |= (acc >> 48) != 0;
+        if (slot.ch >= 0 && vout_frame) vout_frame[slot.ch] = isqrt64_round_below48(acc & 0xFFFFFFFFFFFFull) >> sh;
+    }
+#if defined(__CUDA_ARCH__)
+    big = __any_sync(0xFFFFFFFFu, big);
+#endif
+    if (!big || !vout_frame) return;
+    for (int s = 0; s < kFbSlots; ++s) {
+        if (fb_len(s) == 0) continue;
+        const FbSlot slot = P.fb_slots[l * kFbSlots + s];
+        if (slot.ch >= 0) vout_frame[slot.ch] = isqrt64_round_fast((uint64_t)k1_fb_accumulate(sm, fl, slot, fb_len(s))) >> sh;
     }
 }
 
 // ---------------------------------------------------------------------------------------------
 // K2: per-(stream, channel) temporal chain
 
+// Branch-free.  frac is the 10 bits below the msb (zero filled), so it is 0 for x <= 2, where the interpolation then
+// returns p[0] = lut[x] by itself; p[0..2] stay inside the 125 used entries for every x (x <= 2: lut[0..4]; msb 32: lut[122..124]).
 MWW_HD int32_t wide_dynamic_function(uint32_t x, const int16_t *lut) {
-    if (x <= 2) return lut[x];
-    const int interval = msb32(x);
-    const int16_t *p = lut + 4 * interval - 6;
-    const int32_t frac = (int32_t)(((interval < 11) ? (x << (11 - interval)) : (x >> (interval - 11))) & 0x3FF);
+    const int lz = clz32(x);
+    const int16_t *p = lut + (x <= 2 ? (int)x : 122 - 4 * lz);            // 4 * msb - 6
+    const int32_t frac = (int32_t)((shl_clamp32(x, lz) >> 21) & 0x3FF);
     int32_t r = ((int32_t)p[2] * frac) >> 5;
     r += (int32_t)((uint32_t)(int32_t)p[1] << 5);
     r *= frac;
@@ -461,15 +509,17 @@ MWW_HD int32_t wide_dynamic_function(uint32_t x, const int16_t *lut) {
 }
 
 MWW_HD uint32_t pcan_shrink(uint32_t x) {
-    if (x < (2u << 12)) return (x * x) >> 20;
-    return (x >> 6) - 64u;
+    const uint32_t quad = (x * x) >> 20, lin = (x >> 6) - 64u;     // both formed, one selected (x * x may wrap unused)
+    return x < (2u << 12) ? quad : lin;
 }
 
 MWW_HD uint32_t log_scale(uint32_t x, const uint16_t *lut) {
-    // natural log of x, scaled by 2^scale_shift (SURVEY.md Appendix B step 9)
-    const uint32_t integer = (uint32_t)msb32(x) - 1;
-    int32_t frac = (int32_t)(x - (1u << integer));
-    if (integer < 16) frac <<= (16 - integer); else frac >>= (integer - 16);
+    // natural log of x, scaled by 2^scale_shift (SURVEY.md Appendix B step 9); defined for x >= 2.  Branch-free: frac is
+    // the bits below the msb aligned to 16 bits (shifted up, zero filled, or down, truncated), which normalising x to
+    // bit 31 gives in one shift.  Any x, 0 and 1 included, reads lut[0..128] only.
+    const int lz = clz32(x);
+    const uint32_t integer = 31u - (uint32_t)lz;
+    const int32_t frac = (int32_t)(shl_clamp32(x, lz + 1) >> 16);
     const uint32_t seg = (uint32_t)frac >> 9;
     const int32_t c0 = lut[seg], c1 = lut[seg + 1];
     const int32_t rel = ((c1 - c0) * (frac - (int32_t)(seg << 9))) >> 16;
@@ -496,7 +546,8 @@ MWW_HD uint16_t k2_output(uint32_t v, uint32_t est, const int16_t *gain_lut, con
     const uint32_t snr = (uint32_t)(((uint64_t)sig * gain) >> kPcanSnrShift);
     sig = pcan_shrink(snr);
     sig <<= kLogCorrectionBits;
-    sig = sig > 1 ? log_scale(sig, log_lut) : 0;
+    const uint32_t lg = log_scale(sig, log_lut);                   // formed for every sig, kept for sig > 1
+    sig = sig > 1 ? lg : 0;
     return (uint16_t)(sig < 0xFFFFu ? sig : 0xFFFFu);
 }
 
