@@ -37,8 +37,8 @@ MWW_HD int clz32(uint32_t x) {
 MWW_HD int msb32(uint32_t x) { return 32 - clz32(x); }
 
 // The helpers below have a host form and a device intrinsic form.  The CPU tests (tests/test_frontend_scalar_forms.py,
-// tests/test_host_emul.py) run the host forms; the device forms are covered by the GPU parity tests, which compare the
-// kernels' features bit for bit with the oracle.
+// tests/test_host_emul.py) run the host forms; tests/test_gpu_device_forms.py runs the device forms on the GPU, on whole
+// input domains, against portable references (tests/host_emul/scalar_refs.h).
 
 // x << s for 0 <= s <= 33, zero once s >= 32 (one clamped funnel shift on the device)
 MWW_HD uint32_t shl_clamp32(uint32_t x, int s) {

@@ -151,8 +151,10 @@ MWW_HD uint32_t isqrt64_round(uint64_t x) {
 // trunc(s + 0.5) is exact.  ~22 instructions (MUFU.RSQ64H + 10 FP64 ops) instead of ~70 integer ones; the FP64
 // pipe is otherwise idle in K1.  Rejected: a branch-free variant (hand-written
 // RSQ64H seed + two Newton steps + an exact integer check, all of a lane's roots in one block) -- the extra
-// instructions cost more than the slow-path branch of sqrt() and the serial FP64 chains.  x >= 2^48 -- only reachable through the library's int32 view of an energy of
-// exactly 2^31 -- takes the integer routine above.
+// instructions cost more than the slow-path branch of sqrt() and the serial FP64 chains.  No accumulator reaches 2^48: every
+// energy is below 2 * 32767^2 (k1_real_energy) and no channel's coefficients sum to more than 56 902, so accumulators stay
+// below 1.23e14 < 2^47 for any int16 or float audio (tests/test_host_emul.py::test_filterbank_accumulators_stay_below_2_48).
+// isqrt64_round_fast keeps the integer routine above for x >= 2^48 as a guard only.
 MWW_HD uint32_t isqrt64_round_below48(uint64_t x) {   // x < 2^48
 #if defined(__CUDA_ARCH__)
     const uint32_t r = __double2uint_rz(sqrt(__ull2double_rn(x)) + 0.5);
@@ -468,9 +470,9 @@ MWW_HD int64_t k1_fb_accumulate(const K1Smem &sm, int fl, const FbSlot &slot, in
 MWW_HD void k1_filterbank(int tid, K1Smem &sm, const FrontendParams &P, uint32_t *vout_frame /* [40] or nullptr */) {
     const int fl = tid >> 4, l = tid & 15;
     const int sh = sm.shift[fl];
-    // An accumulator >= 2^48 needs the integer square root, and it takes a full-scale energy to make one.  The common path
-    // takes the double root for every channel; if any lane of the warp met such an accumulator, the warp recomputes its
-    // channels with the exact routine.  One vote per frame instead of a branch per channel.
+    // The double root is exact below 2^48, and the range argument at isqrt64_round_below48 bounds every accumulator below
+    // 2^47, so the vote below cannot fire for any int16 or float audio.  It stays as a guard: if a lane of the warp ever met
+    // an accumulator >= 2^48, the warp would recompute its channels with the exact integer routine.  One vote per frame.
     bool big = false;
 #pragma unroll
     for (int s = 0; s < kFbSlots; ++s) {

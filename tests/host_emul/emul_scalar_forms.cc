@@ -1,8 +1,10 @@
 // Host build of the frontend's branch-free scalar functions (mww_frontend_dev.cuh) next to the branching forms they
-// replaced, kept here verbatim as the reference.  Each entry point returns the first input where the two disagree, or -1.
+// replaced (scalar_refs.h, shared with the device harness device_forms.cu).  Each entry point returns the first input where
+// the two disagree, or -1.
 #include <stdint.h>
 
 #include "../../microwakeword_b200/csrc/mww_frontend_dev.cuh"
+#include "scalar_refs.h"
 
 using namespace mww;
 
@@ -15,50 +17,6 @@ const HostTables &tables() {
     return g_tables;
 }
 
-int32_t wide_dynamic_function_branching(uint32_t x, const int16_t *lut) {
-    if (x <= 2) return lut[x];
-    const int interval = msb32(x);
-    const int16_t *p = lut + 4 * interval - 6;
-    const int32_t frac = (int32_t)(((interval < 11) ? (x << (11 - interval)) : (x >> (interval - 11))) & 0x3FF);
-    int32_t r = ((int32_t)p[2] * frac) >> 5;
-    r += (int32_t)((uint32_t)(int32_t)p[1] << 5);
-    r *= frac;
-    r = (r + (1 << 14)) >> 15;
-    r += p[0];
-    return (int32_t)(int16_t)r;
-}
-
-uint32_t pcan_shrink_branching(uint32_t x) {
-    if (x < (2u << 12)) return (x * x) >> 20;
-    return (x >> 6) - 64u;
-}
-
-uint32_t log_scale_branching(uint32_t x, const uint16_t *lut) {
-    const uint32_t integer = (uint32_t)msb32(x) - 1;
-    int32_t frac = (int32_t)(x - (1u << integer));
-    if (integer < 16) frac <<= (16 - integer); else frac >>= (integer - 16);
-    const uint32_t seg = (uint32_t)frac >> 9;
-    const int32_t c0 = lut[seg], c1 = lut[seg + 1];
-    const int32_t rel = ((c1 - c0) * (frac - (int32_t)(seg << 9))) >> 16;
-    const uint32_t log2v = (integer << 16) + (uint32_t)(frac + c0 + rel);
-    const uint32_t loge = (uint32_t)((45426ull * log2v + 32768u) >> 16);
-    return ((loge << kLogScaleShift) + 32768u) >> 16;
-}
-
-uint16_t k2_output_branching(uint32_t v, uint32_t est, const int16_t *gain_lut, const uint16_t *log_lut) {
-    const uint32_t scaled = v << kSmoothingBits;
-    const uint32_t e = est > scaled ? scaled : est;
-    const uint32_t fl = (uint32_t)(((uint64_t)v * kMinSignalRemaining) >> kNoiseBits);
-    const uint32_t sub = (scaled - e) >> kSmoothingBits;
-    uint32_t sig = sub > fl ? sub : fl;
-    const uint32_t gain = (uint32_t)wide_dynamic_function_branching(est, gain_lut);
-    const uint32_t snr = (uint32_t)(((uint64_t)sig * gain) >> kPcanSnrShift);
-    sig = pcan_shrink_branching(snr);
-    sig <<= kLogCorrectionBits;
-    sig = sig > 1 ? log_scale_branching(sig, log_lut) : 0;
-    return (uint16_t)(sig < 0xFFFFu ? sig : 0xFFFFu);
-}
-
 }  // namespace
 
 extern "C" {
@@ -67,8 +25,8 @@ extern "C" {
 long long emul_forms_wdf_pcan_mismatch(uint32_t lo, uint32_t hi) {
     const int16_t *g = tables().gain_lut;
     for (uint64_t x = lo; x <= hi; ++x) {
-        if (wide_dynamic_function((uint32_t)x, g) != wide_dynamic_function_branching((uint32_t)x, g)) return (long long)x;
-        if (pcan_shrink((uint32_t)x) != pcan_shrink_branching((uint32_t)x)) return (long long)x;
+        if (wide_dynamic_function((uint32_t)x, g) != ref::wide_dynamic_function((uint32_t)x, g)) return (long long)x;
+        if (pcan_shrink((uint32_t)x) != ref::pcan_shrink((uint32_t)x)) return (long long)x;
     }
     return -1;
 }
@@ -77,7 +35,7 @@ long long emul_forms_wdf_pcan_mismatch(uint32_t lo, uint32_t hi) {
 long long emul_forms_log_scale_range_mismatch(uint32_t lo, uint32_t hi) {
     const uint16_t *g = tables().log_lut;
     for (uint64_t x = lo; x <= hi; ++x)
-        if (log_scale((uint32_t)x, g) != log_scale_branching((uint32_t)x, g)) return (long long)x;
+        if (log_scale((uint32_t)x, g) != ref::log_scale((uint32_t)x, g)) return (long long)x;
     return -1;
 }
 
@@ -85,7 +43,7 @@ long long emul_forms_log_scale_range_mismatch(uint32_t lo, uint32_t hi) {
 long long emul_forms_log_scale_list_mismatch(const uint32_t *x, long long n) {
     const uint16_t *g = tables().log_lut;
     for (long long i = 0; i < n; ++i)
-        if (log_scale(x[i], g) != log_scale_branching(x[i], g)) return i;
+        if (log_scale(x[i], g) != ref::log_scale(x[i], g)) return i;
     return -1;
 }
 
@@ -93,7 +51,7 @@ long long emul_forms_log_scale_list_mismatch(const uint32_t *x, long long n) {
 long long emul_forms_k2_output_mismatch(const uint32_t *v, const uint32_t *est, long long n) {
     const HostTables &t = tables();
     for (long long i = 0; i < n; ++i)
-        if (k2_output(v[i], est[i], t.gain_lut, t.log_lut) != k2_output_branching(v[i], est[i], t.gain_lut, t.log_lut)) return i;
+        if (k2_output(v[i], est[i], t.gain_lut, t.log_lut) != ref::k2_output(v[i], est[i], t.gain_lut, t.log_lut)) return i;
     return -1;
 }
 

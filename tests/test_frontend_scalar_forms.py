@@ -1,5 +1,5 @@
 """The branch-free scalar functions of the frontend's temporal chain and windowing (mww_frontend_dev.cuh), compiled for the
-CPU, equal the branching forms they replaced (kept in tests/host_emul/emul_scalar_forms.cc) on every input the kernels can
+CPU, equal the branching forms they replaced (kept in tests/host_emul/scalar_refs.h) on every input the kernels can
 reach; and the fused clip kernels stay within 64 registers, without spills, so that four CTAs fit an SM."""
 
 import ctypes
@@ -85,3 +85,12 @@ def test_fused_clip_kernels_fit_four_ctas_per_sm(tmp_path):
     assert len(fused) == 2, sorted(regs)                  # int16 and float32 audio
     for k in fused:
         assert regs[k] <= 64 and spills[k] == 0, (k, regs[k], spills[k])
+
+
+@pytest.mark.skipif(not os.path.exists(NVCC) or shutil.which("g++") is None, reason="needs nvcc")
+def test_device_forms_harness_compiles_for_sm_90a(tmp_path):
+    """The harness tests/test_gpu_device_forms.py runs on the GPU, compiled with the same command."""
+    import test_gpu_device_forms as T
+    res = subprocess.run([NVCC] + T.NVCC_FLAGS + ["-shared", "-Xcompiler", "-fPIC", "-o", str(tmp_path / "forms.so")] + T.HARNESS_SOURCES,
+                         capture_output=True, text=True)
+    assert res.returncode == 0, res.stderr

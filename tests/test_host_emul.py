@@ -112,6 +112,37 @@ def test_filterbank_schedule_is_bank_conflict_free_and_complete():
     assert seen_channels == set(range(40))
 
 
+def test_filterbank_accumulators_stay_below_2_48():
+    """k1_filterbank takes the FP64 square root, exact below 2^48, for every channel; a warp vote sends accumulators >= 2^48
+    to the integer routine.  Bound every accumulator from the product's tables: each real-FFT half out of k1_real_energy is
+    (f1 +- t) >> 1 with f1 the sum of two C_FIXDIV(., 2) of int16 values and t an int16, so every energy is at most
+    2 * max|half|^2, and an accumulator is at most that times the sum of its slot's coefficients.  Below 2^48 the vote
+    cannot fire for any int16 or float audio."""
+    i16 = np.arange(-32768, 32768, dtype=np.int64)
+    fixdiv2 = (i16 * 16383 + 16384) >> 15
+    f1 = (2 * int(fixdiv2.min()), 2 * int(fixdiv2.max()))
+    # (f1 + t) >> 1, (f1 - t) >> 1 and (t - f1) >> 1 are monotone in f1 and t: the extremes sit at the corners
+    halves = [(a + s * t) >> 1 for a in f1 for t in (-32768, 32767) for s in (1, -1)] + [(t - a) >> 1 for a in f1 for t in (-32768, 32767)]
+    half = max(abs(h) for h in halves)
+    assert half == 32767
+    energy = 2 * half * half
+    assert energy < 1 << 31                              # also below the int32 view the accumulation widens from
+    slots, coef = emul.fb_schedule()
+    lens = [int(v) for v in emul.tables()["info"][4:8]]
+    worst = 0
+    for lane in range(16):
+        for s, L in enumerate(lens):
+            ch, _, _, off = (int(v) for v in slots[lane, s])
+            if L == 0:
+                continue
+            row = coef[off:off + L].astype(np.int64)
+            assert (row >= 0).all()
+            worst = max(worst, int(row.sum()) * energy)
+            assert ch >= 0 or not row.any()
+    assert 0 < worst < 1 << 48, worst
+    assert worst < 1 << 47                              # 1.22e14 (coefficient sum 56 902): a factor two to spare
+
+
 def test_fused_clip_frontend_phases_bit_exact_and_order_independent():
     """The one-launch clip frontend (filterbank -> estimate recurrence on 40 threads -> 640 independent outputs per group,
     all from shared memory) against the oracle: multi-group calls, a ragged last group, chunked feeding with carried state,
