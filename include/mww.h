@@ -179,19 +179,37 @@ int mww_get_state(mww_t *h, int16_t *h_carry, uint32_t *h_estimate, void *h_nn, 
 int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const uint32_t *h_estimate,
                   const void *h_nn, const void *h_pending, int pending_rows);
 
+/* Device-to-device copy of the NN ring state of n streams: stream h_dst_ids[i] of `dst` takes the rings of stream
+ * h_src_ids[i] of `src`, for i = 0 .. n-1 in order, asynchronously on cu_stream.  Both handles' rings are first put
+ * back into the canonical layout (live calls leave them rotated), so the copy is valid whatever calls came before.
+ * Frontend state (window carry, noise estimates) and the lockstep counters are not touched.  dst == src is allowed.
+ * MWW_EINVAL when the handles are on different devices, were created from different model containers, either holds
+ * pending rows, either is frontend-only, or an id is outside [0, n_streams).  This is how a batched evaluation hands
+ * one stream's state to and from a single-stream handle without a host round trip of every stream's state.  Each id
+ * pair is one cudaMemcpyAsync (the copies must stay ordered for dst == src), so the call is meant for a few streams;
+ * moving the state of many streams at once is what mww_get_state / mww_set_state do. */
+int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src, const int32_t *h_src_ids, int n, void *cu_stream);
+
 /* ---- detection post-processing (microwakeword/test.py:337-341, :94-137, :364-373) -------------------------
  * Tracks are ragged: track i is d_probs[d_offsets[i] .. d_offsets[i] + d_lengths[i]) (float32 probabilities as
- * produced by mww_infer_features / mww_predict_clip).  All three are stateless and asynchronous on cu_stream.
+ * produced by mww_infer_features / mww_predict_clip).  All four are stateless and asynchronous on cu_stream.
  *   mww_moving_average       out_i[j] = mean(probs_i[j .. j+window)), written at d_out[d_out_offsets[i] + j]
  *   mww_false_accept_counts  d_counts[i][c] = detections of track i at cutoff c (float64 cutoffs) with the
  *                            reference's cooldown rule, evaluated on the moving average
- *   mww_positive_scores      d_scores[i] = max of the moving average of probs_i[ignore:], NaN if too short */
+ *   mww_positive_scores      d_scores[i] = max of the moving average of probs_i[ignore:], NaN if too short
+ *   mww_accuracy_counts      the per-track rule of test.py:452-484 (tflite_model_accuracy):
+ *                            d_false_accepts[i] = crossings prev <= 0.5 < p at index j with j - last > min_gap, where
+ *                            prev and last start at 0 on every track and last = j after each counted crossing;
+ *                            d_last_positive[i] = 1 if the track's last probability is > 0.5, else 0 (also for an
+ *                            empty track).  Either output may be NULL. */
 int mww_moving_average(const float *d_probs, const long long *d_offsets, const int *d_lengths, int n_tracks, int max_length,
                        int window, float *d_out, const long long *d_out_offsets, void *cu_stream);
 int mww_false_accept_counts(const float *d_probs, const long long *d_offsets, const int *d_lengths, int n_tracks, int window,
                             const double *d_cutoffs, int n_cutoffs, int ignore_slices_after_accept, int *d_counts, void *cu_stream);
 int mww_positive_scores(const float *d_probs, const long long *d_offsets, const int *d_lengths, int n_tracks, int window,
                         int ignore_slices_after_accept, float *d_scores, void *cu_stream);
+int mww_accuracy_counts(const float *d_probs, const long long *d_offsets, const int *d_lengths, int n_tracks, int min_gap,
+                        int *d_false_accepts, int *d_last_positive, void *cu_stream);
 
 /* Per-kernel device timing for roofline reporting.  While enabled, every launch of the four kernel
  * classes is bracketed by CUDA events on the launching stream.  mww_profile_read synchronises the

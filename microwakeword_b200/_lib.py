@@ -23,7 +23,7 @@ EXPORTS = (
     "mww_moving_average", "mww_false_accept_counts", "mww_positive_scores", "mww_copy_async",
     "mww_ipc_alloc", "mww_ipc_open", "mww_ipc_close", "mww_ipc_free",
     "mww_predict_clip_remote", "mww_reset_device_ids", "mww_host_alloc", "mww_host_alloc_wc", "mww_host_free", "mww_bind_host_thread",
-    "mww_set_window_step", "mww_features_f32", "mww_predict_clip_f32",
+    "mww_set_window_step", "mww_features_f32", "mww_predict_clip_f32", "mww_copy_nn_state", "mww_accuracy_counts",
 )
 
 
@@ -100,6 +100,10 @@ def lib() -> ctypes.CDLL:
     L.mww_false_accept_counts.argtypes = [vp, vp, vp, i32, i32, vp, i32, i32, vp, vp]
     L.mww_positive_scores.restype = i32
     L.mww_positive_scores.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
+    L.mww_accuracy_counts.restype = i32
+    L.mww_accuracy_counts.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp]
+    L.mww_copy_nn_state.restype = i32
+    L.mww_copy_nn_state.argtypes = [vp, vp, vp, vp, i32, vp]
     L.mww_launch_count.restype = ll
     L.mww_launch_count.argtypes = [vp]
     L.mww_copy_async.restype = i32

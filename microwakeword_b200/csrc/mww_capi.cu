@@ -59,6 +59,7 @@ struct mww_handle {
     int device = 0, n_streams = 0, sm_count = 132;
     bool quantized = false;
     bool has_nn = true;
+    uint64_t model_hash = 0;        // FNV-1a of the model container: mww_copy_nn_state only moves state between equal models
     std::string err;
     // constant tables
     uint8_t *d_tables = nullptr;
@@ -714,6 +715,11 @@ int mww_create(const void *model_blob, size_t n_bytes, int device, int n_streams
     if (const char *mb = getenv("MWW_SCRATCH_MB")) { const long v = atol(mb); if (v > 0) h->scratch_budget = (size_t)v << 20; }
     if (const char *mt = getenv("MWW_MIN_TILE_STREAMS")) { const long v = atol(mt); if (v > 0) h->min_tile_streams = (int)v; }
     h->has_nn = model_blob != nullptr;
+    if (h->has_nn) {
+        uint64_t x = 1469598103934665603ull;
+        for (size_t i = 0; i < n_bytes; ++i) x = (x ^ static_cast<const uint8_t *>(model_blob)[i]) * 1099511628211ull;
+        h->model_hash = x;
+    }
     int rc = upload_tables(h);
     if (rc == MWW_OK && h->has_nn) rc = upload_weights(h, static_cast<const uint8_t *>(model_blob), n_bytes);
     if (rc == MWW_OK) {
@@ -1305,6 +1311,35 @@ int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const
     if (h_pending) CU(h, cudaMemcpy(h->d_pend, h_pending, S * h->pend_cap * kNumChannels * elem_size(h), cudaMemcpyHostToDevice));
     h->used = frontend_buffered;
     h->n_pend = pending_rows;
+    return MWW_OK;
+}
+
+int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src_c, const int32_t *h_src_ids, int n, void *cu_stream) {
+    if (!dst) return MWW_EINVAL;
+    // canonicalising the source's rings changes their layout, not the state they hold
+    mww_t *src = const_cast<mww_t *>(src_c);
+    if (!src || n < 0 || (n > 0 && (!h_dst_ids || !h_src_ids))) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: bad arguments");
+    if (src->device != dst->device) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: the handles are on different devices");
+    if (!src->has_nn || !dst->has_nn) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: frontend-only handle has no NN state");
+    if (src->model_hash != dst->model_hash || src->quantized != dst->quantized || src->state_elems != dst->state_elems)
+        return fail(dst, MWW_EINVAL, "mww_copy_nn_state: the handles were created from different models");
+    if (src->n_pend != 0 || dst->n_pend != 0) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: a handle holds pending rows");
+    for (int i = 0; i < n; ++i)
+        if (h_dst_ids[i] < 0 || h_dst_ids[i] >= dst->n_streams || h_src_ids[i] < 0 || h_src_ids[i] >= src->n_streams)
+            return fail(dst, MWW_EINVAL, "mww_copy_nn_state: stream id out of range");
+    ENTER_STATEFUL(dst);
+    if (src->poisoned) return fail(dst, MWW_ECUDA, "mww_copy_nn_state: the source handle needs mww_reset(h, NULL, 0, stream)");
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    int rc = canonicalise_rings(src, st);
+    if (rc) return fail(dst, rc, "mww_copy_nn_state: " + src->err);
+    if (dst != src && (rc = canonicalise_rings(dst, st)) != MWW_OK) return rc;
+    const size_t bytes = (size_t)dst->state_elems * elem_size(dst);
+    char *d = static_cast<char *>(dst->d_nn_state);
+    const char *s = static_cast<const char *>(src->d_nn_state);
+    for (int i = 0; i < n; ++i) {
+        if (dst == src && h_dst_ids[i] == h_src_ids[i]) continue;     // same bytes: nothing to copy (and memcpy needs disjoint ranges)
+        CU(dst, cudaMemcpyAsync(d + (size_t)h_dst_ids[i] * bytes, s + (size_t)h_src_ids[i] * bytes, bytes, cudaMemcpyDeviceToDevice, st));
+    }
     return MWW_OK;
 }
 

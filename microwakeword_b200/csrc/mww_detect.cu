@@ -4,6 +4,8 @@
 //   false-accept counting ..... microwakeword/test.py:118-135  (per cutoff: cooldown, re-armed by a detection)
 //   positive-sample score ..... microwakeword/test.py:364-373  (max of the moving average after the first
 //                               `ignore_slices_after_accept` probabilities)
+//   accuracy counts ........... microwakeword/test.py:452-484  (tflite_model_accuracy: 0.5 crossings per ambient track,
+//                               last probability > 0.5 per test clip)
 // Keeping this on the device means only detections / scores leave the GPU instead of every probability.
 // Parity is PINNED: tests/golden/detection_golden.npz comes from executing the reference's own function.
 #include <cuda_runtime.h>
@@ -67,6 +69,31 @@ __global__ void positive_score_kernel(const float *__restrict__ probs, const lon
     if (lane == 0) score[trk] = n > 0 ? m : NAN;
 }
 
+// one warp per track, 32 consecutive steps per pass (coalesced): whether step i is a rising crossing prev <= 0.5 < p
+// (test.py:479) does not depend on the chain, so the lanes find the crossings in parallel and only the min_gap chain over
+// the crossings (last_positive_index, :480-483) is walked in order -- by every lane alike, from the same ballot mask.
+__global__ void accuracy_kernel(const float *__restrict__ probs, const long long *__restrict__ offsets, const int *__restrict__ lengths,
+                                int n_tracks, int min_gap, int *__restrict__ false_accepts, int *__restrict__ last_positive) {
+    const int trk = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+    if (trk >= n_tracks) return;
+    const int lane = threadIdx.x & 31;
+    const int n = lengths[trk];
+    const float *p = probs + offsets[trk];
+    if (false_accepts) {
+        int last = 0, count = 0;                                // previous_probability and last_positive_index restart at 0 (:475-476)
+        for (int base = 0; base < n; base += 32) {
+            const int i = base + lane;
+            const bool crossing = i < n && (i == 0 ? 0.f : p[i - 1]) <= 0.5f && p[i] > 0.5f;
+            for (unsigned mask = __ballot_sync(0xffffffffu, crossing); mask; mask &= mask - 1) {
+                const int j = base + __ffs(mask) - 1;
+                if (j - last > min_gap) { ++count; last = j; }
+            }
+        }
+        if (lane == 0) false_accepts[trk] = count;
+    }
+    if (last_positive && lane == 0) last_positive[trk] = (n > 0 && p[n - 1] > 0.5f) ? 1 : 0;   // probabilities[-1] > 0.5 (:462-463)
+}
+
 }  // namespace
 
 extern "C" {
@@ -98,6 +125,15 @@ int mww_positive_scores(const float *d_probs, const long long *d_offsets, const 
     if (n_tracks == 0) return MWW_OK;
     positive_score_kernel<<<(unsigned)((n_tracks + 3) / 4), 128, 0, static_cast<cudaStream_t>(cu_stream)>>>(
         d_probs, d_offsets, d_lengths, n_tracks, window, ignore_slices_after_accept, d_scores);
+    return cudaGetLastError() == cudaSuccess ? MWW_OK : MWW_ECUDA;
+}
+
+int mww_accuracy_counts(const float *d_probs, const long long *d_offsets, const int *d_lengths, int n_tracks, int min_gap,
+                        int *d_false_accepts, int *d_last_positive, void *cu_stream) {
+    if (!d_probs || !d_offsets || !d_lengths || n_tracks < 0) return MWW_EINVAL;
+    if (n_tracks == 0 || (!d_false_accepts && !d_last_positive)) return MWW_OK;
+    accuracy_kernel<<<(unsigned)((n_tracks + 3) / 4), 128, 0, static_cast<cudaStream_t>(cu_stream)>>>(
+        d_probs, d_offsets, d_lengths, n_tracks, min_gap, d_false_accepts, d_last_positive);
     return cudaGetLastError() == cudaSuccess ? MWW_OK : MWW_ECUDA;
 }
 

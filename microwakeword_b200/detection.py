@@ -22,8 +22,24 @@ import numpy as np
 from . import _lib
 
 
+class _Packed:
+    """Tracks already on the device: track i is flat[offsets[i] : offsets[i] + lengths[i]] (the layout
+    Model._predict_spectrograms_device returns).  Accepted wherever a list of tracks is, so the detection kernels read
+    the probabilities in place."""
+
+    def __init__(self, flat, offsets, lengths):
+        self.flat = flat
+        self.offsets = np.ascontiguousarray(offsets, np.int64)
+        self.lengths = np.ascontiguousarray(lengths, np.int32)
+
+    def __len__(self):
+        return self.lengths.size
+
+
 def _pack(tracks, device):
     import torch
+    if isinstance(tracks, _Packed):       # the model may live on another GPU than the detection kernels: bring the buffer over
+        return (tracks.flat.to(device), torch.from_numpy(tracks.offsets).to(device), torch.from_numpy(tracks.lengths).to(device), tracks.lengths)
     lengths = np.asarray([len(t) for t in tracks], np.int32)
     offsets = np.zeros(len(tracks), np.int64)
     if len(tracks) > 1:
@@ -79,9 +95,11 @@ def compute_false_accepts_per_hour(streaming_probabilities_list, cutoffs, ignore
     in which case the duration is counted on the averaged length like the reference does."""
     cutoffs = np.asarray(cutoffs, np.float64)
     counts = false_accept_counts(streaming_probabilities_list, cutoffs, ignore_slices_after_accept, window, device)
+    tracks = streaming_probabilities_list
+    lengths = tracks.lengths if isinstance(tracks, _Packed) else [len(t) for t in tracks]
     duration_h = 0
-    for t in streaming_probabilities_list:
-        duration_h += max(len(t) - window + 1, 0) * stride * step_s / 3600.0
+    for n in lengths:
+        duration_h += max(int(n) - window + 1, 0) * stride * step_s / 3600.0
     return counts.sum(0).astype(np.float64) / duration_h
 
 
@@ -96,6 +114,42 @@ def positive_scores(tracks, window: int = 5, ignore_slices_after_accept: int = 2
     if rc != 0:
         raise _lib.MwwError(rc, "mww_positive_scores failed")
     return out.cpu().numpy()[:len(tracks)]
+
+
+def accuracy_counts(tracks, min_gap: int, device: int = 0):
+    """Per track, the rule of microwakeword.test.tflite_model_accuracy (test.py:452-484): (int32 [n_tracks] count of
+    0.5 crossings prev <= 0.5 < p at index j with j - last > min_gap, prev and last restarting at 0 on every track and
+    last = j after each counted crossing; bool [n_tracks] last probability > 0.5, False for an empty track)."""
+    import torch
+    dev = torch.device("cuda", device)
+    flat, offs, lens_d, _ = _pack(tracks, dev)
+    out = torch.empty((2, max(len(tracks), 1)), dtype=torch.int32, device=dev)
+    rc = _lib.lib().mww_accuracy_counts(flat.data_ptr(), offs.data_ptr(), lens_d.data_ptr(), len(tracks), int(min_gap),
+                                        out[0].data_ptr(), out[1].data_ptr(), _stream(dev))
+    if rc != 0:
+        raise _lib.MwwError(rc, "mww_accuracy_counts failed")
+    host = out.cpu().numpy()[:, :len(tracks)]
+    return host[0].copy(), host[1].astype(bool)
+
+
+def model_probabilities(model, spectrograms, device: int = 0):
+    """The probabilities of `spectrograms` fed one after another to `model`, as the reference's harness feeds them
+    (one model, state carried from track to track).  A microwakeword_b200 Model runs them as one batched pass and the
+    result stays on the GPU (a packed form every function of this module accepts); an object that has only
+    predict_spectrogram is called once per track."""
+    spectrograms = list(spectrograms)
+    if hasattr(model, "_predict_spectrograms_device"):
+        return _Packed(*model._predict_spectrograms_device(spectrograms))
+    if hasattr(model, "predict_spectrograms"):
+        return [np.asarray(p, np.float32) for p in model.predict_spectrograms(spectrograms)]
+    return [np.asarray(model.predict_spectrogram(t), np.float32) for t in spectrograms]
+
+
+def _split(tracks, k):
+    """(tracks[:k], tracks[k:]) for a list or a packed form (views of the same device buffer)."""
+    if isinstance(tracks, _Packed):
+        return (_Packed(tracks.flat, tracks.offsets[:k], tracks.lengths[:k]), _Packed(tracks.flat, tracks.offsets[k:], tracks.lengths[k:]))
+    return tracks[:k], tracks[k:]
 
 
 def false_rejection_rates(positive_sample_scores, cutoffs) -> np.ndarray:
@@ -152,13 +206,15 @@ def streaming_model_roc(model, ambient_spectrograms, positive_spectrograms, stri
     """The body of microwakeword.test.tflite_streaming_model_roc (test.py:321-403) on lists of spectrogram tracks: ambient
     tracks -> streaming probabilities -> moving average -> false accepts per hour; positive clips -> score -> false
     rejection rate; ROC coordinates and the area under them.  `model` is a microwakeword_b200.inference.Model (or anything
-    with predict_spectrogram); the detection arithmetic runs on the GPU, the ROC bookkeeping on the host.
-    Returns dict(auc, faph, frr, cutoffs, roc=(x, y, cutoff_at_point))."""
+    with predict_spectrograms or predict_spectrogram); the ambient tracks and then the positive clips go through it in
+    that order with the state carried over, as in the reference (model_probabilities).  The detection arithmetic runs on
+    the GPU, the ROC bookkeeping on the host.  Returns dict(auc, faph, frr, cutoffs, roc=(x, y, cutoff_at_point))."""
     cutoffs = np.arange(0, 1.01, 0.01) if cutoffs is None else np.asarray(cutoffs, np.float64)          # test.py:343
-    ambient = [np.asarray(model.predict_spectrogram(t), np.float32) for t in ambient_spectrograms]      # test.py:335-336
+    ambient_spectrograms = list(ambient_spectrograms)
+    probs = model_probabilities(model, ambient_spectrograms + list(positive_spectrograms), device)      # test.py:335-336, :367
+    ambient, positives = _split(probs, len(ambient_spectrograms))
     faph = compute_false_accepts_per_hour(ambient, cutoffs, ignore_slices_after_accept, stride=stride, step_s=window_step_ms / 1000.0,
                                           window=sliding_window_length, device=device)                 # :337-352 (average fused)
-    positives = [np.asarray(model.predict_spectrogram(t), np.float32) for t in positive_spectrograms]   # :367
     scores = positive_scores(positives, sliding_window_length, ignore_slices_after_accept, device)      # :368-373
     scores = scores[~np.isnan(scores)]
     frr = false_rejection_rates(scores, cutoffs)

@@ -199,6 +199,24 @@ class StreamEngine:
                                                        max(steps, 1), ctypes.byref(got), self._cu_stream()))
         return probs[:, :got.value]
 
+    def infer_strided(self, rows_ptr: int, row_type: int, n_rows: int, rows_stride: int, probs_ptr: int, max_probs: int) -> int:
+        """mww_infer_features on raw device pointers: stream s reads n_rows rows at rows_ptr + s * rows_stride rows and
+        writes its probabilities at probs_ptr + s * max_probs.  Returns the steps run.  For callers that lay the rows of
+        all streams out in one buffer themselves (Model.predict_spectrograms)."""
+        got = ctypes.c_int(0)
+        _lib.check(self._h, self._L.mww_infer_features(self._h, ctypes.c_void_p(int(rows_ptr)), int(row_type), int(n_rows), int(rows_stride),
+                                                       ctypes.c_void_p(int(probs_ptr)), int(max_probs), ctypes.byref(got), self._cu_stream()))
+        return got.value
+
+    def copy_nn_state(self, dst_ids, src: "StreamEngine", src_ids) -> None:
+        """Stream dst_ids[i] of this engine takes the NN ring state of stream src_ids[i] of `src` (same model, same
+        device, no pending rows), device to device and ordered on the current CUDA stream (mww_copy_nn_state)."""
+        d = np.ascontiguousarray(dst_ids, np.int32).reshape(-1)
+        s = np.ascontiguousarray(src_ids, np.int32).reshape(-1)
+        if d.size != s.size:
+            raise ValueError("dst_ids and src_ids must have the same length")
+        _lib.check(self._h, self._L.mww_copy_nn_state(self._h, d.ctypes.data, src._h, s.ctypes.data, d.size, self._cu_stream()))
+
     def predict_clip(self, audio, out=None):
         """int16 or float32 CUDA tensor [S, N] -> float32 probabilities [S, steps]; state carries over between calls.  float32
         samples are converted to int16 inside the frontend kernels (x * 32768, clipped, as audio_utils.to_int16)."""

@@ -3,6 +3,10 @@
 bookkeeping of ``microwakeword.train.validate_nonstreaming`` (train.py:41-163), with ``model.evaluate(batch_size=1024)``
 replaced by ``Model.predict_nonstreaming`` (the GPU clip kernel evaluated on whole windows).
 
+Streaming accuracy (``microwakeword.test.tflite_model_accuracy``, test.py:406-517, with ``compute_metrics`` and
+``metrics_to_string`` of test.py:30-91): ``tflite_model_accuracy`` below, on the batched state-carrying pass of
+``Model.predict_spectrograms`` and the accuracy kernel of csrc/mww_detect.cu.
+
 Training itself (train.py:166-), the Keras metric objects and the feature store are out of scope; these functions take
 plain arrays so the reference's harness can call them with what it already has."""
 
@@ -95,3 +99,82 @@ def validate_nonstreaming(model, test_fingerprints, test_ground_truth, ambient_s
         # the reference accumulates both sets in one metric object and subtracts the test set's false positives (:95-97)
         metrics.update(viable_recall_metrics(counts["tp"], amb["fp"], counts["fn"], ambient_duration_h))
     return metrics
+
+
+def compute_metrics(true_positives, true_negatives, false_positives, false_negatives) -> dict:
+    """Drop-in for microwakeword.test.compute_metrics (test.py:30-73): accuracy, recall, precision, false positive and
+    false negative rates and the sample count; a rate whose denominator is 0 is NaN."""
+    tp, tn, fp, fn = true_positives, true_negatives, false_positives, false_negatives
+    nan = float("nan")
+    count = tp + tn + fp + fn
+    has_pos, has_neg = tp + fn > 0, fp + tn > 0
+    return {
+        "accuracy": (tp + tn) / count if count > 0 else nan,
+        "recall": tp / (tp + fn) if has_pos else nan,
+        "precision": tp / (tp + fp) if tp + fp > 0 else nan,
+        "false_positive_rate": fp / (fp + tn) if has_neg else nan,
+        "false_negative_rate": fn / (tp + fn) if has_pos else nan,
+        "count": count,
+    }
+
+
+def metrics_to_string(metrics: dict) -> str:
+    """Drop-in for microwakeword.test.metrics_to_string (test.py:76-91): rates as percentages with 4 decimals."""
+    rates = [("accuracy", "accuracy"), ("recall", "recall"), ("precision", "precision"), ("fpr", "false_positive_rate"),
+             ("fnr", "false_negative_rate")]
+    return "; ".join("%s = %s" % (label, format(metrics[key], ".4%")) for label, key in rates) + "; (N=%s)" % (metrics["count"],)
+
+
+def _chunk_count(model, n_rows: int) -> int:
+    """Steps predict_spectrogram runs on a track of n_rows rows (inference.py:98-105)."""
+    return len(range(model.input_feature_slices, n_rows + 1, model.stride))
+
+
+def tflite_model_accuracy(model, fingerprints, ground_truth, ambient: bool, spectrogram_length_final_layer: int,
+                          ambient_duration_s: float | None = None):
+    """microwakeword.test.tflite_model_accuracy (test.py:406-517) on arrays: the spectrograms the reference's
+    ``audio_processor.get_data`` returns, their labels, and whether the set is an ambient one (``data_set`` ending in
+    "ambient", truncation strategy "none").  Returns (metrics dict, metrics string) -- the dict the reference returns and
+    the string it logs and writes to its accuracy file.
+
+    Every fingerprint is cast to float32 (test.py:447; uint16 features are therefore NOT scaled by 0.0390625 here) and
+    fed to one model in order with the state carried over, as the reference does; a microwakeword_b200 Model does this
+    as one batched pass (Model.predict_spectrograms) and the per-track rule runs on the GPU (detection.accuracy_counts).
+      * ambient=False: each track is one prediction, its last probability > 0.5, against its label.  A track too short
+        for one model step raises IndexError, as ``probabilities[-1]`` does in the reference.  For a model that has
+        ``input_feature_slices`` and ``stride`` (a Model), only the tracks up to that one are fed, as in the reference;
+        any other model object has been fed every track when the error is raised.
+      * ambient=True: false accepts are rising crossings of 0.5 (previous <= 0.5 < current), counted only when more
+        than spectrogram_length_final_layer steps after the last counted one; the previous probability and the last
+        index restart at 0 on every track, so crossings in a track's first spectrogram_length_final_layer steps are never
+        counted.  The string gives false accepts per hour over ambient_duration_s (audio_processor.get_mode_duration).
+    An empty set fails as the reference does (its metrics are never assigned)."""
+    from . import detection
+    fps = [np.asarray(f).astype(np.float32) for f in fingerprints]
+    if not fps:
+        raise UnboundLocalError("tflite_model_accuracy: no fingerprints (the reference's metrics are never assigned)")
+    if ambient and ambient_duration_s is None:
+        raise ValueError("tflite_model_accuracy: an ambient set needs ambient_duration_s")
+    if not ambient and hasattr(model, "input_feature_slices") and hasattr(model, "stride"):
+        empty = next((i for i, f in enumerate(fps) if _chunk_count(model, f.shape[0] if f.ndim else 0) == 0), None)
+        if empty is not None:
+            fps = fps[:empty + 1]                       # the reference stops at this track
+    device = getattr(getattr(model, "engine", None), "device", 0)
+    probs = detection.model_probabilities(model, fps, device)
+    lengths = probs.lengths if isinstance(probs, detection._Packed) else [len(p) for p in probs]
+    empty = next((i for i, n in enumerate(lengths) if n == 0), None)
+    if not ambient and empty is not None:
+        raise IndexError("list index out of range (track %d gives no probabilities: probabilities[-1])" % empty)
+    false_accepts, last_positive = detection.accuracy_counts(probs, spectrogram_length_final_layer, device)
+    tp = tn = fp = fn = 0.0
+    if ambient:
+        fp = float(false_accepts.sum())
+        metrics = compute_metrics(tp, tn, fp, fn)
+        return metrics, "false accepts = {}; false accepts per hour = {:.4}".format(fp, fp / (ambient_duration_s / 3600.0))
+    truth = np.asarray(ground_truth).reshape(-1)[:len(fps)]
+    hit = truth == last_positive                                    # sample_ground_truth == prediction
+    positive = truth.astype(bool)                                   # if sample_ground_truth
+    tp, tn = float((hit & positive).sum()), float((hit & ~positive).sum())
+    fn, fp = float((~hit & positive).sum()), float((~hit & ~positive).sum())
+    metrics = compute_metrics(tp, tn, fp, fn)
+    return metrics, metrics_to_string(metrics)

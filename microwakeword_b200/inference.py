@@ -91,27 +91,40 @@ class Model:
         """
         self._single()
         torch = _torch()
-        spectrogram = np.asarray(spectrogram)
-        if spectrogram.ndim != 2 or spectrogram.shape[1] != NUM_FEATURES:
-            raise ValueError("spectrogram must have shape [T, %d]" % NUM_FEATURES)
-        # inference.py:93-96 dtype normalisation.  uint16 rows are scaled by 0.0390625 on load in the kernel.
-        if np.issubdtype(spectrogram.dtype, np.uint16):
-            pass
-        elif spectrogram.dtype == np.int8 and self.is_quantized_model:
-            pass                                                  # already quantised: inference.py:110 skips quantisation
-        elif spectrogram.dtype != np.float32:
-            spectrogram = spectrogram.astype(np.float32)
-        # inference.py:98-105 chunking
-        slices, chunks = self.input_feature_slices, []
-        for last_index in range(slices, len(spectrogram) + 1, self.stride):
-            chunks.append(spectrogram[last_index - slices:last_index])
-        if not chunks:
+        rows = self._chunk_rows(spectrogram)
+        if rows.shape[0] == 0:
             return []
-        rows = np.ascontiguousarray(np.concatenate(chunks, 0))    # each chunk = one invoke
         dev = torch.from_numpy(rows.view(np.int16) if rows.dtype == np.uint16 else rows).to(self.engine._dev())
         if rows.dtype == np.uint16:
             dev = dev.view(torch.uint16)
         return self._predict_rows(dev.unsqueeze(0))
+
+    def predict_spectrograms(self, spectrograms, max_streams: int = 65536):
+        """``[self.predict_spectrogram(s) for s in spectrograms]`` -- same probabilities, same list-of-np.float32 type,
+        same state afterwards -- computed in one batched pass over up to `max_streams` streams (microwakeword_b200.batched).
+
+        This is the loop the reference's evaluation harness runs (test.py:335-367, :452-454): one interpreter, never reset,
+        so every track starts from the state the previous one left.  Int8 models give bit-identical probabilities and
+        state; fp32 ones agree to rounding (the batched pass may use a different kernel for a call than a per-track call).
+        Pre-quantised int8 tracks cannot be mixed with tracks of other dtypes (ValueError).
+
+        The pass keeps two things on the Model for the next call: a pinned host buffer the size of the largest test set
+        uploaded so far, and an engine of as many streams as the last plan used (its NN state: up to 65 536 x 16.7 KB
+        for fp32 okay_nabu).  release_batched() frees both."""
+        flat, offsets, lengths = self._predict_spectrograms_device(spectrograms, max_streams)
+        host = flat.cpu().numpy()
+        return [list(host[o:o + n]) for o, n in zip(offsets, lengths)]
+
+    def release_batched(self):
+        """Free the pinned upload buffer and the batched engine predict_spectrograms keeps between calls; the next call
+        allocates them again."""
+        done = getattr(self, "_staging_done", None)
+        if done is not None:
+            done.synchronize()
+        eng = getattr(self, "_pe_engine", None)
+        if eng is not None:
+            eng.close()
+        self._pe_engine = self._staging_buf = self._staging_done = None
 
     def quantize_input_data(self, data: np.ndarray, input_details: dict) -> np.ndarray:
         """quantize the input data using scale and zero point (inference.py:127-147: truncating astype, no clamp)"""
@@ -197,6 +210,109 @@ class Model:
         return out
 
     # ------------------------------------------------------------------ helpers
+    def _chunk_rows(self, spectrogram) -> np.ndarray:
+        """One track -> the rows predict_spectrogram feeds, [steps * input_feature_slices, 40] (inference.py:93-105)."""
+        spectrogram = np.asarray(spectrogram)
+        if spectrogram.ndim != 2 or spectrogram.shape[1] != NUM_FEATURES:
+            raise ValueError("spectrogram must have shape [T, %d]" % NUM_FEATURES)
+        # inference.py:93-96 dtype normalisation.  uint16 rows are scaled by 0.0390625 on load in the kernel.
+        if np.issubdtype(spectrogram.dtype, np.uint16):
+            pass
+        elif spectrogram.dtype == np.int8 and self.is_quantized_model:
+            pass                                                  # already quantised: inference.py:110 skips quantisation
+        elif spectrogram.dtype != np.float32:
+            spectrogram = spectrogram.astype(np.float32)
+        # inference.py:98-105 chunking; each chunk = one invoke
+        slices = self.input_feature_slices
+        n_chunks = len(range(slices, len(spectrogram) + 1, self.stride))
+        if self.stride == slices:
+            return np.ascontiguousarray(spectrogram[:n_chunks * slices])
+        idx = (np.arange(n_chunks) * self.stride)[:, None] + np.arange(slices)[None, :]
+        return np.ascontiguousarray(spectrogram[idx.reshape(-1)])
+
+    def _predict_spectrograms_device(self, spectrograms, max_streams: int = 65536):
+        """predict_spectrograms with the probabilities left on the GPU: (float32 CUDA tensor, int64 offsets, int32
+        lengths); track k's probabilities are flat[offsets[k] : offsets[k] + lengths[k]].  The detection kernels read
+        them there (detection.streaming_model_roc, evaluation.tflite_model_accuracy)."""
+        from . import _lib, batched
+        torch = _torch()
+        self._single()
+        if int(max_streams) < 1:
+            raise ValueError("max_streams must be >= 1")
+        tracks = [self._chunk_rows(s) for s in spectrograms]
+        slices = self.input_feature_slices
+        lengths = np.asarray([t.shape[0] // slices for t in tracks], np.int32)
+        dev = self.engine._dev()
+        if any(t.shape[0] for t in tracks) and self.engine.pending_rows:
+            raise RuntimeError("engine holds pending rows from step(); call reset() before predict_spectrogram")
+        kinds = {t.dtype for t in tracks if t.shape[0]}
+        if np.dtype(np.int8) in kinds and len(kinds) > 1:
+            raise ValueError("predict_spectrograms: pre-quantised int8 tracks cannot be mixed with tracks of other dtypes")
+        # the narrowest exact row type: uint16 -> float32 is exact (x * 0.0390625 = x * 5 / 128 fits float32's mantissa)
+        if kinds == {np.dtype(np.uint16)}:
+            dtype, row_type = np.uint16, _lib.MWW_ROWS_U16
+        elif kinds == {np.dtype(np.int8)}:
+            dtype, row_type = np.int8, _lib.MWW_ROWS_I8
+        else:
+            dtype, row_type = np.float32, _lib.MWW_ROWS_F32
+        a = self._arch()
+        p = batched.plan(lengths, slices, slices * batched.warmup_steps(a), max_streams)
+        n = p.total_steps
+        if n == 0:
+            return torch.zeros(1, dtype=torch.float32, device=dev)[:0], p.track_offsets, lengths   # a real pointer for the kernels
+        # Int8 model kernels need 16-byte aligned row pointers: with int8 rows (40 bytes) every pointer below must sit an
+        # even number of rows from the buffer start.  One extra warm-up / replay step keeps it so; more history is exact too.
+        odd_rows = (lambda steps: (steps * slices) % 2) if row_type == _lib.MWW_ROWS_I8 else (lambda steps: 0)
+        s, seg = (p.n_streams, p.seg_steps) if p.n_streams > 1 else (1, n)
+        warm = p.warmup_steps + odd_rows(p.warmup_steps) if s > 1 else 0
+        replay = p.warmup_steps + odd_rows(n - p.warmup_steps)
+        prefix = warm * slices
+        total_rows = prefix + s * seg * slices
+        host = self._staging(total_rows * NUM_FEATURES * np.dtype(dtype).itemsize).view(dtype)[:total_rows * NUM_FEATURES]
+        host = host.reshape(total_rows, NUM_FEATURES)
+        host[:prefix] = 0
+        at = prefix
+        for t in tracks:
+            if t.shape[0]:
+                host[at:at + t.shape[0]] = t if t.dtype == dtype else t.astype(np.float32) * np.float32(FEATURE_SCALE)
+                at += t.shape[0]
+        host[at:] = 0
+        rows = torch.from_numpy(host.view(np.int16) if dtype == np.uint16 else host).to(dev, non_blocking=True)
+        self._staging_done = torch.cuda.Event()
+        self._staging_done.record(torch.cuda.current_stream(dev))
+        row_bytes = NUM_FEATURES * np.dtype(dtype).itemsize
+        base = rows.data_ptr() + prefix * row_bytes
+        probs = torch.empty((s, seg), dtype=torch.float32, device=dev)
+        if s == 1:
+            self.engine.infer_strided(base, row_type, n * slices, n * slices, probs.data_ptr(), n)
+            return probs.reshape(-1), p.track_offsets, lengths
+        eng = getattr(self, "_pe_engine", None)
+        if eng is None or eng.n_streams != s:
+            if eng is not None:
+                eng.close()
+            eng = self._pe_engine = StreamEngine(self.engine._blob, n_streams=s, device=self.engine.device)
+        pitch = seg * slices
+        scratch = torch.empty((s, max(warm, replay)), dtype=torch.float32, device=dev)
+        # stream i > 0: the rows just before its segment flush whatever state it held; stream 0 takes the model's state
+        eng.infer_strided(base - prefix * row_bytes, row_type, prefix, pitch, scratch.data_ptr(), warm)
+        eng.copy_nn_state([0], self.engine, [0])
+        eng.infer_strided(base, row_type, pitch, pitch, probs.data_ptr(), seg)
+        # the model ends in the state after the last real row: that state depends only on the last `replay` steps
+        self.engine.infer_strided(base + (n - replay) * slices * row_bytes, row_type, replay * slices, replay * slices,
+                                  scratch.data_ptr(), replay)
+        return probs.reshape(-1), p.track_offsets, lengths
+
+    def _staging(self, nbytes: int) -> np.ndarray:
+        """Pinned upload buffer of predict_spectrograms, kept between calls and grown on demand."""
+        from .engine import host_array
+        done = getattr(self, "_staging_done", None)
+        if done is not None:
+            done.synchronize()                                   # the previous upload has left the buffer
+        buf = getattr(self, "_staging_buf", None)
+        if buf is None or buf.size < nbytes:
+            buf = self._staging_buf = host_array((max(int(nbytes), 1),), np.uint8, self.engine.device)
+        return buf[:max(int(nbytes), 1)]
+
     def _single(self):
         if self.engine.n_streams != 1:
             raise ValueError("predict_clip / predict_spectrogram are the reference's single-stream calls; use step() with batch > 1")
