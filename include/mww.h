@@ -85,7 +85,12 @@ typedef struct mww_info {
  * (tap 1, bias 0; int8: weight 1, multiplier 1.0, the previous tensor's quantisation) so the block structure stays
  * uniform and results are those of the reference graph.  Topologies outside that family -- repeat_in_block > 1,
  * residual branches (mixednet.py:336-358), pooled / attention heads (:362-381), first_conv_kernel_size < stride --
- * are answered with MWW_EUNSUPPORTED; okay_nabu and the models of esphome/micro-wake-word-models' v2 family use none. */
+ * are answered with MWW_EUNSUPPORTED; okay_nabu and the models of esphome/micro-wake-word-models' v2 family use none.
+ * Hybrid models: an fp32 container with `hy/mode` (the float .tflite the reference writes with quantize=False, whose
+ * large conv / depthwise / dense weights the converter stores as per-channel int8) runs TFLite's hybrid arithmetic --
+ * each such op quantises its float input to int8 on every step -- on the run-time-geometry hybrid kernel, whatever the
+ * architecture, okay_nabu's included.  It reads as an fp32 model everywhere (mww_info.is_quantized 0, float rows and
+ * probabilities, fp32 ring state in the layout above). */
 int mww_create(const void *model_blob, size_t n_bytes, int device, int n_streams, mww_t **out);
 int mww_destroy(mww_t *h);
 const char *mww_last_error(const mww_t *h);

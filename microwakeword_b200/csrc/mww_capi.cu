@@ -85,6 +85,8 @@ struct mww_handle {
     GenArch G{};
     GenWeightsF32 GW{};
     GenWeightsI8 GQ{};
+    bool hybrid = false;            // fp32 graph with int8-weight ops (container tensor hy/mode): generic hybrid kernel only
+    GenHybrid GH{};
     int stride = 3;                 // feature rows per model step
     int pend_cap = 2;               // rows of the pending buffer
     int state_elems = kStateFloats; // ring-state elements per stream
@@ -281,6 +283,10 @@ int run_nn_tile(mww_t *h, int first, int n, const void *d_rows, int row_type, lo
             CU(h, launch_nn_generic_i8(h->G, h->GQ, static_cast<int8_t *>(h->d_nn_state) + (size_t)first * h->state_elems,
                                        static_cast<int8_t *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
                                        rows_stream_stride_rows * kNumChannels * (long long)rb, n_rows, rt, d_probs, probs_stride, n, st));
+        else if (h->hybrid)
+            CU(h, launch_nn_generic_hybrid(h->G, h->GW, h->GH, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
+                                           static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
+                                           rows_stream_stride_rows * kNumChannels * (long long)rb, n_rows, rt, d_probs, probs_stride, n, st));
         else
             CU(h, launch_nn_generic_f32(h->G, h->GW, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
                                         static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
@@ -423,6 +429,36 @@ int upload_weights_generic(mww_t *h, const uint8_t *blob, size_t n, const Tensor
         }
         if ((rc = get("head/w", 0, (size_t)G.head_rows * G.c_last, (const void **)&W.head_w))) return rc;
         if ((rc = get("head/b", 0, 1, (const void **)&W.head_b))) return rc;
+        Tensor mode;
+        if (!find_tensor(blob, n, "hy/mode", &mode)) return MWW_OK;
+        // hybrid layers (model_file.py): int8 weights + per-channel scales next to the fp32 tensors
+        GenHybrid &H = h->GH;
+        if (mode.dtype != 2 || mode.nbytes % 4 != 0 || mode.nbytes > 4 * (2 + 5 * kGenMaxBlocks)) return fail(h, MWW_EMODEL, "model container: malformed 'hy/mode'");
+        int32_t modes[2 + 5 * kGenMaxBlocks];
+        memcpy(modes, mode.data, mode.nbytes);
+        if (gen_hybrid_layout(G, reinterpret_cast<const int32_t *>(arch.data), modes, (int)(mode.nbytes / 4), &H) != 0)
+            return fail(h, MWW_EMODEL, "model container: 'hy/mode' does not match the architecture (one entry per first conv, MixConv group, 1x1 conv, head; 0..2)");
+        if ((size_t)H.sm_elems * 4 > 200 * 1024)
+            return fail(h, MWW_EUNSUPPORTED, "model container: rings and quantisation buffers of one stream exceed 200 KB of shared memory");
+        h->hybrid = true;
+        if (H.mode0) {
+            if ((rc = get("hy/first_conv/w", 1, k0f, (const void **)&H.w0))) return rc;
+            if ((rc = get("hy/first_conv/scale", 0, G.c0, (const void **)&H.s0))) return rc;
+        }
+        for (int i = 0; i < G.n_blocks; ++i) {
+            if (H.any_dw[i]) {
+                snprintf(name, sizeof name, "hy/b%d/dw/w", i); if ((rc = get(name, 1, (size_t)G.kmax[i] * G.cin[i], (const void **)&H.dw_w[i]))) return rc;
+                snprintf(name, sizeof name, "hy/b%d/dw/scale", i); if ((rc = get(name, 0, G.cin[i], (const void **)&H.dw_s[i]))) return rc;
+            }
+            if (H.mode_pw[i]) {
+                snprintf(name, sizeof name, "hy/b%d/pw/w", i); if ((rc = get(name, 1, (size_t)G.cin[i] * G.cout[i], (const void **)&H.pw_w[i]))) return rc;
+                snprintf(name, sizeof name, "hy/b%d/pw/scale", i); if ((rc = get(name, 0, G.cout[i], (const void **)&H.pw_s[i]))) return rc;
+            }
+        }
+        if (H.mode_head) {
+            if ((rc = get("hy/head/w", 1, (size_t)G.head_rows * G.c_last, (const void **)&H.head_w))) return rc;
+            if ((rc = get("hy/head/scale", 0, 1, (const void **)&H.head_s))) return rc;
+        }
         return MWW_OK;
     }
     GenWeightsI8 &Q = h->GQ;
@@ -462,7 +498,11 @@ int upload_weights(mww_t *h, const uint8_t *blob, size_t n) {
     // the tensor-core kernels are compiled for the okay_nabu MixedNet (first conv 32x5 stride 3; MixConv [5],[7,11],[9,15],[23];
     // pointwise 64x4; 17-row head); every other architecture takes the run-time-geometry path.  MWW_FORCE_GENERIC=1 sends
     // okay_nabu through it as well (tests compare the two paths).
-    if (arch.nbytes != sizeof kOkayNabuArch || memcmp(arch.data, kOkayNabuArch, sizeof kOkayNabuArch) != 0 || getenv("MWW_FORCE_GENERIC") != nullptr)
+    // A hybrid container (fp32 graph with int8-weight ops, model_file.py) of any architecture, okay_nabu's included, runs on the
+    // generic hybrid kernel: the compiled-in fp32 kernels' arithmetic is not TFLite's hybrid arithmetic.
+    Tensor hy_mode;
+    if (find_tensor(blob, n, "hy/mode", &hy_mode) || arch.nbytes != sizeof kOkayNabuArch || memcmp(arch.data, kOkayNabuArch, sizeof kOkayNabuArch) != 0 ||
+        getenv("MWW_FORCE_GENERIC") != nullptr)
         return upload_weights_generic(h, blob, n, arch);
     Tensor probe;
     h->quantized = find_tensor(blob, n, "q/scales", &probe);

@@ -93,4 +93,8 @@ cudaError_t launch_nn_generic_i8(const GenArch &A, const GenWeightsI8 &W, int8_t
                                  int n_streams, cudaStream_t st);
 cudaError_t launch_gen_fill_state_i8(const GenArch &A, const GenWeightsI8 &W, int8_t *state, int8_t *pend, int n, const int32_t *ids, int n_streams,
                                      cudaStream_t st);
+// fp32 graph with int8-weight (hybrid) ops, any architecture including okay_nabu's; fp32 state layout
+cudaError_t launch_nn_generic_hybrid(const GenArch &A, const GenWeightsF32 &W, const GenHybrid &H, float *state, float *pend, int n_pend,
+                                     const void *rows, long long rows_stream_stride_bytes, int n_rows, int row_type, float *probs,
+                                     long long probs_stream_stride, int n_streams, cudaStream_t st);
 }  // namespace mww

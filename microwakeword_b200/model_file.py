@@ -30,6 +30,17 @@ Integer graph (prefix ``q/``; TFLite int8 semantics, SURVEY.md Appendix C):
                                      [in, c0, d1, p1, d2, p2, d3, p3, d4, p4, fc, prob]
     q/<layer>/w i8, q/<layer>/bias i32, q/<layer>/mult i32, q/<layer>/shift i32
     q/logistic_lut i8[256]           indexed by the uint8 view of the int8 logit
+Hybrid layers (prefix ``hy/``; optional, in an fp32 container): the float graph the converter writes without a
+representative dataset stores the weights of large CONV_2D / DEPTHWISE_CONV_2D / FULLY_CONNECTED ops as symmetric
+per-channel int8, and TFLite runs those ops with its hybrid kernels (input quantised to int8 on every invoke):
+    hy/mode              i32   one entry per op: first conv, per block its MixConv groups then its 1x1 conv, head
+                               (``hybrid_slots``); HYBRID_FLOAT, HYBRID_ASYMMETRIC or HYBRID_SYMMETRIC input quantisation
+    hy/first_conv/w i8 [kernel, 40, filters], hy/first_conv/scale f32 [filters]
+    hy/b{i}/dw/w i8 [max_k, C] (0 in float groups), hy/b{i}/dw/scale f32 [C]    when a group of block i is hybrid
+    hy/b{i}/pw/w i8 [Cin, Cout], hy/b{i}/pw/scale f32 [Cout]
+    hy/head/w i8 [T_head, C], hy/head/scale f32 [1]
+The fp32 tensors stay present; a hybrid layer's fp32 weights are its dequantised int8 weights (code * scale).  Biases are
+the fp32 ones.  A container without ``hy/mode`` is a plain fp32 one.
 """
 
 from __future__ import annotations
@@ -191,3 +202,19 @@ def save(path: str, tensors: dict) -> None:
 
 def is_quantized(tensors: dict) -> bool:
     return "q/scales" in tensors
+
+
+HYBRID_FLOAT, HYBRID_ASYMMETRIC, HYBRID_SYMMETRIC = 0, 1, 2
+
+
+def hybrid_slots(arch: Arch) -> list:
+    """names of the ``hy/mode`` entries in order: first conv, per block its MixConv groups then its 1x1 conv, head"""
+    names = ["first_conv"]
+    for i in range(arch.n_blocks):
+        names += ["b%d/dw%d" % (i, j) for j in range(len(arch.mixconv_kernel_sizes[i]))] + ["b%d/pw" % i]
+    return names + ["head"]
+
+
+def is_hybrid(tensors: dict) -> bool:
+    """fp32 graph whose large layers carry int8 weights (TFLite dynamic-range quantisation); not ``is_quantized``"""
+    return "hy/mode" in tensors

@@ -357,6 +357,30 @@ class _Recogniser:
                 self.fail(op, "bias has %s elements, expected %d" % (b.shape, n))
             return b
 
+        # float graph: every weight tensor is float32, or -- dynamic-range quantisation (utils.py:328 without a representative
+        # dataset) -- symmetric int8 with one float scale per output channel, executed by TFLite's hybrid kernels.  Decided per
+        # op from the file.  Returns (float32 values in the file's layout, int8 codes or None, scales or None).
+        hy = {}
+        modes = []
+
+        def float_weights(op, w_t, n_out, qdim, bias_t):
+            if w_t.dtype == np.float32:
+                return w_t.data().astype(np.float32), None, None
+            if w_t.dtype != np.int8:
+                self.fail(op, "weights are %s in a float graph (float32, or int8 with per-channel scales)" % w_t.dtype)
+            if w_t.scale.size != n_out or (w_t.scale.size > 1 and w_t.quantized_dimension != qdim):
+                self.fail(op, "int8 weights in a float graph need one scale per output channel on dimension %d; have %d scale(s) for %d "
+                              "channels on dimension %d" % (qdim, w_t.scale.size, n_out, w_t.quantized_dimension))
+            if w_t.zero_point.size not in (1, n_out) or np.any(w_t.zero_point != 0):
+                self.fail(op, "int8 weights in a float graph must have zero points 0 (symmetric quantisation)")
+            if bias_t is not None and bias_t.dtype != np.float32:
+                self.fail(op, "hybrid op with a %s bias, expected float32" % bias_t.dtype)
+            codes = w_t.data()
+            s = w_t.scale.astype(np.float32)
+            shape = [1] * codes.ndim
+            shape[qdim] = n_out
+            return (codes.astype(np.float32) * s.reshape(shape)).astype(np.float32), codes, s
+
         # ---- first conv: Stream(Conv2D(k x 1, strides=(stride, 1), valid, no bias)) + ReLU (mixednet.py:317-331)
         c0 = compute[0]
         w_t = self.t(c0.inputs[1])
@@ -385,7 +409,12 @@ class _Recogniser:
         else:
             if b0 is not None and np.any(b0.data() != 0):
                 self.fail(c0, "first conv carries a non-zero bias; mixednet.py:323 builds it with use_bias=False")
-            out["first_conv/w"] = np.ascontiguousarray(w0.astype(np.float32))
+            wf, codes, s = float_weights(c0, w_t, f0, 0, b0)
+            out["first_conv/w"] = np.ascontiguousarray(np.transpose(wf[:, :, 0, :], (1, 2, 0)))
+            modes.append(MF.HYBRID_FLOAT if codes is None else MF.HYBRID_ASYMMETRIC)
+            if codes is not None:
+                hy["hy/first_conv/w"] = np.ascontiguousarray(np.transpose(codes[:, :, 0, :], (1, 2, 0)))
+                hy["hy/first_conv/scale"] = s
 
         # ---- MixConv blocks (mixednet.py:341-360)
         pw_filters, ksizes = [], []
@@ -431,11 +460,16 @@ class _Recogniser:
                     out["q/b%d/dw/shift" % b] = np.full(cin, s1, np.int32)
                     weights_q("b%d/pw" % b, pf, pw_w, pb, cout, scales[-2], scales[-1])
                 else:
+                    wf, codes, s = float_weights(pw, pf, cout, 0, pb)
                     out["b%d/dw/w" % b] = np.ones((1, cin), np.float32)
                     out["b%d/dw/b" % b] = np.zeros(cin, np.float32)
                     out["b%d/dw/ksize" % b] = np.ones(cin, np.int32)
-                    out["b%d/pw/w" % b] = np.ascontiguousarray(pw_w.astype(np.float32))
+                    out["b%d/pw/w" % b] = np.ascontiguousarray(wf[:, 0, 0, :].T)
                     out["b%d/pw/b" % b] = (np.zeros(cout, np.float32) if pb is None else pb.data().reshape(-1).astype(np.float32))
+                    modes.extend([MF.HYBRID_FLOAT, MF.HYBRID_FLOAT if codes is None else MF.HYBRID_ASYMMETRIC])
+                    if codes is not None:
+                        hy["hy/b%d/pw/w" % b] = np.ascontiguousarray(codes[:, 0, 0, :].T)
+                        hy["hy/b%d/pw/scale" % b] = s
                 pw_filters.append(cout)
                 ksizes.append((1,))
                 cur, cin = nxt, cout
@@ -529,10 +563,19 @@ class _Recogniser:
             dw_k = np.zeros(cin, np.int32)
             c_off = 0
             dw_bias_f, dw_bias_q, dw_scale = [], [], []
+            hdw_w, hdw_s, dw_modes = np.zeros((kmax, cin), np.int8), np.zeros(cin, np.float32), []
             for slot, k, cg, dw, _, _, f in groups:
-                dw_w[kmax - k:, c_off:c_off + cg] = f.data()[0, :, 0, :]
-                dw_k[c_off:c_off + cg] = k
                 bt = bias_of(dw, cg)
+                if quantized:
+                    dw_w[kmax - k:, c_off:c_off + cg] = f.data()[0, :, 0, :]
+                else:
+                    wf, codes, s = float_weights(dw, f, cg, 3, bt)
+                    dw_w[kmax - k:, c_off:c_off + cg] = wf[0, :, 0, :]
+                    dw_modes.append(MF.HYBRID_FLOAT if codes is None else MF.HYBRID_ASYMMETRIC)
+                    if codes is not None:
+                        hdw_w[kmax - k:, c_off:c_off + cg] = codes[0, :, 0, :]
+                        hdw_s[c_off:c_off + cg] = s
+                dw_k[c_off:c_off + cg] = k
                 if quantized:
                     if f.dtype != np.int8 or np.any(f.zero_point != 0):
                         self.fail(dw, "depthwise weights must be symmetric int8")
@@ -560,10 +603,18 @@ class _Recogniser:
                 out["q/b%d/dw/shift" % b] = np.asarray([s for _, s in ms], np.int32)
                 weights_q("b%d/pw" % b, pf, pw_w, pb, cout, s_d, s_p)
             else:
+                wf, codes, s = float_weights(pw, pf, cout, 0, pb)
                 out["b%d/dw/w" % b] = dw_w.astype(np.float32)
                 out["b%d/dw/b" % b] = np.concatenate(dw_bias_f)
-                out["b%d/pw/w" % b] = np.ascontiguousarray(pw_w.astype(np.float32))
+                out["b%d/pw/w" % b] = np.ascontiguousarray(wf[:, 0, 0, :].T)
                 out["b%d/pw/b" % b] = (np.zeros(cout, np.float32) if pb is None else pb.data().reshape(-1).astype(np.float32))
+                modes.extend(dw_modes + [MF.HYBRID_FLOAT if codes is None else MF.HYBRID_ASYMMETRIC])
+                if any(dw_modes):
+                    hy["hy/b%d/dw/w" % b] = hdw_w
+                    hy["hy/b%d/dw/scale" % b] = hdw_s
+                if codes is not None:
+                    hy["hy/b%d/pw/w" % b] = np.ascontiguousarray(codes[:, 0, 0, :].T)
+                    hy["hy/b%d/pw/scale" % b] = s
             if not quantized:
                 out["b%d/dw/ksize" % b] = dw_k
             pw_filters.append(cout)
@@ -608,12 +659,23 @@ class _Recogniser:
         else:
             if final != g.outputs[0] or tout.dtype != np.float32:
                 self.fail(lg, "float graph must end in LOGISTIC")
-            out["head/w"] = np.ascontiguousarray(hw.astype(np.float32))
+            wf, codes, s = float_weights(fc, fw, 1, 0, fb)
+            out["head/w"] = np.ascontiguousarray(wf.reshape(t_head, cin))
             out["head/b"] = np.zeros(1, np.float32) if fb is None else fb.data().reshape(-1).astype(np.float32)
+            # FullyConnectedOptions.asymmetric_quantize_inputs (field 3) picks the hybrid kernel's input quantiser
+            modes.append(MF.HYBRID_FLOAT if codes is None else
+                         (MF.HYBRID_ASYMMETRIC if fc.opt(3, "B") else MF.HYBRID_SYMMETRIC))
+            if codes is not None:
+                hy["hy/head/w"] = np.ascontiguousarray(codes.reshape(t_head, cin))
+                hy["hy/head/scale"] = s
 
         self.check_initial_state(zps if quantized else None)
         arch = MF.Arch(f0, k0, stride, tuple(pw_filters), tuple(ksizes), t_head)
         out["arch"] = arch.encode()
+        if any(modes):
+            assert len(modes) == len(MF.hybrid_slots(arch))
+            out["hy/mode"] = np.asarray(modes, np.int32)
+            out.update(hy)
         return out
 
     def check_initial_state(self, zps):
