@@ -24,6 +24,8 @@
 
 #define NF 40
 #define MAX_BLOCKS 8
+#define MAX_CHANNELS 512                          /* per layer; the per-step buffers below hold this many */
+#define MAX_KERNEL 64                             /* taps of the first conv (and so its largest stride), of a MixConv group, rows of the head */
 
 struct tensor { const void *data; uint32_t dtype, ndim, shape[4]; uint64_t nbytes; };
 
@@ -89,10 +91,20 @@ mwwo_mixednet *mwwo_mixednet_create(const void *blob, size_t n) {
     struct tensor arch;
     if (!find_tensor(m->blob, n, "arch", &arch)) { mwwo_mixednet_free(m); return NULL; }
     const int32_t *a = (const int32_t *)arch.data;
+    const size_t n_arch = arch.nbytes / 4;
+    /* a model outside what the fixed-size step buffers hold is refused, never run */
+    if (n_arch < 6) { mwwo_mixednet_free(m); return NULL; }
     m->c0 = a[0]; m->k0 = a[1]; m->stride = a[2]; m->n_blocks = a[4]; m->head_rows = a[5];
-    if (a[3] != NF || m->n_blocks > MAX_BLOCKS) { mwwo_mixednet_free(m); return NULL; }
+    if (a[3] != NF || m->n_blocks < 1 || m->n_blocks > MAX_BLOCKS || n_arch < 6 + 6 * (size_t)m->n_blocks ||
+        m->c0 < 1 || m->c0 > MAX_CHANNELS || m->k0 < 1 || m->k0 > MAX_KERNEL || m->stride < 1 || m->stride > m->k0 ||
+        m->head_rows < 1 || m->head_rows > MAX_KERNEL) { mwwo_mixednet_free(m); return NULL; }
+    for (int i = 0; i < m->n_blocks; ++i) {
+        const int32_t *e = a + 6 + 6 * i;
+        if (e[0] < 1 || e[0] > MAX_CHANNELS || e[1] < 1 || e[1] > 4) { mwwo_mixednet_free(m); return NULL; }
+        for (int j = 0; j < e[1]; ++j)
+            if (e[2 + j] < 1 || e[2 + j] > MAX_KERNEL) { mwwo_mixednet_free(m); return NULL; }
+    }
     m->ring0 = m->k0 - 1 - (m->stride - 1);
-    if (m->ring0 < 0) m->ring0 = 0;
     struct tensor probe;
     m->quantized = find_tensor(m->blob, n, "q/scales", &probe);
     int ok = 1;
@@ -180,8 +192,8 @@ void mwwo_mixednet_reset(mwwo_mixednet *m) {
 /* fp32 invoke                                                               */
 
 float mwwo_mixednet_step_f32(mwwo_mixednet *m, const float *x /* [stride][40] */, float *logit_out) {
-    float mem[64 * NF];         /* concat(state, input) of the first conv: k0 rows */
-    float a[256], d[256], nxt[256];
+    float mem[MAX_KERNEL * NF];         /* concat(state, input) of the first conv: k0 rows */
+    float a[MAX_CHANNELS], d[MAX_CHANNELS], nxt[MAX_CHANNELS];
     const int k0 = m->k0, c0 = m->c0;
     memcpy(mem, m->ring_first, sizeof(float) * m->ring0 * NF);
     memcpy(mem + m->ring0 * NF, x, sizeof(float) * m->stride * NF);
@@ -257,7 +269,7 @@ static int8_t requant(int32_t acc, int32_t mult, int shift, int zp_out, int relu
 }
 
 int mwwo_mixednet_step_int8(mwwo_mixednet *m, const int8_t *x /* [stride][40] */, int *logit_out) {
-    int8_t mem[64 * NF], a[256], d[256], nxt[256];
+    int8_t mem[MAX_KERNEL * NF], a[MAX_CHANNELS], d[MAX_CHANNELS], nxt[MAX_CHANNELS];
     const int k0 = m->k0, c0 = m->c0;
     const int32_t *zp = m->qzps;
     memcpy(mem, m->qring_first, (size_t)m->ring0 * NF);
@@ -315,8 +327,8 @@ int mwwo_mixednet_step_int8(mwwo_mixednet *m, const int8_t *x /* [stride][40] */
 size_t mwwo_mixednet_predict_u16(mwwo_mixednet *m, const uint16_t *feat, size_t rows, float *probs, size_t max_probs) {
     const int s = m->stride;
     size_t n = 0;
-    float xf[16 * NF];
-    int8_t xq[16 * NF];
+    float xf[MAX_KERNEL * NF];                     /* one step's rows: stride <= k0 <= MAX_KERNEL */
+    int8_t xq[MAX_KERNEL * NF];
     for (size_t last = (size_t)s; last <= rows; last += (size_t)s) {
         const uint16_t *chunk = feat + (last - s) * NF;
         for (int i = 0; i < s * NF; ++i) xf[i] = (float)chunk[i] * 0.0390625f;      /* inference.py:94 */

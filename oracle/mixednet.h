@@ -12,7 +12,9 @@ extern "C" {
 
 typedef struct mwwo_mixednet mwwo_mixednet;
 
-/* blob = MWW container bytes (copied).  NULL on a malformed / incomplete container. */
+/* blob = MWW container bytes (copied).  NULL on a malformed / incomplete container, or on an architecture outside what the
+ * per-step buffers hold: 1..8 blocks, 1..4 MixConv groups per block, 1..512 channels per layer, 1..64 taps per kernel,
+ * 1..64 head rows, 1 <= stride <= first_conv_kernel_size. */
 mwwo_mixednet *mwwo_mixednet_create(const void *blob, size_t n);
 void mwwo_mixednet_free(mwwo_mixednet *m);
 void mwwo_mixednet_reset(mwwo_mixednet *m);

@@ -201,7 +201,8 @@ class KerasStreamingF32:
             net = np.maximum(net, np.float32(0)).astype(np.float32)
         # Stream(Identity, ring=T-1) -> Flatten -> Dense(1, sigmoid)   mixednet.py:362-384
         mem = np.concatenate([self.st_head, net], 0)
-        self.st_head = mem[-self.st_head.shape[0]:]
+        if self.st_head.shape[0]:                    # a 1-row head keeps no history: mem[-0:] would be the whole window
+            self.st_head = mem[-self.st_head.shape[0]:]
         logit = (mem.reshape(1, -1) @ p["dense/kernel"])[0, 0] + p["dense/bias"][0]
         return _sigmoid(logit)
 
@@ -235,7 +236,8 @@ class FoldedStreamingF32:
             d = (mem * t["b%d/dw/w" % i]).sum(0, dtype=np.float32) + t["b%d/dw/b" % i]
             net = np.maximum((d @ t["b%d/pw/w" % i]).astype(np.float32) + t["b%d/pw/b" % i], np.float32(0))
         mem = np.concatenate([self.st_head, net[None, :]], 0)
-        self.st_head = mem[-self.st_head.shape[0]:]
+        if self.st_head.shape[0]:                    # a 1-row head keeps no history: mem[-0:] would be the whole window
+            self.st_head = mem[-self.st_head.shape[0]:]
         logit = np.float32((mem * t["head/w"]).sum(dtype=np.float32) + t["head/b"][0])
         return logit if want_logit else _sigmoid(logit)
 
@@ -259,9 +261,100 @@ class FoldedStreamingF32:
             net = np.maximum((d @ t["b%d/pw/w" % i]).astype(np.float32) + t["b%d/pw/b" % i], np.float32(0))
             acts["p%d" % (i + 1)] = net
         mem = np.concatenate([self.st_head, net[None, :]], 0)
-        self.st_head = mem[-self.st_head.shape[0]:]
+        if self.st_head.shape[0]:                    # a 1-row head keeps no history: mem[-0:] would be the whole window
+            self.st_head = mem[-self.st_head.shape[0]:]
         acts["fc"] = np.float32((mem * t["head/w"]).sum(dtype=np.float32) + t["head/b"][0])
         return acts
+
+
+# --------------------------------------------------------------------------------------
+# float64 streaming model with a running bound on the error of ANY fp32 evaluation of the same folded graph
+
+U32 = 2.0 ** -24            # unit roundoff of float32
+PROB_SLACK = 2.0 ** -20     # expf and the division of a float32 sigmoid
+
+
+def gamma(n: int) -> float:
+    """gamma_n = n u / (1 - n u): a sum of n products in float32, in any order, with or without fused multiply-adds, is
+    within gamma_n * sum |products| of the exact sum (Higham, Accuracy and Stability of Numerical Algorithms, 3.1)."""
+    return n * U32 / (1.0 - n * U32)
+
+
+def _dot_bound(x, ex, w, b=None, axis=0):
+    """exact (float64) value of sum(x * w, axis) (+ b) and the bound on its fp32 evaluation from inputs known to within ex:
+    E = sum |w| ex + gamma_{n+1} (sum |w| (|x| + ex) + |b|)  -- the n + 1 counts the bias add; |x| + ex bounds the
+    fp32 input the evaluation actually multiplies."""
+    aw = np.abs(w)
+    n = x.shape[axis] + (b is not None)
+    y = (x * w).sum(axis)
+    e = (ex * aw).sum(axis) + gamma(n) * ((np.abs(x) + ex) * aw).sum(axis)
+    if b is not None:
+        y = y + b
+        e = e + gamma(n) * np.abs(b)
+    return y, e
+
+
+def _relu_bound(y, e):
+    """ReLU of a value known to within e: relu is 1-Lipschitz, and an input below -e is negative in fp32 too, so its output
+    is exactly 0 there -- the bound is the widest move of relu over [y - e, y + e]"""
+    r = np.maximum(y, 0.0)
+    return r, np.maximum(np.maximum(y + e, 0.0) - r, r - np.maximum(y - e, 0.0))
+
+
+class StreamingF64:
+    """FoldedStreamingF32's graph in float64.  Next to every value it carries E, a bound on how far an fp32 evaluation of
+    the same graph (any summation order, fmaf or not) can be from it: inputs are exact (E = 0; a uint16 feature x
+    0.0390625 is exact in float32), every dot product adds its rounding bound (_dot_bound), ReLU passes E through (_relu_bound), every
+    ring entry keeps its own E, and |p - p64| <= E_logit / 4 + PROB_SLACK (the sigmoid's slope is at most 1/4).
+    The bound assumes nothing about loop structure, so it checks a kernel whatever order it sums in."""
+
+    def __init__(self, tensors: dict):
+        self.spec = Spec.decode(tensors["arch"])
+        self.w0 = tensors["first_conv/w"].astype(np.float64).reshape(-1, self.spec.first_conv_filters)
+        self.blk = [tuple(tensors["b%d/%s" % (i, n)].astype(np.float64) for n in ("dw/w", "dw/b", "pw/w", "pw/b"))
+                    for i in range(self.spec.n_blocks)]
+        self.head_w = tensors["head/w"].astype(np.float64)
+        self.head_b = float(tensors["head/b"][0])
+        self.reset()
+
+    def reset(self):
+        s = self.spec
+        self.st_first = np.zeros((s.first_conv_kernel_size - s.stride, NUM_FEATURES))
+        self.st_block = [np.zeros((max(s.mixconv_kernel_sizes[i]) - 1, s.cin(i))) for i in range(s.n_blocks)]
+        self.st_head = np.zeros((s.head_rows - 1, s.pointwise_filters[-1]))
+        self.e_block = [np.zeros_like(r) for r in self.st_block]
+        self.e_head = np.zeros_like(self.st_head)
+
+    @staticmethod
+    def _push(ring, row):
+        mem = np.concatenate([ring, row[None, :]], 0)
+        return mem, (mem[1:] if ring.shape[0] else ring)
+
+    def step(self, x):
+        """x: [stride, 40] rows as the fp32 model sees them -> (p64, bound on |p - p64|, logit64, bound on the logit)"""
+        s = self.spec
+        x = np.asarray(x, np.float32).astype(np.float64).reshape(s.stride, NUM_FEATURES)
+        mem = np.concatenate([self.st_first, x], 0)
+        if self.st_first.shape[0]:
+            self.st_first = mem[-self.st_first.shape[0]:]
+        flat = mem.reshape(-1, 1)
+        net, e = _relu_bound(*_dot_bound(flat, np.zeros_like(flat), self.w0))
+        for i, (dw, db, pw, pb) in enumerate(self.blk):
+            mem, self.st_block[i] = self._push(self.st_block[i], net)
+            emem, self.e_block[i] = self._push(self.e_block[i], e)
+            d, ed = _dot_bound(mem, emem, dw, db)
+            net, e = _relu_bound(*_dot_bound(d[:, None], ed[:, None], pw, pb))
+        mem, self.st_head = self._push(self.st_head, net)
+        emem, self.e_head = self._push(self.e_head, e)
+        logit, el = _dot_bound(mem.reshape(-1), emem.reshape(-1), self.head_w.reshape(-1), np.float64(self.head_b))
+        p = 1.0 / (1.0 + np.exp(-logit))
+        return float(p), float(el / 4.0 + PROB_SLACK), float(logit), float(el)
+
+    def state(self):
+        """(values, bounds) of the ring state in the engine's per-stream layout: first-conv ring, block rings, head ring"""
+        vals = np.concatenate([self.st_first.ravel()] + [r.ravel() for r in self.st_block] + [self.st_head.ravel()])
+        errs = np.concatenate([np.zeros(self.st_first.size)] + [r.ravel() for r in self.e_block] + [self.e_head.ravel()])
+        return vals, errs
 
 
 def nonstreaming_logits(tensors: dict, spectrogram: np.ndarray) -> np.ndarray:
@@ -513,7 +606,8 @@ class StreamingInt8:
             net = self._requant(acc, "q/b%d/pw" % i, zp[pn], True)
             prev = pn
         mem = np.concatenate([self.st_head, net[None, :]], 0)
-        self.st_head = mem[-self.st_head.shape[0]:]
+        if self.st_head.shape[0]:                    # a 1-row head keeps no history: mem[-0:] would be the whole window
+            self.st_head = mem[-self.st_head.shape[0]:]
         acc = ((mem.astype(np.int64) - zp[prev]) * q["q/head/w"].astype(np.int64)).sum() + int(q["q/head/bias"][0])
         logit = int(np.clip(mbqm(acc, int(q["q/head/mult"][0]), int(q["q/head/shift"][0])) + zp["fc"], -128, 127))
         if want_logit:

@@ -25,6 +25,8 @@
 
 #define NF 40
 #define MAX_BLOCKS 8
+#define MAX_CHANNELS 512                           /* per layer; the per-step buffers of hyref_step hold this many */
+#define MAX_KERNEL 64                              /* taps of the first conv (and so its largest stride), of a MixConv group, head rows */
 
 struct tensor { const void *data; uint32_t dtype, nbytes; };
 struct dir_entry { char name[48]; uint32_t dtype, ndim, shape[4]; uint64_t offset, nbytes; };
@@ -101,7 +103,16 @@ hyref *hyref_create(const void *blob, size_t n) {
     const int n_arch = (int)(arch.nbytes / 4);
     m->c0 = a[0]; m->k0 = a[1]; m->stride = a[2]; m->n_blocks = a[4]; m->head_rows = a[5];
     if (a[3] != NF || m->n_blocks < 1 || m->n_blocks > MAX_BLOCKS || n_arch < 6 + 6 * m->n_blocks) { hyref_free(m); return NULL; }
-    m->ring0 = m->k0 - m->stride > 0 ? m->k0 - m->stride : 0;
+    /* a model outside what the fixed-size step buffers hold is refused, never run */
+    if (m->c0 < 1 || m->c0 > MAX_CHANNELS || m->k0 < 1 || m->k0 > MAX_KERNEL || m->stride < 1 || m->stride > m->k0 ||
+        m->head_rows < 1 || m->head_rows > MAX_KERNEL) { hyref_free(m); return NULL; }
+    for (int i = 0; i < m->n_blocks; ++i) {
+        const int32_t *e = a + 6 + 6 * i;
+        if (e[0] < 1 || e[0] > MAX_CHANNELS || e[1] < 1 || e[1] > 4) { hyref_free(m); return NULL; }
+        for (int j = 0; j < e[1]; ++j)
+            if (e[2 + j] < 1 || e[2 + j] > MAX_KERNEL) { hyref_free(m); return NULL; }
+    }
+    m->ring0 = m->k0 - m->stride;
     int n_slots = 2;
     for (int i = 0; i < m->n_blocks; ++i) n_slots += a[6 + 6 * i + 1] + 1;
     int32_t mode[2 + MAX_BLOCKS * 5];
@@ -145,7 +156,7 @@ hyref *hyref_create(const void *blob, size_t n) {
         }
         if ((size_t)cin > max_in) max_in = (size_t)cin;
         b->ring = (float *)calloc((size_t)(b->kmax - 1) * cin + 1, sizeof(float));
-        if (!b->ring || cin > 256 || b->cout > 256) ok = 0;
+        if (!b->ring) ok = 0;
         cin = b->cout;
     }
     m->head_w = (const float *)need(m, "head/w", &ok);
@@ -157,7 +168,7 @@ hyref *hyref_create(const void *blob, size_t n) {
     m->ring_head = (float *)calloc((size_t)(m->head_rows - 1) * cin + 1, sizeof(float));
     m->hx = (float *)malloc(max_in * sizeof(float));
     m->hq = (int8_t *)malloc(max_in);
-    if (!ok || m->k0 > 64 || m->c0 > 256 || !m->ring_first || !m->ring_head || !m->hx || !m->hq) { hyref_free(m); return NULL; }
+    if (!ok || !m->ring_first || !m->ring_head || !m->hx || !m->hq) { hyref_free(m); return NULL; }
     hyref_reset(m);
     return m;
 }
@@ -223,7 +234,7 @@ static float conv_out(int32_t acc, float w_scale, float in_scale, float bias) {
 }
 
 float hyref_step(hyref *m, const float *x /* [stride][40] */, float *logit_out) {
-    float mem[64 * NF], a[256], d[256], nxt[256];
+    float mem[MAX_KERNEL * NF], a[MAX_CHANNELS], d[MAX_CHANNELS], nxt[MAX_CHANNELS];
     const int k0 = m->k0, c0 = m->c0;
     float *hx = m->hx;
     int8_t *hq = m->hq;
@@ -329,7 +340,7 @@ float hyref_step(hyref *m, const float *x /* [stride][40] */, float *logit_out) 
 size_t hyref_predict_u16(hyref *m, const uint16_t *feat, size_t rows, float *probs, size_t max_probs) {
     const int s = m->stride;
     size_t n = 0;
-    float xf[64 * NF];
+    float xf[MAX_KERNEL * NF];
     for (size_t last = (size_t)s; last <= rows; last += (size_t)s) {
         const uint16_t *chunk = feat + (last - s) * NF;
         for (int i = 0; i < s * NF; ++i) xf[i] = (float)chunk[i] * 0.0390625f;      /* inference.py:94 */

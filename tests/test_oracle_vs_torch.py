@@ -21,6 +21,7 @@ SPECS = {
     "stride2_three_groups": R.Spec(16, 6, 2, (40,), ((7, 11, 13),), head_rows=9),
     "uneven_split": R.Spec(20, 4, 1, (50, 30), ((3, 5, 7), (5, 9)), head_rows=4),       # 50 channels / 3 groups -> 18, 16, 16
     "block_without_mixconv": R.Spec(24, 6, 2, (32, 16, 24), ((3, 5), (1,), (7,)), head_rows=4),   # mixednet.py:346-348
+    "one_row_head": R.Spec(32, 6, 3, (48, 24), ((3,), (5,)), head_rows=1),                  # the head keeps no history
 }
 
 
