@@ -173,6 +173,46 @@ int mww_predict_clip_host(mww_t *h, const int16_t *h_audio, int n_samples, long 
 int mww_predict_clip_remote(mww_t *h, const int16_t *src_audio, int n_samples, long long audio_stride,
                             float *d_probs, int max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
 
+/* ---- several models over one frontend ---------------------------------------------------------------------------
+ * A deployment that listens for several wake words (and a VAD model) on the same audio runs one frontend and K models on
+ * its rows.  mww_create_multi makes a handle that carries K >= 1 models of any kind the containers describe (fp32
+ * okay_nabu, int8, other geometries and strides, hybrid) over ONE shared frontend: one window carry, one set of noise
+ * estimates, one buffered-sample counter and one hop; each model has its own weights, ring state, pending rows and stride.
+ * Each predict call runs the frontend once per stream tile and every model on that tile's rows, and on the staged paths
+ * copies each audio tile once.  Model k's probabilities, state and pending rows are bit-identical to those of a
+ * one-model handle of the same container given the same calls; the frontend state is that of any of them.
+ *   - mww_create_multi: blobs[k] / n_bytes[k] for k in [0, n_models), 1 <= n_models <= 64.  A model that fails to load
+ *     fails the create; mww_last_error(NULL) starts with "model <k>: ".  mww_create(blob, ...) is the K = 1 case.
+ *   - mww_model_count: K (0 for a frontend-only handle).  mww_get_model_info: model k's stride (input_feature_slices),
+ *     quantisation, state_bytes_per_stream, pending_rows and macs_per_step; the frontend fields are the shared ones.
+ *     mww_get_info reports model 0.
+ *   - the _multi predict calls take the arguments of their one-model counterparts with K output buffers: d_probs[k]
+ *     [n_streams][max_probs[k]], and h_probs_out[k] (may be NULL) = steps model k ran, which differ between models of
+ *     different strides or pending rows.  Every model's buffer is checked before anything is launched.  A 480-sample
+ *     call runs each okay_nabu model's live-step kernel (each model's rings rotate on their own).  The staged paths
+ *     (_host_multi, _remote_multi) poison the whole handle on a half-way failure, as their one-model counterparts do.
+ *   - mww_get_model_state / mww_set_model_state: model k's h_nn / h_pending in the layout of mww_get_state (with model
+ *     k's state_bytes_per_stream and stride - 1 pending rows) and its pending_rows counter; NULL pointers are skipped.
+ *   - mww_reset (all or by id), mww_reset_device_ids reset the frontend and every model; mww_reset_frontend,
+ *     mww_set_window_step and mww_features act on the shared frontend; mww_launch_count and mww_profile_* count every
+ *     model's launches.
+ *   - on a handle with K > 1, mww_predict_clip[_f32/_host/_remote], mww_infer_features and mww_copy_nn_state return
+ *     MWW_EINVAL, as do mww_get_state / mww_set_state given NN arrays or a nonzero pending_rows (called with those NULL /
+ *     0 they read / write the frontend state only): each would advance or replace state for one model only. */
+int mww_create_multi(const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams, mww_t **out);
+int mww_model_count(const mww_t *h);
+int mww_get_model_info(const mww_t *h, int k, mww_info *out);
+int mww_predict_clip_multi(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride,
+                           float *const *d_probs, const int *max_probs, int *h_probs_out, void *cu_stream);
+int mww_predict_clip_multi_f32(mww_t *h, const float *d_audio, int n_samples, long long audio_stride,
+                               float *const *d_probs, const int *max_probs, int *h_probs_out, void *cu_stream);
+int mww_predict_clip_host_multi(mww_t *h, const int16_t *h_audio, int n_samples, long long audio_stride,
+                                float *const *h_probs, const int *max_probs, int *h_probs_out);
+int mww_predict_clip_remote_multi(mww_t *h, const int16_t *src_audio, int n_samples, long long audio_stride,
+                                  float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
+int mww_get_model_state(mww_t *h, int k, void *h_nn, void *h_pending);
+int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending, int pending_rows);
+
 /* Per-stream state snapshot for checkpoint / tests (host buffers, synchronous).
  *   h_carry    int16 [n_streams][480]   window buffer (first `frontend_buffered` samples valid)
  *   h_estimate uint32 [n_streams][40]   noise estimates

@@ -24,6 +24,8 @@ EXPORTS = (
     "mww_ipc_alloc", "mww_ipc_open", "mww_ipc_close", "mww_ipc_free",
     "mww_predict_clip_remote", "mww_reset_device_ids", "mww_host_alloc", "mww_host_alloc_wc", "mww_host_free", "mww_bind_host_thread",
     "mww_set_window_step", "mww_features_f32", "mww_predict_clip_f32", "mww_copy_nn_state", "mww_accuracy_counts",
+    "mww_create_multi", "mww_model_count", "mww_get_model_info", "mww_predict_clip_multi", "mww_predict_clip_multi_f32",
+    "mww_predict_clip_host_multi", "mww_predict_clip_remote_multi", "mww_get_model_state", "mww_set_model_state",
 )
 
 
@@ -130,6 +132,23 @@ def lib() -> ctypes.CDLL:
     L.mww_set_window_step.argtypes = [vp, i32]
     L.mww_bind_host_thread.restype = i32
     L.mww_bind_host_thread.argtypes = [i32, pi]
+    L.mww_create_multi.restype = i32
+    L.mww_create_multi.argtypes = [vp, vp, i32, i32, i32, ctypes.POINTER(vp)]
+    L.mww_model_count.restype = i32
+    L.mww_model_count.argtypes = [vp]
+    L.mww_get_model_info.restype = i32
+    L.mww_get_model_info.argtypes = [vp, i32, ctypes.POINTER(MwwInfo)]
+    for name in ("mww_predict_clip_multi", "mww_predict_clip_multi_f32"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, ll, vp, vp, vp, vp]
+    L.mww_predict_clip_host_multi.restype = i32
+    L.mww_predict_clip_host_multi.argtypes = [vp, vp, i32, ll, vp, vp, vp]
+    L.mww_predict_clip_remote_multi.restype = i32
+    L.mww_predict_clip_remote_multi.argtypes = [vp, vp, i32, ll, vp, vp, vp, i32, vp]
+    L.mww_get_model_state.restype = i32
+    L.mww_get_model_state.argtypes = [vp, i32, vp, vp]
+    L.mww_set_model_state.restype = i32
+    L.mww_set_model_state.argtypes = [vp, i32, vp, vp, i32]
     _lib = L
     return L
 

@@ -51,7 +51,9 @@ bool find_tensor(const uint8_t *blob, size_t n, const char *name, Tensor *out) {
     return false;
 }
 
-const int32_t kOkayNabuArch[30] = {32, 5, 3, 40, 4, 17, 64, 1, 5, 0, 0, 0, 64, 2, 7, 11, 0, 0, 64, 2, 9, 15, 0, 0, 64, 1, 23, 0, 0, 0};
+constexpr int kMaxModels = 64;      // models one handle can carry (mww_create_multi)
+
+const int32_t kOkayNabuArch[30] ={32, 5, 3, 40, 4, 17, 64, 1, 5, 0, 0, 0, 64, 2, 7, 11, 0, 0, 64, 2, 9, 15, 0, 0, 64, 1, 23, 0, 0, 0};
 
 }  // namespace
 
@@ -109,6 +111,10 @@ struct mww_handle {
     LiveHeads live_heads{};
     bool no_live = false, no_fuse = false;
     long long launches = 0;
+    // the NN models the frontend feeds: {this} for a one-model handle, {} for a frontend-only one.  mww_create_multi adds
+    // models 1..K-1 as sub-handles that hold weights, ring state, pending rows and live heads only (no frontend state,
+    // scratch or pipeline); the handle owns them
+    std::vector<mww_t *> models;
     // optional per-kernel timing (mww_profile_*)
     bool profiling = false;
     std::vector<cudaEvent_t> prof_ev[4];   // start/stop pairs per kernel class
@@ -622,13 +628,16 @@ int upload_weights(mww_t *h, const uint8_t *blob, size_t n) {
     return MWW_OK;
 }
 
-int zero_state(mww_t *h, cudaStream_t st) {
+// a failure of model m's call is reported on the handle h the caller holds
+int model_rc(mww_t *h, const mww_t *m, int rc) {
+    if (rc != MWW_OK && m != h) h->err = m->err;
+    return rc;
+}
+
+// fresh rings and no pending rows for every stream of one model
+int zero_nn_state(mww_t *h, cudaStream_t st) {
     const size_t S = (size_t)h->n_streams;
-    CU(h, cudaMemsetAsync(h->d_carry, 0, S * kWindow * sizeof(int16_t), st));
-    CU(h, cudaMemsetAsync(h->d_estimate, 0, S * kNumChannels * sizeof(uint32_t), st));
-    h->used = 0;
     h->n_pend = 0;
-    if (!h->has_nn) return MWW_OK;
     if (h->quantized && h->generic) {
         CU(h, launch_gen_fill_state_i8(h->G, h->GQ, static_cast<int8_t *>(h->d_nn_state), static_cast<int8_t *>(h->d_pend), h->n_streams, nullptr, h->n_streams, st));
         h->launches += 1;
@@ -640,14 +649,24 @@ int zero_state(mww_t *h, cudaStream_t st) {
         CU(h, cudaMemsetAsync(h->d_pend, 0, S * h->pend_cap * kNumChannels * 4, st));
     }
     h->live_heads = LiveHeads{};
-    h->used = 0;
     h->n_pend = 0;
+    return MWW_OK;
+}
+
+int zero_state(mww_t *h, cudaStream_t st) {
+    const size_t S = (size_t)h->n_streams;
+    CU(h, cudaMemsetAsync(h->d_carry, 0, S * kWindow * sizeof(int16_t), st));
+    CU(h, cudaMemsetAsync(h->d_estimate, 0, S * kNumChannels * sizeof(uint32_t), st));
+    h->used = 0;
+    for (mww_t *m : h->models)
+        if (int rc = model_rc(h, m, zero_nn_state(m, st))) return rc;
     return MWW_OK;
 }
 
 void destroy_impl(mww_t *h) {
     if (!h) return;
     DeviceGuard guard(h->device);
+    for (size_t k = 1; k < h->models.size(); ++k) destroy_impl(h->models[k]);
     cudaFree(h->d_tables); cudaFree(h->d_weights); cudaFree(h->d_carry); cudaFree(h->d_estimate);
     cudaFree(h->d_nn_state); cudaFree(h->d_pend); cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
     for (int b = 0; b < 2; ++b) {
@@ -694,39 +713,92 @@ int features_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, lo
     return MWW_OK;
 }
 
-// mww_predict_clip / mww_predict_clip_f32
+// Per-model arguments of a predict call: model k writes its probabilities to probs[k] ([n_streams][max_probs[k]]) and runs
+// steps[k] model steps (its own stride and pending rows decide how many).  Checked for every model before anything is
+// launched, so a too-small buffer for one model leaves the whole handle untouched.
+struct NnOuts {
+    float *const *probs; const int *max_probs; int steps[kMaxModels];
+};
+int check_outs(mww_t *h, const char *who, int n_frames, float *const *probs, const int *max_probs, NnOuts *o) {
+    if (h->models.size() > 1 && (!probs || !max_probs)) return fail(h, MWW_EINVAL, std::string(who) + ": NULL output arrays");
+    o->probs = probs; o->max_probs = max_probs;
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        const mww_t *m = h->models[k];
+        o->steps[k] = (m->n_pend + n_frames) / m->stride;
+        if (o->steps[k] > max_probs[k] || (o->steps[k] > 0 && !probs[k]))
+            return fail(h, MWW_EINVAL, std::string(who) + ": probability buffer too small" +
+                                           (h->models.size() > 1 ? " for model " + std::to_string(k) : std::string()));
+    }
+    return MWW_OK;
+}
+// once per call, after the last tile: every model's pending rows and live ring heads move on
+void end_models_call(mww_t *h, int n_frames, const NnOuts &o, int *h_probs_out) {
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        mww_t *m = h->models[k];
+        end_nn_call(m, n_frames);
+        m->n_pend = (m->n_pend + n_frames) % m->stride;
+        if (h_probs_out) h_probs_out[k] = o.steps[k];
+    }
+}
+int begin_models_call(mww_t *h, int n_frames, cudaStream_t st) {
+    for (mww_t *m : h->models)
+        if (int rc = model_rc(h, m, begin_nn_call(m, n_frames, st))) return rc;
+    return MWW_OK;
+}
+// every model on one tile of frontend rows; probs[k] (pitch probs_stride[k]) points at the tile's first stream
+int run_models_tile(mww_t *h, int first, int n, int n_frames, float *const *probs, const long long *probs_stride, cudaStream_t st) {
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        mww_t *m = h->models[k];
+        if (int rc = model_rc(h, m, run_nn_tile(m, first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, probs[k], probs_stride[k], st))) return rc;
+    }
+    return MWW_OK;
+}
+
+// mww_predict_clip[_multi] / mww_predict_clip[_multi]_f32: the frontend runs once per stream tile, then every model on its rows
 template <typename T>
-int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
-                      int *h_probs_out, void *cu_stream) {
+int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                      const int *max_probs, int *h_probs_out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
     if (!h->has_nn) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     ENTER_STATEFUL(h);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
     const int n_frames = frames_for(h, n_samples);
-    const int n_steps = (h->n_pend + n_frames) / h->stride;
-    if (n_steps > max_probs || (n_steps > 0 && !d_probs)) return fail(h, MWW_EINVAL, std::string(who) + ": probability buffer too small");
+    NnOuts o;
+    int rc = check_outs(h, who, n_frames, d_probs, max_probs, &o);
+    if (rc) return rc;
     const int tile = tile_streams(h, n_frames, true);
-    int rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
+    rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
     if (rc) return rc;
-    rc = begin_nn_call(h, n_frames, st);
+    rc = begin_models_call(h, n_frames, st);
     if (rc) return rc;
+    const size_t K = h->models.size();
+    float *tile_probs[kMaxModels];
+    long long probs_stride[kMaxModels];
+    for (size_t k = 0; k < K; ++k) probs_stride[k] = max_probs[k];
     for (int first = 0; first < h->n_streams; first += tile) {
         const int n = std::min(tile, h->n_streams - first);
         rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames, h->d_feat,
                                (long long)n_frames * kNumChannels, st);
         if (rc) return rc;
-        rc = run_nn_tile(h, first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, d_probs + (size_t)first * max_probs, max_probs, st);
+        for (size_t k = 0; k < K; ++k) tile_probs[k] = d_probs[k] + (size_t)first * max_probs[k];
+        rc = run_models_tile(h, first, n, n_frames, tile_probs, probs_stride, st);
         if (rc) return rc;
     }
-    end_nn_call(h, n_frames);
+    end_models_call(h, n_frames, o, h_probs_out);
     if (n_samples > 0) {
         rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
         if (rc) return rc;
     }
     h->used = h->used + n_samples - n_frames * h->hop;
-    h->n_pend = (h->n_pend + n_frames) % h->stride;
-    if (h_probs_out) *h_probs_out = n_steps;
+    return MWW_OK;
+}
+
+// the one-model entry points refuse a handle that carries several models: advancing the shared frontend for one model
+// would leave the others' rows behind
+int refuse_multi(mww_t *h, const char *who, const char *instead) {
+    if (h && h->models.size() > 1)
+        return fail(h, MWW_EINVAL, std::string(who) + ": the handle carries " + std::to_string(h->models.size()) + " models; use " + instead);
     return MWW_OK;
 }
 
@@ -734,16 +806,9 @@ int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples
 
 extern "C" {
 
-int mww_create(const void *model_blob, size_t n_bytes, int device, int n_streams, mww_t **out) {
-    if (out) *out = nullptr;
-    if (!out || n_streams < 1) return fail(nullptr, MWW_EINVAL, "mww_create: bad arguments");
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0)
-        return fail(nullptr, MWW_ECUDA, std::string("no CUDA device available (this library has no CPU fallback): ") + cudaGetErrorString(e));
-    if (device < 0 || device >= count) return fail(nullptr, MWW_EINVAL, "mww_create: device index out of range");
-    DeviceGuard guard(device);
-    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+namespace {
+
+mww_t *new_handle(int device, int n_streams) {
     mww_t *h = new mww_handle();
     h->device = device;
     h->n_streams = n_streams;
@@ -754,20 +819,46 @@ int mww_create(const void *model_blob, size_t n_bytes, int device, int n_streams
     h->live_variant = getenv("MWW_LIVE_VARIANT") != nullptr ? atoi(getenv("MWW_LIVE_VARIANT")) : (getenv("MWW_LIVE_V2") != nullptr ? 2 : 3);
     if (const char *mb = getenv("MWW_SCRATCH_MB")) { const long v = atol(mb); if (v > 0) h->scratch_budget = (size_t)v << 20; }
     if (const char *mt = getenv("MWW_MIN_TILE_STREAMS")) { const long v = atol(mt); if (v > 0) h->min_tile_streams = (int)v; }
-    h->has_nn = model_blob != nullptr;
-    if (h->has_nn) {
-        uint64_t x = 1469598103934665603ull;
-        for (size_t i = 0; i < n_bytes; ++i) x = (x ^ static_cast<const uint8_t *>(model_blob)[i]) * 1099511628211ull;
-        h->model_hash = x;
-    }
+    return h;
+}
+
+// weights and per-stream NN state of one model container
+int load_model(mww_t *m, const void *model_blob, size_t n_bytes) {
+    uint64_t x = 1469598103934665603ull;
+    for (size_t i = 0; i < n_bytes; ++i) x = (x ^ static_cast<const uint8_t *>(model_blob)[i]) * 1099511628211ull;
+    m->model_hash = x;
+    int rc = upload_weights(m, static_cast<const uint8_t *>(model_blob), n_bytes);
+    if (rc) return rc;
+    const size_t S = (size_t)m->n_streams;
+    cudaError_t a = cudaMalloc(&m->d_nn_state, S * m->state_elems * elem_size(m));
+    if (a == cudaSuccess) a = cudaMalloc(&m->d_pend, S * m->pend_cap * kNumChannels * elem_size(m));
+    if (a != cudaSuccess) return fail(m, a == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("state allocation: ") + cudaGetErrorString(a));
+    return MWW_OK;
+}
+
+// mww_create (n_models 0: frontend-only, 1: one model) and mww_create_multi (`multi`: messages name the failing model's index)
+int create_impl(const char *who, const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams, mww_t **out, bool multi) {
+    int count = 0;
+    cudaError_t e = cudaGetDeviceCount(&count);
+    if (e != cudaSuccess || count == 0)
+        return fail(nullptr, MWW_ECUDA, std::string("no CUDA device available (this library has no CPU fallback): ") + cudaGetErrorString(e));
+    if (device < 0 || device >= count) return fail(nullptr, MWW_EINVAL, std::string(who) + ": device index out of range");
+    DeviceGuard guard(device);
+    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+    mww_t *h = new_handle(device, n_streams);
+    h->has_nn = n_models > 0;
     int rc = upload_tables(h);
-    if (rc == MWW_OK && h->has_nn) rc = upload_weights(h, static_cast<const uint8_t *>(model_blob), n_bytes);
+    for (int k = 0; rc == MWW_OK && k < n_models; ++k) {
+        mww_t *m = k == 0 ? h : new_handle(device, n_streams);
+        h->models.push_back(m);
+        rc = load_model(m, blobs[k], n_bytes[k]);
+        if (rc != MWW_OK && multi) h->err = "model " + std::to_string(k) + ": " + m->err;
+        else if (rc != MWW_OK) h->err = m->err;
+    }
     if (rc == MWW_OK) {
         const size_t S = (size_t)n_streams;
         cudaError_t a = cudaMalloc(&h->d_carry, S * kWindow * sizeof(int16_t));
         if (a == cudaSuccess) a = cudaMalloc(&h->d_estimate, S * kNumChannels * sizeof(uint32_t));
-        if (a == cudaSuccess && h->has_nn) a = cudaMalloc(&h->d_nn_state, S * h->state_elems * elem_size(h));
-        if (a == cudaSuccess && h->has_nn) a = cudaMalloc(&h->d_pend, S * h->pend_cap * kNumChannels * elem_size(h));
         if (a != cudaSuccess) rc = fail(h, a == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("state allocation: ") + cudaGetErrorString(a));
     }
     if (rc == MWW_OK) rc = zero_state(h, nullptr);
@@ -777,11 +868,36 @@ int mww_create(const void *model_blob, size_t n_bytes, int device, int n_streams
     return MWW_OK;
 }
 
+}  // namespace
+
+int mww_create(const void *model_blob, size_t n_bytes, int device, int n_streams, mww_t **out) {
+    if (out) *out = nullptr;
+    if (!out || n_streams < 1) return fail(nullptr, MWW_EINVAL, "mww_create: bad arguments");
+    return create_impl("mww_create", &model_blob, &n_bytes, model_blob != nullptr ? 1 : 0, device, n_streams, out, false);
+}
+
+int mww_create_multi(const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams, mww_t **out) {
+    if (out) *out = nullptr;
+    if (!out || n_streams < 1 || !blobs || !n_bytes) return fail(nullptr, MWW_EINVAL, "mww_create_multi: bad arguments");
+    if (n_models < 1 || n_models > kMaxModels)
+        return fail(nullptr, MWW_EINVAL, "mww_create_multi: n_models must be in [1, " + std::to_string(kMaxModels) + "]");
+    for (int k = 0; k < n_models; ++k)
+        if (!blobs[k]) return fail(nullptr, MWW_EINVAL, "mww_create_multi: model " + std::to_string(k) + " is NULL");
+    return create_impl("mww_create_multi", blobs, n_bytes, n_models, device, n_streams, out, true);
+}
+
+int mww_model_count(const mww_t *h) { return h ? (int)h->models.size() : 0; }
+
 int mww_destroy(mww_t *h) { destroy_impl(h); return MWW_OK; }
 
 const char *mww_last_error(const mww_t *h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
-long long mww_launch_count(const mww_t *h) { return h ? h->launches : 0; }
+long long mww_launch_count(const mww_t *h) {
+    if (!h) return 0;
+    long long n = h->launches;
+    for (size_t k = 1; k < h->models.size(); ++k) n += h->models[k]->launches;
+    return n;
+}
 
 int mww_copy_async(void *d_dst, const void *d_src, size_t bytes, void *cu_stream) {
     if (bytes == 0) return MWW_OK;
@@ -845,6 +961,7 @@ int mww_ipc_free(void *d_ptr, int device) {
 int mww_profile_enable(mww_t *h, int on) {
     if (!h) return MWW_EINVAL;
     h->profiling = on != 0;
+    for (mww_t *m : h->models) m->profiling = h->profiling;
     return MWW_OK;
 }
 
@@ -852,14 +969,17 @@ int mww_profile_read(mww_t *h, double *ms4, long long *counts4) {
     if (!h || !ms4 || !counts4) return MWW_EINVAL;
     ENTER(h);
     CU(h, cudaDeviceSynchronize());
-    for (int c = 0; c < 4; ++c) {
-        std::vector<cudaEvent_t> &v = h->prof_ev[c];
-        for (size_t i = 0; i + 1 < v.size(); i += 2) {
-            float ms = 0.f;
-            if (cudaEventElapsedTime(&ms, v[i], v[i + 1]) == cudaSuccess) { ms4[c] += ms; counts4[c] += 1; }
-            cudaEventDestroy(v[i]); cudaEventDestroy(v[i + 1]);
+    for (size_t k = 0; k < std::max<size_t>(h->models.size(), 1); ++k) {
+        mww_t *m = k == 0 ? h : h->models[k];
+        for (int c = 0; c < 4; ++c) {
+            std::vector<cudaEvent_t> &v = m->prof_ev[c];
+            for (size_t i = 0; i + 1 < v.size(); i += 2) {
+                float ms = 0.f;
+                if (cudaEventElapsedTime(&ms, v[i], v[i + 1]) == cudaSuccess) { ms4[c] += ms; counts4[c] += 1; }
+                cudaEventDestroy(v[i]); cudaEventDestroy(v[i + 1]);
+            }
+            v.clear();
         }
-        v.clear();
     }
     return MWW_OK;
 }
@@ -895,6 +1015,21 @@ int mww_get_info(const mww_t *h, mww_info *o) {
     return MWW_OK;
 }
 
+int mww_get_model_info(const mww_t *h, int k, mww_info *o) {
+    if (!h || !o || k < 0 || k >= (int)h->models.size()) return MWW_EINVAL;
+    const mww_t *m = h->models[k];
+    int rc = mww_get_info(h, o);             // the shared frontend's fields
+    if (rc) return rc;
+    o->is_quantized = m->quantized;
+    o->input_feature_slices = m->stride;
+    o->input_scale = m->in_scale; o->input_zero_point = m->in_zp;
+    o->output_scale = m->out_scale; o->output_zero_point = m->out_zp;
+    o->state_bytes_per_stream = (int)(m->state_elems * elem_size(m));
+    o->pending_rows = m->n_pend;
+    o->macs_per_step = (int)m->macs_per_step;
+    return MWW_OK;
+}
+
 namespace {
 
 // 4-byte fill of one per-stream record for a list of stream ids (device memory); ids outside [0, n_streams) are skipped
@@ -920,12 +1055,9 @@ int fill_by_id(mww_t *h, void *base, size_t bytes_per_stream, const int32_t *d_i
     return MWW_OK;
 }
 
-// fresh state for the listed streams: a handful of launches whatever the length of the list
-int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
-    if (n <= 0) return MWW_OK;
-    int rc = fill_by_id(h, h->d_carry, kWindow * sizeof(int16_t), d_ids, n, st);
-    if (rc == MWW_OK) rc = fill_by_id(h, h->d_estimate, kNumChannels * sizeof(uint32_t), d_ids, n, st);
-    if (rc != MWW_OK || !h->has_nn) return rc;
+// fresh rings for the listed streams of one model
+int reset_nn_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
+    int rc = MWW_OK;
     if (h->quantized && h->generic) {
         CU(h, launch_gen_fill_state_i8(h->G, h->GQ, static_cast<int8_t *>(h->d_nn_state), static_cast<int8_t *>(h->d_pend), n, d_ids, h->n_streams, st));
         h->launches += 1;
@@ -937,6 +1069,15 @@ int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
         rc = fill_by_id(h, h->d_nn_state, (size_t)h->state_elems * 4, d_ids, n, st);
         if (rc == MWW_OK) rc = fill_by_id(h, h->d_pend, (size_t)h->pend_cap * kNumChannels * 4, d_ids, n, st);
     }
+    return rc;
+}
+
+// fresh state for the listed streams: a handful of launches whatever the length of the list
+int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
+    if (n <= 0) return MWW_OK;
+    int rc = fill_by_id(h, h->d_carry, kWindow * sizeof(int16_t), d_ids, n, st);
+    if (rc == MWW_OK) rc = fill_by_id(h, h->d_estimate, kNumChannels * sizeof(uint32_t), d_ids, n, st);
+    for (size_t k = 0; rc == MWW_OK && k < h->models.size(); ++k) rc = model_rc(h, h->models[k], reset_nn_by_id(h->models[k], d_ids, n, st));
     return rc;
 }
 
@@ -1004,16 +1145,27 @@ int mww_features_f32(mww_t *h, const float *d_audio, int n_samples, long long au
 
 int mww_predict_clip(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
                      int *h_probs_out, void *cu_stream) {
-    return predict_clip_impl(h, "mww_predict_clip", d_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
+    if (int rc = refuse_multi(h, "mww_predict_clip", "mww_predict_clip_multi")) return rc;
+    return predict_clip_impl(h, "mww_predict_clip", d_audio, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out, cu_stream);
 }
 int mww_predict_clip_f32(mww_t *h, const float *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
                          int *h_probs_out, void *cu_stream) {
-    return predict_clip_impl(h, "mww_predict_clip_f32", d_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
+    if (int rc = refuse_multi(h, "mww_predict_clip_f32", "mww_predict_clip_multi_f32")) return rc;
+    return predict_clip_impl(h, "mww_predict_clip_f32", d_audio, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out, cu_stream);
+}
+int mww_predict_clip_multi(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                           const int *max_probs, int *h_probs_out, void *cu_stream) {
+    return predict_clip_impl(h, "mww_predict_clip_multi", d_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
+}
+int mww_predict_clip_multi_f32(mww_t *h, const float *d_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                               const int *max_probs, int *h_probs_out, void *cu_stream) {
+    return predict_clip_impl(h, "mww_predict_clip_multi_f32", d_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
 }
 
 int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, long long rows_stride, float *d_probs,
                        int max_probs, int *h_probs_out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
+    if (int rc = refuse_multi(h, "mww_infer_features", "mww_predict_clip_multi")) return rc;
     if (n_rows < 0 || (n_rows > 0 && !d_rows) || rows_stride < n_rows) return fail(h, MWW_EINVAL, "mww_infer_features: bad row arguments");
     if (row_type < 0 || row_type > 2) return fail(h, MWW_EINVAL, "mww_infer_features: unknown row_type");
     if (!h->has_nn) return fail(h, MWW_EINVAL, "mww_infer_features: frontend-only handle (created without a model)");
@@ -1054,8 +1206,20 @@ int ensure_pipeline(mww_t *h) {
 }
 
 // the tile loop proper; any error leaves work in flight -- the caller drains the streams and poisons the handle
-int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_stride, float *dst, int max_probs, bool dst_is_host,
-                 int tile, int n_frames, int n_steps) {
+// Model k's scores of a tile go to dst[k] at its stream pitch; for a host destination they are first written to the score
+// staging buffer, where model k's block of tile x max(steps, 1) floats starts at probs_tile_offset(o, tile, k).
+size_t probs_tile_offset(const mww_t *h, const NnOuts &o, int tile, size_t k) {
+    size_t off = 0;
+    for (size_t j = 0; j < k && j < h->models.size(); ++j) off += (size_t)tile * std::max(o.steps[j], 1);
+    return off;
+}
+
+int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_stride, const NnOuts &o, bool dst_is_host,
+                 int tile, int n_frames) {
+    const size_t K = h->models.size();
+    float *tile_probs[kMaxModels];
+    long long tile_probs_stride[kMaxModels];
+    for (size_t k = 0; k < K; ++k) tile_probs_stride[k] = dst_is_host ? std::max(o.steps[k], 1) : o.max_probs[k];
     int it = 0;
     for (int first = 0; first < h->n_streams; first += tile, ++it) {
         const int n = std::min(tile, h->n_streams - first);
@@ -1082,9 +1246,9 @@ int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_st
         if (dst_is_host && it >= 2) CU(h, cudaStreamWaitEvent(h->st_compute, h->ev_d2h[b], 0));   // score staging buffer drained
         int rc = run_frontend_tile(h, first, n, h->d_audio_tile[b], n_samples, n_samples, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
         if (rc) return rc;
-        float *tile_probs = dst_is_host ? h->d_probs_tile[b] : dst + (size_t)first * max_probs;
-        const long long tile_probs_stride = dst_is_host ? std::max(n_steps, 1) : max_probs;
-        rc = run_nn_tile(h, first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, tile_probs, tile_probs_stride, h->st_compute);
+        for (size_t k = 0; k < K; ++k)
+            tile_probs[k] = dst_is_host ? h->d_probs_tile[b] + probs_tile_offset(h, o, tile, k) : o.probs[k] + (size_t)first * o.max_probs[k];
+        rc = run_models_tile(h, first, n, n_frames, tile_probs, tile_probs_stride, h->st_compute);
         if (rc) return rc;
         if (n_samples > 0) {
             rc = run_carry_tile(h, first, n, h->d_audio_tile[b], n_samples, n_samples, n_frames, h->st_compute);
@@ -1094,9 +1258,10 @@ int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_st
         CU(h, cudaEventRecord(h->ev_compute[b], h->st_compute));
         if (dst_is_host) {
             CU(h, cudaStreamWaitEvent(h->st_d2h, h->ev_compute[b], 0));
-            if (n_steps > 0)
-                CU(h, cudaMemcpy2DAsync(dst + (size_t)first * max_probs, (size_t)max_probs * 4, h->d_probs_tile[b], (size_t)std::max(n_steps, 1) * 4,
-                                        (size_t)n_steps * 4, n, cudaMemcpyDeviceToHost, h->st_d2h));
+            for (size_t k = 0; k < K; ++k)
+                if (o.steps[k] > 0)
+                    CU(h, cudaMemcpy2DAsync(o.probs[k] + (size_t)first * o.max_probs[k], (size_t)o.max_probs[k] * 4, tile_probs[k],
+                                            (size_t)tile_probs_stride[k] * 4, (size_t)o.steps[k] * 4, n, cudaMemcpyDeviceToHost, h->st_d2h));
             CU(h, cudaEventRecord(h->ev_d2h[b], h->st_d2h));
         }
     }
@@ -1105,12 +1270,13 @@ int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_st
 
 // `caller` != nullptr-or-legacy semantics: the call is ordered after everything queued on `caller` so far, and `caller`
 // is made to wait for the call's last kernel (asynchronous variant).  host_sync: return only when dst is complete.
-int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_samples, long long audio_stride, float *dst, int max_probs,
-                        int *h_probs_out, bool dst_is_host, int want_tiles, cudaStream_t caller, bool host_sync) {
+int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_samples, long long audio_stride, float *const *dst,
+                        const int *max_probs, int *h_probs_out, bool dst_is_host, int want_tiles, cudaStream_t caller, bool host_sync) {
     const int n_frames = frames_for(h, n_samples);
-    const int n_steps = (h->n_pend + n_frames) / h->stride;
-    if (n_steps > max_probs || (n_steps > 0 && !dst)) return fail(h, MWW_EINVAL, std::string(who) + ": probability buffer too small");
-    int rc = ensure_pipeline(h);
+    NnOuts o;
+    int rc = check_outs(h, who, n_frames, dst, max_probs, &o);
+    if (rc) return rc;
+    rc = ensure_pipeline(h);
     if (rc) return rc;
     // tile so that copies and kernels of neighbouring tiles overlap: 16 tiles by default when there are enough streams (the
     // first tile's copy and the last tile's kernels are the only parts that cannot hide behind each other), but never
@@ -1121,7 +1287,7 @@ int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_sam
     rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
     if (rc) return rc;
     const size_t a_bytes = (size_t)tile * std::max(n_samples, 1) * sizeof(int16_t);
-    const size_t p_bytes = dst_is_host ? (size_t)tile * std::max(n_steps, 1) * sizeof(float) : 0;
+    const size_t p_bytes = dst_is_host ? probs_tile_offset(h, o, tile, h->models.size()) * sizeof(float) : 0;
     if (a_bytes > h->audio_tile_bytes || p_bytes > h->probs_tile_bytes) {
         CU(h, cudaDeviceSynchronize());
         for (int b = 0; b < 2; ++b) {
@@ -1145,10 +1311,10 @@ int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_sam
         for (int b = 0; b < 2; ++b) CU(h, cudaStreamWaitEvent(h->st_h2d, h->ev_compute[b], 0));
     for (cudaEvent_t e : h->tl_ev) cudaEventDestroy(e);       // a timeline describes the most recent staged call only
     h->tl_ev.clear();
-    rc = begin_nn_call(h, n_frames, h->st_compute);
+    rc = begin_models_call(h, n_frames, h->st_compute);
     if (rc == MWW_OK) {
         h->staged_used = true;
-        rc = staged_tiles(h, src, n_samples, audio_stride, dst, max_probs, dst_is_host, tile, n_frames, n_steps);
+        rc = staged_tiles(h, src, n_samples, audio_stride, o, dst_is_host, tile, n_frames);
     }
     if (rc != MWW_OK) {
         // some tiles' carry / ring state may already be updated, others not: drain and refuse further stateful calls
@@ -1165,32 +1331,28 @@ int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_sam
         CU(h, cudaEventRecord(h->ev_exit, h->st_compute));
         CU(h, cudaStreamWaitEvent(caller, h->ev_exit, 0));
     }
-    end_nn_call(h, n_frames);
+    end_models_call(h, n_frames, o, h_probs_out);
     h->used = h->used + n_samples - n_frames * h->hop;
-    h->n_pend = (h->n_pend + n_frames) % h->stride;
-    if (h_probs_out) *h_probs_out = n_steps;
     return MWW_OK;
 }
 
-}  // namespace
-
-int mww_predict_clip_host(mww_t *h, const int16_t *h_audio, int n_samples, long long audio_stride, float *h_probs, int max_probs,
-                          int *h_probs_out) {
+int predict_clip_host_impl(mww_t *h, const char *who, const int16_t *h_audio, int n_samples, long long audio_stride, float *const *h_probs,
+                           const int *max_probs, int *h_probs_out) {
     if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !h_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, "mww_predict_clip_host: bad audio arguments");
-    if (!h->has_nn) return fail(h, MWW_EINVAL, "mww_predict_clip_host: frontend-only handle (created without a model)");
+    if (n_samples < 0 || (n_samples > 0 && !h_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (!h->has_nn) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     ENTER_STATEFUL(h);
     // The call has no stream argument, so it cannot be ordered after one particular stream: it waits for everything the
     // device has been given so far (mww_reset / live calls queued on any stream touch the same per-stream state).
     CU(h, cudaDeviceSynchronize());
-    return predict_clip_staged(h, "mww_predict_clip_host", h_audio, n_samples, audio_stride, h_probs, max_probs, h_probs_out, true, 0, nullptr, true);
+    return predict_clip_staged(h, who, h_audio, n_samples, audio_stride, h_probs, max_probs, h_probs_out, true, 0, nullptr, true);
 }
 
-int mww_predict_clip_remote(mww_t *h, const int16_t *src_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
-                            int *h_probs_out, int n_tiles, void *cu_stream) {
+int predict_clip_remote_impl(mww_t *h, const char *who, const int16_t *src_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                             const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
     if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !src_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, "mww_predict_clip_remote: bad audio arguments");
-    if (!h->has_nn) return fail(h, MWW_EINVAL, "mww_predict_clip_remote: frontend-only handle (created without a model)");
+    if (n_samples < 0 || (n_samples > 0 && !src_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (!h->has_nn) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     bool local = n_samples == 0;
     if (!local) {
         DeviceGuard guard(h->device);
@@ -1201,10 +1363,34 @@ int mww_predict_clip_remote(mww_t *h, const int16_t *src_audio, int n_samples, l
     }
     // a source this GPU's kernels can address -- its own memory, or a peer's buffer mapped with mww_ipc_open, which reports this
     // device too -- is read in place by the frontend kernel unless the caller asks for the staged pipeline (n_tiles > 0)
-    if (local && n_tiles <= 0) return mww_predict_clip(h, src_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
+    if (local && n_tiles <= 0) return predict_clip_impl(h, who, src_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
     ENTER_STATEFUL(h);
-    return predict_clip_staged(h, "mww_predict_clip_remote", src_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, false, n_tiles,
+    return predict_clip_staged(h, who, src_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out, false, n_tiles,
                                static_cast<cudaStream_t>(cu_stream), false);
+}
+
+}  // namespace
+
+int mww_predict_clip_host(mww_t *h, const int16_t *h_audio, int n_samples, long long audio_stride, float *h_probs, int max_probs,
+                          int *h_probs_out) {
+    if (int rc = refuse_multi(h, "mww_predict_clip_host", "mww_predict_clip_host_multi")) return rc;
+    return predict_clip_host_impl(h, "mww_predict_clip_host", h_audio, n_samples, audio_stride, &h_probs, &max_probs, h_probs_out);
+}
+int mww_predict_clip_host_multi(mww_t *h, const int16_t *h_audio, int n_samples, long long audio_stride, float *const *h_probs,
+                                const int *max_probs, int *h_probs_out) {
+    return predict_clip_host_impl(h, "mww_predict_clip_host_multi", h_audio, n_samples, audio_stride, h_probs, max_probs, h_probs_out);
+}
+
+int mww_predict_clip_remote(mww_t *h, const int16_t *src_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                            int *h_probs_out, int n_tiles, void *cu_stream) {
+    if (int rc = refuse_multi(h, "mww_predict_clip_remote", "mww_predict_clip_remote_multi")) return rc;
+    return predict_clip_remote_impl(h, "mww_predict_clip_remote", src_audio, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out, n_tiles,
+                                    cu_stream);
+}
+int mww_predict_clip_remote_multi(mww_t *h, const int16_t *src_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                                  const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
+    return predict_clip_remote_impl(h, "mww_predict_clip_remote_multi", src_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out,
+                                    n_tiles, cu_stream);
 }
 
 // ---- host memory next to the GPU ---------------------------------------------------------------------------------
@@ -1317,6 +1503,8 @@ int mww_host_free(void *h_ptr) {
 
 int mww_get_state(mww_t *h, int16_t *h_carry, uint32_t *h_estimate, void *h_nn, void *h_pending) {
     if (!h) return MWW_EINVAL;
+    if (h_nn || h_pending)
+        if (int rc = refuse_multi(h, "mww_get_state", "mww_get_model_state for the NN state")) return rc;
     ENTER_STATEFUL(h);
     CU(h, cudaDeviceSynchronize());
     if (h_nn) {                                    // the exported layout is always the canonical oldest-first one
@@ -1336,6 +1524,8 @@ int mww_get_state(mww_t *h, int16_t *h_carry, uint32_t *h_estimate, void *h_nn, 
 int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const uint32_t *h_estimate, const void *h_nn,
                   const void *h_pending, int pending_rows) {
     if (!h) return MWW_EINVAL;
+    if (h_nn || h_pending || pending_rows != 0)
+        if (int rc = refuse_multi(h, "mww_set_state", "mww_set_model_state for the NN state and pending rows")) return rc;
     if (frontend_buffered < 0 || frontend_buffered >= kWindow || pending_rows < 0 || pending_rows > h->stride - 1)
         return fail(h, MWW_EINVAL, "mww_set_state: counters out of range");
     ENTER(h);
@@ -1350,12 +1540,47 @@ int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const
     }
     if (h_pending) CU(h, cudaMemcpy(h->d_pend, h_pending, S * h->pend_cap * kNumChannels * elem_size(h), cudaMemcpyHostToDevice));
     h->used = frontend_buffered;
-    h->n_pend = pending_rows;
+    if (h->models.size() <= 1) h->n_pend = pending_rows;     // several models: each keeps its own (mww_set_model_state)
+    return MWW_OK;
+}
+
+int mww_get_model_state(mww_t *h, int k, void *h_nn, void *h_pending) {
+    if (!h) return MWW_EINVAL;
+    if (k < 0 || k >= (int)h->models.size()) return fail(h, MWW_EINVAL, "mww_get_model_state: model index out of range");
+    ENTER_STATEFUL(h);
+    mww_t *m = h->models[k];
+    CU(h, cudaDeviceSynchronize());
+    if (h_nn) {                                    // the exported layout is always the canonical oldest-first one
+        if (int rc = model_rc(h, m, canonicalise_rings(m, nullptr))) return rc;
+        CU(h, cudaDeviceSynchronize());
+    }
+    const size_t S = (size_t)h->n_streams;
+    if (h_nn) CU(h, cudaMemcpy(h_nn, m->d_nn_state, S * m->state_elems * elem_size(m), cudaMemcpyDeviceToHost));
+    if (h_pending) CU(h, cudaMemcpy(h_pending, m->d_pend, S * m->pend_cap * kNumChannels * elem_size(m), cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+
+int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending, int pending_rows) {
+    if (!h) return MWW_EINVAL;
+    if (k < 0 || k >= (int)h->models.size()) return fail(h, MWW_EINVAL, "mww_set_model_state: model index out of range");
+    mww_t *m = h->models[k];
+    if (pending_rows < 0 || pending_rows > m->stride - 1) return fail(h, MWW_EINVAL, "mww_set_model_state: pending_rows out of range");
+    ENTER(h);
+    CU(h, cudaDeviceSynchronize());
+    const size_t S = (size_t)h->n_streams;
+    if (h_nn) {
+        CU(h, cudaMemcpy(m->d_nn_state, h_nn, S * m->state_elems * elem_size(m), cudaMemcpyHostToDevice));
+        m->live_heads = LiveHeads{};
+    }
+    if (h_pending) CU(h, cudaMemcpy(m->d_pend, h_pending, S * m->pend_cap * kNumChannels * elem_size(m), cudaMemcpyHostToDevice));
+    m->n_pend = pending_rows;
     return MWW_OK;
 }
 
 int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src_c, const int32_t *h_src_ids, int n, void *cu_stream) {
     if (!dst) return MWW_EINVAL;
+    if (int rc = refuse_multi(dst, "mww_copy_nn_state", "a one-model handle")) return rc;
+    if (src_c && src_c->models.size() > 1) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: the source handle carries several models");
     // canonicalising the source's rings changes their layout, not the state they hold
     mww_t *src = const_cast<mww_t *>(src_c);
     if (!src || n < 0 || (n > 0 && (!h_dst_ids || !h_src_ids))) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: bad arguments");

@@ -63,37 +63,39 @@ def bind_host_thread(device: int) -> int:
     return node.value
 
 
-class StreamEngine:
-    """`model`: path to (or bytes of) an MWW container or a streaming ``.tflite`` flatbuffer (recognised and converted by
-    ``tflite_file``, inference.py:36-45), or None for a frontend-only engine."""
+def load_model_blob(model) -> bytes | None:
+    """bytes of an MWW container from `model`: a path to (or bytes of) a container or a streaming ``.tflite`` flatbuffer
+    (recognised and converted by ``tflite_file``, inference.py:36-45); None stays None (a frontend-only engine)."""
+    if isinstance(model, (bytes, bytearray, memoryview)):
+        blob = bytes(model)
+    elif model is None:
+        return None
+    else:
+        with open(model, "rb") as f:
+            blob = f.read()
+    from . import tflite_file
+    if tflite_file.is_tflite(blob):
+        blob = tflite_file.container_from_tflite(blob)      # raises TfliteError for graphs outside the hot path
+    return blob
 
-    def __init__(self, model, n_streams: int = 1, device: int = 0):
-        if isinstance(model, (bytes, bytearray, memoryview)):
-            blob = bytes(model)
-        elif model is None:
-            blob = None
-        else:
-            with open(model, "rb") as f:
-                blob = f.read()
-        if blob is not None:
-            from . import tflite_file
-            if tflite_file.is_tflite(blob):
-                blob = tflite_file.container_from_tflite(blob)      # raises TfliteError for graphs outside the hot path
-        self._L = _lib.lib()
-        self._h = ctypes.c_void_p()
-        self._blob = blob  # keep alive during create
-        rc = self._L.mww_create(blob, len(blob) if blob else 0, int(device), int(n_streams), ctypes.byref(self._h))
-        if rc != 0:
-            msg = self._L.mww_last_error(None)
-            raise _lib.MwwError(rc, msg.decode() if msg else "mww_create failed")
-        self.n_streams = int(n_streams)
-        self.device = int(device)
-        self.info = self._info()
-        self.is_quantized = bool(self.info.is_quantized)
-        # geometry of the loaded model (mww_get_info): feature rows per model step, ring-state elements per stream
-        self.stride = max(int(self.info.input_feature_slices), 1)
-        self.state_elements = int(self.info.state_bytes_per_stream) // (1 if self.is_quantized else 4) if blob is not None else 0
-        self.hop = HOP          # samples between feature windows (set_window_step)
+
+def rows_for(buffered: int, n_samples: int, hop: int) -> int:
+    """feature rows a call of n_samples emits per stream when the frontend holds `buffered` samples"""
+    return (buffered + n_samples - WINDOW) // hop + 1 if buffered + n_samples >= WINDOW else 0
+
+
+def call_plan(buffered: int, n_samples: int, hop: int, pending_rows, strides):
+    """Bookkeeping of one call on a shared frontend feeding models of the given strides, each holding pending_rows[k]:
+    -> (rows emitted, [steps model k runs], samples buffered after the call, [rows model k holds after the call])."""
+    rows = rows_for(buffered, n_samples, hop)
+    steps = [(p + rows) // s for p, s in zip(pending_rows, strides)]
+    pending = [(p + rows) % s for p, s in zip(pending_rows, strides)]
+    return rows, steps, buffered + n_samples - rows * hop, pending
+
+
+class _Engine:
+    """What every engine has: a handle whose `n_streams` streams share one frontend, its argument checks, resets,
+    features, pinned host buffers and timing.  Subclasses create the handle and run the models."""
 
     # ------------------------------------------------------------------ plumbing
     def close(self):
@@ -124,10 +126,6 @@ class StreamEngine:
         return self._info().frontend_buffered
 
     @property
-    def pending_rows(self) -> int:
-        return self._info().pending_rows
-
-    @property
     def launch_count(self) -> int:
         return int(self._L.mww_launch_count(self._h))
 
@@ -142,6 +140,19 @@ class StreamEngine:
         if audio.stride(1) != 1 and audio.shape[1] > 1:
             raise ValueError("audio samples must be contiguous along the last dimension")
         return audio.shape[1], (audio.stride(0) if audio.shape[1] > 0 else 0), audio.dtype == torch.float32
+
+    def _check_host_audio(self, audio: np.ndarray) -> np.ndarray:
+        """int16 host audio [S, N] with contiguous samples (copied when they are not)"""
+        if audio.dtype != np.int16 or audio.ndim != 2 or audio.shape[0] != self.n_streams:
+            raise ValueError("audio must be an int16 array of shape [n_streams=%d, n_samples]" % self.n_streams)
+        if audio.strides[1] != 2 and audio.shape[1] > 1:
+            audio = np.ascontiguousarray(audio)
+        return audio
+
+    def _check_probs_out(self, out) -> None:
+        torch = _torch()
+        if out.dtype != torch.float32 or not out.is_cuda or not out.is_contiguous() or out.dim() != 2 or out.shape[0] != self.n_streams:
+            raise ValueError("out must be a contiguous CUDA float32 tensor [n_streams, >= steps]")
 
     # ------------------------------------------------------------------ operations
     def reset(self, stream_ids=None):
@@ -173,7 +184,7 @@ class StreamEngine:
         """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer."""
         torch = _torch()
         n, stride, is_f32 = self._check_audio(audio)
-        rows = max((self.frontend_buffered + n - WINDOW) // self.hop + 1, 0) if self.frontend_buffered + n >= WINDOW else 0
+        rows = rows_for(self.frontend_buffered, n, self.hop)
         if out is None:
             out = torch.empty((self.n_streams, max(rows, 1), NUM_FEATURES), dtype=torch.uint16, device=self._dev())
         elif (out.dtype != torch.uint16 or not out.is_cuda or not out.is_contiguous() or out.dim() != 3 or out.shape[0] != self.n_streams
@@ -183,6 +194,63 @@ class StreamEngine:
         fn = self._L.mww_features_f32 if is_f32 else self._L.mww_features
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
+
+    # ------------------------------------------------------------------ pinned host buffers next to the GPU
+    def host_buffer(self, shape, dtype=np.int16, write_combined: bool = False) -> np.ndarray:
+        """Pinned host array on the NUMA node this engine's GPU hangs off (mww_host_alloc): full-rate predict_clip_host copies
+        on a two-socket box whatever CPU the caller runs on.  Freed when the array (and every view of it) is gone."""
+        return host_array(shape, dtype, self.device, write_combined)
+
+    # ------------------------------------------------------------------ per-kernel device timing
+    KERNEL_CLASSES = ("k1_spectral", "k2_temporal", "mixednet", "carry_update")
+
+    def profile(self, on: bool) -> None:
+        _lib.check(self._h, self._L.mww_profile_enable(self._h, int(bool(on))))
+
+    def profile_read(self) -> dict:
+        """{class: (total_ms, launches)} accumulated since the last read (synchronises the device)."""
+        ms = (ctypes.c_double * 4)(0, 0, 0, 0)
+        cnt = (ctypes.c_longlong * 4)(0, 0, 0, 0)
+        _lib.check(self._h, self._L.mww_profile_read(self._h, ms, cnt))
+        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.KERNEL_CLASSES)}
+
+    def timeline_read(self, max_tiles: int = 256) -> np.ndarray:
+        """[tiles, 4] float32 ms (copy start, copy end, kernels start, kernels end; relative to tile 0's copy start) of the
+        most recent staged call made while profile(True) -- predict_clip_host / predict_clip_remote from a peer or host source."""
+        buf = (ctypes.c_float * (4 * max_tiles))()
+        n = ctypes.c_int32(0)
+        _lib.check(self._h, self._L.mww_timeline_read(self._h, buf, max_tiles, ctypes.byref(n)))
+        return np.ctypeslib.as_array(buf).reshape(max_tiles, 4)[:min(n.value, max_tiles)].copy()
+
+
+class StreamEngine(_Engine):
+    """`model`: path to (or bytes of) an MWW container or a streaming ``.tflite`` flatbuffer (recognised and converted by
+    ``tflite_file``, inference.py:36-45), or None for a frontend-only engine."""
+
+    def __init__(self, model, n_streams: int = 1, device: int = 0):
+        blob = load_model_blob(model)
+        self._L = _lib.lib()
+        self._h = ctypes.c_void_p()
+        self._blob = blob  # keep alive during create
+        rc = self._L.mww_create(blob, len(blob) if blob else 0, int(device), int(n_streams), ctypes.byref(self._h))
+        if rc != 0:
+            msg = self._L.mww_last_error(None)
+            raise _lib.MwwError(rc, msg.decode() if msg else "mww_create failed")
+        self.n_streams = int(n_streams)
+        self.device = int(device)
+        self.info = self._info()
+        self.is_quantized = bool(self.info.is_quantized)
+        # geometry of the loaded model (mww_get_info): feature rows per model step, ring-state elements per stream
+        self.stride = max(int(self.info.input_feature_slices), 1)
+        self.state_elements = int(self.info.state_bytes_per_stream) // (1 if self.is_quantized else 4) if blob is not None else 0
+        self.hop = HOP          # samples between feature windows (set_window_step)
+
+    @property
+    def pending_rows(self) -> int:
+        return self._info().pending_rows
+
+    def _steps(self, n_samples: int) -> int:
+        return (self.pending_rows + rows_for(self.frontend_buffered, n_samples, self.hop)) // self.stride
 
     def infer(self, rows):
         """feature rows [S, R, 40] (uint16 / float32 / int8 CUDA tensor) -> float32 probabilities [S, steps]."""
@@ -222,9 +290,7 @@ class StreamEngine:
         samples are converted to int16 inside the frontend kernels (x * 32768, clipped, as audio_utils.to_int16)."""
         torch = _torch()
         n, stride, is_f32 = self._check_audio(audio)
-        buffered = self.frontend_buffered
-        rows = (buffered + n - WINDOW) // self.hop + 1 if buffered + n >= WINDOW else 0
-        steps = (self.pending_rows + rows) // self.stride
+        steps = self._steps(n)
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
         got = ctypes.c_int(0)
@@ -236,14 +302,9 @@ class StreamEngine:
 
     def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None) -> np.ndarray:
         """int16 HOST array [S, N] -> float32 HOST array [S, steps]; copies are pipelined inside the library."""
-        if audio.dtype != np.int16 or audio.ndim != 2 or audio.shape[0] != self.n_streams:
-            raise ValueError("audio must be an int16 array of shape [n_streams=%d, n_samples]" % self.n_streams)
-        if audio.strides[1] != 2 and audio.shape[1] > 1:
-            audio = np.ascontiguousarray(audio)
+        audio = self._check_host_audio(audio)
         n = audio.shape[1]
-        buffered = self.frontend_buffered
-        rows = (buffered + n - WINDOW) // self.hop + 1 if buffered + n >= WINDOW else 0
-        steps = (self.pending_rows + rows) // self.stride
+        steps = self._steps(n)
         if out is None:
             out = np.empty((self.n_streams, max(steps, 1)), np.float32)
         got = ctypes.c_int(0)
@@ -259,44 +320,15 @@ class StreamEngine:
         stream-ordered like predict_clip."""
         torch = _torch()
         n = int(n_samples)
-        buffered = self.frontend_buffered
-        rows = (buffered + n - WINDOW) // self.hop + 1 if buffered + n >= WINDOW else 0
-        steps = (self.pending_rows + rows) // self.stride
+        steps = self._steps(n)
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
-        elif out.dtype != torch.float32 or not out.is_cuda or not out.is_contiguous() or out.dim() != 2 or out.shape[0] != self.n_streams:
-            raise ValueError("out must be a contiguous CUDA float32 tensor [n_streams, >= steps]")
+        else:
+            self._check_probs_out(out)
         got = ctypes.c_int(0)
         _lib.check(self._h, self._L.mww_predict_clip_remote(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n, out.data_ptr(),
                                                            out.shape[1], ctypes.byref(got), int(tiles), self._cu_stream()))
         return out[:, :got.value]
-
-    # ------------------------------------------------------------------ pinned host buffers next to the GPU
-    def host_buffer(self, shape, dtype=np.int16, write_combined: bool = False) -> np.ndarray:
-        """Pinned host array on the NUMA node this engine's GPU hangs off (mww_host_alloc): full-rate predict_clip_host copies
-        on a two-socket box whatever CPU the caller runs on.  Freed when the array (and every view of it) is gone."""
-        return host_array(shape, dtype, self.device, write_combined)
-
-    # ------------------------------------------------------------------ per-kernel device timing
-    KERNEL_CLASSES = ("k1_spectral", "k2_temporal", "mixednet", "carry_update")
-
-    def profile(self, on: bool) -> None:
-        _lib.check(self._h, self._L.mww_profile_enable(self._h, int(bool(on))))
-
-    def profile_read(self) -> dict:
-        """{class: (total_ms, launches)} accumulated since the last read (synchronises the device)."""
-        ms = (ctypes.c_double * 4)(0, 0, 0, 0)
-        cnt = (ctypes.c_longlong * 4)(0, 0, 0, 0)
-        _lib.check(self._h, self._L.mww_profile_read(self._h, ms, cnt))
-        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.KERNEL_CLASSES)}
-
-    def timeline_read(self, max_tiles: int = 256) -> np.ndarray:
-        """[tiles, 4] float32 ms (copy start, copy end, kernels start, kernels end; relative to tile 0's copy start) of the
-        most recent staged call made while profile(True) -- predict_clip_host / predict_clip_remote from a peer or host source."""
-        buf = (ctypes.c_float * (4 * max_tiles))()
-        n = ctypes.c_int32(0)
-        _lib.check(self._h, self._L.mww_timeline_read(self._h, buf, max_tiles, ctypes.byref(n)))
-        return np.ctypeslib.as_array(buf).reshape(max_tiles, 4)[:min(n.value, max_tiles)].copy()
 
     # ------------------------------------------------------------------ state (checkpoint / tests)
     def state_dict(self) -> dict:
@@ -323,3 +355,123 @@ class StreamEngine:
         _lib.check(self._h, self._L.mww_set_state(self._h, carry.ctypes.data, int(d["frontend_buffered"]), est.ctypes.data,
                                                   nn.ctypes.data if nn is not None else None, pend.ctypes.data if pend is not None else None,
                                                   int(d.get("pending_rows", 0))))
+
+
+class MultiModelEngine(_Engine):
+    """K wake-word / VAD models over ONE frontend (mww_create_multi): every call runs the frontend once per stream tile and
+    each model on its rows, and the staged host / peer paths copy the audio once.  `models`: a list of paths to (or bytes
+    of) MWW containers or streaming ``.tflite`` flatbuffers, converted as StreamEngine converts them; any mix of kinds,
+    geometries and strides.  Calls return one result per model, in the order of `models`; model k's results and state are
+    bit-identical to a StreamEngine of models[k] given the same calls.  `stride`, `is_quantized`, `state_elements` and
+    `pending_rows` are per-model lists."""
+
+    def __init__(self, models, n_streams: int = 1, device: int = 0):
+        blobs = [load_model_blob(m) for m in models]
+        if any(b is None for b in blobs):
+            raise ValueError("every model must be a path or the bytes of a model file")
+        self._L = _lib.lib()
+        self._h = ctypes.c_void_p()
+        K = len(blobs)
+        self._bufs = [ctypes.create_string_buffer(b, len(b)) for b in blobs]
+        ptrs = (ctypes.c_void_p * max(K, 1))(*[ctypes.addressof(b) for b in self._bufs])
+        sizes = (ctypes.c_size_t * max(K, 1))(*[len(b) for b in blobs])
+        rc = self._L.mww_create_multi(ptrs, sizes, K, int(device), int(n_streams), ctypes.byref(self._h))
+        if rc != 0:
+            msg = self._L.mww_last_error(None)
+            raise _lib.MwwError(rc, msg.decode() if msg else "mww_create_multi failed")
+        self._bufs = None
+        self.n_streams = int(n_streams)
+        self.device = int(device)
+        self.n_models = K
+        infos = [self._model_info(k) for k in range(K)]
+        self.is_quantized = [bool(i.is_quantized) for i in infos]
+        self.stride = [max(int(i.input_feature_slices), 1) for i in infos]
+        self.state_elements = [int(i.state_bytes_per_stream) // (1 if q else 4) for i, q in zip(infos, self.is_quantized)]
+        self.hop = HOP
+
+    def _model_info(self, k: int):
+        info = _lib.MwwInfo()
+        _lib.check(self._h, self._L.mww_get_model_info(self._h, int(k), ctypes.byref(info)))
+        return info
+
+    @property
+    def pending_rows(self) -> list:
+        return [self._model_info(k).pending_rows for k in range(self.n_models)]
+
+    def _steps(self, n_samples: int) -> list:
+        return call_plan(self.frontend_buffered, n_samples, self.hop, self.pending_rows, self.stride)[1]
+
+    def _outs(self, steps, out, host: bool):
+        """-> (K buffers, their ctypes pointer / max_probs / steps-out arrays)"""
+        torch = _torch()
+        if out is None:
+            out = [np.empty((self.n_streams, max(s, 1)), np.float32) if host else
+                   torch.empty((self.n_streams, max(s, 1)), dtype=torch.float32, device=self._dev()) for s in steps]
+        elif len(out) != self.n_models:
+            raise ValueError("out must hold one buffer per model (%d)" % self.n_models)
+        elif host:
+            if any(o.dtype != np.float32 or o.ndim != 2 or o.shape[0] != self.n_streams or not o.flags.c_contiguous for o in out):
+                raise ValueError("out must be C-contiguous float32 host arrays [n_streams, >= steps]")
+        else:
+            for o in out:
+                self._check_probs_out(o)
+        K = self.n_models
+        ptrs = (ctypes.c_void_p * K)(*[o.ctypes.data if host else o.data_ptr() for o in out])
+        maxp = (ctypes.c_int * K)(*[o.shape[1] for o in out])
+        return out, ptrs, maxp, (ctypes.c_int * K)()
+
+    def predict_clip(self, audio, out=None) -> list:
+        """int16 or float32 CUDA tensor [S, N] -> [float32 probabilities [S, steps_k] for each model k]; state carries over
+        between calls.  `out`: one CUDA float32 buffer [S, >= steps_k] per model to write into."""
+        n, stride, is_f32 = self._check_audio(audio)
+        out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
+        fn = self._L.mww_predict_clip_multi_f32 if is_f32 else self._L.mww_predict_clip_multi
+        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), ptrs, maxp, got, self._cu_stream()))
+        return [o[:, :g] for o, g in zip(out, got)]
+
+    step = predict_clip
+
+    def predict_clip_host(self, audio: np.ndarray, out=None) -> list:
+        """int16 HOST array [S, N] -> [float32 HOST array [S, steps_k] for each model k]; each audio tile is copied once."""
+        audio = self._check_host_audio(audio)
+        n = audio.shape[1]
+        out, ptrs, maxp, got = self._outs(self._steps(n), out, True)
+        _lib.check(self._h, self._L.mww_predict_clip_host_multi(self._h, audio.ctypes.data, n, audio.strides[0] // 2 if n else 0, ptrs,
+                                                                maxp, got))
+        return [o[:, :g] for o, g in zip(out, got)]
+
+    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None) -> list:
+        """StreamEngine.predict_clip_remote for every model: one result per model, each audio tile pulled once."""
+        n = int(n_samples)
+        out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
+        _lib.check(self._h, self._L.mww_predict_clip_remote_multi(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n,
+                                                                  ptrs, maxp, got, int(tiles), self._cu_stream()))
+        return [o[:, :g] for o, g in zip(out, got)]
+
+    # ------------------------------------------------------------------ state (checkpoint / tests)
+    def state_dict(self) -> dict:
+        """{carry, estimate, frontend_buffered: the shared frontend; models: [{nn, pending, pending_rows} per model]}"""
+        S = self.n_streams
+        d = dict(carry=np.zeros((S, WINDOW), np.int16), estimate=np.zeros((S, NUM_FEATURES), np.uint32))
+        _lib.check(self._h, self._L.mww_get_state(self._h, d["carry"].ctypes.data, d["estimate"].ctypes.data, None, None))
+        d["frontend_buffered"] = self._info().frontend_buffered
+        d["models"] = []
+        for k in range(self.n_models):
+            dt = np.int8 if self.is_quantized[k] else np.float32
+            m = dict(nn=np.zeros((S, self.state_elements[k]), dt), pending=np.zeros((S, max(self.stride[k] - 1, 1), NUM_FEATURES), dt))
+            _lib.check(self._h, self._L.mww_get_model_state(self._h, k, m["nn"].ctypes.data, m["pending"].ctypes.data))
+            m["pending_rows"] = self._model_info(k).pending_rows
+            d["models"].append(m)
+        return d
+
+    def load_state_dict(self, d: dict) -> None:
+        if len(d["models"]) != self.n_models:
+            raise ValueError("the state holds %d models, this engine %d" % (len(d["models"]), self.n_models))
+        carry = np.ascontiguousarray(d["carry"], np.int16)
+        est = np.ascontiguousarray(d["estimate"], np.uint32)
+        _lib.check(self._h, self._L.mww_set_state(self._h, carry.ctypes.data, int(d["frontend_buffered"]), est.ctypes.data, None, None, 0))
+        for k, m in enumerate(d["models"]):
+            dt = np.int8 if self.is_quantized[k] else np.float32
+            nn = np.ascontiguousarray(m["nn"], dt)
+            pend = np.ascontiguousarray(m["pending"], dt)
+            _lib.check(self._h, self._L.mww_set_model_state(self._h, k, nn.ctypes.data, pend.ctypes.data, int(m["pending_rows"])))
