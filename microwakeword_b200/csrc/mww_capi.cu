@@ -71,6 +71,12 @@ struct mww_handle {
     NnWeightsF32 W;
     TcWeights TW{};                 // fp32 okay_nabu: pre-split weights for the wgmma clip kernel (mww_nn_tc.cu)
     bool no_tc = false;             // MWW_NO_TC: keep the mma.sync clip kernel (A/B measurements)
+    bool tc_tf32 = false;           // MWW_TC_TF32: keep the wgmma kernel's 3xTF32 operands (A/B measurements)
+    bool tc_f16 = false;            // the first conv's weights admit fp16 hi / lo operands (tc_f16_scales) and MWW_TC_TF32 is unset
+    // every carried first-conv ring / pending row is a feature (<= 2048) x 0.0390625: true after a full reset and after a predict
+    // call of >= kTcFreshSteps steps; false after infer_features (rows of any value); checked on a state set from outside
+    // (note_state_set).  The fp16 first conv needs it.
+    bool tc_rows_bounded = true;
     int live_variant = 3;           // MWW_LIVE_VARIANT: 3 = bulk-copy stages (default), 2 = warp-specialised with register loads, 1 = r01 kernel
     NnWeightsI8 Wq;
     float in_scale = 0.f, out_scale = 0.f;
@@ -335,7 +341,7 @@ int run_nn_tile(mww_t *h, int first, int n, const void *d_rows, int row_type, lo
     if (!h->no_tc && row_type == MWW_ROWS_U16 && (h->n_pend + n_rows) / 3 >= kTcMinSteps && reinterpret_cast<uintptr_t>(d_rows) % 16 == 0 &&
         (rows_stream_stride_rows * kNumChannels * 2) % 16 == 0) {
         // long calls on raw frontend rows: time is the M dimension of wgmma (mww_nn_tc.cu)
-        CU(h, launch_nn_f32_tc(h->W, h->TW, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
+        CU(h, launch_nn_f32_tc(h->W, h->TW, h->tc_f16 && h->tc_rows_bounded, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
                                static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend,
                                static_cast<const uint16_t *>(d_rows), rows_stream_stride_rows * kNumChannels, n_rows, d_probs, probs_stride, n,
                                h->sm_count, st));
@@ -538,7 +544,8 @@ int upload_weights(mww_t *h, const uint8_t *blob, size_t n) {
         if ((rc = get("head/w", 0, 17 * 64, (const void **)&h->W.head_w))) return rc;
         if ((rc = get("head/b", 0, 1, (const void **)&h->W.head_b))) return rc;
         {
-            // tensor-core operands: 3xTF32 split + slot layout, once per model (mww_nn_tc.h)
+            // tensor-core operands: 3xTF32 split + slot layout, and the first conv's fp16 operands where its weights admit them,
+            // once per model (mww_nn_tc.h)
             Tensor tw0, tpw[4];
             bool ok = find_tensor(blob, n, "first_conv/w", &tw0);
             const float *pw_host[4];
@@ -556,14 +563,20 @@ int upload_weights(mww_t *h, const uint8_t *blob, size_t n) {
                 memcpy(pw_copy[i].data(), pw_host[i], pw_copy[i].size() * 4);
                 pw_al[i] = pw_copy[i].data();
             }
+            const TcF16Scales sc = tc_f16_scales(w0_copy.data());
+            h->tc_f16 = sc.ok && !h->tc_tf32;
             std::vector<unsigned char> tcb;
-            size_t offs[5];
-            build_tc_weights(w0_copy.data(), pw_al, &tcb, offs);
+            size_t offs[6];
+            build_tc_weights(w0_copy.data(), pw_al, h->tc_f16 ? &sc : nullptr, &tcb, offs);
             const unsigned char *dev_tc = nullptr;
             if (cur + tcb.size() + 256 > total) return fail(h, MWW_EMODEL, "weight arena too small for the tensor-core operands");
             if (!upload(h->d_weights, cur, tcb.data(), tcb.size(), &dev_tc, &e)) return cuda_fail(h, e, "weight upload");
             h->TW.fc = dev_tc + offs[0];
             for (int i = 0; i < 4; ++i) h->TW.pw[i] = dev_tc + offs[1 + i];
+            if (h->tc_f16) {
+                h->TW.fc16 = dev_tc + offs[5];
+                h->TW.fc_out = ldexpf(1.f, -sc.s_fc);
+            }
         }
     } else {
         NnWeightsI8 &Q = h->Wq;
@@ -634,6 +647,27 @@ int model_rc(mww_t *h, const mww_t *m, int rc) {
     return rc;
 }
 
+// A state set from outside keeps the fp16 first conv only if every first-conv ring row (state floats [0, 80) of a stream) it
+// brings and every pending row in use is a feature u <= 2048 times 0.0390625, as the kernels leave them: a snapshot taken from
+// this library continues bit for bit on the kernel it left.
+bool rows_are_features(const float *v, size_t n) {
+    for (size_t i = 0; i < n; ++i) {
+        const float u = nearbyintf(v[i] * 25.6f);
+        if (!(u >= 0.f && u <= 2048.f && u * kFeatureScale == v[i])) return false;
+    }
+    return true;
+}
+void note_state_set(mww_t *m, const void *h_nn, const void *h_pending, int pending_rows) {
+    if (!h_nn && !h_pending) return;
+    bool ok = m->tc_f16 && (h_nn || m->tc_rows_bounded) && (h_pending || m->tc_rows_bounded);
+    for (int s = 0; ok && s < m->n_streams; ++s) {
+        if (h_nn) ok = rows_are_features(static_cast<const float *>(h_nn) + (size_t)s * m->state_elems, 2 * kNumChannels);
+        if (ok && h_pending)
+            ok = rows_are_features(static_cast<const float *>(h_pending) + (size_t)s * m->pend_cap * kNumChannels, (size_t)pending_rows * kNumChannels);
+    }
+    m->tc_rows_bounded = ok;
+}
+
 // fresh rings and no pending rows for every stream of one model
 int zero_nn_state(mww_t *h, cudaStream_t st) {
     const size_t S = (size_t)h->n_streams;
@@ -650,6 +684,7 @@ int zero_nn_state(mww_t *h, cudaStream_t st) {
     }
     h->live_heads = LiveHeads{};
     h->n_pend = 0;
+    h->tc_rows_bounded = true;
     return MWW_OK;
 }
 
@@ -736,6 +771,7 @@ void end_models_call(mww_t *h, int n_frames, const NnOuts &o, int *h_probs_out) 
     for (size_t k = 0; k < h->models.size(); ++k) {
         mww_t *m = h->models[k];
         end_nn_call(m, n_frames);
+        if (o.steps[k] >= kTcFreshSteps) m->tc_rows_bounded = true;      // first-conv ring, pending rows: this call's own rows
         m->n_pend = (m->n_pend + n_frames) % m->stride;
         if (h_probs_out) h_probs_out[k] = o.steps[k];
     }
@@ -816,6 +852,7 @@ mww_t *new_handle(int device, int n_streams) {
     h->no_live = getenv("MWW_NO_LIVE") != nullptr;
     h->no_fuse = getenv("MWW_NO_FUSE") != nullptr;
     h->no_tc = getenv("MWW_NO_TC") != nullptr;
+    h->tc_tf32 = getenv("MWW_TC_TF32") != nullptr;
     h->live_variant = getenv("MWW_LIVE_VARIANT") != nullptr ? atoi(getenv("MWW_LIVE_VARIANT")) : (getenv("MWW_LIVE_V2") != nullptr ? 2 : 3);
     if (const char *mb = getenv("MWW_SCRATCH_MB")) { const long v = atol(mb); if (v > 0) h->scratch_budget = (size_t)v << 20; }
     if (const char *mt = getenv("MWW_MIN_TILE_STREAMS")) { const long v = atol(mt); if (v > 0) h->min_tile_streams = (int)v; }
@@ -1174,6 +1211,7 @@ int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, l
     if (n_steps > max_probs || (n_steps > 0 && !d_probs)) return fail(h, MWW_EINVAL, "mww_infer_features: probability buffer too small");
     int rc = begin_nn_call(h, n_rows, static_cast<cudaStream_t>(cu_stream));
     if (rc) return rc;
+    h->tc_rows_bounded = false;         // the caller's rows may hold any value, and the state will carry them
     rc = run_nn_tile(h, 0, h->n_streams, d_rows, row_type, rows_stride, n_rows, d_probs, max_probs, static_cast<cudaStream_t>(cu_stream));
     if (rc == MWW_OK) end_nn_call(h, n_rows);
     if (rc) return rc;
@@ -1534,6 +1572,7 @@ int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const
     if (h_carry) CU(h, cudaMemcpy(h->d_carry, h_carry, S * kWindow * 2, cudaMemcpyHostToDevice));
     if (h_estimate) CU(h, cudaMemcpy(h->d_estimate, h_estimate, S * kNumChannels * 4, cudaMemcpyHostToDevice));
     if ((h_nn || h_pending) && !h->has_nn) return fail(h, MWW_EINVAL, "frontend-only handle has no NN state");
+    note_state_set(h, h_nn, h_pending, pending_rows);
     if (h_nn) {
         CU(h, cudaMemcpy(h->d_nn_state, h_nn, S * h->state_elems * elem_size(h), cudaMemcpyHostToDevice));
         h->live_heads = LiveHeads{};
@@ -1568,6 +1607,7 @@ int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending
     ENTER(h);
     CU(h, cudaDeviceSynchronize());
     const size_t S = (size_t)h->n_streams;
+    note_state_set(m, h_nn, h_pending, pending_rows);
     if (h_nn) {
         CU(h, cudaMemcpy(m->d_nn_state, h_nn, S * m->state_elems * elem_size(m), cudaMemcpyHostToDevice));
         m->live_heads = LiveHeads{};
@@ -1598,6 +1638,7 @@ int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src_c, 
     int rc = canonicalise_rings(src, st);
     if (rc) return fail(dst, rc, "mww_copy_nn_state: " + src->err);
     if (dst != src && (rc = canonicalise_rings(dst, st)) != MWW_OK) return rc;
+    dst->tc_rows_bounded = dst->tc_rows_bounded && src->tc_rows_bounded;
     const size_t bytes = (size_t)dst->state_elems * elem_size(dst);
     char *d = static_cast<char *>(dst->d_nn_state);
     const char *s = static_cast<const char *>(src->d_nn_state);

@@ -19,8 +19,11 @@
 //   * the epilogue takes the accumulator straight from the registers, adds the folded-BatchNorm bias, applies ReLU and writes the
 //     next layer's activations [channel][time] for the depthwise stage.
 // Depthwise taps, ring buffers, the 17-row head and the sigmoid stay on CUDA cores, in shared memory for the whole call.
+// The first conv runs on fp16 operands where it can (nn_f32_clip_tc_kernel<true>): the feature rows are integers, exact in fp16,
+// against fp16 hi / lo weights -- two wgmma.m64n32k16.f32.f16.f16 per K = 16 step.
 //
 // The mma.sync kernel (mww_nn.cu) remains the path for float32 feature rows and for calls shorter than kTcMinSteps steps.
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdlib>
 #include <cstring>
@@ -55,9 +58,11 @@ constexpr int kOffRing = kOffSmall + 8 * kNumChannels * 4;   // the next block's
 constexpr int kRingStageBytes = 22 * 64 * 4;                 // the largest ring: block 3's input
 constexpr int kOffBar = kOffRing + kRingStageBytes;          // mbarriers "B buffer b holds its slot" [2], release counters [2],
                                                              // mbarrier "the first conv's weights are in place"
-constexpr int kTcSmemBytes = kOffBar + 32;
+constexpr int kOffSmallU = kOffBar + 32;                      // fp16 kernel: the first-conv ring rows and pending rows as the
+                                                             // integer features they were made from [4][40] uint16
+constexpr int kTcSmemBytes = kOffSmallU + 4 * kNumChannels * 2;
 static_assert(2 * (kTcSmemBytes + 1024) <= 232448, "two CTAs per SM");
-static_assert(kOffRing % 16 == 0 && kOffBar % 8 == 0, "cp.async destinations and mbarriers are aligned");
+static_assert(kOffRing % 16 == 0 && kOffBar % 8 == 0 && kOffSmallU % 4 == 0, "cp.async destinations and mbarriers are aligned");
 static_assert(kFeatRows * kNumChannels * 2 <= 64 * kLdx * 4, "feature rows alias the activation buffer");
 static_assert(kOffA % 1024 == 0 && kOffB % 1024 == 0, "swizzled operand slots need 1024-byte alignment");
 
@@ -127,6 +132,16 @@ __device__ __forceinline__ void mma_tf32_ra32(float (&d)[32], const uint32_t (&a
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
                  "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+                   "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+// D[64 x 32] (+)= A[64 x 16] B[16 x 32], fp16 operands (B K-major), fp32 accumulator; A from registers: a[e] holds the fp16 pair
+// A[16 w + lane / 4 + 8 (e % 2)][2 (lane % 4) + 8 (e / 2) + {0, 1}] (low half first)
+__device__ __forceinline__ void mma_f16_ra32(float (&d)[32], const uint32_t (&a)[4], uint64_t db, int accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+                 "{%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}\n"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
                    "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
@@ -258,10 +273,10 @@ __device__ __forceinline__ void depthwise_slot(int tid, int n, const float *x, u
     depthwise_k<L, K>(32 * H + (tid & 31), t0, t1, x, a_base, W);
 }
 
-// accumulator [128 steps x N] -> (+ bias) ReLU -> X[o][hist + t] for t < n.  wgmma's fragment of warp w of warpgroup g: steps
-// 64 g + 16 (w % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1) in d[4 j + 2 h + e]
-template <int N_, int HIST>
-__device__ __forceinline__ void epilogue(int tid, int n, const float (&d)[32], float *x, const float *bias /* nullptr: none */) {
+// accumulator [128 steps x N] -> (x sc, the fp16 first conv's exact power of two) (+ bias) ReLU -> X[o][hist + t] for t < n.  wgmma's
+// fragment of warp w of warpgroup g: steps 64 g + 16 (w % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1) in d[4 j + 2 h + e]
+template <bool F16, int N_, int HIST>
+__device__ __forceinline__ void epilogue(int tid, int n, const float (&d)[32], float *x, const float *bias /* nullptr: none */, float sc) {
     const int lane = tid & 31;
     const int t0 = 64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + (lane >> 2);
     if (t0 - (lane >> 2) >= n) return;                        // warp-uniform: this warp's 16 steps are all beyond the chunk
@@ -273,7 +288,8 @@ __device__ __forceinline__ void epilogue(int tid, int n, const float (&d)[32], f
         for (int h = 0; h < 2; ++h) {
             const int t = t0 + 8 * h;
             if (t < n) {
-                const float r0 = d[4 * j + 2 * h] + b2.x, r1 = d[4 * j + 2 * h + 1] + b2.y;
+                const float r0 = F16 ? fmaf(d[4 * j + 2 * h], sc, b2.x) : d[4 * j + 2 * h] + b2.x;
+                const float r1 = F16 ? fmaf(d[4 * j + 2 * h + 1], sc, b2.y) : d[4 * j + 2 * h + 1] + b2.y;
                 x[c * kLdx + HIST + t] = r0 > 0.f ? r0 : 0.f;
                 x[(c + 1) * kLdx + HIST + t] = r1 > 0.f ? r1 : 0.f;
             }
@@ -288,6 +304,10 @@ __device__ __forceinline__ void epilogue(int tid, int n, const float (&d)[32], f
 // A slot), so between block ends the two warpgroups only meet at the weight buffers: a warpgroup waits on the mbarrier of the buffer
 // that holds slot i, and the second warpgroup to finish slot i refills that buffer with slot i + 2 (a bulk copy from L2).  The
 // CTA-wide barriers are left to the chunk start and the block ends, where the epilogues hand time steps across warpgroups.
+// F16: the first conv on fp16 operands in place of 3xTF32 -- its A is the integer feature itself (u <= kTcMaxFeature, exact in fp16;
+// 0.0390625 is folded into the weights, which are an fp16 hi / lo pair), so a K = 16 step takes two products, u W_hi and u W_lo,
+// where 3xTF32 takes six for the same K.  The 1x1 projections stay on 3xTF32: their activations have no usable a-priori range.
+template <bool F16>
 __global__ void __launch_bounds__(kTcThreads, 2)
 nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, float *__restrict__ pend, int n_pend, const uint16_t *__restrict__ rows,
                       long long rows_stream_stride, int n_rows, float *__restrict__ probs, long long probs_stream_stride, int n_streams) {
@@ -300,7 +320,8 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
     float *ring_stage = reinterpret_cast<float *>(smem + kOffRing);
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + kOffBar);        // full[b]: B buffer b holds the slot it was last loaded with
     unsigned *released = reinterpret_cast<unsigned *>(smem + kOffBar + 16);   // warpgroups done with B buffer b, counted for ever
-    uint64_t *fc_full = reinterpret_cast<uint64_t *>(smem + kOffBar + 24);     // the first conv's seven weight slots are in place
+    uint64_t *fc_full = reinterpret_cast<uint64_t *>(smem + kOffBar + 24);     // the first conv's weight slots are in place
+    uint16_t *small_u = reinterpret_cast<uint16_t *>(smem + kOffSmallU);        // fp16 kernel: small[0, 160) as integer features
     const int tid = threadIdx.x, wg = tid >> 7;
     // this warpgroup's 64 rows of the A slot (8 KB, a whole number of 1024-byte swizzle atoms)
     const uint32_t a_s = (uint32_t)__cvta_generic_to_shared(a_base) + (uint32_t)wg * 64 * 128, b_s = (uint32_t)__cvta_generic_to_shared(b_base);
@@ -310,12 +331,16 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
     // The 14 K-slots of a chunk, in order: first conv 0..6 (N = 32; the last holds K = 8), block 0 (one slot), blocks 1..3 (two each).
     // The first conv's seven slots (56 KB) arrive in one bulk copy at the start of a chunk and lie in the A slot and the B buffers, all
     // idle then: its A operand never touches shared memory (register fragments).  Slot i >= 7 sits in B buffer i % 2.
+    // fp16: the first conv's four 64-wide slots (32 KB) fill the A slot alone, so slots 7 and 8 are fetched into the B buffers with
+    // them.
+    constexpr unsigned kFcBytes = F16 ? 4 * 8192 : 7 * 8192;
     auto load_slot = [&](int i) {                        // one thread; 7 <= i < 14
         // pointers picked by comparison, not by index: an indexed kernel parameter array would be copied to local memory
         const unsigned char *src = i == 7 ? TW.pw[0] : (i < 10 ? TW.pw[1] : i < 12 ? TW.pw[2] : TW.pw[3]) + (size_t)((i - 8) & 1) * kBSlotBytes;
         bulk_load(b_base + (i & 1) * kBSlotBytes, src, (unsigned)kBSlotBytes, full + (i & 1));
     };
-    static_assert(kOffA == 0 && kOffB == 2 * kAPlaneBytes && 7 * 8192 <= kOffX, "the first conv's weights fit the A slot + B buffers");
+    static_assert(kOffA == 0 && kOffB == 2 * kAPlaneBytes && 7 * 8192 <= kOffX && 4 * 8192 <= kOffB,
+                  "the first conv's weights fit the A slot + B buffers (tf32) / the A slot (fp16)");
     if (tid == 0) {
         mbar_init(full, 1);
         mbar_init(full + 1, 1);
@@ -374,10 +399,12 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
             TC_PHASE(kPhStream);
             if (tid == 0) {
                 // every thread fenced its generic-proxy use of these bytes before the barrier that ended the previous chunk
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(fc_full)), "r"(7 * 8192) : "memory");
+                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(fc_full)), "r"(kFcBytes) : "memory");
                 asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem)),
-                             "l"(__cvta_generic_to_global(TW.fc)), "r"(7 * 8192), "r"(smem_u32(fc_full))
+                             "l"(__cvta_generic_to_global(F16 ? TW.fc16 : TW.fc)), "r"(kFcBytes), "r"(smem_u32(fc_full))
                              : "memory");
+                // fp16: the B buffers are idle during the first conv (the previous chunk's last MMAs completed before its head)
+                if constexpr (F16) { load_slot(7); load_slot(8); }
             }
             {
                 const int n16 = (row_hi - row_lo) * (kNumChannels * 2 / 16);                               // 5 x 16 bytes per row
@@ -403,6 +430,9 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
                 } else {
                     small[tid] = my_pend[tid - 80];
                 }
+                // these rows hold u x 0.0390625 for integer features u (the handle checks this before it picks the fp16 kernel):
+                // u = v x 25.6 to well within rounding
+                if constexpr (F16) small_u[tid] = (uint16_t)__float2int_rn(small[tid] * 25.6f);
             }
             cp_wait<0>();                                                  // the feature rows and block 0's ring are here
             __syncthreads();
@@ -423,49 +453,88 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
                 const int g_ta = 40 * (vr0 + 2) + 120 * ta + (lane & 3), g_pend = 40 * (n_pend + 2), g_rows = 40 * (n_pend + 2 + row_lo);
                 auto fc_slot = [&](auto ksteps, int slot) {
                     constexpr int KS = decltype(ksteps)::value;
-                    uint32_t a_hi[KS][4], a_lo[KS][4];
+                    if constexpr (F16) {
+                        // 64-wide slot: element pair (t, k, k + 1), k = 64 slot + 16 ks + 2 (lane % 4) + 8 (e / 2), is the two
+                        // features at g, g + 1 (g even: one 32-bit load), converted exactly to an fp16 pair
+                        uint32_t a[KS][4];
+                        const uint32_t *small2 = reinterpret_cast<const uint32_t *>(small_u), *feat2 = reinterpret_cast<const uint32_t *>(feat);
+                        const int g_ta2 = g_ta + (lane & 3);                  // 2 (lane % 4) from row -2
 #pragma unroll
-                    for (int ks = 0; ks < KS; ++ks)
+                        for (int ks = 0; ks < KS; ++ks)
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            // steps 0 and 1 of a call's first chunk can touch the first-conv ring / the pending rows (virtual rows
-                            // -2 .. n_pend - 1, in small); steps beyond the chunk contribute zero rows, never stored.  Both
-                            // loads are made and one is selected: register fragments fed by divergent code would serialise the wgmmas
-                            const int t = ta + 8 * (e & 1), g = g_ta + 960 * (e & 1) + 32 * slot + 8 * ks + 4 * (e >> 1);
-                            const float from_small = small[min(g, 4 * kNumChannels - 1)];
-                            const float from_rows = (float)feat[max(g - g_rows, 0)] * kFeatureScale;
-                            const float v = t < n ? (g < g_pend ? from_small : from_rows) : 0.f;
-                            float hi, lo;
-                            split_tf32f(v, hi, lo);
-                            a_hi[ks][e] = __float_as_uint(hi);
-                            a_lo[ks][e] = __float_as_uint(lo);
+                            for (int e = 0; e < 4; ++e) {
+                                const int t = ta + 8 * (e & 1), g = g_ta2 + 960 * (e & 1) + 64 * slot + 16 * ks + 8 * (e >> 1);
+                                const uint32_t from_small = small2[min(g, 4 * kNumChannels - 2) >> 1];
+                                const uint32_t from_rows = feat2[max(g - g_rows, 0) >> 1];
+                                // k >= 200 (the second half of the last slot's K = 16 step) reads past the chunk's rows: zero, not
+                                // whatever the buffer holds (its weights are zero, but an fp16 inf times zero is not)
+                                const uint32_t v = (t < n && !(KS == 1 && e >= 2)) ? (g < g_pend ? from_small : from_rows) : 0u;
+                                const __half2 h = __halves2half2(__ushort2half_rn((unsigned short)(v & 0xFFFFu)), __ushort2half_rn((unsigned short)(v >> 16)));
+                                a[ks][e] = *reinterpret_cast<const uint32_t *>(&h);
+                            }
+                        const uint32_t b_hi0 = fc_s + (uint32_t)slot * 8192;
+                        fence_acc(acc);
+                        asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
+#pragma unroll
+                        for (int ks = 0; ks < KS; ++ks) {
+                            const uint32_t b_hi = b_hi0 + (uint32_t)ks * 32, b_lo = b_hi + 4096;
+                            mma_f16_ra32(acc, a[ks], desc_sw128(b_lo), !(slot == 0 && ks == 0));
+                            mma_f16_ra32(acc, a[ks], desc_sw128(b_hi), 1);
                         }
-                    const uint32_t b_hi0 = fc_s + (uint32_t)slot * 8192;
-                    fence_acc(acc);
-                    asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
+                        asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
+                        asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
+                        fence_acc(acc);
+                    } else {
+                        uint32_t a_hi[KS][4], a_lo[KS][4];
 #pragma unroll
-                    for (int ks = 0; ks < KS; ++ks) {
-                        const uint32_t b_hi = b_hi0 + (uint32_t)ks * 32, b_lo = b_hi + 4096;
-                        mma_tf32_ra32(acc, a_lo[ks], desc_sw128(b_hi), !(slot == 0 && ks == 0));
-                        mma_tf32_ra32(acc, a_hi[ks], desc_sw128(b_lo), 1);
-                        mma_tf32_ra32(acc, a_hi[ks], desc_sw128(b_hi), 1);
+                        for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) {
+                                // steps 0 and 1 of a call's first chunk can touch the first-conv ring / the pending rows (virtual rows
+                                // -2 .. n_pend - 1, in small); steps beyond the chunk contribute zero rows, never stored.  Both
+                                // loads are made and one is selected: register fragments fed by divergent code would serialise the wgmmas
+                                const int t = ta + 8 * (e & 1), g = g_ta + 960 * (e & 1) + 32 * slot + 8 * ks + 4 * (e >> 1);
+                                const float from_small = small[min(g, 4 * kNumChannels - 1)];
+                                const float from_rows = (float)feat[max(g - g_rows, 0)] * kFeatureScale;
+                                const float v = t < n ? (g < g_pend ? from_small : from_rows) : 0.f;
+                                float hi, lo;
+                                split_tf32f(v, hi, lo);
+                                a_hi[ks][e] = __float_as_uint(hi);
+                                a_lo[ks][e] = __float_as_uint(lo);
+                            }
+                        const uint32_t b_hi0 = fc_s + (uint32_t)slot * 8192;
+                        fence_acc(acc);
+                        asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory");
+#pragma unroll
+                        for (int ks = 0; ks < KS; ++ks) {
+                            const uint32_t b_hi = b_hi0 + (uint32_t)ks * 32, b_lo = b_hi + 4096;
+                            mma_tf32_ra32(acc, a_lo[ks], desc_sw128(b_hi), !(slot == 0 && ks == 0));
+                            mma_tf32_ra32(acc, a_hi[ks], desc_sw128(b_lo), 1);
+                            mma_tf32_ra32(acc, a_hi[ks], desc_sw128(b_hi), 1);
+                        }
+                        asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
+                        asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
+                        fence_acc(acc);
                     }
-                    asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
-                    asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
-                    fence_acc(acc);
                 };
+                if constexpr (F16) {
 #pragma unroll 1
-                for (int slot = 0; slot < 6; ++slot) fc_slot(K4{}, slot);
-                fc_slot(K1{}, 6);                                          // slot 6 only has the K = 8 step 192..199
+                    for (int slot = 0; slot < 3; ++slot) fc_slot(K4{}, slot);
+                    fc_slot(K1{}, 3);                                      // slot 3 only has the K = 16 step 192..207, 200.. zero
+                } else {
+#pragma unroll 1
+                    for (int slot = 0; slot < 6; ++slot) fc_slot(K4{}, slot);
+                    fc_slot(K1{}, 6);                                      // slot 6 only has the K = 8 step 192..199
+                }
             }
             TC_PHASE(kPhMmaFc);
             // first conv epilogue: ReLU, no bias -> X (block 0's input), its ring history in front.  The feature rows under X are dead once
             // both warpgroups are past their first-conv MMAs, and so are its weights: the B buffers take block 0's and block 1's first slot.
             __syncthreads();
-            if (tid == 0) { load_slot(7); load_slot(8); }
+            if (!F16 && tid == 0) { load_slot(7); load_slot(8); }
             ring_to_x<0>(tid, x, ring_stage);
             TC_PHASE(kPhRingIn);
-            epilogue<32, 4>(tid, n, acc, x, nullptr);
+            epilogue<F16, 32, 4>(tid, n, acc, x, nullptr, TW.fc_out);
             __syncthreads();
             stage_ring<1>(tid, ring_stage, my_state);
             TC_PHASE(kPhEpilogue);
@@ -477,7 +546,7 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
             TC_PHASE(kPhRingOut);                                                                                                           \
             ring_to_x<L + 1>(tid, x, ring_stage);                                                                                           \
             TC_PHASE(kPhRingIn);                                                                                                            \
-            epilogue<64, tc_ring(L + 1)>(tid, n, acc, x, W.pw_b[L]);                                                                        \
+            epilogue<false, 64, tc_ring(L + 1)>(tid, n, acc, x, W.pw_b[L], 1.f);                                                             \
             __syncthreads();                                                                                                                \
             stage_ring<L + 2>(tid, ring_stage, my_state);                                                                                   \
             TC_PHASE(kPhEpilogue);
@@ -552,9 +621,11 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
 
 // ---- host side -------------------------------------------------------------------------------------------------------
 
-// 3xTF32 split and slot layout of one [K][N] weight matrix (the container's layout: input-major): slots of 32 K-values,
-// each [N rows][128 B] swizzled, hi plane then lo plane
-void build_tc_weights(const float *w0 /* [200][32] */, const float *const pw[4] /* [cin][64] */, std::vector<unsigned char> *blob, size_t offsets[5]) {
+// 3xTF32 split and slot layout of the [K][N] weight matrices (the container's layout: input-major): slots of 32 K-values,
+// each [N rows][128 B] swizzled, hi plane then lo plane; and, for a model that passed tc_f16_scales, the first conv's fp16 hi / lo
+// weights with 0.0390625 folded in
+void build_tc_weights(const float *w0 /* [200][32] */, const float *const pw[4] /* [cin][64] */, const TcF16Scales *f16,
+                      std::vector<unsigned char> *blob, size_t offsets[6]) {
     blob->clear();
     std::vector<unsigned char> part;
     auto add = [&](size_t *off) {
@@ -568,20 +639,28 @@ void build_tc_weights(const float *w0 /* [200][32] */, const float *const pw[4] 
         tc_layout(pw[i], i == 0 ? 32 : 64, 64, &part);
         add(&offsets[1 + i]);
     }
+    if (!f16) return;
+    tc_layout_f16(w0, 200, 32, 0.0390625, f16->s_fc, &part);
+    add(&offsets[5]);
 }
 
-cudaError_t launch_nn_f32_tc(const NnWeightsF32 &W, const TcWeights &TW, float *state, float *pend, int n_pend, const uint16_t *rows,
+cudaError_t launch_nn_f32_tc(const NnWeightsF32 &W, const TcWeights &TW, bool f16, float *state, float *pend, int n_pend, const uint16_t *rows,
                              long long rows_stream_stride, int n_rows, float *probs, long long probs_stream_stride, int n_streams, int sm_count,
                              cudaStream_t st) {
     if (n_streams <= 0) return cudaSuccess;
     static bool done[64] = {};
     if (first_launch_on_this_device(done)) {
-        cudaError_t e = cudaFuncSetAttribute(nn_f32_clip_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes);
+        cudaError_t e = cudaFuncSetAttribute(nn_f32_clip_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(nn_f32_clip_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes);
         if (e != cudaSuccess) return e;
     }
     const int grid = n_streams < 2 * sm_count ? n_streams : 2 * sm_count;
-    nn_f32_clip_tc_kernel<<<grid, kTcThreads, kTcSmemBytes, st>>>(W, TW, state, pend, n_pend, rows, rows_stream_stride, n_rows, probs,
-                                                                  probs_stream_stride, n_streams);
+    if (f16)
+        nn_f32_clip_tc_kernel<true><<<grid, kTcThreads, kTcSmemBytes, st>>>(W, TW, state, pend, n_pend, rows, rows_stream_stride, n_rows, probs,
+                                                                            probs_stream_stride, n_streams);
+    else
+        nn_f32_clip_tc_kernel<false><<<grid, kTcThreads, kTcSmemBytes, st>>>(W, TW, state, pend, n_pend, rows, rows_stream_stride, n_rows, probs,
+                                                                             probs_stream_stride, n_streams);
     return cudaGetLastError();
 }
 

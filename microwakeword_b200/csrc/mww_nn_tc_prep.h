@@ -3,6 +3,7 @@
 // core does (tests/host_emul).  No CUDA dependency.
 #pragma once
 
+#include <math.h>
 #include <stddef.h>
 #include <stdint.h>
 #include <string.h>
@@ -39,6 +40,86 @@ inline void tc_layout(const float *w, int K, int N, std::vector<unsigned char> *
             memcpy(slot + sw128_off(n, k & 31), &hi, 4);
             memcpy(slot + plane + sw128_off(n, k & 31), &lo, 4);
         }
+}
+
+// ---- fp16 hi / lo operands ------------------------------------------------------------------------------------------------
+// The same 128-byte rows hold 64 fp16 along K: byte offset of element (row, kk), kk in [0, 64).
+MWW_HD uint32_t sw128_off_h(int row, int kk) {
+    return (uint32_t)row * 128u + (uint32_t)((((kk >> 3) ^ (row & 7)) << 4) + ((kk & 7) << 1));
+}
+
+// Largest uint16 feature the frontend emits: log_scale() (mww_frontend_dev.cuh) of any 32-bit input is at most
+// ((loge << 6) + 32768) >> 16 with log2 in [31, 32), i.e. 1 420 (tests/test_tc_f16.py derives it from the table).  Every
+// integer up to 2048 is exact in fp16, so a feature row is an exact fp16 A operand.
+constexpr int kTcMaxFeature = 1420;
+// A call of at least this many model steps leaves first-conv ring and pending rows made of its own rows only: 3 x 2 - 2 >= the
+// at most 2 rows pending before it.
+constexpr int kTcFreshSteps = 2;
+
+// fp16 round-to-nearest-even of |x| < 65520 (subnormals included), as bits
+inline uint16_t f16_bits_rn(double x) {
+    const uint16_t sign = x < 0 ? 0x8000 : 0;
+    const double a = fabs(x);
+    if (a < 0x1p-14) return (uint16_t)(sign | (uint16_t)nearbyint(a * 0x1p24));    // 1024 rounds up to the smallest normal's bits
+    int e;
+    frexp(a, &e);                                                                   // a in [2^(e-1), 2^e)
+    double m = nearbyint(ldexp(a, 11 - e));                                         // 11 significant bits: [1024, 2048]
+    int E = e - 1;
+    if (m == 2048.0) { m = 1024.0; E += 1; }
+    return (uint16_t)(sign | (uint16_t)((E + 15) << 10) | (uint16_t)(m - 1024.0));
+}
+inline double f16_value(uint16_t h) {
+    const int E = (h >> 10) & 31, m = h & 1023;
+    const double v = E == 0 ? ldexp((double)m, -24) : ldexp((double)(1024 + m), E - 25);
+    return (h & 0x8000) ? -v : v;
+}
+
+// Power-of-two exponent s with max_abs * 2^s in [2^14, 2^15): the scaled values and their fp16 hi parts stay below 2^15, half of
+// fp16's range, and lo = x - hi stays normal for every |x| >= max_abs * 2^-17.
+inline int f16_scale_exp(double max_abs) {
+    if (!(max_abs > 0)) return 0;
+    int e;
+    frexp(max_abs, &e);                                                             // max_abs in [2^(e-1), 2^e)
+    return 15 - e;
+}
+
+// [K][N] weights times `mul` (exact in double) times 2^s -> K cut into slots of 64; per slot an fp16 hi plane [N rows][128 B
+// swizzled] followed by the lo plane, hi = fp16(x), lo = fp16(x - hi); positions k >= K of the last slot are zero.
+inline void tc_layout_f16(const float *w, int K, int N, double mul, int s, std::vector<unsigned char> *out) {
+    const int slots = (K + 63) / 64, plane = N * 128;
+    out->assign((size_t)slots * 2 * plane, 0);
+    for (int k = 0; k < K; ++k)
+        for (int n = 0; n < N; ++n) {
+            const double x = ldexp((double)w[(size_t)k * N + n] * mul, s);
+            const uint16_t hi = f16_bits_rn(x), lo = f16_bits_rn(x - f16_value(hi));
+            unsigned char *slot = out->data() + (size_t)(k >> 6) * 2 * plane;
+            memcpy(slot + sw128_off_h(n, k & 63), &hi, 2);
+            memcpy(slot + plane + sw128_off_h(n, k & 63), &lo, 2);
+        }
+}
+
+// The first conv's fp16 scheme for a model: A = u is exact, the weights w0' = w0 x 0.0390625 x 2^s_fc are an fp16 hi / lo pair
+// (f16_scale_exp of the largest |w0'|).  ok = false keeps the 3xTF32 first conv: a weight that is not finite or not below 2^100, or
+// an output channel whose largest |w0'| lies more than 2^17 below the tensor's largest -- there lo drops into fp16's subnormals and
+// that channel keeps fewer than the 22 significant bits of a tf32 hi / lo pair.
+struct TcF16Scales {
+    bool ok;
+    int s_fc;
+};
+inline TcF16Scales tc_f16_scales(const float *w0 /* [200][32] */) {
+    double col[32] = {}, mx = 0;
+    bool finite = true;
+    for (int k = 0; k < 200; ++k)
+        for (int n = 0; n < 32; ++n) {
+            const double a = fabs((double)w0[k * 32 + n] * 0.0390625);
+            finite = finite && a < 0x1p100;                 // false for a NaN too
+            col[n] = a > col[n] ? a : col[n];
+            mx = a > mx ? a : mx;
+        }
+    TcF16Scales r{finite, f16_scale_exp(mx)};
+    for (int n = 0; n < 32; ++n)
+        if (col[n] != 0 && col[n] < ldexp(mx, -17)) r.ok = false;
+    return r;
 }
 
 }  // namespace mww
