@@ -173,6 +173,18 @@ int mww_predict_clip_host(mww_t *h, const int16_t *h_audio, int n_samples, long 
 int mww_predict_clip_remote(mww_t *h, const int16_t *src_audio, int n_samples, long long audio_stride,
                             float *d_probs, int max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
 
+/* mww_predict_clip_host / mww_predict_clip_remote with float32 audio (nominally in [-1, 1]; audio_stride in samples): the
+ * staged pipeline copies the float samples as they are, and the frontend kernels convert them on the GPU as
+ * mww_features_f32 does.  Probabilities and state are bit-identical to the int16 call on the converted samples, and int16
+ * and float32 calls may alternate on one handle.  Ordering, poisoning on a half-way failure and the n_tiles rule are those
+ * of the int16 calls; a source this GPU can address with n_tiles <= 0 is read in place (= mww_predict_clip_f32).  Each
+ * staging tile holds twice the bytes of an int16 one, so the two float staging tiles count against the scratch budget
+ * (MWW_SCRATCH_MB, default 2048): a tile takes at most budget / (2 * 4 * n_samples + the per-stream scratch) streams. */
+int mww_predict_clip_host_f32(mww_t *h, const float *h_audio, int n_samples, long long audio_stride,
+                              float *h_probs, int max_probs, int *h_probs_out);
+int mww_predict_clip_remote_f32(mww_t *h, const float *src_audio, int n_samples, long long audio_stride,
+                                float *d_probs, int max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
+
 /* ---- several models over one frontend ---------------------------------------------------------------------------
  * A deployment that listens for several wake words (and a VAD model) on the same audio runs one frontend and K models on
  * its rows.  mww_create_multi makes a handle that carries K >= 1 models of any kind the containers describe (fp32
@@ -196,8 +208,8 @@ int mww_predict_clip_remote(mww_t *h, const int16_t *src_audio, int n_samples, l
  *   - mww_reset (all or by id), mww_reset_device_ids reset the frontend and every model; mww_reset_frontend,
  *     mww_set_window_step and mww_features act on the shared frontend; mww_launch_count and mww_profile_* count every
  *     model's launches.
- *   - on a handle with K > 1, mww_predict_clip[_f32/_host/_remote], mww_infer_features and mww_copy_nn_state return
- *     MWW_EINVAL, as do mww_get_state / mww_set_state given NN arrays or a nonzero pending_rows (called with those NULL /
+ *   - on a handle with K > 1, mww_predict_clip[_f32/_host/_remote/_host_f32/_remote_f32], mww_infer_features and
+ *     mww_copy_nn_state return MWW_EINVAL, as do mww_get_state / mww_set_state given NN arrays or a nonzero pending_rows (called with those NULL /
  *     0 they read / write the frontend state only): each would advance or replace state for one model only. */
 int mww_create_multi(const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams, mww_t **out);
 int mww_model_count(const mww_t *h);
@@ -210,6 +222,10 @@ int mww_predict_clip_host_multi(mww_t *h, const int16_t *h_audio, int n_samples,
                                 float *const *h_probs, const int *max_probs, int *h_probs_out);
 int mww_predict_clip_remote_multi(mww_t *h, const int16_t *src_audio, int n_samples, long long audio_stride,
                                   float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
+int mww_predict_clip_host_multi_f32(mww_t *h, const float *h_audio, int n_samples, long long audio_stride,
+                                    float *const *h_probs, const int *max_probs, int *h_probs_out);
+int mww_predict_clip_remote_multi_f32(mww_t *h, const float *src_audio, int n_samples, long long audio_stride,
+                                      float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
 int mww_get_model_state(mww_t *h, int k, void *h_nn, void *h_pending);
 int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending, int pending_rows);
 

@@ -26,6 +26,7 @@ EXPORTS = (
     "mww_set_window_step", "mww_features_f32", "mww_predict_clip_f32", "mww_copy_nn_state", "mww_accuracy_counts",
     "mww_create_multi", "mww_model_count", "mww_get_model_info", "mww_predict_clip_multi", "mww_predict_clip_multi_f32",
     "mww_predict_clip_host_multi", "mww_predict_clip_remote_multi", "mww_get_model_state", "mww_set_model_state",
+    "mww_predict_clip_host_f32", "mww_predict_clip_host_multi_f32", "mww_predict_clip_remote_f32", "mww_predict_clip_remote_multi_f32",
 )
 
 
@@ -84,8 +85,9 @@ def lib() -> ctypes.CDLL:
     L.mww_features_f32.argtypes = [vp, vp, i32, ll, vp, i32, pi, vp]
     L.mww_predict_clip_f32.restype = i32
     L.mww_predict_clip_f32.argtypes = [vp, vp, i32, ll, vp, i32, pi, vp]
-    L.mww_predict_clip_host.restype = i32
-    L.mww_predict_clip_host.argtypes = [vp, vp, i32, ll, vp, i32, pi]
+    for name in ("mww_predict_clip_host", "mww_predict_clip_host_f32"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, ll, vp, i32, pi]
     L.mww_get_state.restype = i32
     L.mww_get_state.argtypes = [vp, vp, vp, vp, vp]
     L.mww_set_state.restype = i32
@@ -118,8 +120,9 @@ def lib() -> ctypes.CDLL:
     L.mww_ipc_close.argtypes = [vp, i32]
     L.mww_ipc_free.restype = i32
     L.mww_ipc_free.argtypes = [vp, i32]
-    L.mww_predict_clip_remote.restype = i32
-    L.mww_predict_clip_remote.argtypes = [vp, vp, i32, ll, vp, i32, pi, i32, vp]
+    for name in ("mww_predict_clip_remote", "mww_predict_clip_remote_f32"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, ll, vp, i32, pi, i32, vp]
     L.mww_reset_device_ids.restype = i32
     L.mww_reset_device_ids.argtypes = [vp, vp, i32, vp]
     L.mww_host_alloc.restype = i32
@@ -141,10 +144,12 @@ def lib() -> ctypes.CDLL:
     for name in ("mww_predict_clip_multi", "mww_predict_clip_multi_f32"):
         getattr(L, name).restype = i32
         getattr(L, name).argtypes = [vp, vp, i32, ll, vp, vp, vp, vp]
-    L.mww_predict_clip_host_multi.restype = i32
-    L.mww_predict_clip_host_multi.argtypes = [vp, vp, i32, ll, vp, vp, vp]
-    L.mww_predict_clip_remote_multi.restype = i32
-    L.mww_predict_clip_remote_multi.argtypes = [vp, vp, i32, ll, vp, vp, vp, i32, vp]
+    for name in ("mww_predict_clip_host_multi", "mww_predict_clip_host_multi_f32"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, ll, vp, vp, vp]
+    for name in ("mww_predict_clip_remote_multi", "mww_predict_clip_remote_multi_f32"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, ll, vp, vp, vp, i32, vp]
     L.mww_get_model_state.restype = i32
     L.mww_get_model_state.argtypes = [vp, i32, vp, vp]
     L.mww_set_model_state.restype = i32

@@ -111,7 +111,7 @@ struct mww_handle {
     bool staged_used = false;      // ev_compute[] have been recorded by an earlier staged call
     bool poisoned = false;
     int32_t *d_ids = nullptr; size_t ids_cap = 0;      // device copy of a host id list (mww_reset)         // a staged call failed half-way: per-stream state is inconsistent until mww_reset(all)
-    int16_t *d_audio_tile[2] = {nullptr, nullptr}; size_t audio_tile_bytes = 0;
+    void *d_audio_tile[2] = {nullptr, nullptr}; size_t audio_tile_bytes = 0;     // int16 or float32 samples of one tile
     float *d_probs_tile[2] = {nullptr, nullptr}; size_t probs_tile_bytes = 0;
     // live-step path: rings stay rotated between live calls (mww_nn_live.cuh); all streams advance in lockstep
     LiveHeads live_heads{};
@@ -196,9 +196,11 @@ size_t v_scratch_bytes(const mww_t *h, int tile, int n_frames) {
     return clip_fuses(h, n_frames) ? 0 : (size_t)tile * std::max(n_frames, 1) * kNumChannels * 4;
 }
 
-// streams per tile so that the K1->K2 scratch (when the call needs one) and the optional feature scratch fit the budget
-int tile_streams(const mww_t *h, int n_frames, bool need_feat) {
-    const size_t per_stream = (size_t)std::max(n_frames, 1) * kNumChannels * ((clip_fuses(h, n_frames) ? 0 : 4) + (need_feat ? 2 : 0));
+// streams per tile so that the K1->K2 scratch (when the call needs one), the optional feature scratch and `extra_per_stream`
+// further bytes of each stream fit the budget
+int tile_streams(const mww_t *h, int n_frames, bool need_feat, size_t extra_per_stream = 0) {
+    const size_t per_stream = (size_t)std::max(n_frames, 1) * kNumChannels * ((clip_fuses(h, n_frames) ? 0 : 4) + (need_feat ? 2 : 0)) +
+                              extra_per_stream;
     if (per_stream == 0) return h->n_streams;
     size_t t = h->scratch_budget / per_stream;
     if (t < 1) t = 1;
@@ -1225,7 +1227,9 @@ int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, l
 // host memory or device memory of a PEER GPU mapped into this process, destination = this GPU).  The streams are cut into
 // tiles; a copy stream brings tile t+1 into one of two staging buffers (cudaMemcpyAsync, cudaMemcpyDefault: the copy
 // engine of THIS GPU pulls over PCIe or NVLink, no SM is involved on either side) while the kernels of tile t run on the
-// compute stream, and for a host destination a third stream drains the scores.
+// compute stream, and for a host destination a third stream drains the scores.  The bodies are templates over the sample
+// type (int16_t or float), hence C++ linkage.
+extern "C++" {
 namespace {
 
 int ensure_pipeline(mww_t *h) {
@@ -1252,9 +1256,13 @@ size_t probs_tile_offset(const mww_t *h, const NnOuts &o, int tile, size_t k) {
     return off;
 }
 
-int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_stride, const NnOuts &o, bool dst_is_host,
+// T = int16_t or float: the staging buffers hold the caller's samples as they are, and the frontend and carry kernels of
+// that sample type convert them (as on the device path)
+template <typename T>
+int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, const NnOuts &o, bool dst_is_host,
                  int tile, int n_frames) {
     const size_t K = h->models.size();
+    const T *audio_tile[2] = {static_cast<const T *>(h->d_audio_tile[0]), static_cast<const T *>(h->d_audio_tile[1])};
     float *tile_probs[kMaxModels];
     long long tile_probs_stride[kMaxModels];
     for (size_t k = 0; k < K; ++k) tile_probs_stride[k] = dst_is_host ? std::max(o.steps[k], 1) : o.max_probs[k];
@@ -1270,11 +1278,12 @@ int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_st
             CU(h, cudaEventRecord(tl[0], h->st_h2d));
         }
         if (n_samples > 0) {
-            const int16_t *from = src + (size_t)first * audio_stride;
+            const T *from = src + (size_t)first * audio_stride;
+            const size_t row = (size_t)n_samples * sizeof(T);
             if (audio_stride == n_samples)       // contiguous block: one linear DMA
-                CU(h, cudaMemcpyAsync(h->d_audio_tile[b], from, (size_t)n * n_samples * 2, cudaMemcpyDefault, h->st_h2d));
+                CU(h, cudaMemcpyAsync(h->d_audio_tile[b], from, (size_t)n * row, cudaMemcpyDefault, h->st_h2d));
             else
-                CU(h, cudaMemcpy2DAsync(h->d_audio_tile[b], (size_t)n_samples * 2, from, (size_t)audio_stride * 2, (size_t)n_samples * 2, n,
+                CU(h, cudaMemcpy2DAsync(h->d_audio_tile[b], row, from, (size_t)audio_stride * sizeof(T), row, n,
                                         cudaMemcpyDefault, h->st_h2d));
         }
         if (tl[1]) CU(h, cudaEventRecord(tl[1], h->st_h2d));
@@ -1282,14 +1291,14 @@ int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_st
         CU(h, cudaStreamWaitEvent(h->st_compute, h->ev_h2d[b], 0));
         if (tl[2]) CU(h, cudaEventRecord(tl[2], h->st_compute));
         if (dst_is_host && it >= 2) CU(h, cudaStreamWaitEvent(h->st_compute, h->ev_d2h[b], 0));   // score staging buffer drained
-        int rc = run_frontend_tile(h, first, n, h->d_audio_tile[b], n_samples, n_samples, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
+        int rc = run_frontend_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
         if (rc) return rc;
         for (size_t k = 0; k < K; ++k)
             tile_probs[k] = dst_is_host ? h->d_probs_tile[b] + probs_tile_offset(h, o, tile, k) : o.probs[k] + (size_t)first * o.max_probs[k];
         rc = run_models_tile(h, first, n, n_frames, tile_probs, tile_probs_stride, h->st_compute);
         if (rc) return rc;
         if (n_samples > 0) {
-            rc = run_carry_tile(h, first, n, h->d_audio_tile[b], n_samples, n_samples, n_frames, h->st_compute);
+            rc = run_carry_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->st_compute);
             if (rc) return rc;
         }
         if (tl[3]) CU(h, cudaEventRecord(tl[3], h->st_compute));
@@ -1308,7 +1317,8 @@ int staged_tiles(mww_t *h, const int16_t *src, int n_samples, long long audio_st
 
 // `caller` != nullptr-or-legacy semantics: the call is ordered after everything queued on `caller` so far, and `caller`
 // is made to wait for the call's last kernel (asynchronous variant).  host_sync: return only when dst is complete.
-int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_samples, long long audio_stride, float *const *dst,
+template <typename T>
+int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, long long audio_stride, float *const *dst,
                         const int *max_probs, int *h_probs_out, bool dst_is_host, int want_tiles, cudaStream_t caller, bool host_sync) {
     const int n_frames = frames_for(h, n_samples);
     NnOuts o;
@@ -1320,11 +1330,14 @@ int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_sam
     // first tile's copy and the last tile's kernels are the only parts that cannot hide behind each other), but never
     // fewer than 2 048 streams per tile so that every launch still fills the GPU
     if (want_tiles <= 0) want_tiles = 16;
-    int tile = tile_streams(h, n_frames, true);
+    // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
+    // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone
+    const size_t staged_bytes = sizeof(T) == sizeof(int16_t) ? 0 : 2 * (size_t)std::max(n_samples, 1) * sizeof(T);
+    int tile = tile_streams(h, n_frames, true, staged_bytes);
     tile = std::max(1, std::min(tile, std::max((h->n_streams + want_tiles - 1) / want_tiles, std::min(h->n_streams, h->min_tile_streams))));
     rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
     if (rc) return rc;
-    const size_t a_bytes = (size_t)tile * std::max(n_samples, 1) * sizeof(int16_t);
+    const size_t a_bytes = (size_t)tile * std::max(n_samples, 1) * sizeof(T);
     const size_t p_bytes = dst_is_host ? probs_tile_offset(h, o, tile, h->models.size()) * sizeof(float) : 0;
     if (a_bytes > h->audio_tile_bytes || p_bytes > h->probs_tile_bytes) {
         CU(h, cudaDeviceSynchronize());
@@ -1374,7 +1387,8 @@ int predict_clip_staged(mww_t *h, const char *who, const int16_t *src, int n_sam
     return MWW_OK;
 }
 
-int predict_clip_host_impl(mww_t *h, const char *who, const int16_t *h_audio, int n_samples, long long audio_stride, float *const *h_probs,
+template <typename T>
+int predict_clip_host_impl(mww_t *h, const char *who, const T *h_audio, int n_samples, long long audio_stride, float *const *h_probs,
                            const int *max_probs, int *h_probs_out) {
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !h_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
@@ -1386,7 +1400,8 @@ int predict_clip_host_impl(mww_t *h, const char *who, const int16_t *h_audio, in
     return predict_clip_staged(h, who, h_audio, n_samples, audio_stride, h_probs, max_probs, h_probs_out, true, 0, nullptr, true);
 }
 
-int predict_clip_remote_impl(mww_t *h, const char *who, const int16_t *src_audio, int n_samples, long long audio_stride, float *const *d_probs,
+template <typename T>
+int predict_clip_remote_impl(mww_t *h, const char *who, const T *src_audio, int n_samples, long long audio_stride, float *const *d_probs,
                              const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !src_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
@@ -1408,6 +1423,7 @@ int predict_clip_remote_impl(mww_t *h, const char *who, const int16_t *src_audio
 }
 
 }  // namespace
+}  // extern "C++"
 
 int mww_predict_clip_host(mww_t *h, const int16_t *h_audio, int n_samples, long long audio_stride, float *h_probs, int max_probs,
                           int *h_probs_out) {
@@ -1429,6 +1445,28 @@ int mww_predict_clip_remote_multi(mww_t *h, const int16_t *src_audio, int n_samp
                                   const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
     return predict_clip_remote_impl(h, "mww_predict_clip_remote_multi", src_audio, n_samples, audio_stride, d_probs, max_probs, h_probs_out,
                                     n_tiles, cu_stream);
+}
+
+int mww_predict_clip_host_f32(mww_t *h, const float *h_audio, int n_samples, long long audio_stride, float *h_probs, int max_probs,
+                              int *h_probs_out) {
+    if (int rc = refuse_multi(h, "mww_predict_clip_host_f32", "mww_predict_clip_host_multi_f32")) return rc;
+    return predict_clip_host_impl(h, "mww_predict_clip_host_f32", h_audio, n_samples, audio_stride, &h_probs, &max_probs, h_probs_out);
+}
+int mww_predict_clip_host_multi_f32(mww_t *h, const float *h_audio, int n_samples, long long audio_stride, float *const *h_probs,
+                                    const int *max_probs, int *h_probs_out) {
+    return predict_clip_host_impl(h, "mww_predict_clip_host_multi_f32", h_audio, n_samples, audio_stride, h_probs, max_probs, h_probs_out);
+}
+
+int mww_predict_clip_remote_f32(mww_t *h, const float *src_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                                int *h_probs_out, int n_tiles, void *cu_stream) {
+    if (int rc = refuse_multi(h, "mww_predict_clip_remote_f32", "mww_predict_clip_remote_multi_f32")) return rc;
+    return predict_clip_remote_impl(h, "mww_predict_clip_remote_f32", src_audio, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out,
+                                    n_tiles, cu_stream);
+}
+int mww_predict_clip_remote_multi_f32(mww_t *h, const float *src_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                                      const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
+    return predict_clip_remote_impl(h, "mww_predict_clip_remote_multi_f32", src_audio, n_samples, audio_stride, d_probs, max_probs,
+                                    h_probs_out, n_tiles, cu_stream);
 }
 
 // ---- host memory next to the GPU ---------------------------------------------------------------------------------

@@ -141,13 +141,31 @@ class _Engine:
             raise ValueError("audio samples must be contiguous along the last dimension")
         return audio.shape[1], (audio.stride(0) if audio.shape[1] > 0 else 0), audio.dtype == torch.float32
 
-    def _check_host_audio(self, audio: np.ndarray) -> np.ndarray:
-        """int16 host audio [S, N] with contiguous samples (copied when they are not)"""
-        if audio.dtype != np.int16 or audio.ndim != 2 or audio.shape[0] != self.n_streams:
-            raise ValueError("audio must be an int16 array of shape [n_streams=%d, n_samples]" % self.n_streams)
-        if audio.strides[1] != 2 and audio.shape[1] > 1:
+    def _check_host_audio(self, audio: np.ndarray):
+        """int16 or float32 host audio [S, N] -> (the array with contiguous samples, its row pitch in samples, is_float32).
+        An array whose samples are not contiguous, or whose row stride is not a whole number of samples >= N (a view made
+        with as_strided or an explicit strides= argument, a broadcast, reversed rows), is copied first.  float32 goes through
+        the staged pipeline as it is and is converted on the GPU as _check_audio describes; float64, other dtypes and wrong
+        shapes raise ValueError here, before the library is called, as they do on the device path."""
+        if (not isinstance(audio, np.ndarray) or audio.dtype not in (np.int16, np.float32) or audio.ndim != 2
+                or audio.shape[0] != self.n_streams):
+            raise ValueError("audio must be an int16 or float32 array of shape [n_streams=%d, n_samples]" % self.n_streams)
+        n, size = audio.shape[1], audio.itemsize
+        if n > 0 and ((audio.strides[1] != size and n > 1) or audio.strides[0] % size or audio.strides[0] < n * size):
             audio = np.ascontiguousarray(audio)
-        return audio
+        return audio, (audio.strides[0] // audio.itemsize if n else 0), audio.dtype == np.float32
+
+    def _remote_fn(self, dtype, name: str):
+        """the int16 or float32 form of the raw-pointer entry point `name`, from a numpy (or torch) sample dtype"""
+        if str(dtype) in ("torch.int16", "torch.float32"):
+            dtype = str(dtype)[len("torch."):]
+        try:
+            dt = np.dtype(dtype)
+        except TypeError:
+            dt = None
+        if dt not in (np.dtype(np.int16), np.dtype(np.float32)):
+            raise ValueError("dtype must be int16 or float32, not %r" % (dtype,))
+        return getattr(self._L, name + "_f32" if dt == np.float32 else name)
 
     def _check_probs_out(self, out) -> None:
         torch = _torch()
@@ -301,24 +319,27 @@ class StreamEngine(_Engine):
     step = predict_clip  # the live "one chunk of new audio per call" surface (north_star step())
 
     def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None) -> np.ndarray:
-        """int16 HOST array [S, N] -> float32 HOST array [S, steps]; copies are pipelined inside the library."""
-        audio = self._check_host_audio(audio)
+        """int16 or float32 HOST array [S, N] -> float32 HOST array [S, steps]; copies are pipelined inside the library.
+        float32 samples cross PCIe as they are and are converted in the frontend kernels (as predict_clip converts them).
+        Other dtypes (float64 included) and wrong shapes: ValueError; a too-small `out`: MwwError."""
+        audio, stride, is_f32 = self._check_host_audio(audio)
         n = audio.shape[1]
         steps = self._steps(n)
         if out is None:
             out = np.empty((self.n_streams, max(steps, 1)), np.float32)
         got = ctypes.c_int(0)
-        _lib.check(self._h, self._L.mww_predict_clip_host(self._h, audio.ctypes.data, n, audio.strides[0] // 2 if n else 0, out.ctypes.data,
-                                                          out.shape[1], ctypes.byref(got)))
+        fn = self._L.mww_predict_clip_host_f32 if is_f32 else self._L.mww_predict_clip_host
+        _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, out.ctypes.data, out.shape[1], ctypes.byref(got)))
         return out[:, :got.value]
 
-    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None):
-        """Audio int16 [S, n_samples] at address `src_ptr` -- device memory of a PEER GPU mapped into this process
-        (sharding.IngestBuffer.block_ptr) or host memory (mww_predict_clip_remote).  tiles = 0: a peer-mapped (or local) buffer
-        is read in place by the frontend kernel, over NVLink; host memory is staged in 16 tiles.  tiles > 0: always staged --
-        this GPU's copy engine pulls tile t+1 while tile t computes.  Returns float32 CUDA probabilities [S, steps];
-        stream-ordered like predict_clip."""
+    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None, dtype=np.int16):
+        """Audio [S, n_samples] of `dtype` (int16 or float32; stride in samples) at address `src_ptr` -- device memory of a PEER
+        GPU mapped into this process (sharding.IngestBuffer.block_ptr) or host memory (mww_predict_clip_remote[_f32]).
+        tiles = 0: a peer-mapped (or local) buffer is read in place by the frontend kernel, over NVLink; host memory is staged
+        in 16 tiles.  tiles > 0: always staged -- this GPU's copy engine pulls tile t+1 while tile t computes.  Returns float32
+        CUDA probabilities [S, steps]; stream-ordered like predict_clip."""
         torch = _torch()
+        fn = self._remote_fn(dtype, "mww_predict_clip_remote")
         n = int(n_samples)
         steps = self._steps(n)
         if out is None:
@@ -326,8 +347,8 @@ class StreamEngine(_Engine):
         else:
             self._check_probs_out(out)
         got = ctypes.c_int(0)
-        _lib.check(self._h, self._L.mww_predict_clip_remote(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n, out.data_ptr(),
-                                                           out.shape[1], ctypes.byref(got), int(tiles), self._cu_stream()))
+        _lib.check(self._h, fn(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n, out.data_ptr(),
+                               out.shape[1], ctypes.byref(got), int(tiles), self._cu_stream()))
         return out[:, :got.value]
 
     # ------------------------------------------------------------------ state (checkpoint / tests)
@@ -432,20 +453,23 @@ class MultiModelEngine(_Engine):
     step = predict_clip
 
     def predict_clip_host(self, audio: np.ndarray, out=None) -> list:
-        """int16 HOST array [S, N] -> [float32 HOST array [S, steps_k] for each model k]; each audio tile is copied once."""
-        audio = self._check_host_audio(audio)
+        """int16 or float32 HOST array [S, N] -> [float32 HOST array [S, steps_k] for each model k]; each audio tile is copied
+        once."""
+        audio, stride, is_f32 = self._check_host_audio(audio)
         n = audio.shape[1]
         out, ptrs, maxp, got = self._outs(self._steps(n), out, True)
-        _lib.check(self._h, self._L.mww_predict_clip_host_multi(self._h, audio.ctypes.data, n, audio.strides[0] // 2 if n else 0, ptrs,
-                                                                maxp, got))
+        fn = self._L.mww_predict_clip_host_multi_f32 if is_f32 else self._L.mww_predict_clip_host_multi
+        _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, ptrs, maxp, got))
         return [o[:, :g] for o, g in zip(out, got)]
 
-    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None) -> list:
+    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None,
+                            dtype=np.int16) -> list:
         """StreamEngine.predict_clip_remote for every model: one result per model, each audio tile pulled once."""
+        fn = self._remote_fn(dtype, "mww_predict_clip_remote_multi")
         n = int(n_samples)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
-        _lib.check(self._h, self._L.mww_predict_clip_remote_multi(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n,
-                                                                  ptrs, maxp, got, int(tiles), self._cu_stream()))
+        _lib.check(self._h, fn(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n, ptrs, maxp, got, int(tiles),
+                               self._cu_stream()))
         return [o[:, :g] for o, g in zip(out, got)]
 
     # ------------------------------------------------------------------ state (checkpoint / tests)

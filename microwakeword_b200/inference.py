@@ -142,11 +142,13 @@ class Model:
 
     # ------------------------------------------------------------------ many-stream extension (north_star step surface)
     def step(self, audio):
-        """Feed new audio for every stream: int16 [batch, n] (numpy or CUDA tensor; a CUDA tensor may also be float32 in [-1, 1],
-        converted on the GPU as to_int16 converts it) -> probabilities [batch, steps].
+        """Feed new audio for every stream: int16 or float32 in [-1, 1] [batch, n] (numpy or CUDA tensor; float32 is converted
+        on the GPU as to_int16 converts it, float64 numpy on the host by to_int16) -> probabilities [batch, steps].
         n is typically 480 (one 30 ms model step); state carries over between calls."""
         torch = _torch()
         if isinstance(audio, np.ndarray):
+            if audio.dtype == np.float32:
+                return self.engine.predict_clip_host(audio)
             return self.engine.predict_clip_host(np.ascontiguousarray(to_int16(audio)))
         return self.engine.predict_clip(audio)
 
