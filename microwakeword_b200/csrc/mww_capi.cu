@@ -1,6 +1,6 @@
 // mww_capi.cu -- the extern "C" boundary declared in include/mww.h.
 //
-// Host-side orchestration only: model-container parsing, weight/table upload, per-stream state,
+// Host-side orchestration only: weight/table upload (container parsing: mww_container.cc), per-stream state,
 // stream tiling against a scratch budget, and the pipelined host-buffer path.  All arithmetic is
 // in the kernels (mww_frontend.cu, mww_nn.cu, mww_nn_int8.cu); there is no CPU fallback.
 #include <cuda_runtime.h>
@@ -16,8 +16,8 @@
 #include <vector>
 
 #include "../../include/mww.h"
+#include "mww_container.h"
 #include "mww_kernels.h"
-#include "mww_nn_i8_prep.h"
 #include "mww_nn_tc.h"
 
 using namespace mww;
@@ -26,79 +26,43 @@ namespace {
 
 thread_local std::string g_create_error;
 
-struct DirEntry { char name[48]; uint32_t dtype, ndim, shape[4]; uint64_t offset, nbytes; };
-static_assert(sizeof(DirEntry) == 88, "container directory entry layout");
-
-struct Tensor { const uint8_t *data = nullptr; uint32_t dtype = 0, ndim = 0, shape[4] = {0, 0, 0, 0}; uint64_t nbytes = 0; };
-
-bool find_tensor(const uint8_t *blob, size_t n, const char *name, Tensor *out) {
-    if (n < 24 || memcmp(blob, "MWWB200", 8) != 0) return false;
-    uint32_t hdr[4];
-    memcpy(hdr, blob + 8, 16);
-    if (hdr[0] != 1) return false;
-    const uint32_t count = hdr[1], dir_off = hdr[2];
-    for (uint32_t i = 0; i < count; ++i) {
-        if ((size_t)dir_off + (size_t)(i + 1) * sizeof(DirEntry) > n) return false;
-        DirEntry e;
-        memcpy(&e, blob + dir_off + (size_t)i * sizeof e, sizeof e);
-        if (strncmp(e.name, name, 48) == 0) {
-            if (e.offset > n || e.nbytes > n - e.offset) return false;
-            out->data = blob + e.offset; out->dtype = e.dtype; out->ndim = e.ndim; out->nbytes = e.nbytes;
-            memcpy(out->shape, e.shape, sizeof e.shape);
-            return true;
-        }
-    }
-    return false;
-}
-
 constexpr int kMaxModels = 64;      // models one handle can carry (mww_create_multi)
 
-const int32_t kOkayNabuArch[30] ={32, 5, 3, 40, 4, 17, 64, 1, 5, 0, 0, 0, 64, 2, 7, 11, 0, 0, 64, 2, 9, 15, 0, 0, 64, 1, 23, 0, 0, 0};
+// one NN model the frontend feeds: its weights (mww_container.h), per-stream ring state and pending rows
+struct Model : ModelWeights {
+    uint64_t model_hash = 0;        // FNV-1a of the model container: mww_copy_nn_state only moves state between equal models
+    void *d_weights = nullptr;      // the arena of ModelWeights
+    void *d_nn_state = nullptr;     // float or int8 [S][G.state_elems]   (4176 for okay_nabu)
+    void *d_pend = nullptr;         // float or int8 [S][G.pend_cap][40]  (2 rows for stride 3)
+    int n_pend = 0;
+    // live-step path: rings stay rotated between live calls (mww_nn_live.cuh); all streams advance in lockstep
+    LiveHeads live_heads{};
+    // every carried first-conv ring / pending row is a feature (<= 2048) x 0.0390625: true after a full reset and after a predict
+    // call of >= kTcFreshSteps steps; false after infer_features (rows of any value); checked on a state set from outside
+    // (note_state_set).  The fp16 first conv needs it.
+    bool tc_rows_bounded = true;
+
+    size_t elem_size() const { return quantized() ? 1 : 4; }
+    // stream `first`'s ring state and pending rows
+    template <typename T> T *state(int first) const { return static_cast<T *>(d_nn_state) + (size_t)first * G.state_elems; }
+    template <typename T> T *pend(int first) const { return static_cast<T *>(d_pend) + (size_t)first * G.pend_cap * kNumChannels; }
+};
 
 }  // namespace
 
 struct mww_handle {
     int device = 0, n_streams = 0, sm_count = 132;
-    bool quantized = false;
-    bool has_nn = true;
-    uint64_t model_hash = 0;        // FNV-1a of the model container: mww_copy_nn_state only moves state between equal models
     std::string err;
     // constant tables
     uint8_t *d_tables = nullptr;
     FrontendParams P;
-    // weights
-    uint8_t *d_weights = nullptr;
-    NnWeightsF32 W;
-    TcWeights TW{};                 // fp32 okay_nabu: pre-split weights for the wgmma clip kernel (mww_nn_tc.cu)
     bool no_tc = false;             // MWW_NO_TC: keep the mma.sync clip kernel (A/B measurements)
-    bool tc_tf32 = false;           // MWW_TC_TF32: keep the wgmma kernel's 3xTF32 operands (A/B measurements)
-    bool tc_f16 = false;            // the first conv's weights admit fp16 hi / lo operands (tc_f16_scales) and MWW_TC_TF32 is unset
-    // every carried first-conv ring / pending row is a feature (<= 2048) x 0.0390625: true after a full reset and after a predict
-    // call of >= kTcFreshSteps steps; false after infer_features (rows of any value); checked on a state set from outside
-    // (note_state_set).  The fp16 first conv needs it.
-    bool tc_rows_bounded = true;
     int live_variant = 3;           // MWW_LIVE_VARIANT: 3 = bulk-copy stages (default), 2 = warp-specialised with register loads, 1 = r01 kernel
-    NnWeightsI8 Wq;
-    float in_scale = 0.f, out_scale = 0.f;
-    int in_zp = 0, out_zp = 0;
-    // per-stream state
+    // per-stream frontend state
     int16_t *d_carry = nullptr;
     uint32_t *d_estimate = nullptr;
-    void *d_nn_state = nullptr;     // float or int8 [S][state_elems]   (4176 for okay_nabu)
-    void *d_pend = nullptr;         // float or int8 [S][pend_cap][40]  (2 rows for stride 3)
-    int used = 0, n_pend = 0;
+    int used = 0;
     int hop = kHop;                 // samples between feature windows (mww_set_window_step; 160 = the 10 ms of every shipped model)
-    // geometry: the compiled-in okay_nabu kernels, or the run-time-geometry path (mww_nn_generic.cuh) for any other arch
-    bool generic = false;
-    GenArch G{};
-    GenWeightsF32 GW{};
-    GenWeightsI8 GQ{};
-    bool hybrid = false;            // fp32 graph with int8-weight ops (container tensor hy/mode): generic hybrid kernel only
-    GenHybrid GH{};
-    int stride = 3;                 // feature rows per model step
-    int pend_cap = 2;               // rows of the pending buffer
-    int state_elems = kStateFloats; // ring-state elements per stream
-    long long macs_per_step = 24800;
     // scratch
     uint32_t *d_v = nullptr; size_t v_bytes = 0;
     uint16_t *d_feat = nullptr; size_t feat_bytes = 0;
@@ -109,18 +73,14 @@ struct mww_handle {
     cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_compute[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
     cudaEvent_t ev_entry = nullptr, ev_exit = nullptr;
     bool staged_used = false;      // ev_compute[] have been recorded by an earlier staged call
-    bool poisoned = false;
-    int32_t *d_ids = nullptr; size_t ids_cap = 0;      // device copy of a host id list (mww_reset)         // a staged call failed half-way: per-stream state is inconsistent until mww_reset(all)
+    bool poisoned = false;         // a staged call failed half-way: per-stream state is inconsistent until mww_reset(all)
+    int32_t *d_ids = nullptr; size_t ids_cap = 0;      // device copy of a host id list (mww_reset)
     void *d_audio_tile[2] = {nullptr, nullptr}; size_t audio_tile_bytes = 0;     // int16 or float32 samples of one tile
     float *d_probs_tile[2] = {nullptr, nullptr}; size_t probs_tile_bytes = 0;
-    // live-step path: rings stay rotated between live calls (mww_nn_live.cuh); all streams advance in lockstep
-    LiveHeads live_heads{};
     bool no_live = false, no_fuse = false;
     long long launches = 0;
-    // the NN models the frontend feeds: {this} for a one-model handle, {} for a frontend-only one.  mww_create_multi adds
-    // models 1..K-1 as sub-handles that hold weights, ring state, pending rows and live heads only (no frontend state,
-    // scratch or pipeline); the handle owns them
-    std::vector<mww_t *> models;
+    // the NN models the frontend feeds: one for mww_create with a model, none for a frontend-only handle, K for mww_create_multi
+    std::vector<Model> models;
     // optional per-kernel timing (mww_profile_*)
     bool profiling = false;
     std::vector<cudaEvent_t> prof_ev[4];   // start/stop pairs per kernel class
@@ -137,8 +97,6 @@ int cuda_fail(mww_t *h, cudaError_t e, const char *what) {
     return fail(h, MWW_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
 #define CU(h, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(h, e_, #call); } while (0)
-
-size_t elem_size(const mww_t *h) { return h->quantized ? 1 : 4; }
 
 // every entry point runs with the handle's device current and puts the caller's device back on return (a process that
 // holds engines on several GPUs, or torch's current device, is not disturbed)
@@ -264,96 +222,72 @@ int run_carry_tile(mww_t *h, int first, int n, const T *d_audio, long long audio
 }
 
 // one model step per stream -> the stream-parallel live-step kernels (fp32: mww_nn_live.cuh, int8: mww_nn_i8_live.cuh)
-bool use_live(const mww_t *h, int n_rows) { return h->has_nn && !h->generic && n_rows == 3 && !h->no_live; }
+bool use_live(const mww_t *h, const Model &m, int n_rows) { return m.compiled() && n_rows == 3 && !h->no_live; }
 
 // rotate every ring back to the canonical layout before anything that assumes it (clip kernels, mww_get_state)
-int canonicalise_rings(mww_t *h, cudaStream_t st) {
+int canonicalise_rings(mww_t *h, Model &m, cudaStream_t st) {
     bool any = false;
-    for (int i = 0; i < 5; ++i) any = any || h->live_heads.h[i] != 0;
-    if (!any || !h->has_nn) return MWW_OK;
-    if (h->quantized) CU(h, launch_nn_i8_live_canonicalise(static_cast<int8_t *>(h->d_nn_state), h->n_streams, h->live_heads, st));
-    else CU(h, launch_nn_live_canonicalise(static_cast<float *>(h->d_nn_state), h->n_streams, h->live_heads, st));
+    for (int i = 0; i < 5; ++i) any = any || m.live_heads.h[i] != 0;
+    if (!any) return MWW_OK;
+    if (m.quantized()) CU(h, launch_nn_i8_live_canonicalise(m.state<int8_t>(0), h->n_streams, m.live_heads, st));
+    else CU(h, launch_nn_live_canonicalise(m.state<float>(0), h->n_streams, m.live_heads, st));
     h->launches += 1;
-    h->live_heads = LiveHeads{};
+    m.live_heads = LiveHeads{};
     return MWW_OK;
 }
 // once per API call, around the tile loop
-int begin_nn_call(mww_t *h, int n_rows, cudaStream_t st) { return use_live(h, n_rows) ? MWW_OK : canonicalise_rings(h, st); }
-void end_nn_call(mww_t *h, int n_rows) {
-    if (!use_live(h, n_rows)) return;
-    for (int i = 0; i < 5; ++i) h->live_heads.h[i] = (h->live_heads.h[i] + 1) % kLiveRingRows[i];
+int begin_nn_call(mww_t *h, Model &m, int n_rows, cudaStream_t st) { return use_live(h, m, n_rows) ? MWW_OK : canonicalise_rings(h, m, st); }
+void end_nn_call(mww_t *h, Model &m, int n_rows) {
+    if (!use_live(h, m, n_rows)) return;
+    for (int i = 0; i < 5; ++i) m.live_heads.h[i] = (m.live_heads.h[i] + 1) % kLiveRingRows[i];
 }
 
-int run_nn_tile(mww_t *h, int first, int n, const void *d_rows, int row_type, long long rows_stream_stride_rows, int n_rows,
+int run_nn_tile(mww_t *h, Model &m, int first, int n, const void *d_rows, int row_type, long long rows_stream_stride_rows, int n_rows,
                 float *d_probs, long long probs_stride, cudaStream_t st) {
     ProfScope p(h, 2, st);
-    if (h->generic) {
-        // any architecture other than the compiled-in one: run-time-geometry kernels (mww_nn_generic.cuh)
-        if (row_type != MWW_ROWS_F32 && row_type != MWW_ROWS_U16 && row_type != MWW_ROWS_I8) return fail(h, MWW_EINVAL, "unknown row_type");
-        if (row_type == MWW_ROWS_I8 && !h->quantized) return fail(h, MWW_EINVAL, "int8 rows need a quantised model (inference.py:110)");
-        const size_t rb = row_type == MWW_ROWS_F32 ? 4 : (row_type == MWW_ROWS_U16 ? 2 : 1);
-        const int rt = row_type == MWW_ROWS_U16 ? 0 : (row_type == MWW_ROWS_F32 ? 1 : 2);
-        if (h->quantized)
-            CU(h, launch_nn_generic_i8(h->G, h->GQ, static_cast<int8_t *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                                       static_cast<int8_t *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
-                                       rows_stream_stride_rows * kNumChannels * (long long)rb, n_rows, rt, d_probs, probs_stride, n, st));
-        else if (h->hybrid)
-            CU(h, launch_nn_generic_hybrid(h->G, h->GW, h->GH, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                                           static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
-                                           rows_stream_stride_rows * kNumChannels * (long long)rb, n_rows, rt, d_probs, probs_stride, n, st));
+    if (row_type != MWW_ROWS_F32 && row_type != MWW_ROWS_U16 && row_type != MWW_ROWS_I8) return fail(h, MWW_EINVAL, "unknown row_type");
+    if (row_type == MWW_ROWS_I8 && !m.quantized()) return fail(h, MWW_EINVAL, "int8 rows need a quantised model (inference.py:110)");
+    const long long rows_stride_bytes = rows_stream_stride_rows * kNumChannels * (row_type == MWW_ROWS_F32 ? 4 : (row_type == MWW_ROWS_U16 ? 2 : 1));
+    switch (m.kind) {
+    // any architecture other than the compiled-in one: run-time-geometry kernels (mww_nn_generic.cuh)
+    case ModelKind::kGenericI8:
+        CU(h, launch_nn_generic_i8(m.G, m.GQ, m.state<int8_t>(first), m.pend<int8_t>(first), m.n_pend, d_rows, rows_stride_bytes, n_rows, row_type,
+                                   d_probs, probs_stride, n, st));
+        break;
+    case ModelKind::kHybrid:
+        CU(h, launch_nn_generic_hybrid(m.G, m.GW, m.GH, m.state<float>(first), m.pend<float>(first), m.n_pend, d_rows, rows_stride_bytes, n_rows,
+                                       row_type, d_probs, probs_stride, n, st));
+        break;
+    case ModelKind::kGenericF32:
+        CU(h, launch_nn_generic_f32(m.G, m.GW, m.state<float>(first), m.pend<float>(first), m.n_pend, d_rows, rows_stride_bytes, n_rows, row_type,
+                                    d_probs, probs_stride, n, st));
+        break;
+    case ModelKind::kCompiledI8:
+        if (reinterpret_cast<uintptr_t>(d_rows) % 16 != 0)          // the integer kernels read rows 8 / 16 bytes at a time
+            return fail(h, MWW_EINVAL, "feature rows for an int8 model must be 16-byte aligned");
+        if (use_live(h, m, n_rows))
+            CU(h, launch_nn_i8_live(m.Wq, m.state<int8_t>(first), m.pend<int8_t>(first), m.n_pend, d_rows, rows_stride_bytes, row_type, d_probs,
+                                    probs_stride, n, m.live_heads, h->sm_count, st));
         else
-            CU(h, launch_nn_generic_f32(h->G, h->GW, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                                        static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
-                                        rows_stream_stride_rows * kNumChannels * (long long)rb, n_rows, rt, d_probs, probs_stride, n, st));
-        h->launches += 1;
-        return MWW_OK;
+            CU(h, launch_nn_i8(m.Wq, m.state<int8_t>(first), m.pend<int8_t>(first), m.n_pend, d_rows, rows_stride_bytes, n_rows, row_type, d_probs,
+                               probs_stride, n, st));
+        break;
+    case ModelKind::kCompiledF32:
+        if (use_live(h, m, n_rows))
+            // exactly one model step per stream: the stream-parallel live-step kernel (HBM-bound on the ring state)
+            CU(h, launch_nn_f32_live(m.W, m.state<float>(first), m.pend<float>(first), m.n_pend, d_rows, rows_stride_bytes, row_type == MWW_ROWS_F32,
+                                     d_probs, probs_stride, n, m.live_heads, h->sm_count, h->live_variant, st));
+        else if (!h->no_tc && row_type == MWW_ROWS_U16 && (m.n_pend + n_rows) / 3 >= kTcMinSteps && reinterpret_cast<uintptr_t>(d_rows) % 16 == 0 &&
+                 rows_stride_bytes % 16 == 0)
+            // long calls on raw frontend rows: time is the M dimension of wgmma (mww_nn_tc.cu)
+            CU(h, launch_nn_f32_tc(m.W, m.TW, m.tc_f16 && m.tc_rows_bounded, m.state<float>(first), m.pend<float>(first), m.n_pend,
+                                   static_cast<const uint16_t *>(d_rows), rows_stream_stride_rows * kNumChannels, n_rows, d_probs, probs_stride, n,
+                                   h->sm_count, st));
+        else
+            CU(h, launch_nn_f32(m.W, m.state<float>(first), m.pend<float>(first), m.n_pend, d_rows, rows_stride_bytes, n_rows,
+                                row_type == MWW_ROWS_F32, d_probs, probs_stride, nullptr, n, st));
+        break;
     }
-    if (h->quantized) {
-        if (row_type == MWW_ROWS_F32 || row_type == MWW_ROWS_U16 || row_type == MWW_ROWS_I8) {
-            const size_t rb = row_type == MWW_ROWS_F32 ? 4 : (row_type == MWW_ROWS_U16 ? 2 : 1);
-            if (reinterpret_cast<uintptr_t>(d_rows) % 16 != 0)          // the integer kernels read rows 8 / 16 bytes at a time
-                return fail(h, MWW_EINVAL, "feature rows for an int8 model must be 16-byte aligned");
-            if (use_live(h, n_rows)) {
-                CU(h, launch_nn_i8_live(h->Wq, static_cast<int8_t *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                                        static_cast<int8_t *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
-                                        rows_stream_stride_rows * kNumChannels * (long long)rb, row_type, d_probs, probs_stride, n,
-                                        h->live_heads, h->sm_count, st));
-                h->launches += 1;
-                return MWW_OK;
-            }
-            CU(h, launch_nn_i8(h->Wq, static_cast<int8_t *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                               static_cast<int8_t *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
-                               rows_stream_stride_rows * kNumChannels * (long long)rb, n_rows, row_type, d_probs, probs_stride, n, st));
-            h->launches += 1;
-            return MWW_OK;
-        }
-        return fail(h, MWW_EINVAL, "unknown row_type");
-    }
-    if (row_type == MWW_ROWS_I8) return fail(h, MWW_EINVAL, "int8 rows need a quantised model (inference.py:110)");
-    const size_t rb = row_type == MWW_ROWS_F32 ? 4 : 2;
-    if (use_live(h, n_rows)) {
-        // exactly one model step per stream: the stream-parallel live-step kernel (HBM-bound on the ring state)
-        CU(h, launch_nn_f32_live(h->W, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                                 static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
-                                 rows_stream_stride_rows * kNumChannels * (long long)rb, row_type == MWW_ROWS_F32, d_probs, probs_stride, n,
-                                 h->live_heads, h->sm_count, h->live_variant, st));
-        h->launches += 1;
-        return MWW_OK;
-    }
-    if (!h->no_tc && row_type == MWW_ROWS_U16 && (h->n_pend + n_rows) / 3 >= kTcMinSteps && reinterpret_cast<uintptr_t>(d_rows) % 16 == 0 &&
-        (rows_stream_stride_rows * kNumChannels * 2) % 16 == 0) {
-        // long calls on raw frontend rows: time is the M dimension of wgmma (mww_nn_tc.cu)
-        CU(h, launch_nn_f32_tc(h->W, h->TW, h->tc_f16 && h->tc_rows_bounded, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                               static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend,
-                               static_cast<const uint16_t *>(d_rows), rows_stream_stride_rows * kNumChannels, n_rows, d_probs, probs_stride, n,
-                               h->sm_count, st));
-        h->launches += 1;
-        return MWW_OK;
-    }
-    CU(h, launch_nn_f32(h->W, static_cast<float *>(h->d_nn_state) + (size_t)first * h->state_elems,
-                        static_cast<float *>(h->d_pend) + (size_t)first * h->pend_cap * kNumChannels, h->n_pend, d_rows,
-                        rows_stream_stride_rows * kNumChannels * (long long)rb, n_rows, row_type == MWW_ROWS_F32, d_probs, probs_stride,
-                        nullptr, n, st));
     h->launches += 1;
     return MWW_OK;
 }
@@ -390,263 +324,21 @@ int upload_tables(mww_t *h) {
     return MWW_OK;
 }
 
-struct Need { const char *name; uint32_t dtype; size_t count; };
-
-// weights of an architecture other than the compiled-in one (tensor names and layouts: microwakeword_b200/model_file.py,
-// the same names the CPU checker reads)
-int upload_weights_generic(mww_t *h, const uint8_t *blob, size_t n, const Tensor &arch) {
-    GenArch &G = h->G;
-    const int rc_arch = gen_arch_from_tensor(reinterpret_cast<const int32_t *>(arch.data), (int)(arch.nbytes / 4), &G);
-    if (rc_arch == -1) return fail(h, MWW_EMODEL, "model container: malformed 'arch' tensor");
-    if (rc_arch != 0 || (size_t)G.sm_elems * 4 > 200 * 1024)
-        return fail(h, MWW_EUNSUPPORTED, "model container: architecture outside the supported range (first_conv_kernel_size >= stride, <= 8 blocks, "
-                                         "<= 512 channels, kernels <= 64 taps, ring buffers of one stream within 200 KB)");
-    Tensor probe;
-    h->quantized = find_tensor(blob, n, "q/scales", &probe);
-    h->generic = true;
-    h->stride = G.stride; h->pend_cap = G.pend_cap; h->state_elems = G.state_elems; h->macs_per_step = G.macs_per_step;
-    size_t total = 1 << 16;                          // room for alignment padding; tensors are added below
-    {
-        uint32_t hdr[4];
-        memcpy(hdr, blob + 8, 16);
-        total += n + (size_t)hdr[1] * 256;
-    }
-    CU(h, cudaMalloc(&h->d_weights, total));
-    size_t cur = 0;
-    cudaError_t e = cudaSuccess;
-    char name[64];
-    auto get = [&](const char *nm, uint32_t dtype, size_t count, const void **dev) -> int {
-        Tensor t;
-        static const size_t esz[6] = {4, 1, 4, 1, 2, 2};
-        if (!find_tensor(blob, n, nm, &t)) return fail(h, MWW_EMODEL, std::string("model container: missing tensor ") + nm);
-        if (t.dtype != dtype || t.nbytes != count * esz[dtype]) return fail(h, MWW_EMODEL, std::string("model container: wrong dtype/size for ") + nm);
-        if (cur + t.nbytes + 256 > total) return fail(h, MWW_EMODEL, "model container: tensors larger than the container");
-        if (!upload(h->d_weights, cur, t.data, (size_t)t.nbytes, reinterpret_cast<const uint8_t **>(dev), &e)) return cuda_fail(h, e, "weight upload");
-        return MWW_OK;
-    };
-    auto scalar = [&](const char *nm, int32_t *out) -> int {
-        Tensor t;
-        if (!find_tensor(blob, n, nm, &t) || t.nbytes != 4) return fail(h, MWW_EMODEL, std::string("model container: ") + nm);
-        memcpy(out, t.data, 4);
-        return MWW_OK;
-    };
-    int rc;
-    const size_t k0f = (size_t)G.k0 * kNumChannels * G.c0;
-    if (!h->quantized) {
-        GenWeightsF32 &W = h->GW;
-        if ((rc = get("first_conv/w", 0, k0f, (const void **)&W.w0))) return rc;
-        for (int i = 0; i < G.n_blocks; ++i) {
-            snprintf(name, sizeof name, "b%d/dw/w", i); if ((rc = get(name, 0, (size_t)G.kmax[i] * G.cin[i], (const void **)&W.dw_w[i]))) return rc;
-            snprintf(name, sizeof name, "b%d/dw/b", i); if ((rc = get(name, 0, G.cin[i], (const void **)&W.dw_b[i]))) return rc;
-            snprintf(name, sizeof name, "b%d/pw/w", i); if ((rc = get(name, 0, (size_t)G.cin[i] * G.cout[i], (const void **)&W.pw_w[i]))) return rc;
-            snprintf(name, sizeof name, "b%d/pw/b", i); if ((rc = get(name, 0, G.cout[i], (const void **)&W.pw_b[i]))) return rc;
-        }
-        if ((rc = get("head/w", 0, (size_t)G.head_rows * G.c_last, (const void **)&W.head_w))) return rc;
-        if ((rc = get("head/b", 0, 1, (const void **)&W.head_b))) return rc;
-        Tensor mode;
-        if (!find_tensor(blob, n, "hy/mode", &mode)) return MWW_OK;
-        // hybrid layers (model_file.py): int8 weights + per-channel scales next to the fp32 tensors
-        GenHybrid &H = h->GH;
-        if (mode.dtype != 2 || mode.nbytes % 4 != 0 || mode.nbytes > 4 * (2 + 5 * kGenMaxBlocks)) return fail(h, MWW_EMODEL, "model container: malformed 'hy/mode'");
-        int32_t modes[2 + 5 * kGenMaxBlocks];
-        memcpy(modes, mode.data, mode.nbytes);
-        if (gen_hybrid_layout(G, reinterpret_cast<const int32_t *>(arch.data), modes, (int)(mode.nbytes / 4), &H) != 0)
-            return fail(h, MWW_EMODEL, "model container: 'hy/mode' does not match the architecture (one entry per first conv, MixConv group, 1x1 conv, head; 0..2)");
-        if ((size_t)H.sm_elems * 4 > 200 * 1024)
-            return fail(h, MWW_EUNSUPPORTED, "model container: rings and quantisation buffers of one stream exceed 200 KB of shared memory");
-        h->hybrid = true;
-        if (H.mode0) {
-            if ((rc = get("hy/first_conv/w", 1, k0f, (const void **)&H.w0))) return rc;
-            if ((rc = get("hy/first_conv/scale", 0, G.c0, (const void **)&H.s0))) return rc;
-        }
-        for (int i = 0; i < G.n_blocks; ++i) {
-            if (H.any_dw[i]) {
-                snprintf(name, sizeof name, "hy/b%d/dw/w", i); if ((rc = get(name, 1, (size_t)G.kmax[i] * G.cin[i], (const void **)&H.dw_w[i]))) return rc;
-                snprintf(name, sizeof name, "hy/b%d/dw/scale", i); if ((rc = get(name, 0, G.cin[i], (const void **)&H.dw_s[i]))) return rc;
-            }
-            if (H.mode_pw[i]) {
-                snprintf(name, sizeof name, "hy/b%d/pw/w", i); if ((rc = get(name, 1, (size_t)G.cin[i] * G.cout[i], (const void **)&H.pw_w[i]))) return rc;
-                snprintf(name, sizeof name, "hy/b%d/pw/scale", i); if ((rc = get(name, 0, G.cout[i], (const void **)&H.pw_s[i]))) return rc;
-            }
-        }
-        if (H.mode_head) {
-            if ((rc = get("hy/head/w", 1, (size_t)G.head_rows * G.c_last, (const void **)&H.head_w))) return rc;
-            if ((rc = get("hy/head/scale", 0, 1, (const void **)&H.head_s))) return rc;
-        }
-        return MWW_OK;
-    }
-    GenWeightsI8 &Q = h->GQ;
-    if ((rc = get("q/first_conv/w", 1, k0f, (const void **)&Q.w0))) return rc;
-    if ((rc = get("q/first_conv/bias", 2, G.c0, (const void **)&Q.b0))) return rc;
-    if ((rc = get("q/first_conv/mult", 2, G.c0, (const void **)&Q.m0))) return rc;
-    if ((rc = get("q/first_conv/shift", 2, G.c0, (const void **)&Q.s0))) return rc;
-    for (int i = 0; i < G.n_blocks; ++i) {
-        snprintf(name, sizeof name, "q/b%d/dw/w", i); if ((rc = get(name, 1, (size_t)G.kmax[i] * G.cin[i], (const void **)&Q.dw_w[i]))) return rc;
-        snprintf(name, sizeof name, "q/b%d/dw/bias", i); if ((rc = get(name, 2, G.cin[i], (const void **)&Q.dw_b[i]))) return rc;
-        snprintf(name, sizeof name, "q/b%d/dw/mult", i); if ((rc = get(name, 2, G.cin[i], (const void **)&Q.dw_m[i]))) return rc;
-        snprintf(name, sizeof name, "q/b%d/dw/shift", i); if ((rc = get(name, 2, G.cin[i], (const void **)&Q.dw_s[i]))) return rc;
-        snprintf(name, sizeof name, "q/b%d/pw/w", i); if ((rc = get(name, 1, (size_t)G.cin[i] * G.cout[i], (const void **)&Q.pw_w[i]))) return rc;
-        snprintf(name, sizeof name, "q/b%d/pw/bias", i); if ((rc = get(name, 2, G.cout[i], (const void **)&Q.pw_b[i]))) return rc;
-        snprintf(name, sizeof name, "q/b%d/pw/mult", i); if ((rc = get(name, 2, G.cout[i], (const void **)&Q.pw_m[i]))) return rc;
-        snprintf(name, sizeof name, "q/b%d/pw/shift", i); if ((rc = get(name, 2, G.cout[i], (const void **)&Q.pw_s[i]))) return rc;
-    }
-    if ((rc = get("q/head/w", 1, (size_t)G.head_rows * G.c_last, (const void **)&Q.head_w))) return rc;
-    if ((rc = get("q/logistic_lut", 1, 256, (const void **)&Q.lut))) return rc;
-    if ((rc = scalar("q/head/bias", &Q.head_bias)) || (rc = scalar("q/head/mult", &Q.head_mult)) || (rc = scalar("q/head/shift", &Q.head_shift))) return rc;
-    const size_t n_q = 4 + 2 * (size_t)G.n_blocks;       // in, first conv, (depthwise, pointwise) per block, logit, prob
-    Tensor sc, zp;
-    if (!find_tensor(blob, n, "q/scales", &sc) || sc.nbytes != n_q * 4 || !find_tensor(blob, n, "q/zps", &zp) || zp.nbytes != n_q * 4)
-        return fail(h, MWW_EMODEL, "model container: q/scales / q/zps must hold 4 + 2 * n_blocks entries");
-    std::vector<float> scales(n_q);
-    memcpy(scales.data(), sc.data, n_q * 4);
-    memcpy(Q.zp, zp.data, n_q * 4);
-    Q.in_scale = scales[0];
-    h->in_scale = scales[0]; h->in_zp = Q.zp[0];
-    h->out_scale = scales[n_q - 1]; h->out_zp = 0;      // uint8 output tensor: zero point -128 + 128 (utils.py:338)
+// weights and per-stream NN state of one model container
+int load_model(mww_t *h, Model &m, const void *model_blob, size_t n_bytes) {
+    uint64_t x = 1469598103934665603ull;
+    for (size_t i = 0; i < n_bytes; ++i) x = (x ^ static_cast<const uint8_t *>(model_blob)[i]) * 1099511628211ull;
+    m.model_hash = x;
+    std::string msg;
+    if (int rc = parse_container(static_cast<const uint8_t *>(model_blob), n_bytes, &m, &msg)) return fail(h, rc, msg);
+    CU(h, cudaMalloc(&m.d_weights, m.arena.size()));
+    if (cudaError_t e = cudaMemcpy(m.d_weights, m.arena.data(), m.arena.size(), cudaMemcpyHostToDevice)) return cuda_fail(h, e, "weight upload");
+    m.rebase(m.d_weights);
+    const size_t S = (size_t)h->n_streams;
+    cudaError_t a = cudaMalloc(&m.d_nn_state, S * m.G.state_elems * m.elem_size());
+    if (a == cudaSuccess) a = cudaMalloc(&m.d_pend, S * m.G.pend_cap * kNumChannels * m.elem_size());
+    if (a != cudaSuccess) return fail(h, a == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("state allocation: ") + cudaGetErrorString(a));
     return MWW_OK;
-}
-
-int upload_weights(mww_t *h, const uint8_t *blob, size_t n) {
-    Tensor arch;
-    if (!find_tensor(blob, n, "arch", &arch) || arch.dtype != 2) return fail(h, MWW_EMODEL, "model container: missing 'arch' tensor or bad magic/version");
-    // the tensor-core kernels are compiled for the okay_nabu MixedNet (first conv 32x5 stride 3; MixConv [5],[7,11],[9,15],[23];
-    // pointwise 64x4; 17-row head); every other architecture takes the run-time-geometry path.  MWW_FORCE_GENERIC=1 sends
-    // okay_nabu through it as well (tests compare the two paths).
-    // A hybrid container (fp32 graph with int8-weight ops, model_file.py) of any architecture, okay_nabu's included, runs on the
-    // generic hybrid kernel: the compiled-in fp32 kernels' arithmetic is not TFLite's hybrid arithmetic.
-    Tensor hy_mode;
-    if (find_tensor(blob, n, "hy/mode", &hy_mode) || arch.nbytes != sizeof kOkayNabuArch || memcmp(arch.data, kOkayNabuArch, sizeof kOkayNabuArch) != 0 ||
-        getenv("MWW_FORCE_GENERIC") != nullptr)
-        return upload_weights_generic(h, blob, n, arch);
-    Tensor probe;
-    h->quantized = find_tensor(blob, n, "q/scales", &probe);
-    const size_t total = 1 << 20;
-    CU(h, cudaMalloc(&h->d_weights, total));
-    size_t cur = 0;
-    cudaError_t e = cudaSuccess;
-    char name[64];
-    auto get = [&](const char *nm, uint32_t dtype, size_t count, const void **dev) -> int {
-        Tensor t;
-        static const size_t esz[6] = {4, 1, 4, 1, 2, 2};
-        if (!find_tensor(blob, n, nm, &t)) return fail(h, MWW_EMODEL, std::string("model container: missing tensor ") + nm);
-        if (t.dtype != dtype || t.nbytes != count * esz[dtype]) return fail(h, MWW_EMODEL, std::string("model container: wrong dtype/size for ") + nm);
-        if (!upload(h->d_weights, cur, t.data, (size_t)t.nbytes, reinterpret_cast<const uint8_t **>(dev), &e)) return cuda_fail(h, e, "weight upload");
-        return MWW_OK;
-    };
-    static const int cin[4] = {32, 64, 64, 64}, kmax[4] = {5, 11, 15, 23};
-    int rc;
-    if (!h->quantized) {
-        if ((rc = get("first_conv/w", 0, 5 * 40 * 32, (const void **)&h->W.w0))) return rc;
-        for (int i = 0; i < 4; ++i) {
-            snprintf(name, sizeof name, "b%d/dw/w", i); if ((rc = get(name, 0, (size_t)kmax[i] * cin[i], (const void **)&h->W.dw_w[i]))) return rc;
-            snprintf(name, sizeof name, "b%d/dw/b", i); if ((rc = get(name, 0, cin[i], (const void **)&h->W.dw_b[i]))) return rc;
-            snprintf(name, sizeof name, "b%d/pw/w", i); if ((rc = get(name, 0, (size_t)cin[i] * 64, (const void **)&h->W.pw_w[i]))) return rc;
-            snprintf(name, sizeof name, "b%d/pw/b", i); if ((rc = get(name, 0, 64, (const void **)&h->W.pw_b[i]))) return rc;
-        }
-        if ((rc = get("head/w", 0, 17 * 64, (const void **)&h->W.head_w))) return rc;
-        if ((rc = get("head/b", 0, 1, (const void **)&h->W.head_b))) return rc;
-        {
-            // tensor-core operands: 3xTF32 split + slot layout, and the first conv's fp16 operands where its weights admit them,
-            // once per model (mww_nn_tc.h)
-            Tensor tw0, tpw[4];
-            bool ok = find_tensor(blob, n, "first_conv/w", &tw0);
-            const float *pw_host[4];
-            for (int i = 0; i < 4 && ok; ++i) {
-                snprintf(name, sizeof name, "b%d/pw/w", i);
-                ok = find_tensor(blob, n, name, &tpw[i]);
-                pw_host[i] = reinterpret_cast<const float *>(tpw[i].data);
-            }
-            if (!ok) return fail(h, MWW_EMODEL, "model container: fp32 weights missing");
-            std::vector<float> w0_copy(5 * 40 * 32), pw_copy[4];
-            memcpy(w0_copy.data(), tw0.data, w0_copy.size() * 4);                    // container tensors are not necessarily 4-byte aligned
-            const float *pw_al[4];
-            for (int i = 0; i < 4; ++i) {
-                pw_copy[i].resize((size_t)cin[i] * 64);
-                memcpy(pw_copy[i].data(), pw_host[i], pw_copy[i].size() * 4);
-                pw_al[i] = pw_copy[i].data();
-            }
-            const TcF16Scales sc = tc_f16_scales(w0_copy.data());
-            h->tc_f16 = sc.ok && !h->tc_tf32;
-            std::vector<unsigned char> tcb;
-            size_t offs[6];
-            build_tc_weights(w0_copy.data(), pw_al, h->tc_f16 ? &sc : nullptr, &tcb, offs);
-            const unsigned char *dev_tc = nullptr;
-            if (cur + tcb.size() + 256 > total) return fail(h, MWW_EMODEL, "weight arena too small for the tensor-core operands");
-            if (!upload(h->d_weights, cur, tcb.data(), tcb.size(), &dev_tc, &e)) return cuda_fail(h, e, "weight upload");
-            h->TW.fc = dev_tc + offs[0];
-            for (int i = 0; i < 4; ++i) h->TW.pw[i] = dev_tc + offs[1 + i];
-            if (h->tc_f16) {
-                h->TW.fc16 = dev_tc + offs[5];
-                h->TW.fc_out = ldexpf(1.f, -sc.s_fc);
-            }
-        }
-    } else {
-        NnWeightsI8 &Q = h->Wq;
-        if ((rc = get("q/first_conv/w", 1, 5 * 40 * 32, (const void **)&Q.w0))) return rc;
-        if ((rc = get("q/first_conv/bias", 2, 32, (const void **)&Q.b0))) return rc;
-        if ((rc = get("q/first_conv/mult", 2, 32, (const void **)&Q.m0))) return rc;
-        if ((rc = get("q/first_conv/shift", 2, 32, (const void **)&Q.s0))) return rc;
-        for (int i = 0; i < 4; ++i) {
-            snprintf(name, sizeof name, "q/b%d/dw/w", i); if ((rc = get(name, 1, (size_t)kmax[i] * cin[i], (const void **)&Q.dw_w[i]))) return rc;
-            snprintf(name, sizeof name, "q/b%d/dw/bias", i); if ((rc = get(name, 2, cin[i], (const void **)&Q.dw_b[i]))) return rc;
-            snprintf(name, sizeof name, "q/b%d/dw/mult", i); if ((rc = get(name, 2, cin[i], (const void **)&Q.dw_m[i]))) return rc;
-            snprintf(name, sizeof name, "q/b%d/dw/shift", i); if ((rc = get(name, 2, cin[i], (const void **)&Q.dw_s[i]))) return rc;
-            snprintf(name, sizeof name, "q/b%d/pw/w", i); if ((rc = get(name, 1, (size_t)cin[i] * 64, (const void **)&Q.pw_w[i]))) return rc;
-            snprintf(name, sizeof name, "q/b%d/pw/bias", i); if ((rc = get(name, 2, 64, (const void **)&Q.pw_b[i]))) return rc;
-            snprintf(name, sizeof name, "q/b%d/pw/mult", i); if ((rc = get(name, 2, 64, (const void **)&Q.pw_m[i]))) return rc;
-            snprintf(name, sizeof name, "q/b%d/pw/shift", i); if ((rc = get(name, 2, 64, (const void **)&Q.pw_s[i]))) return rc;
-        }
-        if ((rc = get("q/head/w", 1, 17 * 64, (const void **)&Q.head_w))) return rc;
-        if ((rc = get("q/logistic_lut", 1, 256, (const void **)&Q.lut))) return rc;
-        Tensor t;
-        if (!find_tensor(blob, n, "q/head/bias", &t) || t.nbytes != 4) return fail(h, MWW_EMODEL, "model container: q/head/bias");
-        memcpy(&Q.head_bias, t.data, 4);
-        if (!find_tensor(blob, n, "q/head/mult", &t) || t.nbytes != 4) return fail(h, MWW_EMODEL, "model container: q/head/mult");
-        memcpy(&Q.head_mult, t.data, 4);
-        if (!find_tensor(blob, n, "q/head/shift", &t) || t.nbytes != 4) return fail(h, MWW_EMODEL, "model container: q/head/shift");
-        memcpy(&Q.head_shift, t.data, 4);
-        Tensor sc, zp;
-        if (!find_tensor(blob, n, "q/scales", &sc) || sc.nbytes != 12 * 4 || !find_tensor(blob, n, "q/zps", &zp) || zp.nbytes != 12 * 4)
-            return fail(h, MWW_EMODEL, "model container: q/scales / q/zps must hold 12 entries");
-        float scales[12];
-        memcpy(scales, sc.data, sizeof scales);
-        memcpy(Q.zp, zp.data, sizeof Q.zp);
-        Q.in_scale = scales[0];
-        h->in_scale = scales[0]; h->in_zp = Q.zp[0];
-        // tensor-core operands: K-contiguous weight rows and zero-point-folded biases (mww_nn_i8_prep.h)
-        {
-            Tensor tw0, tb0, tpw[4], tpb[4];
-            bool ok = find_tensor(blob, n, "q/first_conv/w", &tw0) && find_tensor(blob, n, "q/first_conv/bias", &tb0);
-            const int8_t *pw_w[4]; const int32_t *pw_b[4];
-            for (int i = 0; i < 4 && ok; ++i) {
-                snprintf(name, sizeof name, "q/b%d/pw/w", i); ok = ok && find_tensor(blob, n, name, &tpw[i]);
-                snprintf(name, sizeof name, "q/b%d/pw/bias", i); ok = ok && find_tensor(blob, n, name, &tpb[i]);
-                pw_w[i] = reinterpret_cast<const int8_t *>(tpw[i].data); pw_b[i] = reinterpret_cast<const int32_t *>(tpb[i].data);
-            }
-            if (!ok) return fail(h, MWW_EMODEL, "model container: int8 weights missing");
-            I8MmaOperands ops;
-            build_i8_mma_operands(reinterpret_cast<const int8_t *>(tw0.data), reinterpret_cast<const int32_t *>(tb0.data), pw_w, pw_b, Q.zp, &ops);
-            bool up = upload(h->d_weights, cur, ops.w0t.data(), ops.w0t.size(), &Q.w0t, &e) &&
-                      upload(h->d_weights, cur, ops.b0f.data(), ops.b0f.size() * 4, &Q.b0f, &e);
-            for (int i = 0; i < 4 && up; ++i)
-                up = upload(h->d_weights, cur, ops.pwt[i].data(), ops.pwt[i].size(), &Q.pwt[i], &e) &&
-                     upload(h->d_weights, cur, ops.pw_bf[i].data(), ops.pw_bf[i].size() * 4, &Q.pw_bf[i], &e);
-            if (!up) return cuda_fail(h, e, "weight upload");
-            if (getenv("MWW_NO_QLUT") == nullptr) {
-                std::vector<int8_t> qlut;
-                build_feature_qlut(Q.in_scale, Q.zp[0], &qlut);
-                if (!upload(h->d_weights, cur, qlut.data(), qlut.size(), &Q.qlut, &e)) return cuda_fail(h, e, "weight upload");
-            }
-        }
-        h->out_scale = scales[11]; h->out_zp = 0;   // uint8 output tensor: zero point -128 + 128 (utils.py:338)
-    }
-    return MWW_OK;
-}
-
-// a failure of model m's call is reported on the handle h the caller holds
-int model_rc(mww_t *h, const mww_t *m, int rc) {
-    if (rc != MWW_OK && m != h) h->err = m->err;
-    return rc;
 }
 
 // A state set from outside keeps the fp16 first conv only if every first-conv ring row (state floats [0, 80) of a stream) it
@@ -659,53 +351,57 @@ bool rows_are_features(const float *v, size_t n) {
     }
     return true;
 }
-void note_state_set(mww_t *m, const void *h_nn, const void *h_pending, int pending_rows) {
+void note_state_set(mww_t *h, Model &m, const void *h_nn, const void *h_pending, int pending_rows) {
     if (!h_nn && !h_pending) return;
-    bool ok = m->tc_f16 && (h_nn || m->tc_rows_bounded) && (h_pending || m->tc_rows_bounded);
-    for (int s = 0; ok && s < m->n_streams; ++s) {
-        if (h_nn) ok = rows_are_features(static_cast<const float *>(h_nn) + (size_t)s * m->state_elems, 2 * kNumChannels);
+    bool ok = m.tc_f16 && (h_nn || m.tc_rows_bounded) && (h_pending || m.tc_rows_bounded);
+    for (int s = 0; ok && s < h->n_streams; ++s) {
+        if (h_nn) ok = rows_are_features(static_cast<const float *>(h_nn) + (size_t)s * m.G.state_elems, 2 * kNumChannels);
         if (ok && h_pending)
-            ok = rows_are_features(static_cast<const float *>(h_pending) + (size_t)s * m->pend_cap * kNumChannels, (size_t)pending_rows * kNumChannels);
+            ok = rows_are_features(static_cast<const float *>(h_pending) + (size_t)s * m.G.pend_cap * kNumChannels, (size_t)pending_rows * kNumChannels);
     }
-    m->tc_rows_bounded = ok;
+    m.tc_rows_bounded = ok;
 }
 
 // fresh rings and no pending rows for every stream of one model
-int zero_nn_state(mww_t *h, cudaStream_t st) {
+int zero_nn_state(mww_t *h, Model &m, cudaStream_t st) {
     const size_t S = (size_t)h->n_streams;
-    h->n_pend = 0;
-    if (h->quantized && h->generic) {
-        CU(h, launch_gen_fill_state_i8(h->G, h->GQ, static_cast<int8_t *>(h->d_nn_state), static_cast<int8_t *>(h->d_pend), h->n_streams, nullptr, h->n_streams, st));
+    m.n_pend = 0;
+    if (m.kind == ModelKind::kGenericI8) {
+        CU(h, launch_gen_fill_state_i8(m.G, m.GQ, m.state<int8_t>(0), m.pend<int8_t>(0), h->n_streams, nullptr, h->n_streams, st));
         h->launches += 1;
-    } else if (h->quantized) {
-        CU(h, launch_fill_state_i8(h->Wq, static_cast<int8_t *>(h->d_nn_state), static_cast<int8_t *>(h->d_pend), nullptr, h->n_streams, h->n_streams, st));
+    } else if (m.kind == ModelKind::kCompiledI8) {
+        CU(h, launch_fill_state_i8(m.Wq, m.state<int8_t>(0), m.pend<int8_t>(0), nullptr, h->n_streams, h->n_streams, st));
         h->launches += 1;
     } else {
-        CU(h, cudaMemsetAsync(h->d_nn_state, 0, S * h->state_elems * 4, st));
-        CU(h, cudaMemsetAsync(h->d_pend, 0, S * h->pend_cap * kNumChannels * 4, st));
+        CU(h, cudaMemsetAsync(m.d_nn_state, 0, S * m.G.state_elems * 4, st));
+        CU(h, cudaMemsetAsync(m.d_pend, 0, S * m.G.pend_cap * kNumChannels * 4, st));
     }
-    h->live_heads = LiveHeads{};
-    h->n_pend = 0;
-    h->tc_rows_bounded = true;
+    m.live_heads = LiveHeads{};
+    m.tc_rows_bounded = true;
     return MWW_OK;
 }
 
-int zero_state(mww_t *h, cudaStream_t st) {
+int zero_frontend(mww_t *h, cudaStream_t st) {
     const size_t S = (size_t)h->n_streams;
     CU(h, cudaMemsetAsync(h->d_carry, 0, S * kWindow * sizeof(int16_t), st));
     CU(h, cudaMemsetAsync(h->d_estimate, 0, S * kNumChannels * sizeof(uint32_t), st));
     h->used = 0;
-    for (mww_t *m : h->models)
-        if (int rc = model_rc(h, m, zero_nn_state(m, st))) return rc;
+    return MWW_OK;
+}
+
+int zero_state(mww_t *h, cudaStream_t st) {
+    if (int rc = zero_frontend(h, st)) return rc;
+    for (Model &m : h->models)
+        if (int rc = zero_nn_state(h, m, st)) return rc;
     return MWW_OK;
 }
 
 void destroy_impl(mww_t *h) {
     if (!h) return;
     DeviceGuard guard(h->device);
-    for (size_t k = 1; k < h->models.size(); ++k) destroy_impl(h->models[k]);
-    cudaFree(h->d_tables); cudaFree(h->d_weights); cudaFree(h->d_carry); cudaFree(h->d_estimate);
-    cudaFree(h->d_nn_state); cudaFree(h->d_pend); cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
+    for (Model &m : h->models) { cudaFree(m.d_weights); cudaFree(m.d_nn_state); cudaFree(m.d_pend); }
+    cudaFree(h->d_tables); cudaFree(h->d_carry); cudaFree(h->d_estimate);
+    cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
     for (int b = 0; b < 2; ++b) {
         cudaFree(h->d_audio_tile[b]); cudaFree(h->d_probs_tile[b]);
         if (h->ev_h2d[b]) cudaEventDestroy(h->ev_h2d[b]);
@@ -760,8 +456,8 @@ int check_outs(mww_t *h, const char *who, int n_frames, float *const *probs, con
     if (h->models.size() > 1 && (!probs || !max_probs)) return fail(h, MWW_EINVAL, std::string(who) + ": NULL output arrays");
     o->probs = probs; o->max_probs = max_probs;
     for (size_t k = 0; k < h->models.size(); ++k) {
-        const mww_t *m = h->models[k];
-        o->steps[k] = (m->n_pend + n_frames) / m->stride;
+        const Model &m = h->models[k];
+        o->steps[k] = (m.n_pend + n_frames) / m.G.stride;
         if (o->steps[k] > max_probs[k] || (o->steps[k] > 0 && !probs[k]))
             return fail(h, MWW_EINVAL, std::string(who) + ": probability buffer too small" +
                                            (h->models.size() > 1 ? " for model " + std::to_string(k) : std::string()));
@@ -771,24 +467,22 @@ int check_outs(mww_t *h, const char *who, int n_frames, float *const *probs, con
 // once per call, after the last tile: every model's pending rows and live ring heads move on
 void end_models_call(mww_t *h, int n_frames, const NnOuts &o, int *h_probs_out) {
     for (size_t k = 0; k < h->models.size(); ++k) {
-        mww_t *m = h->models[k];
-        end_nn_call(m, n_frames);
-        if (o.steps[k] >= kTcFreshSteps) m->tc_rows_bounded = true;      // first-conv ring, pending rows: this call's own rows
-        m->n_pend = (m->n_pend + n_frames) % m->stride;
+        Model &m = h->models[k];
+        end_nn_call(h, m, n_frames);
+        if (o.steps[k] >= kTcFreshSteps) m.tc_rows_bounded = true;      // first-conv ring, pending rows: this call's own rows
+        m.n_pend = (m.n_pend + n_frames) % m.G.stride;
         if (h_probs_out) h_probs_out[k] = o.steps[k];
     }
 }
 int begin_models_call(mww_t *h, int n_frames, cudaStream_t st) {
-    for (mww_t *m : h->models)
-        if (int rc = model_rc(h, m, begin_nn_call(m, n_frames, st))) return rc;
+    for (Model &m : h->models)
+        if (int rc = begin_nn_call(h, m, n_frames, st)) return rc;
     return MWW_OK;
 }
 // every model on one tile of frontend rows; probs[k] (pitch probs_stride[k]) points at the tile's first stream
 int run_models_tile(mww_t *h, int first, int n, int n_frames, float *const *probs, const long long *probs_stride, cudaStream_t st) {
-    for (size_t k = 0; k < h->models.size(); ++k) {
-        mww_t *m = h->models[k];
-        if (int rc = model_rc(h, m, run_nn_tile(m, first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, probs[k], probs_stride[k], st))) return rc;
-    }
+    for (size_t k = 0; k < h->models.size(); ++k)
+        if (int rc = run_nn_tile(h, h->models[k], first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, probs[k], probs_stride[k], st)) return rc;
     return MWW_OK;
 }
 
@@ -798,7 +492,7 @@ int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples
                       const int *max_probs, int *h_probs_out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
-    if (!h->has_nn) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
+    if (h->models.empty()) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     ENTER_STATEFUL(h);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
     const int n_frames = frames_for(h, n_samples);
@@ -854,25 +548,10 @@ mww_t *new_handle(int device, int n_streams) {
     h->no_live = getenv("MWW_NO_LIVE") != nullptr;
     h->no_fuse = getenv("MWW_NO_FUSE") != nullptr;
     h->no_tc = getenv("MWW_NO_TC") != nullptr;
-    h->tc_tf32 = getenv("MWW_TC_TF32") != nullptr;
     h->live_variant = getenv("MWW_LIVE_VARIANT") != nullptr ? atoi(getenv("MWW_LIVE_VARIANT")) : (getenv("MWW_LIVE_V2") != nullptr ? 2 : 3);
     if (const char *mb = getenv("MWW_SCRATCH_MB")) { const long v = atol(mb); if (v > 0) h->scratch_budget = (size_t)v << 20; }
     if (const char *mt = getenv("MWW_MIN_TILE_STREAMS")) { const long v = atol(mt); if (v > 0) h->min_tile_streams = (int)v; }
     return h;
-}
-
-// weights and per-stream NN state of one model container
-int load_model(mww_t *m, const void *model_blob, size_t n_bytes) {
-    uint64_t x = 1469598103934665603ull;
-    for (size_t i = 0; i < n_bytes; ++i) x = (x ^ static_cast<const uint8_t *>(model_blob)[i]) * 1099511628211ull;
-    m->model_hash = x;
-    int rc = upload_weights(m, static_cast<const uint8_t *>(model_blob), n_bytes);
-    if (rc) return rc;
-    const size_t S = (size_t)m->n_streams;
-    cudaError_t a = cudaMalloc(&m->d_nn_state, S * m->state_elems * elem_size(m));
-    if (a == cudaSuccess) a = cudaMalloc(&m->d_pend, S * m->pend_cap * kNumChannels * elem_size(m));
-    if (a != cudaSuccess) return fail(m, a == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("state allocation: ") + cudaGetErrorString(a));
-    return MWW_OK;
 }
 
 // mww_create (n_models 0: frontend-only, 1: one model) and mww_create_multi (`multi`: messages name the failing model's index)
@@ -885,14 +564,11 @@ int create_impl(const char *who, const void *const *blobs, const size_t *n_bytes
     DeviceGuard guard(device);
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
     mww_t *h = new_handle(device, n_streams);
-    h->has_nn = n_models > 0;
     int rc = upload_tables(h);
     for (int k = 0; rc == MWW_OK && k < n_models; ++k) {
-        mww_t *m = k == 0 ? h : new_handle(device, n_streams);
-        h->models.push_back(m);
-        rc = load_model(m, blobs[k], n_bytes[k]);
-        if (rc != MWW_OK && multi) h->err = "model " + std::to_string(k) + ": " + m->err;
-        else if (rc != MWW_OK) h->err = m->err;
+        h->models.emplace_back();
+        rc = load_model(h, h->models.back(), blobs[k], n_bytes[k]);
+        if (rc != MWW_OK && multi) h->err = "model " + std::to_string(k) + ": " + h->err;
     }
     if (rc == MWW_OK) {
         const size_t S = (size_t)n_streams;
@@ -931,12 +607,7 @@ int mww_destroy(mww_t *h) { destroy_impl(h); return MWW_OK; }
 
 const char *mww_last_error(const mww_t *h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
-long long mww_launch_count(const mww_t *h) {
-    if (!h) return 0;
-    long long n = h->launches;
-    for (size_t k = 1; k < h->models.size(); ++k) n += h->models[k]->launches;
-    return n;
-}
+long long mww_launch_count(const mww_t *h) { return h ? h->launches : 0; }
 
 int mww_copy_async(void *d_dst, const void *d_src, size_t bytes, void *cu_stream) {
     if (bytes == 0) return MWW_OK;
@@ -1000,7 +671,6 @@ int mww_ipc_free(void *d_ptr, int device) {
 int mww_profile_enable(mww_t *h, int on) {
     if (!h) return MWW_EINVAL;
     h->profiling = on != 0;
-    for (mww_t *m : h->models) m->profiling = h->profiling;
     return MWW_OK;
 }
 
@@ -1008,17 +678,14 @@ int mww_profile_read(mww_t *h, double *ms4, long long *counts4) {
     if (!h || !ms4 || !counts4) return MWW_EINVAL;
     ENTER(h);
     CU(h, cudaDeviceSynchronize());
-    for (size_t k = 0; k < std::max<size_t>(h->models.size(), 1); ++k) {
-        mww_t *m = k == 0 ? h : h->models[k];
-        for (int c = 0; c < 4; ++c) {
-            std::vector<cudaEvent_t> &v = m->prof_ev[c];
-            for (size_t i = 0; i + 1 < v.size(); i += 2) {
-                float ms = 0.f;
-                if (cudaEventElapsedTime(&ms, v[i], v[i + 1]) == cudaSuccess) { ms4[c] += ms; counts4[c] += 1; }
-                cudaEventDestroy(v[i]); cudaEventDestroy(v[i + 1]);
-            }
-            v.clear();
+    for (int c = 0; c < 4; ++c) {
+        std::vector<cudaEvent_t> &v = h->prof_ev[c];
+        for (size_t i = 0; i + 1 < v.size(); i += 2) {
+            float ms = 0.f;
+            if (cudaEventElapsedTime(&ms, v[i], v[i + 1]) == cudaSuccess) { ms4[c] += ms; counts4[c] += 1; }
+            cudaEventDestroy(v[i]); cudaEventDestroy(v[i + 1]);
         }
+        v.clear();
     }
     return MWW_OK;
 }
@@ -1040,32 +707,39 @@ int mww_timeline_read(mww_t *h, float *ms, int max_tiles, int *n_tiles) {
     return MWW_OK;
 }
 
+namespace {
+void model_info(const Model &m, mww_info *o) {
+    o->is_quantized = m.quantized();
+    o->input_feature_slices = m.G.stride;
+    o->input_scale = m.in_scale; o->input_zero_point = m.in_zp;
+    o->output_scale = m.out_scale; o->output_zero_point = m.out_zp;
+    o->state_bytes_per_stream = (int)(m.G.state_elems * m.elem_size());
+    o->pending_rows = m.n_pend;
+    o->macs_per_step = (int)m.G.macs_per_step;
+}
+}  // namespace
+
 int mww_get_info(const mww_t *h, mww_info *o) {
     if (!h || !o) return MWW_EINVAL;
     memset(o, 0, sizeof *o);
-    o->n_streams = h->n_streams; o->device = h->device; o->is_quantized = h->quantized;
-    o->input_feature_slices = h->stride; o->num_features = kNumChannels;
-    o->input_scale = h->in_scale; o->input_zero_point = h->in_zp;
-    o->output_scale = h->out_scale; o->output_zero_point = h->out_zp;
-    o->state_bytes_per_stream = (int)(h->state_elems * elem_size(h));
-    o->frontend_buffered = h->used; o->pending_rows = h->n_pend;
-    o->sm_count = h->sm_count; o->macs_per_step = (int)h->macs_per_step;
-    o->hop_samples = h->hop;
+    o->n_streams = h->n_streams; o->device = h->device; o->num_features = kNumChannels;
+    o->frontend_buffered = h->used; o->sm_count = h->sm_count; o->hop_samples = h->hop;
+    if (!h->models.empty()) {
+        model_info(h->models[0], o);
+    } else {                                 // a frontend-only handle reports okay_nabu's geometry, unquantised
+        const GenArch &G = okay_nabu_arch();
+        o->input_feature_slices = G.stride;
+        o->state_bytes_per_stream = G.state_elems * 4;
+        o->macs_per_step = (int)G.macs_per_step;
+    }
     return MWW_OK;
 }
 
 int mww_get_model_info(const mww_t *h, int k, mww_info *o) {
     if (!h || !o || k < 0 || k >= (int)h->models.size()) return MWW_EINVAL;
-    const mww_t *m = h->models[k];
     int rc = mww_get_info(h, o);             // the shared frontend's fields
     if (rc) return rc;
-    o->is_quantized = m->quantized;
-    o->input_feature_slices = m->stride;
-    o->input_scale = m->in_scale; o->input_zero_point = m->in_zp;
-    o->output_scale = m->out_scale; o->output_zero_point = m->out_zp;
-    o->state_bytes_per_stream = (int)(m->state_elems * elem_size(m));
-    o->pending_rows = m->n_pend;
-    o->macs_per_step = (int)m->macs_per_step;
+    model_info(h->models[k], o);
     return MWW_OK;
 }
 
@@ -1095,18 +769,18 @@ int fill_by_id(mww_t *h, void *base, size_t bytes_per_stream, const int32_t *d_i
 }
 
 // fresh rings for the listed streams of one model
-int reset_nn_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
+int reset_nn_by_id(mww_t *h, Model &m, const int32_t *d_ids, int n, cudaStream_t st) {
     int rc = MWW_OK;
-    if (h->quantized && h->generic) {
-        CU(h, launch_gen_fill_state_i8(h->G, h->GQ, static_cast<int8_t *>(h->d_nn_state), static_cast<int8_t *>(h->d_pend), n, d_ids, h->n_streams, st));
+    if (m.kind == ModelKind::kGenericI8) {
+        CU(h, launch_gen_fill_state_i8(m.G, m.GQ, m.state<int8_t>(0), m.pend<int8_t>(0), n, d_ids, h->n_streams, st));
         h->launches += 1;
-    } else if (h->quantized) {
-        CU(h, launch_fill_state_i8(h->Wq, static_cast<int8_t *>(h->d_nn_state), static_cast<int8_t *>(h->d_pend), d_ids, n, h->n_streams, st));
+    } else if (m.kind == ModelKind::kCompiledI8) {
+        CU(h, launch_fill_state_i8(m.Wq, m.state<int8_t>(0), m.pend<int8_t>(0), d_ids, n, h->n_streams, st));
         h->launches += 1;
     } else {
         // zero rings are rotation-invariant, so streams of a handle whose rings are rotated (live mode) can be reset in place
-        rc = fill_by_id(h, h->d_nn_state, (size_t)h->state_elems * 4, d_ids, n, st);
-        if (rc == MWW_OK) rc = fill_by_id(h, h->d_pend, (size_t)h->pend_cap * kNumChannels * 4, d_ids, n, st);
+        rc = fill_by_id(h, m.d_nn_state, (size_t)m.G.state_elems * 4, d_ids, n, st);
+        if (rc == MWW_OK) rc = fill_by_id(h, m.d_pend, (size_t)m.G.pend_cap * kNumChannels * 4, d_ids, n, st);
     }
     return rc;
 }
@@ -1116,7 +790,7 @@ int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
     if (n <= 0) return MWW_OK;
     int rc = fill_by_id(h, h->d_carry, kWindow * sizeof(int16_t), d_ids, n, st);
     if (rc == MWW_OK) rc = fill_by_id(h, h->d_estimate, kNumChannels * sizeof(uint32_t), d_ids, n, st);
-    for (size_t k = 0; rc == MWW_OK && k < h->models.size(); ++k) rc = model_rc(h, h->models[k], reset_nn_by_id(h->models[k], d_ids, n, st));
+    for (size_t k = 0; rc == MWW_OK && k < h->models.size(); ++k) rc = reset_nn_by_id(h, h->models[k], d_ids, n, st);
     return rc;
 }
 
@@ -1165,12 +839,7 @@ int mww_set_window_step(mww_t *h, int hop_samples) {
 int mww_reset_frontend(mww_t *h, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     ENTER_STATEFUL(h);
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    const size_t S = (size_t)h->n_streams;
-    CU(h, cudaMemsetAsync(h->d_carry, 0, S * kWindow * sizeof(int16_t), st));
-    CU(h, cudaMemsetAsync(h->d_estimate, 0, S * kNumChannels * sizeof(uint32_t), st));
-    h->used = 0;
-    return MWW_OK;
+    return zero_frontend(h, static_cast<cudaStream_t>(cu_stream));
 }
 
 int mww_features(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
@@ -1207,17 +876,18 @@ int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, l
     if (int rc = refuse_multi(h, "mww_infer_features", "mww_predict_clip_multi")) return rc;
     if (n_rows < 0 || (n_rows > 0 && !d_rows) || rows_stride < n_rows) return fail(h, MWW_EINVAL, "mww_infer_features: bad row arguments");
     if (row_type < 0 || row_type > 2) return fail(h, MWW_EINVAL, "mww_infer_features: unknown row_type");
-    if (!h->has_nn) return fail(h, MWW_EINVAL, "mww_infer_features: frontend-only handle (created without a model)");
+    if (h->models.empty()) return fail(h, MWW_EINVAL, "mww_infer_features: frontend-only handle (created without a model)");
     ENTER_STATEFUL(h);
-    const int n_steps = (h->n_pend + n_rows) / h->stride;
+    Model &m = h->models[0];
+    const int n_steps = (m.n_pend + n_rows) / m.G.stride;
     if (n_steps > max_probs || (n_steps > 0 && !d_probs)) return fail(h, MWW_EINVAL, "mww_infer_features: probability buffer too small");
-    int rc = begin_nn_call(h, n_rows, static_cast<cudaStream_t>(cu_stream));
+    int rc = begin_nn_call(h, m, n_rows, static_cast<cudaStream_t>(cu_stream));
     if (rc) return rc;
-    h->tc_rows_bounded = false;         // the caller's rows may hold any value, and the state will carry them
-    rc = run_nn_tile(h, 0, h->n_streams, d_rows, row_type, rows_stride, n_rows, d_probs, max_probs, static_cast<cudaStream_t>(cu_stream));
-    if (rc == MWW_OK) end_nn_call(h, n_rows);
+    m.tc_rows_bounded = false;          // the caller's rows may hold any value, and the state will carry them
+    rc = run_nn_tile(h, m, 0, h->n_streams, d_rows, row_type, rows_stride, n_rows, d_probs, max_probs, static_cast<cudaStream_t>(cu_stream));
+    if (rc == MWW_OK) end_nn_call(h, m, n_rows);
     if (rc) return rc;
-    h->n_pend = (h->n_pend + n_rows) % h->stride;
+    m.n_pend = (m.n_pend + n_rows) % m.G.stride;
     if (h_probs_out) *h_probs_out = n_steps;
     return MWW_OK;
 }
@@ -1392,7 +1062,7 @@ int predict_clip_host_impl(mww_t *h, const char *who, const T *h_audio, int n_sa
                            const int *max_probs, int *h_probs_out) {
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !h_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
-    if (!h->has_nn) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
+    if (h->models.empty()) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     ENTER_STATEFUL(h);
     // The call has no stream argument, so it cannot be ordered after one particular stream: it waits for everything the
     // device has been given so far (mww_reset / live calls queued on any stream touch the same per-stream state).
@@ -1405,7 +1075,7 @@ int predict_clip_remote_impl(mww_t *h, const char *who, const T *src_audio, int 
                              const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !src_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
-    if (!h->has_nn) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
+    if (h->models.empty()) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     bool local = n_samples == 0;
     if (!local) {
         DeviceGuard guard(h->device);
@@ -1577,24 +1247,43 @@ int mww_host_free(void *h_ptr) {
     return e == cudaSuccess ? MWW_OK : ipc_fail("mww_host_free", e);
 }
 
+namespace {
+// one model's NN state to / from the host; the exported ring layout is always the canonical oldest-first one
+int get_model_state(mww_t *h, Model &m, void *h_nn, void *h_pending) {
+    const size_t S = (size_t)h->n_streams;
+    if (h_nn) {
+        if (int rc = canonicalise_rings(h, m, nullptr)) return rc;
+        CU(h, cudaDeviceSynchronize());
+        CU(h, cudaMemcpy(h_nn, m.d_nn_state, S * m.G.state_elems * m.elem_size(), cudaMemcpyDeviceToHost));
+    }
+    if (h_pending) CU(h, cudaMemcpy(h_pending, m.d_pend, S * m.G.pend_cap * kNumChannels * m.elem_size(), cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+int set_model_state(mww_t *h, Model &m, const void *h_nn, const void *h_pending, int pending_rows) {
+    const size_t S = (size_t)h->n_streams;
+    note_state_set(h, m, h_nn, h_pending, pending_rows);
+    if (h_nn) {
+        CU(h, cudaMemcpy(m.d_nn_state, h_nn, S * m.G.state_elems * m.elem_size(), cudaMemcpyHostToDevice));
+        m.live_heads = LiveHeads{};
+    }
+    if (h_pending) CU(h, cudaMemcpy(m.d_pend, h_pending, S * m.G.pend_cap * kNumChannels * m.elem_size(), cudaMemcpyHostToDevice));
+    m.n_pend = pending_rows;
+    return MWW_OK;
+}
+}  // namespace
+
 int mww_get_state(mww_t *h, int16_t *h_carry, uint32_t *h_estimate, void *h_nn, void *h_pending) {
     if (!h) return MWW_EINVAL;
     if (h_nn || h_pending)
         if (int rc = refuse_multi(h, "mww_get_state", "mww_get_model_state for the NN state")) return rc;
     ENTER_STATEFUL(h);
     CU(h, cudaDeviceSynchronize());
-    if (h_nn) {                                    // the exported layout is always the canonical oldest-first one
-        const int rc = canonicalise_rings(h, nullptr);
-        if (rc) return rc;
-        CU(h, cudaDeviceSynchronize());
-    }
     const size_t S = (size_t)h->n_streams;
     if (h_carry) CU(h, cudaMemcpy(h_carry, h->d_carry, S * kWindow * 2, cudaMemcpyDeviceToHost));
     if (h_estimate) CU(h, cudaMemcpy(h_estimate, h->d_estimate, S * kNumChannels * 4, cudaMemcpyDeviceToHost));
-    if ((h_nn || h_pending) && !h->has_nn) return fail(h, MWW_EINVAL, "frontend-only handle has no NN state");
-    if (h_nn) CU(h, cudaMemcpy(h_nn, h->d_nn_state, S * h->state_elems * elem_size(h), cudaMemcpyDeviceToHost));
-    if (h_pending) CU(h, cudaMemcpy(h_pending, h->d_pend, S * h->pend_cap * kNumChannels * elem_size(h), cudaMemcpyDeviceToHost));
-    return MWW_OK;
+    if (!h_nn && !h_pending) return MWW_OK;
+    if (h->models.empty()) return fail(h, MWW_EINVAL, "frontend-only handle has no NN state");
+    return get_model_state(h, h->models[0], h_nn, h_pending);
 }
 
 int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const uint32_t *h_estimate, const void *h_nn,
@@ -1602,22 +1291,19 @@ int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const
     if (!h) return MWW_EINVAL;
     if (h_nn || h_pending || pending_rows != 0)
         if (int rc = refuse_multi(h, "mww_set_state", "mww_set_model_state for the NN state and pending rows")) return rc;
-    if (frontend_buffered < 0 || frontend_buffered >= kWindow || pending_rows < 0 || pending_rows > h->stride - 1)
+    const int stride = h->models.empty() ? okay_nabu_arch().stride : h->models[0].G.stride;
+    if (frontend_buffered < 0 || frontend_buffered >= kWindow || pending_rows < 0 || pending_rows > stride - 1)
         return fail(h, MWW_EINVAL, "mww_set_state: counters out of range");
     ENTER(h);
     CU(h, cudaDeviceSynchronize());
     const size_t S = (size_t)h->n_streams;
     if (h_carry) CU(h, cudaMemcpy(h->d_carry, h_carry, S * kWindow * 2, cudaMemcpyHostToDevice));
     if (h_estimate) CU(h, cudaMemcpy(h->d_estimate, h_estimate, S * kNumChannels * 4, cudaMemcpyHostToDevice));
-    if ((h_nn || h_pending) && !h->has_nn) return fail(h, MWW_EINVAL, "frontend-only handle has no NN state");
-    note_state_set(h, h_nn, h_pending, pending_rows);
-    if (h_nn) {
-        CU(h, cudaMemcpy(h->d_nn_state, h_nn, S * h->state_elems * elem_size(h), cudaMemcpyHostToDevice));
-        h->live_heads = LiveHeads{};
-    }
-    if (h_pending) CU(h, cudaMemcpy(h->d_pend, h_pending, S * h->pend_cap * kNumChannels * elem_size(h), cudaMemcpyHostToDevice));
+    if ((h_nn || h_pending) && h->models.empty()) return fail(h, MWW_EINVAL, "frontend-only handle has no NN state");
+    // several models: each keeps its own pending rows (mww_set_model_state)
+    if (h->models.size() == 1)
+        if (int rc = set_model_state(h, h->models[0], h_nn, h_pending, pending_rows)) return rc;
     h->used = frontend_buffered;
-    if (h->models.size() <= 1) h->n_pend = pending_rows;     // several models: each keeps its own (mww_set_model_state)
     return MWW_OK;
 }
 
@@ -1625,34 +1311,18 @@ int mww_get_model_state(mww_t *h, int k, void *h_nn, void *h_pending) {
     if (!h) return MWW_EINVAL;
     if (k < 0 || k >= (int)h->models.size()) return fail(h, MWW_EINVAL, "mww_get_model_state: model index out of range");
     ENTER_STATEFUL(h);
-    mww_t *m = h->models[k];
     CU(h, cudaDeviceSynchronize());
-    if (h_nn) {                                    // the exported layout is always the canonical oldest-first one
-        if (int rc = model_rc(h, m, canonicalise_rings(m, nullptr))) return rc;
-        CU(h, cudaDeviceSynchronize());
-    }
-    const size_t S = (size_t)h->n_streams;
-    if (h_nn) CU(h, cudaMemcpy(h_nn, m->d_nn_state, S * m->state_elems * elem_size(m), cudaMemcpyDeviceToHost));
-    if (h_pending) CU(h, cudaMemcpy(h_pending, m->d_pend, S * m->pend_cap * kNumChannels * elem_size(m), cudaMemcpyDeviceToHost));
-    return MWW_OK;
+    return get_model_state(h, h->models[k], h_nn, h_pending);
 }
 
 int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending, int pending_rows) {
     if (!h) return MWW_EINVAL;
     if (k < 0 || k >= (int)h->models.size()) return fail(h, MWW_EINVAL, "mww_set_model_state: model index out of range");
-    mww_t *m = h->models[k];
-    if (pending_rows < 0 || pending_rows > m->stride - 1) return fail(h, MWW_EINVAL, "mww_set_model_state: pending_rows out of range");
+    Model &m = h->models[k];
+    if (pending_rows < 0 || pending_rows > m.G.stride - 1) return fail(h, MWW_EINVAL, "mww_set_model_state: pending_rows out of range");
     ENTER(h);
     CU(h, cudaDeviceSynchronize());
-    const size_t S = (size_t)h->n_streams;
-    note_state_set(m, h_nn, h_pending, pending_rows);
-    if (h_nn) {
-        CU(h, cudaMemcpy(m->d_nn_state, h_nn, S * m->state_elems * elem_size(m), cudaMemcpyHostToDevice));
-        m->live_heads = LiveHeads{};
-    }
-    if (h_pending) CU(h, cudaMemcpy(m->d_pend, h_pending, S * m->pend_cap * kNumChannels * elem_size(m), cudaMemcpyHostToDevice));
-    m->n_pend = pending_rows;
-    return MWW_OK;
+    return set_model_state(h, m, h_nn, h_pending, pending_rows);
 }
 
 int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src_c, const int32_t *h_src_ids, int n, void *cu_stream) {
@@ -1663,23 +1333,24 @@ int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src_c, 
     mww_t *src = const_cast<mww_t *>(src_c);
     if (!src || n < 0 || (n > 0 && (!h_dst_ids || !h_src_ids))) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: bad arguments");
     if (src->device != dst->device) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: the handles are on different devices");
-    if (!src->has_nn || !dst->has_nn) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: frontend-only handle has no NN state");
-    if (src->model_hash != dst->model_hash || src->quantized != dst->quantized || src->state_elems != dst->state_elems)
+    if (src->models.empty() || dst->models.empty()) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: frontend-only handle has no NN state");
+    Model &ms = src->models[0], &md = dst->models[0];
+    if (ms.model_hash != md.model_hash || ms.quantized() != md.quantized() || ms.G.state_elems != md.G.state_elems)
         return fail(dst, MWW_EINVAL, "mww_copy_nn_state: the handles were created from different models");
-    if (src->n_pend != 0 || dst->n_pend != 0) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: a handle holds pending rows");
+    if (ms.n_pend != 0 || md.n_pend != 0) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: a handle holds pending rows");
     for (int i = 0; i < n; ++i)
         if (h_dst_ids[i] < 0 || h_dst_ids[i] >= dst->n_streams || h_src_ids[i] < 0 || h_src_ids[i] >= src->n_streams)
             return fail(dst, MWW_EINVAL, "mww_copy_nn_state: stream id out of range");
     ENTER_STATEFUL(dst);
     if (src->poisoned) return fail(dst, MWW_ECUDA, "mww_copy_nn_state: the source handle needs mww_reset(h, NULL, 0, stream)");
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    int rc = canonicalise_rings(src, st);
+    int rc = canonicalise_rings(src, ms, st);
     if (rc) return fail(dst, rc, "mww_copy_nn_state: " + src->err);
-    if (dst != src && (rc = canonicalise_rings(dst, st)) != MWW_OK) return rc;
-    dst->tc_rows_bounded = dst->tc_rows_bounded && src->tc_rows_bounded;
-    const size_t bytes = (size_t)dst->state_elems * elem_size(dst);
-    char *d = static_cast<char *>(dst->d_nn_state);
-    const char *s = static_cast<const char *>(src->d_nn_state);
+    if (dst != src && (rc = canonicalise_rings(dst, md, st)) != MWW_OK) return rc;
+    md.tc_rows_bounded = md.tc_rows_bounded && ms.tc_rows_bounded;
+    const size_t bytes = (size_t)md.G.state_elems * md.elem_size();
+    char *d = static_cast<char *>(md.d_nn_state);
+    const char *s = static_cast<const char *>(ms.d_nn_state);
     for (int i = 0; i < n; ++i) {
         if (dst == src && h_dst_ids[i] == h_src_ids[i]) continue;     // same bytes: nothing to copy (and memcpy needs disjoint ranges)
         CU(dst, cudaMemcpyAsync(d + (size_t)h_dst_ids[i] * bytes, s + (size_t)h_src_ids[i] * bytes, bytes, cudaMemcpyDeviceToDevice, st));

@@ -11,7 +11,7 @@
 //     output goes to shared memory in the layout the tensor core reads: K cut into slots of 32 values = 128 bytes, a slot =
 //     [128 steps][128 B] with the hardware's 128-byte XOR swizzle, so a warp whose lanes are 32 consecutive channels of one step
 //     stores 128 contiguous bytes (no bank conflicts);
-//   * the weights are split and laid out the same way once, at mww_create (build_tc_weights), and arrive by bulk copies from L2
+//   * the weights are split and laid out the same way once, at mww_create (mww_container.cc), and arrive by bulk copies from L2
 //     completing on mbarriers: the first conv's seven slots at once at the start of a chunk, each 1x1 slot two slots ahead;
 //   * both warpgroups issue wgmma.mma_async.m64nNk8.f32.tf32.tf32 with B (and the 1x1 projections' A) through shared-memory matrix
 //     descriptors: per K = 8 step the three 3xTF32 products lo*hi, hi*lo, hi*hi accumulate into the same fp32 register tile
@@ -29,7 +29,6 @@
 #include <cstring>
 
 #include <type_traits>
-#include <vector>
 
 #include "mww_kernels.h"
 #include "mww_nn_tc.h"
@@ -617,31 +616,6 @@ nn_f32_clip_tc_kernel(NnWeightsF32 W, TcWeights TW, float *__restrict__ state, f
         if (tid == 0) atomicAdd(&g_tc_phase_cycles[kTcPhases], 1ull);
 #endif
     }
-}
-
-// ---- host side -------------------------------------------------------------------------------------------------------
-
-// 3xTF32 split and slot layout of the [K][N] weight matrices (the container's layout: input-major): slots of 32 K-values,
-// each [N rows][128 B] swizzled, hi plane then lo plane; and, for a model that passed tc_f16_scales, the first conv's fp16 hi / lo
-// weights with 0.0390625 folded in
-void build_tc_weights(const float *w0 /* [200][32] */, const float *const pw[4] /* [cin][64] */, const TcF16Scales *f16,
-                      std::vector<unsigned char> *blob, size_t offsets[6]) {
-    blob->clear();
-    std::vector<unsigned char> part;
-    auto add = [&](size_t *off) {
-        while (blob->size() % 256) blob->push_back(0);
-        *off = blob->size();
-        blob->insert(blob->end(), part.begin(), part.end());
-    };
-    tc_layout(w0, 200, 32, &part);
-    add(&offsets[0]);
-    for (int i = 0; i < 4; ++i) {
-        tc_layout(pw[i], i == 0 ? 32 : 64, 64, &part);
-        add(&offsets[1 + i]);
-    }
-    if (!f16) return;
-    tc_layout_f16(w0, 200, 32, 0.0390625, f16->s_fc, &part);
-    add(&offsets[5]);
 }
 
 cudaError_t launch_nn_f32_tc(const NnWeightsF32 &W, const TcWeights &TW, bool f16, float *state, float *pend, int n_pend, const uint16_t *rows,

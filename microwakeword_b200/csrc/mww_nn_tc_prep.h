@@ -14,6 +14,17 @@
 
 namespace mww {
 
+// Device pointers to the 3xTF32-split weights in tensor-core slot layout (laid out by mww_container.cc): K cut into slots of 32 values, a slot =
+// hi plane [N rows][128 B, 128-byte swizzle] followed by the lo plane.  fc: first conv, K = 200 (7 slots), N = 32; pw[i]: 1x1 of block i.
+// fc16: the first conv's weights x 0.0390625 x 2^s_fc as fp16 hi / lo operands (tc_layout_f16): K = 200 cut into 4 slots of 64, a
+// slot = hi plane [32 rows][128 B] followed by the lo plane; its epilogue undoes the scale with the exact multiply fc_out = 2^-s_fc.
+struct TcWeights {
+    const unsigned char *fc;
+    const unsigned char *pw[4];
+    const unsigned char *fc16;
+    float fc_out;
+};
+
 // 128-byte-swizzled K-major slot (wgmma shared-memory matrix descriptor with SWIZZLE_128B, stride byte offset 1024): rows of 128
 // bytes = 32 fp32 along K; within each group of 8 rows the 16-byte chunk index is XORed with (row & 7).  Byte offset of element
 // (row, kk), kk in [0, 32).
