@@ -229,6 +229,44 @@ int mww_predict_clip_remote_multi_f32(mww_t *h, const float *src_audio, int n_sa
 int mww_get_model_state(mww_t *h, int k, void *h_nn, void *h_pending);
 int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending, int pending_rows);
 
+/* ---- each model on its own streams ------------------------------------------------------------------------------
+ * A server whose satellites each listen for their own wake word runs one frontend over all streams and each model only on
+ * the streams that asked for it.  Model k of a handle has a STREAM SET: a strictly increasing list of n_k stream ids in
+ * [0, n_streams), 0 <= n_k <= n_streams; the default (mww_create_multi, ids[k] == NULL) is all streams.
+ *   - model k's ring state, pending rows and probabilities cover its own streams only, in list order: row j of d_probs[k] /
+ *     h_probs[k] ([n_k][max_probs[k]]) belongs to stream ids_k[j].  The buffer of a model with n_k = 0 may be NULL.  The
+ *     state is allocated for the n_k members only.
+ *   - the frontend still runs once per stream tile over all n_streams streams, and the lockstep counters (buffered samples,
+ *     each model's pending rows and ring rotation) are those of a handle without stream sets: the step counts
+ *     h_probs_out[k] reports do not depend on n_k.
+ *   - bit identity: for every member stream, model k's probabilities and state row are bit-identical to those of the same
+ *     stream in a handle where model k covers all streams, given the same calls.
+ *   - a model whose members in a stream tile are consecutive stream ids (all streams, or one block) reads that tile's
+ *     feature rows in place, with the launches of a handle without stream sets; any other set costs one row-gather launch
+ *     per model per tile, into a buffer that counts against MWW_SCRATCH_MB.
+ *   - mww_set_model_streams replaces model k's set (h_ids == NULL: all streams), stream-ordered on cu_stream and allowed
+ *     wherever a stateful call is (rotated rings and pending rows included).  Streams in both sets keep their ring and
+ *     pending-row state exactly; streams that join get the model's fresh state (what mww_reset(ids) gives them: zero rings
+ *     for fp32 and hybrid, zero points for int8, zero pending rows); streams that leave lose it.  The frontend is not
+ *     touched.  The call returns once the old state is freed (it synchronises cu_stream).  Ids out of range, unsorted or
+ *     duplicate ids, n < 0 or a bad k: MWW_EINVAL before any device work, the handle unchanged.
+ *   - mww_reset(ids) / mww_reset_device_ids take GLOBAL stream ids: they reset those streams' frontend and, for each model,
+ *     the listed streams that are members of it (non-members are ignored for that model).
+ *   - mww_get_model_state / mww_set_model_state move [n_k][state elements] / [n_k][stride - 1][40], in list order.
+ *     mww_get_model_info reports n_streams = n_k; mww_get_info keeps the handle's n_streams.
+ *   - the one-model entry points (mww_predict_clip*, mww_infer_features, mww_copy_nn_state, mww_get_state / mww_set_state
+ *     with NN arrays) return MWW_EINVAL on any handle where a model's set is not all streams, K = 1 included: they move
+ *     [n_streams]-shaped NN buffers.  The _multi calls are the interface for stream sets. */
+/* K models over one frontend, model k only on streams ids[k][0 .. n_ids[k]) (strictly increasing; ids == NULL or
+ * ids[k] == NULL: all streams).  State is allocated per model for its own streams only: this is what keeps K models on a
+ * large handle within device memory. */
+int mww_create_multi_streams(const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams,
+                             const int32_t *const *ids, const int *n_ids, mww_t **out);
+/* Replace model k's stream set (h_ids == NULL: all streams); stream-ordered on cu_stream, rules above. */
+int mww_set_model_streams(mww_t *h, int k, const int32_t *h_ids, int n, void *cu_stream);
+/* Model k's stream ids; *n_out = n_k, at most max_ids written. */
+int mww_get_model_streams(const mww_t *h, int k, int32_t *h_ids, int max_ids, int *n_out);
+
 /* Per-stream state snapshot for checkpoint / tests (host buffers, synchronous).
  *   h_carry    int16 [n_streams][480]   window buffer (first `frontend_buffered` samples valid)
  *   h_estimate uint32 [n_streams][40]   noise estimates

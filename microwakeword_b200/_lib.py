@@ -27,6 +27,7 @@ EXPORTS = (
     "mww_create_multi", "mww_model_count", "mww_get_model_info", "mww_predict_clip_multi", "mww_predict_clip_multi_f32",
     "mww_predict_clip_host_multi", "mww_predict_clip_remote_multi", "mww_get_model_state", "mww_set_model_state",
     "mww_predict_clip_host_f32", "mww_predict_clip_host_multi_f32", "mww_predict_clip_remote_f32", "mww_predict_clip_remote_multi_f32",
+    "mww_create_multi_streams", "mww_set_model_streams", "mww_get_model_streams",
 )
 
 
@@ -154,6 +155,12 @@ def lib() -> ctypes.CDLL:
     L.mww_get_model_state.argtypes = [vp, i32, vp, vp]
     L.mww_set_model_state.restype = i32
     L.mww_set_model_state.argtypes = [vp, i32, vp, vp, i32]
+    L.mww_create_multi_streams.restype = i32
+    L.mww_create_multi_streams.argtypes = [vp, vp, i32, i32, i32, vp, vp, ctypes.POINTER(vp)]
+    L.mww_set_model_streams.restype = i32
+    L.mww_set_model_streams.argtypes = [vp, i32, vp, i32, vp]
+    L.mww_get_model_streams.restype = i32
+    L.mww_get_model_streams.argtypes = [vp, i32, vp, i32, pi]
     _lib = L
     return L
 

@@ -19,6 +19,7 @@
 #include "mww_container.h"
 #include "mww_kernels.h"
 #include "mww_nn_tc.h"
+#include "mww_streams.h"
 
 using namespace mww;
 
@@ -28,12 +29,21 @@ thread_local std::string g_create_error;
 
 constexpr int kMaxModels = 64;      // models one handle can carry (mww_create_multi)
 
+// the streams one model runs on (mww_create_multi_streams / mww_set_model_streams): strictly increasing global ids; the
+// model's state, pending rows and probabilities are indexed by position in this list (the compact index)
+struct Members {
+    std::vector<int32_t> ids;
+    int32_t *d_ids = nullptr;       // device copy of ids (the row gather reads it)
+    int32_t *d_inv = nullptr;       // [n_streams]: compact index of each global stream id, -1 for a non-member (reset by id)
+};
+
 // one NN model the frontend feeds: its weights (mww_container.h), per-stream ring state and pending rows
 struct Model : ModelWeights {
     uint64_t model_hash = 0;        // FNV-1a of the model container: mww_copy_nn_state only moves state between equal models
     void *d_weights = nullptr;      // the arena of ModelWeights
-    void *d_nn_state = nullptr;     // float or int8 [S][G.state_elems]   (4176 for okay_nabu)
-    void *d_pend = nullptr;         // float or int8 [S][G.pend_cap][40]  (2 rows for stride 3)
+    Members mem;
+    void *d_nn_state = nullptr;     // float or int8 [M][G.state_elems]   (4176 for okay_nabu; M = members)
+    void *d_pend = nullptr;         // float or int8 [M][G.pend_cap][40]  (2 rows for stride 3)
     int n_pend = 0;
     // live-step path: rings stay rotated between live calls (mww_nn_live.cuh); all streams advance in lockstep
     LiveHeads live_heads{};
@@ -43,7 +53,10 @@ struct Model : ModelWeights {
     bool tc_rows_bounded = true;
 
     size_t elem_size() const { return quantized() ? 1 : 4; }
-    // stream `first`'s ring state and pending rows
+    int members() const { return (int)mem.ids.size(); }
+    size_t state_bytes() const { return (size_t)G.state_elems * elem_size(); }                   // per stream
+    size_t pend_bytes() const { return (size_t)G.pend_cap * kNumChannels * elem_size(); }       // per stream
+    // compact index `first`'s ring state and pending rows
     template <typename T> T *state(int first) const { return static_cast<T *>(d_nn_state) + (size_t)first * G.state_elems; }
     template <typename T> T *pend(int first) const { return static_cast<T *>(d_pend) + (size_t)first * G.pend_cap * kNumChannels; }
 };
@@ -66,6 +79,8 @@ struct mww_handle {
     // scratch
     uint32_t *d_v = nullptr; size_t v_bytes = 0;
     uint16_t *d_feat = nullptr; size_t feat_bytes = 0;
+    uint16_t *d_gather = nullptr; size_t gather_bytes = 0;     // one tile's rows of one model whose members are not consecutive
+    int32_t *d_cids = nullptr; size_t cids_cap = 0;            // reset by id: the ids translated to one model's compact indices
     size_t scratch_budget = (size_t)2048 << 20;
     int min_tile_streams = 2048;       // staged path: a tile never gets fewer streams than this (MWW_MIN_TILE_STREAMS)
     // host-buffer pipeline
@@ -125,7 +140,13 @@ struct ProfScope {
     ~ProfScope() { if (stop) cudaEventRecord(stop, st); }
 };
 
-int ensure_scratch(mww_t *h, size_t v_bytes, size_t feat_bytes) {
+int ensure_scratch(mww_t *h, size_t v_bytes, size_t feat_bytes, size_t gather_bytes = 0) {
+    if (gather_bytes > h->gather_bytes) {
+        if (h->d_gather) cudaFree(h->d_gather);
+        h->d_gather = nullptr; h->gather_bytes = 0;
+        CU(h, cudaMalloc(&h->d_gather, gather_bytes));
+        h->gather_bytes = gather_bytes;
+    }
     if (v_bytes > h->v_bytes) {
         if (h->d_v) cudaFree(h->d_v);
         h->d_v = nullptr; h->v_bytes = 0;
@@ -164,6 +185,16 @@ int tile_streams(const mww_t *h, int n_frames, bool need_feat, size_t extra_per_
     if (t < 1) t = 1;
     if (t > (size_t)h->n_streams) t = (size_t)h->n_streams;
     return (int)t;
+}
+
+// Bytes per stream of the row-gather buffer a predict call needs: none while every model's members are consecutive stream
+// ids (all streams, or one block), so such handles keep the tiles and launches of a handle without stream sets.
+size_t gather_bytes_per_stream(const mww_t *h, int n_frames) {
+    for (const Model &m : h->models) {
+        const std::vector<int32_t> &ids = m.mem.ids;
+        if (!ids.empty() && ids.back() - ids.front() != (int)ids.size() - 1) return (size_t)std::max(n_frames, 1) * kNumChannels * 2;
+    }
+    return 0;
 }
 
 // frontend for streams [first, first+n): audio tile pointer is already offset to the tile's first stream.  T = int16_t or
@@ -229,9 +260,11 @@ int canonicalise_rings(mww_t *h, Model &m, cudaStream_t st) {
     bool any = false;
     for (int i = 0; i < 5; ++i) any = any || m.live_heads.h[i] != 0;
     if (!any) return MWW_OK;
-    if (m.quantized()) CU(h, launch_nn_i8_live_canonicalise(m.state<int8_t>(0), h->n_streams, m.live_heads, st));
-    else CU(h, launch_nn_live_canonicalise(m.state<float>(0), h->n_streams, m.live_heads, st));
-    h->launches += 1;
+    if (m.members() > 0) {
+        if (m.quantized()) CU(h, launch_nn_i8_live_canonicalise(m.state<int8_t>(0), m.members(), m.live_heads, st));
+        else CU(h, launch_nn_live_canonicalise(m.state<float>(0), m.members(), m.live_heads, st));
+        h->launches += 1;
+    }
     m.live_heads = LiveHeads{};
     return MWW_OK;
 }
@@ -324,8 +357,36 @@ int upload_tables(mww_t *h) {
     return MWW_OK;
 }
 
-// weights and per-stream NN state of one model container
-int load_model(mww_t *h, Model &m, const void *model_blob, size_t n_bytes) {
+// A stream set's host list and device copies, and NN state for its members (state stays uninitialised): what a model needs
+// for a given membership.  ids == nullptr: all streams.  On failure everything it allocated is freed again.
+struct MemberState {
+    Members mem;
+    void *d_nn_state = nullptr, *d_pend = nullptr;
+    void release() { cudaFree(mem.d_ids); cudaFree(mem.d_inv); cudaFree(d_nn_state); cudaFree(d_pend); *this = MemberState{}; }
+};
+int alloc_members(mww_t *h, const Model &m, const int32_t *ids, int n, MemberState *out) {
+    MemberState r;
+    if (ids) r.mem.ids.assign(ids, ids + n);
+    else for (int s = 0; s < h->n_streams; ++s) r.mem.ids.push_back(s);
+    const size_t M = r.mem.ids.size(), S = (size_t)h->n_streams;
+    std::vector<int32_t> inv(S, -1);
+    for (size_t j = 0; j < M; ++j) inv[(size_t)r.mem.ids[j]] = (int32_t)j;
+    cudaError_t a = cudaMalloc(&r.mem.d_inv, S * sizeof(int32_t));
+    if (a == cudaSuccess && M > 0) a = cudaMalloc(&r.mem.d_ids, M * sizeof(int32_t));
+    if (a == cudaSuccess && M > 0) a = cudaMalloc(&r.d_nn_state, M * m.state_bytes());
+    if (a == cudaSuccess && M > 0) a = cudaMalloc(&r.d_pend, M * m.pend_bytes());
+    if (a == cudaSuccess) a = cudaMemcpy(r.mem.d_inv, inv.data(), S * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (a == cudaSuccess && M > 0) a = cudaMemcpy(r.mem.d_ids, r.mem.ids.data(), M * sizeof(int32_t), cudaMemcpyHostToDevice);
+    if (a != cudaSuccess) {
+        r.release();
+        return fail(h, a == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("state allocation: ") + cudaGetErrorString(a));
+    }
+    *out = std::move(r);
+    return MWW_OK;
+}
+
+// weights and per-stream NN state of one model container, for its members (ids == nullptr: all streams)
+int load_model(mww_t *h, Model &m, const void *model_blob, size_t n_bytes, const int32_t *ids, int n_ids) {
     uint64_t x = 1469598103934665603ull;
     for (size_t i = 0; i < n_bytes; ++i) x = (x ^ static_cast<const uint8_t *>(model_blob)[i]) * 1099511628211ull;
     m.model_hash = x;
@@ -334,11 +395,19 @@ int load_model(mww_t *h, Model &m, const void *model_blob, size_t n_bytes) {
     CU(h, cudaMalloc(&m.d_weights, m.arena.size()));
     if (cudaError_t e = cudaMemcpy(m.d_weights, m.arena.data(), m.arena.size(), cudaMemcpyHostToDevice)) return cuda_fail(h, e, "weight upload");
     m.rebase(m.d_weights);
-    const size_t S = (size_t)h->n_streams;
-    cudaError_t a = cudaMalloc(&m.d_nn_state, S * m.G.state_elems * m.elem_size());
-    if (a == cudaSuccess) a = cudaMalloc(&m.d_pend, S * m.G.pend_cap * kNumChannels * m.elem_size());
-    if (a != cudaSuccess) return fail(h, a == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("state allocation: ") + cudaGetErrorString(a));
+    MemberState ms;
+    if (int rc = alloc_members(h, m, ids, n_ids, &ms)) return rc;
+    m.mem = std::move(ms.mem);
+    m.d_nn_state = ms.d_nn_state;
+    m.d_pend = ms.d_pend;
     return MWW_OK;
+}
+
+// every model runs on all streams: what the one-model entry points, which move [n_streams]-shaped NN buffers, require
+bool all_streams(const mww_t *h) {
+    for (const Model &m : h->models)
+        if (m.members() != h->n_streams) return false;
+    return true;
 }
 
 // A state set from outside keeps the fp16 first conv only if every first-conv ring row (state floats [0, 80) of a stream) it
@@ -354,7 +423,7 @@ bool rows_are_features(const float *v, size_t n) {
 void note_state_set(mww_t *h, Model &m, const void *h_nn, const void *h_pending, int pending_rows) {
     if (!h_nn && !h_pending) return;
     bool ok = m.tc_f16 && (h_nn || m.tc_rows_bounded) && (h_pending || m.tc_rows_bounded);
-    for (int s = 0; ok && s < h->n_streams; ++s) {
+    for (int s = 0; ok && s < m.members(); ++s) {
         if (h_nn) ok = rows_are_features(static_cast<const float *>(h_nn) + (size_t)s * m.G.state_elems, 2 * kNumChannels);
         if (ok && h_pending)
             ok = rows_are_features(static_cast<const float *>(h_pending) + (size_t)s * m.G.pend_cap * kNumChannels, (size_t)pending_rows * kNumChannels);
@@ -364,17 +433,19 @@ void note_state_set(mww_t *h, Model &m, const void *h_nn, const void *h_pending,
 
 // fresh rings and no pending rows for every stream of one model
 int zero_nn_state(mww_t *h, Model &m, cudaStream_t st) {
-    const size_t S = (size_t)h->n_streams;
+    const int M = m.members();
     m.n_pend = 0;
-    if (m.kind == ModelKind::kGenericI8) {
-        CU(h, launch_gen_fill_state_i8(m.G, m.GQ, m.state<int8_t>(0), m.pend<int8_t>(0), h->n_streams, nullptr, h->n_streams, st));
+    if (M == 0) {
+        // a model without members holds no state
+    } else if (m.kind == ModelKind::kGenericI8) {
+        CU(h, launch_gen_fill_state_i8(m.G, m.GQ, m.state<int8_t>(0), m.pend<int8_t>(0), M, nullptr, M, st));
         h->launches += 1;
     } else if (m.kind == ModelKind::kCompiledI8) {
-        CU(h, launch_fill_state_i8(m.Wq, m.state<int8_t>(0), m.pend<int8_t>(0), nullptr, h->n_streams, h->n_streams, st));
+        CU(h, launch_fill_state_i8(m.Wq, m.state<int8_t>(0), m.pend<int8_t>(0), nullptr, M, M, st));
         h->launches += 1;
     } else {
-        CU(h, cudaMemsetAsync(m.d_nn_state, 0, S * m.G.state_elems * 4, st));
-        CU(h, cudaMemsetAsync(m.d_pend, 0, S * m.G.pend_cap * kNumChannels * 4, st));
+        CU(h, cudaMemsetAsync(m.d_nn_state, 0, (size_t)M * m.state_bytes(), st));
+        CU(h, cudaMemsetAsync(m.d_pend, 0, (size_t)M * m.pend_bytes(), st));
     }
     m.live_heads = LiveHeads{};
     m.tc_rows_bounded = true;
@@ -399,9 +470,13 @@ int zero_state(mww_t *h, cudaStream_t st) {
 void destroy_impl(mww_t *h) {
     if (!h) return;
     DeviceGuard guard(h->device);
-    for (Model &m : h->models) { cudaFree(m.d_weights); cudaFree(m.d_nn_state); cudaFree(m.d_pend); }
+    for (Model &m : h->models) {
+        cudaFree(m.d_weights); cudaFree(m.d_nn_state); cudaFree(m.d_pend);
+        cudaFree(m.mem.d_ids); cudaFree(m.mem.d_inv);
+    }
     cudaFree(h->d_tables); cudaFree(h->d_carry); cudaFree(h->d_estimate);
     cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
+    cudaFree(h->d_gather); cudaFree(h->d_cids);
     for (int b = 0; b < 2; ++b) {
         cudaFree(h->d_audio_tile[b]); cudaFree(h->d_probs_tile[b]);
         if (h->ev_h2d[b]) cudaEventDestroy(h->ev_h2d[b]);
@@ -446,9 +521,9 @@ int features_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, lo
     return MWW_OK;
 }
 
-// Per-model arguments of a predict call: model k writes its probabilities to probs[k] ([n_streams][max_probs[k]]) and runs
+// Per-model arguments of a predict call: model k writes its probabilities to probs[k] ([members][max_probs[k]]) and runs
 // steps[k] model steps (its own stride and pending rows decide how many).  Checked for every model before anything is
-// launched, so a too-small buffer for one model leaves the whole handle untouched.
+// launched, so a too-small buffer for one model leaves the whole handle untouched; a model without members needs none.
 struct NnOuts {
     float *const *probs; const int *max_probs; int steps[kMaxModels];
 };
@@ -458,7 +533,7 @@ int check_outs(mww_t *h, const char *who, int n_frames, float *const *probs, con
     for (size_t k = 0; k < h->models.size(); ++k) {
         const Model &m = h->models[k];
         o->steps[k] = (m.n_pend + n_frames) / m.G.stride;
-        if (o->steps[k] > max_probs[k] || (o->steps[k] > 0 && !probs[k]))
+        if (m.members() > 0 && (o->steps[k] > max_probs[k] || (o->steps[k] > 0 && !probs[k])))
             return fail(h, MWW_EINVAL, std::string(who) + ": probability buffer too small" +
                                            (h->models.size() > 1 ? " for model " + std::to_string(k) : std::string()));
     }
@@ -479,10 +554,33 @@ int begin_models_call(mww_t *h, int n_frames, cudaStream_t st) {
         if (int rc = begin_nn_call(h, m, n_frames, st)) return rc;
     return MWW_OK;
 }
-// every model on one tile of frontend rows; probs[k] (pitch probs_stride[k]) points at the tile's first stream
-int run_models_tile(mww_t *h, int first, int n, int n_frames, float *const *probs, const long long *probs_stride, cudaStream_t st) {
-    for (size_t k = 0; k < h->models.size(); ++k)
-        if (int rc = run_nn_tile(h, h->models[k], first, n, h->d_feat, MWW_ROWS_U16, n_frames, n_frames, probs[k], probs_stride[k], st)) return rc;
+// model k's members in the stream tile [first, first + n): compact indices [a, b), consecutive stream ids or not
+struct TileSpan { int a = 0, b = 0; bool consecutive = true; };
+void tile_spans(const mww_t *h, int first, int n, TileSpan *span) {
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        const Members &mem = h->models[k].mem;
+        span[k].consecutive = tile_members(mem.ids.data(), (int)mem.ids.size(), first, n, &span[k].a, &span[k].b);
+    }
+}
+
+// every model on one tile of frontend rows (h->d_feat, from stream `first`); probs[k] (pitch probs_stride[k]) points at the
+// row of model k's first member in the tile, compact index span[k].a.  A model whose members are consecutive reads the rows
+// in place -- for all streams this is exactly the one launch per model of a handle without stream sets -- any other is
+// run on a gathered copy of its members' rows.  The models share one gather buffer: they run in order on one stream.
+int run_models_tile(mww_t *h, int first, int n_frames, const TileSpan *span, float *const *probs, const long long *probs_stride, cudaStream_t st) {
+    const long long rows_stride = (long long)n_frames * kNumChannels;
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        Model &m = h->models[k];
+        const TileSpan &s = span[k];
+        if (s.b == s.a) continue;
+        const uint16_t *rows = h->d_feat + (size_t)(m.mem.ids[s.a] - first) * rows_stride;
+        if (!s.consecutive && n_frames > 0) {
+            CU(h, launch_gather_rows(h->d_feat, m.mem.d_ids, s.a, first, s.b - s.a, n_frames, h->d_gather, h->sm_count, st));
+            h->launches += 1;
+            rows = h->d_gather;
+        }
+        if (int rc = run_nn_tile(h, m, s.a, s.b - s.a, rows, MWW_ROWS_U16, n_frames, n_frames, probs[k], probs_stride[k], st)) return rc;
+    }
     return MWW_OK;
 }
 
@@ -499,22 +597,25 @@ int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples
     NnOuts o;
     int rc = check_outs(h, who, n_frames, d_probs, max_probs, &o);
     if (rc) return rc;
-    const int tile = tile_streams(h, n_frames, true);
-    rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
+    const size_t gather = gather_bytes_per_stream(h, n_frames);
+    const int tile = tile_streams(h, n_frames, true, gather);
+    rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2, (size_t)tile * gather);
     if (rc) return rc;
     rc = begin_models_call(h, n_frames, st);
     if (rc) return rc;
     const size_t K = h->models.size();
     float *tile_probs[kMaxModels];
     long long probs_stride[kMaxModels];
+    TileSpan span[kMaxModels];
     for (size_t k = 0; k < K; ++k) probs_stride[k] = max_probs[k];
     for (int first = 0; first < h->n_streams; first += tile) {
         const int n = std::min(tile, h->n_streams - first);
         rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames, h->d_feat,
                                (long long)n_frames * kNumChannels, st);
         if (rc) return rc;
-        for (size_t k = 0; k < K; ++k) tile_probs[k] = d_probs[k] + (size_t)first * max_probs[k];
-        rc = run_models_tile(h, first, n, n_frames, tile_probs, probs_stride, st);
+        tile_spans(h, first, n, span);
+        for (size_t k = 0; k < K; ++k) tile_probs[k] = d_probs[k] + (size_t)span[k].a * max_probs[k];
+        rc = run_models_tile(h, first, n_frames, span, tile_probs, probs_stride, st);
         if (rc) return rc;
     }
     end_models_call(h, n_frames, o, h_probs_out);
@@ -527,10 +628,13 @@ int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples
 }
 
 // the one-model entry points refuse a handle that carries several models: advancing the shared frontend for one model
-// would leave the others' rows behind
+// would leave the others' rows behind.  They also refuse a model on a subset of the streams: their NN buffers are
+// [n_streams]-shaped.
 int refuse_multi(mww_t *h, const char *who, const char *instead) {
     if (h && h->models.size() > 1)
         return fail(h, MWW_EINVAL, std::string(who) + ": the handle carries " + std::to_string(h->models.size()) + " models; use " + instead);
+    if (h && !all_streams(h))
+        return fail(h, MWW_EINVAL, std::string(who) + ": the model runs on a subset of the streams; use " + instead);
     return MWW_OK;
 }
 
@@ -555,7 +659,9 @@ mww_t *new_handle(int device, int n_streams) {
 }
 
 // mww_create (n_models 0: frontend-only, 1: one model) and mww_create_multi (`multi`: messages name the failing model's index)
-int create_impl(const char *who, const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams, mww_t **out, bool multi) {
+// ids / n_ids (may be NULL; ids[k] == NULL: all streams): each model's stream set, already validated
+int create_impl(const char *who, const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams, mww_t **out, bool multi,
+                const int32_t *const *ids = nullptr, const int *n_ids = nullptr) {
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
     if (e != cudaSuccess || count == 0)
@@ -567,7 +673,8 @@ int create_impl(const char *who, const void *const *blobs, const size_t *n_bytes
     int rc = upload_tables(h);
     for (int k = 0; rc == MWW_OK && k < n_models; ++k) {
         h->models.emplace_back();
-        rc = load_model(h, h->models.back(), blobs[k], n_bytes[k]);
+        const bool subset = ids && ids[k];
+        rc = load_model(h, h->models.back(), blobs[k], n_bytes[k], subset ? ids[k] : nullptr, subset ? n_ids[k] : 0);
         if (rc != MWW_OK && multi) h->err = "model " + std::to_string(k) + ": " + h->err;
     }
     if (rc == MWW_OK) {
@@ -599,6 +706,21 @@ int mww_create_multi(const void *const *blobs, const size_t *n_bytes, int n_mode
     for (int k = 0; k < n_models; ++k)
         if (!blobs[k]) return fail(nullptr, MWW_EINVAL, "mww_create_multi: model " + std::to_string(k) + " is NULL");
     return create_impl("mww_create_multi", blobs, n_bytes, n_models, device, n_streams, out, true);
+}
+
+int mww_create_multi_streams(const void *const *blobs, const size_t *n_bytes, int n_models, int device, int n_streams,
+                             const int32_t *const *ids, const int *n_ids, mww_t **out) {
+    if (out) *out = nullptr;
+    if (!out || n_streams < 1 || !blobs || !n_bytes) return fail(nullptr, MWW_EINVAL, "mww_create_multi_streams: bad arguments");
+    if (n_models < 1 || n_models > kMaxModels)
+        return fail(nullptr, MWW_EINVAL, "mww_create_multi_streams: n_models must be in [1, " + std::to_string(kMaxModels) + "]");
+    for (int k = 0; k < n_models; ++k) {
+        if (!blobs[k]) return fail(nullptr, MWW_EINVAL, "mww_create_multi_streams: model " + std::to_string(k) + " is NULL");
+        if (ids && ids[k] && (!n_ids || n_ids[k] < 0 || n_ids[k] > n_streams || !valid_stream_set(ids[k], n_ids[k], n_streams)))
+            return fail(nullptr, MWW_EINVAL, "mww_create_multi_streams: model " + std::to_string(k) +
+                                                 ": stream ids must be strictly increasing and in [0, n_streams)");
+    }
+    return create_impl("mww_create_multi_streams", blobs, n_bytes, n_models, device, n_streams, out, true, ids, n_ids);
 }
 
 int mww_model_count(const mww_t *h) { return h ? (int)h->models.size() : 0; }
@@ -740,6 +862,7 @@ int mww_get_model_info(const mww_t *h, int k, mww_info *o) {
     int rc = mww_get_info(h, o);             // the shared frontend's fields
     if (rc) return rc;
     model_info(h->models[k], o);
+    o->n_streams = h->models[k].members();
     return MWW_OK;
 }
 
@@ -757,40 +880,60 @@ __global__ void fill_by_id_kernel(uint32_t *__restrict__ base, long long words_p
     }
 }
 
-int fill_by_id(mww_t *h, void *base, size_t bytes_per_stream, const int32_t *d_ids, int n, cudaStream_t st) {
+// records [0, bound) of `base`; ids outside that range are skipped
+int fill_by_id(mww_t *h, void *base, size_t bytes_per_stream, const int32_t *d_ids, int n, int bound, cudaStream_t st) {
     const long long words = (long long)(bytes_per_stream / 4);
     const long long total = words * n;
     if (total <= 0) return MWW_OK;
     const unsigned blocks = (unsigned)std::min<long long>((total + 255) / 256, (long long)h->sm_count * 16);
-    fill_by_id_kernel<<<blocks, 256, 0, st>>>(static_cast<uint32_t *>(base), words, 0u, d_ids, n, h->n_streams);
+    fill_by_id_kernel<<<blocks, 256, 0, st>>>(static_cast<uint32_t *>(base), words, 0u, d_ids, n, bound);
     CU(h, cudaGetLastError());
     h->launches += 1;
     return MWW_OK;
 }
 
-// fresh rings for the listed streams of one model
-int reset_nn_by_id(mww_t *h, Model &m, const int32_t *d_ids, int n, cudaStream_t st) {
+// fresh rings and pending rows for the listed compact indices of state / pend holding `bound` streams of model m's layout;
+// indices outside [0, bound) are skipped
+int reset_nn_by_id(mww_t *h, const Model &m, void *state, void *pend, const int32_t *d_ids, int n, int bound, cudaStream_t st) {
     int rc = MWW_OK;
     if (m.kind == ModelKind::kGenericI8) {
-        CU(h, launch_gen_fill_state_i8(m.G, m.GQ, m.state<int8_t>(0), m.pend<int8_t>(0), n, d_ids, h->n_streams, st));
+        CU(h, launch_gen_fill_state_i8(m.G, m.GQ, static_cast<int8_t *>(state), static_cast<int8_t *>(pend), n, d_ids, bound, st));
         h->launches += 1;
     } else if (m.kind == ModelKind::kCompiledI8) {
-        CU(h, launch_fill_state_i8(m.Wq, m.state<int8_t>(0), m.pend<int8_t>(0), d_ids, n, h->n_streams, st));
+        CU(h, launch_fill_state_i8(m.Wq, static_cast<int8_t *>(state), static_cast<int8_t *>(pend), d_ids, n, bound, st));
         h->launches += 1;
     } else {
         // zero rings are rotation-invariant, so streams of a handle whose rings are rotated (live mode) can be reset in place
-        rc = fill_by_id(h, m.d_nn_state, (size_t)m.G.state_elems * 4, d_ids, n, st);
-        if (rc == MWW_OK) rc = fill_by_id(h, m.d_pend, (size_t)m.G.pend_cap * kNumChannels * 4, d_ids, n, st);
+        rc = fill_by_id(h, state, m.state_bytes(), d_ids, n, bound, st);
+        if (rc == MWW_OK) rc = fill_by_id(h, pend, m.pend_bytes(), d_ids, n, bound, st);
     }
     return rc;
 }
 
-// fresh state for the listed streams: a handful of launches whatever the length of the list
+// fresh state for the listed global stream ids: a handful of launches whatever the length of the list.  A model on all
+// streams takes the ids as they are; any other first has them translated to its compact indices (-1 for a non-member,
+// which the fill kernels skip).
 int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
     if (n <= 0) return MWW_OK;
-    int rc = fill_by_id(h, h->d_carry, kWindow * sizeof(int16_t), d_ids, n, st);
-    if (rc == MWW_OK) rc = fill_by_id(h, h->d_estimate, kNumChannels * sizeof(uint32_t), d_ids, n, st);
-    for (size_t k = 0; rc == MWW_OK && k < h->models.size(); ++k) rc = reset_nn_by_id(h, h->models[k], d_ids, n, st);
+    int rc = fill_by_id(h, h->d_carry, kWindow * sizeof(int16_t), d_ids, n, h->n_streams, st);
+    if (rc == MWW_OK) rc = fill_by_id(h, h->d_estimate, kNumChannels * sizeof(uint32_t), d_ids, n, h->n_streams, st);
+    for (size_t k = 0; rc == MWW_OK && k < h->models.size(); ++k) {
+        Model &m = h->models[k];
+        if (m.members() == h->n_streams) {
+            rc = reset_nn_by_id(h, m, m.d_nn_state, m.d_pend, d_ids, n, h->n_streams, st);
+            continue;
+        }
+        if (m.members() == 0) continue;
+        if ((size_t)n > h->cids_cap) {
+            if (h->d_cids) { CU(h, cudaStreamSynchronize(st)); cudaFree(h->d_cids); h->d_cids = nullptr; h->cids_cap = 0; }
+            const size_t cap = std::max<size_t>((size_t)n, 1024);
+            CU(h, cudaMalloc(&h->d_cids, cap * sizeof(int32_t)));
+            h->cids_cap = cap;
+        }
+        CU(h, launch_compact_ids(h->d_cids, d_ids, n, m.mem.d_inv, h->n_streams, h->sm_count, st));
+        h->launches += 1;
+        rc = reset_nn_by_id(h, m, m.d_nn_state, m.d_pend, h->d_cids, n, m.members(), st);
+    }
     return rc;
 }
 
@@ -935,6 +1078,7 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
     const T *audio_tile[2] = {static_cast<const T *>(h->d_audio_tile[0]), static_cast<const T *>(h->d_audio_tile[1])};
     float *tile_probs[kMaxModels];
     long long tile_probs_stride[kMaxModels];
+    TileSpan span[kMaxModels];
     for (size_t k = 0; k < K; ++k) tile_probs_stride[k] = dst_is_host ? std::max(o.steps[k], 1) : o.max_probs[k];
     int it = 0;
     for (int first = 0; first < h->n_streams; first += tile, ++it) {
@@ -963,9 +1107,10 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
         if (dst_is_host && it >= 2) CU(h, cudaStreamWaitEvent(h->st_compute, h->ev_d2h[b], 0));   // score staging buffer drained
         int rc = run_frontend_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
         if (rc) return rc;
+        tile_spans(h, first, n, span);
         for (size_t k = 0; k < K; ++k)
-            tile_probs[k] = dst_is_host ? h->d_probs_tile[b] + probs_tile_offset(h, o, tile, k) : o.probs[k] + (size_t)first * o.max_probs[k];
-        rc = run_models_tile(h, first, n, n_frames, tile_probs, tile_probs_stride, h->st_compute);
+            tile_probs[k] = dst_is_host ? h->d_probs_tile[b] + probs_tile_offset(h, o, tile, k) : o.probs[k] + (size_t)span[k].a * o.max_probs[k];
+        rc = run_models_tile(h, first, n_frames, span, tile_probs, tile_probs_stride, h->st_compute);
         if (rc) return rc;
         if (n_samples > 0) {
             rc = run_carry_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->st_compute);
@@ -976,9 +1121,10 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
         if (dst_is_host) {
             CU(h, cudaStreamWaitEvent(h->st_d2h, h->ev_compute[b], 0));
             for (size_t k = 0; k < K; ++k)
-                if (o.steps[k] > 0)
-                    CU(h, cudaMemcpy2DAsync(o.probs[k] + (size_t)first * o.max_probs[k], (size_t)o.max_probs[k] * 4, tile_probs[k],
-                                            (size_t)tile_probs_stride[k] * 4, (size_t)o.steps[k] * 4, n, cudaMemcpyDeviceToHost, h->st_d2h));
+                if (o.steps[k] > 0 && span[k].b > span[k].a)      // model k's rows [a, b) of the tile
+                    CU(h, cudaMemcpy2DAsync(o.probs[k] + (size_t)span[k].a * o.max_probs[k], (size_t)o.max_probs[k] * 4, tile_probs[k],
+                                            (size_t)tile_probs_stride[k] * 4, (size_t)o.steps[k] * 4, span[k].b - span[k].a,
+                                            cudaMemcpyDeviceToHost, h->st_d2h));
             CU(h, cudaEventRecord(h->ev_d2h[b], h->st_d2h));
         }
     }
@@ -1003,9 +1149,10 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
     // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
     // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone
     const size_t staged_bytes = sizeof(T) == sizeof(int16_t) ? 0 : 2 * (size_t)std::max(n_samples, 1) * sizeof(T);
-    int tile = tile_streams(h, n_frames, true, staged_bytes);
+    const size_t gather = gather_bytes_per_stream(h, n_frames);
+    int tile = tile_streams(h, n_frames, true, staged_bytes + gather);
     tile = std::max(1, std::min(tile, std::max((h->n_streams + want_tiles - 1) / want_tiles, std::min(h->n_streams, h->min_tile_streams))));
-    rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2);
+    rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2, (size_t)tile * gather);
     if (rc) return rc;
     const size_t a_bytes = (size_t)tile * std::max(n_samples, 1) * sizeof(T);
     const size_t p_bytes = dst_is_host ? probs_tile_offset(h, o, tile, h->models.size()) * sizeof(float) : 0;
@@ -1250,23 +1397,23 @@ int mww_host_free(void *h_ptr) {
 namespace {
 // one model's NN state to / from the host; the exported ring layout is always the canonical oldest-first one
 int get_model_state(mww_t *h, Model &m, void *h_nn, void *h_pending) {
-    const size_t S = (size_t)h->n_streams;
+    const size_t M = (size_t)m.members();
     if (h_nn) {
         if (int rc = canonicalise_rings(h, m, nullptr)) return rc;
         CU(h, cudaDeviceSynchronize());
-        CU(h, cudaMemcpy(h_nn, m.d_nn_state, S * m.G.state_elems * m.elem_size(), cudaMemcpyDeviceToHost));
+        if (M > 0) CU(h, cudaMemcpy(h_nn, m.d_nn_state, M * m.state_bytes(), cudaMemcpyDeviceToHost));
     }
-    if (h_pending) CU(h, cudaMemcpy(h_pending, m.d_pend, S * m.G.pend_cap * kNumChannels * m.elem_size(), cudaMemcpyDeviceToHost));
+    if (h_pending && M > 0) CU(h, cudaMemcpy(h_pending, m.d_pend, M * m.pend_bytes(), cudaMemcpyDeviceToHost));
     return MWW_OK;
 }
 int set_model_state(mww_t *h, Model &m, const void *h_nn, const void *h_pending, int pending_rows) {
-    const size_t S = (size_t)h->n_streams;
+    const size_t M = (size_t)m.members();
     note_state_set(h, m, h_nn, h_pending, pending_rows);
     if (h_nn) {
-        CU(h, cudaMemcpy(m.d_nn_state, h_nn, S * m.G.state_elems * m.elem_size(), cudaMemcpyHostToDevice));
+        if (M > 0) CU(h, cudaMemcpy(m.d_nn_state, h_nn, M * m.state_bytes(), cudaMemcpyHostToDevice));
         m.live_heads = LiveHeads{};
     }
-    if (h_pending) CU(h, cudaMemcpy(m.d_pend, h_pending, S * m.G.pend_cap * kNumChannels * m.elem_size(), cudaMemcpyHostToDevice));
+    if (h_pending && M > 0) CU(h, cudaMemcpy(m.d_pend, h_pending, M * m.pend_bytes(), cudaMemcpyHostToDevice));
     m.n_pend = pending_rows;
     return MWW_OK;
 }
@@ -1325,10 +1472,62 @@ int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending
     return set_model_state(h, m, h_nn, h_pending, pending_rows);
 }
 
+int mww_set_model_streams(mww_t *h, int k, const int32_t *h_ids, int n, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (k < 0 || k >= (int)h->models.size()) return fail(h, MWW_EINVAL, "mww_set_model_streams: model index out of range");
+    if (h_ids && (n < 0 || n > h->n_streams || !valid_stream_set(h_ids, n, h->n_streams)))
+        return fail(h, MWW_EINVAL, "mww_set_model_streams: stream ids must be strictly increasing and in [0, n_streams)");
+    ENTER_STATEFUL(h);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    Model &m = h->models[k];
+    MemberState ns;
+    if (int rc = alloc_members(h, m, h_ids, n, &ns)) return rc;
+    // new member j takes the rows of old compact index old_index[j]; the joiners (-1) get fresh state.  Every model's ring
+    // rotation is the same for all its streams, so rows copied as they are stay valid while the rings are rotated.
+    const int M = (int)ns.mem.ids.size();
+    std::vector<int32_t> old_index(M), joiners;
+    for (int j = 0; j < M; ++j) {
+        const int s = ns.mem.ids[j];
+        const int o = lower_bound_ids(m.mem.ids.data(), m.members(), s);
+        old_index[j] = o < m.members() && m.mem.ids[o] == s ? o : -1;
+        if (old_index[j] < 0) joiners.push_back(j);
+    }
+    std::vector<int32_t> maps(old_index);
+    maps.insert(maps.end(), joiners.begin(), joiners.end());
+    int32_t *d_maps = nullptr;
+    cudaError_t e = maps.empty() ? cudaSuccess : cudaMalloc(&d_maps, maps.size() * sizeof(int32_t));
+    if (e == cudaSuccess && d_maps) e = cudaMemcpyAsync(d_maps, maps.data(), maps.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && (int)joiners.size() < M) {
+        e = launch_remap_rows(ns.d_nn_state, m.d_nn_state, m.state_bytes(), d_maps, M, h->sm_count, st);
+        if (e == cudaSuccess) e = launch_remap_rows(ns.d_pend, m.d_pend, m.pend_bytes(), d_maps, M, h->sm_count, st);
+        if (e == cudaSuccess) h->launches += 2;
+    }
+    int rc = e == cudaSuccess ? MWW_OK : cuda_fail(h, e, "mww_set_model_streams: state remap");
+    if (rc == MWW_OK && !joiners.empty()) rc = reset_nn_by_id(h, m, ns.d_nn_state, ns.d_pend, d_maps + M, (int)joiners.size(), M, st);
+    // the old buffers (and the id maps) are freed only once the remap that reads them is done
+    if (cudaError_t s = cudaStreamSynchronize(st)) if (rc == MWW_OK) rc = cuda_fail(h, s, "cudaStreamSynchronize");
+    cudaFree(d_maps);
+    if (rc != MWW_OK) { ns.release(); return rc; }
+    cudaFree(m.mem.d_ids); cudaFree(m.mem.d_inv); cudaFree(m.d_nn_state); cudaFree(m.d_pend);
+    m.mem = std::move(ns.mem);
+    m.d_nn_state = ns.d_nn_state;
+    m.d_pend = ns.d_pend;
+    return MWW_OK;
+}
+
+int mww_get_model_streams(const mww_t *h, int k, int32_t *h_ids, int max_ids, int *n_out) {
+    if (!h || k < 0 || k >= (int)h->models.size() || max_ids < 0 || (max_ids > 0 && !h_ids)) return MWW_EINVAL;
+    const std::vector<int32_t> &ids = h->models[k].mem.ids;
+    std::copy(ids.begin(), ids.begin() + std::min<size_t>(ids.size(), (size_t)max_ids), h_ids);
+    if (n_out) *n_out = (int)ids.size();
+    return MWW_OK;
+}
+
 int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src_c, const int32_t *h_src_ids, int n, void *cu_stream) {
     if (!dst) return MWW_EINVAL;
     if (int rc = refuse_multi(dst, "mww_copy_nn_state", "a one-model handle")) return rc;
     if (src_c && src_c->models.size() > 1) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: the source handle carries several models");
+    if (src_c && !all_streams(src_c)) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: the source model runs on a subset of the streams");
     // canonicalising the source's rings changes their layout, not the state they hold
     mww_t *src = const_cast<mww_t *>(src_c);
     if (!src || n < 0 || (n > 0 && (!h_dst_ids || !h_src_ids))) return fail(dst, MWW_EINVAL, "mww_copy_nn_state: bad arguments");

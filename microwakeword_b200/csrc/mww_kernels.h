@@ -97,4 +97,14 @@ cudaError_t launch_gen_fill_state_i8(const GenArch &A, const GenWeightsI8 &W, in
 cudaError_t launch_nn_generic_hybrid(const GenArch &A, const GenWeightsF32 &W, const GenHybrid &H, float *state, float *pend, int n_pend,
                                      const void *rows, long long rows_stream_stride_bytes, int n_rows, int row_type, float *probs,
                                      long long probs_stream_stride, int n_streams, cudaStream_t st);
+
+// per-model stream sets (mww_streams.cu, index math in mww_streams.h)
+// rows [n_rows][40] of the m members ids[a, a + m) of the tile whose rows start at stream `first` -> compact out [m][n_rows][40]
+cudaError_t launch_gather_rows(const uint16_t *feat, const int32_t *ids, int a, int first, int m, int n_rows, uint16_t *out, int sm_count,
+                               cudaStream_t st);
+// new row j of dst [n_new][bytes_per_row] = old row old_index[j] of src; rows with old_index -1 are not written
+cudaError_t launch_remap_rows(void *dst, const void *src, size_t bytes_per_row, const int32_t *old_index, int n_new, int sm_count,
+                              cudaStream_t st);
+// out[i] = compact index of global stream id ids[i] from the inverse map inv[n_streams], -1 for a non-member or an id out of range
+cudaError_t launch_compact_ids(int32_t *out, const int32_t *ids, int n, const int32_t *inv, int n_streams, int sm_count, cudaStream_t st);
 }  // namespace mww

@@ -384,19 +384,32 @@ class MultiModelEngine(_Engine):
     of) MWW containers or streaming ``.tflite`` flatbuffers, converted as StreamEngine converts them; any mix of kinds,
     geometries and strides.  Calls return one result per model, in the order of `models`; model k's results and state are
     bit-identical to a StreamEngine of models[k] given the same calls.  `stride`, `is_quantized`, `state_elements` and
-    `pending_rows` are per-model lists."""
+    `pending_rows` are per-model lists.
 
-    def __init__(self, models, n_streams: int = 1, device: int = 0):
+    `streams`: None (every model on every stream) or one entry per model, None (all streams) or a strictly increasing
+    sequence of stream ids (mww_create_multi_streams): model k then runs on those streams only, its state is allocated for
+    them only, and its results have one row per id, in that order (row j belongs to stream streams[k][j]).  Unsorted,
+    duplicate or out-of-range ids raise ValueError.  `engine.streams[k]` is model k's set (int32), `set_streams` changes it."""
+
+    def __init__(self, models, n_streams: int = 1, device: int = 0, streams=None):
         blobs = [load_model_blob(m) for m in models]
         if any(b is None for b in blobs):
             raise ValueError("every model must be a path or the bytes of a model file")
+        K = len(blobs)
+        if streams is not None and len(streams) != K:
+            raise ValueError("streams must hold one entry per model (%d), not %d" % (K, len(streams)))
+        sets = [None if streams is None or streams[k] is None else self._stream_set(streams[k], n_streams) for k in range(K)]
         self._L = _lib.lib()
         self._h = ctypes.c_void_p()
-        K = len(blobs)
         self._bufs = [ctypes.create_string_buffer(b, len(b)) for b in blobs]
         ptrs = (ctypes.c_void_p * max(K, 1))(*[ctypes.addressof(b) for b in self._bufs])
         sizes = (ctypes.c_size_t * max(K, 1))(*[len(b) for b in blobs])
-        rc = self._L.mww_create_multi(ptrs, sizes, K, int(device), int(n_streams), ctypes.byref(self._h))
+        if any(s is not None for s in sets):
+            ids = (ctypes.c_void_p * K)(*[None if s is None else s.ctypes.data for s in sets])
+            n_ids = (ctypes.c_int * K)(*[0 if s is None else s.size for s in sets])
+            rc = self._L.mww_create_multi_streams(ptrs, sizes, K, int(device), int(n_streams), ids, n_ids, ctypes.byref(self._h))
+        else:
+            rc = self._L.mww_create_multi(ptrs, sizes, K, int(device), int(n_streams), ctypes.byref(self._h))
         if rc != 0:
             msg = self._L.mww_last_error(None)
             raise _lib.MwwError(rc, msg.decode() if msg else "mww_create_multi failed")
@@ -409,6 +422,35 @@ class MultiModelEngine(_Engine):
         self.stride = [max(int(i.input_feature_slices), 1) for i in infos]
         self.state_elements = [int(i.state_bytes_per_stream) // (1 if q else 4) for i, q in zip(infos, self.is_quantized)]
         self.hop = HOP
+        self.streams = [self._get_streams(k) for k in range(K)]
+
+    @staticmethod
+    def _stream_set(ids, n_streams: int) -> np.ndarray:
+        """a caller's stream ids -> int32 array; ValueError unless strictly increasing in [0, n_streams) (never sorted here:
+        row j of a model's results belongs to its j-th id)"""
+        a = np.asarray(ids)
+        if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise ValueError("stream ids must be a 1-D sequence of integers")
+        a = a.astype(np.int64)
+        if a.size and (a[0] < 0 or a[-1] >= n_streams or (a.size > 1 and not (np.diff(a) > 0).all())):
+            raise ValueError("stream ids must be strictly increasing and in [0, n_streams=%d)" % n_streams)
+        return np.ascontiguousarray(a, np.int32)
+
+    def _get_streams(self, k: int) -> np.ndarray:
+        out = np.zeros(self.n_streams, np.int32)
+        n = ctypes.c_int(0)
+        _lib.check(self._h, self._L.mww_get_model_streams(self._h, int(k), out.ctypes.data, out.size, ctypes.byref(n)))
+        return out[:n.value].copy()
+
+    def set_streams(self, k: int, ids) -> None:
+        """Model k runs on stream ids `ids` from now on (None: all streams), ordered on the current CUDA stream
+        (mww_set_model_streams): streams it keeps continue exactly, streams that join start from fresh state."""
+        if not 0 <= int(k) < self.n_models:
+            raise ValueError("model index out of range")
+        s = None if ids is None else self._stream_set(ids, self.n_streams)
+        _lib.check(self._h, self._L.mww_set_model_streams(self._h, int(k), None if s is None else s.ctypes.data,
+                                                          0 if s is None else s.size, self._cu_stream()))
+        self.streams[int(k)] = self._get_streams(k)
 
     def _model_info(self, k: int):
         info = _lib.MwwInfo()
@@ -423,19 +465,22 @@ class MultiModelEngine(_Engine):
         return call_plan(self.frontend_buffered, n_samples, self.hop, self.pending_rows, self.stride)[1]
 
     def _outs(self, steps, out, host: bool):
-        """-> (K buffers, their ctypes pointer / max_probs / steps-out arrays)"""
+        """-> (K buffers, their ctypes pointer / max_probs / steps-out arrays); model k's buffer has one row per stream of
+        its set"""
         torch = _torch()
+        rows = [s.size for s in self.streams]
         if out is None:
-            out = [np.empty((self.n_streams, max(s, 1)), np.float32) if host else
-                   torch.empty((self.n_streams, max(s, 1)), dtype=torch.float32, device=self._dev()) for s in steps]
+            out = [np.empty((r, max(s, 1)), np.float32) if host else
+                   torch.empty((r, max(s, 1)), dtype=torch.float32, device=self._dev()) for r, s in zip(rows, steps)]
         elif len(out) != self.n_models:
             raise ValueError("out must hold one buffer per model (%d)" % self.n_models)
         elif host:
-            if any(o.dtype != np.float32 or o.ndim != 2 or o.shape[0] != self.n_streams or not o.flags.c_contiguous for o in out):
-                raise ValueError("out must be C-contiguous float32 host arrays [n_streams, >= steps]")
+            if any(o.dtype != np.float32 or o.ndim != 2 or o.shape[0] != r or not o.flags.c_contiguous for o, r in zip(out, rows)):
+                raise ValueError("out must be C-contiguous float32 host arrays [streams of model k, >= steps]")
         else:
-            for o in out:
-                self._check_probs_out(o)
+            for o, r in zip(out, rows):
+                if o.dtype != torch.float32 or not o.is_cuda or not o.is_contiguous() or o.dim() != 2 or o.shape[0] != r:
+                    raise ValueError("out must be contiguous CUDA float32 tensors [streams of model k, >= steps]")
         K = self.n_models
         ptrs = (ctypes.c_void_p * K)(*[o.ctypes.data if host else o.data_ptr() for o in out])
         maxp = (ctypes.c_int * K)(*[o.shape[1] for o in out])
@@ -474,7 +519,8 @@ class MultiModelEngine(_Engine):
 
     # ------------------------------------------------------------------ state (checkpoint / tests)
     def state_dict(self) -> dict:
-        """{carry, estimate, frontend_buffered: the shared frontend; models: [{nn, pending, pending_rows} per model]}"""
+        """{carry, estimate, frontend_buffered: the shared frontend; models: [{streams, nn, pending, pending_rows} per model]},
+        model k's nn / pending arrays one row per stream of its set"""
         S = self.n_streams
         d = dict(carry=np.zeros((S, WINDOW), np.int16), estimate=np.zeros((S, NUM_FEATURES), np.uint32))
         _lib.check(self._h, self._L.mww_get_state(self._h, d["carry"].ctypes.data, d["estimate"].ctypes.data, None, None))
@@ -482,20 +528,30 @@ class MultiModelEngine(_Engine):
         d["models"] = []
         for k in range(self.n_models):
             dt = np.int8 if self.is_quantized[k] else np.float32
-            m = dict(nn=np.zeros((S, self.state_elements[k]), dt), pending=np.zeros((S, max(self.stride[k] - 1, 1), NUM_FEATURES), dt))
+            M = self.streams[k].size
+            m = dict(streams=self.streams[k].copy(), nn=np.zeros((M, self.state_elements[k]), dt),
+                     pending=np.zeros((M, max(self.stride[k] - 1, 1), NUM_FEATURES), dt))
             _lib.check(self._h, self._L.mww_get_model_state(self._h, k, m["nn"].ctypes.data, m["pending"].ctypes.data))
             m["pending_rows"] = self._model_info(k).pending_rows
             d["models"].append(m)
         return d
 
     def load_state_dict(self, d: dict) -> None:
+        """the state of state_dict(); each model's stream set is restored first (a state without `streams`: all streams)"""
         if len(d["models"]) != self.n_models:
             raise ValueError("the state holds %d models, this engine %d" % (len(d["models"]), self.n_models))
         carry = np.ascontiguousarray(d["carry"], np.int16)
         est = np.ascontiguousarray(d["estimate"], np.uint32)
+        for k, m in enumerate(d["models"]):
+            want = self._stream_set(m["streams"], self.n_streams) if m.get("streams") is not None else np.arange(self.n_streams, dtype=np.int32)
+            if not np.array_equal(want, self.streams[k]):
+                self.set_streams(k, want)
         _lib.check(self._h, self._L.mww_set_state(self._h, carry.ctypes.data, int(d["frontend_buffered"]), est.ctypes.data, None, None, 0))
         for k, m in enumerate(d["models"]):
             dt = np.int8 if self.is_quantized[k] else np.float32
             nn = np.ascontiguousarray(m["nn"], dt)
             pend = np.ascontiguousarray(m["pending"], dt)
+            M = self.streams[k].size
+            if nn.shape != (M, self.state_elements[k]) or pend.shape != (M, max(self.stride[k] - 1, 1), NUM_FEATURES):
+                raise ValueError("model %d: nn / pending must have one row per stream of its set (%d)" % (k, M))
             _lib.check(self._h, self._L.mww_set_model_state(self._h, k, nn.ctypes.data, pend.ctypes.data, int(m["pending_rows"])))
