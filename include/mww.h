@@ -289,6 +289,62 @@ int mww_set_state(mww_t *h, const int16_t *h_carry, int frontend_buffered, const
  * moving the state of many streams at once is what mww_get_state / mww_set_state do. */
 int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src, const int32_t *h_src_ids, int n, void *cu_stream);
 
+/* ---- moving streams between handles -------------------------------------------------------------------------------
+ * A handle serves a fixed number of streams.  A server that grows or compacts a handle, rebalances streams across the GPUs
+ * of a box or checkpoints some streams moves them as STREAM RECORDS: everything one stream carries (frontend and every
+ * model), packed on the device by mww_export_streams and written into another handle by mww_import_streams, in a number of
+ * launches that does not depend on how many streams move.  The state arrives bit-exact, and a stream that moves continues
+ * bit for bit as if it had stayed wherever the arithmetic does not depend on the ring rotation: int8, hybrid and
+ * run-time-geometry models, every clip call, and fp32 okay_nabu live calls when the destination's rings are at the
+ * rotation the stream left (the same number of live calls since the last clip call, modulo each ring's length).  The
+ * fp32 live-step kernel adds a ring's taps in physical row order, so at another rotation the last bits may differ.
+ *   - one record, record_bytes long (a multiple of 16), every part padded to 16 bytes:
+ *         uint64  member_mask          bit k set: the stream was a member of model k and slot k holds its state
+ *         int16   carry[480]           window buffer (first frontend_buffered samples valid)
+ *         uint32  estimate[40]         noise estimates
+ *         for each model k, in order:  nn[state elements of model k]  float32 or int8, the layout of mww_get_model_state:
+ *                                                                     rings CANONICAL, oldest row first
+ *                                      pending[max(stride_k - 1, 1)][40]  float32 or int8
+ *     d_records is [n][record_bytes], 16-byte aligned, in memory the handle's GPU can address: its own, or a peer buffer
+ *     mapped with mww_ipc_open (read or written in place over NVLink).  Between GPUs without a mapping: export on the
+ *     source GPU and pull the buffer with mww_copy_async.
+ *   - the lockstep counters belong to the handle, not to a stream: they travel beside the records in mww_stream_layout,
+ *     which mww_export_streams fills (out may be NULL) and mww_import_streams checks.  mww_stream_layout_get gives a
+ *     handle's own layout and current counters without device work (record_bytes sizes the buffer).
+ *   - both calls are asynchronous and stream-ordered on cu_stream and take GLOBAL stream ids from host memory, in any
+ *     order; export allows an id to appear twice, import refuses it.  n == 0 launches nothing and still fills / checks the
+ *     layout.
+ *   - mww_export_streams does not change the handle, not even the rotation live calls leave its rings in: the pack kernel
+ *     reads each ring row where it lies and writes it oldest first.  For a model the stream is not a member of, its mask
+ *     bit is clear and its slot is zero.
+ *   - mww_import_streams overwrites exactly the listed streams' state and leaves every other stream's bytes untouched; it
+ *     writes each ring at the destination's own rotation, so the two handles may have made different numbers of live
+ *     calls.  Per model k: a destination stream that is not a member ignores slot k; a member whose mask bit is set takes
+ *     the state; a member whose bit is clear gets the model's fresh state (what mww_reset(ids) and mww_set_model_streams
+ *     give: zero rings for fp32 and hybrid, zero points for int8).  Import lowers model k's rows_are_features flag
+ *     to the records' for every model with members, whatever the streams listed.
+ *   - import is refused with MWW_EINVAL, before any device work and with the handle unchanged, when the records do not fit
+ *     the destination: n_models, a model (container, precision, state size), record_bytes, hop_samples, frontend_buffered
+ *     or a model's pending_rows differs -- the message names the first such field -- or an id is out of range or listed
+ *     twice.  The counters must match because a handle's streams advance in lockstep; two handles that serve 480-sample
+ *     live calls always match (320 buffered samples, a constant pending-row count).
+ *   - rows_are_features[k] says whether model k's carried first-conv rows are exact feature rows, which is what lets the
+ *     fp16 first conv of the okay_nabu clip kernel run; import lowers the destination's flag to match, so an imported
+ *     stream continues on the kernel it would have run in the source.
+ *   - a poisoned handle refuses both calls; n < 0, NULL or misaligned buffers with n > 0: MWW_EINVAL.  Frontend-only
+ *     handles work (record = mask, carry, estimate). */
+typedef struct mww_stream_layout {
+    int64_t record_bytes;
+    int32_t n_models, frontend_buffered, hop_samples;
+    int32_t pending_rows[64];
+    uint64_t model_hash[64];          /* hash of model k's container, its precision and state size */
+    uint8_t rows_are_features[64];
+} mww_stream_layout;
+int mww_stream_layout_get(const mww_t *h, mww_stream_layout *out);
+int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out, void *cu_stream);
+int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout,
+                       void *cu_stream);
+
 /* ---- detection post-processing (microwakeword/test.py:337-341, :94-137, :364-373) -------------------------
  * Tracks are ragged: track i is d_probs[d_offsets[i] .. d_offsets[i] + d_lengths[i]) (float32 probabilities as
  * produced by mww_infer_features / mww_predict_clip).  All four are stateless and asynchronous on cu_stream.

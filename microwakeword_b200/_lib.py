@@ -28,6 +28,7 @@ EXPORTS = (
     "mww_predict_clip_host_multi", "mww_predict_clip_remote_multi", "mww_get_model_state", "mww_set_model_state",
     "mww_predict_clip_host_f32", "mww_predict_clip_host_multi_f32", "mww_predict_clip_remote_f32", "mww_predict_clip_remote_multi_f32",
     "mww_create_multi_streams", "mww_set_model_streams", "mww_get_model_streams",
+    "mww_stream_layout_get", "mww_export_streams", "mww_import_streams",
 )
 
 
@@ -40,6 +41,15 @@ class MwwInfo(ctypes.Structure):
         ("state_bytes_per_stream", ctypes.c_int32), ("frontend_buffered", ctypes.c_int32),
         ("pending_rows", ctypes.c_int32), ("sm_count", ctypes.c_int32), ("macs_per_step", ctypes.c_int32),
         ("hop_samples", ctypes.c_int32),
+    ]
+
+
+class MwwStreamLayout(ctypes.Structure):
+    """mww_stream_layout of include/mww.h: what travels beside exported stream records"""
+    _fields_ = [
+        ("record_bytes", ctypes.c_int64), ("n_models", ctypes.c_int32), ("frontend_buffered", ctypes.c_int32),
+        ("hop_samples", ctypes.c_int32), ("pending_rows", ctypes.c_int32 * 64), ("model_hash", ctypes.c_uint64 * 64),
+        ("rows_are_features", ctypes.c_uint8 * 64),
     ]
 
 
@@ -161,6 +171,12 @@ def lib() -> ctypes.CDLL:
     L.mww_set_model_streams.argtypes = [vp, i32, vp, i32, vp]
     L.mww_get_model_streams.restype = i32
     L.mww_get_model_streams.argtypes = [vp, i32, vp, i32, pi]
+    L.mww_stream_layout_get.restype = i32
+    L.mww_stream_layout_get.argtypes = [vp, ctypes.POINTER(MwwStreamLayout)]
+    L.mww_export_streams.restype = i32
+    L.mww_export_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), vp]
+    L.mww_import_streams.restype = i32
+    L.mww_import_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), vp]
     _lib = L
     return L
 

@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmww_b200.so")
-SOURCES = ["mww_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_streams.cu", "mww_detect.cu", "mww_tables.cc", "mww_container.cc"]
+SOURCES = ["mww_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_streams.cu", "mww_records.cu", "mww_detect.cu", "mww_tables.cc", "mww_container.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]

@@ -910,6 +910,22 @@ int reset_nn_by_id(mww_t *h, const Model &m, void *state, void *pend, const int3
     return rc;
 }
 
+// a device int32 buffer of at least n entries; growing it first waits for the work on st that may still read the old one
+int ensure_ids(mww_t *h, int32_t **buf, size_t *cap, int n, cudaStream_t st) {
+    if ((size_t)n <= *cap) return MWW_OK;
+    if (*buf) { CU(h, cudaStreamSynchronize(st)); cudaFree(*buf); *buf = nullptr; *cap = 0; }
+    const size_t want = std::max<size_t>((size_t)n, 1024);
+    CU(h, cudaMalloc(buf, want * sizeof(int32_t)));
+    *cap = want;
+    return MWW_OK;
+}
+// a host id list -> h->d_ids, ordered on st
+int upload_ids(mww_t *h, const int32_t *h_ids, int n, cudaStream_t st) {
+    if (int rc = ensure_ids(h, &h->d_ids, &h->ids_cap, n, st)) return rc;
+    CU(h, cudaMemcpyAsync(h->d_ids, h_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return MWW_OK;
+}
+
 // fresh state for the listed global stream ids: a handful of launches whatever the length of the list.  A model on all
 // streams takes the ids as they are; any other first has them translated to its compact indices (-1 for a non-member,
 // which the fill kernels skip).
@@ -924,12 +940,7 @@ int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
             continue;
         }
         if (m.members() == 0) continue;
-        if ((size_t)n > h->cids_cap) {
-            if (h->d_cids) { CU(h, cudaStreamSynchronize(st)); cudaFree(h->d_cids); h->d_cids = nullptr; h->cids_cap = 0; }
-            const size_t cap = std::max<size_t>((size_t)n, 1024);
-            CU(h, cudaMalloc(&h->d_cids, cap * sizeof(int32_t)));
-            h->cids_cap = cap;
-        }
+        if (int rc2 = ensure_ids(h, &h->d_cids, &h->cids_cap, n, st)) return rc2;
         CU(h, launch_compact_ids(h->d_cids, d_ids, n, m.mem.d_inv, h->n_streams, h->sm_count, st));
         h->launches += 1;
         rc = reset_nn_by_id(h, m, m.d_nn_state, m.d_pend, h->d_cids, n, m.members(), st);
@@ -954,13 +965,7 @@ int mww_reset(mww_t *h, const int32_t *h_ids, int n, void *cu_stream) {
     if (n <= 0) return MWW_OK;
     for (int i = 0; i < n; ++i)
         if (h_ids[i] < 0 || h_ids[i] >= h->n_streams) return fail(h, MWW_EINVAL, "mww_reset: stream id out of range");
-    if ((size_t)n > h->ids_cap) {
-        if (h->d_ids) { CU(h, cudaStreamSynchronize(st)); cudaFree(h->d_ids); h->d_ids = nullptr; h->ids_cap = 0; }
-        const size_t cap = std::max<size_t>((size_t)n, 1024);
-        CU(h, cudaMalloc(&h->d_ids, cap * sizeof(int32_t)));
-        h->ids_cap = cap;
-    }
-    CU(h, cudaMemcpyAsync(h->d_ids, h_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
     return reset_by_id(h, h->d_ids, n, st);
 }
 
@@ -1553,6 +1558,126 @@ int mww_copy_nn_state(mww_t *dst, const int32_t *h_dst_ids, const mww_t *src_c, 
     for (int i = 0; i < n; ++i) {
         if (dst == src && h_dst_ids[i] == h_src_ids[i]) continue;     // same bytes: nothing to copy (and memcpy needs disjoint ranges)
         CU(dst, cudaMemcpyAsync(d + (size_t)h_dst_ids[i] * bytes, s + (size_t)h_src_ids[i] * bytes, bytes, cudaMemcpyDeviceToDevice, st));
+    }
+    return MWW_OK;
+}
+
+// ---- stream records: a stream's whole state between handles (layout and index math: mww_records.h) ------------------
+namespace {
+static_assert(kMaxModels == kRecordMaxModels, "one bit of the member mask per model");
+
+RecordModel record_model(const Model &m) { return RecordModel{(long long)m.state_bytes(), (long long)m.pend_bytes()}; }
+
+RecordLayout handle_record_layout(const mww_t *h) {
+    RecordModel rm[kMaxModels];
+    for (size_t k = 0; k < h->models.size(); ++k) rm[k] = record_model(h->models[k]);
+    return record_layout(rm, (int)h->models.size());
+}
+
+void fill_stream_layout(const mww_t *h, mww_stream_layout *o) {
+    memset(o, 0, sizeof *o);
+    o->record_bytes = handle_record_layout(h).record_bytes;
+    o->n_models = (int)h->models.size();
+    o->frontend_buffered = h->used;
+    o->hop_samples = h->hop;
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        const Model &m = h->models[k];
+        o->pending_rows[k] = m.n_pend;
+        o->model_hash[k] = record_model_hash(m.model_hash, m.quantized(), m.G.state_elems);
+        o->rows_are_features[k] = m.tc_rows_bounded;
+    }
+}
+
+// model k's ring state and pending rows, with the rotation live calls have left its rings in.  Only the compiled-in
+// okay_nabu kernels rotate (blocks 0..3 and the head ring, after the first-conv ring); every other kind keeps canonical
+// rings, so its state is one plain span.
+RecordJob model_record_job(const RecordLayout &L, int k, const Model &m) {
+    RecordJob J = record_job_model(L, k, record_model(m));
+    J.zero_fresh = !m.quantized();
+    if (m.compiled()) {
+        const int es = (int)m.elem_size();
+        int off = 2 * kNumChannels;
+        for (int i = 0; i < 5; ++i) {
+            record_add_ring(&J, off * es, live_ring_cols(i) * es, kLiveRingRows[i], m.live_heads.h[i]);
+            off += kLiveRingRows[i] * live_ring_cols(i);
+        }
+    }
+    return J;
+}
+
+// argument checks shared by export and import; returns MWW_OK or the failure already recorded on h
+int check_record_args(mww_t *h, const char *who, const int32_t *h_ids, int n, const void *d_records) {
+    if (n < 0 || (n > 0 && (!h_ids || !d_records))) return fail(h, MWW_EINVAL, std::string(who) + ": bad arguments");
+    if (reinterpret_cast<uintptr_t>(d_records) % 16 != 0) return fail(h, MWW_EINVAL, std::string(who) + ": the records must be 16-byte aligned");
+    for (int i = 0; i < n; ++i)
+        if (h_ids[i] < 0 || h_ids[i] >= h->n_streams) return fail(h, MWW_EINVAL, std::string(who) + ": stream id out of range");
+    return MWW_OK;
+}
+}  // namespace
+
+int mww_stream_layout_get(const mww_t *h, mww_stream_layout *out) {
+    if (!h || !out) return MWW_EINVAL;
+    fill_stream_layout(h, out);
+    return MWW_OK;
+}
+
+int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (int rc = check_record_args(h, "mww_export_streams", h_ids, n, d_records)) return rc;
+    ENTER_STATEFUL(h);
+    if (out) fill_stream_layout(h, out);
+    if (n == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+    const RecordLayout L = handle_record_layout(h);
+    const void *fe[kRecordMaxParts] = {nullptr, h->d_carry, h->d_estimate};
+    CU(h, launch_pack_streams(record_job_frontend(L), d_records, L.record_bytes, h->d_ids, n, fe, nullptr, h->sm_count, st));
+    h->launches += 1;
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        const Model &m = h->models[k];
+        const void *nn[kRecordMaxParts] = {m.d_nn_state, m.d_pend, nullptr};
+        CU(h, launch_pack_streams(model_record_job(L, (int)k, m), d_records, L.record_bytes, h->d_ids, n, nn, m.mem.d_inv, h->sm_count, st));
+        h->launches += 1;
+    }
+    return MWW_OK;
+}
+
+int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (!layout) return fail(h, MWW_EINVAL, "mww_import_streams: bad arguments");
+    if (int rc = check_record_args(h, "mww_import_streams", h_ids, n, d_records)) return rc;
+    std::vector<uint8_t> listed((size_t)h->n_streams, 0);
+    for (int i = 0; i < n; ++i) {
+        if (listed[(size_t)h_ids[i]]) return fail(h, MWW_EINVAL, "mww_import_streams: a stream id is listed twice");
+        listed[(size_t)h_ids[i]] = 1;
+    }
+    mww_stream_layout mine;
+    fill_stream_layout(h, &mine);
+    int which = -1;
+    if (const char *field = stream_layout_mismatch(*layout, mine, &which))
+        return fail(h, MWW_EINVAL, std::string("mww_import_streams: the records' ") + field +
+                                       (which >= 0 ? " of model " + std::to_string(which) : std::string()) + " differs from the handle's");
+    ENTER_STATEFUL(h);
+    if (n == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = ensure_ids(h, &h->d_cids, &h->cids_cap, n, st)) return rc;
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+    const RecordLayout L = handle_record_layout(h);
+    void *fe[kRecordMaxParts] = {nullptr, h->d_carry, h->d_estimate};
+    CU(h, launch_unpack_streams(record_job_frontend(L), d_records, L.record_bytes, h->d_ids, n, fe, nullptr, nullptr, h->sm_count, st));
+    h->launches += 1;
+    for (size_t k = 0; k < h->models.size(); ++k) {
+        Model &m = h->models[k];
+        if (m.members() == 0) continue;
+        void *nn[kRecordMaxParts] = {m.d_nn_state, m.d_pend, nullptr};
+        // members the records hold no state for start fresh, as the joiners of mww_set_model_streams do: zeros (fp32, hybrid)
+        // are written by the unpack kernel, zero points (int8) by the model's fill kernel over the list it leaves in d_cids
+        const RecordJob J = model_record_job(L, (int)k, m);
+        CU(h, launch_unpack_streams(J, d_records, L.record_bytes, h->d_ids, n, nn, m.mem.d_inv, J.zero_fresh ? nullptr : h->d_cids, h->sm_count, st));
+        h->launches += 1;
+        if (!J.zero_fresh)
+            if (int rc = reset_nn_by_id(h, m, m.d_nn_state, m.d_pend, h->d_cids, n, m.members(), st)) return rc;
+        m.tc_rows_bounded = m.tc_rows_bounded && layout->rows_are_features[k];
     }
     return MWW_OK;
 }

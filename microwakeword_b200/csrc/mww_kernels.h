@@ -108,3 +108,15 @@ cudaError_t launch_remap_rows(void *dst, const void *src, size_t bytes_per_row, 
 // out[i] = compact index of global stream id ids[i] from the inverse map inv[n_streams], -1 for a non-member or an id out of range
 cudaError_t launch_compact_ids(int32_t *out, const int32_t *ids, int n, const int32_t *inv, int n_streams, int sm_count, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_records.h"
+namespace mww {
+// stream records (mww_records.cu, layout and index math in mww_records.h): the parts of job J of the n streams ids[0, n)
+// between the handle (base[p]: part p of stream / compact index 0) and records [n][record_bytes].  inv: the model's
+// compact index of each global stream id, nullptr for the frontend parts.  Unpack also writes fresh[0, n) when given:
+// the compact index of each listed member the records hold no state for, else -1 (a job with zero_fresh zeroes them itself).
+cudaError_t launch_pack_streams(const RecordJob &J, void *records, long long record_bytes, const int32_t *ids, int n, const void *const *base,
+                                const int32_t *inv, int sm_count, cudaStream_t st);
+cudaError_t launch_unpack_streams(const RecordJob &J, const void *records, long long record_bytes, const int32_t *ids, int n, void *const *base,
+                                  const int32_t *inv, int32_t *fresh, int sm_count, cudaStream_t st);
+}  // namespace mww

@@ -93,6 +93,36 @@ def call_plan(buffered: int, n_samples: int, hop: int, pending_rows, strides):
     return rows, steps, buffered + n_samples - rows * hop, pending
 
 
+class StreamRecords:
+    """Streams exported from an engine (mww_export_streams): `data`, torch.uint8 [n, record_bytes] on the exporting
+    engine's device, one packed record per stream (include/mww.h), and `layout`, the _lib.MwwStreamLayout that travels with
+    them: the sizes, models and lockstep counters an importing engine must share."""
+
+    _SCALARS = ("record_bytes", "n_models", "frontend_buffered", "hop_samples")
+    _ARRAYS = ("pending_rows", "model_hash", "rows_are_features")
+
+    def __init__(self, data, layout):
+        self.data, self.layout = data, layout
+
+    def save(self, path) -> None:
+        """np.savez of the records and the layout's fields: a checkpoint of some streams"""
+        fields = {k: np.asarray(getattr(self.layout, k)) for k in self._SCALARS}
+        fields.update({k: np.ctypeslib.as_array(getattr(self.layout, k)).copy() for k in self._ARRAYS})
+        np.savez(path, data=self.data.cpu().numpy(), **fields)
+
+    @classmethod
+    def load(cls, path, device) -> "StreamRecords":
+        torch = _torch()
+        layout = _lib.MwwStreamLayout()
+        with np.load(path) as z:
+            for k in cls._SCALARS:
+                setattr(layout, k, int(z[k]))
+            for k in cls._ARRAYS:
+                np.ctypeslib.as_array(getattr(layout, k))[:] = z[k]
+            data = torch.from_numpy(z["data"]).to(device)
+        return cls(data, layout)
+
+
 class _Engine:
     """What every engine has: a handle whose `n_streams` streams share one frontend, its argument checks, resets,
     features, pinned host buffers and timing.  Subclasses create the handle and run the models."""
@@ -212,6 +242,51 @@ class _Engine:
         fn = self._L.mww_features_f32 if is_f32 else self._L.mww_features
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
+
+    # ------------------------------------------------------------------ moving streams between engines
+    @staticmethod
+    def _ids(ids) -> np.ndarray:
+        """a list, NumPy array or CPU tensor of global stream ids -> contiguous int32 array"""
+        if hasattr(ids, "is_cuda"):
+            if ids.is_cuda:
+                raise ValueError("stream ids must be in host memory")
+            ids = ids.numpy()
+        a = np.asarray(ids)
+        if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise ValueError("stream ids must be a 1-D sequence of integers")
+        return np.ascontiguousarray(a, np.int32)
+
+    def stream_layout(self) -> "_lib.MwwStreamLayout":
+        """record size, models and current lockstep counters of this engine (mww_stream_layout_get; no device work)"""
+        layout = _lib.MwwStreamLayout()
+        _lib.check(self._h, self._L.mww_stream_layout_get(self._h, ctypes.byref(layout)))
+        return layout
+
+    def export_streams(self, ids) -> StreamRecords:
+        """The whole state (frontend and every model) of streams `ids` as packed records on this engine's device, ordered on
+        the current CUDA stream in a constant number of launches (mww_export_streams).  The engine is not changed."""
+        torch = _torch()
+        ids = self._ids(ids)
+        data = torch.empty((ids.size, int(self.stream_layout().record_bytes)), dtype=torch.uint8, device=self._dev())
+        layout = _lib.MwwStreamLayout()
+        _lib.check(self._h, self._L.mww_export_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
+                                                       self._cu_stream()))
+        return StreamRecords(data, layout)
+
+    def import_streams(self, ids, records: StreamRecords) -> None:
+        """Stream ids[i] of this engine takes the state of records.data[i] (mww_import_streams): it continues bit for bit as
+        the exported stream would have.  Every other stream is untouched.  The records must be a contiguous uint8 tensor
+        [len(ids), record_bytes] on this engine's device (ValueError otherwise); records that do not fit this engine's
+        models or lockstep counters, duplicate or out-of-range ids: MwwError, nothing changed."""
+        torch = _torch()
+        ids = self._ids(ids)
+        data = records.data
+        if (not isinstance(data, torch.Tensor) or data.dtype != torch.uint8 or data.dim() != 2 or data.shape[0] != ids.size
+                or data.shape[1] != records.layout.record_bytes or not data.is_contiguous() or data.device != self._dev()):
+            raise ValueError("records.data must be a contiguous uint8 tensor [len(ids)=%d, record_bytes=%d] on %s"
+                             % (ids.size, records.layout.record_bytes, self._dev()))
+        _lib.check(self._h, self._L.mww_import_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(records.layout),
+                                                       self._cu_stream()))
 
     # ------------------------------------------------------------------ pinned host buffers next to the GPU
     def host_buffer(self, shape, dtype=np.int16, write_combined: bool = False) -> np.ndarray:
