@@ -118,6 +118,43 @@ int mww_reset_frontend(mww_t *h, void *cu_stream);
  * call runs the run-time-hop kernel (one CTA per stream); the row counts below use this hop in place of 160. */
 int mww_set_window_step(mww_t *h, int hop_samples);
 
+/* ---- Input sample rate ----------------------------------------------------------------------------------------------
+ * A handle takes audio at one input rate, 16000 Hz unless mww_set_input_rate says otherwise: 8000, 22050, 24000, 32000,
+ * 44100 or 48000 Hz (L / M = 16000 / rate in lowest terms: 2/1, 320/441, 2/3, 1/2, 160/441, 1/3).  At any rate but 16000 a
+ * resampler kernel turns each stream tile's samples into 16 kHz int16 samples before the frontend, one launch per tile;
+ * at 16000 nothing changes.  Every audio entry point then takes n_samples AT THE INPUT RATE (float32 audio is first
+ * converted to int16 as everywhere else); rows and model steps follow from the 16 kHz count the call yields.
+ *
+ * The resampler is defined in integers.  Taps h[0, N): a Kaiser-windowed sinc designed in double (scipy.signal.kaiserord
+ * for 80 dB attenuation over the transition band, length made odd; scipy.signal.firwin with cutoff at the band's centre,
+ * unit DC gain), times L, in Q15, rounded and clamped to int16.  Decimating rates pass to 7 500 Hz and stop from 8 500 Hz
+ * (the mel filterbank ends at 7 500 Hz, so whatever folds back stays above every feature); 8 kHz passes to 3 600 Hz and
+ * stops from 4 400 Hz.  After Q15 rounding the stopband is at least 70 dB down at every rate (72.8 dB at 32 kHz, 70.4 dB
+ * at 48 kHz, where the 243 taps are shortest) and the passband ripple is within 0.0004.  Output n is
+ *     y[n] = sat16((sum_j h[j] x_up[n M - j] + 2^14) >> 15),   x_up = the input zero-stuffed by L,
+ * scipy.signal.upfirdn(h, x, L, M) followed by the rounding shift, computed exactly.  Calls concatenate exactly: after N
+ * input samples a stream has been given ceil(N L / M) 16 kHz samples, the prefix of one upfirdn over all of its input.
+ * Each stream keeps the last H = ceil(N_taps / L) input samples as history; one counter of input samples seen belongs to
+ * the handle (all streams advance in lockstep).  A 30 ms call (e.g. 1 440 samples at 48 kHz, 1 323 at 44.1 kHz) yields
+ * 480 samples and takes the live-step kernels.  One call must keep n_samples * L below 2^31 (MWW_EINVAL otherwise).
+ *
+ * mww_reset(NULL) and mww_reset_frontend zero the history and the counter; mww_reset(ids) / mww_reset_device_ids zero
+ * those streams' history.  mww_export_streams / mww_import_streams return MWW_EUNSUPPORTED on a handle whose rate is not
+ * 16000 (the records have no room for the history).  The staged paths tile input-rate audio; the 16 kHz tile scratch
+ * counts against MWW_SCRATCH_MB. */
+/* Allowed when mww_set_window_step is (no buffered samples) and the counter is 0; any hop.  A rate outside the list:
+ * MWW_EUNSUPPORTED; buffered samples: MWW_EINVAL.  Either way the handle is unchanged. */
+int mww_set_input_rate(mww_t *h, int rate);
+/* *rate = the input rate, *inputs_seen = input samples every stream has been given since the last reset (0 at 16000) */
+int mww_get_input_rate(const mww_t *h, int *rate, long long *inputs_seen);
+/* history int16 [n_streams][H] (may be NULL) and the counter; at 16000 there is no history and the counter is 0.  Set
+ * synchronises the device; a negative counter (or a non-zero one at 16000) is MWW_EINVAL. */
+int mww_get_resampler_state(mww_t *h, int16_t *h_history, long long *inputs_seen);
+int mww_set_resampler_state(mww_t *h, const int16_t *h_history, long long inputs_seen);
+/* The taps of `rate` without a handle or a GPU: *n_taps, *L, *M (each may be NULL), and the taps (int16 values) in
+ * out[0, n_taps) when max_taps >= n_taps.  16000: n_taps = 0.  A rate outside the list: MWW_EUNSUPPORTED. */
+int mww_resample_taps(int rate, int32_t *out, int max_taps, int *n_taps, int *L, int *M);
+
 /* Frontend only.  d_audio: int16 [n_streams][n_samples] with row pitch `audio_stride` samples.
  * Appends the samples to every stream's window buffer and emits one uint16[40] row per completed
  * 10 ms hop into d_feat [n_streams][max_rows][40].  *h_rows_out = rows emitted per stream

@@ -29,6 +29,7 @@ EXPORTS = (
     "mww_predict_clip_host_f32", "mww_predict_clip_host_multi_f32", "mww_predict_clip_remote_f32", "mww_predict_clip_remote_multi_f32",
     "mww_create_multi_streams", "mww_set_model_streams", "mww_get_model_streams",
     "mww_stream_layout_get", "mww_export_streams", "mww_import_streams",
+    "mww_set_input_rate", "mww_get_input_rate", "mww_get_resampler_state", "mww_set_resampler_state", "mww_resample_taps",
 )
 
 
@@ -177,6 +178,16 @@ def lib() -> ctypes.CDLL:
     L.mww_export_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), vp]
     L.mww_import_streams.restype = i32
     L.mww_import_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), vp]
+    L.mww_set_input_rate.restype = i32
+    L.mww_set_input_rate.argtypes = [vp, i32]
+    L.mww_get_input_rate.restype = i32
+    L.mww_get_input_rate.argtypes = [vp, pi, ctypes.POINTER(ll)]
+    L.mww_get_resampler_state.restype = i32
+    L.mww_get_resampler_state.argtypes = [vp, vp, ctypes.POINTER(ll)]
+    L.mww_set_resampler_state.restype = i32
+    L.mww_set_resampler_state.argtypes = [vp, vp, ll]
+    L.mww_resample_taps.restype = i32
+    L.mww_resample_taps.argtypes = [i32, vp, i32, pi, pi, pi]
     _lib = L
     return L
 

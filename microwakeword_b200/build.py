@@ -11,6 +11,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmww_b200.so")
 SOURCES = ["mww_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_streams.cu", "mww_records.cu", "mww_detect.cu", "mww_tables.cc", "mww_container.cc"]
+# the input-rate resampler kernel (mww_set_input_rate) is a companion library that libmww_b200.so links (rpath $ORIGIN): the
+# main library's own kernel set stays the one the SASS fixtures under tests/golden/ record
+RS_OUT = os.path.join(HERE, "libmww_resample.so")
+RS_SOURCES = ["mww_resample.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -33,7 +37,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not os.path.exists(OUT) or not os.path.exists(STAMP):
+    if not os.path.exists(OUT) or not os.path.exists(RS_OUT) or not os.path.exists(STAMP):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -51,17 +55,19 @@ def build(force: bool = False, verbose: bool = False) -> str:
         fcntl.flock(lock, fcntl.LOCK_EX)
         if not force and not _stale():
             return OUT
-        tmp = OUT + ".tmp.%d" % os.getpid()
-        cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in SOURCES]
-        res = subprocess.run(cmd, capture_output=True, text=True)
-        if res.returncode != 0:
-            sys.stderr.write(res.stdout + res.stderr)
-            if os.path.exists(tmp):
-                os.unlink(tmp)
-            raise RuntimeError("nvcc failed building libmww_b200.so")
-        if verbose:
-            sys.stderr.write(res.stderr)
-        os.replace(tmp, OUT)                               # a process that has the old file mapped keeps its own copy
+        for out, sources, extra in ((RS_OUT, RS_SOURCES, []),
+                                    (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-Xlinker", "-rpath,$ORIGIN"])):
+            tmp = out + ".tmp.%d" % os.getpid()
+            cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra
+            res = subprocess.run(cmd, capture_output=True, text=True)
+            if res.returncode != 0:
+                sys.stderr.write(res.stdout + res.stderr)
+                if os.path.exists(tmp):
+                    os.unlink(tmp)
+                raise RuntimeError("nvcc failed building %s" % os.path.basename(out))
+            if verbose:
+                sys.stderr.write(res.stderr)
+            os.replace(tmp, out)                           # a process that has the old file mapped keeps its own copy
         with open(STAMP, "w") as f:
             f.write(source_hash() + "\n")
     return OUT

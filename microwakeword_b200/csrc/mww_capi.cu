@@ -76,6 +76,13 @@ struct mww_handle {
     uint32_t *d_estimate = nullptr;
     int used = 0;
     int hop = kHop;                 // samples between feature windows (mww_set_window_step; 160 = the 10 ms of every shipped model)
+    // input-rate resampler (mww_set_input_rate; mww_resample.h): none at 16 kHz
+    ResamplePlan rs;
+    int16_t *d_rs_table = nullptr;  // [L][pitch]
+    int16_t *d_rs_hist = nullptr;   // [n_streams][rs_hist_stride], the first H samples of each row used
+    int rs_hist_stride = 0;         // H rounded up to even: whole 4-byte words per stream (reset by id)
+    long long rs_seen = 0;          // input samples every stream has been given since the last full / frontend reset
+    int16_t *d_rs_out = nullptr; size_t rs_out_bytes = 0;     // one tile's 16 kHz samples
     // scratch
     uint32_t *d_v = nullptr; size_t v_bytes = 0;
     uint16_t *d_feat = nullptr; size_t feat_bytes = 0;
@@ -159,6 +166,36 @@ int ensure_scratch(mww_t *h, size_t v_bytes, size_t feat_bytes, size_t gather_by
         CU(h, cudaMalloc(&h->d_feat, feat_bytes));
         h->feat_bytes = feat_bytes;
     }
+    return MWW_OK;
+}
+
+bool resampling(const mww_t *h) { return h->rs.rate != 16000; }
+// 16 kHz samples a call of n input-rate samples gives every stream
+int samples16(const mww_t *h, int n) { return resampling(h) ? resample_call_outputs(h->rs_seen, n, h->rs.L, h->rs.M) : n; }
+// the resampler's index math is int32 in upsampled samples: a call must keep n L below 2^31 (about 100 s at 22.05 kHz)
+bool resample_call_fits(const mww_t *h, int n) { return !resampling(h) || (long long)n * h->rs.L + h->rs.M < (1ll << 31); }
+
+int ensure_rs_out(mww_t *h, size_t bytes) {
+    if (bytes <= h->rs_out_bytes) return MWW_OK;
+    if (h->d_rs_out) cudaFree(h->d_rs_out);
+    h->d_rs_out = nullptr; h->rs_out_bytes = 0;
+    CU(h, cudaMalloc(&h->d_rs_out, bytes));
+    h->rs_out_bytes = bytes;
+    return MWW_OK;
+}
+
+// streams [first, first + n) of a call of n_in input-rate samples -> their n16 16 kHz samples in h->d_rs_out [n][n16], each
+// stream's history moved on.  One launch; the caller advances h->rs_seen once the whole call is issued.
+template <typename T>
+int run_resample_tile(mww_t *h, int first, int n, const T *d_audio, long long audio_stride, int n_in, int n16, cudaStream_t st) {
+    if (n_in <= 0) return MWW_OK;
+    ResampleArgs a;
+    a.table = h->d_rs_table; a.hist = h->d_rs_hist + (size_t)first * h->rs_hist_stride; a.hist_stride = h->rs_hist_stride;
+    a.audio_stride = audio_stride; a.out_stride = n16;
+    a.L = h->rs.L; a.M = h->rs.M; a.T = h->rs.T; a.H = h->rs.H; a.pitch = h->rs.pitch;
+    a.t0 = resample_t0(h->rs_seen, h->rs.L, h->rs.M); a.n_in = n_in; a.n_out = n16; a.n_streams = n;
+    CU(h, launch_resample(a, d_audio, h->d_rs_out, h->sm_count, st));
+    h->launches += 1;
     return MWW_OK;
 }
 
@@ -456,7 +493,9 @@ int zero_frontend(mww_t *h, cudaStream_t st) {
     const size_t S = (size_t)h->n_streams;
     CU(h, cudaMemsetAsync(h->d_carry, 0, S * kWindow * sizeof(int16_t), st));
     CU(h, cudaMemsetAsync(h->d_estimate, 0, S * kNumChannels * sizeof(uint32_t), st));
+    if (h->d_rs_hist) CU(h, cudaMemsetAsync(h->d_rs_hist, 0, S * h->rs_hist_stride * sizeof(int16_t), st));
     h->used = 0;
+    h->rs_seen = 0;
     return MWW_OK;
 }
 
@@ -477,6 +516,7 @@ void destroy_impl(mww_t *h) {
     cudaFree(h->d_tables); cudaFree(h->d_carry); cudaFree(h->d_estimate);
     cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
     cudaFree(h->d_gather); cudaFree(h->d_cids);
+    cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist); cudaFree(h->d_rs_out);
     for (int b = 0; b < 2; ++b) {
         cudaFree(h->d_audio_tile[b]); cudaFree(h->d_probs_tile[b]);
         if (h->ev_h2d[b]) cudaEventDestroy(h->ev_h2d[b]);
@@ -498,25 +538,37 @@ int features_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, lo
                   int *h_rows_out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (!resample_call_fits(h, n_samples)) return fail(h, MWW_EINVAL, std::string(who) + ": call too long for the resampler; split it");
     ENTER_STATEFUL(h);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    const int n_frames = frames_for(h, n_samples);
+    const int n16 = samples16(h, n_samples);
+    const int n_frames = frames_for(h, n16);
     if (n_frames > max_rows || (n_frames > 0 && !d_feat))
         return fail(h, MWW_EINVAL, std::string(who) + ": feature buffer too small for the rows this call emits");
-    const int tile = tile_streams(h, n_frames, false);
+    const int tile = tile_streams(h, n_frames, false, resampling(h) ? (size_t)n16 * 2 : 0);
     int rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), 0);
+    if (rc == MWW_OK && resampling(h)) rc = ensure_rs_out(h, (size_t)tile * std::max(n16, 1) * 2);
     if (rc) return rc;
     for (int first = 0; first < h->n_streams; first += tile) {
         const int n = std::min(tile, h->n_streams - first);
+        uint16_t *feat = d_feat + (size_t)first * max_rows * kNumChannels;
+        if (resampling(h)) {
+            // the tile's 16 kHz samples, then the int16 frontend and window carry on them
+            if ((rc = run_resample_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n16, st))) return rc;
+            if ((rc = run_frontend_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, feat, (long long)max_rows * kNumChannels, st))) return rc;
+            if (n16 > 0 && (rc = run_carry_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, st))) return rc;
+            continue;
+        }
         rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames,
-                               d_feat + (size_t)first * max_rows * kNumChannels, (long long)max_rows * kNumChannels, st);
+                               feat, (long long)max_rows * kNumChannels, st);
         if (rc) return rc;
     }
-    if (n_samples > 0) {
+    if (n_samples > 0 && !resampling(h)) {
         rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
         if (rc) return rc;
     }
-    h->used = h->used + n_samples - n_frames * h->hop;
+    h->used = h->used + n16 - n_frames * h->hop;
+    if (resampling(h)) h->rs_seen += n_samples;
     if (h_rows_out) *h_rows_out = n_frames;
     return MWW_OK;
 }
@@ -591,15 +643,18 @@ int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples
     if (!h) return MWW_EINVAL;
     if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
     if (h->models.empty()) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
+    if (!resample_call_fits(h, n_samples)) return fail(h, MWW_EINVAL, std::string(who) + ": call too long for the resampler; split it");
     ENTER_STATEFUL(h);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    const int n_frames = frames_for(h, n_samples);
+    const int n16 = samples16(h, n_samples);
+    const int n_frames = frames_for(h, n16);
     NnOuts o;
     int rc = check_outs(h, who, n_frames, d_probs, max_probs, &o);
     if (rc) return rc;
     const size_t gather = gather_bytes_per_stream(h, n_frames);
-    const int tile = tile_streams(h, n_frames, true, gather);
+    const int tile = tile_streams(h, n_frames, true, gather + (resampling(h) ? (size_t)n16 * 2 : 0));
     rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2, (size_t)tile * gather);
+    if (rc == MWW_OK && resampling(h)) rc = ensure_rs_out(h, (size_t)tile * std::max(n16, 1) * 2);
     if (rc) return rc;
     rc = begin_models_call(h, n_frames, st);
     if (rc) return rc;
@@ -610,20 +665,28 @@ int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples
     for (size_t k = 0; k < K; ++k) probs_stride[k] = max_probs[k];
     for (int first = 0; first < h->n_streams; first += tile) {
         const int n = std::min(tile, h->n_streams - first);
-        rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames, h->d_feat,
-                               (long long)n_frames * kNumChannels, st);
+        if (resampling(h)) {
+            rc = run_resample_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n16, st);
+            if (rc == MWW_OK) rc = run_frontend_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, h->d_feat, (long long)n_frames * kNumChannels, st);
+        } else {
+            rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames, h->d_feat,
+                                   (long long)n_frames * kNumChannels, st);
+        }
         if (rc) return rc;
         tile_spans(h, first, n, span);
         for (size_t k = 0; k < K; ++k) tile_probs[k] = d_probs[k] + (size_t)span[k].a * max_probs[k];
         rc = run_models_tile(h, first, n_frames, span, tile_probs, probs_stride, st);
         if (rc) return rc;
+        // a resampling handle's carry update reads the tile's 16 kHz samples, so it runs per tile
+        if (resampling(h) && n16 > 0 && (rc = run_carry_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, st))) return rc;
     }
     end_models_call(h, n_frames, o, h_probs_out);
-    if (n_samples > 0) {
+    if (n_samples > 0 && !resampling(h)) {
         rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
         if (rc) return rc;
     }
-    h->used = h->used + n_samples - n_frames * h->hop;
+    h->used = h->used + n16 - n_frames * h->hop;
+    if (resampling(h)) h->rs_seen += n_samples;
     return MWW_OK;
 }
 
@@ -933,6 +996,7 @@ int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
     if (n <= 0) return MWW_OK;
     int rc = fill_by_id(h, h->d_carry, kWindow * sizeof(int16_t), d_ids, n, h->n_streams, st);
     if (rc == MWW_OK) rc = fill_by_id(h, h->d_estimate, kNumChannels * sizeof(uint32_t), d_ids, n, h->n_streams, st);
+    if (rc == MWW_OK && h->d_rs_hist) rc = fill_by_id(h, h->d_rs_hist, (size_t)h->rs_hist_stride * sizeof(int16_t), d_ids, n, h->n_streams, st);
     for (size_t k = 0; rc == MWW_OK && k < h->models.size(); ++k) {
         Model &m = h->models[k];
         if (m.members() == h->n_streams) {
@@ -988,6 +1052,83 @@ int mww_reset_frontend(mww_t *h, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     ENTER_STATEFUL(h);
     return zero_frontend(h, static_cast<cudaStream_t>(cu_stream));
+}
+
+int mww_resample_taps(int rate, int32_t *out, int max_taps, int *n_taps, int *L, int *M) {
+    ResamplePlan P;
+    if (!resample_plan(rate, &P)) { g_create_error = "mww_resample_taps: unsupported input rate"; return MWW_EUNSUPPORTED; }
+    if (n_taps) *n_taps = P.n_taps;
+    if (L) *L = P.L;
+    if (M) *M = P.M;
+    if (!out || max_taps < P.n_taps) return MWW_OK;
+    if (!resample_taps(P, out)) { g_create_error = "mww_resample_taps: a phase breaks the partial-sum bound"; return MWW_EINVAL; }
+    return MWW_OK;
+}
+
+int mww_set_input_rate(mww_t *h, int rate) {
+    if (!h) return MWW_EINVAL;
+    ResamplePlan P;
+    if (!resample_plan(rate, &P))
+        return fail(h, MWW_EUNSUPPORTED, "mww_set_input_rate: the input rate must be one of 8000, 16000, 22050, 24000, 32000, 44100, 48000 Hz");
+    if (h->used != 0 || h->rs_seen != 0)
+        return fail(h, MWW_EINVAL, "mww_set_input_rate: the frontend holds buffered samples; reset it first");
+    ENTER_STATEFUL(h);
+    int16_t *table = nullptr, *hist = nullptr;
+    const int hist_stride = (P.H + 1) / 2 * 2;
+    if (P.n_taps > 0) {
+        std::vector<int32_t> taps((size_t)P.n_taps);
+        if (!resample_taps(P, taps.data())) return fail(h, MWW_EINVAL, "mww_set_input_rate: a phase breaks the partial-sum bound");
+        std::vector<int16_t> host((size_t)P.L * P.pitch);
+        resample_table(P, taps.data(), host.data());
+        const size_t hist_bytes = (size_t)h->n_streams * hist_stride * sizeof(int16_t);
+        cudaError_t e = cudaMalloc(&table, host.size() * sizeof(int16_t));
+        if (e == cudaSuccess) e = cudaMalloc(&hist, hist_bytes);
+        if (e == cudaSuccess) e = cudaMemcpy(table, host.data(), host.size() * sizeof(int16_t), cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaMemset(hist, 0, hist_bytes);
+        if (e != cudaSuccess) {
+            cudaFree(table); cudaFree(hist);
+            return fail(h, e == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("mww_set_input_rate: ") + cudaGetErrorString(e));
+        }
+    }
+    // earlier calls may still read the old table and history
+    if (h->d_rs_table || h->d_rs_hist) CU(h, cudaDeviceSynchronize());
+    cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist);
+    h->d_rs_table = table; h->d_rs_hist = hist;
+    h->rs_hist_stride = P.n_taps > 0 ? hist_stride : 0;
+    h->rs = P;
+    h->rs_seen = 0;
+    return MWW_OK;
+}
+
+int mww_get_input_rate(const mww_t *h, int *rate, long long *inputs_seen) {
+    if (!h) return MWW_EINVAL;
+    if (rate) *rate = h->rs.rate;
+    if (inputs_seen) *inputs_seen = h->rs_seen;
+    return MWW_OK;
+}
+
+int mww_get_resampler_state(mww_t *h, int16_t *h_history, long long *inputs_seen) {
+    if (!h) return MWW_EINVAL;
+    ENTER_STATEFUL(h);
+    if (inputs_seen) *inputs_seen = h->rs_seen;
+    if (!h_history || !resampling(h)) return MWW_OK;
+    CU(h, cudaDeviceSynchronize());
+    CU(h, cudaMemcpy2D(h_history, (size_t)h->rs.H * 2, h->d_rs_hist, (size_t)h->rs_hist_stride * 2, (size_t)h->rs.H * 2, h->n_streams,
+                       cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+
+int mww_set_resampler_state(mww_t *h, const int16_t *h_history, long long inputs_seen) {
+    if (!h) return MWW_EINVAL;
+    if (inputs_seen < 0 || (!resampling(h) && inputs_seen != 0))
+        return fail(h, MWW_EINVAL, "mww_set_resampler_state: inputs_seen out of range (always 0 at 16 kHz)");
+    ENTER(h);
+    CU(h, cudaDeviceSynchronize());
+    if (h_history && resampling(h))
+        CU(h, cudaMemcpy2D(h->d_rs_hist, (size_t)h->rs_hist_stride * 2, h_history, (size_t)h->rs.H * 2, (size_t)h->rs.H * 2, h->n_streams,
+                           cudaMemcpyHostToDevice));
+    h->rs_seen = inputs_seen;
+    return MWW_OK;
 }
 
 int mww_features(mww_t *h, const int16_t *d_audio, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
@@ -1078,7 +1219,7 @@ size_t probs_tile_offset(const mww_t *h, const NnOuts &o, int tile, size_t k) {
 // that sample type convert them (as on the device path)
 template <typename T>
 int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, const NnOuts &o, bool dst_is_host,
-                 int tile, int n_frames) {
+                 int tile, int n_frames, int n16) {
     const size_t K = h->models.size();
     const T *audio_tile[2] = {static_cast<const T *>(h->d_audio_tile[0]), static_cast<const T *>(h->d_audio_tile[1])};
     float *tile_probs[kMaxModels];
@@ -1110,15 +1251,23 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
         CU(h, cudaStreamWaitEvent(h->st_compute, h->ev_h2d[b], 0));
         if (tl[2]) CU(h, cudaEventRecord(tl[2], h->st_compute));
         if (dst_is_host && it >= 2) CU(h, cudaStreamWaitEvent(h->st_compute, h->ev_d2h[b], 0));   // score staging buffer drained
-        int rc = run_frontend_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
+        int rc = MWW_OK;
+        if (resampling(h)) {
+            // one 16 kHz scratch serves every tile: all kernels run in order on the compute stream
+            rc = run_resample_tile(h, first, n, audio_tile[b], n_samples, n_samples, n16, h->st_compute);
+            if (rc == MWW_OK) rc = run_frontend_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
+        } else {
+            rc = run_frontend_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
+        }
         if (rc) return rc;
         tile_spans(h, first, n, span);
         for (size_t k = 0; k < K; ++k)
             tile_probs[k] = dst_is_host ? h->d_probs_tile[b] + probs_tile_offset(h, o, tile, k) : o.probs[k] + (size_t)span[k].a * o.max_probs[k];
         rc = run_models_tile(h, first, n_frames, span, tile_probs, tile_probs_stride, h->st_compute);
         if (rc) return rc;
-        if (n_samples > 0) {
-            rc = run_carry_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->st_compute);
+        if (resampling(h) ? n16 > 0 : n_samples > 0) {
+            rc = resampling(h) ? run_carry_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, h->st_compute)
+                               : run_carry_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->st_compute);
             if (rc) return rc;
         }
         if (tl[3]) CU(h, cudaEventRecord(tl[3], h->st_compute));
@@ -1141,7 +1290,9 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
 template <typename T>
 int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, long long audio_stride, float *const *dst,
                         const int *max_probs, int *h_probs_out, bool dst_is_host, int want_tiles, cudaStream_t caller, bool host_sync) {
-    const int n_frames = frames_for(h, n_samples);
+    if (!resample_call_fits(h, n_samples)) return fail(h, MWW_EINVAL, std::string(who) + ": call too long for the resampler; split it");
+    const int n16 = samples16(h, n_samples);
+    const int n_frames = frames_for(h, n16);
     NnOuts o;
     int rc = check_outs(h, who, n_frames, dst, max_probs, &o);
     if (rc) return rc;
@@ -1153,11 +1304,15 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
     if (want_tiles <= 0) want_tiles = 16;
     // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
     // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone
+    // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
+    // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone.  A resampling handle adds its
+    // 16 kHz tile scratch.
     const size_t staged_bytes = sizeof(T) == sizeof(int16_t) ? 0 : 2 * (size_t)std::max(n_samples, 1) * sizeof(T);
     const size_t gather = gather_bytes_per_stream(h, n_frames);
-    int tile = tile_streams(h, n_frames, true, staged_bytes + gather);
+    int tile = tile_streams(h, n_frames, true, staged_bytes + gather + (resampling(h) ? (size_t)n16 * 2 : 0));
     tile = std::max(1, std::min(tile, std::max((h->n_streams + want_tiles - 1) / want_tiles, std::min(h->n_streams, h->min_tile_streams))));
     rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2, (size_t)tile * gather);
+    if (rc == MWW_OK && resampling(h)) rc = ensure_rs_out(h, (size_t)tile * std::max(n16, 1) * 2);
     if (rc) return rc;
     const size_t a_bytes = (size_t)tile * std::max(n_samples, 1) * sizeof(T);
     const size_t p_bytes = dst_is_host ? probs_tile_offset(h, o, tile, h->models.size()) * sizeof(float) : 0;
@@ -1187,7 +1342,7 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
     rc = begin_models_call(h, n_frames, h->st_compute);
     if (rc == MWW_OK) {
         h->staged_used = true;
-        rc = staged_tiles(h, src, n_samples, audio_stride, o, dst_is_host, tile, n_frames);
+        rc = staged_tiles(h, src, n_samples, audio_stride, o, dst_is_host, tile, n_frames, n16);
     }
     if (rc != MWW_OK) {
         // some tiles' carry / ring state may already be updated, others not: drain and refuse further stateful calls
@@ -1205,7 +1360,8 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
         CU(h, cudaStreamWaitEvent(caller, h->ev_exit, 0));
     }
     end_models_call(h, n_frames, o, h_probs_out);
-    h->used = h->used + n_samples - n_frames * h->hop;
+    h->used = h->used + n16 - n_frames * h->hop;
+    if (resampling(h)) h->rs_seen += n_samples;
     return MWW_OK;
 }
 
@@ -1623,6 +1779,7 @@ int mww_stream_layout_get(const mww_t *h, mww_stream_layout *out) {
 
 int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
+    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_export_streams: stream records do not carry resampler history (input rate != 16000)");
     if (int rc = check_record_args(h, "mww_export_streams", h_ids, n, d_records)) return rc;
     ENTER_STATEFUL(h);
     if (out) fill_stream_layout(h, out);
@@ -1644,6 +1801,7 @@ int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, m
 
 int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout, void *cu_stream) {
     if (!h) return MWW_EINVAL;
+    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_import_streams: stream records do not carry resampler history (input rate != 16000)");
     if (!layout) return fail(h, MWW_EINVAL, "mww_import_streams: bad arguments");
     if (int rc = check_record_args(h, "mww_import_streams", h_ids, n, d_records)) return rc;
     std::vector<uint8_t> listed((size_t)h->n_streams, 0);

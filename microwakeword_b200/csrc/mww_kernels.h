@@ -109,6 +109,14 @@ cudaError_t launch_remap_rows(void *dst, const void *src, size_t bytes_per_row, 
 cudaError_t launch_compact_ids(int32_t *out, const int32_t *ids, int n, const int32_t *inv, int n_streams, int sm_count, cudaStream_t st);
 }  // namespace mww
 
+#include "mww_resample.h"
+namespace mww {
+// input-rate resampler (mww_resample.cu, definition and index math in mww_resample.h): a tile's input samples -> its 16 kHz
+// int16 samples out [n_streams][out_stride], history moved on.  T = int16_t or float (pcm16_from_f32 on load).
+template <typename T>
+cudaError_t launch_resample(const ResampleArgs &a, const T *audio, int16_t *out, int sm_count, cudaStream_t st);
+}  // namespace mww
+
 #include "mww_records.h"
 namespace mww {
 // stream records (mww_records.cu, layout and index math in mww_records.h): the parts of job J of the n streams ids[0, n)

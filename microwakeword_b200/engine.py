@@ -84,13 +84,29 @@ def rows_for(buffered: int, n_samples: int, hop: int) -> int:
     return (buffered + n_samples - WINDOW) // hop + 1 if buffered + n_samples >= WINDOW else 0
 
 
-def call_plan(buffered: int, n_samples: int, hop: int, pending_rows, strides):
+INPUT_RATES = (8000, 16000, 22050, 24000, 32000, 44100, 48000)
+
+
+def samples16(inputs_seen: int, n_samples: int, input_rate: int = 16000) -> int:
+    """16 kHz samples a call of n_samples at `input_rate` yields after inputs_seen input samples (mww_set_input_rate):
+    ceil((seen + n) L / M) - ceil(seen L / M) with L / M = 16000 / input_rate"""
+    if input_rate == 16000:
+        return int(n_samples)
+    from math import gcd
+    g = gcd(16000, int(input_rate))
+    L, M = 16000 // g, int(input_rate) // g
+    return -(-(inputs_seen + n_samples) * L // M) + (-inputs_seen * L // M)
+
+
+def call_plan(buffered: int, n_samples: int, hop: int, pending_rows, strides, input_rate: int = 16000, inputs_seen: int = 0):
     """Bookkeeping of one call on a shared frontend feeding models of the given strides, each holding pending_rows[k]:
-    -> (rows emitted, [steps model k runs], samples buffered after the call, [rows model k holds after the call])."""
-    rows = rows_for(buffered, n_samples, hop)
+    -> (rows emitted, [steps model k runs], samples buffered after the call, [rows model k holds after the call]).
+    n_samples is at `input_rate`, after `inputs_seen` input samples; the frontend sees samples16() of them."""
+    n16 = samples16(inputs_seen, n_samples, input_rate)
+    rows = rows_for(buffered, n16, hop)
     steps = [(p + rows) // s for p, s in zip(pending_rows, strides)]
     pending = [(p + rows) % s for p, s in zip(pending_rows, strides)]
-    return rows, steps, buffered + n_samples - rows * hop, pending
+    return rows, steps, buffered + n16 - rows * hop, pending
 
 
 class StreamRecords:
@@ -154,6 +170,53 @@ class _Engine:
     @property
     def frontend_buffered(self) -> int:
         return self._info().frontend_buffered
+
+    @property
+    def input_rate(self) -> int:
+        return self._rate()[0]
+
+    def _rate(self):
+        """-> (input rate, input samples seen since the last reset)"""
+        rate, seen = ctypes.c_int(0), ctypes.c_longlong(0)
+        _lib.check(self._h, self._L.mww_get_input_rate(self._h, ctypes.byref(rate), ctypes.byref(seen)))
+        return rate.value, seen.value
+
+    def _samples16(self, n_samples: int) -> int:
+        rate, seen = self._rate()
+        return samples16(seen, n_samples, rate)
+
+    def set_input_rate(self, rate: int):
+        """Sample rate of the audio this engine is given (mww_set_input_rate): one of INPUT_RATES, 16000 by default.  Any other
+        rate is resampled to 16 kHz on the GPU in front of the frontend; every call then takes samples at this rate.  Only
+        while no samples are buffered (after create / reset / reset_frontend)."""
+        _lib.check(self._h, self._L.mww_set_input_rate(self._h, int(rate)))
+
+    def resampler_history(self) -> int:
+        """input samples each stream keeps as resampler history (0 at 16 kHz)"""
+        rate = self.input_rate
+        n, L = ctypes.c_int(0), ctypes.c_int(1)
+        _lib.check(None, self._L.mww_resample_taps(rate, None, 0, ctypes.byref(n), ctypes.byref(L), None))
+        return -(-n.value // L.value)
+
+    def _get_resampler(self, d: dict) -> None:
+        """the resampler's part of state_dict (nothing at 16 kHz)"""
+        if self.input_rate == 16000:
+            return
+        hist = np.zeros((self.n_streams, self.resampler_history()), np.int16)
+        seen = ctypes.c_longlong(0)
+        _lib.check(self._h, self._L.mww_get_resampler_state(self._h, hist.ctypes.data, ctypes.byref(seen)))
+        d.update(input_rate=self.input_rate, resampler_history=hist, inputs_seen=seen.value)
+
+    def _set_resampler(self, d: dict) -> None:
+        rate = int(d.get("input_rate", 16000))
+        if rate != self.input_rate:
+            raise ValueError("the state was taken at %d Hz, this engine runs at %d Hz" % (rate, self.input_rate))
+        if rate == 16000:
+            return
+        hist = np.ascontiguousarray(d["resampler_history"], np.int16)
+        if hist.shape != (self.n_streams, self.resampler_history()):
+            raise ValueError("resampler_history must be int16 [n_streams, %d]" % self.resampler_history())
+        _lib.check(self._h, self._L.mww_set_resampler_state(self._h, hist.ctypes.data, int(d["inputs_seen"])))
 
     @property
     def launch_count(self) -> int:
@@ -232,7 +295,7 @@ class _Engine:
         """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer."""
         torch = _torch()
         n, stride, is_f32 = self._check_audio(audio)
-        rows = rows_for(self.frontend_buffered, n, self.hop)
+        rows = rows_for(self.frontend_buffered, self._samples16(n), self.hop)
         if out is None:
             out = torch.empty((self.n_streams, max(rows, 1), NUM_FEATURES), dtype=torch.uint16, device=self._dev())
         elif (out.dtype != torch.uint16 or not out.is_cuda or not out.is_contiguous() or out.dim() != 3 or out.shape[0] != self.n_streams
@@ -320,7 +383,7 @@ class StreamEngine(_Engine):
     """`model`: path to (or bytes of) an MWW container or a streaming ``.tflite`` flatbuffer (recognised and converted by
     ``tflite_file``, inference.py:36-45), or None for a frontend-only engine."""
 
-    def __init__(self, model, n_streams: int = 1, device: int = 0):
+    def __init__(self, model, n_streams: int = 1, device: int = 0, input_rate: int = 16000):
         blob = load_model_blob(model)
         self._L = _lib.lib()
         self._h = ctypes.c_void_p()
@@ -337,13 +400,15 @@ class StreamEngine(_Engine):
         self.stride = max(int(self.info.input_feature_slices), 1)
         self.state_elements = int(self.info.state_bytes_per_stream) // (1 if self.is_quantized else 4) if blob is not None else 0
         self.hop = HOP          # samples between feature windows (set_window_step)
+        if input_rate != 16000:
+            self.set_input_rate(input_rate)
 
     @property
     def pending_rows(self) -> int:
         return self._info().pending_rows
 
     def _steps(self, n_samples: int) -> int:
-        return (self.pending_rows + rows_for(self.frontend_buffered, n_samples, self.hop)) // self.stride
+        return (self.pending_rows + rows_for(self.frontend_buffered, self._samples16(n_samples), self.hop)) // self.stride
 
     def infer(self, rows):
         """feature rows [S, R, 40] (uint16 / float32 / int8 CUDA tensor) -> float32 probabilities [S, steps]."""
@@ -440,9 +505,11 @@ class StreamEngine(_Engine):
         info = self._info()
         d["frontend_buffered"] = info.frontend_buffered
         d["pending_rows"] = info.pending_rows
+        self._get_resampler(d)
         return d
 
     def load_state_dict(self, d: dict) -> None:
+        self._set_resampler(d)
         nn_dtype = np.int8 if self.is_quantized else np.float32
         carry = np.ascontiguousarray(d["carry"], np.int16)
         est = np.ascontiguousarray(d["estimate"], np.uint32)
@@ -466,7 +533,7 @@ class MultiModelEngine(_Engine):
     them only, and its results have one row per id, in that order (row j belongs to stream streams[k][j]).  Unsorted,
     duplicate or out-of-range ids raise ValueError.  `engine.streams[k]` is model k's set (int32), `set_streams` changes it."""
 
-    def __init__(self, models, n_streams: int = 1, device: int = 0, streams=None):
+    def __init__(self, models, n_streams: int = 1, device: int = 0, streams=None, input_rate: int = 16000):
         blobs = [load_model_blob(m) for m in models]
         if any(b is None for b in blobs):
             raise ValueError("every model must be a path or the bytes of a model file")
@@ -498,6 +565,8 @@ class MultiModelEngine(_Engine):
         self.state_elements = [int(i.state_bytes_per_stream) // (1 if q else 4) for i, q in zip(infos, self.is_quantized)]
         self.hop = HOP
         self.streams = [self._get_streams(k) for k in range(K)]
+        if input_rate != 16000:
+            self.set_input_rate(input_rate)
 
     @staticmethod
     def _stream_set(ids, n_streams: int) -> np.ndarray:
@@ -537,7 +606,8 @@ class MultiModelEngine(_Engine):
         return [self._model_info(k).pending_rows for k in range(self.n_models)]
 
     def _steps(self, n_samples: int) -> list:
-        return call_plan(self.frontend_buffered, n_samples, self.hop, self.pending_rows, self.stride)[1]
+        rate, seen = self._rate()
+        return call_plan(self.frontend_buffered, n_samples, self.hop, self.pending_rows, self.stride, rate, seen)[1]
 
     def _outs(self, steps, out, host: bool):
         """-> (K buffers, their ctypes pointer / max_probs / steps-out arrays); model k's buffer has one row per stream of
@@ -609,12 +679,14 @@ class MultiModelEngine(_Engine):
             _lib.check(self._h, self._L.mww_get_model_state(self._h, k, m["nn"].ctypes.data, m["pending"].ctypes.data))
             m["pending_rows"] = self._model_info(k).pending_rows
             d["models"].append(m)
+        self._get_resampler(d)
         return d
 
     def load_state_dict(self, d: dict) -> None:
         """the state of state_dict(); each model's stream set is restored first (a state without `streams`: all streams)"""
         if len(d["models"]) != self.n_models:
             raise ValueError("the state holds %d models, this engine %d" % (len(d["models"]), self.n_models))
+        self._set_resampler(d)
         carry = np.ascontiguousarray(d["carry"], np.int16)
         est = np.ascontiguousarray(d["estimate"], np.uint32)
         for k, m in enumerate(d["models"]):
