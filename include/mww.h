@@ -455,6 +455,56 @@ int mww_host_alloc_wc(size_t bytes, int device, void **h_ptr, int *numa_node_out
 int mww_host_free(void *h_ptr);
 int mww_bind_host_thread(int device, int *numa_node_out);
 
+/* ---- Streaming detector: probabilities in, detections out, state carried across calls ---------------------------------
+ * The rule the reference's ROC numbers are made with (microwakeword/test.py:337-341 and :118-135), per row and live.  A
+ * detector is its own object, not part of a handle: it consumes any probability buffer [n_rows][pitch] -- what
+ * mww_predict_clip*, mww_infer_features and the _multi calls write -- and no other call knows of it.
+ *
+ * One (window, cutoff, cooldown_slices) for all rows; per row the last window - 1 probabilities (hist, oldest first,
+ * zeros after a reset), `seen` (probabilities consumed since the row's last reset) and `cooldown` (cooldown_slices after a
+ * reset).  Feeding a row p[0], p[1], ... over any number of calls, split anywhere, gives what mww_false_accept_counts gives
+ * on the whole sequence: with avg[i] = mean(p[i .. i + window)) in float32 (sequential sum oldest first, one division),
+ * for i = 0, 1, ...: cooldown = max(cooldown - 1, 0); if cooldown == 0 and (double)avg[i] > cutoff the row fires and
+ * cooldown = cooldown_slices.  A detection at i is an event with step = i + window - 1, the index since reset of the newest
+ * probability of the window, and score = avg[i].  Nothing happens (no average, no cooldown tick) before a row has seen
+ * `window` probabilities.  NaN never fires.  window = 1 is the plain threshold.
+ *
+ * Events of all rows are appended to one device buffer of `capacity` events through a device counter.  The counter keeps
+ * counting past capacity: those events are dropped, per-row state advances all the same, and mww_detector_drain reports
+ * the true count.  Events of one update call are in no particular order; events of different calls are in call order.
+ * event.stream is the row index, or h_stream_ids[row] when the detector was created with a map (model k of a handle with
+ * stream sets scores its members in list order: pass the list mww_get_model_streams returns).
+ * Beside the events, d_fired [capacity] int32 holds the stream of each used event slot and -1 in every other slot, so
+ * mww_reset_device_ids(h, d_fired, capacity, stream) restarts exactly the streams that fired since the last drain.
+ *
+ *   - create: 1 <= n_rows, 1 <= window <= 32, cooldown_slices >= 0, finite cutoff, capacity >= 1, else MWW_EINVAL; without
+ *     a CUDA device MWW_ECUDA ("no CUDA device").  Messages of every detector call go to mww_last_error(NULL).
+ *   - update: asynchronous on cu_stream; the first n_steps columns of each row are consumed; n_steps == 0 launches
+ *     nothing; pitch >= n_steps.
+ *   - drain: synchronises cu_stream, copies min(count, capacity, max_events) events to h_events (may be NULL with
+ *     max_events 0), *n_events = events fired since the last drain, then clears the counter and refills d_fired with -1.
+ *   - buffers: device views for callers that stay on the GPU (each out pointer may be NULL).
+ *   - reset / reset_device: fresh state for all rows (NULL list) or the listed ROW indices (host / device memory; indices
+ *     out of range are ignored, a row listed twice is reset once more to the same state); a constant number of launches.
+ *     Events already in the buffer stay.
+ *   - get_state / set_state: host buffers, synchronous (they synchronise the device), NULL pointers skipped;
+ *     hist [n_rows][window - 1] oldest first, seen [n_rows], cooldown [n_rows].  set_state refuses (MWW_EINVAL) a negative
+ *     seen or a cooldown outside [0, cooldown_slices]. */
+typedef struct mww_detector mww_detector_t;
+typedef struct mww_event { int32_t stream, reserved; int64_t step; float score; int32_t pad; } mww_event;
+
+int mww_detector_create(int device, int n_rows, int window, double cutoff, int cooldown_slices, int capacity,
+                        const int32_t *h_stream_ids, mww_detector_t **out);
+int mww_detector_destroy(mww_detector_t *d);
+int mww_detector_update(mww_detector_t *d, const float *d_probs, int n_steps, long long pitch, void *cu_stream);
+int mww_detector_drain(mww_detector_t *d, mww_event *h_events, int max_events, long long *n_events, void *cu_stream);
+int mww_detector_buffers(mww_detector_t *d, const long long **d_count, const mww_event **d_events, const int32_t **d_fired,
+                         int *capacity);
+int mww_detector_reset(mww_detector_t *d, const int32_t *h_rows, int n, void *cu_stream);
+int mww_detector_reset_device(mww_detector_t *d, const int32_t *d_rows, int n, void *cu_stream);
+int mww_detector_get_state(mww_detector_t *d, float *h_hist, long long *h_seen, int32_t *h_cooldown);
+int mww_detector_set_state(mww_detector_t *d, const float *h_hist, const long long *h_seen, const int32_t *h_cooldown);
+
 #ifdef __cplusplus
 }
 #endif

@@ -30,6 +30,8 @@ EXPORTS = (
     "mww_create_multi_streams", "mww_set_model_streams", "mww_get_model_streams",
     "mww_stream_layout_get", "mww_export_streams", "mww_import_streams",
     "mww_set_input_rate", "mww_get_input_rate", "mww_get_resampler_state", "mww_set_resampler_state", "mww_resample_taps",
+    "mww_detector_create", "mww_detector_destroy", "mww_detector_update", "mww_detector_drain", "mww_detector_buffers",
+    "mww_detector_reset", "mww_detector_reset_device", "mww_detector_get_state", "mww_detector_set_state",
 )
 
 
@@ -52,6 +54,12 @@ class MwwStreamLayout(ctypes.Structure):
         ("hop_samples", ctypes.c_int32), ("pending_rows", ctypes.c_int32 * 64), ("model_hash", ctypes.c_uint64 * 64),
         ("rows_are_features", ctypes.c_uint8 * 64),
     ]
+
+
+class MwwEvent(ctypes.Structure):
+    """mww_event of include/mww.h: one detection of a streaming detector"""
+    _fields_ = [("stream", ctypes.c_int32), ("reserved", ctypes.c_int32), ("step", ctypes.c_int64), ("score", ctypes.c_float),
+                ("pad", ctypes.c_int32)]
 
 
 class MwwError(RuntimeError):
@@ -188,6 +196,22 @@ def lib() -> ctypes.CDLL:
     L.mww_set_resampler_state.argtypes = [vp, vp, ll]
     L.mww_resample_taps.restype = i32
     L.mww_resample_taps.argtypes = [i32, vp, i32, pi, pi, pi]
+    L.mww_detector_create.restype = i32
+    L.mww_detector_create.argtypes = [i32, i32, i32, ctypes.c_double, i32, i32, vp, ctypes.POINTER(vp)]
+    L.mww_detector_destroy.restype = i32
+    L.mww_detector_destroy.argtypes = [vp]
+    L.mww_detector_update.restype = i32
+    L.mww_detector_update.argtypes = [vp, vp, i32, ll, vp]
+    L.mww_detector_drain.restype = i32
+    L.mww_detector_drain.argtypes = [vp, vp, i32, ctypes.POINTER(ll), vp]
+    L.mww_detector_buffers.restype = i32
+    L.mww_detector_buffers.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp), pi]
+    for name in ("mww_detector_reset", "mww_detector_reset_device"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, vp]
+    for name in ("mww_detector_get_state", "mww_detector_set_state"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, vp, vp]
     _lib = L
     return L
 

@@ -15,6 +15,9 @@ SOURCES = ["mww_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww
 # main library's own kernel set stays the one the SASS fixtures under tests/golden/ record
 RS_OUT = os.path.join(HERE, "libmww_resample.so")
 RS_SOURCES = ["mww_resample.cu"]
+# likewise the streaming detector's kernels (mww_detector_*)
+DET_OUT = os.path.join(HERE, "libmww_detector.so")
+DET_SOURCES = ["mww_detector.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -37,7 +40,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not os.path.exists(OUT) or not os.path.exists(RS_OUT) or not os.path.exists(STAMP):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, DET_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -55,8 +58,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
         fcntl.flock(lock, fcntl.LOCK_EX)
         if not force and not _stale():
             return OUT
-        for out, sources, extra in ((RS_OUT, RS_SOURCES, []),
-                                    (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-Xlinker", "-rpath,$ORIGIN"])):
+        for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (DET_OUT, DET_SOURCES, []),
+                                    (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_detector", "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra
             res = subprocess.run(cmd, capture_output=True, text=True)

@@ -1841,3 +1841,187 @@ int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_reco
 }
 
 }  // extern "C"
+
+// ---- streaming detector (include/mww.h; rule and kernels: mww_detector.h, mww_detector.cu) -------------------------------
+// An object of its own: no handle knows of it, and its messages go where a failed create's go (mww_last_error(NULL)).
+struct mww_detector {
+    int device = 0;
+    DetectorArgs a;                  // the device state and buffers, as the kernels take them
+    int32_t *d_stream_ids = nullptr;
+    int32_t *d_rows = nullptr;       // staging for a host row list (mww_detector_reset)
+    size_t rows_cap = 0;
+};
+
+namespace {
+
+#define DCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(nullptr, e_, #call); } while (0)
+#define DENTER(d) DeviceGuard guard_((d)->device); if (guard_.err != cudaSuccess) return cuda_fail(nullptr, guard_.err, "cudaSetDevice")
+
+void detector_free(mww_detector_t *d) {
+    cudaFree(d->a.hist); cudaFree(d->a.seen); cudaFree(d->a.cooldown); cudaFree(d->a.count); cudaFree(d->a.events);
+    cudaFree(d->a.fired); cudaFree(d->d_stream_ids); cudaFree(d->d_rows);
+    delete d;
+}
+
+size_t detector_hist_elems(const mww_detector_t *d) { return (size_t)(d->a.rule.window - 1) * d->a.n_rows; }
+
+int detector_alloc(mww_detector_t *d, const int32_t *h_stream_ids) {
+    DetectorArgs &a = d->a;
+    const size_t R = (size_t)a.n_rows, C = (size_t)a.capacity;
+    DCU(cudaMalloc(&a.hist, std::max<size_t>(detector_hist_elems(d), 1) * sizeof(float)));
+    DCU(cudaMalloc(&a.seen, R * sizeof(long long)));
+    DCU(cudaMalloc(&a.cooldown, R * sizeof(int32_t)));
+    DCU(cudaMalloc(&a.count, sizeof(unsigned long long)));
+    DCU(cudaMalloc(&a.events, C * sizeof(mww_event)));
+    DCU(cudaMalloc(&a.fired, C * sizeof(int32_t)));
+    if (h_stream_ids) {
+        DCU(cudaMalloc(&d->d_stream_ids, R * sizeof(int32_t)));
+        DCU(cudaMemcpy(d->d_stream_ids, h_stream_ids, R * sizeof(int32_t), cudaMemcpyHostToDevice));
+        a.stream_ids = d->d_stream_ids;
+    }
+    DCU(cudaMemset(a.count, 0, sizeof(unsigned long long)));
+    DCU(cudaMemset(a.events, 0, C * sizeof(mww_event)));
+    DCU(cudaMemset(a.fired, 0xFF, C * sizeof(int32_t)));              // -1 in every slot
+    DCU(launch_detector_reset(a, nullptr, a.n_rows, nullptr));
+    DCU(cudaDeviceSynchronize());
+    return MWW_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mww_detector_create(int device, int n_rows, int window, double cutoff, int cooldown_slices, int capacity,
+                        const int32_t *h_stream_ids, mww_detector_t **out) {
+    if (!out) return fail(nullptr, MWW_EINVAL, "mww_detector_create: out is NULL");
+    *out = nullptr;
+    if (n_rows < 1) return fail(nullptr, MWW_EINVAL, "mww_detector_create: n_rows must be at least 1");
+    if (window < 1 || window > kDetectorMaxWindow) return fail(nullptr, MWW_EINVAL, "mww_detector_create: window must be in [1, 32]");
+    if (!(cutoff - cutoff == 0.0)) return fail(nullptr, MWW_EINVAL, "mww_detector_create: cutoff must be finite");
+    if (cooldown_slices < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_create: cooldown_slices must not be negative");
+    if (capacity < 1) return fail(nullptr, MWW_EINVAL, "mww_detector_create: capacity must be at least 1");
+    int count = 0;
+    cudaError_t e = cudaGetDeviceCount(&count);
+    if (e != cudaSuccess || count == 0)
+        return fail(nullptr, MWW_ECUDA, std::string("no CUDA device available (this library has no CPU fallback): ") + cudaGetErrorString(e));
+    if (device < 0 || device >= count) return fail(nullptr, MWW_EINVAL, "mww_detector_create: device index out of range");
+    DeviceGuard guard(device);
+    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+    mww_detector_t *d = new mww_detector;
+    d->device = device;
+    d->a.rule.window = window; d->a.rule.cutoff = cutoff; d->a.rule.cooldown_slices = cooldown_slices;
+    d->a.n_rows = n_rows; d->a.capacity = capacity;
+    if (int rc = detector_alloc(d, h_stream_ids)) { detector_free(d); return rc; }
+    *out = d;
+    return MWW_OK;
+}
+
+int mww_detector_destroy(mww_detector_t *d) {
+    if (!d) return MWW_OK;
+    DENTER(d);
+    cudaDeviceSynchronize();
+    detector_free(d);
+    return MWW_OK;
+}
+
+int mww_detector_update(mww_detector_t *d, const float *d_probs, int n_steps, long long pitch, void *cu_stream) {
+    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_update: detector is NULL");
+    if (n_steps < 0 || (n_steps > 0 && (!d_probs || pitch < n_steps)))
+        return fail(nullptr, MWW_EINVAL, "mww_detector_update: needs d_probs and n_steps >= 0 columns within the row pitch");
+    if (n_steps == 0) return MWW_OK;
+    DENTER(d);
+    DCU(launch_detector_update(d->a, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
+    return MWW_OK;
+}
+
+int mww_detector_drain(mww_detector_t *d, mww_event *h_events, int max_events, long long *n_events, void *cu_stream) {
+    if (!d || !n_events || max_events < 0 || (max_events > 0 && !h_events))
+        return fail(nullptr, MWW_EINVAL, "mww_detector_drain: needs a detector, n_events and room for max_events >= 0 events");
+    DENTER(d);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    unsigned long long count = 0;
+    DCU(cudaMemcpyAsync(&count, d->a.count, sizeof(count), cudaMemcpyDeviceToHost, st));
+    DCU(cudaStreamSynchronize(st));
+    const size_t stored = (size_t)std::min<unsigned long long>(count, (unsigned long long)d->a.capacity);
+    const size_t n = std::min(stored, (size_t)max_events);
+    if (n) DCU(cudaMemcpyAsync(h_events, d->a.events, n * sizeof(mww_event), cudaMemcpyDeviceToHost, st));
+    if (stored) {
+        DCU(cudaMemsetAsync(d->a.count, 0, sizeof(count), st));
+        DCU(cudaMemsetAsync(d->a.fired, 0xFF, stored * sizeof(int32_t), st));
+    }
+    if (n) DCU(cudaStreamSynchronize(st));
+    *n_events = (long long)count;
+    return MWW_OK;
+}
+
+int mww_detector_buffers(mww_detector_t *d, const long long **d_count, const mww_event **d_events, const int32_t **d_fired, int *capacity) {
+    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_buffers: detector is NULL");
+    if (d_count) *d_count = reinterpret_cast<const long long *>(d->a.count);
+    if (d_events) *d_events = d->a.events;
+    if (d_fired) *d_fired = d->a.fired;
+    if (capacity) *capacity = d->a.capacity;
+    return MWW_OK;
+}
+
+int mww_detector_reset_device(mww_detector_t *d, const int32_t *d_rows, int n, void *cu_stream) {
+    if (!d || n < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_reset_device: needs a detector and n >= 0");
+    DENTER(d);
+    DCU(launch_detector_reset(d->a, d_rows, d_rows ? n : d->a.n_rows, static_cast<cudaStream_t>(cu_stream)));
+    return MWW_OK;
+}
+
+int mww_detector_reset(mww_detector_t *d, const int32_t *h_rows, int n, void *cu_stream) {
+    if (!d || n < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_reset: needs a detector and n >= 0");
+    if (!h_rows) return mww_detector_reset_device(d, nullptr, 0, cu_stream);
+    if (n == 0) return MWW_OK;
+    DENTER(d);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if ((size_t)n > d->rows_cap) {                 // growing the staging buffer first waits for the reset that may still read it
+        if (d->d_rows) { DCU(cudaStreamSynchronize(st)); cudaFree(d->d_rows); d->d_rows = nullptr; d->rows_cap = 0; }
+        const size_t want = std::max<size_t>((size_t)n, 1024);
+        DCU(cudaMalloc(&d->d_rows, want * sizeof(int32_t)));
+        d->rows_cap = want;
+    }
+    DCU(cudaMemcpyAsync(d->d_rows, h_rows, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    DCU(launch_detector_reset(d->a, d->d_rows, n, st));
+    return MWW_OK;
+}
+
+int mww_detector_get_state(mww_detector_t *d, float *h_hist, long long *h_seen, int32_t *h_cooldown) {
+    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_get_state: detector is NULL");
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    const size_t R = (size_t)d->a.n_rows, W = (size_t)d->a.rule.window - 1;
+    if (h_hist && W) {                              // device [window - 1][n_rows] -> host [n_rows][window - 1]
+        std::vector<float> t(W * R);
+        DCU(cudaMemcpy(t.data(), d->a.hist, W * R * sizeof(float), cudaMemcpyDeviceToHost));
+        for (size_t j = 0; j < W; ++j)
+            for (size_t r = 0; r < R; ++r) h_hist[r * W + j] = t[j * R + r];
+    }
+    if (h_seen) DCU(cudaMemcpy(h_seen, d->a.seen, R * sizeof(long long), cudaMemcpyDeviceToHost));
+    if (h_cooldown) DCU(cudaMemcpy(h_cooldown, d->a.cooldown, R * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+
+int mww_detector_set_state(mww_detector_t *d, const float *h_hist, const long long *h_seen, const int32_t *h_cooldown) {
+    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: detector is NULL");
+    const size_t R = (size_t)d->a.n_rows, W = (size_t)d->a.rule.window - 1;
+    for (size_t r = 0; r < R; ++r) {
+        if (h_seen && h_seen[r] < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: seen must not be negative");
+        if (h_cooldown && (h_cooldown[r] < 0 || h_cooldown[r] > d->a.rule.cooldown_slices))
+            return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: cooldown outside [0, cooldown_slices]");
+    }
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    if (h_hist && W) {
+        std::vector<float> t(W * R);
+        for (size_t j = 0; j < W; ++j)
+            for (size_t r = 0; r < R; ++r) t[j * R + r] = h_hist[r * W + j];
+        DCU(cudaMemcpy(d->a.hist, t.data(), W * R * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    if (h_seen) DCU(cudaMemcpy(d->a.seen, h_seen, R * sizeof(long long), cudaMemcpyHostToDevice));
+    if (h_cooldown) DCU(cudaMemcpy(d->a.cooldown, h_cooldown, R * sizeof(int32_t), cudaMemcpyHostToDevice));
+    return MWW_OK;
+}
+
+}  // extern "C"

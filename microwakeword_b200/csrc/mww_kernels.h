@@ -128,3 +128,12 @@ cudaError_t launch_pack_streams(const RecordJob &J, void *records, long long rec
 cudaError_t launch_unpack_streams(const RecordJob &J, const void *records, long long record_bytes, const int32_t *ids, int n, void *const *base,
                                   const int32_t *inv, int32_t *fresh, int sm_count, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_detector.h"
+namespace mww {
+// streaming detector (mww_detector.cu, rule and kernel forms in mww_detector.h): every row consumes the first n_steps
+// columns of probs [n_rows][pitch]; thread per row below kDetectorWarpMinSteps steps, warp per row from there on
+cudaError_t launch_detector_update(const DetectorArgs &a, const float *probs, int n_steps, long long pitch, cudaStream_t st);
+// fresh state for the n listed rows (device memory; indices out of range ignored) or, rows == nullptr, for rows [0, n)
+cudaError_t launch_detector_reset(const DetectorArgs &a, const int32_t *rows, int n, cudaStream_t st);
+}  // namespace mww

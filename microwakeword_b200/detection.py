@@ -11,6 +11,10 @@ scores -- not every probability -- have to leave the GPU.
     false_rejection_rates(scores, cutoffs)    test.py:376-381
     generate_roc_curve(faph, frr, cutoffs)    test.py:140-204 (same name, arguments and quirks)
     streaming_model_roc(model, ambient, positives, ...)   the body of test.py:293-403 on spectrogram tracks
+
+Live, the same rule runs per stream with its state carried across calls:
+
+    StreamDetector(n_rows, cutoff, window=5, cooldown_slices=25)   probabilities in (update), detections out (drain)
 """
 
 from __future__ import annotations
@@ -220,3 +224,143 @@ def streaming_model_roc(model, ambient_spectrograms, positive_spectrograms, stri
     frr = false_rejection_rates(scores, cutoffs)
     x, y, c = generate_roc_curve(faph, frr, cutoffs)
     return dict(auc=roc_auc(x, y), faph=faph, frr=frr, cutoffs=cutoffs, roc=(x, y, c))
+
+
+# ---- the streaming detector ----------------------------------------------------------------------------------------------
+EVENT_DTYPE = np.dtype([("stream", np.int32), ("reserved", np.int32), ("step", np.int64), ("score", np.float32), ("pad", np.int32)])
+
+
+class _DetectorHandle:
+    """owner of one mww_detector_t: destroyed when the detector and every tensor over its buffers are gone"""
+
+    def __init__(self, L, ptr):
+        self.L, self.ptr = L, ptr
+
+    def close(self):
+        if self.ptr:
+            self.L.mww_detector_destroy(self.ptr)
+            self.ptr = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _DeviceArray:
+    """a span of a detector's device memory, as torch.as_tensor takes it; the tensor keeps this object, and through it the
+    detector's handle, alive"""
+
+    def __init__(self, handle: _DetectorHandle, ptr: int, n: int, typestr: str):
+        self.handle = handle
+        self.__cuda_array_interface__ = dict(shape=(n,), typestr=typestr, data=(ptr, False), version=2, strides=None)
+
+
+class StreamDetector:
+    """The detection rule of the reference's evaluation (moving average of `window` probabilities above `cutoff`, then
+    `cooldown_slices` steps of silence; test.py:337-341, :118-135) for `n_rows` live streams, state carried across calls
+    (mww_detector_* of include/mww.h).  A row's events over any sequence of update calls are those of false_accept_counts on
+    everything it was given; an event's `step` counts the row's probabilities since its last reset, `score` is the average
+    that fired.  It consumes what step() / predict_clip() return and knows nothing else of the engine:
+
+        det = StreamDetector(eng.n_streams, cutoff=0.9)
+        det.update(eng.step(chunk))            # nothing leaves the GPU
+        events, dropped = det.drain()          # now and then: a few events
+        eng.reset(det.fired_ids)               # before a drain: restart the streams that fired, no host round trip
+
+    `stream_ids`: event.stream of each row when it is not the row index (model k of an engine with stream sets scores its
+    members in list order: pass MultiModelEngine.streams[k]).  `capacity`: events kept between drains; more are
+    counted and dropped."""
+
+    def __init__(self, n_rows: int, cutoff: float, window: int = 5, cooldown_slices: int = 25, capacity: int = 65536,
+                 stream_ids=None, device: int = 0):
+        self._L = _lib.lib()
+        d = ctypes.c_void_p()
+        ids = None
+        if stream_ids is not None:
+            ids = np.ascontiguousarray(stream_ids, np.int32).reshape(-1)
+            if ids.size != int(n_rows):
+                raise ValueError("stream_ids must name one stream per row")
+        rc = self._L.mww_detector_create(int(device), int(n_rows), int(window), float(cutoff), int(cooldown_slices), int(capacity),
+                                         ids.ctypes.data if ids is not None else None, ctypes.byref(d))
+        self._check(rc)
+        self._handle = _DetectorHandle(self._L, d)
+        self.n_rows, self.window, self.cutoff, self.cooldown_slices = int(n_rows), int(window), float(cutoff), int(cooldown_slices)
+        self.capacity, self.device = int(capacity), int(device)
+        count, events, fired = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+        self._check(self._L.mww_detector_buffers(self._d, ctypes.byref(count), ctypes.byref(events), ctypes.byref(fired), None))
+        import torch
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(dev):
+            # device views: the stream of every event since the last drain (-1 in unused slots), and how many fired
+            self.fired_ids = torch.as_tensor(_DeviceArray(self._handle, fired.value, self.capacity, "<i4"), device=dev)
+            self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
+
+    def _check(self, rc: int) -> None:
+        if rc != 0:
+            msg = self._L.mww_last_error(None)
+            raise _lib.MwwError(rc, msg.decode() if msg else "detector call failed")
+
+    @property
+    def _d(self):
+        return self._handle.ptr
+
+    def close(self):
+        """free the detector now; fired_ids and event_count must not be used afterwards"""
+        self._handle.close()
+
+    def update(self, probs) -> None:
+        """CUDA float32 [n_rows, steps], any row pitch (a slice of a wider buffer is read in place); zero columns: nothing
+        happens.  Asynchronous on the current CUDA stream."""
+        import torch
+        if (not isinstance(probs, torch.Tensor) or not probs.is_cuda or probs.dtype != torch.float32 or probs.dim() != 2
+                or probs.shape[0] != self.n_rows or probs.device.index != self.device):
+            raise ValueError("probs must be a CUDA float32 tensor [n_rows=%d, steps] on device %d" % (self.n_rows, self.device))
+        n = probs.shape[1]
+        if n == 0:
+            return
+        if (n > 1 and probs.stride(1) != 1) or (self.n_rows > 1 and probs.stride(0) < n):
+            probs = probs.contiguous()
+        pitch = probs.stride(0) if self.n_rows > 1 else n
+        self._check(self._L.mww_detector_update(self._d, probs.data_ptr(), n, pitch, _stream(probs.device)))
+
+    def drain(self):
+        """-> (events, dropped): the events since the last drain as a structured array (EVENT_DTYPE) sorted by (step, stream),
+        and how many more fired than `capacity` could hold.  Waits for the current CUDA stream; clears the event buffer and
+        fired_ids."""
+        import torch
+        buf = np.empty(self.capacity, EVENT_DTYPE)
+        n = ctypes.c_longlong(0)
+        self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), _stream(torch.device("cuda", self.device))))
+        ev = buf[:min(n.value, self.capacity)]
+        return ev[np.lexsort((ev["stream"], ev["step"]))], max(n.value - self.capacity, 0)
+
+    def reset(self, rows=None) -> None:
+        """Fresh detector state (warm-up and cooldown start again) for all rows (None) or the given ROW indices: a host
+        sequence, or a contiguous 1-D CUDA int32 tensor.  Indices out of range are ignored."""
+        import torch
+        st = _stream(torch.device("cuda", self.device))
+        if rows is None:
+            self._check(self._L.mww_detector_reset(self._d, None, 0, st))
+        elif isinstance(rows, torch.Tensor) and rows.is_cuda:
+            if rows.dtype != torch.int32 or rows.dim() != 1 or not rows.is_contiguous():
+                raise ValueError("device row indices must be a contiguous 1-D CUDA int32 tensor")
+            self._check(self._L.mww_detector_reset_device(self._d, rows.data_ptr(), rows.numel(), st))
+        else:
+            r = np.ascontiguousarray(rows, np.int32).reshape(-1)
+            self._check(self._L.mww_detector_reset(self._d, r.ctypes.data, r.size, st))
+
+    def state_dict(self) -> dict:
+        d = dict(hist=np.zeros((self.n_rows, self.window - 1), np.float32), seen=np.zeros(self.n_rows, np.int64),
+                 cooldown=np.zeros(self.n_rows, np.int32))
+        self._check(self._L.mww_detector_get_state(self._d, d["hist"].ctypes.data, d["seen"].ctypes.data, d["cooldown"].ctypes.data))
+        return d
+
+    def load_state_dict(self, d: dict) -> None:
+        hist = np.ascontiguousarray(d["hist"], np.float32)
+        seen = np.ascontiguousarray(d["seen"], np.int64)
+        cooldown = np.ascontiguousarray(d["cooldown"], np.int32)
+        if hist.shape != (self.n_rows, self.window - 1) or seen.shape != (self.n_rows,) or cooldown.shape != (self.n_rows,):
+            raise ValueError("state must be hist [n_rows, window - 1], seen [n_rows], cooldown [n_rows]")
+        self._check(self._L.mww_detector_set_state(self._d, hist.ctypes.data, seen.ctypes.data, cooldown.ctypes.data))
