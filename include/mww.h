@@ -155,6 +155,48 @@ int mww_set_resampler_state(mww_t *h, const int16_t *h_history, long long inputs
  * out[0, n_taps) when max_taps >= n_taps.  16000: n_taps = 0.  A rate outside the list: MWW_EUNSUPPORTED. */
 int mww_resample_taps(int rate, int32_t *out, int max_taps, int *n_taps, int *L, int *M);
 
+/* ---- Per-stream input rates ------------------------------------------------------------------------------------------
+ * A handle in per-stream-rate mode gives each stream s its own rate r_s from the list above (L_s / M_s = 16000 / r_s), so
+ * one handle serves telephony, files and WebRTC at once.  The handle keeps one lockstep counter t: the 16 kHz samples every
+ * stream has been given since the last full reset.  Every audio call names its length n16 in 16 kHz samples, passed as
+ * n_samples; n16 must be even (an 8 kHz stream yields 16 kHz samples in pairs), 0 included.  Row s of the caller's audio
+ * holds the stream's next
+ *     D_s = N(t + n16, r_s) - N(t, r_s)   input samples,   N(t, r) = floor(t M / L)   (mww_rate_inputs),
+ * and the call advances t by n16.  The N identity: for even t, ceil(N(t, r) L / M) = t at every rate.  Proof: write
+ * t M = N L + rho with 0 <= rho < L, so N L <= t M.  At 8 kHz (L = 2, M = 1) rho = t mod 2 = 0, so N L = t M.  At every
+ * other rate M >= L > rho, so N L > t M - M.  Either way (t - 1) M < N L <= t M.  After N(t, r_s) inputs the causal rule
+ * above has therefore emitted exactly t samples at 16 kHz, and every call gives every stream n16 of them.  A 30 ms call is
+ * n16 = 480 at every rate: 240 / 480 / 720 / 960 / 1 323 / 1 440 samples at 8 / 16 / 24 / 32 / 44.1 / 48 kHz, and 661 or
+ * 662 in turn at 22.05 kHz.
+ *
+ * Stream s is bit-identical to a stream of a handle at the single rate r_s (a plain 16 kHz handle when r_s = 16000) given
+ * the same D_s samples in every call: features, every model's probabilities and state, and its resampler history.
+ * Changing a stream's rate zeroes its resampler history and nothing else: it then continues as a stream at the new rate
+ * that has been given N(t, r_new) samples of silence.  Call mww_reset(ids) as well to restart its frontend and models.
+ *
+ * In this mode every audio entry point (mww_features*, mww_predict_clip*, host, remote, _multi, _f32) reads n_samples as
+ * n16; an odd n16, or an audio_stride below the call's largest D_s, is MWW_EINVAL before any work.  Each tile runs one
+ * resampler launch per rate with streams in it, on those streams only; 16 kHz streams are copied.  mww_get_input_rate
+ * reports MWW_RATE_PER_STREAM and t.  mww_get_resampler_state / mww_set_resampler_state move history
+ * int16 [n_streams][H_max] and t, H_max = 243 (the largest H of any rate; 52, 111, 122, 163, 222 and 243 at 8, 22.05, 24,
+ * 32, 44.1 and 48 kHz): each stream uses the first H of its own rate, and set refuses an odd t.  mww_reset(NULL) and
+ * mww_reset_frontend zero every history and t and keep the rates; mww_reset(ids) zeroes those streams' histories.
+ * mww_export_streams / mww_import_streams return MWW_EUNSUPPORTED.  mww_set_input_rate(h, r), allowed at t = 0, returns
+ * the handle to one rate for every stream. */
+#define MWW_RATE_PER_STREAM 0
+/* Rate h_rates[i] for stream h_ids[i].  The first call puts the handle into per-stream-rate mode, with every stream not
+ * listed at 16000; it is allowed only where mww_set_input_rate is (no buffered samples, counter 0) and on a 16 kHz handle
+ * (MWW_EINVAL otherwise).  Later calls are allowed wherever a stateful call is.  Ordered on cu_stream; the listed streams'
+ * histories are zeroed, whether their rate changes or not.  A rate outside the list: MWW_EUNSUPPORTED; an id out of range
+ * or listed twice, or n < 0: MWW_EINVAL.  Every refusal leaves the handle unchanged. */
+int mww_set_stream_rates(mww_t *h, const int32_t *h_ids, const int32_t *h_rates, int n, void *cu_stream);
+/* h_rates [n_streams] (may be NULL): each stream's rate, the handle's rate for every stream on a single-rate handle.
+ * *samples16_seen (may be NULL): t; on a single-rate handle the 16 kHz samples its resampler has emitted (0 at 16000). */
+int mww_get_stream_rates(const mww_t *h, int32_t *h_rates, long long *samples16_seen);
+/* *inputs = N(samples16, rate) = floor(samples16 M / L), without a handle or a GPU.  A rate outside the list:
+ * MWW_EUNSUPPORTED; samples16 outside [0, 2^50] or inputs NULL: MWW_EINVAL. */
+int mww_rate_inputs(int rate, long long samples16, long long *inputs);
+
 /* Frontend only.  d_audio: int16 [n_streams][n_samples] with row pitch `audio_stride` samples.
  * Appends the samples to every stream's window buffer and emits one uint16[40] row per completed
  * 10 ms hop into d_feat [n_streams][max_rows][40].  *h_rows_out = rows emitted per stream

@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(_HERE, "libmww_b200.so")
 
 MWW_ROWS_U16, MWW_ROWS_F32, MWW_ROWS_I8 = 0, 1, 2
+MWW_RATE_PER_STREAM = 0
 
 # every symbol include/mww.h declares (checked by tests/test_capi_symbols.py)
 EXPORTS = (
@@ -30,6 +31,7 @@ EXPORTS = (
     "mww_create_multi_streams", "mww_set_model_streams", "mww_get_model_streams",
     "mww_stream_layout_get", "mww_export_streams", "mww_import_streams",
     "mww_set_input_rate", "mww_get_input_rate", "mww_get_resampler_state", "mww_set_resampler_state", "mww_resample_taps",
+    "mww_set_stream_rates", "mww_get_stream_rates", "mww_rate_inputs",
     "mww_detector_create", "mww_detector_destroy", "mww_detector_update", "mww_detector_drain", "mww_detector_buffers",
     "mww_detector_reset", "mww_detector_reset_device", "mww_detector_get_state", "mww_detector_set_state",
 )
@@ -196,6 +198,12 @@ def lib() -> ctypes.CDLL:
     L.mww_set_resampler_state.argtypes = [vp, vp, ll]
     L.mww_resample_taps.restype = i32
     L.mww_resample_taps.argtypes = [i32, vp, i32, pi, pi, pi]
+    L.mww_set_stream_rates.restype = i32
+    L.mww_set_stream_rates.argtypes = [vp, vp, vp, i32, vp]
+    L.mww_get_stream_rates.restype = i32
+    L.mww_get_stream_rates.argtypes = [vp, vp, ctypes.POINTER(ll)]
+    L.mww_rate_inputs.restype = i32
+    L.mww_rate_inputs.argtypes = [i32, ll, ctypes.POINTER(ll)]
     L.mww_detector_create.restype = i32
     L.mww_detector_create.argtypes = [i32, i32, i32, ctypes.c_double, i32, i32, vp, ctypes.POINTER(vp)]
     L.mww_detector_destroy.restype = i32

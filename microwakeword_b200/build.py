@@ -15,6 +15,10 @@ SOURCES = ["mww_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww
 # main library's own kernel set stays the one the SASS fixtures under tests/golden/ record
 RS_OUT = os.path.join(HERE, "libmww_resample.so")
 RS_SOURCES = ["mww_resample.cu"]
+# the same kernel on one rate's members of a tile (per-stream rates, mww_set_stream_rates), likewise apart, so that
+# libmww_resample.so keeps the two instantiations a handle with one input rate runs
+RR_OUT = os.path.join(HERE, "libmww_resample_rates.so")
+RR_SOURCES = ["mww_resample_rates.cu"]
 # likewise the streaming detector's kernels (mww_detector_*)
 DET_OUT = os.path.join(HERE, "libmww_detector.so")
 DET_SOURCES = ["mww_detector.cu"]
@@ -40,7 +44,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, DET_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -58,8 +62,9 @@ def build(force: bool = False, verbose: bool = False) -> str:
         fcntl.flock(lock, fcntl.LOCK_EX)
         if not force and not _stale():
             return OUT
-        for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (DET_OUT, DET_SOURCES, []),
-                                    (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_detector", "-Xlinker", "-rpath,$ORIGIN"])):
+        for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (RR_OUT, RR_SOURCES, []), (DET_OUT, DET_SOURCES, []),
+                                    (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector", "-Xlinker",
+                                                    "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra
             res = subprocess.run(cmd, capture_output=True, text=True)

@@ -61,6 +61,15 @@ struct Model : ModelWeights {
     template <typename T> T *pend(int first) const { return static_cast<T *>(d_pend) + (size_t)first * G.pend_cap * kNumChannels; }
 };
 
+// the streams of one input rate of a handle with per-stream rates (mww_set_stream_rates): the rate's plan and polyphase
+// table, and its members, rate_ids[off, off + n) (sorted)
+constexpr int kNumRates = (int)(sizeof kResampleRates / sizeof kResampleRates[0]);
+struct RateGroup {
+    ResamplePlan P;
+    int16_t *d_table = nullptr;     // [L][pitch]; none at 16 kHz (the identity plan)
+    int off = 0, n = 0;
+};
+
 }  // namespace
 
 struct mww_handle {
@@ -83,6 +92,13 @@ struct mww_handle {
     int rs_hist_stride = 0;         // H rounded up to even: whole 4-byte words per stream (reset by id)
     long long rs_seen = 0;          // input samples every stream has been given since the last full / frontend reset
     int16_t *d_rs_out = nullptr; size_t rs_out_bytes = 0;     // one tile's 16 kHz samples
+    // per-stream rates (mww_set_stream_rates): rs stays the 16 kHz plan, rs_seen counts t (16 kHz samples every stream has
+    // been given), d_rs_hist rows hold resample_max_history() samples, and each rate has its table and member list
+    bool per_rate = false;
+    std::vector<int32_t> stream_rate;                   // [n_streams]
+    RateGroup groups[kNumRates];
+    std::vector<int32_t> rate_ids;                      // every group's members, group after group
+    int32_t *d_rate_ids = nullptr;                      // device copy of rate_ids
     // scratch
     uint32_t *d_v = nullptr; size_t v_bytes = 0;
     uint16_t *d_feat = nullptr; size_t feat_bytes = 0;
@@ -169,11 +185,40 @@ int ensure_scratch(mww_t *h, size_t v_bytes, size_t feat_bytes, size_t gather_by
     return MWW_OK;
 }
 
-bool resampling(const mww_t *h) { return h->rs.rate != 16000; }
-// 16 kHz samples a call of n input-rate samples gives every stream
-int samples16(const mww_t *h, int n) { return resampling(h) ? resample_call_outputs(h->rs_seen, n, h->rs.L, h->rs.M) : n; }
-// the resampler's index math is int32 in upsampled samples: a call must keep n L below 2^31 (about 100 s at 22.05 kHz)
-bool resample_call_fits(const mww_t *h, int n) { return !resampling(h) || (long long)n * h->rs.L + h->rs.M < (1ll << 31); }
+bool resampling(const mww_t *h) { return h->per_rate || h->rs.rate != 16000; }
+// 16 kHz samples a call of n input-rate samples gives every stream (per-stream rates: n is n16 already)
+int samples16(const mww_t *h, int n) {
+    return h->per_rate ? n : (resampling(h) ? resample_call_outputs(h->rs_seen, n, h->rs.L, h->rs.M) : n);
+}
+// per-stream rates: the input samples a call of n16 takes from each stream of group g, N(t + n16) - N(t)
+long long rate_inputs(const mww_t *h, const RateGroup &g, int n16) {
+    return resample_inputs(h->rs_seen + n16, g.P.L, g.P.M) - resample_inputs(h->rs_seen, g.P.L, g.P.M);
+}
+// the samples a row of the caller's audio holds for a call of n: n, or per-stream rates the largest D_s of any rate present
+long long input_width(const mww_t *h, int n) {
+    if (!h->per_rate || n <= 0) return n;
+    long long w = 0;
+    for (const RateGroup &g : h->groups)
+        if (g.n > 0) w = std::max(w, rate_inputs(h, g, n));
+    return w;
+}
+// the resampler's index math is int32 in upsampled samples: a call must keep n L below 2^31 (about 100 s at 22.05 kHz), at
+// every rate present
+bool resample_call_fits(const mww_t *h, int n) {
+    if (h->per_rate) {
+        for (const RateGroup &g : h->groups)
+            if (g.n > 0 && rate_inputs(h, g, n) * g.P.L + g.P.M >= (1ll << 31)) return false;
+        return true;
+    }
+    return !resampling(h) || (long long)n * h->rs.L + h->rs.M < (1ll << 31);
+}
+// the audio arguments every audio entry point checks first.  Per-stream rates: n_samples is n16 and must be even, and each
+// row must hold the call's largest D_s.
+bool bad_audio(const mww_t *h, int n_samples, const void *audio, long long audio_stride) {
+    return n_samples < 0 || (h->per_rate && (n_samples & 1)) || (n_samples > 0 && !audio) || audio_stride < input_width(h, n_samples);
+}
+// samples of the resampler history a stream keeps (the row length of mww_get_resampler_state)
+int hist_len(const mww_t *h) { return h->per_rate ? resample_max_history() : h->rs.H; }
 
 int ensure_rs_out(mww_t *h, size_t bytes) {
     if (bytes <= h->rs_out_bytes) return MWW_OK;
@@ -186,8 +231,29 @@ int ensure_rs_out(mww_t *h, size_t bytes) {
 
 // streams [first, first + n) of a call of n_in input-rate samples -> their n16 16 kHz samples in h->d_rs_out [n][n16], each
 // stream's history moved on.  One launch; the caller advances h->rs_seen once the whole call is issued.
+// Per-stream rates: one launch per rate with members in the tile [first, first + n), over those members only; the 16 kHz
+// members' samples are copied (the identity plan).
+template <typename T>
+int run_rates_tile(mww_t *h, int first, int n, const T *d_audio, long long audio_stride, int n16, cudaStream_t st) {
+    for (const RateGroup &g : h->groups) {
+        int a = 0, b = 0;
+        tile_members(h->rate_ids.data() + g.off, g.n, first, n, &a, &b);
+        const int n_in = (int)rate_inputs(h, g, n16);      // below 2^31 / L: resample_call_fits
+        if (b == a || n_in <= 0) continue;
+        ResampleArgs r;
+        r.table = g.d_table; r.hist = h->d_rs_hist; r.hist_stride = h->rs_hist_stride;
+        r.audio_stride = audio_stride; r.out_stride = n16;
+        r.L = g.P.L; r.M = g.P.M; r.T = g.P.T; r.H = g.P.H; r.pitch = g.P.pitch;
+        r.t0 = resample_t0(resample_inputs(h->rs_seen, g.P.L, g.P.M), g.P.L, g.P.M); r.n_in = n_in; r.n_out = n16; r.n_streams = b - a;
+        CU(h, launch_resample_members(r, h->d_rate_ids + g.off + a, first, d_audio, h->d_rs_out, h->sm_count, st));
+        h->launches += 1;
+    }
+    return MWW_OK;
+}
+
 template <typename T>
 int run_resample_tile(mww_t *h, int first, int n, const T *d_audio, long long audio_stride, int n_in, int n16, cudaStream_t st) {
+    if (h->per_rate) return run_rates_tile(h, first, n, d_audio, audio_stride, n16, st);
     if (n_in <= 0) return MWW_OK;
     ResampleArgs a;
     a.table = h->d_rs_table; a.hist = h->d_rs_hist + (size_t)first * h->rs_hist_stride; a.hist_stride = h->rs_hist_stride;
@@ -516,7 +582,8 @@ void destroy_impl(mww_t *h) {
     cudaFree(h->d_tables); cudaFree(h->d_carry); cudaFree(h->d_estimate);
     cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
     cudaFree(h->d_gather); cudaFree(h->d_cids);
-    cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist); cudaFree(h->d_rs_out);
+    cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist); cudaFree(h->d_rs_out); cudaFree(h->d_rate_ids);
+    for (RateGroup &g : h->groups) cudaFree(g.d_table);
     for (int b = 0; b < 2; ++b) {
         cudaFree(h->d_audio_tile[b]); cudaFree(h->d_probs_tile[b]);
         if (h->ev_h2d[b]) cudaEventDestroy(h->ev_h2d[b]);
@@ -537,7 +604,7 @@ template <typename T>
 int features_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
                   int *h_rows_out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (bad_audio(h, n_samples, d_audio, audio_stride)) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
     if (!resample_call_fits(h, n_samples)) return fail(h, MWW_EINVAL, std::string(who) + ": call too long for the resampler; split it");
     ENTER_STATEFUL(h);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
@@ -641,7 +708,7 @@ template <typename T>
 int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, long long audio_stride, float *const *d_probs,
                       const int *max_probs, int *h_probs_out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !d_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (bad_audio(h, n_samples, d_audio, audio_stride)) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
     if (h->models.empty()) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     if (!resample_call_fits(h, n_samples)) return fail(h, MWW_EINVAL, std::string(who) + ": call too long for the resampler; split it");
     ENTER_STATEFUL(h);
@@ -1090,9 +1157,17 @@ int mww_set_input_rate(mww_t *h, int rate) {
             return fail(h, e == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("mww_set_input_rate: ") + cudaGetErrorString(e));
         }
     }
-    // earlier calls may still read the old table and history
+    // earlier calls may still read the old tables, history and member lists
     if (h->d_rs_table || h->d_rs_hist) CU(h, cudaDeviceSynchronize());
     cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist);
+    if (h->per_rate) {                 // back to one rate for every stream
+        for (RateGroup &g : h->groups) cudaFree(g.d_table);
+        cudaFree(h->d_rate_ids);
+        for (RateGroup &g : h->groups) g = RateGroup{};
+        h->d_rate_ids = nullptr;
+        h->rate_ids.clear(); h->stream_rate.clear();
+        h->per_rate = false;
+    }
     h->d_rs_table = table; h->d_rs_hist = hist;
     h->rs_hist_stride = P.n_taps > 0 ? hist_stride : 0;
     h->rs = P;
@@ -1102,7 +1177,7 @@ int mww_set_input_rate(mww_t *h, int rate) {
 
 int mww_get_input_rate(const mww_t *h, int *rate, long long *inputs_seen) {
     if (!h) return MWW_EINVAL;
-    if (rate) *rate = h->rs.rate;
+    if (rate) *rate = h->per_rate ? MWW_RATE_PER_STREAM : h->rs.rate;
     if (inputs_seen) *inputs_seen = h->rs_seen;
     return MWW_OK;
 }
@@ -1113,21 +1188,131 @@ int mww_get_resampler_state(mww_t *h, int16_t *h_history, long long *inputs_seen
     if (inputs_seen) *inputs_seen = h->rs_seen;
     if (!h_history || !resampling(h)) return MWW_OK;
     CU(h, cudaDeviceSynchronize());
-    CU(h, cudaMemcpy2D(h_history, (size_t)h->rs.H * 2, h->d_rs_hist, (size_t)h->rs_hist_stride * 2, (size_t)h->rs.H * 2, h->n_streams,
-                       cudaMemcpyDeviceToHost));
+    const size_t H = (size_t)hist_len(h);
+    CU(h, cudaMemcpy2D(h_history, H * 2, h->d_rs_hist, (size_t)h->rs_hist_stride * 2, H * 2, h->n_streams, cudaMemcpyDeviceToHost));
     return MWW_OK;
 }
 
 int mww_set_resampler_state(mww_t *h, const int16_t *h_history, long long inputs_seen) {
     if (!h) return MWW_EINVAL;
-    if (inputs_seen < 0 || (!resampling(h) && inputs_seen != 0))
-        return fail(h, MWW_EINVAL, "mww_set_resampler_state: inputs_seen out of range (always 0 at 16 kHz)");
+    if (inputs_seen < 0 || (!resampling(h) && inputs_seen != 0) || (h->per_rate && (inputs_seen & 1)))
+        return fail(h, MWW_EINVAL, "mww_set_resampler_state: inputs_seen out of range (always 0 at 16 kHz, even with per-stream rates)");
     ENTER(h);
     CU(h, cudaDeviceSynchronize());
-    if (h_history && resampling(h))
-        CU(h, cudaMemcpy2D(h->d_rs_hist, (size_t)h->rs_hist_stride * 2, h_history, (size_t)h->rs.H * 2, (size_t)h->rs.H * 2, h->n_streams,
-                           cudaMemcpyHostToDevice));
+    if (h_history && resampling(h)) {
+        const size_t H = (size_t)hist_len(h);
+        CU(h, cudaMemcpy2D(h->d_rs_hist, (size_t)h->rs_hist_stride * 2, h_history, H * 2, H * 2, h->n_streams, cudaMemcpyHostToDevice));
+    }
     h->rs_seen = inputs_seen;
+    return MWW_OK;
+}
+
+namespace {
+
+int rate_slot(int rate) {
+    for (int i = 0; i < kNumRates; ++i)
+        if (kResampleRates[i] == rate) return i;
+    return -1;
+}
+
+// every group's member list from stream_rate, on the host; the device copy is the caller's
+void plan_rate_groups(mww_t *h) {
+    h->rate_ids.clear();
+    for (RateGroup &g : h->groups) {
+        g.off = (int)h->rate_ids.size();
+        for (int s = 0; s < h->n_streams; ++s)
+            if (h->stream_rate[s] == g.P.rate) h->rate_ids.push_back(s);
+        g.n = (int)h->rate_ids.size() - g.off;
+    }
+}
+
+// the first mww_set_stream_rates: every rate's table, the [n_streams][H_max] history (zero) and the member list, all streams
+// at 16 kHz.  Nothing of the handle changes unless all of it could be allocated.
+int enter_per_rate(mww_t *h) {
+    RateGroup g[kNumRates];
+    const int stride = (resample_max_history() + 1) / 2 * 2;
+    int16_t *hist = nullptr;
+    int32_t *ids = nullptr;
+    const size_t S = (size_t)h->n_streams;
+    cudaError_t e = cudaMalloc(&hist, S * stride * sizeof(int16_t));
+    if (e == cudaSuccess) e = cudaMemset(hist, 0, S * stride * sizeof(int16_t));
+    if (e == cudaSuccess) e = cudaMalloc(&ids, S * sizeof(int32_t));
+    bool bound = true;
+    for (int i = 0; i < kNumRates && e == cudaSuccess && bound; ++i) {
+        resample_plan(kResampleRates[i], &g[i].P);
+        if (g[i].P.n_taps == 0) continue;
+        std::vector<int32_t> taps((size_t)g[i].P.n_taps);
+        bound = resample_taps(g[i].P, taps.data());
+        std::vector<int16_t> host((size_t)g[i].P.L * g[i].P.pitch);
+        resample_table(g[i].P, taps.data(), host.data());
+        e = cudaMalloc(&g[i].d_table, host.size() * sizeof(int16_t));
+        if (e == cudaSuccess) e = cudaMemcpy(g[i].d_table, host.data(), host.size() * sizeof(int16_t), cudaMemcpyHostToDevice);
+    }
+    if (e != cudaSuccess || !bound) {
+        cudaFree(hist); cudaFree(ids);
+        for (RateGroup &r : g) cudaFree(r.d_table);
+        if (!bound) return fail(h, MWW_EINVAL, "mww_set_stream_rates: a phase breaks the partial-sum bound");
+        return fail(h, e == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("mww_set_stream_rates: ") + cudaGetErrorString(e));
+    }
+    h->stream_rate.assign(S, 16000);
+    for (int i = 0; i < kNumRates; ++i) h->groups[i] = g[i];
+    plan_rate_groups(h);
+    if ((e = cudaMemcpy(ids, h->rate_ids.data(), S * sizeof(int32_t), cudaMemcpyHostToDevice)) != cudaSuccess) {
+        cudaFree(hist); cudaFree(ids);
+        for (RateGroup &r : h->groups) { cudaFree(r.d_table); r = RateGroup{}; }
+        h->stream_rate.clear(); h->rate_ids.clear();
+        return cuda_fail(h, e, "mww_set_stream_rates");
+    }
+    h->d_rs_hist = hist;
+    h->rs_hist_stride = stride;
+    h->d_rate_ids = ids;
+    h->per_rate = true;
+    return MWW_OK;
+}
+
+}  // namespace
+
+int mww_set_stream_rates(mww_t *h, const int32_t *h_ids, const int32_t *h_rates, int n, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (n < 0 || (n > 0 && (!h_ids || !h_rates))) return fail(h, MWW_EINVAL, "mww_set_stream_rates: bad arguments");
+    std::vector<char> listed((size_t)h->n_streams, 0);
+    for (int i = 0; i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= h->n_streams) return fail(h, MWW_EINVAL, "mww_set_stream_rates: stream id out of range");
+        if (listed[(size_t)h_ids[i]]) return fail(h, MWW_EINVAL, "mww_set_stream_rates: duplicate stream id");
+        listed[(size_t)h_ids[i]] = 1;
+    }
+    for (int i = 0; i < n; ++i)
+        if (rate_slot(h_rates[i]) < 0)
+            return fail(h, MWW_EUNSUPPORTED, "mww_set_stream_rates: every rate must be one of 8000, 16000, 22050, 24000, 32000, 44100, 48000 Hz");
+    if (!h->per_rate && (h->used != 0 || h->rs_seen != 0 || h->rs.rate != 16000))
+        return fail(h, MWW_EINVAL, "mww_set_stream_rates: per-stream rates start on a 16 kHz handle that holds no buffered samples; reset it first");
+    ENTER_STATEFUL(h);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (!h->per_rate)
+        if (int rc = enter_per_rate(h)) return rc;
+    if (n == 0) return MWW_OK;
+    // the listed streams' histories are zeroed, then the member lists change, both in stream order
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+    if (int rc = fill_by_id(h, h->d_rs_hist, (size_t)h->rs_hist_stride * sizeof(int16_t), h->d_ids, n, h->n_streams, st)) return rc;
+    for (int i = 0; i < n; ++i) h->stream_rate[(size_t)h_ids[i]] = h_rates[i];
+    plan_rate_groups(h);
+    CU(h, cudaMemcpyAsync(h->d_rate_ids, h->rate_ids.data(), (size_t)h->n_streams * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return MWW_OK;
+}
+
+int mww_get_stream_rates(const mww_t *h, int32_t *h_rates, long long *samples16_seen) {
+    if (!h) return MWW_EINVAL;
+    if (h_rates)
+        for (int s = 0; s < h->n_streams; ++s) h_rates[s] = h->per_rate ? h->stream_rate[(size_t)s] : h->rs.rate;
+    if (samples16_seen) *samples16_seen = h->per_rate ? h->rs_seen : resample_outputs(h->rs_seen, h->rs.L, h->rs.M);
+    return MWW_OK;
+}
+
+int mww_rate_inputs(int rate, long long samples16, long long *inputs) {
+    ResamplePlan P;
+    if (!resample_plan(rate, &P)) { g_create_error = "mww_rate_inputs: unsupported input rate"; return MWW_EUNSUPPORTED; }
+    if (samples16 < 0 || samples16 > (1ll << 50) || !inputs) { g_create_error = "mww_rate_inputs: bad arguments"; return MWW_EINVAL; }
+    *inputs = resample_inputs(samples16, P.L, P.M);
     return MWW_OK;
 }
 
@@ -1222,6 +1407,7 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
                  int tile, int n_frames, int n16) {
     const size_t K = h->models.size();
     const T *audio_tile[2] = {static_cast<const T *>(h->d_audio_tile[0]), static_cast<const T *>(h->d_audio_tile[1])};
+    const long long width = input_width(h, n_samples);      // samples per staged row
     float *tile_probs[kMaxModels];
     long long tile_probs_stride[kMaxModels];
     TileSpan span[kMaxModels];
@@ -1237,10 +1423,10 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
             for (int i = 0; i < 4; ++i) { CU(h, cudaEventCreate(&tl[i])); h->tl_ev.push_back(tl[i]); }
             CU(h, cudaEventRecord(tl[0], h->st_h2d));
         }
-        if (n_samples > 0) {
+        if (width > 0) {
             const T *from = src + (size_t)first * audio_stride;
-            const size_t row = (size_t)n_samples * sizeof(T);
-            if (audio_stride == n_samples)       // contiguous block: one linear DMA
+            const size_t row = (size_t)width * sizeof(T);
+            if (audio_stride == width)           // contiguous block: one linear DMA
                 CU(h, cudaMemcpyAsync(h->d_audio_tile[b], from, (size_t)n * row, cudaMemcpyDefault, h->st_h2d));
             else
                 CU(h, cudaMemcpy2DAsync(h->d_audio_tile[b], row, from, (size_t)audio_stride * sizeof(T), row, n,
@@ -1254,7 +1440,7 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
         int rc = MWW_OK;
         if (resampling(h)) {
             // one 16 kHz scratch serves every tile: all kernels run in order on the compute stream
-            rc = run_resample_tile(h, first, n, audio_tile[b], n_samples, n_samples, n16, h->st_compute);
+            rc = run_resample_tile(h, first, n, audio_tile[b], width, n_samples, n16, h->st_compute);
             if (rc == MWW_OK) rc = run_frontend_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
         } else {
             rc = run_frontend_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->d_feat, (long long)n_frames * kNumChannels, h->st_compute);
@@ -1307,14 +1493,15 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
     // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
     // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone.  A resampling handle adds its
     // 16 kHz tile scratch.
-    const size_t staged_bytes = sizeof(T) == sizeof(int16_t) ? 0 : 2 * (size_t)std::max(n_samples, 1) * sizeof(T);
+    const long long width = input_width(h, n_samples);      // per-stream rates: the call's largest D_s
+    const size_t staged_bytes = sizeof(T) == sizeof(int16_t) ? 0 : 2 * (size_t)std::max<long long>(width, 1) * sizeof(T);
     const size_t gather = gather_bytes_per_stream(h, n_frames);
     int tile = tile_streams(h, n_frames, true, staged_bytes + gather + (resampling(h) ? (size_t)n16 * 2 : 0));
     tile = std::max(1, std::min(tile, std::max((h->n_streams + want_tiles - 1) / want_tiles, std::min(h->n_streams, h->min_tile_streams))));
     rc = ensure_scratch(h, v_scratch_bytes(h, tile, n_frames), (size_t)tile * std::max(n_frames, 1) * kNumChannels * 2, (size_t)tile * gather);
     if (rc == MWW_OK && resampling(h)) rc = ensure_rs_out(h, (size_t)tile * std::max(n16, 1) * 2);
     if (rc) return rc;
-    const size_t a_bytes = (size_t)tile * std::max(n_samples, 1) * sizeof(T);
+    const size_t a_bytes = (size_t)tile * std::max<long long>(width, 1) * sizeof(T);
     const size_t p_bytes = dst_is_host ? probs_tile_offset(h, o, tile, h->models.size()) * sizeof(float) : 0;
     if (a_bytes > h->audio_tile_bytes || p_bytes > h->probs_tile_bytes) {
         CU(h, cudaDeviceSynchronize());
@@ -1369,7 +1556,7 @@ template <typename T>
 int predict_clip_host_impl(mww_t *h, const char *who, const T *h_audio, int n_samples, long long audio_stride, float *const *h_probs,
                            const int *max_probs, int *h_probs_out) {
     if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !h_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (bad_audio(h, n_samples, h_audio, audio_stride)) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
     if (h->models.empty()) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     ENTER_STATEFUL(h);
     // The call has no stream argument, so it cannot be ordered after one particular stream: it waits for everything the
@@ -1382,7 +1569,7 @@ template <typename T>
 int predict_clip_remote_impl(mww_t *h, const char *who, const T *src_audio, int n_samples, long long audio_stride, float *const *d_probs,
                              const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
     if (!h) return MWW_EINVAL;
-    if (n_samples < 0 || (n_samples > 0 && !src_audio) || audio_stride < n_samples) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
+    if (bad_audio(h, n_samples, src_audio, audio_stride)) return fail(h, MWW_EINVAL, std::string(who) + ": bad audio arguments");
     if (h->models.empty()) return fail(h, MWW_EINVAL, std::string(who) + ": frontend-only handle (created without a model)");
     bool local = n_samples == 0;
     if (!local) {
@@ -1779,7 +1966,7 @@ int mww_stream_layout_get(const mww_t *h, mww_stream_layout *out) {
 
 int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out, void *cu_stream) {
     if (!h) return MWW_EINVAL;
-    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_export_streams: stream records do not carry resampler history (input rate != 16000)");
+    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_export_streams: stream records do not carry resampler history (input rate != 16000, or per-stream rates)");
     if (int rc = check_record_args(h, "mww_export_streams", h_ids, n, d_records)) return rc;
     ENTER_STATEFUL(h);
     if (out) fill_stream_layout(h, out);
@@ -1801,7 +1988,7 @@ int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, m
 
 int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout, void *cu_stream) {
     if (!h) return MWW_EINVAL;
-    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_import_streams: stream records do not carry resampler history (input rate != 16000)");
+    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_import_streams: stream records do not carry resampler history (input rate != 16000, or per-stream rates)");
     if (!layout) return fail(h, MWW_EINVAL, "mww_import_streams: bad arguments");
     if (int rc = check_record_args(h, "mww_import_streams", h_ids, n, d_records)) return rc;
     std::vector<uint8_t> listed((size_t)h->n_streams, 0);

@@ -115,6 +115,12 @@ namespace mww {
 // int16 samples out [n_streams][out_stride], history moved on.  T = int16_t or float (pcm16_from_f32 on load).
 template <typename T>
 cudaError_t launch_resample(const ResampleArgs &a, const T *audio, int16_t *out, int sm_count, cudaStream_t st);
+// the same for the a.n_streams members ids[0, n) (device memory, sorted global ids) of one rate in the tile that starts at
+// stream `first`: audio and out rows ids[i] - first, history rows ids[i] of a.hist (not offset).  A plan without taps
+// (a.T == 0, 16 kHz) copies pcm16 of the input.
+template <typename T>
+cudaError_t launch_resample_members(const ResampleArgs &a, const int32_t *ids, int first, const T *audio, int16_t *out, int sm_count,
+                                    cudaStream_t st);
 }  // namespace mww
 
 #include "mww_records.h"

@@ -140,6 +140,41 @@ inline int resample_t0(long long seen, int L, int M) {
     return (int)((M - r) % M);
 }
 
+// Per-stream rates (mww_set_stream_rates).  The handle counts t, the 16 kHz samples every stream has been given.  A stream at
+// rate r (L / M = 16000 / r) has then been given N(t) = floor(t M / L) input samples, and a call of n16 takes
+// N(t + n16) - N(t) of them.  For even t, ceil(N(t) L / M) = t: write t M = N L + rho with 0 <= rho < L.  Then N L <= t M,
+// and at 8 kHz (L = 2, M = 1) rho = 0 since t is even, so N L = t M; at every other rate M >= L > rho, so N L > t M - M.
+// Either way (t - 1) M < N L <= t M.  So the stream's resampler has emitted exactly t outputs, and a call of even n16 gives
+// every stream n16 of them, whatever its rate.
+MWW_HD long long resample_inputs(long long t16, int L, int M) { return t16 * M / L; }
+
+// the largest history H of any listed rate: the row length of the per-stream-rate history
+inline int resample_max_history() {
+    int h = 0;
+    for (int r : kResampleRates) {
+        ResamplePlan P;
+        resample_plan(r, &P);
+        h = P.H > h ? P.H : h;
+    }
+    return h;
+}
+
+// Which rows stream index s of a resample_kernel launch reads and writes.  TileRows: the tile's streams in order (a handle
+// with one input rate).  MemberRows: the members of one rate in the tile, ids[0, n) sorted global ids (per-stream rates):
+// input and output rows ids[s] - first of the tile, history row ids[s] of the handle.  A plan without taps (16 kHz) is the
+// identity there: output q = pcm16(input q), no history.
+struct TileRows {
+    static constexpr bool kGathered = false;
+    MWW_HD int io(int s) const { return s; }
+    MWW_HD int hist(int s) const { return s; }
+};
+struct MemberRows {
+    static constexpr bool kGathered = true;
+    const int32_t *ids; int first;
+    MWW_HD int io(int s) const { return ids[s] - first; }
+    MWW_HD int hist(int s) const { return ids[s]; }
+};
+
 // Output q of a call: t = t0 + q M upsampled samples past the call's first input, newest input k = floor(t / L), phase
 // p = t mod L, and y = sat16((sum_i table[p][i] x(k - i) + 2^14) >> 15) over i < T.  x(j) is the call's input j for j >= 0 and
 // history[H + j] before it.  X is any accessor with int32_t operator()(int j).

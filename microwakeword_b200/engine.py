@@ -85,23 +85,59 @@ def rows_for(buffered: int, n_samples: int, hop: int) -> int:
 
 
 INPUT_RATES = (8000, 16000, 22050, 24000, 32000, 44100, 48000)
+RATE_PER_STREAM = _lib.MWW_RATE_PER_STREAM      # input_rate of an engine with per-stream rates (set_stream_rates)
+LIVE_SAMPLES16 = 480                            # one 30 ms live call, in 16 kHz samples
+
+
+def _ratio(rate: int):
+    from math import gcd
+    g = gcd(16000, int(rate))
+    return 16000 // g, int(rate) // g
 
 
 def samples16(inputs_seen: int, n_samples: int, input_rate: int = 16000) -> int:
     """16 kHz samples a call of n_samples at `input_rate` yields after inputs_seen input samples (mww_set_input_rate):
-    ceil((seen + n) L / M) - ceil(seen L / M) with L / M = 16000 / input_rate"""
-    if input_rate == 16000:
+    ceil((seen + n) L / M) - ceil(seen L / M) with L / M = 16000 / input_rate.  With per-stream rates (RATE_PER_STREAM)
+    n_samples is n16 already."""
+    if input_rate in (16000, RATE_PER_STREAM):
         return int(n_samples)
-    from math import gcd
-    g = gcd(16000, int(input_rate))
-    L, M = 16000 // g, int(input_rate) // g
+    L, M = _ratio(input_rate)
     return -(-(inputs_seen + n_samples) * L // M) + (-inputs_seen * L // M)
+
+
+def rate_inputs(samples16: int, rate: int) -> int:
+    """N(t, r) = floor(t M / L): the input samples a stream at `rate` has been given once the handle's counter of 16 kHz
+    samples is t (mww_rate_inputs).  For even t the resampler has then emitted exactly t samples (include/mww.h)."""
+    L, M = _ratio(rate)
+    return int(samples16) * M // L
+
+
+def inputs_for_rates(rates, samples16_seen: int, n16: int) -> np.ndarray:
+    """int32 [len(rates)]: D_s = N(t + n16, r_s) - N(t, r_s), the samples row s of a call of n16 holds after t = samples16_seen"""
+    rates = np.asarray(rates, np.int64)
+    out = np.zeros(rates.shape, np.int32)
+    for r in np.unique(rates):
+        out[rates == r] = rate_inputs(samples16_seen + n16, int(r)) - rate_inputs(samples16_seen, int(r))
+    return out
+
+
+def resampler_history_len(rate: int) -> int:
+    """input samples a stream at `rate` keeps as resampler history, H = ceil(n_taps / L) (0 at 16 kHz); for RATE_PER_STREAM
+    the largest of any rate, the row length of a per-stream-rate engine's history"""
+    if rate == RATE_PER_STREAM:
+        return max(resampler_history_len(r) for r in INPUT_RATES)
+    n, L = ctypes.c_int(0), ctypes.c_int(1)
+    _lib.check(None, _lib.lib().mww_resample_taps(int(rate), None, 0, ctypes.byref(n), ctypes.byref(L), None))
+    return -(-n.value // L.value)
 
 
 def call_plan(buffered: int, n_samples: int, hop: int, pending_rows, strides, input_rate: int = 16000, inputs_seen: int = 0):
     """Bookkeeping of one call on a shared frontend feeding models of the given strides, each holding pending_rows[k]:
     -> (rows emitted, [steps model k runs], samples buffered after the call, [rows model k holds after the call]).
-    n_samples is at `input_rate`, after `inputs_seen` input samples; the frontend sees samples16() of them."""
+    n_samples is at `input_rate`, after `inputs_seen` input samples; the frontend sees samples16() of them.  With per-stream
+    rates (input_rate RATE_PER_STREAM) n_samples is n16, which must be even, and inputs_seen is the counter t."""
+    if input_rate == RATE_PER_STREAM and (int(n_samples) < 0 or int(n_samples) % 2):
+        raise ValueError("with per-stream rates a call is an even number of 16 kHz samples, not %d" % n_samples)
     n16 = samples16(inputs_seen, n_samples, input_rate)
     rows = rows_for(buffered, n16, hop)
     steps = [(p + rows) // s for p, s in zip(pending_rows, strides)]
@@ -188,15 +224,78 @@ class _Engine:
     def set_input_rate(self, rate: int):
         """Sample rate of the audio this engine is given (mww_set_input_rate): one of INPUT_RATES, 16000 by default.  Any other
         rate is resampled to 16 kHz on the GPU in front of the frontend; every call then takes samples at this rate.  Only
-        while no samples are buffered (after create / reset / reset_frontend)."""
+        while no samples are buffered (after create / reset / reset_frontend).  On an engine with per-stream rates it returns
+        every stream to this one rate."""
         _lib.check(self._h, self._L.mww_set_input_rate(self._h, int(rate)))
+        self._rate_set = None
+
+    # ------------------------------------------------------------------ per-stream input rates
+    @property
+    def per_stream_rates(self) -> bool:
+        return self.input_rate == RATE_PER_STREAM
+
+    @property
+    def stream_rates(self) -> np.ndarray:
+        """int32 [n_streams]: each stream's input rate (the engine's rate for every stream unless per_stream_rates)"""
+        out = np.zeros(self.n_streams, np.int32)
+        _lib.check(self._h, self._L.mww_get_stream_rates(self._h, out.ctypes.data, None))
+        return out
+
+    def set_stream_rates(self, ids, rates) -> None:
+        """Stream ids[i] takes audio at rates[i] (one of INPUT_RATES; a single rate applies to every listed id), ordered on
+        the current CUDA stream (mww_set_stream_rates).  The first call turns a 16 kHz engine with nothing buffered into an
+        engine with per-stream rates, every stream not listed at 16 kHz.  Each listed stream's resampler history is zeroed:
+        a client joining a slot calls reset(ids) as well to restart its frontend and models.  Every call then takes
+        samples16= (an even number of 16 kHz samples) and row s holds inputs_for(samples16)[s] samples."""
+        ids = self._ids(ids)
+        r = np.asarray(rates)
+        if r.ndim == 0:
+            r = np.full(ids.size, int(r))
+        if r.shape != ids.shape or (r.size and not np.issubdtype(r.dtype, np.integer)):
+            raise ValueError("rates must be one integer rate per id")
+        r = np.ascontiguousarray(r, np.int32)
+        self._rate_set = None
+        _lib.check(self._h, self._L.mww_set_stream_rates(self._h, ids.ctypes.data, r.ctypes.data, ids.size, self._cu_stream()))
+
+    def _rates_present(self) -> tuple:
+        """the distinct stream rates, kept until the rates change (a call's row width needs them, not every stream's)"""
+        if getattr(self, "_rate_set", None) is None:
+            self._rate_set = tuple(int(r) for r in np.unique(self.stream_rates))
+        return self._rate_set
+
+    def inputs_for(self, samples16: int) -> np.ndarray:
+        """int32 [n_streams]: the samples each stream's row holds in the next call of samples16 (per_stream_rates only):
+        D_s = N(t + samples16, r_s) - N(t, r_s), N(t, r) = floor(t M / L)"""
+        rate, t = self._rate()
+        if rate != RATE_PER_STREAM:
+            raise ValueError("inputs_for is for an engine with per-stream rates (set_stream_rates)")
+        n16 = self._check_samples16(samples16)
+        return inputs_for_rates(self.stream_rates, t, n16)
+
+    @staticmethod
+    def _check_samples16(samples16) -> int:
+        if samples16 is None or int(samples16) != samples16 or int(samples16) < 0 or int(samples16) % 2:
+            raise ValueError("with per-stream rates every call needs samples16=, an even number of 16 kHz samples >= 0 (got %r)"
+                             % (samples16,))
+        return int(samples16)
+
+    def _call_len(self, width: int, samples16) -> int:
+        """-> n_samples for the library.  One input rate: the audio's width (samples16 must be None).  Per-stream rates: the
+        checked samples16, once the rows (`width` samples) are known to hold every stream's D_s."""
+        rate, t = self._rate()
+        if rate != RATE_PER_STREAM:
+            if samples16 is not None:
+                raise ValueError("samples16= is for an engine with per-stream rates (set_stream_rates)")
+            return int(width)
+        n16 = self._check_samples16(samples16)
+        need = int(inputs_for_rates(self._rates_present(), t, n16).max()) if n16 and self.n_streams else 0
+        if width < need:
+            raise ValueError("audio rows hold %d samples; this call of %d 16 kHz samples needs %d (inputs_for)" % (width, n16, need))
+        return n16
 
     def resampler_history(self) -> int:
-        """input samples each stream keeps as resampler history (0 at 16 kHz)"""
-        rate = self.input_rate
-        n, L = ctypes.c_int(0), ctypes.c_int(1)
-        _lib.check(None, self._L.mww_resample_taps(rate, None, 0, ctypes.byref(n), ctypes.byref(L), None))
-        return -(-n.value // L.value)
+        """input samples each stream keeps as resampler history (0 at 16 kHz; with per-stream rates the row length H_max)"""
+        return resampler_history_len(self.input_rate)
 
     def _get_resampler(self, d: dict) -> None:
         """the resampler's part of state_dict (nothing at 16 kHz)"""
@@ -206,16 +305,24 @@ class _Engine:
         seen = ctypes.c_longlong(0)
         _lib.check(self._h, self._L.mww_get_resampler_state(self._h, hist.ctypes.data, ctypes.byref(seen)))
         d.update(input_rate=self.input_rate, resampler_history=hist, inputs_seen=seen.value)
+        if self.input_rate == RATE_PER_STREAM:
+            d["stream_rates"] = self.stream_rates
 
     def _set_resampler(self, d: dict) -> None:
         rate = int(d.get("input_rate", 16000))
-        if rate != self.input_rate:
+        if rate != self.input_rate and not (rate == RATE_PER_STREAM and self.input_rate == 16000):
             raise ValueError("the state was taken at %d Hz, this engine runs at %d Hz" % (rate, self.input_rate))
         if rate == 16000:
             return
         hist = np.ascontiguousarray(d["resampler_history"], np.int16)
-        if hist.shape != (self.n_streams, self.resampler_history()):
-            raise ValueError("resampler_history must be int16 [n_streams, %d]" % self.resampler_history())
+        if hist.shape != (self.n_streams, resampler_history_len(rate)):
+            raise ValueError("resampler_history must be int16 [n_streams, %d]" % resampler_history_len(rate))
+        if rate == RATE_PER_STREAM:
+            # the rates first (an engine at 16 kHz enters the mode), then the histories and the counter
+            rates = np.ascontiguousarray(d["stream_rates"], np.int32)
+            if rates.shape != (self.n_streams,):
+                raise ValueError("stream_rates must be int32 [n_streams]")
+            self.set_stream_rates(np.arange(self.n_streams, dtype=np.int32), rates)
         _lib.check(self._h, self._L.mww_set_resampler_state(self._h, hist.ctypes.data, int(d["inputs_seen"])))
 
     @property
@@ -291,10 +398,13 @@ class _Engine:
     def reset_frontend(self):
         _lib.check(self._h, self._L.mww_reset_frontend(self._h, self._cu_stream()))
 
-    def features(self, audio, out=None):
-        """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer."""
+    def features(self, audio, out=None, samples16=None):
+        """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer.
+        With per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16)."""
         torch = _torch()
-        n, stride, is_f32 = self._check_audio(audio)
+        width, stride, is_f32 = self._check_audio(audio)
+        n = self._call_len(width, samples16)
+        stride = max(stride, width)
         rows = rows_for(self.frontend_buffered, self._samples16(n), self.hop)
         if out is None:
             out = torch.empty((self.n_streams, max(rows, 1), NUM_FEATURES), dtype=torch.uint16, device=self._dev())
@@ -303,7 +413,7 @@ class _Engine:
             raise ValueError("out must be a contiguous CUDA uint16 tensor [n_streams, >= rows, 40]")
         got = ctypes.c_int(0)
         fn = self._L.mww_features_f32 if is_f32 else self._L.mww_features
-        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
+        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, stride, out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
     # ------------------------------------------------------------------ moving streams between engines
@@ -383,7 +493,9 @@ class StreamEngine(_Engine):
     """`model`: path to (or bytes of) an MWW container or a streaming ``.tflite`` flatbuffer (recognised and converted by
     ``tflite_file``, inference.py:36-45), or None for a frontend-only engine."""
 
-    def __init__(self, model, n_streams: int = 1, device: int = 0, input_rate: int = 16000):
+    def __init__(self, model, n_streams: int = 1, device: int = 0, input_rate: int = 16000, stream_rates=None):
+        if stream_rates is not None and input_rate != 16000:
+            raise ValueError("give input_rate= or stream_rates=, not both")
         blob = load_model_blob(model)
         self._L = _lib.lib()
         self._h = ctypes.c_void_p()
@@ -402,6 +514,8 @@ class StreamEngine(_Engine):
         self.hop = HOP          # samples between feature windows (set_window_step)
         if input_rate != 16000:
             self.set_input_rate(input_rate)
+        if stream_rates is not None:
+            self.set_stream_rates(np.arange(self.n_streams, dtype=np.int32), stream_rates)
 
     @property
     def pending_rows(self) -> int:
@@ -443,27 +557,33 @@ class StreamEngine(_Engine):
             raise ValueError("dst_ids and src_ids must have the same length")
         _lib.check(self._h, self._L.mww_copy_nn_state(self._h, d.ctypes.data, src._h, s.ctypes.data, d.size, self._cu_stream()))
 
-    def predict_clip(self, audio, out=None):
+    def predict_clip(self, audio, out=None, samples16=None):
         """int16 or float32 CUDA tensor [S, N] -> float32 probabilities [S, steps]; state carries over between calls.  float32
-        samples are converted to int16 inside the frontend kernels (x * 32768, clipped, as audio_utils.to_int16)."""
+        samples are converted to int16 inside the frontend kernels (x * 32768, clipped, as audio_utils.to_int16).  With
+        per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16)."""
         torch = _torch()
-        n, stride, is_f32 = self._check_audio(audio)
+        width, stride, is_f32 = self._check_audio(audio)
+        n = self._call_len(width, samples16)
+        stride = max(stride, width)
         steps = self._steps(n)
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
         got = ctypes.c_int(0)
         fn = self._L.mww_predict_clip_f32 if is_f32 else self._L.mww_predict_clip
-        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
+        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, stride, out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
-    step = predict_clip  # the live "one chunk of new audio per call" surface (north_star step())
+    def step(self, audio, out=None):
+        """the live "one chunk of new audio per call" surface (north_star step()): predict_clip; with per-stream rates a
+        30 ms call (samples16 = 480)"""
+        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None)
 
-    def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None) -> np.ndarray:
+    def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None, samples16=None) -> np.ndarray:
         """int16 or float32 HOST array [S, N] -> float32 HOST array [S, steps]; copies are pipelined inside the library.
         float32 samples cross PCIe as they are and are converted in the frontend kernels (as predict_clip converts them).
         Other dtypes (float64 included) and wrong shapes: ValueError; a too-small `out`: MwwError."""
         audio, stride, is_f32 = self._check_host_audio(audio)
-        n = audio.shape[1]
+        n = self._call_len(audio.shape[1], samples16)
         steps = self._steps(n)
         if out is None:
             out = np.empty((self.n_streams, max(steps, 1)), np.float32)
@@ -472,23 +592,27 @@ class StreamEngine(_Engine):
         _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, out.ctypes.data, out.shape[1], ctypes.byref(got)))
         return out[:, :got.value]
 
-    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None, dtype=np.int16):
+    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None, dtype=np.int16,
+                            samples16=None):
         """Audio [S, n_samples] of `dtype` (int16 or float32; stride in samples) at address `src_ptr` -- device memory of a PEER
         GPU mapped into this process (sharding.IngestBuffer.block_ptr) or host memory (mww_predict_clip_remote[_f32]).
         tiles = 0: a peer-mapped (or local) buffer is read in place by the frontend kernel, over NVLink; host memory is staged
         in 16 tiles.  tiles > 0: always staged -- this GPU's copy engine pulls tile t+1 while tile t computes.  Returns float32
-        CUDA probabilities [S, steps]; stream-ordered like predict_clip."""
+        CUDA probabilities [S, steps]; stream-ordered like predict_clip.  With per-stream rates n_samples is the samples each
+        row holds (>= every inputs_for(samples16)) and samples16= the call."""
         torch = _torch()
         fn = self._remote_fn(dtype, "mww_predict_clip_remote")
-        n = int(n_samples)
+        width = int(n_samples)
+        n = self._call_len(width, samples16)
+        stride = int(stride) if stride else width
         steps = self._steps(n)
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
         else:
             self._check_probs_out(out)
         got = ctypes.c_int(0)
-        _lib.check(self._h, fn(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n, out.data_ptr(),
-                               out.shape[1], ctypes.byref(got), int(tiles), self._cu_stream()))
+        _lib.check(self._h, fn(self._h, ctypes.c_void_p(int(src_ptr)), n, stride, out.data_ptr(), out.shape[1], ctypes.byref(got),
+                               int(tiles), self._cu_stream()))
         return out[:, :got.value]
 
     # ------------------------------------------------------------------ state (checkpoint / tests)
@@ -533,7 +657,9 @@ class MultiModelEngine(_Engine):
     them only, and its results have one row per id, in that order (row j belongs to stream streams[k][j]).  Unsorted,
     duplicate or out-of-range ids raise ValueError.  `engine.streams[k]` is model k's set (int32), `set_streams` changes it."""
 
-    def __init__(self, models, n_streams: int = 1, device: int = 0, streams=None, input_rate: int = 16000):
+    def __init__(self, models, n_streams: int = 1, device: int = 0, streams=None, input_rate: int = 16000, stream_rates=None):
+        if stream_rates is not None and input_rate != 16000:
+            raise ValueError("give input_rate= or stream_rates=, not both")
         blobs = [load_model_blob(m) for m in models]
         if any(b is None for b in blobs):
             raise ValueError("every model must be a path or the bytes of a model file")
@@ -567,6 +693,8 @@ class MultiModelEngine(_Engine):
         self.streams = [self._get_streams(k) for k in range(K)]
         if input_rate != 16000:
             self.set_input_rate(input_rate)
+        if stream_rates is not None:
+            self.set_stream_rates(np.arange(self.n_streams, dtype=np.int32), stream_rates)
 
     @staticmethod
     def _stream_set(ids, n_streams: int) -> np.ndarray:
@@ -631,34 +759,39 @@ class MultiModelEngine(_Engine):
         maxp = (ctypes.c_int * K)(*[o.shape[1] for o in out])
         return out, ptrs, maxp, (ctypes.c_int * K)()
 
-    def predict_clip(self, audio, out=None) -> list:
+    def predict_clip(self, audio, out=None, samples16=None) -> list:
         """int16 or float32 CUDA tensor [S, N] -> [float32 probabilities [S, steps_k] for each model k]; state carries over
-        between calls.  `out`: one CUDA float32 buffer [S, >= steps_k] per model to write into."""
-        n, stride, is_f32 = self._check_audio(audio)
+        between calls.  `out`: one CUDA float32 buffer [S, >= steps_k] per model to write into.  samples16=: as
+        StreamEngine.predict_clip."""
+        width, stride, is_f32 = self._check_audio(audio)
+        n = self._call_len(width, samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
         fn = self._L.mww_predict_clip_multi_f32 if is_f32 else self._L.mww_predict_clip_multi
-        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, n), ptrs, maxp, got, self._cu_stream()))
+        _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, width), ptrs, maxp, got, self._cu_stream()))
         return [o[:, :g] for o, g in zip(out, got)]
 
-    step = predict_clip
+    def step(self, audio, out=None) -> list:
+        """predict_clip; with per-stream rates a 30 ms call (samples16 = 480)"""
+        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None)
 
-    def predict_clip_host(self, audio: np.ndarray, out=None) -> list:
+    def predict_clip_host(self, audio: np.ndarray, out=None, samples16=None) -> list:
         """int16 or float32 HOST array [S, N] -> [float32 HOST array [S, steps_k] for each model k]; each audio tile is copied
         once."""
         audio, stride, is_f32 = self._check_host_audio(audio)
-        n = audio.shape[1]
+        n = self._call_len(audio.shape[1], samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, True)
         fn = self._L.mww_predict_clip_host_multi_f32 if is_f32 else self._L.mww_predict_clip_host_multi
         _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, ptrs, maxp, got))
         return [o[:, :g] for o, g in zip(out, got)]
 
     def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None,
-                            dtype=np.int16) -> list:
+                            dtype=np.int16, samples16=None) -> list:
         """StreamEngine.predict_clip_remote for every model: one result per model, each audio tile pulled once."""
         fn = self._remote_fn(dtype, "mww_predict_clip_remote_multi")
-        n = int(n_samples)
+        width = int(n_samples)
+        n = self._call_len(width, samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
-        _lib.check(self._h, fn(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else n, ptrs, maxp, got, int(tiles),
+        _lib.check(self._h, fn(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else width, ptrs, maxp, got, int(tiles),
                                self._cu_stream()))
         return [o[:, :g] for o, g in zip(out, got)]
 
