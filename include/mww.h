@@ -547,6 +547,76 @@ int mww_detector_reset_device(mww_detector_t *d, const int32_t *d_rows, int n, v
 int mww_detector_get_state(mww_detector_t *d, float *h_hist, long long *h_seen, int32_t *h_cooldown);
 int mww_detector_set_state(mww_detector_t *d, const float *h_hist, const long long *h_seen, const int32_t *h_cooldown);
 
+/* ---- Multi-model streaming detector: a rule per model of a handle, WAKE detections gated by a VAD model ---------------
+ * A deployment that runs K wake-word and VAD models over one frontend (mww_create_multi) turns all their probabilities into
+ * one event stream with one launch per call, and lets the VAD stop a wake word from firing while nobody speaks.
+ *
+ * The detector is created from a handle with K models.  At creation it copies each model's stride s_k and stream set S_k,
+ * and it keeps them.  Each model gets a rule with one of three roles:
+ *   - WAKE: (window_k, cutoff_k, cooldown_k).
+ *   - VAD: (window_v, cutoff_v).  At most one model may be the VAD.
+ *   - OFF: ignored.
+ * At least one model must be WAKE.  Each model has one state row per member of S_k, in list order, as its probabilities do.
+ * A WAKE row keeps what a plain detector row keeps: hist, seen and cooldown.  A VAD row keeps hist, seen and active, a 0/1
+ * flag.
+ *
+ * Step timing.  An update describes one handle call.  For each model k it gives:
+ *   - n_k, the steps model k ran in that call;
+ *   - p_k, the model's pending rows before that call.
+ * Step j of the call (0 <= j < n_k) ends at call-relative feature row e_k(j) = (j + 1) s_k - p_k - 1.  The rows that call
+ * produced, R, are not passed in.  The update is accepted only if one R >= 0 fits every non-OFF model: n_k = (p_k + R) div
+ * s_k and 0 <= p_k < s_k.  Otherwise it returns MWW_EINVAL before any launch.  This catches a skipped call, or a handle reset
+ * that the detector was not told about, in most cases.
+ *
+ * Order within a stream.  A stream's steps are processed in order of e.  When a VAD step and a WAKE step end on the same
+ * row, the VAD step goes first.
+ *
+ * VAD step.  It runs the moving average of the plain detector: float32 window_mean, a sequential sum and one division.  Then
+ * active = (seen_v >= window_v) && (double)avg > cutoff_v, with seen_v counting this step.  So NaN gives false, and the flag
+ * stays false until the row has seen a full window.  A stream that is not in S_v is never active.
+ *
+ * WAKE step (stream s = S_k[r]).  It is the plain detector's rule with one extra condition:
+ *   - cooldown = max(cooldown - 1, 0);
+ *   - the row fires iff cooldown == 0 && (double)avg > cutoff_k && gate, and then cooldown = cooldown_k;
+ *   - gate is the active flag of stream s's VAD row, or true when no model is the VAD.
+ * If the gate refuses a candidate, the row does not fire and the cooldown is not set.  Nothing happens before the row has
+ * seen window_k probabilities.
+ *
+ * Events use the mww_event layout: stream = the global stream id; reserved = the model index k (it stays 0 for the plain
+ * detector); step = model k's probability index since the row's last reset; score = the average.  d_fired holds global
+ * stream ids, so mww_reset_device_ids(h, d_fired, capacity, stream) restarts every stream on which any wake word fired.
+ *
+ * Resets take GLOBAL stream ids.  For each listed stream it resets the stream's VAD row (zero hist, seen = 0, active = 0) and
+ * every WAKE row of that stream (zero hist, seen = 0, cooldown = cooldown_k).
+ *
+ * Consequences: without a VAD, model k's events and state are bit-identical to those of a plain detector (n_k rows,
+ * cutoff_k, window_k, cooldown_k, stream map S_k) fed the same probabilities; and events and state do not depend on how the
+ * audio was split into calls, as long as every call's probabilities are passed.
+ *
+ *   - create: reads the handle through host-side calls only (K, strides, device, n_streams, stream sets) and does no device
+ *     work on it.  MWW_EINVAL with a message for a frontend-only handle, a role outside the three, zero WAKE models or two
+ *     VAD models, a window outside [1, 32], a non-finite cutoff or a negative cooldown of a used model, capacity < 1; without
+ *     a CUDA device MWW_ECUDA ("no CUDA device").  The VAD's cooldown_slices is not used.
+ *   - update: d_probs[k] is [n_k members][pitch[k]] in device memory (pitch[k] >= n_steps[k]); OFF models' entries,
+ *     and those of models with no members or no steps, may be NULL.  One launch, or none when every n_k is 0; no
+ *     host-to-device copy.  Asynchronous on cu_stream.
+ *   - shared with the plain detector: mww_detector_destroy, _drain, _buffers, _reset and _reset_device (global stream ids
+ *     here; a NULL list resets every stream).  mww_detector_update, _get_state and _set_state on a models detector return
+ *     MWW_EINVAL, and so does mww_multi_detector_update on a plain detector.
+ *   - get_state / set_state: model k's rows in list order, host buffers, synchronous, NULL pointers skipped:
+ *     hist [n_k][window_k - 1] oldest first, seen [n_k], and cooldown [n_k] (WAKE) or active [n_k] (VAD).  set refuses a
+ *     negative seen, a cooldown outside [0, cooldown_k] and an active outside {0, 1}; an OFF model is MWW_EINVAL. */
+#define MWW_DETECT_OFF 0
+#define MWW_DETECT_WAKE 1
+#define MWW_DETECT_VAD 2
+typedef struct mww_detect_rule { int32_t role, window, cooldown_slices, pad; double cutoff; } mww_detect_rule;
+int mww_multi_detector_create(const mww_t *h, const mww_detect_rule *rules /* [K] */, int capacity, mww_detector_t **out);
+int mww_multi_detector_update(mww_detector_t *d, const float *const *d_probs, const long long *pitch,
+                               const int *n_steps, const int *pending_before, void *cu_stream);
+int mww_multi_detector_get_state(mww_detector_t *d, int k, float *h_hist, long long *h_seen, int32_t *h_cooldown_or_active);
+int mww_multi_detector_set_state(mww_detector_t *d, int k, const float *h_hist, const long long *h_seen,
+                                 const int32_t *h_cooldown_or_active);
+
 #ifdef __cplusplus
 }
 #endif

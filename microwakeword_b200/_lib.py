@@ -34,6 +34,7 @@ EXPORTS = (
     "mww_set_stream_rates", "mww_get_stream_rates", "mww_rate_inputs",
     "mww_detector_create", "mww_detector_destroy", "mww_detector_update", "mww_detector_drain", "mww_detector_buffers",
     "mww_detector_reset", "mww_detector_reset_device", "mww_detector_get_state", "mww_detector_set_state",
+    "mww_multi_detector_create", "mww_multi_detector_update", "mww_multi_detector_get_state", "mww_multi_detector_set_state",
 )
 
 
@@ -62,6 +63,15 @@ class MwwEvent(ctypes.Structure):
     """mww_event of include/mww.h: one detection of a streaming detector"""
     _fields_ = [("stream", ctypes.c_int32), ("reserved", ctypes.c_int32), ("step", ctypes.c_int64), ("score", ctypes.c_float),
                 ("pad", ctypes.c_int32)]
+
+
+MWW_DETECT_OFF, MWW_DETECT_WAKE, MWW_DETECT_VAD = 0, 1, 2
+
+
+class MwwDetectRule(ctypes.Structure):
+    """mww_detect_rule of include/mww.h: one model's rule in a models detector"""
+    _fields_ = [("role", ctypes.c_int32), ("window", ctypes.c_int32), ("cooldown_slices", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("cutoff", ctypes.c_double)]
 
 
 class MwwError(RuntimeError):
@@ -220,6 +230,13 @@ def lib() -> ctypes.CDLL:
     for name in ("mww_detector_get_state", "mww_detector_set_state"):
         getattr(L, name).restype = i32
         getattr(L, name).argtypes = [vp, vp, vp, vp]
+    L.mww_multi_detector_create.restype = i32
+    L.mww_multi_detector_create.argtypes = [vp, ctypes.POINTER(MwwDetectRule), i32, ctypes.POINTER(vp)]
+    L.mww_multi_detector_update.restype = i32
+    L.mww_multi_detector_update.argtypes = [vp, vp, vp, vp, vp, vp]
+    for name in ("mww_multi_detector_get_state", "mww_multi_detector_set_state"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, i32, vp, vp, vp]
     _lib = L
     return L
 

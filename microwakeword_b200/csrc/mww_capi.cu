@@ -2037,6 +2037,12 @@ struct mww_detector {
     int32_t *d_stream_ids = nullptr;
     int32_t *d_rows = nullptr;       // staging for a host row list (mww_detector_reset)
     size_t rows_cap = 0;
+    // a models detector (mww_multi_detector_create): a.count / events / fired / capacity are its event buffers, the rest of
+    // `a` is unused; `m` holds the kernels' arguments, models[k] the descriptors d_models holds on the device
+    bool multi = false;
+    DetectModelsArgs m;
+    std::vector<DetectModel> models;
+    DetectModel *d_models = nullptr;
 };
 
 namespace {
@@ -2047,6 +2053,10 @@ namespace {
 void detector_free(mww_detector_t *d) {
     cudaFree(d->a.hist); cudaFree(d->a.seen); cudaFree(d->a.cooldown); cudaFree(d->a.count); cudaFree(d->a.events);
     cudaFree(d->a.fired); cudaFree(d->d_stream_ids); cudaFree(d->d_rows);
+    for (DetectModel &M : d->models) {
+        cudaFree(M.hist); cudaFree(M.seen); cudaFree(M.flag); cudaFree(const_cast<int32_t *>(M.inv));
+    }
+    cudaFree(d->d_models);
     delete d;
 }
 
@@ -2113,6 +2123,7 @@ int mww_detector_destroy(mww_detector_t *d) {
 
 int mww_detector_update(mww_detector_t *d, const float *d_probs, int n_steps, long long pitch, void *cu_stream) {
     if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_update: detector is NULL");
+    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_detector_update: a models detector takes mww_multi_detector_update");
     if (n_steps < 0 || (n_steps > 0 && (!d_probs || pitch < n_steps)))
         return fail(nullptr, MWW_EINVAL, "mww_detector_update: needs d_probs and n_steps >= 0 columns within the row pitch");
     if (n_steps == 0) return MWW_OK;
@@ -2153,7 +2164,8 @@ int mww_detector_buffers(mww_detector_t *d, const long long **d_count, const mww
 int mww_detector_reset_device(mww_detector_t *d, const int32_t *d_rows, int n, void *cu_stream) {
     if (!d || n < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_reset_device: needs a detector and n >= 0");
     DENTER(d);
-    DCU(launch_detector_reset(d->a, d_rows, d_rows ? n : d->a.n_rows, static_cast<cudaStream_t>(cu_stream)));
+    if (d->multi) DCU(launch_detector_models_reset(d->m, d_rows, d_rows ? n : d->m.n_streams, static_cast<cudaStream_t>(cu_stream)));
+    else DCU(launch_detector_reset(d->a, d_rows, d_rows ? n : d->a.n_rows, static_cast<cudaStream_t>(cu_stream)));
     return MWW_OK;
 }
 
@@ -2170,12 +2182,14 @@ int mww_detector_reset(mww_detector_t *d, const int32_t *h_rows, int n, void *cu
         d->rows_cap = want;
     }
     DCU(cudaMemcpyAsync(d->d_rows, h_rows, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    DCU(launch_detector_reset(d->a, d->d_rows, n, st));
+    if (d->multi) DCU(launch_detector_models_reset(d->m, d->d_rows, n, st));
+    else DCU(launch_detector_reset(d->a, d->d_rows, n, st));
     return MWW_OK;
 }
 
 int mww_detector_get_state(mww_detector_t *d, float *h_hist, long long *h_seen, int32_t *h_cooldown) {
     if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_get_state: detector is NULL");
+    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_detector_get_state: a models detector takes mww_multi_detector_get_state");
     DENTER(d);
     DCU(cudaDeviceSynchronize());
     const size_t R = (size_t)d->a.n_rows, W = (size_t)d->a.rule.window - 1;
@@ -2192,6 +2206,7 @@ int mww_detector_get_state(mww_detector_t *d, float *h_hist, long long *h_seen, 
 
 int mww_detector_set_state(mww_detector_t *d, const float *h_hist, const long long *h_seen, const int32_t *h_cooldown) {
     if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: detector is NULL");
+    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: a models detector takes mww_multi_detector_set_state");
     const size_t R = (size_t)d->a.n_rows, W = (size_t)d->a.rule.window - 1;
     for (size_t r = 0; r < R; ++r) {
         if (h_seen && h_seen[r] < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: seen must not be negative");
@@ -2208,6 +2223,198 @@ int mww_detector_set_state(mww_detector_t *d, const float *h_hist, const long lo
     }
     if (h_seen) DCU(cudaMemcpy(d->a.seen, h_seen, R * sizeof(long long), cudaMemcpyHostToDevice));
     if (h_cooldown) DCU(cudaMemcpy(d->a.cooldown, h_cooldown, R * sizeof(int32_t), cudaMemcpyHostToDevice));
+    return MWW_OK;
+}
+
+}  // extern "C"
+
+// ---- multi-model detector (include/mww.h; rule and kernels: mww_detector_models.h, mww_detector_models.cu) ----------------
+namespace {
+
+int models_fail(const char *what) { return fail(nullptr, MWW_EINVAL, std::string("mww_multi_detector_create: ") + what); }
+
+// device state for the rules the create checked: each used model's rows, its inverse map unless it runs on every stream,
+// the descriptors, and the event buffers the plain detector's calls drain
+int models_alloc(mww_detector_t *d, const std::vector<std::vector<int32_t>> &ids) {
+    DetectModelsArgs &m = d->m;
+    const size_t C = (size_t)d->a.capacity, S = (size_t)m.n_streams;
+    for (int k = 0; k < m.n_models; ++k) {
+        DetectModel &M = d->models[k];
+        if (M.role == MWW_DETECT_OFF) continue;
+        const size_t R = (size_t)M.n_rows, W = (size_t)M.rule.window - 1;
+        DCU(cudaMalloc(&M.hist, std::max<size_t>(W * R, 1) * sizeof(float)));
+        DCU(cudaMalloc(&M.seen, std::max<size_t>(R, 1) * sizeof(long long)));
+        DCU(cudaMalloc(&M.flag, std::max<size_t>(R, 1) * sizeof(int32_t)));
+        if (R != S) {                                   // a stream set is all streams exactly when it has every id
+            std::vector<int32_t> inv(S, -1);
+            for (size_t r = 0; r < R; ++r) inv[ids[k][r]] = (int32_t)r;
+            int32_t *d_inv = nullptr;
+            DCU(cudaMalloc(&d_inv, S * sizeof(int32_t)));
+            M.inv = d_inv;
+            DCU(cudaMemcpy(d_inv, inv.data(), S * sizeof(int32_t), cudaMemcpyHostToDevice));
+        }
+    }
+    DCU(cudaMalloc(&d->d_models, d->models.size() * sizeof(DetectModel)));
+    DCU(cudaMemcpy(d->d_models, d->models.data(), d->models.size() * sizeof(DetectModel), cudaMemcpyHostToDevice));
+    m.models = d->d_models;
+    DCU(cudaMalloc(&d->a.count, sizeof(unsigned long long)));
+    DCU(cudaMalloc(&d->a.events, C * sizeof(mww_event)));
+    DCU(cudaMalloc(&d->a.fired, C * sizeof(int32_t)));
+    m.count = d->a.count; m.events = d->a.events; m.fired = d->a.fired; m.capacity = d->a.capacity;
+    DCU(cudaMemset(d->a.count, 0, sizeof(unsigned long long)));
+    DCU(cudaMemset(d->a.events, 0, C * sizeof(mww_event)));
+    DCU(cudaMemset(d->a.fired, 0xFF, C * sizeof(int32_t)));           // -1 in every slot
+    DCU(launch_detector_models_reset(m, nullptr, m.n_streams, nullptr));
+    DCU(cudaDeviceSynchronize());
+    return MWW_OK;
+}
+
+// model k of a models detector, or a refusal naming the call
+int model_arg(mww_detector_t *d, int k, const char *call, const DetectModel **out) {
+    if (!d) return fail(nullptr, MWW_EINVAL, std::string(call) + ": detector is NULL");
+    if (!d->multi) return fail(nullptr, MWW_EINVAL, std::string(call) + ": not a models detector (mww_multi_detector_create)");
+    if (k < 0 || k >= d->m.n_models) return fail(nullptr, MWW_EINVAL, std::string(call) + ": model index out of range");
+    if (d->models[k].role == MWW_DETECT_OFF) return fail(nullptr, MWW_EINVAL, std::string(call) + ": model is OFF");
+    *out = &d->models[k];
+    return MWW_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mww_multi_detector_create(const mww_t *h, const mww_detect_rule *rules, int capacity, mww_detector_t **out) {
+    if (!out) return models_fail("out is NULL");
+    *out = nullptr;
+    if (!rules) return models_fail("rules is NULL");
+    if (capacity < 1) return models_fail("capacity must be at least 1");
+    int count = 0;
+    cudaError_t e = cudaGetDeviceCount(&count);
+    if (e != cudaSuccess || count == 0)
+        return fail(nullptr, MWW_ECUDA, std::string("no CUDA device available (this library has no CPU fallback): ") + cudaGetErrorString(e));
+    if (!h) return models_fail("handle is NULL");
+    const int K = mww_model_count(h);
+    if (K < 1) return models_fail("the handle is frontend-only: it has no models to detect with");
+    int n_wake = 0, vad = -1;
+    for (int k = 0; k < K; ++k) {
+        const mww_detect_rule &r = rules[k];
+        const std::string at = "model " + std::to_string(k) + ": ";
+        if (r.role != MWW_DETECT_OFF && r.role != MWW_DETECT_WAKE && r.role != MWW_DETECT_VAD)
+            return models_fail((at + "role must be MWW_DETECT_OFF, _WAKE or _VAD").c_str());
+        if (r.role == MWW_DETECT_OFF) continue;
+        if (r.window < 1 || r.window > kDetectorMaxWindow) return models_fail((at + "window must be in [1, 32]").c_str());
+        if (!(r.cutoff - r.cutoff == 0.0)) return models_fail((at + "cutoff must be finite").c_str());
+        if (r.role == MWW_DETECT_WAKE && r.cooldown_slices < 0) return models_fail((at + "cooldown_slices must not be negative").c_str());
+        if (r.role == MWW_DETECT_WAKE) ++n_wake;
+        if (r.role == MWW_DETECT_VAD) {
+            if (vad >= 0) return models_fail("at most one model may be the VAD");
+            vad = k;
+        }
+    }
+    if (n_wake == 0) return models_fail("at least one model must be WAKE");
+    mww_info info;
+    if (mww_get_info(h, &info) != MWW_OK) return models_fail("cannot read the handle");
+    std::vector<std::vector<int32_t>> ids(K);
+    mww_detector_t *d = new mww_detector;
+    d->device = info.device;
+    d->multi = true;
+    d->a.capacity = capacity;
+    d->models.resize(K);
+    DetectModelsArgs &m = d->m;
+    m.n_streams = info.n_streams; m.n_models = K; m.vad = vad;
+    for (int k = 0; k < K; ++k) {
+        const mww_detect_rule &r = rules[k];
+        DetectModel &M = d->models[k];
+        M.role = r.role;
+        if (r.role == MWW_DETECT_OFF) continue;
+        mww_info mi;
+        int n = 0;
+        if (mww_get_model_info(h, k, &mi) != MWW_OK || mww_get_model_streams(h, k, nullptr, 0, &n) != MWW_OK) { delete d; return models_fail("cannot read a model"); }
+        ids[k].resize((size_t)n);
+        if (n > 0 && mww_get_model_streams(h, k, ids[k].data(), n, &n) != MWW_OK) { delete d; return models_fail("cannot read a stream set"); }
+        M.rule.window = r.window; M.rule.cutoff = r.cutoff; M.rule.cooldown_slices = r.role == MWW_DETECT_WAKE ? r.cooldown_slices : 0;
+        M.stride = std::max(mi.input_feature_slices, 1);
+        M.n_rows = n;
+        if (r.role == MWW_DETECT_WAKE) m.wake[m.n_wake++] = (int8_t)k;
+    }
+    DeviceGuard guard(d->device);
+    if (guard.err != cudaSuccess) { delete d; return cuda_fail(nullptr, guard.err, "cudaSetDevice"); }
+    if (int rc = models_alloc(d, ids)) { detector_free(d); return rc; }
+    *out = d;
+    return MWW_OK;
+}
+
+int mww_multi_detector_update(mww_detector_t *d, const float *const *d_probs, const long long *pitch, const int *n_steps,
+                               const int *pending_before, void *cu_stream) {
+    if (!d) return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: detector is NULL");
+    if (!d->multi) return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: not a models detector (mww_multi_detector_create)");
+    if (!d_probs || !pitch || !n_steps || !pending_before)
+        return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: d_probs, pitch, n_steps and pending_before must not be NULL");
+    DetectModelsArgs &m = d->m;
+    DetectCall call[kDetectMaxModels];
+    bool any = false;
+    for (int k = 0; k < m.n_models; ++k) {
+        const DetectModel &M = d->models[k];
+        if (M.role == MWW_DETECT_OFF) continue;
+        DetectCall &c = call[k];
+        c.probs = d_probs[k]; c.pitch = pitch[k]; c.n_steps = n_steps[k]; c.pending = pending_before[k];
+        if (c.n_steps > 0 && M.n_rows > 0) {
+            if (!c.probs || c.pitch < c.n_steps)
+                return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: model " + std::to_string(k) +
+                                                     " needs d_probs and n_steps columns within the row pitch");
+            any = true;
+        }
+    }
+    if (!detect_call_fits(d->models.data(), call, m.n_models))
+        return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: the step counts and pending rows do not describe one call "
+                                         "(n_k = (p_k + R) div s_k with 0 <= p_k < s_k for one R >= 0)");
+    if (!any) return MWW_OK;
+    DENTER(d);
+    for (int k = 0; k < m.n_models; ++k) m.call[k] = call[k];
+    DCU(launch_detector_models_update(m, static_cast<cudaStream_t>(cu_stream)));
+    return MWW_OK;
+}
+
+int mww_multi_detector_get_state(mww_detector_t *d, int k, float *h_hist, long long *h_seen, int32_t *h_cooldown_or_active) {
+    const DetectModel *M = nullptr;
+    if (int rc = model_arg(d, k, "mww_multi_detector_get_state", &M)) return rc;
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    const size_t R = (size_t)M->n_rows, W = (size_t)M->rule.window - 1;
+    if (R == 0) return MWW_OK;
+    if (h_hist && W) {                              // device [window - 1][n_k] -> host [n_k][window - 1]
+        std::vector<float> t(W * R);
+        DCU(cudaMemcpy(t.data(), M->hist, W * R * sizeof(float), cudaMemcpyDeviceToHost));
+        for (size_t j = 0; j < W; ++j)
+            for (size_t r = 0; r < R; ++r) h_hist[r * W + j] = t[j * R + r];
+    }
+    if (h_seen) DCU(cudaMemcpy(h_seen, M->seen, R * sizeof(long long), cudaMemcpyDeviceToHost));
+    if (h_cooldown_or_active) DCU(cudaMemcpy(h_cooldown_or_active, M->flag, R * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+
+int mww_multi_detector_set_state(mww_detector_t *d, int k, const float *h_hist, const long long *h_seen, const int32_t *h_cooldown_or_active) {
+    const DetectModel *M = nullptr;
+    if (int rc = model_arg(d, k, "mww_multi_detector_set_state", &M)) return rc;
+    const size_t R = (size_t)M->n_rows, W = (size_t)M->rule.window - 1;
+    const int hi = M->role == MWW_DETECT_WAKE ? M->rule.cooldown_slices : 1;
+    for (size_t r = 0; r < R; ++r) {
+        if (h_seen && h_seen[r] < 0) return fail(nullptr, MWW_EINVAL, "mww_multi_detector_set_state: seen must not be negative");
+        if (h_cooldown_or_active && (h_cooldown_or_active[r] < 0 || h_cooldown_or_active[r] > hi))
+            return fail(nullptr, MWW_EINVAL, M->role == MWW_DETECT_WAKE ? "mww_multi_detector_set_state: cooldown outside [0, cooldown_slices]"
+                                                                        : "mww_multi_detector_set_state: active must be 0 or 1");
+    }
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    if (R == 0) return MWW_OK;
+    if (h_hist && W) {
+        std::vector<float> t(W * R);
+        for (size_t j = 0; j < W; ++j)
+            for (size_t r = 0; r < R; ++r) t[j * R + r] = h_hist[r * W + j];
+        DCU(cudaMemcpy(M->hist, t.data(), W * R * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    if (h_seen) DCU(cudaMemcpy(M->seen, h_seen, R * sizeof(long long), cudaMemcpyHostToDevice));
+    if (h_cooldown_or_active) DCU(cudaMemcpy(M->flag, h_cooldown_or_active, R * sizeof(int32_t), cudaMemcpyHostToDevice));
     return MWW_OK;
 }
 

@@ -143,3 +143,13 @@ cudaError_t launch_detector_update(const DetectorArgs &a, const float *probs, in
 // fresh state for the n listed rows (device memory; indices out of range ignored) or, rows == nullptr, for rows [0, n)
 cudaError_t launch_detector_reset(const DetectorArgs &a, const int32_t *rows, int n, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_detector_models.h"
+namespace mww {
+// multi-model detector (mww_detector_models.cu, rule and per-stream body in mww_detector_models.h): one call of every model,
+// a thread per stream of the handle
+cudaError_t launch_detector_models_update(const DetectModelsArgs &a, cudaStream_t st);
+// fresh state of every model's row of the n listed GLOBAL stream ids (device memory; out of range ignored) or, ids ==
+// nullptr, of streams [0, n)
+cudaError_t launch_detector_models_reset(const DetectModelsArgs &a, const int32_t *ids, int n, cudaStream_t st);
+}  // namespace mww

@@ -15,6 +15,8 @@ scores -- not every probability -- have to leave the GPU.
 Live, the same rule runs per stream with its state carried across calls:
 
     StreamDetector(n_rows, cutoff, window=5, cooldown_slices=25)   probabilities in (update), detections out (drain)
+    MultiModelDetector(engine, cutoffs, windows, cooldown_slices, vad)   the same for every model of a MultiModelEngine in
+                                                                       one launch, wake words gated by a VAD model
 """
 
 from __future__ import annotations
@@ -364,3 +366,183 @@ class StreamDetector:
         if hist.shape != (self.n_rows, self.window - 1) or seen.shape != (self.n_rows,) or cooldown.shape != (self.n_rows,):
             raise ValueError("state must be hist [n_rows, window - 1], seen [n_rows], cooldown [n_rows]")
         self._check(self._L.mww_detector_set_state(self._d, hist.ctypes.data, seen.ctypes.data, cooldown.ctypes.data))
+
+
+# ---- the multi-model streaming detector ----------------------------------------------------------------------------------
+MODEL_EVENT_DTYPE = np.dtype([("stream", np.int32), ("model", np.int32), ("step", np.int64), ("score", np.float32), ("pad", np.int32)])
+
+
+def _per_model(value, K, name):
+    v = list(value) if isinstance(value, (list, tuple, np.ndarray)) else [value] * K
+    if len(v) != K:
+        raise ValueError("%s must be one value or one per model (%d)" % (name, K))
+    return v
+
+
+class MultiModelDetector:
+    """One detector over the K models of a MultiModelEngine (mww_multi_detector_create of include/mww.h): each model WAKE
+    (the StreamDetector rule), the VAD or OFF, every model's probabilities of a call in one launch, one event stream.  A WAKE
+    model fires only on streams whose VAD row is active (the VAD's moving average above its cutoff); without a VAD each
+    WAKE model is exactly a StreamDetector over its stream set.
+
+        det = MultiModelDetector(eng, cutoffs=[0.97, 0.95, 0.5], windows=[5, 5, 10], vad=2)
+        det.update(eng.step(chunk))            # one launch for every model
+        events, dropped = det.drain()          # now and then: events with a `model` field
+        eng.reset(det.fired_ids)               # the streams on which any wake word fired, global ids
+        det.reset(det.fired_ids)
+
+    `cutoffs[k] = None` makes model k OFF; `windows` and `cooldown_slices` are one value or one per model (the VAD's
+    cooldown is not used).  The detector copies the engine's strides and stream sets at creation and reads its pending rows
+    then and after every update: it must see every call the engine makes, and after `engine.reset()` it needs `reset()`;
+    after `engine.set_streams` make a new one."""
+
+    def __init__(self, engine, cutoffs, windows=5, cooldown_slices: int = 25, vad=None, capacity: int = 65536):
+        K = engine.n_models
+        cutoffs = _per_model(cutoffs, K, "cutoffs")
+        windows = _per_model(windows, K, "windows")
+        cooldowns = _per_model(cooldown_slices, K, "cooldown_slices")
+        if vad is not None and not 0 <= int(vad) < K:
+            raise ValueError("vad must be a model index in [0, %d)" % K)
+        if vad is not None and cutoffs[int(vad)] is None:
+            raise ValueError("the VAD model needs a cutoff")
+        rules = (_lib.MwwDetectRule * K)()
+        for k in range(K):
+            role = (_lib.MWW_DETECT_OFF if cutoffs[k] is None else
+                    _lib.MWW_DETECT_VAD if vad is not None and k == int(vad) else _lib.MWW_DETECT_WAKE)
+            rules[k] = _lib.MwwDetectRule(role, int(windows[k]), int(cooldowns[k]), 0, 0.0 if cutoffs[k] is None else float(cutoffs[k]))
+        self._L = _lib.lib()
+        d = ctypes.c_void_p()
+        self._check(self._L.mww_multi_detector_create(engine._h, rules, int(capacity), ctypes.byref(d)))
+        self._handle = _DetectorHandle(self._L, d)
+        self.engine, self.n_models, self.device, self.capacity = engine, K, int(engine.device), int(capacity)
+        self.roles = [r.role for r in rules]
+        self.vad = None if vad is None else int(vad)
+        self.windows = [int(w) for w in windows]
+        self.cutoffs = [None if c is None else float(c) for c in cutoffs]
+        self.cooldown_slices = [int(c) for c in cooldowns]
+        self.streams = [s.copy() for s in engine.streams]
+        self._pending = list(engine.pending_rows)
+        count, fired = ctypes.c_void_p(), ctypes.c_void_p()
+        self._check(self._L.mww_detector_buffers(self._d, ctypes.byref(count), None, ctypes.byref(fired), None))
+        import torch
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(dev):
+            # device views: the global stream of every event since the last drain (-1 in unused slots), and how many fired
+            self.fired_ids = torch.as_tensor(_DeviceArray(self._handle, fired.value, self.capacity, "<i4"), device=dev)
+            self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
+
+    def _check(self, rc: int) -> None:
+        if rc != 0:
+            msg = self._L.mww_last_error(None)
+            raise _lib.MwwError(rc, msg.decode() if msg else "detector call failed")
+
+    @property
+    def _d(self):
+        return self._handle.ptr
+
+    def close(self):
+        """free the detector now; fired_ids and event_count must not be used afterwards"""
+        self._handle.close()
+
+    @property
+    def pending_rows(self) -> list:
+        """each model's pending rows before the next call, as the detector will describe it"""
+        return list(self._pending)
+
+    def update(self, probs) -> None:
+        """`probs`: what one engine call returned, one CUDA float32 tensor [members of model k, steps_k] per model (any row
+        pitch; an OFF model's entry is not read and may be None).  Asynchronous on the current CUDA stream."""
+        import torch
+        K = self.n_models
+        if len(probs) != K:
+            raise ValueError("probs must hold one entry per model (%d)" % K)
+        if any(not np.array_equal(a, b) for a, b in zip(self.streams, self.engine.streams)):
+            raise ValueError("the engine's stream sets changed since this detector was made: make a new detector")
+        ptrs, pitch, steps = (ctypes.c_void_p * K)(), (ctypes.c_longlong * K)(), (ctypes.c_int * K)()
+        keep = []
+        for k, p in enumerate(probs):
+            if self.roles[k] == _lib.MWW_DETECT_OFF:
+                continue
+            rows = self.streams[k].size
+            if (not isinstance(p, torch.Tensor) or not p.is_cuda or p.dtype != torch.float32 or p.dim() != 2 or p.shape[0] != rows
+                    or p.device.index != self.device):
+                raise ValueError("probs[%d] must be a CUDA float32 tensor [%d streams of model %d, steps] on device %d" % (k, rows, k, self.device))
+            n = p.shape[1]
+            if n and ((n > 1 and p.stride(1) != 1) or (rows > 1 and p.stride(0) < n)):
+                p = p.contiguous()
+            keep.append(p)
+            ptrs[k] = p.data_ptr() if n and rows else None
+            pitch[k] = p.stride(0) if rows > 1 else n
+            steps[k] = n
+        pend = (ctypes.c_int * K)(*self._pending)
+        self._check(self._L.mww_multi_detector_update(self._d, ptrs, pitch, steps, pend, _stream(torch.device("cuda", self.device))))
+        self._pending = list(self.engine.pending_rows)
+
+    def drain(self):
+        """-> (events, dropped): the events since the last drain (MODEL_EVENT_DTYPE, global stream ids) sorted by (model, step,
+        stream), and how many more fired than `capacity` could hold.  Waits for the current CUDA stream; clears the event
+        buffer and fired_ids."""
+        import torch
+        buf = np.empty(self.capacity, MODEL_EVENT_DTYPE)
+        n = ctypes.c_longlong(0)
+        self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), _stream(torch.device("cuda", self.device))))
+        ev = buf[:min(n.value, self.capacity)]
+        return ev[np.lexsort((ev["stream"], ev["step"], ev["model"]))], max(n.value - self.capacity, 0)
+
+    def reset(self, stream_ids=None) -> None:
+        """Fresh detector state of every model for all streams (None; the engine's pending rows are read again, so this is
+        the call to make after engine.reset()) or the given GLOBAL stream ids: a host sequence, or a contiguous 1-D CUDA
+        int32 tensor such as fired_ids.  Ids out of range are ignored."""
+        import torch
+        st = _stream(torch.device("cuda", self.device))
+        if stream_ids is None:
+            self._check(self._L.mww_detector_reset(self._d, None, 0, st))
+            self._pending = list(self.engine.pending_rows)
+        elif isinstance(stream_ids, torch.Tensor) and stream_ids.is_cuda:
+            if stream_ids.dtype != torch.int32 or stream_ids.dim() != 1 or not stream_ids.is_contiguous():
+                raise ValueError("device stream ids must be a contiguous 1-D CUDA int32 tensor")
+            self._check(self._L.mww_detector_reset_device(self._d, stream_ids.data_ptr(), stream_ids.numel(), st))
+        else:
+            ids = np.ascontiguousarray(stream_ids, np.int32).reshape(-1)
+            self._check(self._L.mww_detector_reset(self._d, ids.ctypes.data, ids.size, st))
+
+    def _flag_name(self, k):
+        return "active" if self.roles[k] == _lib.MWW_DETECT_VAD else "cooldown"
+
+    def state_dict(self) -> dict:
+        """{pending_rows: [p_k], models: [None for an OFF model, else {hist [n_k, window - 1], seen [n_k], cooldown or active [n_k]}]}"""
+        models = []
+        for k in range(self.n_models):
+            if self.roles[k] == _lib.MWW_DETECT_OFF:
+                models.append(None)
+                continue
+            n = self.streams[k].size
+            m = {"hist": np.zeros((n, self.windows[k] - 1), np.float32), "seen": np.zeros(n, np.int64), self._flag_name(k): np.zeros(n, np.int32)}
+            self._check(self._L.mww_multi_detector_get_state(self._d, k, m["hist"].ctypes.data, m["seen"].ctypes.data, m[self._flag_name(k)].ctypes.data))
+            models.append(m)
+        return dict(pending_rows=list(self._pending), models=models)
+
+    def load_state_dict(self, d: dict) -> None:
+        if len(d["models"]) != self.n_models or len(d["pending_rows"]) != self.n_models:
+            raise ValueError("the state holds %d models, this detector %d" % (len(d["models"]), self.n_models))
+        arrays = []
+        for k, m in enumerate(d["models"]):
+            if self.roles[k] == _lib.MWW_DETECT_OFF:
+                arrays.append(None)
+                continue
+            if m is None:
+                raise ValueError("model %d has no state" % k)
+            n, flag = self.streams[k].size, self._flag_name(k)
+            hist = np.ascontiguousarray(m["hist"], np.float32)
+            seen = np.ascontiguousarray(m["seen"], np.int64)
+            f = np.ascontiguousarray(m[flag], np.int32)
+            if hist.shape != (n, self.windows[k] - 1) or seen.shape != (n,) or f.shape != (n,):
+                raise ValueError("model %d: state must be hist [%d, window - 1], seen [%d], %s [%d]" % (k, n, n, flag, n))
+            hi = 1 if self.roles[k] == _lib.MWW_DETECT_VAD else self.cooldown_slices[k]
+            if (seen < 0).any() or (f < 0).any() or (f > hi).any():       # checked for every model before any is written
+                raise ValueError("model %d: seen must not be negative and %s must be in [0, %d]" % (k, flag, hi))
+            arrays.append((hist, seen, f))
+        for k, a in enumerate(arrays):
+            if a is not None:
+                self._check(self._L.mww_multi_detector_set_state(self._d, k, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data))
+        self._pending = [int(p) for p in d["pending_rows"]]
