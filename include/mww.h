@@ -617,6 +617,35 @@ int mww_multi_detector_get_state(mww_detector_t *d, int k, float *h_hist, long l
 int mww_multi_detector_set_state(mww_detector_t *d, int k, const float *h_hist, const long long *h_seen,
                                  const int32_t *h_cooldown_or_active);
 
+/* ---- per-row cutoffs: each stream's own sensitivity ------------------------------------------------------------------------
+ * A detector starts in uniform mode: one cutoff per detector (plain) or per model (models detector), as above.  The first
+ * set call with n > 0 switches it to per-row mode for good: every row keeps a cutoff c_r, all set to the create-time
+ * value, and then the listed rows are written.  For a models detector that is every member row of every WAKE and VAD model.
+ * The rule of a per-row detector is the rule above with (double)avg > c_r in place of (double)avg > cutoff, for WAKE firing
+ * and for the VAD's active flag alike; windows, cooldowns, gating, the event layout, d_fired and step numbering do not change.
+ * Consequences:
+ *   1. Per-row mode with every c_r = c is bit-identical to uniform mode at c: the same set of events, and the same state.
+ *   2. Row r of a per-row plain detector is bit-identical to that row of a uniform detector at c_r as long as c_r never
+ *      changes; so its events are mww_false_accept_counts at c_r on everything the row was given.
+ *   3. Events and state do not depend on how the probabilities were split into calls, as long as cutoff changes fall
+ *      between the same steps.
+ * Calls:
+ *   - set: n (row, cutoff) pairs.  The plain call takes row indices; the multi call takes GLOBAL stream ids, which must be
+ *     members of S_k.  Ordered on cu_stream: an update enqueued before the call uses the old cutoffs, one enqueued after it
+ *     the new ones.  The host arrays may be reused as soon as the call returns.  Detector state (hist, seen, cooldown,
+ *     active) is untouched, and resets keep the cutoffs.  n == 0 does nothing and does not switch mode.
+ *   - MWW_EINVAL, before any device work and with the detector unchanged: a non-finite cutoff; an id out of range, listed
+ *     twice or (multi) not a member of S_k; n < 0; NULL arrays with n > 0; an OFF model or a k out of range; the plain
+ *     calls on a models detector and the multi calls on a plain detector.
+ *   - get: every row's cutoff, host buffer [n_rows] (plain) or [n_k] in list order (multi), synchronous; the create-time
+ *     value in every slot while the detector is in uniform mode.
+ * The per-row kernels read 8 bytes more per row per call than the uniform ones; uniform mode runs exactly as before. */
+int mww_set_detector_cutoffs(mww_detector_t *d, const int32_t *h_rows, const double *h_cutoffs, int n, void *cu_stream);
+int mww_get_detector_cutoffs(mww_detector_t *d, double *h_cutoffs /* [n_rows] */);
+int mww_set_multi_detector_cutoffs(mww_detector_t *d, int k, const int32_t *h_stream_ids, const double *h_cutoffs, int n,
+                                   void *cu_stream);
+int mww_get_multi_detector_cutoffs(mww_detector_t *d, int k, double *h_cutoffs /* [n_k], list order */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -35,6 +35,7 @@ EXPORTS = (
     "mww_detector_create", "mww_detector_destroy", "mww_detector_update", "mww_detector_drain", "mww_detector_buffers",
     "mww_detector_reset", "mww_detector_reset_device", "mww_detector_get_state", "mww_detector_set_state",
     "mww_multi_detector_create", "mww_multi_detector_update", "mww_multi_detector_get_state", "mww_multi_detector_set_state",
+    "mww_set_detector_cutoffs", "mww_get_detector_cutoffs", "mww_set_multi_detector_cutoffs", "mww_get_multi_detector_cutoffs",
 )
 
 
@@ -237,6 +238,14 @@ def lib() -> ctypes.CDLL:
     for name in ("mww_multi_detector_get_state", "mww_multi_detector_set_state"):
         getattr(L, name).restype = i32
         getattr(L, name).argtypes = [vp, i32, vp, vp, vp]
+    L.mww_set_detector_cutoffs.restype = i32
+    L.mww_set_detector_cutoffs.argtypes = [vp, vp, vp, i32, vp]
+    L.mww_get_detector_cutoffs.restype = i32
+    L.mww_get_detector_cutoffs.argtypes = [vp, vp]
+    L.mww_set_multi_detector_cutoffs.restype = i32
+    L.mww_set_multi_detector_cutoffs.argtypes = [vp, i32, vp, vp, i32, vp]
+    L.mww_get_multi_detector_cutoffs.restype = i32
+    L.mww_get_multi_detector_cutoffs.argtypes = [vp, i32, vp]
     _lib = L
     return L
 

@@ -25,6 +25,10 @@ DET_SOURCES = ["mww_detector.cu"]
 # and the multi-model detector's (mww_multi_detector_create), so that libmww_detector.so keeps the plain detector's three
 MD_OUT = os.path.join(HERE, "libmww_detector_models.so")
 MD_SOURCES = ["mww_detector_models.cu"]
+# and both detectors' per-row-cutoff kernels (mww_set_detector_cutoffs, mww_set_multi_detector_cutoffs), so that those two
+# libraries keep exactly the kernels uniform mode runs
+DC_OUT = os.path.join(HERE, "libmww_detector_cutoffs.so")
+DC_SOURCES = ["mww_detector_cutoffs.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -47,7 +51,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -66,9 +70,9 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if not force and not _stale():
             return OUT
         for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (RR_OUT, RR_SOURCES, []), (DET_OUT, DET_SOURCES, []),
-                                    (MD_OUT, MD_SOURCES, []),
+                                    (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
-                                                    "-lmww_detector_models", "-Xlinker", "-rpath,$ORIGIN"])):
+                                                    "-lmww_detector_models", "-lmww_detector_cutoffs", "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra
             res = subprocess.run(cmd, capture_output=True, text=True)

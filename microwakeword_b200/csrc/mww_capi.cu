@@ -2043,6 +2043,14 @@ struct mww_detector {
     DetectModelsArgs m;
     std::vector<DetectModel> models;
     DetectModel *d_models = nullptr;
+    std::vector<std::vector<int32_t>> member_row;     // [k][n_streams]: row of each global stream in model k, -1 for none
+    // per-row mode (mww_set_detector_cutoffs, mww_set_multi_detector_cutoffs): host copies of every row's cutoff and the
+    // device arrays the per-row kernels read; empty and nullptr in uniform mode
+    std::vector<double> cutoffs;                      // plain: [n_rows]
+    double *d_cutoffs = nullptr;
+    std::vector<std::vector<double>> model_cutoffs;   // models: [k][n_k]
+    std::vector<DetectModelRows> models_rows;         // the descriptors d_models_rows holds, each with its d_row_cutoff
+    DetectModelRows *d_models_rows = nullptr;
 };
 
 namespace {
@@ -2057,7 +2065,32 @@ void detector_free(mww_detector_t *d) {
         cudaFree(M.hist); cudaFree(M.seen); cudaFree(M.flag); cudaFree(const_cast<int32_t *>(M.inv));
     }
     cudaFree(d->d_models);
+    cudaFree(d->d_cutoffs);
+    for (DetectModelRows &M : d->models_rows) cudaFree(const_cast<double *>(M.row_cutoff));
+    cudaFree(d->d_models_rows);
     delete d;
+}
+
+// The (id, cutoff) list of a set-cutoffs call, checked before anything changes: finite cutoffs, ids in [0, n_ids), each
+// naming a row (row_of[id] >= 0; row_of == nullptr: the id is the row) of the n_rows, none twice.  rows: the rows named,
+// [lo, hi] the span they cover.
+int check_cutoff_list(const std::string &call, const int32_t *ids, const double *c, int n, int n_ids, const int32_t *row_of, int n_rows,
+                      std::vector<int32_t> &rows, int &lo, int &hi) {
+    std::vector<char> listed((size_t)std::max(n_rows, 1), 0);
+    rows.resize((size_t)n);
+    lo = n_rows; hi = -1;
+    for (int i = 0; i < n; ++i) {
+        if (!(c[i] - c[i] == 0.0)) return fail(nullptr, MWW_EINVAL, call + ": cutoffs must be finite");
+        const int32_t id = ids[i];
+        if (id < 0 || id >= n_ids) return fail(nullptr, MWW_EINVAL, call + ": id " + std::to_string(id) + " out of range");
+        const int32_t r = row_of ? row_of[id] : id;
+        if (r < 0) return fail(nullptr, MWW_EINVAL, call + ": stream " + std::to_string(id) + " is not a member of the model's stream set");
+        if (listed[r]) return fail(nullptr, MWW_EINVAL, call + ": id " + std::to_string(id) + " listed twice");
+        listed[r] = 1;
+        rows[i] = r;
+        lo = std::min(lo, (int)r); hi = std::max(hi, (int)r);
+    }
+    return MWW_OK;
 }
 
 size_t detector_hist_elems(const mww_detector_t *d) { return (size_t)(d->a.rule.window - 1) * d->a.n_rows; }
@@ -2128,7 +2161,8 @@ int mww_detector_update(mww_detector_t *d, const float *d_probs, int n_steps, lo
         return fail(nullptr, MWW_EINVAL, "mww_detector_update: needs d_probs and n_steps >= 0 columns within the row pitch");
     if (n_steps == 0) return MWW_OK;
     DENTER(d);
-    DCU(launch_detector_update(d->a, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
+    if (d->d_cutoffs) DCU(launch_detector_update_cutoffs(d->a, d->d_cutoffs, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
+    else DCU(launch_detector_update(d->a, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
     return MWW_OK;
 }
 
@@ -2226,6 +2260,37 @@ int mww_detector_set_state(mww_detector_t *d, const float *h_hist, const long lo
     return MWW_OK;
 }
 
+int mww_set_detector_cutoffs(mww_detector_t *d, const int32_t *h_rows, const double *h_cutoffs, int n, void *cu_stream) {
+    const std::string call = "mww_set_detector_cutoffs";
+    if (!d) return fail(nullptr, MWW_EINVAL, call + ": detector is NULL");
+    if (d->multi) return fail(nullptr, MWW_EINVAL, call + ": a models detector takes mww_set_multi_detector_cutoffs");
+    if (n < 0) return fail(nullptr, MWW_EINVAL, call + ": n must not be negative");
+    if (n == 0) return MWW_OK;
+    if (!h_rows || !h_cutoffs) return fail(nullptr, MWW_EINVAL, call + ": h_rows and h_cutoffs must not be NULL");
+    const int R = d->a.n_rows;
+    std::vector<int32_t> rows;
+    int lo = 0, hi = 0;
+    if (int rc = check_cutoff_list(call, h_rows, h_cutoffs, n, R, nullptr, R, rows, lo, hi)) return rc;
+    DENTER(d);
+    if (!d->d_cutoffs) {                           // to per-row mode: every row at the create-time cutoff, all copied
+        DCU(cudaMalloc(&d->d_cutoffs, (size_t)R * sizeof(double)));
+        d->cutoffs.assign((size_t)R, d->a.rule.cutoff);
+        lo = 0; hi = R - 1;
+    }
+    for (int i = 0; i < n; ++i) d->cutoffs[rows[i]] = h_cutoffs[i];
+    // from pageable memory: the call returns once the span is staged, so later changes to the host copy cannot reach it
+    DCU(cudaMemcpyAsync(d->d_cutoffs + lo, d->cutoffs.data() + lo, (size_t)(hi - lo + 1) * sizeof(double), cudaMemcpyHostToDevice,
+                        static_cast<cudaStream_t>(cu_stream)));
+    return MWW_OK;
+}
+
+int mww_get_detector_cutoffs(mww_detector_t *d, double *h_cutoffs) {
+    if (!d || !h_cutoffs) return fail(nullptr, MWW_EINVAL, "mww_get_detector_cutoffs: needs a detector and h_cutoffs");
+    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_get_detector_cutoffs: a models detector takes mww_get_multi_detector_cutoffs");
+    for (int r = 0; r < d->a.n_rows; ++r) h_cutoffs[r] = d->d_cutoffs ? d->cutoffs[r] : d->a.rule.cutoff;
+    return MWW_OK;
+}
+
 }  // extern "C"
 
 // ---- multi-model detector (include/mww.h; rule and kernels: mww_detector_models.h, mww_detector_models.cu) ----------------
@@ -2238,10 +2303,13 @@ int models_fail(const char *what) { return fail(nullptr, MWW_EINVAL, std::string
 int models_alloc(mww_detector_t *d, const std::vector<std::vector<int32_t>> &ids) {
     DetectModelsArgs &m = d->m;
     const size_t C = (size_t)d->a.capacity, S = (size_t)m.n_streams;
+    d->member_row.resize((size_t)m.n_models);
     for (int k = 0; k < m.n_models; ++k) {
         DetectModel &M = d->models[k];
         if (M.role == MWW_DETECT_OFF) continue;
         const size_t R = (size_t)M.n_rows, W = (size_t)M.rule.window - 1;
+        d->member_row[k].assign(S, -1);
+        for (size_t r = 0; r < R; ++r) d->member_row[k][ids[k][r]] = (int32_t)r;
         DCU(cudaMalloc(&M.hist, std::max<size_t>(W * R, 1) * sizeof(float)));
         DCU(cudaMalloc(&M.seen, std::max<size_t>(R, 1) * sizeof(long long)));
         DCU(cudaMalloc(&M.flag, std::max<size_t>(R, 1) * sizeof(int32_t)));
@@ -2276,6 +2344,37 @@ int model_arg(mww_detector_t *d, int k, const char *call, const DetectModel **ou
     if (k < 0 || k >= d->m.n_models) return fail(nullptr, MWW_EINVAL, std::string(call) + ": model index out of range");
     if (d->models[k].role == MWW_DETECT_OFF) return fail(nullptr, MWW_EINVAL, std::string(call) + ": model is OFF");
     *out = &d->models[k];
+    return MWW_OK;
+}
+
+// a models detector to per-row mode: every member row of every used model at its model's cutoff, and the descriptors that
+// carry those arrays; on a failure nothing is kept and the detector stays in uniform mode
+int models_to_row_cutoffs(mww_detector_t *d, cudaStream_t st) {
+    const int K = d->m.n_models;
+    std::vector<DetectModelRows> rows((size_t)K);
+    std::vector<std::vector<double>> cut((size_t)K);
+    DetectModelRows *d_rows = nullptr;
+    auto undo = [&](cudaError_t e, const char *what) {
+        for (DetectModelRows &M : rows) cudaFree(const_cast<double *>(M.row_cutoff));
+        cudaFree(d_rows);
+        return cuda_fail(nullptr, e, what);
+    };
+    for (int k = 0; k < K; ++k) {
+        static_cast<DetectModel &>(rows[k]) = d->models[k];
+        const DetectModel &M = d->models[k];
+        if (M.role == MWW_DETECT_OFF || M.n_rows == 0) continue;
+        cut[k].assign((size_t)M.n_rows, M.rule.cutoff);
+        double *p = nullptr;
+        if (cudaError_t e = cudaMalloc(&p, (size_t)M.n_rows * sizeof(double))) return undo(e, "cudaMalloc");
+        rows[k].row_cutoff = p;
+        if (cudaError_t e = cudaMemcpyAsync(p, cut[k].data(), (size_t)M.n_rows * sizeof(double), cudaMemcpyHostToDevice, st)) return undo(e, "cudaMemcpyAsync");
+    }
+    if (cudaError_t e = cudaMalloc(&d_rows, (size_t)K * sizeof(DetectModelRows))) return undo(e, "cudaMalloc");
+    if (cudaError_t e = cudaMemcpyAsync(d_rows, rows.data(), (size_t)K * sizeof(DetectModelRows), cudaMemcpyHostToDevice, st))
+        return undo(e, "cudaMemcpyAsync");
+    d->models_rows = std::move(rows);
+    d->model_cutoffs = std::move(cut);
+    d->d_models_rows = d_rows;
     return MWW_OK;
 }
 
@@ -2371,7 +2470,8 @@ int mww_multi_detector_update(mww_detector_t *d, const float *const *d_probs, co
     if (!any) return MWW_OK;
     DENTER(d);
     for (int k = 0; k < m.n_models; ++k) m.call[k] = call[k];
-    DCU(launch_detector_models_update(m, static_cast<cudaStream_t>(cu_stream)));
+    if (d->d_models_rows) DCU(launch_detector_models_update_cutoffs(detect_args_rows(m, d->d_models_rows), static_cast<cudaStream_t>(cu_stream)));
+    else DCU(launch_detector_models_update(m, static_cast<cudaStream_t>(cu_stream)));
     return MWW_OK;
 }
 
@@ -2415,6 +2515,38 @@ int mww_multi_detector_set_state(mww_detector_t *d, int k, const float *h_hist, 
     }
     if (h_seen) DCU(cudaMemcpy(M->seen, h_seen, R * sizeof(long long), cudaMemcpyHostToDevice));
     if (h_cooldown_or_active) DCU(cudaMemcpy(M->flag, h_cooldown_or_active, R * sizeof(int32_t), cudaMemcpyHostToDevice));
+    return MWW_OK;
+}
+
+int mww_set_multi_detector_cutoffs(mww_detector_t *d, int k, const int32_t *h_stream_ids, const double *h_cutoffs, int n, void *cu_stream) {
+    const std::string call = "mww_set_multi_detector_cutoffs";
+    const DetectModel *M = nullptr;
+    if (int rc = model_arg(d, k, call.c_str(), &M)) return rc;
+    if (n < 0) return fail(nullptr, MWW_EINVAL, call + ": n must not be negative");
+    if (n == 0) return MWW_OK;
+    if (!h_stream_ids || !h_cutoffs) return fail(nullptr, MWW_EINVAL, call + ": h_stream_ids and h_cutoffs must not be NULL");
+    std::vector<int32_t> rows;
+    int lo = 0, hi = 0;
+    if (int rc = check_cutoff_list(call, h_stream_ids, h_cutoffs, n, d->m.n_streams, d->member_row[k].data(), M->n_rows, rows, lo, hi)) return rc;
+    DENTER(d);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (!d->d_models_rows) {
+        if (int rc = models_to_row_cutoffs(d, st)) return rc;
+        lo = 0; hi = M->n_rows - 1;
+    }
+    std::vector<double> &c = d->model_cutoffs[k];
+    for (int i = 0; i < n; ++i) c[rows[i]] = h_cutoffs[i];
+    // from pageable memory: the call returns once the span is staged, so later changes to the host copy cannot reach it
+    DCU(cudaMemcpyAsync(const_cast<double *>(d->models_rows[k].row_cutoff) + lo, c.data() + lo, (size_t)(hi - lo + 1) * sizeof(double),
+                        cudaMemcpyHostToDevice, st));
+    return MWW_OK;
+}
+
+int mww_get_multi_detector_cutoffs(mww_detector_t *d, int k, double *h_cutoffs) {
+    const DetectModel *M = nullptr;
+    if (int rc = model_arg(d, k, "mww_get_multi_detector_cutoffs", &M)) return rc;
+    if (!h_cutoffs && M->n_rows > 0) return fail(nullptr, MWW_EINVAL, "mww_get_multi_detector_cutoffs: h_cutoffs is NULL");
+    for (int r = 0; r < M->n_rows; ++r) h_cutoffs[r] = d->d_models_rows ? d->model_cutoffs[k][r] : M->rule.cutoff;
     return MWW_OK;
 }
 

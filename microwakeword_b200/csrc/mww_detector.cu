@@ -1,106 +1,9 @@
-// mww_detector.cu -- the streaming detector's kernels (rule and both forms: mww_detector.h).
-//
-// detector_update_kernel<false>, thread per row: the live shape, one or a few steps for very many rows.  State is
-// struct-of-arrays and the history [window - 1][n_rows], so every access of a warp is one coalesced line; a one-step call
-// moves 8 (window - 1) + 28 bytes per row (history, counter and cooldown read and written, one probability read).
-// detector_update_kernel<true>, warp per row: the clip shape, many steps per row.  32 consecutive steps per pass are loaded
-// coalesced; the window - 1 values before them come from the history on the first pass and from the previous pass's
-// registers afterwards, by shuffles; every lane forms one average and detector_chain_pass walks the cooldown chain.
-// Events go to the shared buffer through one atomicAdd per warp.
-#include <cuda_runtime.h>
-
-#include "mww_kernels.h"
+// mww_detector.cu -- the streaming detector's kernels with one cutoff for every row: the update kernel's two forms
+// (mww_detector.cuh) and the reset kernel.  The per-row instantiations live in mww_detector_cutoffs.cu, a library of their
+// own, so that this one keeps exactly these three kernels.
+#include "mww_detector.cuh"
 
 namespace mww {
-
-namespace {
-
-constexpr unsigned kFull = 0xffffffffu;
-constexpr int kThreads = 256;
-
-// history of one row in global memory, entry j at hist[j * n_rows]
-struct RowHistory {
-    float *h; long long stride;
-    MWW_D float get(int j) const { return h[j * stride]; }
-    MWW_D void set(int j, float v) { h[j * stride] = v; }
-};
-
-// steps of a pass and the one before it, spread over the lanes: x(i) is step i of the pass for i >= 0 and step 32 + i of
-// the previous pass for i < 0.  Every lane of the warp must call it together.
-struct PassWindow {
-    float cur, prev;
-    MWW_D float operator()(int i) const {
-        const float c = __shfl_sync(kFull, cur, i & 31), p = __shfl_sync(kFull, prev, i & 31);
-        return i >= 0 ? c : p;
-    }
-};
-
-// the warp's lanes whose `fire` is set append one event each: one atomicAdd for all of them.  Called by whole warps.
-MWW_D void append_events(const DetectorArgs &a, bool fire, int row, long long step, float score) {
-    const unsigned mask = __ballot_sync(kFull, fire);
-    if (mask == 0) return;
-    const int lane = threadIdx.x & 31;
-    unsigned long long base = 0;
-    if (lane == 0) base = atomicAdd(a.count, (unsigned long long)__popc(mask));
-    base = __shfl_sync(kFull, base, 0);
-    const unsigned long long slot = base + __popc(mask & ((1u << lane) - 1));
-    if (!fire || slot >= (unsigned long long)a.capacity) return;      // past capacity: counted, not stored
-    const int32_t stream = a.stream_ids ? a.stream_ids[row] : row;
-    mww_event e;
-    e.stream = stream; e.reserved = 0; e.step = step; e.score = score; e.pad = 0;
-    a.events[slot] = e;
-    a.fired[slot] = stream;
-}
-
-}  // namespace
-
-template <bool kWarpPerRow>
-__global__ void __launch_bounds__(kThreads) detector_update_kernel(DetectorArgs a, const float *__restrict__ probs, int n_steps, long long pitch) {
-    const DetectorRule &r = a.rule;
-    if (!kWarpPerRow) {
-        const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-        const bool active = row < a.n_rows;                          // idle lanes stay for the ballots
-        long long seen = 0;
-        int cooldown = 0;
-        if (active) { seen = a.seen[row]; cooldown = a.cooldown[row]; }
-        RowHistory hist{a.hist + row, a.n_rows};
-        for (int t = 0; t < n_steps; ++t) {
-            float score = 0.f;
-            bool fire = false;
-            if (active) {
-                fire = detector_step(hist, r, seen, cooldown, probs[row * pitch + t], &score);
-                ++seen;
-            }
-            append_events(a, fire, (int)row, seen - 1, score);
-        }
-        if (active) { a.seen[row] = seen; a.cooldown[row] = cooldown; }
-    } else {
-        const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-        if (row >= a.n_rows) return;                                 // whole warps leave
-        const int lane = threadIdx.x & 31, w = r.window;
-        const long long seen = a.seen[row];
-        int cooldown = a.cooldown[row];
-        const float *p = probs + row * pitch;
-        RowHistory hist{a.hist + row, a.n_rows};
-        // the history stands in for the pass before the first: its entry j is step 32 - (w - 1) + j of that pass
-        PassWindow x{0.f, lane >= 32 - (w - 1) ? hist.get(lane - (32 - (w - 1))) : 0.f};
-        int n = 0;
-        for (int base = 0; base < n_steps; base += 32) {
-            n = min(32, n_steps - base);
-            x.cur = lane < n ? p[base + lane] : 0.f;
-            const float avg = detector_window_mean(x, lane, w);
-            const int first = detector_first_full(seen + base, w, n);
-            const unsigned candidates = __ballot_sync(kFull, lane >= first && lane < n && (double)avg > r.cutoff);
-            const unsigned fired = detector_chain_pass(r, candidates, first, n, cooldown);
-            append_events(a, (fired >> lane) & 1u, (int)row, seen + base + lane, avg);
-            if (base + 32 < n_steps) x.prev = x.cur;
-        }
-        // new history: the last w - 1 of (old history, this call's steps), i.e. steps n - (w - 1) .. n - 1 of the last pass
-        const float keep = x(lane < w - 1 ? n - (w - 1) + lane : 0);
-        if (lane < w - 1) hist.set(lane, keep);
-        if (lane == 0) { a.seen[row] = seen + n_steps; a.cooldown[row] = cooldown; }
-    }
-}
 
 // fresh state for rows[0, n) (indices out of range ignored) or, rows == nullptr, for every row
 __global__ void __launch_bounds__(kThreads) detector_reset_kernel(DetectorArgs a, const int32_t *__restrict__ rows, int n) {
@@ -114,14 +17,7 @@ __global__ void __launch_bounds__(kThreads) detector_reset_kernel(DetectorArgs a
 }
 
 cudaError_t launch_detector_update(const DetectorArgs &a, const float *probs, int n_steps, long long pitch, cudaStream_t st) {
-    if (n_steps <= 0 || a.n_rows <= 0) return cudaSuccess;
-    if (n_steps >= kDetectorWarpMinSteps) {
-        const long long blocks = ((long long)a.n_rows * 32 + kThreads - 1) / kThreads;
-        detector_update_kernel<true><<<(unsigned)blocks, kThreads, 0, st>>>(a, probs, n_steps, pitch);
-    } else {
-        detector_update_kernel<false><<<(unsigned)((a.n_rows + kThreads - 1) / kThreads), kThreads, 0, st>>>(a, probs, n_steps, pitch);
-    }
-    return cudaGetLastError();
+    return launch_update_form<false>(a, nullptr, probs, n_steps, pitch, st);
 }
 
 cudaError_t launch_detector_reset(const DetectorArgs &a, const int32_t *rows, int n, cudaStream_t st) {

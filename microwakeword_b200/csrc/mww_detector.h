@@ -6,7 +6,8 @@
 // i = 0, 1, ...: cooldown = max(cooldown - 1, 0); if cooldown == 0 and (double)avg[i] > cutoff the row fires (step
 // i + window - 1, score avg[i]) and cooldown = cooldown_slices.  That is false_accept_kernel (mww_detect.cu) on the
 // concatenation of everything the row was given; the state carried between calls is the last window - 1 probabilities,
-// the count of probabilities seen and the cooldown.
+// the count of probabilities seen and the cooldown.  In per-row mode (mww_set_detector_cutoffs) `cutoff` is the row's
+// c_r, which the _at and _from forms of the rule take as an argument; nothing else changes.
 #pragma once
 
 #include <stdint.h>
@@ -72,19 +73,31 @@ MWW_HD float detector_window_mean(const X &x, int newest, int window) {
     return det_div(s, (float)window);
 }
 
-// the rule at one moving-average index: true when it fires
-MWW_HD bool detector_tick(const DetectorRule &r, float avg, int &cooldown) {
+// a cutoff held as a value
+struct CutoffValue {
+    double c = 0.0;
+    MWW_HD double get() const { return c; }
+};
+
+// the rule at one moving-average index against a cutoff (C: double get() const; the rule's, or the row's in per-row mode),
+// which is read only once the cooldown has run out: true when it fires
+template <typename C>
+MWW_HD bool detector_tick_from(const DetectorRule &r, const C &cutoff, float avg, int &cooldown) {
     cooldown = cooldown > 0 ? cooldown - 1 : 0;
-    if (cooldown != 0 || !((double)avg > r.cutoff)) return false;
+    if (cooldown != 0 || !((double)avg > cutoff.get())) return false;
     cooldown = r.cooldown_slices;
     return true;
 }
+MWW_HD bool detector_tick_at(const DetectorRule &r, double cutoff, float avg, int &cooldown) {
+    return detector_tick_from(r, CutoffValue{cutoff}, avg, cooldown);
+}
+MWW_HD bool detector_tick(const DetectorRule &r, float avg, int &cooldown) { return detector_tick_at(r, r.cutoff, avg, cooldown); }
 
 // Thread form: one row takes one probability.  `seen` counts the probabilities before this one (the caller adds one
 // afterwards).  The history is streamed, never held: entry j is read, summed and written back to j - 1, so a window of
 // any length needs no array.  H: float get(int) const, void set(int, float) over the row's window - 1 entries.
 template <typename H>
-MWW_HD bool detector_step(H &hist, const DetectorRule &r, long long seen, int &cooldown, float p, float *score) {
+MWW_HD bool detector_step_at(H &hist, const DetectorRule &r, double cutoff, long long seen, int &cooldown, float p, float *score) {
     const int w = r.window;
     float s = p;
     if (w > 1) {
@@ -99,9 +112,13 @@ MWW_HD bool detector_step(H &hist, const DetectorRule &r, long long seen, int &c
     }
     if (seen + 1 < w) return false;              // warming up: the sum holds entries from before the reset
     const float avg = det_div(s, (float)w);
-    if (!detector_tick(r, avg, cooldown)) return false;
+    if (!detector_tick_at(r, cutoff, avg, cooldown)) return false;
     *score = avg;
     return true;
+}
+template <typename H>
+MWW_HD bool detector_step(H &hist, const DetectorRule &r, long long seen, int &cooldown, float p, float *score) {
+    return detector_step_at(hist, r, r.cutoff, seen, cooldown, p, score);
 }
 
 // Warp form: a pass covers n <= 32 consecutive steps of one row, lane i forming the average whose newest probability is

@@ -39,17 +39,43 @@ struct DetectCall {
     int n_steps = 0, pending = 0;            // steps run in the call, pending rows before it
 };
 
+// a model's descriptor in per-row mode (mww_set_multi_detector_cutoffs): the same, and the cutoff of each of its rows
+struct DetectModelRows : DetectModel {
+    const double *row_cutoff = nullptr;      // [n_rows], list order
+};
+
+// The cutoff row `row` of model m compares against (row -1: a non-member, never compared).  Uniform mode reads the rule's
+// where the comparison is; per-row mode loads the row's where it loads the row's state (for a WAKE row, once per VAD step).
+struct RuleCutoff {
+    const DetectModel *m = nullptr;
+    MWW_HD double get() const { return m->rule.cutoff; }
+};
+MWW_HD RuleCutoff detect_cutoff(const DetectModel &m, int) { return RuleCutoff{&m}; }
+MWW_HD CutoffValue detect_cutoff(const DetectModelRows &m, int row) { return CutoffValue{row >= 0 ? m.row_cutoff[row] : 0.0}; }
+
 // what the update and reset kernels get: descriptors (device memory), the event buffer, its counter and the fired-id list
-// shared with the plain detector, and the call -- pointers, pitches and step timing travel in the parameters, not by copy
-struct DetectModelsArgs {
+// shared with the plain detector, and the call -- pointers, pitches and step timing travel in the parameters, not by copy.
+// M: DetectModel, or DetectModelRows in per-row mode.
+template <typename M>
+struct DetectModelsArgsT {
     int n_streams = 0, n_models = 0, vad = -1, n_wake = 0, capacity = 0;
-    const DetectModel *models = nullptr;
+    const M *models = nullptr;
     unsigned long long *count = nullptr;
     mww_event *events = nullptr;
     int32_t *fired = nullptr;
     int8_t wake[kDetectMaxModels] = {};      // the WAKE models' indices
     DetectCall call[kDetectMaxModels];
 };
+using DetectModelsArgs = DetectModelsArgsT<DetectModel>;
+
+// the same arguments over per-row descriptors
+inline DetectModelsArgsT<DetectModelRows> detect_args_rows(const DetectModelsArgs &a, const DetectModelRows *models) {
+    DetectModelsArgsT<DetectModelRows> r;
+    r.n_streams = a.n_streams; r.n_models = a.n_models; r.vad = a.vad; r.n_wake = a.n_wake; r.capacity = a.capacity;
+    r.models = models; r.count = a.count; r.events = a.events; r.fired = a.fired;
+    for (int k = 0; k < kDetectMaxModels; ++k) { r.wake[k] = a.wake[k]; r.call[k] = a.call[k]; }
+    return r;
+}
 
 // one row's history, entry j at h[j * stride]
 struct DetectHistory {
@@ -110,51 +136,54 @@ inline bool detect_call_fits(const DetectModel *models, const DetectCall *call, 
 
 // One call for one stream.  emit(fire, k, stream, step, score) is called for every WAKE step of every WAKE model in the
 // same order on every stream, member or not (fire false for a non-member), so that the kernel's warps can ballot on it.
-template <typename Emit>
-MWW_HD void detect_models_stream(const DetectModelsArgs &a, int stream, Emit &emit) {
-    const DetectModel *V = a.vad >= 0 ? &a.models[a.vad] : nullptr;
+template <typename M, typename Emit>
+MWW_HD void detect_models_stream(const DetectModelsArgsT<M> &a, int stream, Emit &emit) {
+    const M *V = a.vad >= 0 ? &a.models[a.vad] : nullptr;
     int n_v = 0, vrow = -1, s_v = 1, p_v = 0;
     long long vseen = 0;
+    decltype(detect_cutoff(*V, 0)) vcut;
     bool active = V == nullptr;                                  // no VAD: the gate is open
     if (V) {
         n_v = a.call[a.vad].n_steps; s_v = V->stride; p_v = a.call[a.vad].pending;
         vrow = detect_row(*V, stream, a.n_streams);
         if (vrow >= 0) { vseen = V->seen[vrow]; active = V->flag[vrow] != 0; }
+        vcut = detect_cutoff(*V, vrow);
     }
     for (int i = 0; i <= n_v; ++i) {
         // the WAKE steps ending in [end of VAD step i - 1, end of VAD step i): they see the flag VAD step i - 1 left
         for (int w = 0; w < a.n_wake; ++w) {
             const int k = a.wake[w];
             const DetectCall &c = a.call[k];
-            const DetectModel &M = a.models[k];
-            const int j0 = i == 0 ? 0 : detect_steps_below(detect_end_row(i - 1, s_v, p_v), M.stride, c.pending, c.n_steps);
-            const int j1 = i == n_v ? c.n_steps : detect_steps_below(detect_end_row(i, s_v, p_v), M.stride, c.pending, c.n_steps);
+            const M &W = a.models[k];
+            const int j0 = i == 0 ? 0 : detect_steps_below(detect_end_row(i - 1, s_v, p_v), W.stride, c.pending, c.n_steps);
+            const int j1 = i == n_v ? c.n_steps : detect_steps_below(detect_end_row(i, s_v, p_v), W.stride, c.pending, c.n_steps);
             if (j0 >= j1) continue;
-            const int row = detect_row(M, stream, a.n_streams);
+            const int row = detect_row(W, stream, a.n_streams);
             long long seen = 0;
             int cooldown = 0;
-            if (row >= 0) { seen = M.seen[row]; cooldown = M.flag[row]; }
-            const DetectHistory hist{M.hist + (row >= 0 ? row : 0), M.n_rows};
+            if (row >= 0) { seen = W.seen[row]; cooldown = W.flag[row]; }
+            const auto cutoff = detect_cutoff(W, row);
+            const DetectHistory hist{W.hist + (row >= 0 ? row : 0), W.n_rows};
             for (int j = j0; j < j1; ++j) {
                 bool fire = false;
                 float avg = 0.f;
                 if (row >= 0) {
-                    avg = detect_push(hist, M.rule.window, c.probs[row * c.pitch + j]);
-                    if (seen + 1 >= M.rule.window) {                // warming up: no average, no tick
-                        if (active) fire = detector_tick(M.rule, avg, cooldown);
+                    avg = detect_push(hist, W.rule.window, c.probs[row * c.pitch + j]);
+                    if (seen + 1 >= W.rule.window) {                // warming up: no average, no tick
+                        if (active) fire = detector_tick_from(W.rule, cutoff, avg, cooldown);
                         else cooldown = cooldown > 0 ? cooldown - 1 : 0;
                     }
                     ++seen;
                 }
                 emit(fire, k, stream, seen - 1, avg);
             }
-            if (row >= 0) { M.seen[row] = seen; M.flag[row] = cooldown; }
+            if (row >= 0) { W.seen[row] = seen; W.flag[row] = cooldown; }
         }
         if (i < n_v && vrow >= 0) {
             const DetectCall &c = a.call[a.vad];
             const float avg = detect_push(DetectHistory{V->hist + vrow, V->n_rows}, V->rule.window, c.probs[vrow * c.pitch + i]);
             ++vseen;
-            active = vseen >= V->rule.window && (double)avg > V->rule.cutoff;
+            active = vseen >= V->rule.window && (double)avg > vcut.get();
         }
     }
     if (vrow >= 0) { V->seen[vrow] = vseen; V->flag[vrow] = active ? 1 : 0; }

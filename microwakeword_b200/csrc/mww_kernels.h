@@ -152,4 +152,10 @@ cudaError_t launch_detector_models_update(const DetectModelsArgs &a, cudaStream_
 // fresh state of every model's row of the n listed GLOBAL stream ids (device memory; out of range ignored) or, ids ==
 // nullptr, of streams [0, n)
 cudaError_t launch_detector_models_reset(const DetectModelsArgs &a, const int32_t *ids, int n, cudaStream_t st);
+
+// both detectors in per-row mode (mww_detector_cutoffs.cu): launch_detector_update with row r compared against
+// row_cutoff[r] (device memory, [n_rows]), and launch_detector_models_update over descriptors that carry their rows' cutoffs
+cudaError_t launch_detector_update_cutoffs(const DetectorArgs &a, const double *row_cutoff, const float *probs, int n_steps, long long pitch,
+                                           cudaStream_t st);
+cudaError_t launch_detector_models_update_cutoffs(const DetectModelsArgsT<DetectModelRows> &a, cudaStream_t st);
 }  // namespace mww

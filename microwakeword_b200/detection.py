@@ -17,6 +17,7 @@ Live, the same rule runs per stream with its state carried across calls:
     StreamDetector(n_rows, cutoff, window=5, cooldown_slices=25)   probabilities in (update), detections out (drain)
     MultiModelDetector(engine, cutoffs, windows, cooldown_slices, vad)   the same for every model of a MultiModelEngine in
                                                                        one launch, wake words gated by a VAD model
+    set_cutoffs(...)                                                   either one: each stream's own sensitivity
 """
 
 from __future__ import annotations
@@ -368,6 +369,44 @@ class StreamDetector:
         self._check(self._L.mww_detector_set_state(self._d, hist.ctypes.data, seen.ctypes.data, cooldown.ctypes.data))
 
 
+    def set_cutoffs(self, rows, cutoffs) -> None:
+        """Give the listed ROW indices their own cutoffs (mww_set_detector_cutoffs): `cutoffs` is one value or one per row.
+        The first call switches the detector to per-row mode, every other row keeping the create-time cutoff.  Ordered on
+        the current CUDA stream: updates made before it use the old cutoffs, updates after it the new ones.  The state and
+        resets are unaffected."""
+        import torch
+        r, c = _cutoff_list(rows, cutoffs, "rows")
+        self._check(self._L.mww_set_detector_cutoffs(self._d, r.ctypes.data, c.ctypes.data, r.size, _stream(torch.device("cuda", self.device))))
+
+    @property
+    def cutoffs(self) -> np.ndarray:
+        """float64 [n_rows]: every row's cutoff (the create-time one everywhere until set_cutoffs is called)"""
+        out = np.empty(self.n_rows, np.float64)
+        self._check(self._L.mww_get_detector_cutoffs(self._d, out.ctypes.data))
+        return out
+
+
+def _cutoff_list(ids, cutoffs, name):
+    """(int32 ids, float64 cutoffs) of one set-cutoffs call, or ValueError: ids a 1-D integer sequence, cutoffs one finite
+    real value or one per id"""
+    i = np.asarray(ids)
+    if i.ndim != 1 or not (np.issubdtype(i.dtype, np.integer) or i.size == 0):
+        raise ValueError("%s must be a 1-D sequence of integers" % name)
+    if i.size and (i.min() < np.iinfo(np.int32).min or i.max() > np.iinfo(np.int32).max):
+        raise ValueError("%s must fit in int32" % name)
+    c = np.asarray(cutoffs)
+    if c.dtype == bool or not (np.issubdtype(c.dtype, np.floating) or np.issubdtype(c.dtype, np.integer)):
+        raise ValueError("cutoffs must be real numbers")
+    if c.ndim == 0:
+        c = np.full(i.size, c, np.float64)
+    if c.shape != i.shape:
+        raise ValueError("cutoffs must be one value or one per entry of %s (%d)" % (name, i.size))
+    c = np.ascontiguousarray(c, np.float64)
+    if not np.isfinite(c).all():
+        raise ValueError("cutoffs must be finite")
+    return np.ascontiguousarray(i, np.int32), c
+
+
 # ---- the multi-model streaming detector ----------------------------------------------------------------------------------
 MODEL_EVENT_DTYPE = np.dtype([("stream", np.int32), ("model", np.int32), ("step", np.int64), ("score", np.float32), ("pad", np.int32)])
 
@@ -505,6 +544,31 @@ class MultiModelDetector:
         else:
             ids = np.ascontiguousarray(stream_ids, np.int32).reshape(-1)
             self._check(self._L.mww_detector_reset(self._d, ids.ctypes.data, ids.size, st))
+
+    def _used_model(self, k) -> int:
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 0 <= int(k) < self.n_models:
+            raise ValueError("k must be a model index in [0, %d)" % self.n_models)
+        if self.roles[int(k)] == _lib.MWW_DETECT_OFF:
+            raise ValueError("model %d is OFF: it has no rows" % int(k))
+        return int(k)
+
+    def set_cutoffs(self, k: int, stream_ids, cutoffs) -> None:
+        """Give the listed GLOBAL streams of model k (WAKE or the VAD; members of its stream set) their own cutoffs
+        (mww_set_multi_detector_cutoffs): `cutoffs` is one value or one per stream.  The first call switches every model to
+        per-row mode, every other row keeping its model's cutoff.  Ordered on the current CUDA stream; the state and resets
+        are unaffected."""
+        import torch
+        k = self._used_model(k)
+        ids, c = _cutoff_list(stream_ids, cutoffs, "stream_ids")
+        self._check(self._L.mww_set_multi_detector_cutoffs(self._d, k, ids.ctypes.data, c.ctypes.data, ids.size,
+                                                           _stream(torch.device("cuda", self.device))))
+
+    def get_cutoffs(self, k: int) -> np.ndarray:
+        """float64 [members of model k]: each row's cutoff in the order of streams[k]"""
+        k = self._used_model(k)
+        out = np.empty(max(self.streams[k].size, 1), np.float64)
+        self._check(self._L.mww_get_multi_detector_cutoffs(self._d, k, out.ctypes.data))
+        return out[:self.streams[k].size]
 
     def _flag_name(self, k):
         return "active" if self.roles[k] == _lib.MWW_DETECT_VAD else "cooldown"
