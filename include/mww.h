@@ -13,6 +13,7 @@
  *   microwakeword/inference.py:113-119  set_tensor / invoke / get_tensor, once per 30 ms      -> mww_infer_features
  *   microwakeword/inference.py:66-80    predict_clip (features + predict_spectrogram)         -> mww_predict_clip[_host]
  *   microwakeword/audio/audio_utils.py:47-48   float clip -> int16 (x * 32768, clipped)      -> the *_f32 entry points
+ *   (telephony: G.711 mu-law / A-law bytes, decoded on the GPU)                             -> the *_g711 entry points
  *
  * Conventions
  *   - plain C types only; every d_* pointer is DEVICE memory on the handle's GPU (for PyTorch
@@ -174,7 +175,7 @@ int mww_resample_taps(int rate, int32_t *out, int max_taps, int *n_taps, int *L,
  * Changing a stream's rate zeroes its resampler history and nothing else: it then continues as a stream at the new rate
  * that has been given N(t, r_new) samples of silence.  Call mww_reset(ids) as well to restart its frontend and models.
  *
- * In this mode every audio entry point (mww_features*, mww_predict_clip*, host, remote, _multi, _f32) reads n_samples as
+ * In this mode every audio entry point (mww_features*, mww_predict_clip*, host, remote, _multi, _f32, _g711) reads n_samples as
  * n16; an odd n16, or an audio_stride below the call's largest D_s, is MWW_EINVAL before any work.  Each tile runs one
  * resampler launch per rate with streams in it, on those streams only; 16 kHz streams are copied.  mww_get_input_rate
  * reports MWW_RATE_PER_STREAM and t.  mww_get_resampler_state / mww_set_resampler_state move history
@@ -307,6 +308,43 @@ int mww_predict_clip_remote_multi_f32(mww_t *h, const float *src_audio, int n_sa
                                       float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
 int mww_get_model_state(mww_t *h, int k, void *h_nn, void *h_pending);
 int mww_set_model_state(mww_t *h, int k, const void *h_nn, const void *h_pending, int pending_rows);
+
+/* ---- G.711 audio -------------------------------------------------------------------------------------------------
+ * Telephony audio arrives as G.711: RTP payload types 0 (PCMU, mu-law) and 8 (PCMA, A-law), or WAV format tags 7 and 6.
+ * Each sample is one byte, and the frontend kernels (and the resampler kernel, at any input rate but 16000) decode it on
+ * load, so a telephony server sends the bytes as they came: no decode on the host, half the bytes of int16 over PCIe.
+ * The rule is ITU-T G.711 as written in the Sun g711.c reference code (Python's audioop, SoX and FFmpeg decode the same):
+ *   mu-law: u = ~code & 0xFF; t = ((u & 0x0F) << 3) + 0x84; t <<= (u & 0x70) >> 4;
+ *           pcm = (u & 0x80) ? 0x84 - t : t - 0x84                    (range +-32124; codes 0xFF and 0x7F both give 0)
+ *   A-law:  a = code ^ 0x55; t = (a & 0x0F) << 4; seg = (a & 0x70) >> 4;
+ *           t = seg == 0 ? t + 8 : seg == 1 ? t + 0x108 : (t + 0x108) << (seg - 1);
+ *           pcm = (a & 0x80) ? t : -t                                  (range +-32256)
+ * Each _g711 entry point takes the arguments of its _f32 counterpart, with the audio as bytes and `law` (MWW_G711_ULAW or
+ * MWW_G711_ALAW) right after the audio pointer; audio_stride is in samples, which here are bytes.  Results and state are
+ * bit-identical to the int16 call on the decoded samples, and int16, float32, mu-law and A-law calls may alternate on one
+ * handle: the window carry and the resampler history hold int16 whatever the input.  Every rule of the counterpart holds
+ * unchanged: per-stream rates (n_samples is n16, row s holds D_s bytes), the refusals of the one-model calls on a handle
+ * with K > 1 models or stream sets, the n_tiles rule and in-place reads, ordering and poisoning on a half-way staged
+ * failure.  A law other than the two is MWW_EINVAL before any device work, with the handle unchanged.  Any pointer alignment
+ * and pitch work; an 8-byte-aligned buffer whose pitch, n_samples and buffered count are multiples of 8 takes the vector
+ * loads (8 bytes at a time).  A staging tile holds half the bytes of an int16 one, so the staged paths need no staging or
+ * scratch beyond what an int16 call uses.  One call's rows share one law. */
+#define MWW_G711_ULAW 1
+#define MWW_G711_ALAW 2
+int mww_features_g711(mww_t *h, const uint8_t *d_audio, int law, int n_samples, long long audio_stride,
+                      uint16_t *d_feat, int max_rows, int *h_rows_out, void *cu_stream);
+int mww_predict_clip_g711(mww_t *h, const uint8_t *d_audio, int law, int n_samples, long long audio_stride,
+                          float *d_probs, int max_probs, int *h_probs_out, void *cu_stream);
+int mww_predict_clip_host_g711(mww_t *h, const uint8_t *h_audio, int law, int n_samples, long long audio_stride,
+                               float *h_probs, int max_probs, int *h_probs_out);
+int mww_predict_clip_remote_g711(mww_t *h, const uint8_t *src_audio, int law, int n_samples, long long audio_stride,
+                                 float *d_probs, int max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
+int mww_predict_clip_multi_g711(mww_t *h, const uint8_t *d_audio, int law, int n_samples, long long audio_stride,
+                                float *const *d_probs, const int *max_probs, int *h_probs_out, void *cu_stream);
+int mww_predict_clip_host_multi_g711(mww_t *h, const uint8_t *h_audio, int law, int n_samples, long long audio_stride,
+                                     float *const *h_probs, const int *max_probs, int *h_probs_out);
+int mww_predict_clip_remote_multi_g711(mww_t *h, const uint8_t *src_audio, int law, int n_samples, long long audio_stride,
+                                       float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
 
 /* ---- each model on its own streams ------------------------------------------------------------------------------
  * A server whose satellites each listen for their own wake word runs one frontend over all streams and each model only on

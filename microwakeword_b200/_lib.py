@@ -15,6 +15,7 @@ SO_PATH = os.path.join(_HERE, "libmww_b200.so")
 
 MWW_ROWS_U16, MWW_ROWS_F32, MWW_ROWS_I8 = 0, 1, 2
 MWW_RATE_PER_STREAM = 0
+MWW_G711_ULAW, MWW_G711_ALAW = 1, 2
 
 # every symbol include/mww.h declares (checked by tests/test_capi_symbols.py)
 EXPORTS = (
@@ -36,6 +37,8 @@ EXPORTS = (
     "mww_detector_reset", "mww_detector_reset_device", "mww_detector_get_state", "mww_detector_set_state",
     "mww_multi_detector_create", "mww_multi_detector_update", "mww_multi_detector_get_state", "mww_multi_detector_set_state",
     "mww_set_detector_cutoffs", "mww_get_detector_cutoffs", "mww_set_multi_detector_cutoffs", "mww_get_multi_detector_cutoffs",
+    "mww_features_g711", "mww_predict_clip_g711", "mww_predict_clip_host_g711", "mww_predict_clip_remote_g711",
+    "mww_predict_clip_multi_g711", "mww_predict_clip_host_multi_g711", "mww_predict_clip_remote_multi_g711",
 )
 
 
@@ -246,6 +249,12 @@ def lib() -> ctypes.CDLL:
     L.mww_set_multi_detector_cutoffs.argtypes = [vp, i32, vp, vp, i32, vp]
     L.mww_get_multi_detector_cutoffs.restype = i32
     L.mww_get_multi_detector_cutoffs.argtypes = [vp, i32, vp]
+    # G.711 forms: the int16 counterpart's arguments with the law (MWW_G711_*) after the audio pointer
+    for name in ("mww_features", "mww_predict_clip", "mww_predict_clip_host", "mww_predict_clip_remote", "mww_predict_clip_multi",
+                 "mww_predict_clip_host_multi", "mww_predict_clip_remote_multi"):
+        args = getattr(L, name).argtypes
+        getattr(L, name + "_g711").restype = i32
+        getattr(L, name + "_g711").argtypes = args[:2] + [i32] + args[2:]
     _lib = L
     return L
 

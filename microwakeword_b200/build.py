@@ -29,6 +29,10 @@ MD_SOURCES = ["mww_detector_models.cu"]
 # libraries keep exactly the kernels uniform mode runs
 DC_OUT = os.path.join(HERE, "libmww_detector_cutoffs.so")
 DC_SOURCES = ["mww_detector_cutoffs.cu"]
+# and the frontend and resampler kernels for G.711 audio (mww_features_g711 and the other _g711 entry points), so that
+# libmww_b200.so and the two resampler libraries keep exactly the kernels int16 and float32 audio run
+G711_OUT = os.path.join(HERE, "libmww_g711.so")
+G711_SOURCES = ["mww_frontend_g711.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -51,7 +55,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -70,9 +74,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if not force and not _stale():
             return OUT
         for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (RR_OUT, RR_SOURCES, []), (DET_OUT, DET_SOURCES, []),
-                                    (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []),
+                                    (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []), (G711_OUT, G711_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
-                                                    "-lmww_detector_models", "-lmww_detector_cutoffs", "-Xlinker", "-rpath,$ORIGIN"])):
+                                                    "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711",
+                                                    "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra
             res = subprocess.run(cmd, capture_output=True, text=True)

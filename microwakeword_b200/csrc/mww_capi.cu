@@ -17,6 +17,7 @@
 
 #include "../../include/mww.h"
 #include "mww_container.h"
+#include "mww_frontend_dev.cuh"
 #include "mww_kernels.h"
 #include "mww_nn_tc.h"
 #include "mww_streams.h"
@@ -1372,7 +1373,7 @@ int mww_infer_features(mww_t *h, const void *d_rows, int row_type, int n_rows, l
 // tiles; a copy stream brings tile t+1 into one of two staging buffers (cudaMemcpyAsync, cudaMemcpyDefault: the copy
 // engine of THIS GPU pulls over PCIe or NVLink, no SM is involved on either side) while the kernels of tile t run on the
 // compute stream, and for a host destination a third stream drains the scores.  The bodies are templates over the sample
-// type (int16_t or float), hence C++ linkage.
+// type (int16_t, float, or the G.711 types), hence C++ linkage.
 extern "C++" {
 namespace {
 
@@ -1400,8 +1401,8 @@ size_t probs_tile_offset(const mww_t *h, const NnOuts &o, int tile, size_t k) {
     return off;
 }
 
-// T = int16_t or float: the staging buffers hold the caller's samples as they are, and the frontend and carry kernels of
-// that sample type convert them (as on the device path)
+// T = int16_t, float, Ulaw8 or Alaw8: the staging buffers hold the caller's samples as they are, and the frontend and carry
+// kernels of that sample type convert them (as on the device path)
 template <typename T>
 int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, const NnOuts &o, bool dst_is_host,
                  int tile, int n_frames, int n16) {
@@ -1489,12 +1490,10 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
     // fewer than 2 048 streams per tile so that every launch still fills the GPU
     if (want_tiles <= 0) want_tiles = 16;
     // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
-    // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone
-    // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
-    // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone.  A resampling handle adds its
-    // 16 kHz tile scratch.
+    // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone, and G.711 tiles (half an int16
+    // tile) need nothing beyond that either.  A resampling handle adds its 16 kHz tile scratch.
     const long long width = input_width(h, n_samples);      // per-stream rates: the call's largest D_s
-    const size_t staged_bytes = sizeof(T) == sizeof(int16_t) ? 0 : 2 * (size_t)std::max<long long>(width, 1) * sizeof(T);
+    const size_t staged_bytes = sizeof(T) <= sizeof(int16_t) ? 0 : 2 * (size_t)std::max<long long>(width, 1) * sizeof(T);
     const size_t gather = gather_bytes_per_stream(h, n_frames);
     int tile = tile_streams(h, n_frames, true, staged_bytes + gather + (resampling(h) ? (size_t)n16 * 2 : 0));
     tile = std::max(1, std::min(tile, std::max((h->n_streams + want_tiles - 1) / want_tiles, std::min(h->n_streams, h->min_tile_streams))));
@@ -1632,6 +1631,70 @@ int mww_predict_clip_remote_multi_f32(mww_t *h, const float *src_audio, int n_sa
                                       const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
     return predict_clip_remote_impl(h, "mww_predict_clip_remote_multi_f32", src_audio, n_samples, audio_stride, d_probs, max_probs,
                                     h_probs_out, n_tiles, cu_stream);
+}
+
+// ---- G.711 audio: the bodies above with the law as the sample type (Ulaw8 / Alaw8, decoded inside the kernels) ----------
+extern "C++" {
+namespace {
+
+// run(audio as the law's sample type); a law other than the two is refused before anything else looks at the handle's state
+template <typename F>
+int with_law(mww_t *h, const char *who, int law, const uint8_t *audio, F run) {
+    if (!h) return MWW_EINVAL;
+    if (law == MWW_G711_ULAW) return run(reinterpret_cast<const Ulaw8 *>(audio));
+    if (law == MWW_G711_ALAW) return run(reinterpret_cast<const Alaw8 *>(audio));
+    return fail(h, MWW_EINVAL, std::string(who) + ": law must be MWW_G711_ULAW (1) or MWW_G711_ALAW (2), not " + std::to_string(law));
+}
+
+}  // namespace
+}  // extern "C++"
+
+int mww_features_g711(mww_t *h, const uint8_t *d_audio, int law, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
+                      int *h_rows_out, void *cu_stream) {
+    return with_law(h, "mww_features_g711", law, d_audio, [&](auto a) {
+        return features_impl(h, "mww_features_g711", a, n_samples, audio_stride, d_feat, max_rows, h_rows_out, cu_stream);
+    });
+}
+int mww_predict_clip_g711(mww_t *h, const uint8_t *d_audio, int law, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                          int *h_probs_out, void *cu_stream) {
+    return with_law(h, "mww_predict_clip_g711", law, d_audio, [&](auto a) {
+        if (int rc = refuse_multi(h, "mww_predict_clip_g711", "mww_predict_clip_multi_g711")) return rc;
+        return predict_clip_impl(h, "mww_predict_clip_g711", a, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out, cu_stream);
+    });
+}
+int mww_predict_clip_multi_g711(mww_t *h, const uint8_t *d_audio, int law, int n_samples, long long audio_stride, float *const *d_probs,
+                                const int *max_probs, int *h_probs_out, void *cu_stream) {
+    return with_law(h, "mww_predict_clip_multi_g711", law, d_audio, [&](auto a) {
+        return predict_clip_impl(h, "mww_predict_clip_multi_g711", a, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
+    });
+}
+int mww_predict_clip_host_g711(mww_t *h, const uint8_t *h_audio, int law, int n_samples, long long audio_stride, float *h_probs,
+                               int max_probs, int *h_probs_out) {
+    return with_law(h, "mww_predict_clip_host_g711", law, h_audio, [&](auto a) {
+        if (int rc = refuse_multi(h, "mww_predict_clip_host_g711", "mww_predict_clip_host_multi_g711")) return rc;
+        return predict_clip_host_impl(h, "mww_predict_clip_host_g711", a, n_samples, audio_stride, &h_probs, &max_probs, h_probs_out);
+    });
+}
+int mww_predict_clip_host_multi_g711(mww_t *h, const uint8_t *h_audio, int law, int n_samples, long long audio_stride,
+                                     float *const *h_probs, const int *max_probs, int *h_probs_out) {
+    return with_law(h, "mww_predict_clip_host_multi_g711", law, h_audio, [&](auto a) {
+        return predict_clip_host_impl(h, "mww_predict_clip_host_multi_g711", a, n_samples, audio_stride, h_probs, max_probs, h_probs_out);
+    });
+}
+int mww_predict_clip_remote_g711(mww_t *h, const uint8_t *src_audio, int law, int n_samples, long long audio_stride, float *d_probs,
+                                 int max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
+    return with_law(h, "mww_predict_clip_remote_g711", law, src_audio, [&](auto a) {
+        if (int rc = refuse_multi(h, "mww_predict_clip_remote_g711", "mww_predict_clip_remote_multi_g711")) return rc;
+        return predict_clip_remote_impl(h, "mww_predict_clip_remote_g711", a, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out,
+                                        n_tiles, cu_stream);
+    });
+}
+int mww_predict_clip_remote_multi_g711(mww_t *h, const uint8_t *src_audio, int law, int n_samples, long long audio_stride,
+                                       float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
+    return with_law(h, "mww_predict_clip_remote_multi_g711", law, src_audio, [&](auto a) {
+        return predict_clip_remote_impl(h, "mww_predict_clip_remote_multi_g711", a, n_samples, audio_stride, d_probs, max_probs,
+                                        h_probs_out, n_tiles, cu_stream);
+    });
 }
 
 // ---- host memory next to the GPU ---------------------------------------------------------------------------------

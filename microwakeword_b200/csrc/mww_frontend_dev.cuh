@@ -213,6 +213,25 @@ MWW_HD int16_t pcm16_from_f32(float x) {
 MWW_HD int16_t pcm16(int16_t v) { return v; }
 MWW_HD int16_t pcm16(float v) { return pcm16_from_f32(v); }
 
+// G.711 audio (telephony: RTP payload types 0 and 8, WAV format tags 7 and 6) comes one byte per sample.  The two sample
+// types keep the law in the type, so every kernel template decodes on load as it converts float32, and the byte becomes
+// the int16 sample the rule of ITU-T G.711 (as in the Sun g711.c reference code, and Python's audioop) gives it.
+struct Ulaw8 { uint8_t v; };   // mu-law (PCMU): range +-32124, codes 0xFF and 0x7F both decode to 0
+struct Alaw8 { uint8_t v; };   // A-law (PCMA): range +-32256
+MWW_HD int16_t ulaw_decode(uint32_t code) {
+    const uint32_t u = ~code & 0xFFu;
+    const int32_t t = (int32_t)((((u & 0x0Fu) << 3) + 0x84u) << ((u & 0x70u) >> 4));
+    return (int16_t)((u & 0x80u) ? 0x84 - t : t - 0x84);
+}
+MWW_HD int16_t alaw_decode(uint32_t code) {
+    const uint32_t a = code ^ 0x55u, seg = (a & 0x70u) >> 4;
+    const int32_t m = (int32_t)((a & 0x0Fu) << 4);
+    const int32_t t = seg == 0 ? m + 8 : (m + 0x108) << (seg == 1 ? 0 : seg - 1);
+    return (int16_t)((a & 0x80u) ? t : -t);
+}
+MWW_HD int16_t pcm16(Ulaw8 v) { return ulaw_decode(v.v); }
+MWW_HD int16_t pcm16(Alaw8 v) { return alaw_decode(v.v); }
+
 // P0: bring the group's audio span into shared memory.  The stream's sample sequence is
 // carry[0 .. used) followed by audio[0 .. n_samples); group g needs samples [160*f0, 160*f0 + 2880).
 template <typename T>

@@ -19,7 +19,9 @@ inline bool first_launch_on_this_device(bool (&done)[64]) {
 }
 
 // Every launcher that reads caller audio is instantiated for T = int16_t (PCM) and T = float (float32 in [-1, 1], converted
-// on load with pcm16_from_f32); the window carry is int16 either way, so calls of both types can follow each other.
+// on load with pcm16_from_f32) in libmww_b200.so, and for T = Ulaw8 and Alaw8 (G.711 bytes, decoded on load) in
+// libmww_g711.so (mww_frontend_g711.cu); the window carry is int16 whatever T is, so calls of all four types can follow
+// each other.
 template <typename T>
 cudaError_t launch_k1(const FrontendParams &P, const int16_t *carry, int used, const T *audio,
                       long long audio_stride, int n_samples, int n_streams, int n_frames, uint32_t *vout, int sm_count,
@@ -112,7 +114,8 @@ cudaError_t launch_compact_ids(int32_t *out, const int32_t *ids, int n, const in
 #include "mww_resample.h"
 namespace mww {
 // input-rate resampler (mww_resample.cu, definition and index math in mww_resample.h): a tile's input samples -> its 16 kHz
-// int16 samples out [n_streams][out_stride], history moved on.  T = int16_t or float (pcm16_from_f32 on load).
+// int16 samples out [n_streams][out_stride], history moved on.  T = int16_t or float (pcm16_from_f32 on load), or
+// Ulaw8 / Alaw8 (decoded on load; instantiated in libmww_g711.so).
 template <typename T>
 cudaError_t launch_resample(const ResampleArgs &a, const T *audio, int16_t *out, int sm_count, cudaStream_t st);
 // the same for the a.n_streams members ids[0, n) (device memory, sorted global ids) of one rate in the tile that starts at

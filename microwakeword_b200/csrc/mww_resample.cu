@@ -5,11 +5,6 @@
 
 namespace mww {
 
-template <typename T>
-cudaError_t launch_resample(const ResampleArgs &a, const T *audio, int16_t *out, int sm_count, cudaStream_t st) {
-    return launch_rows(a, audio, out, TileRows{}, sm_count, st);
-}
-
 template cudaError_t launch_resample<int16_t>(const ResampleArgs &, const int16_t *, int16_t *, int, cudaStream_t);
 template cudaError_t launch_resample<float>(const ResampleArgs &, const float *, int16_t *, int, cudaStream_t);
 

@@ -1,9 +1,10 @@
-// mww_resample.cuh -- the input-rate resampler kernel (definition and index math: mww_resample.h) and its launcher, included
-// by the two translation units that instantiate it: mww_resample.cu (the tile's streams in order, a handle with one input
-// rate) and mww_resample_rates.cu (one rate's members in the tile, per-stream rates), each in a companion library of its own.
+// mww_resample.cuh -- the input-rate resampler kernel (definition and index math: mww_resample.h) and its launchers, included
+// by the translation units that instantiate them: mww_resample.cu (the tile's streams in order, a handle with one input
+// rate) and mww_resample_rates.cu (one rate's members in the tile, per-stream rates), each in a companion library of its own,
+// and mww_frontend_g711.cu (both, for G.711 audio).
 //
 // One launch per stream tile (per rate in the tile with per-stream rates) turns input-rate samples (int16, or float32
-// converted by pcm16_from_f32 on load) into 16 kHz int16 samples in scratch, which the frontend kernels then read as any
+// converted by pcm16_from_f32, or G.711 decoded, on load) into 16 kHz int16 samples in scratch, which the frontend kernels then read as any
 // int16 audio, and moves each stream's history forward.  Persistent CTAs: each copies the polyphase table into shared memory
 // once and then takes whole streams, so the stream's history is read and rewritten by the one CTA that owns it.  Per stream
 // the outputs go in chunks of kChunk: the chunk's input window (up to T - 1 samples before its first newest input, from the
@@ -96,6 +97,18 @@ cudaError_t launch_rows(const ResampleArgs &a, const T *audio, int16_t *out, Row
     const int grid = std::min(a.n_streams, std::max(per_sm, 1) * sm_count);
     resample_kernel<T, Rows><<<grid, kResampleThreads, smem, st>>>(a, audio, out, rows);
     return cudaGetLastError();
+}
+
+// the launchers of mww_kernels.h, instantiated per sample type by mww_resample.cu and mww_resample_rates.cu (int16_t, float)
+// and by mww_frontend_g711.cu (Ulaw8, Alaw8)
+template <typename T>
+cudaError_t launch_resample(const ResampleArgs &a, const T *audio, int16_t *out, int sm_count, cudaStream_t st) {
+    return launch_rows(a, audio, out, TileRows{}, sm_count, st);
+}
+template <typename T>
+cudaError_t launch_resample_members(const ResampleArgs &a, const int32_t *ids, int first, const T *audio, int16_t *out, int sm_count,
+                                    cudaStream_t st) {
+    return launch_rows(a, audio, out, MemberRows{ids, first}, sm_count, st);
 }
 
 }  // namespace mww

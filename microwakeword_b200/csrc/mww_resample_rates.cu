@@ -5,12 +5,6 @@
 
 namespace mww {
 
-template <typename T>
-cudaError_t launch_resample_members(const ResampleArgs &a, const int32_t *ids, int first, const T *audio, int16_t *out, int sm_count,
-                                    cudaStream_t st) {
-    return launch_rows(a, audio, out, MemberRows{ids, first}, sm_count, st);
-}
-
 template cudaError_t launch_resample_members<int16_t>(const ResampleArgs &, const int32_t *, int, const int16_t *, int16_t *, int, cudaStream_t);
 template cudaError_t launch_resample_members<float>(const ResampleArgs &, const int32_t *, int, const float *, int16_t *, int, cudaStream_t);
 

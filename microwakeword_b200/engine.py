@@ -89,6 +89,26 @@ RATE_PER_STREAM = _lib.MWW_RATE_PER_STREAM      # input_rate of an engine with p
 LIVE_SAMPLES16 = 480                            # one 30 ms live call, in 16 kHz samples
 
 
+G711_LAWS = {"ulaw": _lib.MWW_G711_ULAW, "alaw": _lib.MWW_G711_ALAW}     # law= of the audio calls, for uint8 G.711 audio
+
+
+def _law_code(law, is_uint8: bool):
+    """law= of an audio call -> the MWW_G711_* code for uint8 audio, None for int16 / float32 audio; ValueError for an
+    unknown law, uint8 audio without a law, or a law with other audio"""
+    if law is not None and (not isinstance(law, str) or law not in G711_LAWS):
+        raise ValueError("law must be 'ulaw' or 'alaw', not %r" % (law,))
+    if is_uint8 and law is None:
+        raise ValueError("uint8 audio is G.711: give law='ulaw' or law='alaw'")
+    if law is not None and not is_uint8:
+        raise ValueError("law= is for uint8 G.711 audio, not int16 or float32")
+    return None if law is None else G711_LAWS[law]
+
+
+def _kind(dtype) -> str:
+    """numpy or torch sample dtype -> "int16", "float32", "uint8", ..."""
+    return str(dtype).replace("torch.", "")
+
+
 def _ratio(rate: int):
     from math import gcd
     g = gcd(16000, int(rate))
@@ -329,43 +349,59 @@ class _Engine:
     def launch_count(self) -> int:
         return int(self._L.mww_launch_count(self._h))
 
-    def _check_audio(self, audio):
+    def _check_audio(self, audio, law=None):
         """-> (n_samples, row pitch in samples, is_float32).  float32 audio is converted to int16 inside the frontend kernels,
         exactly as audio_utils.to_int16 converts it on the host; other float dtypes are refused (float64 keeps its exact host
-        conversion: rounding it to float32 first could move a sample across an integer boundary after the x 32768)."""
+        conversion: rounding it to float32 first could move a sample across an integer boundary after the x 32768).  uint8
+        audio is G.711 of the given law (_law_code), decoded inside the kernels."""
         torch = _torch()
-        if (audio.dtype not in (torch.int16, torch.float32) or audio.dim() != 2 or audio.shape[0] != self.n_streams
+        if (audio.dtype not in (torch.int16, torch.float32, torch.uint8) or audio.dim() != 2 or audio.shape[0] != self.n_streams
                 or not audio.is_cuda):
-            raise ValueError("audio must be a CUDA int16 or float32 tensor of shape [n_streams=%d, n_samples]" % self.n_streams)
+            raise ValueError("audio must be a CUDA int16 or float32 tensor (uint8 with law=) of shape [n_streams=%d, n_samples]"
+                             % self.n_streams)
+        _law_code(law, audio.dtype == torch.uint8)
         if audio.stride(1) != 1 and audio.shape[1] > 1:
             raise ValueError("audio samples must be contiguous along the last dimension")
         return audio.shape[1], (audio.stride(0) if audio.shape[1] > 0 else 0), audio.dtype == torch.float32
 
-    def _check_host_audio(self, audio: np.ndarray):
+    def _check_host_audio(self, audio: np.ndarray, law=None):
         """int16 or float32 host audio [S, N] -> (the array with contiguous samples, its row pitch in samples, is_float32).
         An array whose samples are not contiguous, or whose row stride is not a whole number of samples >= N (a view made
         with as_strided or an explicit strides= argument, a broadcast, reversed rows), is copied first.  float32 goes through
         the staged pipeline as it is and is converted on the GPU as _check_audio describes; float64, other dtypes and wrong
-        shapes raise ValueError here, before the library is called, as they do on the device path."""
-        if (not isinstance(audio, np.ndarray) or audio.dtype not in (np.int16, np.float32) or audio.ndim != 2
+        shapes raise ValueError here, before the library is called, as they do on the device path.  uint8 is G.711 audio of
+        the given law, as on the device path."""
+        if (not isinstance(audio, np.ndarray) or audio.dtype not in (np.int16, np.float32, np.uint8) or audio.ndim != 2
                 or audio.shape[0] != self.n_streams):
-            raise ValueError("audio must be an int16 or float32 array of shape [n_streams=%d, n_samples]" % self.n_streams)
+            raise ValueError("audio must be an int16 or float32 array (uint8 with law=) of shape [n_streams=%d, n_samples]"
+                             % self.n_streams)
+        _law_code(law, audio.dtype == np.uint8)
         n, size = audio.shape[1], audio.itemsize
         if n > 0 and ((audio.strides[1] != size and n > 1) or audio.strides[0] % size or audio.strides[0] < n * size):
             audio = np.ascontiguousarray(audio)
         return audio, (audio.strides[0] // audio.itemsize if n else 0), audio.dtype == np.float32
 
-    def _remote_fn(self, dtype, name: str):
-        """the int16 or float32 form of the raw-pointer entry point `name`, from a numpy (or torch) sample dtype"""
-        if str(dtype) in ("torch.int16", "torch.float32"):
-            dtype = str(dtype)[len("torch."):]
+    def _remote_fn(self, dtype, name: str, law=None):
+        """the int16, float32 or G.711 (uint8 with `law`) form of the raw-pointer entry point `name`, from a numpy (or torch)
+        sample dtype"""
+        if str(dtype) in ("torch.int16", "torch.float32", "torch.uint8"):
+            dtype = _kind(dtype)
         try:
             dt = np.dtype(dtype)
         except TypeError:
             dt = None
-        if dt not in (np.dtype(np.int16), np.dtype(np.float32)):
-            raise ValueError("dtype must be int16 or float32, not %r" % (dtype,))
-        return getattr(self._L, name + "_f32" if dt == np.float32 else name)
+        if dt not in (np.dtype(np.int16), np.dtype(np.float32), np.dtype(np.uint8)):
+            raise ValueError("dtype must be int16 or float32 (uint8 with law=), not %r" % (dtype,))
+        return self._audio_fn(name, dt.name, law)
+
+    def _audio_fn(self, name: str, kind: str, law=None):
+        """the entry point `name` for audio of `kind` ("int16", "float32" or "uint8"): `name`, its _f32 form, or its _g711 form
+        with the law's code passed after the audio pointer"""
+        code = _law_code(law, kind == "uint8")
+        if code is None:
+            return getattr(self._L, name + "_f32" if kind == "float32" else name)
+        fn = getattr(self._L, name + "_g711")
+        return lambda h, audio, *rest: fn(h, audio, code, *rest)
 
     def _check_probs_out(self, out) -> None:
         torch = _torch()
@@ -398,11 +434,12 @@ class _Engine:
     def reset_frontend(self):
         _lib.check(self._h, self._L.mww_reset_frontend(self._h, self._cu_stream()))
 
-    def features(self, audio, out=None, samples16=None):
+    def features(self, audio, out=None, samples16=None, law=None):
         """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer.
-        With per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16)."""
+        With per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16).  G.711 audio: a uint8 tensor
+        of codes and law='ulaw' or 'alaw', decoded inside the kernels (include/mww.h gives the rule)."""
         torch = _torch()
-        width, stride, is_f32 = self._check_audio(audio)
+        width, stride, _ = self._check_audio(audio, law)
         n = self._call_len(width, samples16)
         stride = max(stride, width)
         rows = rows_for(self.frontend_buffered, self._samples16(n), self.hop)
@@ -412,7 +449,7 @@ class _Engine:
               or out.shape[1] < max(rows, 1) or out.shape[2] != NUM_FEATURES):
             raise ValueError("out must be a contiguous CUDA uint16 tensor [n_streams, >= rows, 40]")
         got = ctypes.c_int(0)
-        fn = self._L.mww_features_f32 if is_f32 else self._L.mww_features
+        fn = self._audio_fn("mww_features", _kind(audio.dtype), law)
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, stride, out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
@@ -557,51 +594,54 @@ class StreamEngine(_Engine):
             raise ValueError("dst_ids and src_ids must have the same length")
         _lib.check(self._h, self._L.mww_copy_nn_state(self._h, d.ctypes.data, src._h, s.ctypes.data, d.size, self._cu_stream()))
 
-    def predict_clip(self, audio, out=None, samples16=None):
+    def predict_clip(self, audio, out=None, samples16=None, law=None):
         """int16 or float32 CUDA tensor [S, N] -> float32 probabilities [S, steps]; state carries over between calls.  float32
         samples are converted to int16 inside the frontend kernels (x * 32768, clipped, as audio_utils.to_int16).  With
-        per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16)."""
+        per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16).  G.711: uint8 codes with
+        law='ulaw' or 'alaw' (as features)."""
         torch = _torch()
-        width, stride, is_f32 = self._check_audio(audio)
+        width, stride, _ = self._check_audio(audio, law)
         n = self._call_len(width, samples16)
         stride = max(stride, width)
         steps = self._steps(n)
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
         got = ctypes.c_int(0)
-        fn = self._L.mww_predict_clip_f32 if is_f32 else self._L.mww_predict_clip
+        fn = self._audio_fn("mww_predict_clip", _kind(audio.dtype), law)
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, stride, out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
-    def step(self, audio, out=None):
+    def step(self, audio, out=None, law=None):
         """the live "one chunk of new audio per call" surface (north_star step()): predict_clip; with per-stream rates a
         30 ms call (samples16 = 480)"""
-        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None)
+        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None, law=law)
 
-    def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None, samples16=None) -> np.ndarray:
+    def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None, samples16=None, law=None) -> np.ndarray:
         """int16 or float32 HOST array [S, N] -> float32 HOST array [S, steps]; copies are pipelined inside the library.
-        float32 samples cross PCIe as they are and are converted in the frontend kernels (as predict_clip converts them).
-        Other dtypes (float64 included) and wrong shapes: ValueError; a too-small `out`: MwwError."""
-        audio, stride, is_f32 = self._check_host_audio(audio)
+        float32 samples cross PCIe as they are and are converted in the frontend kernels (as predict_clip converts them), and
+        so do uint8 G.711 codes with law='ulaw' or 'alaw' (one byte per sample).  Other dtypes (float64 included) and wrong
+        shapes: ValueError; a too-small `out`: MwwError."""
+        audio, stride, _ = self._check_host_audio(audio, law)
         n = self._call_len(audio.shape[1], samples16)
         steps = self._steps(n)
         if out is None:
             out = np.empty((self.n_streams, max(steps, 1)), np.float32)
         got = ctypes.c_int(0)
-        fn = self._L.mww_predict_clip_host_f32 if is_f32 else self._L.mww_predict_clip_host
+        fn = self._audio_fn("mww_predict_clip_host", _kind(audio.dtype), law)
         _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, out.ctypes.data, out.shape[1], ctypes.byref(got)))
         return out[:, :got.value]
 
     def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None, dtype=np.int16,
-                            samples16=None):
-        """Audio [S, n_samples] of `dtype` (int16 or float32; stride in samples) at address `src_ptr` -- device memory of a PEER
+                            samples16=None, law=None):
+        """Audio [S, n_samples] of `dtype` (int16, float32, or uint8 G.711 codes with law='ulaw' or 'alaw'; stride in samples)
+        at address `src_ptr` -- device memory of a PEER
         GPU mapped into this process (sharding.IngestBuffer.block_ptr) or host memory (mww_predict_clip_remote[_f32]).
         tiles = 0: a peer-mapped (or local) buffer is read in place by the frontend kernel, over NVLink; host memory is staged
         in 16 tiles.  tiles > 0: always staged -- this GPU's copy engine pulls tile t+1 while tile t computes.  Returns float32
         CUDA probabilities [S, steps]; stream-ordered like predict_clip.  With per-stream rates n_samples is the samples each
         row holds (>= every inputs_for(samples16)) and samples16= the call."""
         torch = _torch()
-        fn = self._remote_fn(dtype, "mww_predict_clip_remote")
+        fn = self._remote_fn(dtype, "mww_predict_clip_remote", law)
         width = int(n_samples)
         n = self._call_len(width, samples16)
         stride = int(stride) if stride else width
@@ -759,35 +799,35 @@ class MultiModelEngine(_Engine):
         maxp = (ctypes.c_int * K)(*[o.shape[1] for o in out])
         return out, ptrs, maxp, (ctypes.c_int * K)()
 
-    def predict_clip(self, audio, out=None, samples16=None) -> list:
+    def predict_clip(self, audio, out=None, samples16=None, law=None) -> list:
         """int16 or float32 CUDA tensor [S, N] -> [float32 probabilities [S, steps_k] for each model k]; state carries over
-        between calls.  `out`: one CUDA float32 buffer [S, >= steps_k] per model to write into.  samples16=: as
+        between calls.  `out`: one CUDA float32 buffer [S, >= steps_k] per model to write into.  samples16= and law=: as
         StreamEngine.predict_clip."""
-        width, stride, is_f32 = self._check_audio(audio)
+        width, stride, _ = self._check_audio(audio, law)
         n = self._call_len(width, samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
-        fn = self._L.mww_predict_clip_multi_f32 if is_f32 else self._L.mww_predict_clip_multi
+        fn = self._audio_fn("mww_predict_clip_multi", _kind(audio.dtype), law)
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, width), ptrs, maxp, got, self._cu_stream()))
         return [o[:, :g] for o, g in zip(out, got)]
 
-    def step(self, audio, out=None) -> list:
+    def step(self, audio, out=None, law=None) -> list:
         """predict_clip; with per-stream rates a 30 ms call (samples16 = 480)"""
-        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None)
+        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None, law=law)
 
-    def predict_clip_host(self, audio: np.ndarray, out=None, samples16=None) -> list:
-        """int16 or float32 HOST array [S, N] -> [float32 HOST array [S, steps_k] for each model k]; each audio tile is copied
-        once."""
-        audio, stride, is_f32 = self._check_host_audio(audio)
+    def predict_clip_host(self, audio: np.ndarray, out=None, samples16=None, law=None) -> list:
+        """int16 or float32 HOST array (uint8 with law=) [S, N] -> [float32 HOST array [S, steps_k] for each model k]; each
+        audio tile is copied once."""
+        audio, stride, _ = self._check_host_audio(audio, law)
         n = self._call_len(audio.shape[1], samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, True)
-        fn = self._L.mww_predict_clip_host_multi_f32 if is_f32 else self._L.mww_predict_clip_host_multi
+        fn = self._audio_fn("mww_predict_clip_host_multi", _kind(audio.dtype), law)
         _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, ptrs, maxp, got))
         return [o[:, :g] for o, g in zip(out, got)]
 
     def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None,
-                            dtype=np.int16, samples16=None) -> list:
+                            dtype=np.int16, samples16=None, law=None) -> list:
         """StreamEngine.predict_clip_remote for every model: one result per model, each audio tile pulled once."""
-        fn = self._remote_fn(dtype, "mww_predict_clip_remote_multi")
+        fn = self._remote_fn(dtype, "mww_predict_clip_remote_multi", law)
         width = int(n_samples)
         n = self._call_len(width, samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
