@@ -462,6 +462,45 @@ int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, m
 int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout,
                        void *cu_stream);
 
+/* ---- audio history: the last seconds of each stream's 16 kHz audio, kept on the GPU -----------------------------------
+ * What a stream said around a detection (for a second-stage verifier, the pre-roll of an STT request, or false-accept audio
+ * to retrain on) exists on the GPU only once G.711 decoding and resampling have run there.  A handle can keep it:
+ *   - A handle has an audio history of capacity C 16 kHz samples per stream: C is 0 (off, the default) or a multiple of 8
+ *     in [8, 2^22].
+ *   - A stream's history is an endless run of zeros followed by every 16 kHz int16 sample the frontend consumed for that
+ *     stream since the history was last zeroed: int16 audio at 16 kHz as given, float32 audio as converted (the rule of
+ *     mww_features_f32), G.711 audio as decoded, and at any other input rate (one for all streams or per stream) the
+ *     resampler's output.
+ *   - A read of n samples (0 <= n <= C) returns the last n entries of that run for each listed stream, oldest first: the
+ *     concatenation of the (decoded, resampled) input, zero-padded on the left.
+ *   - Every audio entry point appends (mww_features* and mww_predict_clip*, in every form: device, _host, _remote, _multi,
+ *     _f32, _g711).  mww_infer_features takes rows, not audio, and appends nothing.
+ *   - Every call that zeroes a stream's window carry zeroes its history too: mww_reset (all or by id),
+ *     mww_reset_device_ids and mww_reset_frontend.  mww_import_streams zeroes the history of the streams it writes (records
+ *     do not carry it; their layout is unchanged).  mww_set_audio_history zeroes every stream.  Nothing else touches it:
+ *     not mww_set_state, mww_set_stream_rates, mww_set_model_streams or mww_set_window_step.
+ *   - So after audio calls alone since the last zeroing, a stream's last frontend_buffered history samples equal
+ *     carry[0, frontend_buffered) of mww_get_state whenever C >= frontend_buffered.
+ *   - The history changes nothing else: features, probabilities, all state and the counters are those of a handle without
+ *     it, and with C = 0 the handle issues the launches it issued before.
+ *
+ * mww_set_audio_history: allowed wherever a stateful call is.  Allocates a zeroed ring [n_streams][C] of int16 (ordered on
+ * cu_stream) and synchronises cu_stream before it frees the old ring; C = 0 frees it.  A bad C is MWW_EINVAL, a failed
+ * allocation MWW_ENOMEM; either way the old history is untouched.
+ * mww_get_audio_history: the capacity, and samples_seen, the 16 kHz samples appended since the history was enabled: one
+ * lockstep counter that resets do not clear, to place events on a time axis.
+ * mww_read_audio_history / _device_ids: asynchronous on cu_stream, after every audio call issued before it.  Row i of d_out
+ * ([n][out_stride] int16, device memory) is the last n_samples of stream ids[i]; an id listed twice is read twice.  Host
+ * ids out of range are MWW_EINVAL (as mww_reset); device ids that are negative or >= n_streams give a zero row, which covers
+ * the -1 slots of a detector's d_fired.  MWW_EINVAL before any device work when the handle keeps no history, n < 0,
+ * n_samples is outside [0, C], out_stride < n_samples, or a buffer is NULL with work to do.  A poisoned handle refuses
+ * set and read. */
+int mww_set_audio_history(mww_t *h, int capacity, void *cu_stream);
+int mww_get_audio_history(const mww_t *h, int *capacity, long long *samples_seen);
+int mww_read_audio_history(mww_t *h, const int32_t *h_ids, int n, int n_samples, int16_t *d_out, long long out_stride, void *cu_stream);
+int mww_read_audio_history_device_ids(mww_t *h, const int32_t *d_ids, int n, int n_samples, int16_t *d_out, long long out_stride,
+                                      void *cu_stream);
+
 /* ---- detection post-processing (microwakeword/test.py:337-341, :94-137, :364-373) -------------------------
  * Tracks are ragged: track i is d_probs[d_offsets[i] .. d_offsets[i] + d_lengths[i]) (float32 probabilities as
  * produced by mww_infer_features / mww_predict_clip).  All four are stateless and asynchronous on cu_stream.

@@ -39,6 +39,7 @@ EXPORTS = (
     "mww_set_detector_cutoffs", "mww_get_detector_cutoffs", "mww_set_multi_detector_cutoffs", "mww_get_multi_detector_cutoffs",
     "mww_features_g711", "mww_predict_clip_g711", "mww_predict_clip_host_g711", "mww_predict_clip_remote_g711",
     "mww_predict_clip_multi_g711", "mww_predict_clip_host_multi_g711", "mww_predict_clip_remote_multi_g711",
+    "mww_set_audio_history", "mww_get_audio_history", "mww_read_audio_history", "mww_read_audio_history_device_ids",
 )
 
 
@@ -255,6 +256,13 @@ def lib() -> ctypes.CDLL:
         args = getattr(L, name).argtypes
         getattr(L, name + "_g711").restype = i32
         getattr(L, name + "_g711").argtypes = args[:2] + [i32] + args[2:]
+    L.mww_set_audio_history.restype = i32
+    L.mww_set_audio_history.argtypes = [vp, i32, vp]
+    L.mww_get_audio_history.restype = i32
+    L.mww_get_audio_history.argtypes = [vp, pi, ctypes.POINTER(ll)]
+    for name in ("mww_read_audio_history", "mww_read_audio_history_device_ids"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, i32, vp, ll, vp]
     _lib = L
     return L
 

@@ -18,6 +18,7 @@
 #include "../../include/mww.h"
 #include "mww_container.h"
 #include "mww_frontend_dev.cuh"
+#include "mww_history.h"
 #include "mww_kernels.h"
 #include "mww_nn_tc.h"
 #include "mww_streams.h"
@@ -100,6 +101,11 @@ struct mww_handle {
     RateGroup groups[kNumRates];
     std::vector<int32_t> rate_ids;                      // every group's members, group after group
     int32_t *d_rate_ids = nullptr;                      // device copy of rate_ids
+    // audio history (mww_set_audio_history; mww_history.h): the last hist_cap 16 kHz samples of every stream, a ring row per
+    // stream; hist_seen counts the samples appended since it was enabled (resets zero rows, not the counter)
+    int16_t *d_hist = nullptr;                          // [n_streams][hist_cap]
+    int hist_cap = 0;
+    long long hist_seen = 0;
     // scratch
     uint32_t *d_v = nullptr; size_t v_bytes = 0;
     uint16_t *d_feat = nullptr; size_t feat_bytes = 0;
@@ -356,6 +362,20 @@ int run_carry_tile(mww_t *h, int first, int n, const T *d_audio, long long audio
     return MWW_OK;
 }
 
+// the audio history of streams [first, first + n): the call's n16 16 kHz samples from the source the carry update reads.
+// Unlike the carry update it runs after the fused short-call kernel too.  The caller advances h->hist_seen once per call.
+template <typename T>
+int run_history_tile(mww_t *h, int first, int n, const T *d_audio, long long audio_stride, int n16, cudaStream_t st) {
+    if (!h->d_hist || n16 <= 0) return MWW_OK;
+    CU(h, launch_history_append(h->d_hist + (size_t)first * h->hist_cap, h->hist_cap, h->hist_seen, d_audio, audio_stride, n16, n, h->sm_count, st));
+    h->launches += 1;
+    return MWW_OK;
+}
+// once per call, where the frontend's counters move on
+void end_history_call(mww_t *h, int n16) {
+    if (h->d_hist) h->hist_seen += n16;
+}
+
 // one model step per stream -> the stream-parallel live-step kernels (fp32: mww_nn_live.cuh, int8: mww_nn_i8_live.cuh)
 bool use_live(const mww_t *h, const Model &m, int n_rows) { return m.compiled() && n_rows == 3 && !h->no_live; }
 
@@ -561,6 +581,7 @@ int zero_frontend(mww_t *h, cudaStream_t st) {
     CU(h, cudaMemsetAsync(h->d_carry, 0, S * kWindow * sizeof(int16_t), st));
     CU(h, cudaMemsetAsync(h->d_estimate, 0, S * kNumChannels * sizeof(uint32_t), st));
     if (h->d_rs_hist) CU(h, cudaMemsetAsync(h->d_rs_hist, 0, S * h->rs_hist_stride * sizeof(int16_t), st));
+    if (h->d_hist) CU(h, cudaMemsetAsync(h->d_hist, 0, S * h->hist_cap * sizeof(int16_t), st));
     h->used = 0;
     h->rs_seen = 0;
     return MWW_OK;
@@ -583,7 +604,7 @@ void destroy_impl(mww_t *h) {
     cudaFree(h->d_tables); cudaFree(h->d_carry); cudaFree(h->d_estimate);
     cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
     cudaFree(h->d_gather); cudaFree(h->d_cids);
-    cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist); cudaFree(h->d_rs_out); cudaFree(h->d_rate_ids);
+    cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist); cudaFree(h->d_rs_out); cudaFree(h->d_rate_ids); cudaFree(h->d_hist);
     for (RateGroup &g : h->groups) cudaFree(g.d_table);
     for (int b = 0; b < 2; ++b) {
         cudaFree(h->d_audio_tile[b]); cudaFree(h->d_probs_tile[b]);
@@ -625,6 +646,7 @@ int features_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, lo
             if ((rc = run_resample_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n16, st))) return rc;
             if ((rc = run_frontend_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, feat, (long long)max_rows * kNumChannels, st))) return rc;
             if (n16 > 0 && (rc = run_carry_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, st))) return rc;
+            if ((rc = run_history_tile(h, first, n, h->d_rs_out, n16, n16, st))) return rc;
             continue;
         }
         rc = run_frontend_tile(h, first, n, d_audio + (size_t)first * audio_stride, audio_stride, n_samples, n_frames,
@@ -633,10 +655,12 @@ int features_impl(mww_t *h, const char *who, const T *d_audio, int n_samples, lo
     }
     if (n_samples > 0 && !resampling(h)) {
         rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
+        if (rc == MWW_OK) rc = run_history_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, st);
         if (rc) return rc;
     }
     h->used = h->used + n16 - n_frames * h->hop;
     if (resampling(h)) h->rs_seen += n_samples;
+    end_history_call(h, n16);
     if (h_rows_out) *h_rows_out = n_frames;
     return MWW_OK;
 }
@@ -747,14 +771,17 @@ int predict_clip_impl(mww_t *h, const char *who, const T *d_audio, int n_samples
         if (rc) return rc;
         // a resampling handle's carry update reads the tile's 16 kHz samples, so it runs per tile
         if (resampling(h) && n16 > 0 && (rc = run_carry_tile(h, first, n, h->d_rs_out, n16, n16, n_frames, st))) return rc;
+        if (resampling(h) && (rc = run_history_tile(h, first, n, h->d_rs_out, n16, n16, st))) return rc;
     }
     end_models_call(h, n_frames, o, h_probs_out);
     if (n_samples > 0 && !resampling(h)) {
         rc = run_carry_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, n_frames, st);
+        if (rc == MWW_OK) rc = run_history_tile(h, 0, h->n_streams, d_audio, audio_stride, n_samples, st);
         if (rc) return rc;
     }
     h->used = h->used + n16 - n_frames * h->hop;
     if (resampling(h)) h->rs_seen += n_samples;
+    end_history_call(h, n16);
     return MWW_OK;
 }
 
@@ -1065,6 +1092,7 @@ int reset_by_id(mww_t *h, const int32_t *d_ids, int n, cudaStream_t st) {
     int rc = fill_by_id(h, h->d_carry, kWindow * sizeof(int16_t), d_ids, n, h->n_streams, st);
     if (rc == MWW_OK) rc = fill_by_id(h, h->d_estimate, kNumChannels * sizeof(uint32_t), d_ids, n, h->n_streams, st);
     if (rc == MWW_OK && h->d_rs_hist) rc = fill_by_id(h, h->d_rs_hist, (size_t)h->rs_hist_stride * sizeof(int16_t), d_ids, n, h->n_streams, st);
+    if (rc == MWW_OK && h->d_hist) rc = fill_by_id(h, h->d_hist, (size_t)h->hist_cap * sizeof(int16_t), d_ids, n, h->n_streams, st);
     for (size_t k = 0; rc == MWW_OK && k < h->models.size(); ++k) {
         Model &m = h->models[k];
         if (m.members() == h->n_streams) {
@@ -1457,6 +1485,9 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
                                : run_carry_tile(h, first, n, audio_tile[b], n_samples, n_samples, n_frames, h->st_compute);
             if (rc) return rc;
         }
+        rc = resampling(h) ? run_history_tile(h, first, n, h->d_rs_out, n16, n16, h->st_compute)
+                           : run_history_tile(h, first, n, audio_tile[b], n_samples, n_samples, h->st_compute);
+        if (rc) return rc;
         if (tl[3]) CU(h, cudaEventRecord(tl[3], h->st_compute));
         CU(h, cudaEventRecord(h->ev_compute[b], h->st_compute));
         if (dst_is_host) {
@@ -1548,6 +1579,7 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
     end_models_call(h, n_frames, o, h_probs_out);
     h->used = h->used + n16 - n_frames * h->hop;
     if (resampling(h)) h->rs_seen += n_samples;
+    end_history_call(h, n16);
     return MWW_OK;
 }
 
@@ -2074,6 +2106,9 @@ int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_reco
     void *fe[kRecordMaxParts] = {nullptr, h->d_carry, h->d_estimate};
     CU(h, launch_unpack_streams(record_job_frontend(L), d_records, L.record_bytes, h->d_ids, n, fe, nullptr, nullptr, h->sm_count, st));
     h->launches += 1;
+    // records carry no audio history: the streams written start theirs afresh
+    if (h->d_hist)
+        if (int rc = fill_by_id(h, h->d_hist, (size_t)h->hist_cap * sizeof(int16_t), h->d_ids, n, h->n_streams, st)) return rc;
     for (size_t k = 0; k < h->models.size(); ++k) {
         Model &m = h->models[k];
         if (m.members() == 0) continue;
@@ -2088,6 +2123,77 @@ int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_reco
         m.tc_rows_bounded = m.tc_rows_bounded && layout->rows_are_features[k];
     }
     return MWW_OK;
+}
+
+// ---- audio history: the last C 16 kHz samples of every stream (rule: include/mww.h; ring and kernels: mww_history.{h,cu}) ----
+int mww_set_audio_history(mww_t *h, int capacity, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (!history_capacity_ok(capacity))
+        return fail(h, MWW_EINVAL, "mww_set_audio_history: the capacity must be 0 or a multiple of 8 in [8, " + std::to_string(kHistoryMaxCapacity) + "]");
+    ENTER_STATEFUL(h);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    int16_t *ring = nullptr;
+    if (capacity > 0) {
+        const size_t bytes = (size_t)h->n_streams * capacity * sizeof(int16_t);
+        cudaError_t e = cudaMalloc(&ring, bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(h, e == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("mww_set_audio_history: ") + cudaGetErrorString(e));
+        }
+        if ((e = cudaMemsetAsync(ring, 0, bytes, st)) != cudaSuccess) { cudaFree(ring); return cuda_fail(h, e, "mww_set_audio_history"); }
+    }
+    // earlier calls on the stream may still append to the old ring
+    if (h->d_hist) {
+        if (cudaError_t e = cudaStreamSynchronize(st)) { cudaFree(ring); return cuda_fail(h, e, "cudaStreamSynchronize"); }
+        cudaFree(h->d_hist);
+    }
+    h->d_hist = ring;
+    h->hist_cap = capacity;
+    h->hist_seen = 0;
+    return MWW_OK;
+}
+
+int mww_get_audio_history(const mww_t *h, int *capacity, long long *samples_seen) {
+    if (!h) return MWW_EINVAL;
+    if (capacity) *capacity = h->hist_cap;
+    if (samples_seen) *samples_seen = h->hist_seen;
+    return MWW_OK;
+}
+
+namespace {
+// the checks both reads share, before any device work; ids are the caller's (host or device) list
+int check_history_read(mww_t *h, const char *who, const void *ids, int n, int n_samples, const int16_t *d_out, long long out_stride) {
+    if (!h->d_hist) return fail(h, MWW_EINVAL, std::string(who) + ": the handle keeps no audio history (mww_set_audio_history)");
+    if (n < 0 || n_samples < 0 || n_samples > h->hist_cap || out_stride < n_samples)
+        return fail(h, MWW_EINVAL, std::string(who) + ": needs n >= 0, 0 <= n_samples <= capacity and out_stride >= n_samples");
+    if (n > 0 && n_samples > 0 && (!ids || !d_out)) return fail(h, MWW_EINVAL, std::string(who) + ": NULL ids or output");
+    return MWW_OK;
+}
+int read_history(mww_t *h, const int32_t *d_ids, int n, int n_samples, int16_t *d_out, long long out_stride, cudaStream_t st) {
+    CU(h, launch_history_read(h->d_hist, h->hist_cap, h->hist_seen, d_ids, n, h->n_streams, n_samples, d_out, out_stride, h->sm_count, st));
+    h->launches += 1;
+    return MWW_OK;
+}
+}  // namespace
+
+int mww_read_audio_history(mww_t *h, const int32_t *h_ids, int n, int n_samples, int16_t *d_out, long long out_stride, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (int rc = check_history_read(h, "mww_read_audio_history", h_ids, n, n_samples, d_out, out_stride)) return rc;
+    for (int i = 0; n_samples > 0 && i < n; ++i)
+        if (h_ids[i] < 0 || h_ids[i] >= h->n_streams) return fail(h, MWW_EINVAL, "mww_read_audio_history: stream id out of range");
+    ENTER_STATEFUL(h);
+    if (n == 0 || n_samples == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+    return read_history(h, h->d_ids, n, n_samples, d_out, out_stride, st);
+}
+
+int mww_read_audio_history_device_ids(mww_t *h, const int32_t *d_ids, int n, int n_samples, int16_t *d_out, long long out_stride, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (int rc = check_history_read(h, "mww_read_audio_history_device_ids", d_ids, n, n_samples, d_out, out_stride)) return rc;
+    ENTER_STATEFUL(h);
+    if (n == 0 || n_samples == 0) return MWW_OK;
+    return read_history(h, d_ids, n, n_samples, d_out, out_stride, static_cast<cudaStream_t>(cu_stream));
 }
 
 }  // extern "C"

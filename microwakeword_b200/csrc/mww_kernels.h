@@ -162,3 +162,15 @@ cudaError_t launch_detector_update_cutoffs(const DetectorArgs &a, const double *
                                            cudaStream_t st);
 cudaError_t launch_detector_models_update_cutoffs(const DetectModelsArgsT<DetectModelRows> &a, cudaStream_t st);
 }  // namespace mww
+
+namespace mww {
+// audio history (mww_history.cu, ring layout and index math in mww_history.h; companion library libmww_history.so)
+// the last min(n16, C) of a call's n16 16 kHz samples of streams [0, n_streams) of `audio` (pcm16 of T on load) -> their
+// slots of ring [n_streams][C], `seen` samples having come before the call
+template <typename T>
+cudaError_t launch_history_append(int16_t *ring, int C, long long seen, const T *audio, long long audio_stride, int n16, int n_streams,
+                                  int sm_count, cudaStream_t st);
+// out [n][out_stride]: row i = the last n_samples (<= C) of ring row ids[i] (device memory), zeros for an id outside [0, n_streams)
+cudaError_t launch_history_read(const int16_t *ring, int C, long long seen, const int32_t *ids, int n, int n_streams, int n_samples, int16_t *out,
+                                long long out_stride, int sm_count, cudaStream_t st);
+}  // namespace mww

@@ -86,6 +86,7 @@ def rows_for(buffered: int, n_samples: int, hop: int) -> int:
 
 INPUT_RATES = (8000, 16000, 22050, 24000, 32000, 44100, 48000)
 RATE_PER_STREAM = _lib.MWW_RATE_PER_STREAM      # input_rate of an engine with per-stream rates (set_stream_rates)
+MAX_AUDIO_HISTORY = 1 << 22                      # the largest capacity of set_audio_history, in 16 kHz samples per stream
 LIVE_SAMPLES16 = 480                            # one 30 ms live call, in 16 kHz samples
 
 
@@ -433,6 +434,66 @@ class _Engine:
 
     def reset_frontend(self):
         _lib.check(self._h, self._L.mww_reset_frontend(self._h, self._cu_stream()))
+
+    # ------------------------------------------------------------------ audio history
+    def set_audio_history(self, capacity: int) -> None:
+        """Keep the last `capacity` 16 kHz int16 samples of every stream on the GPU (mww_set_audio_history; the rule is in
+        include/mww.h): 0 (off, the default) or a multiple of 8 in [8, 2**22].  Every stream's history starts as zeros and
+        audio_samples_seen restarts at 0; a reset of a stream zeroes its history."""
+        if isinstance(capacity, bool) or int(capacity) != capacity or not (capacity == 0 or (8 <= capacity <= MAX_AUDIO_HISTORY
+                                                                                          and capacity % 8 == 0)):
+            raise ValueError("capacity must be 0 or a multiple of 8 in [8, %d] (got %r)" % (MAX_AUDIO_HISTORY, capacity))
+        _lib.check(self._h, self._L.mww_set_audio_history(self._h, int(capacity), self._cu_stream()))
+
+    def _audio_history(self):
+        cap, seen = ctypes.c_int(0), ctypes.c_longlong(0)
+        _lib.check(self._h, self._L.mww_get_audio_history(self._h, ctypes.byref(cap), ctypes.byref(seen)))
+        return cap.value, seen.value
+
+    @property
+    def audio_history_capacity(self) -> int:
+        return self._audio_history()[0]
+
+    @property
+    def audio_samples_seen(self) -> int:
+        """16 kHz samples every stream has appended since set_audio_history (resets do not clear it)"""
+        return self._audio_history()[1]
+
+    def audio_history(self, stream_ids, n_samples: int, out=None):
+        """The last n_samples (<= audio_history_capacity) 16 kHz samples of each listed stream, oldest first, zero-padded on
+        the left: a CUDA int16 tensor [len(ids), n_samples], ordered on the current CUDA stream (mww_read_audio_history).
+        `stream_ids`: a host sequence (ids in [0, n_streams)) or a contiguous 1-D CUDA int32 tensor such as a detector's
+        fired_ids, read with no host round trip (ids outside [0, n_streams), the -1 slots, give zero rows).  Read before
+        reset(ids): a reset zeroes the history.  `out`: a CUDA int16 tensor [len(ids), >= n_samples] with contiguous rows."""
+        torch = _torch()
+        cap = self.audio_history_capacity
+        if cap == 0:
+            raise ValueError("the engine keeps no audio history (set_audio_history)")
+        if isinstance(n_samples, bool) or int(n_samples) != n_samples or not 0 <= n_samples <= cap:
+            raise ValueError("n_samples must be an integer in [0, %d] (got %r)" % (cap, n_samples))
+        n_samples = int(n_samples)
+        device_ids = isinstance(stream_ids, torch.Tensor) and stream_ids.is_cuda
+        if device_ids:
+            if stream_ids.dtype != torch.int32 or stream_ids.dim() != 1 or not stream_ids.is_contiguous() or stream_ids.device != self._dev():
+                raise ValueError("device stream ids must be a contiguous 1-D CUDA int32 tensor on %s" % self._dev())
+            n = stream_ids.numel()
+        else:
+            ids = self._ids(stream_ids)
+            if ids.size and (ids.min() < 0 or ids.max() >= self.n_streams):
+                raise ValueError("stream ids must be in [0, %d)" % self.n_streams)
+            n = ids.size
+        if out is None:
+            out = torch.empty((n, n_samples), dtype=torch.int16, device=self._dev())
+        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.int16 or out.device != self._dev() or out.dim() != 2 or out.shape[0] != n
+              or out.shape[1] < n_samples or (out.stride(1) != 1 and out.shape[1] > 1) or (n > 1 and out.stride(0) < n_samples)):
+            raise ValueError("out must be a CUDA int16 tensor [len(ids)=%d, >= %d] with contiguous rows on %s" % (n, n_samples, self._dev()))
+        stride = out.stride(0) if n > 1 else max(out.shape[1], n_samples)
+        if device_ids:
+            rc = self._L.mww_read_audio_history_device_ids(self._h, stream_ids.data_ptr(), n, n_samples, out.data_ptr(), stride, self._cu_stream())
+        else:
+            rc = self._L.mww_read_audio_history(self._h, ids.ctypes.data, n, n_samples, out.data_ptr(), stride, self._cu_stream())
+        _lib.check(self._h, rc)
+        return out[:, :n_samples]
 
     def features(self, audio, out=None, samples16=None, law=None):
         """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer.
