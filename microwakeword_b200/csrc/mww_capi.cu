@@ -2,7 +2,8 @@
 //
 // Host-side orchestration only: weight/table upload (container parsing: mww_container.cc), per-stream state,
 // stream tiling against a scratch budget, and the pipelined host-buffer path.  All arithmetic is
-// in the kernels (mww_frontend.cu, mww_nn.cu, mww_nn_int8.cu); there is no CPU fallback.
+// in the kernels (mww_frontend.cu, mww_nn.cu, mww_nn_int8.cu); there is no CPU fallback.  The streaming detectors'
+// entry points, which reach a handle only through the calls declared in include/mww.h, are in mww_detector_capi.cu.
 #include <cuda_runtime.h>
 #include <sched.h>
 #include <stdio.h>
@@ -16,6 +17,7 @@
 #include <vector>
 
 #include "../../include/mww.h"
+#include "mww_capi.h"
 #include "mww_container.h"
 #include "mww_frontend_dev.cuh"
 #include "mww_history.h"
@@ -132,27 +134,17 @@ struct mww_handle {
     std::vector<cudaEvent_t> tl_ev;        // last staged call while profiling: 4 events per tile (mww_timeline_read)
 };
 
-namespace {
-
-int fail(mww_t *h, int code, const std::string &msg) {
+int mww::fail(mww_t *h, int code, const std::string &msg) {
     if (h) h->err = msg; else g_create_error = msg;
     return code;
 }
-int cuda_fail(mww_t *h, cudaError_t e, const char *what) {
+int mww::cuda_fail(mww_t *h, cudaError_t e, const char *what) {
     return fail(h, MWW_ECUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
-#define CU(h, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(h, e_, #call); } while (0)
 
-// every entry point runs with the handle's device current and puts the caller's device back on return (a process that
-// holds engines on several GPUs, or torch's current device, is not disturbed)
-struct DeviceGuard {
-    int prev = -1; bool switched = false; cudaError_t err = cudaSuccess;
-    explicit DeviceGuard(int device) {
-        if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-        if (prev != device) { err = cudaSetDevice(device); switched = err == cudaSuccess && prev >= 0; }
-    }
-    ~DeviceGuard() { if (switched) cudaSetDevice(prev); }
-};
+namespace {
+
+#define CU(h, call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(h, e_, #call); } while (0)
 #define ENTER(h) DeviceGuard guard_((h)->device); if (guard_.err != cudaSuccess) return cuda_fail((h), guard_.err, "cudaSetDevice")
 #define ENTER_STATEFUL(h) ENTER(h); if ((h)->poisoned) return fail((h), MWW_ECUDA, "an earlier staged call failed half-way; per-stream state is inconsistent until mww_reset(h, NULL, 0, stream)")
 
@@ -2194,529 +2186,6 @@ int mww_read_audio_history_device_ids(mww_t *h, const int32_t *d_ids, int n, int
     ENTER_STATEFUL(h);
     if (n == 0 || n_samples == 0) return MWW_OK;
     return read_history(h, d_ids, n, n_samples, d_out, out_stride, static_cast<cudaStream_t>(cu_stream));
-}
-
-}  // extern "C"
-
-// ---- streaming detector (include/mww.h; rule and kernels: mww_detector.h, mww_detector.cu) -------------------------------
-// An object of its own: no handle knows of it, and its messages go where a failed create's go (mww_last_error(NULL)).
-struct mww_detector {
-    int device = 0;
-    DetectorArgs a;                  // the device state and buffers, as the kernels take them
-    int32_t *d_stream_ids = nullptr;
-    int32_t *d_rows = nullptr;       // staging for a host row list (mww_detector_reset)
-    size_t rows_cap = 0;
-    // a models detector (mww_multi_detector_create): a.count / events / fired / capacity are its event buffers, the rest of
-    // `a` is unused; `m` holds the kernels' arguments, models[k] the descriptors d_models holds on the device
-    bool multi = false;
-    DetectModelsArgs m;
-    std::vector<DetectModel> models;
-    DetectModel *d_models = nullptr;
-    std::vector<std::vector<int32_t>> member_row;     // [k][n_streams]: row of each global stream in model k, -1 for none
-    // per-row mode (mww_set_detector_cutoffs, mww_set_multi_detector_cutoffs): host copies of every row's cutoff and the
-    // device arrays the per-row kernels read; empty and nullptr in uniform mode
-    std::vector<double> cutoffs;                      // plain: [n_rows]
-    double *d_cutoffs = nullptr;
-    std::vector<std::vector<double>> model_cutoffs;   // models: [k][n_k]
-    std::vector<DetectModelRows> models_rows;         // the descriptors d_models_rows holds, each with its d_row_cutoff
-    DetectModelRows *d_models_rows = nullptr;
-};
-
-namespace {
-
-#define DCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(nullptr, e_, #call); } while (0)
-#define DENTER(d) DeviceGuard guard_((d)->device); if (guard_.err != cudaSuccess) return cuda_fail(nullptr, guard_.err, "cudaSetDevice")
-
-void detector_free(mww_detector_t *d) {
-    cudaFree(d->a.hist); cudaFree(d->a.seen); cudaFree(d->a.cooldown); cudaFree(d->a.count); cudaFree(d->a.events);
-    cudaFree(d->a.fired); cudaFree(d->d_stream_ids); cudaFree(d->d_rows);
-    for (DetectModel &M : d->models) {
-        cudaFree(M.hist); cudaFree(M.seen); cudaFree(M.flag); cudaFree(const_cast<int32_t *>(M.inv));
-    }
-    cudaFree(d->d_models);
-    cudaFree(d->d_cutoffs);
-    for (DetectModelRows &M : d->models_rows) cudaFree(const_cast<double *>(M.row_cutoff));
-    cudaFree(d->d_models_rows);
-    delete d;
-}
-
-// The (id, cutoff) list of a set-cutoffs call, checked before anything changes: finite cutoffs, ids in [0, n_ids), each
-// naming a row (row_of[id] >= 0; row_of == nullptr: the id is the row) of the n_rows, none twice.  rows: the rows named,
-// [lo, hi] the span they cover.
-int check_cutoff_list(const std::string &call, const int32_t *ids, const double *c, int n, int n_ids, const int32_t *row_of, int n_rows,
-                      std::vector<int32_t> &rows, int &lo, int &hi) {
-    std::vector<char> listed((size_t)std::max(n_rows, 1), 0);
-    rows.resize((size_t)n);
-    lo = n_rows; hi = -1;
-    for (int i = 0; i < n; ++i) {
-        if (!(c[i] - c[i] == 0.0)) return fail(nullptr, MWW_EINVAL, call + ": cutoffs must be finite");
-        const int32_t id = ids[i];
-        if (id < 0 || id >= n_ids) return fail(nullptr, MWW_EINVAL, call + ": id " + std::to_string(id) + " out of range");
-        const int32_t r = row_of ? row_of[id] : id;
-        if (r < 0) return fail(nullptr, MWW_EINVAL, call + ": stream " + std::to_string(id) + " is not a member of the model's stream set");
-        if (listed[r]) return fail(nullptr, MWW_EINVAL, call + ": id " + std::to_string(id) + " listed twice");
-        listed[r] = 1;
-        rows[i] = r;
-        lo = std::min(lo, (int)r); hi = std::max(hi, (int)r);
-    }
-    return MWW_OK;
-}
-
-size_t detector_hist_elems(const mww_detector_t *d) { return (size_t)(d->a.rule.window - 1) * d->a.n_rows; }
-
-int detector_alloc(mww_detector_t *d, const int32_t *h_stream_ids) {
-    DetectorArgs &a = d->a;
-    const size_t R = (size_t)a.n_rows, C = (size_t)a.capacity;
-    DCU(cudaMalloc(&a.hist, std::max<size_t>(detector_hist_elems(d), 1) * sizeof(float)));
-    DCU(cudaMalloc(&a.seen, R * sizeof(long long)));
-    DCU(cudaMalloc(&a.cooldown, R * sizeof(int32_t)));
-    DCU(cudaMalloc(&a.count, sizeof(unsigned long long)));
-    DCU(cudaMalloc(&a.events, C * sizeof(mww_event)));
-    DCU(cudaMalloc(&a.fired, C * sizeof(int32_t)));
-    if (h_stream_ids) {
-        DCU(cudaMalloc(&d->d_stream_ids, R * sizeof(int32_t)));
-        DCU(cudaMemcpy(d->d_stream_ids, h_stream_ids, R * sizeof(int32_t), cudaMemcpyHostToDevice));
-        a.stream_ids = d->d_stream_ids;
-    }
-    DCU(cudaMemset(a.count, 0, sizeof(unsigned long long)));
-    DCU(cudaMemset(a.events, 0, C * sizeof(mww_event)));
-    DCU(cudaMemset(a.fired, 0xFF, C * sizeof(int32_t)));              // -1 in every slot
-    DCU(launch_detector_reset(a, nullptr, a.n_rows, nullptr));
-    DCU(cudaDeviceSynchronize());
-    return MWW_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
-int mww_detector_create(int device, int n_rows, int window, double cutoff, int cooldown_slices, int capacity,
-                        const int32_t *h_stream_ids, mww_detector_t **out) {
-    if (!out) return fail(nullptr, MWW_EINVAL, "mww_detector_create: out is NULL");
-    *out = nullptr;
-    if (n_rows < 1) return fail(nullptr, MWW_EINVAL, "mww_detector_create: n_rows must be at least 1");
-    if (window < 1 || window > kDetectorMaxWindow) return fail(nullptr, MWW_EINVAL, "mww_detector_create: window must be in [1, 32]");
-    if (!(cutoff - cutoff == 0.0)) return fail(nullptr, MWW_EINVAL, "mww_detector_create: cutoff must be finite");
-    if (cooldown_slices < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_create: cooldown_slices must not be negative");
-    if (capacity < 1) return fail(nullptr, MWW_EINVAL, "mww_detector_create: capacity must be at least 1");
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0)
-        return fail(nullptr, MWW_ECUDA, std::string("no CUDA device available (this library has no CPU fallback): ") + cudaGetErrorString(e));
-    if (device < 0 || device >= count) return fail(nullptr, MWW_EINVAL, "mww_detector_create: device index out of range");
-    DeviceGuard guard(device);
-    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
-    mww_detector_t *d = new mww_detector;
-    d->device = device;
-    d->a.rule.window = window; d->a.rule.cutoff = cutoff; d->a.rule.cooldown_slices = cooldown_slices;
-    d->a.n_rows = n_rows; d->a.capacity = capacity;
-    if (int rc = detector_alloc(d, h_stream_ids)) { detector_free(d); return rc; }
-    *out = d;
-    return MWW_OK;
-}
-
-int mww_detector_destroy(mww_detector_t *d) {
-    if (!d) return MWW_OK;
-    DENTER(d);
-    cudaDeviceSynchronize();
-    detector_free(d);
-    return MWW_OK;
-}
-
-int mww_detector_update(mww_detector_t *d, const float *d_probs, int n_steps, long long pitch, void *cu_stream) {
-    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_update: detector is NULL");
-    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_detector_update: a models detector takes mww_multi_detector_update");
-    if (n_steps < 0 || (n_steps > 0 && (!d_probs || pitch < n_steps)))
-        return fail(nullptr, MWW_EINVAL, "mww_detector_update: needs d_probs and n_steps >= 0 columns within the row pitch");
-    if (n_steps == 0) return MWW_OK;
-    DENTER(d);
-    if (d->d_cutoffs) DCU(launch_detector_update_cutoffs(d->a, d->d_cutoffs, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
-    else DCU(launch_detector_update(d->a, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
-    return MWW_OK;
-}
-
-int mww_detector_drain(mww_detector_t *d, mww_event *h_events, int max_events, long long *n_events, void *cu_stream) {
-    if (!d || !n_events || max_events < 0 || (max_events > 0 && !h_events))
-        return fail(nullptr, MWW_EINVAL, "mww_detector_drain: needs a detector, n_events and room for max_events >= 0 events");
-    DENTER(d);
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    unsigned long long count = 0;
-    DCU(cudaMemcpyAsync(&count, d->a.count, sizeof(count), cudaMemcpyDeviceToHost, st));
-    DCU(cudaStreamSynchronize(st));
-    const size_t stored = (size_t)std::min<unsigned long long>(count, (unsigned long long)d->a.capacity);
-    const size_t n = std::min(stored, (size_t)max_events);
-    if (n) DCU(cudaMemcpyAsync(h_events, d->a.events, n * sizeof(mww_event), cudaMemcpyDeviceToHost, st));
-    if (stored) {
-        DCU(cudaMemsetAsync(d->a.count, 0, sizeof(count), st));
-        DCU(cudaMemsetAsync(d->a.fired, 0xFF, stored * sizeof(int32_t), st));
-    }
-    if (n) DCU(cudaStreamSynchronize(st));
-    *n_events = (long long)count;
-    return MWW_OK;
-}
-
-int mww_detector_buffers(mww_detector_t *d, const long long **d_count, const mww_event **d_events, const int32_t **d_fired, int *capacity) {
-    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_buffers: detector is NULL");
-    if (d_count) *d_count = reinterpret_cast<const long long *>(d->a.count);
-    if (d_events) *d_events = d->a.events;
-    if (d_fired) *d_fired = d->a.fired;
-    if (capacity) *capacity = d->a.capacity;
-    return MWW_OK;
-}
-
-int mww_detector_reset_device(mww_detector_t *d, const int32_t *d_rows, int n, void *cu_stream) {
-    if (!d || n < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_reset_device: needs a detector and n >= 0");
-    DENTER(d);
-    if (d->multi) DCU(launch_detector_models_reset(d->m, d_rows, d_rows ? n : d->m.n_streams, static_cast<cudaStream_t>(cu_stream)));
-    else DCU(launch_detector_reset(d->a, d_rows, d_rows ? n : d->a.n_rows, static_cast<cudaStream_t>(cu_stream)));
-    return MWW_OK;
-}
-
-int mww_detector_reset(mww_detector_t *d, const int32_t *h_rows, int n, void *cu_stream) {
-    if (!d || n < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_reset: needs a detector and n >= 0");
-    if (!h_rows) return mww_detector_reset_device(d, nullptr, 0, cu_stream);
-    if (n == 0) return MWW_OK;
-    DENTER(d);
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    if ((size_t)n > d->rows_cap) {                 // growing the staging buffer first waits for the reset that may still read it
-        if (d->d_rows) { DCU(cudaStreamSynchronize(st)); cudaFree(d->d_rows); d->d_rows = nullptr; d->rows_cap = 0; }
-        const size_t want = std::max<size_t>((size_t)n, 1024);
-        DCU(cudaMalloc(&d->d_rows, want * sizeof(int32_t)));
-        d->rows_cap = want;
-    }
-    DCU(cudaMemcpyAsync(d->d_rows, h_rows, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-    if (d->multi) DCU(launch_detector_models_reset(d->m, d->d_rows, n, st));
-    else DCU(launch_detector_reset(d->a, d->d_rows, n, st));
-    return MWW_OK;
-}
-
-int mww_detector_get_state(mww_detector_t *d, float *h_hist, long long *h_seen, int32_t *h_cooldown) {
-    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_get_state: detector is NULL");
-    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_detector_get_state: a models detector takes mww_multi_detector_get_state");
-    DENTER(d);
-    DCU(cudaDeviceSynchronize());
-    const size_t R = (size_t)d->a.n_rows, W = (size_t)d->a.rule.window - 1;
-    if (h_hist && W) {                              // device [window - 1][n_rows] -> host [n_rows][window - 1]
-        std::vector<float> t(W * R);
-        DCU(cudaMemcpy(t.data(), d->a.hist, W * R * sizeof(float), cudaMemcpyDeviceToHost));
-        for (size_t j = 0; j < W; ++j)
-            for (size_t r = 0; r < R; ++r) h_hist[r * W + j] = t[j * R + r];
-    }
-    if (h_seen) DCU(cudaMemcpy(h_seen, d->a.seen, R * sizeof(long long), cudaMemcpyDeviceToHost));
-    if (h_cooldown) DCU(cudaMemcpy(h_cooldown, d->a.cooldown, R * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    return MWW_OK;
-}
-
-int mww_detector_set_state(mww_detector_t *d, const float *h_hist, const long long *h_seen, const int32_t *h_cooldown) {
-    if (!d) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: detector is NULL");
-    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: a models detector takes mww_multi_detector_set_state");
-    const size_t R = (size_t)d->a.n_rows, W = (size_t)d->a.rule.window - 1;
-    for (size_t r = 0; r < R; ++r) {
-        if (h_seen && h_seen[r] < 0) return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: seen must not be negative");
-        if (h_cooldown && (h_cooldown[r] < 0 || h_cooldown[r] > d->a.rule.cooldown_slices))
-            return fail(nullptr, MWW_EINVAL, "mww_detector_set_state: cooldown outside [0, cooldown_slices]");
-    }
-    DENTER(d);
-    DCU(cudaDeviceSynchronize());
-    if (h_hist && W) {
-        std::vector<float> t(W * R);
-        for (size_t j = 0; j < W; ++j)
-            for (size_t r = 0; r < R; ++r) t[j * R + r] = h_hist[r * W + j];
-        DCU(cudaMemcpy(d->a.hist, t.data(), W * R * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    if (h_seen) DCU(cudaMemcpy(d->a.seen, h_seen, R * sizeof(long long), cudaMemcpyHostToDevice));
-    if (h_cooldown) DCU(cudaMemcpy(d->a.cooldown, h_cooldown, R * sizeof(int32_t), cudaMemcpyHostToDevice));
-    return MWW_OK;
-}
-
-int mww_set_detector_cutoffs(mww_detector_t *d, const int32_t *h_rows, const double *h_cutoffs, int n, void *cu_stream) {
-    const std::string call = "mww_set_detector_cutoffs";
-    if (!d) return fail(nullptr, MWW_EINVAL, call + ": detector is NULL");
-    if (d->multi) return fail(nullptr, MWW_EINVAL, call + ": a models detector takes mww_set_multi_detector_cutoffs");
-    if (n < 0) return fail(nullptr, MWW_EINVAL, call + ": n must not be negative");
-    if (n == 0) return MWW_OK;
-    if (!h_rows || !h_cutoffs) return fail(nullptr, MWW_EINVAL, call + ": h_rows and h_cutoffs must not be NULL");
-    const int R = d->a.n_rows;
-    std::vector<int32_t> rows;
-    int lo = 0, hi = 0;
-    if (int rc = check_cutoff_list(call, h_rows, h_cutoffs, n, R, nullptr, R, rows, lo, hi)) return rc;
-    DENTER(d);
-    if (!d->d_cutoffs) {                           // to per-row mode: every row at the create-time cutoff, all copied
-        DCU(cudaMalloc(&d->d_cutoffs, (size_t)R * sizeof(double)));
-        d->cutoffs.assign((size_t)R, d->a.rule.cutoff);
-        lo = 0; hi = R - 1;
-    }
-    for (int i = 0; i < n; ++i) d->cutoffs[rows[i]] = h_cutoffs[i];
-    // from pageable memory: the call returns once the span is staged, so later changes to the host copy cannot reach it
-    DCU(cudaMemcpyAsync(d->d_cutoffs + lo, d->cutoffs.data() + lo, (size_t)(hi - lo + 1) * sizeof(double), cudaMemcpyHostToDevice,
-                        static_cast<cudaStream_t>(cu_stream)));
-    return MWW_OK;
-}
-
-int mww_get_detector_cutoffs(mww_detector_t *d, double *h_cutoffs) {
-    if (!d || !h_cutoffs) return fail(nullptr, MWW_EINVAL, "mww_get_detector_cutoffs: needs a detector and h_cutoffs");
-    if (d->multi) return fail(nullptr, MWW_EINVAL, "mww_get_detector_cutoffs: a models detector takes mww_get_multi_detector_cutoffs");
-    for (int r = 0; r < d->a.n_rows; ++r) h_cutoffs[r] = d->d_cutoffs ? d->cutoffs[r] : d->a.rule.cutoff;
-    return MWW_OK;
-}
-
-}  // extern "C"
-
-// ---- multi-model detector (include/mww.h; rule and kernels: mww_detector_models.h, mww_detector_models.cu) ----------------
-namespace {
-
-int models_fail(const char *what) { return fail(nullptr, MWW_EINVAL, std::string("mww_multi_detector_create: ") + what); }
-
-// device state for the rules the create checked: each used model's rows, its inverse map unless it runs on every stream,
-// the descriptors, and the event buffers the plain detector's calls drain
-int models_alloc(mww_detector_t *d, const std::vector<std::vector<int32_t>> &ids) {
-    DetectModelsArgs &m = d->m;
-    const size_t C = (size_t)d->a.capacity, S = (size_t)m.n_streams;
-    d->member_row.resize((size_t)m.n_models);
-    for (int k = 0; k < m.n_models; ++k) {
-        DetectModel &M = d->models[k];
-        if (M.role == MWW_DETECT_OFF) continue;
-        const size_t R = (size_t)M.n_rows, W = (size_t)M.rule.window - 1;
-        d->member_row[k].assign(S, -1);
-        for (size_t r = 0; r < R; ++r) d->member_row[k][ids[k][r]] = (int32_t)r;
-        DCU(cudaMalloc(&M.hist, std::max<size_t>(W * R, 1) * sizeof(float)));
-        DCU(cudaMalloc(&M.seen, std::max<size_t>(R, 1) * sizeof(long long)));
-        DCU(cudaMalloc(&M.flag, std::max<size_t>(R, 1) * sizeof(int32_t)));
-        if (R != S) {                                   // a stream set is all streams exactly when it has every id
-            std::vector<int32_t> inv(S, -1);
-            for (size_t r = 0; r < R; ++r) inv[ids[k][r]] = (int32_t)r;
-            int32_t *d_inv = nullptr;
-            DCU(cudaMalloc(&d_inv, S * sizeof(int32_t)));
-            M.inv = d_inv;
-            DCU(cudaMemcpy(d_inv, inv.data(), S * sizeof(int32_t), cudaMemcpyHostToDevice));
-        }
-    }
-    DCU(cudaMalloc(&d->d_models, d->models.size() * sizeof(DetectModel)));
-    DCU(cudaMemcpy(d->d_models, d->models.data(), d->models.size() * sizeof(DetectModel), cudaMemcpyHostToDevice));
-    m.models = d->d_models;
-    DCU(cudaMalloc(&d->a.count, sizeof(unsigned long long)));
-    DCU(cudaMalloc(&d->a.events, C * sizeof(mww_event)));
-    DCU(cudaMalloc(&d->a.fired, C * sizeof(int32_t)));
-    m.count = d->a.count; m.events = d->a.events; m.fired = d->a.fired; m.capacity = d->a.capacity;
-    DCU(cudaMemset(d->a.count, 0, sizeof(unsigned long long)));
-    DCU(cudaMemset(d->a.events, 0, C * sizeof(mww_event)));
-    DCU(cudaMemset(d->a.fired, 0xFF, C * sizeof(int32_t)));           // -1 in every slot
-    DCU(launch_detector_models_reset(m, nullptr, m.n_streams, nullptr));
-    DCU(cudaDeviceSynchronize());
-    return MWW_OK;
-}
-
-// model k of a models detector, or a refusal naming the call
-int model_arg(mww_detector_t *d, int k, const char *call, const DetectModel **out) {
-    if (!d) return fail(nullptr, MWW_EINVAL, std::string(call) + ": detector is NULL");
-    if (!d->multi) return fail(nullptr, MWW_EINVAL, std::string(call) + ": not a models detector (mww_multi_detector_create)");
-    if (k < 0 || k >= d->m.n_models) return fail(nullptr, MWW_EINVAL, std::string(call) + ": model index out of range");
-    if (d->models[k].role == MWW_DETECT_OFF) return fail(nullptr, MWW_EINVAL, std::string(call) + ": model is OFF");
-    *out = &d->models[k];
-    return MWW_OK;
-}
-
-// a models detector to per-row mode: every member row of every used model at its model's cutoff, and the descriptors that
-// carry those arrays; on a failure nothing is kept and the detector stays in uniform mode
-int models_to_row_cutoffs(mww_detector_t *d, cudaStream_t st) {
-    const int K = d->m.n_models;
-    std::vector<DetectModelRows> rows((size_t)K);
-    std::vector<std::vector<double>> cut((size_t)K);
-    DetectModelRows *d_rows = nullptr;
-    auto undo = [&](cudaError_t e, const char *what) {
-        for (DetectModelRows &M : rows) cudaFree(const_cast<double *>(M.row_cutoff));
-        cudaFree(d_rows);
-        return cuda_fail(nullptr, e, what);
-    };
-    for (int k = 0; k < K; ++k) {
-        static_cast<DetectModel &>(rows[k]) = d->models[k];
-        const DetectModel &M = d->models[k];
-        if (M.role == MWW_DETECT_OFF || M.n_rows == 0) continue;
-        cut[k].assign((size_t)M.n_rows, M.rule.cutoff);
-        double *p = nullptr;
-        if (cudaError_t e = cudaMalloc(&p, (size_t)M.n_rows * sizeof(double))) return undo(e, "cudaMalloc");
-        rows[k].row_cutoff = p;
-        if (cudaError_t e = cudaMemcpyAsync(p, cut[k].data(), (size_t)M.n_rows * sizeof(double), cudaMemcpyHostToDevice, st)) return undo(e, "cudaMemcpyAsync");
-    }
-    if (cudaError_t e = cudaMalloc(&d_rows, (size_t)K * sizeof(DetectModelRows))) return undo(e, "cudaMalloc");
-    if (cudaError_t e = cudaMemcpyAsync(d_rows, rows.data(), (size_t)K * sizeof(DetectModelRows), cudaMemcpyHostToDevice, st))
-        return undo(e, "cudaMemcpyAsync");
-    d->models_rows = std::move(rows);
-    d->model_cutoffs = std::move(cut);
-    d->d_models_rows = d_rows;
-    return MWW_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
-int mww_multi_detector_create(const mww_t *h, const mww_detect_rule *rules, int capacity, mww_detector_t **out) {
-    if (!out) return models_fail("out is NULL");
-    *out = nullptr;
-    if (!rules) return models_fail("rules is NULL");
-    if (capacity < 1) return models_fail("capacity must be at least 1");
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0)
-        return fail(nullptr, MWW_ECUDA, std::string("no CUDA device available (this library has no CPU fallback): ") + cudaGetErrorString(e));
-    if (!h) return models_fail("handle is NULL");
-    const int K = mww_model_count(h);
-    if (K < 1) return models_fail("the handle is frontend-only: it has no models to detect with");
-    int n_wake = 0, vad = -1;
-    for (int k = 0; k < K; ++k) {
-        const mww_detect_rule &r = rules[k];
-        const std::string at = "model " + std::to_string(k) + ": ";
-        if (r.role != MWW_DETECT_OFF && r.role != MWW_DETECT_WAKE && r.role != MWW_DETECT_VAD)
-            return models_fail((at + "role must be MWW_DETECT_OFF, _WAKE or _VAD").c_str());
-        if (r.role == MWW_DETECT_OFF) continue;
-        if (r.window < 1 || r.window > kDetectorMaxWindow) return models_fail((at + "window must be in [1, 32]").c_str());
-        if (!(r.cutoff - r.cutoff == 0.0)) return models_fail((at + "cutoff must be finite").c_str());
-        if (r.role == MWW_DETECT_WAKE && r.cooldown_slices < 0) return models_fail((at + "cooldown_slices must not be negative").c_str());
-        if (r.role == MWW_DETECT_WAKE) ++n_wake;
-        if (r.role == MWW_DETECT_VAD) {
-            if (vad >= 0) return models_fail("at most one model may be the VAD");
-            vad = k;
-        }
-    }
-    if (n_wake == 0) return models_fail("at least one model must be WAKE");
-    mww_info info;
-    if (mww_get_info(h, &info) != MWW_OK) return models_fail("cannot read the handle");
-    std::vector<std::vector<int32_t>> ids(K);
-    mww_detector_t *d = new mww_detector;
-    d->device = info.device;
-    d->multi = true;
-    d->a.capacity = capacity;
-    d->models.resize(K);
-    DetectModelsArgs &m = d->m;
-    m.n_streams = info.n_streams; m.n_models = K; m.vad = vad;
-    for (int k = 0; k < K; ++k) {
-        const mww_detect_rule &r = rules[k];
-        DetectModel &M = d->models[k];
-        M.role = r.role;
-        if (r.role == MWW_DETECT_OFF) continue;
-        mww_info mi;
-        int n = 0;
-        if (mww_get_model_info(h, k, &mi) != MWW_OK || mww_get_model_streams(h, k, nullptr, 0, &n) != MWW_OK) { delete d; return models_fail("cannot read a model"); }
-        ids[k].resize((size_t)n);
-        if (n > 0 && mww_get_model_streams(h, k, ids[k].data(), n, &n) != MWW_OK) { delete d; return models_fail("cannot read a stream set"); }
-        M.rule.window = r.window; M.rule.cutoff = r.cutoff; M.rule.cooldown_slices = r.role == MWW_DETECT_WAKE ? r.cooldown_slices : 0;
-        M.stride = std::max(mi.input_feature_slices, 1);
-        M.n_rows = n;
-        if (r.role == MWW_DETECT_WAKE) m.wake[m.n_wake++] = (int8_t)k;
-    }
-    DeviceGuard guard(d->device);
-    if (guard.err != cudaSuccess) { delete d; return cuda_fail(nullptr, guard.err, "cudaSetDevice"); }
-    if (int rc = models_alloc(d, ids)) { detector_free(d); return rc; }
-    *out = d;
-    return MWW_OK;
-}
-
-int mww_multi_detector_update(mww_detector_t *d, const float *const *d_probs, const long long *pitch, const int *n_steps,
-                               const int *pending_before, void *cu_stream) {
-    if (!d) return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: detector is NULL");
-    if (!d->multi) return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: not a models detector (mww_multi_detector_create)");
-    if (!d_probs || !pitch || !n_steps || !pending_before)
-        return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: d_probs, pitch, n_steps and pending_before must not be NULL");
-    DetectModelsArgs &m = d->m;
-    DetectCall call[kDetectMaxModels];
-    bool any = false;
-    for (int k = 0; k < m.n_models; ++k) {
-        const DetectModel &M = d->models[k];
-        if (M.role == MWW_DETECT_OFF) continue;
-        DetectCall &c = call[k];
-        c.probs = d_probs[k]; c.pitch = pitch[k]; c.n_steps = n_steps[k]; c.pending = pending_before[k];
-        if (c.n_steps > 0 && M.n_rows > 0) {
-            if (!c.probs || c.pitch < c.n_steps)
-                return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: model " + std::to_string(k) +
-                                                     " needs d_probs and n_steps columns within the row pitch");
-            any = true;
-        }
-    }
-    if (!detect_call_fits(d->models.data(), call, m.n_models))
-        return fail(nullptr, MWW_EINVAL, "mww_multi_detector_update: the step counts and pending rows do not describe one call "
-                                         "(n_k = (p_k + R) div s_k with 0 <= p_k < s_k for one R >= 0)");
-    if (!any) return MWW_OK;
-    DENTER(d);
-    for (int k = 0; k < m.n_models; ++k) m.call[k] = call[k];
-    if (d->d_models_rows) DCU(launch_detector_models_update_cutoffs(detect_args_rows(m, d->d_models_rows), static_cast<cudaStream_t>(cu_stream)));
-    else DCU(launch_detector_models_update(m, static_cast<cudaStream_t>(cu_stream)));
-    return MWW_OK;
-}
-
-int mww_multi_detector_get_state(mww_detector_t *d, int k, float *h_hist, long long *h_seen, int32_t *h_cooldown_or_active) {
-    const DetectModel *M = nullptr;
-    if (int rc = model_arg(d, k, "mww_multi_detector_get_state", &M)) return rc;
-    DENTER(d);
-    DCU(cudaDeviceSynchronize());
-    const size_t R = (size_t)M->n_rows, W = (size_t)M->rule.window - 1;
-    if (R == 0) return MWW_OK;
-    if (h_hist && W) {                              // device [window - 1][n_k] -> host [n_k][window - 1]
-        std::vector<float> t(W * R);
-        DCU(cudaMemcpy(t.data(), M->hist, W * R * sizeof(float), cudaMemcpyDeviceToHost));
-        for (size_t j = 0; j < W; ++j)
-            for (size_t r = 0; r < R; ++r) h_hist[r * W + j] = t[j * R + r];
-    }
-    if (h_seen) DCU(cudaMemcpy(h_seen, M->seen, R * sizeof(long long), cudaMemcpyDeviceToHost));
-    if (h_cooldown_or_active) DCU(cudaMemcpy(h_cooldown_or_active, M->flag, R * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    return MWW_OK;
-}
-
-int mww_multi_detector_set_state(mww_detector_t *d, int k, const float *h_hist, const long long *h_seen, const int32_t *h_cooldown_or_active) {
-    const DetectModel *M = nullptr;
-    if (int rc = model_arg(d, k, "mww_multi_detector_set_state", &M)) return rc;
-    const size_t R = (size_t)M->n_rows, W = (size_t)M->rule.window - 1;
-    const int hi = M->role == MWW_DETECT_WAKE ? M->rule.cooldown_slices : 1;
-    for (size_t r = 0; r < R; ++r) {
-        if (h_seen && h_seen[r] < 0) return fail(nullptr, MWW_EINVAL, "mww_multi_detector_set_state: seen must not be negative");
-        if (h_cooldown_or_active && (h_cooldown_or_active[r] < 0 || h_cooldown_or_active[r] > hi))
-            return fail(nullptr, MWW_EINVAL, M->role == MWW_DETECT_WAKE ? "mww_multi_detector_set_state: cooldown outside [0, cooldown_slices]"
-                                                                        : "mww_multi_detector_set_state: active must be 0 or 1");
-    }
-    DENTER(d);
-    DCU(cudaDeviceSynchronize());
-    if (R == 0) return MWW_OK;
-    if (h_hist && W) {
-        std::vector<float> t(W * R);
-        for (size_t j = 0; j < W; ++j)
-            for (size_t r = 0; r < R; ++r) t[j * R + r] = h_hist[r * W + j];
-        DCU(cudaMemcpy(M->hist, t.data(), W * R * sizeof(float), cudaMemcpyHostToDevice));
-    }
-    if (h_seen) DCU(cudaMemcpy(M->seen, h_seen, R * sizeof(long long), cudaMemcpyHostToDevice));
-    if (h_cooldown_or_active) DCU(cudaMemcpy(M->flag, h_cooldown_or_active, R * sizeof(int32_t), cudaMemcpyHostToDevice));
-    return MWW_OK;
-}
-
-int mww_set_multi_detector_cutoffs(mww_detector_t *d, int k, const int32_t *h_stream_ids, const double *h_cutoffs, int n, void *cu_stream) {
-    const std::string call = "mww_set_multi_detector_cutoffs";
-    const DetectModel *M = nullptr;
-    if (int rc = model_arg(d, k, call.c_str(), &M)) return rc;
-    if (n < 0) return fail(nullptr, MWW_EINVAL, call + ": n must not be negative");
-    if (n == 0) return MWW_OK;
-    if (!h_stream_ids || !h_cutoffs) return fail(nullptr, MWW_EINVAL, call + ": h_stream_ids and h_cutoffs must not be NULL");
-    std::vector<int32_t> rows;
-    int lo = 0, hi = 0;
-    if (int rc = check_cutoff_list(call, h_stream_ids, h_cutoffs, n, d->m.n_streams, d->member_row[k].data(), M->n_rows, rows, lo, hi)) return rc;
-    DENTER(d);
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    if (!d->d_models_rows) {
-        if (int rc = models_to_row_cutoffs(d, st)) return rc;
-        lo = 0; hi = M->n_rows - 1;
-    }
-    std::vector<double> &c = d->model_cutoffs[k];
-    for (int i = 0; i < n; ++i) c[rows[i]] = h_cutoffs[i];
-    // from pageable memory: the call returns once the span is staged, so later changes to the host copy cannot reach it
-    DCU(cudaMemcpyAsync(const_cast<double *>(d->models_rows[k].row_cutoff) + lo, c.data() + lo, (size_t)(hi - lo + 1) * sizeof(double),
-                        cudaMemcpyHostToDevice, st));
-    return MWW_OK;
-}
-
-int mww_get_multi_detector_cutoffs(mww_detector_t *d, int k, double *h_cutoffs) {
-    const DetectModel *M = nullptr;
-    if (int rc = model_arg(d, k, "mww_get_multi_detector_cutoffs", &M)) return rc;
-    if (!h_cutoffs && M->n_rows > 0) return fail(nullptr, MWW_EINVAL, "mww_get_multi_detector_cutoffs: h_cutoffs is NULL");
-    for (int r = 0; r < M->n_rows; ++r) h_cutoffs[r] = d->d_models_rows ? d->model_cutoffs[k][r] : M->rule.cutoff;
-    return MWW_OK;
 }
 
 }  // extern "C"

@@ -1,0 +1,30 @@
+// mww_capi.h -- what the two C-ABI translation units share: mww_capi.cu (the handle) and mww_detector_capi.cu (the
+// streaming detectors).  Host code only.
+#pragma once
+
+#include <cuda_runtime.h>
+
+#include <string>
+
+#include "../../include/mww.h"
+
+namespace mww {
+
+// a refusal or failure: msg goes to the handle (mww_last_error(h)) or, for h == nullptr, to the calling thread's error of
+// the last call without a handle (mww_last_error(NULL): a failed create, the detectors); returns code
+int fail(mww_t *h, int code, const std::string &msg);
+// MWW_ECUDA with "what: <CUDA error>"
+int cuda_fail(mww_t *h, cudaError_t e, const char *what);
+
+// every entry point runs with the handle's device current and puts the caller's device back on return (a process that
+// holds engines on several GPUs, or torch's current device, is not disturbed)
+struct DeviceGuard {
+    int prev = -1; bool switched = false; cudaError_t err = cudaSuccess;
+    explicit DeviceGuard(int device) {
+        if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
+        if (prev != device) { err = cudaSetDevice(device); switched = err == cudaSuccess && prev >= 0; }
+    }
+    ~DeviceGuard() { if (switched) cudaSetDevice(prev); }
+};
+
+}  // namespace mww

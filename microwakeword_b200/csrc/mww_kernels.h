@@ -1,4 +1,4 @@
-// mww_kernels.h -- launcher prototypes shared by the C-ABI layer (mww_capi.cu) and the kernel files.
+// mww_kernels.h -- launcher prototypes shared by the C-ABI layer (mww_capi.cu, mww_detector_capi.cu) and the kernel files.
 #pragma once
 
 #include <cuda_runtime.h>

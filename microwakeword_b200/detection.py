@@ -260,7 +260,64 @@ class _DeviceArray:
         self.__cuda_array_interface__ = dict(shape=(n,), typestr=typestr, data=(ptr, False), version=2, strides=None)
 
 
-class StreamDetector:
+class _Detector:
+    """what both detectors share: ownership of one mww_detector_t, its device views, drain and the reset dispatch"""
+
+    def _own(self, rc: int, d, device: int, capacity: int) -> None:
+        """take the detector a create call returned (rc, d) and make the views of its event buffers"""
+        self._check(rc)
+        self._handle = _DetectorHandle(self._L, d)
+        self.device, self.capacity = int(device), int(capacity)
+        count, fired = ctypes.c_void_p(), ctypes.c_void_p()
+        self._check(self._L.mww_detector_buffers(self._d, ctypes.byref(count), None, ctypes.byref(fired), None))
+        import torch
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(dev):
+            # device views: the stream of every event since the last drain (-1 in unused slots), and how many fired
+            self.fired_ids = torch.as_tensor(_DeviceArray(self._handle, fired.value, self.capacity, "<i4"), device=dev)
+            self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
+
+    def _check(self, rc: int) -> None:
+        if rc != 0:
+            msg = self._L.mww_last_error(None)
+            raise _lib.MwwError(rc, msg.decode() if msg else "detector call failed")
+
+    @property
+    def _d(self):
+        return self._handle.ptr
+
+    def _cuda_stream(self):
+        import torch
+        return _stream(torch.device("cuda", self.device))
+
+    def close(self):
+        """free the detector now; fired_ids and event_count must not be used afterwards"""
+        self._handle.close()
+
+    def _drain(self, dtype, keys):
+        """(events since the last drain as `dtype`, sorted by `keys`, most significant first; events dropped)"""
+        buf = np.empty(self.capacity, dtype)
+        n = ctypes.c_longlong(0)
+        self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
+        ev = buf[:min(n.value, self.capacity)]
+        return ev[np.lexsort(tuple(ev[k] for k in reversed(keys)))], max(n.value - self.capacity, 0)
+
+    def _reset(self, ids, what: str) -> None:
+        """reset all rows (None), or the ids of a contiguous 1-D CUDA int32 tensor or of a host sequence"""
+        import torch
+        st = self._cuda_stream()
+        if ids is None:
+            self._check(self._L.mww_detector_reset(self._d, None, 0, st))
+        elif isinstance(ids, torch.Tensor) and ids.is_cuda:
+            if ids.dtype != torch.int32 or ids.dim() != 1 or not ids.is_contiguous():
+                raise ValueError("device %s must be a contiguous 1-D CUDA int32 tensor" % what)
+            self._check(self._L.mww_detector_reset_device(self._d, ids.data_ptr(), ids.numel(), st))
+        else:
+            r = np.ascontiguousarray(ids, np.int32).reshape(-1)
+            self._check(self._L.mww_detector_reset(self._d, r.ctypes.data, r.size, st))
+
+
+class StreamDetector(_Detector):
     """The detection rule of the reference's evaluation (moving average of `window` probabilities above `cutoff`, then
     `cooldown_slices` steps of silence; test.py:337-341, :118-135) for `n_rows` live streams, state carried across calls
     (mww_detector_* of include/mww.h).  A row's events over any sequence of update calls are those of false_accept_counts on
@@ -287,31 +344,8 @@ class StreamDetector:
                 raise ValueError("stream_ids must name one stream per row")
         rc = self._L.mww_detector_create(int(device), int(n_rows), int(window), float(cutoff), int(cooldown_slices), int(capacity),
                                          ids.ctypes.data if ids is not None else None, ctypes.byref(d))
-        self._check(rc)
-        self._handle = _DetectorHandle(self._L, d)
+        self._own(rc, d, device, capacity)
         self.n_rows, self.window, self.cutoff, self.cooldown_slices = int(n_rows), int(window), float(cutoff), int(cooldown_slices)
-        self.capacity, self.device = int(capacity), int(device)
-        count, events, fired = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
-        self._check(self._L.mww_detector_buffers(self._d, ctypes.byref(count), ctypes.byref(events), ctypes.byref(fired), None))
-        import torch
-        dev = torch.device("cuda", self.device)
-        with torch.cuda.device(dev):
-            # device views: the stream of every event since the last drain (-1 in unused slots), and how many fired
-            self.fired_ids = torch.as_tensor(_DeviceArray(self._handle, fired.value, self.capacity, "<i4"), device=dev)
-            self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
-
-    def _check(self, rc: int) -> None:
-        if rc != 0:
-            msg = self._L.mww_last_error(None)
-            raise _lib.MwwError(rc, msg.decode() if msg else "detector call failed")
-
-    @property
-    def _d(self):
-        return self._handle.ptr
-
-    def close(self):
-        """free the detector now; fired_ids and event_count must not be used afterwards"""
-        self._handle.close()
 
     def update(self, probs) -> None:
         """CUDA float32 [n_rows, steps], any row pitch (a slice of a wider buffer is read in place); zero columns: nothing
@@ -332,27 +366,12 @@ class StreamDetector:
         """-> (events, dropped): the events since the last drain as a structured array (EVENT_DTYPE) sorted by (step, stream),
         and how many more fired than `capacity` could hold.  Waits for the current CUDA stream; clears the event buffer and
         fired_ids."""
-        import torch
-        buf = np.empty(self.capacity, EVENT_DTYPE)
-        n = ctypes.c_longlong(0)
-        self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), _stream(torch.device("cuda", self.device))))
-        ev = buf[:min(n.value, self.capacity)]
-        return ev[np.lexsort((ev["stream"], ev["step"]))], max(n.value - self.capacity, 0)
+        return self._drain(EVENT_DTYPE, ("step", "stream"))
 
     def reset(self, rows=None) -> None:
         """Fresh detector state (warm-up and cooldown start again) for all rows (None) or the given ROW indices: a host
         sequence, or a contiguous 1-D CUDA int32 tensor.  Indices out of range are ignored."""
-        import torch
-        st = _stream(torch.device("cuda", self.device))
-        if rows is None:
-            self._check(self._L.mww_detector_reset(self._d, None, 0, st))
-        elif isinstance(rows, torch.Tensor) and rows.is_cuda:
-            if rows.dtype != torch.int32 or rows.dim() != 1 or not rows.is_contiguous():
-                raise ValueError("device row indices must be a contiguous 1-D CUDA int32 tensor")
-            self._check(self._L.mww_detector_reset_device(self._d, rows.data_ptr(), rows.numel(), st))
-        else:
-            r = np.ascontiguousarray(rows, np.int32).reshape(-1)
-            self._check(self._L.mww_detector_reset(self._d, r.ctypes.data, r.size, st))
+        self._reset(rows, "row indices")
 
     def state_dict(self) -> dict:
         d = dict(hist=np.zeros((self.n_rows, self.window - 1), np.float32), seen=np.zeros(self.n_rows, np.int64),
@@ -374,9 +393,8 @@ class StreamDetector:
         The first call switches the detector to per-row mode, every other row keeping the create-time cutoff.  Ordered on
         the current CUDA stream: updates made before it use the old cutoffs, updates after it the new ones.  The state and
         resets are unaffected."""
-        import torch
         r, c = _cutoff_list(rows, cutoffs, "rows")
-        self._check(self._L.mww_set_detector_cutoffs(self._d, r.ctypes.data, c.ctypes.data, r.size, _stream(torch.device("cuda", self.device))))
+        self._check(self._L.mww_set_detector_cutoffs(self._d, r.ctypes.data, c.ctypes.data, r.size, self._cuda_stream()))
 
     @property
     def cutoffs(self) -> np.ndarray:
@@ -418,7 +436,7 @@ def _per_model(value, K, name):
     return v
 
 
-class MultiModelDetector:
+class MultiModelDetector(_Detector):
     """One detector over the K models of a MultiModelEngine (mww_multi_detector_create of include/mww.h): each model WAKE
     (the StreamDetector rule), the VAD or OFF, every model's probabilities of a call in one launch, one event stream.  A WAKE
     model fires only on streams whose VAD row is active (the VAD's moving average above its cutoff); without a VAD each
@@ -451,9 +469,8 @@ class MultiModelDetector:
             rules[k] = _lib.MwwDetectRule(role, int(windows[k]), int(cooldowns[k]), 0, 0.0 if cutoffs[k] is None else float(cutoffs[k]))
         self._L = _lib.lib()
         d = ctypes.c_void_p()
-        self._check(self._L.mww_multi_detector_create(engine._h, rules, int(capacity), ctypes.byref(d)))
-        self._handle = _DetectorHandle(self._L, d)
-        self.engine, self.n_models, self.device, self.capacity = engine, K, int(engine.device), int(capacity)
+        self._own(self._L.mww_multi_detector_create(engine._h, rules, int(capacity), ctypes.byref(d)), d, engine.device, capacity)
+        self.engine, self.n_models = engine, K
         self.roles = [r.role for r in rules]
         self.vad = None if vad is None else int(vad)
         self.windows = [int(w) for w in windows]
@@ -461,27 +478,6 @@ class MultiModelDetector:
         self.cooldown_slices = [int(c) for c in cooldowns]
         self.streams = [s.copy() for s in engine.streams]
         self._pending = list(engine.pending_rows)
-        count, fired = ctypes.c_void_p(), ctypes.c_void_p()
-        self._check(self._L.mww_detector_buffers(self._d, ctypes.byref(count), None, ctypes.byref(fired), None))
-        import torch
-        dev = torch.device("cuda", self.device)
-        with torch.cuda.device(dev):
-            # device views: the global stream of every event since the last drain (-1 in unused slots), and how many fired
-            self.fired_ids = torch.as_tensor(_DeviceArray(self._handle, fired.value, self.capacity, "<i4"), device=dev)
-            self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
-
-    def _check(self, rc: int) -> None:
-        if rc != 0:
-            msg = self._L.mww_last_error(None)
-            raise _lib.MwwError(rc, msg.decode() if msg else "detector call failed")
-
-    @property
-    def _d(self):
-        return self._handle.ptr
-
-    def close(self):
-        """free the detector now; fired_ids and event_count must not be used afterwards"""
-        self._handle.close()
 
     @property
     def pending_rows(self) -> list:
@@ -514,36 +510,22 @@ class MultiModelDetector:
             pitch[k] = p.stride(0) if rows > 1 else n
             steps[k] = n
         pend = (ctypes.c_int * K)(*self._pending)
-        self._check(self._L.mww_multi_detector_update(self._d, ptrs, pitch, steps, pend, _stream(torch.device("cuda", self.device))))
+        self._check(self._L.mww_multi_detector_update(self._d, ptrs, pitch, steps, pend, self._cuda_stream()))
         self._pending = list(self.engine.pending_rows)
 
     def drain(self):
         """-> (events, dropped): the events since the last drain (MODEL_EVENT_DTYPE, global stream ids) sorted by (model, step,
         stream), and how many more fired than `capacity` could hold.  Waits for the current CUDA stream; clears the event
         buffer and fired_ids."""
-        import torch
-        buf = np.empty(self.capacity, MODEL_EVENT_DTYPE)
-        n = ctypes.c_longlong(0)
-        self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), _stream(torch.device("cuda", self.device))))
-        ev = buf[:min(n.value, self.capacity)]
-        return ev[np.lexsort((ev["stream"], ev["step"], ev["model"]))], max(n.value - self.capacity, 0)
+        return self._drain(MODEL_EVENT_DTYPE, ("model", "step", "stream"))
 
     def reset(self, stream_ids=None) -> None:
         """Fresh detector state of every model for all streams (None; the engine's pending rows are read again, so this is
         the call to make after engine.reset()) or the given GLOBAL stream ids: a host sequence, or a contiguous 1-D CUDA
         int32 tensor such as fired_ids.  Ids out of range are ignored."""
-        import torch
-        st = _stream(torch.device("cuda", self.device))
+        self._reset(stream_ids, "stream ids")
         if stream_ids is None:
-            self._check(self._L.mww_detector_reset(self._d, None, 0, st))
             self._pending = list(self.engine.pending_rows)
-        elif isinstance(stream_ids, torch.Tensor) and stream_ids.is_cuda:
-            if stream_ids.dtype != torch.int32 or stream_ids.dim() != 1 or not stream_ids.is_contiguous():
-                raise ValueError("device stream ids must be a contiguous 1-D CUDA int32 tensor")
-            self._check(self._L.mww_detector_reset_device(self._d, stream_ids.data_ptr(), stream_ids.numel(), st))
-        else:
-            ids = np.ascontiguousarray(stream_ids, np.int32).reshape(-1)
-            self._check(self._L.mww_detector_reset(self._d, ids.ctypes.data, ids.size, st))
 
     def _used_model(self, k) -> int:
         if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 0 <= int(k) < self.n_models:
@@ -557,11 +539,9 @@ class MultiModelDetector:
         (mww_set_multi_detector_cutoffs): `cutoffs` is one value or one per stream.  The first call switches every model to
         per-row mode, every other row keeping its model's cutoff.  Ordered on the current CUDA stream; the state and resets
         are unaffected."""
-        import torch
         k = self._used_model(k)
         ids, c = _cutoff_list(stream_ids, cutoffs, "stream_ids")
-        self._check(self._L.mww_set_multi_detector_cutoffs(self._d, k, ids.ctypes.data, c.ctypes.data, ids.size,
-                                                           _stream(torch.device("cuda", self.device))))
+        self._check(self._L.mww_set_multi_detector_cutoffs(self._d, k, ids.ctypes.data, c.ctypes.data, ids.size, self._cuda_stream()))
 
     def get_cutoffs(self, k: int) -> np.ndarray:
         """float64 [members of model k]: each row's cutoff in the order of streams[k]"""
