@@ -723,6 +723,56 @@ int mww_set_multi_detector_cutoffs(mww_detector_t *d, int k, const int32_t *h_st
                                    void *cu_stream);
 int mww_get_multi_detector_cutoffs(mww_detector_t *d, int k, double *h_cutoffs /* [n_k], list order */);
 
+/* ---- moving detector rows: export and import as packed records ---------------------------------------------------------
+ * A server that grows, compacts or rebalances a handle moves its streams as stream records (mww_export_streams); their
+ * detector rows move the same way, so that a moved stream keeps its moving average, its warm-up count, its cooldown and
+ * its VAD flag.  The same calls carry the rows of every stream that stays when a new models detector replaces one after
+ * mww_set_model_streams, and checkpoint some streams' rows.
+ *   - Rows and ids.  A plain detector is addressed by ROW index in [0, n_rows), as mww_detector_reset is; a models detector
+ *     by GLOBAL stream id in [0, n_streams) of the handle it was created from, as its reset is.  For the records a plain
+ *     detector is a models detector with one WAKE model whose stream set is every row: its mask bit 0 is always set.
+ *   - One record, record_bytes long (a multiple of 16), every part padded to 16 bytes:
+ *         uint64  member_mask                 bit k: the stream is a member of model k and slot k holds its state
+ *         for each model k whose role is not OFF, in order:
+ *             float32 hist[window_k - 1]      oldest first (no bytes when window_k = 1)
+ *             int64 seen; int32 flag; int32 0 flag = cooldown (WAKE) or active (VAD), as get_state reports them
+ *     A plain detector of window 5 has 48-byte records.
+ *   - mww_detector_layout: record_bytes, whether the detector is a models detector (multi), its model count and each
+ *     model's role, window and cooldown_slices (0 for an OFF model and for the VAD).  mww_get_detector_layout fills it and
+ *     does no device work; export fills it too (out may be NULL); import checks it and refuses (MWW_EINVAL) records whose
+ *     layout differs from its own in multi, n_models, a model's role, a used model's window, a WAKE model's cooldown or
+ *     record_bytes -- the message names the first such field.  A VAD's cooldown is not compared.
+ *   - export writes one record per listed id (an id may appear twice).  For a model the stream is not a member of, the
+ *     mask bit is clear and the slot is zero.  The detector does not change.
+ *   - import, per used model k: a destination stream that is not a member of model k ignores slot k; a member whose
+ *     record bit is set takes the slot's state; a member whose bit is clear gets fresh state, what a reset gives (zero
+ *     hist, seen 0, cooldown = cooldown_k for WAKE, active 0 for VAD).  Every byte of a row that is not listed stays
+ *     untouched.
+ *   - What does not move: the event buffer, its counter and d_fired, which belong to the detector that produced them (drain
+ *     before moving); the plain detector's stream map, because events report the destination's; the cutoffs, which are
+ *     configuration the caller keeps (mww_get_detector_cutoffs / mww_set_detector_cutoffs move them).
+ *   - Continuation.  A moved row that is then given the same probabilities -- for a models detector, updates with the same
+ *     n_k and p_k -- produces the same events and the same state as the source row would have, bit for bit: the same
+ *     model, step and score, with stream from the destination's map or id.  This holds in both kernel forms, and in uniform
+ *     and per-row mode whenever the cutoffs are equal.
+ *   - Both calls take host id lists and device records [n][record_bytes], 16-byte aligned, in memory the detector's GPU
+ *     can address.  They are asynchronous and ordered on cu_stream, with no synchronisation: an update enqueued before an
+ *     export is included in what it reads.  One launch per call whatever n is; n == 0 launches nothing and still fills /
+ *     checks the layout.  The id list is staged in a buffer the detector owns (as mww_detector_reset's is), so calls on
+ *     one detector from different CUDA streams must be ordered by the caller.
+ *   - MWW_EINVAL before any device work, with the detector unchanged: a NULL detector or layout, n < 0, a NULL or
+ *     misaligned d_records with n > 0, an id out of range, an id listed twice on import. */
+typedef struct mww_detector_layout {
+    int64_t record_bytes;
+    int32_t multi, n_models;
+    int32_t role[64], window[64], cooldown_slices[64];
+} mww_detector_layout;
+int mww_get_detector_layout(const mww_detector_t *d, mww_detector_layout *out);
+int mww_export_detector_rows(mww_detector_t *d, const int32_t *h_ids, int n, void *d_records, mww_detector_layout *out,
+                             void *cu_stream);
+int mww_import_detector_rows(mww_detector_t *d, const int32_t *h_ids, int n, const void *d_records,
+                             const mww_detector_layout *layout, void *cu_stream);
+
 #ifdef __cplusplus
 }
 #endif

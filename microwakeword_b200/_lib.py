@@ -40,6 +40,7 @@ EXPORTS = (
     "mww_features_g711", "mww_predict_clip_g711", "mww_predict_clip_host_g711", "mww_predict_clip_remote_g711",
     "mww_predict_clip_multi_g711", "mww_predict_clip_host_multi_g711", "mww_predict_clip_remote_multi_g711",
     "mww_set_audio_history", "mww_get_audio_history", "mww_read_audio_history", "mww_read_audio_history_device_ids",
+    "mww_get_detector_layout", "mww_export_detector_rows", "mww_import_detector_rows",
 )
 
 
@@ -77,6 +78,14 @@ class MwwDetectRule(ctypes.Structure):
     """mww_detect_rule of include/mww.h: one model's rule in a models detector"""
     _fields_ = [("role", ctypes.c_int32), ("window", ctypes.c_int32), ("cooldown_slices", ctypes.c_int32), ("pad", ctypes.c_int32),
                 ("cutoff", ctypes.c_double)]
+
+
+class MwwDetectorLayout(ctypes.Structure):
+    """mww_detector_layout of include/mww.h: what travels beside exported detector records"""
+    _fields_ = [
+        ("record_bytes", ctypes.c_int64), ("multi", ctypes.c_int32), ("n_models", ctypes.c_int32),
+        ("role", ctypes.c_int32 * 64), ("window", ctypes.c_int32 * 64), ("cooldown_slices", ctypes.c_int32 * 64),
+    ]
 
 
 class MwwError(RuntimeError):
@@ -263,6 +272,11 @@ def lib() -> ctypes.CDLL:
     for name in ("mww_read_audio_history", "mww_read_audio_history_device_ids"):
         getattr(L, name).restype = i32
         getattr(L, name).argtypes = [vp, vp, i32, i32, vp, ll, vp]
+    L.mww_get_detector_layout.restype = i32
+    L.mww_get_detector_layout.argtypes = [vp, ctypes.POINTER(MwwDetectorLayout)]
+    for name in ("mww_export_detector_rows", "mww_import_detector_rows"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwDetectorLayout), vp]
     _lib = L
     return L
 

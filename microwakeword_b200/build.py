@@ -36,6 +36,10 @@ G711_SOURCES = ["mww_frontend_g711.cu"]
 # and the audio history's kernels (mww_set_audio_history), so that a handle without a history runs exactly the kernels it ran
 HIST_OUT = os.path.join(HERE, "libmww_history.so")
 HIST_SOURCES = ["mww_history.cu"]
+# and the detector records' kernels (mww_export_detector_rows / mww_import_detector_rows), so that libmww_b200.so and the three
+# detector libraries keep exactly the kernels they had
+DR_OUT = os.path.join(HERE, "libmww_detector_records.so")
+DR_SOURCES = ["mww_detector_records.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -58,7 +62,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -78,9 +82,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
             return OUT
         for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (RR_OUT, RR_SOURCES, []), (DET_OUT, DET_SOURCES, []),
                                     (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []), (G711_OUT, G711_SOURCES, []),
-                                    (HIST_OUT, HIST_SOURCES, []),
+                                    (HIST_OUT, HIST_SOURCES, []), (DR_OUT, DR_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
                                                     "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711", "-lmww_history",
+                                                    "-lmww_detector_records",
                                                     "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra

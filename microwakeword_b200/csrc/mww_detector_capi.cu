@@ -243,6 +243,60 @@ void get_cutoffs(const mww_detector_t *d, const RowSet &s, double *h_cutoffs) {
     for (int r = 0; r < s.n_rows; ++r) h_cutoffs[r] = d->per_row ? s.cutoffs[r] : s.rule.cutoff;
 }
 
+// n ids from host memory into the staging buffer d_rows, on st; growing the buffer first waits for the call that may still
+// read it
+int stage_ids(mww_detector_t *d, const int32_t *h_ids, int n, cudaStream_t st) {
+    if ((size_t)n > d->rows_cap) {
+        if (d->d_rows) { DCU(cudaStreamSynchronize(st)); cudaFree(d->d_rows); d->d_rows = nullptr; d->rows_cap = 0; }
+        const size_t want = std::max<size_t>((size_t)n, 1024);
+        DCU(cudaMalloc(&d->d_rows, want * sizeof(int32_t)));
+        d->rows_cap = want;
+    }
+    DCU(cudaMemcpyAsync(d->d_rows, h_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return MWW_OK;
+}
+
+// ---- detector records: each row set is one model of the record (the plain detector's one WAKE model, row = id)
+void fill_layout(const mww_detector_t *d, mww_detector_layout *o) {
+    *o = mww_detector_layout{};
+    o->multi = d->multi ? 1 : 0;
+    o->n_models = (int32_t)d->sets.size();
+    for (size_t k = 0; k < d->sets.size(); ++k) {
+        const RowSet &s = d->sets[k];
+        o->role[k] = s.role;
+        if (s.role == MWW_DETECT_OFF) continue;
+        o->window[k] = s.rule.window;
+        o->cooldown_slices[k] = s.role == MWW_DETECT_WAKE ? s.rule.cooldown_slices : 0;
+    }
+    const std::vector<DetectModel> models(d->sets.begin(), d->sets.end());
+    o->record_bytes = detector_record_layout(models.data(), o->n_models).record_bytes;
+}
+
+DetRecJob record_job(const mww_detector_t *d) {
+    const std::vector<DetectModel> models(d->sets.begin(), d->sets.end());
+    return detector_record_job(models.data(), (int)models.size());
+}
+
+// the checks both calls make before any device work: n, the records buffer, ids in range (rows of a plain detector,
+// global stream ids of a models detector) and, on import, listed once
+int check_rows(const mww_detector_t *d, const std::string &call, const int32_t *h_ids, int n, const void *d_records, bool once) {
+    if (n < 0) return refuse(call + ": n must not be negative");
+    if (n == 0) return MWW_OK;
+    if (!h_ids) return refuse(call + ": h_ids is NULL");
+    if (!d_records || reinterpret_cast<uintptr_t>(d_records) % 16) return refuse(call + ": d_records must be a 16-byte aligned device buffer");
+    const int n_ids = d->multi ? d->m.n_streams : d->sets[0].n_rows;
+    std::vector<char> listed(once ? (size_t)n_ids : 0, 0);
+    for (int i = 0; i < n; ++i) {
+        const int32_t id = h_ids[i];
+        if (id < 0 || id >= n_ids) return refuse(call + ": id " + std::to_string(id) + " out of range");
+        if (once) {
+            if (listed[id]) return refuse(call + ": id " + std::to_string(id) + " listed twice");
+            listed[id] = 1;
+        }
+    }
+    return MWW_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -298,14 +352,47 @@ int mww_detector_reset(mww_detector_t *d, const int32_t *h_rows, int n, void *cu
     if (n == 0) return MWW_OK;
     DENTER(d);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    if ((size_t)n > d->rows_cap) {                 // growing the staging buffer first waits for the reset that may still read it
-        if (d->d_rows) { DCU(cudaStreamSynchronize(st)); cudaFree(d->d_rows); d->d_rows = nullptr; d->rows_cap = 0; }
-        const size_t want = std::max<size_t>((size_t)n, 1024);
-        DCU(cudaMalloc(&d->d_rows, want * sizeof(int32_t)));
-        d->rows_cap = want;
-    }
-    DCU(cudaMemcpyAsync(d->d_rows, h_rows, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    if (int rc = stage_ids(d, h_rows, n, st)) return rc;
     DCU(reset_rows(d, d->d_rows, n, st));
+    return MWW_OK;
+}
+
+// ---- detector records, both kinds
+int mww_get_detector_layout(const mww_detector_t *d, mww_detector_layout *out) {
+    if (!d || !out) return refuse("mww_get_detector_layout: needs a detector and out");
+    fill_layout(d, out);
+    return MWW_OK;
+}
+
+int mww_export_detector_rows(mww_detector_t *d, const int32_t *h_ids, int n, void *d_records, mww_detector_layout *out, void *cu_stream) {
+    const std::string call = "mww_export_detector_rows";
+    if (!d) return refuse(call + ": detector is NULL");
+    if (int rc = check_rows(d, call, h_ids, n, d_records, false)) return rc;
+    if (out) fill_layout(d, out);
+    if (n == 0) return MWW_OK;
+    DENTER(d);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = stage_ids(d, h_ids, n, st)) return rc;
+    DCU(launch_pack_detector_rows(record_job(d), d_records, d->d_rows, n, st));
+    return MWW_OK;
+}
+
+int mww_import_detector_rows(mww_detector_t *d, const int32_t *h_ids, int n, const void *d_records, const mww_detector_layout *layout,
+                             void *cu_stream) {
+    const std::string call = "mww_import_detector_rows";
+    if (!d || !layout) return refuse(call + ": needs a detector and the records' layout");
+    mww_detector_layout mine;
+    fill_layout(d, &mine);
+    int which = -1;
+    if (const char *field = detector_layout_mismatch(*layout, mine, &which))
+        return refuse(call + ": the records do not fit this detector: " + field + (which >= 0 ? " of model " + std::to_string(which) : std::string()) +
+                      " differs");
+    if (int rc = check_rows(d, call, h_ids, n, d_records, true)) return rc;
+    if (n == 0) return MWW_OK;
+    DENTER(d);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = stage_ids(d, h_ids, n, st)) return rc;
+    DCU(launch_unpack_detector_rows(record_job(d), d_records, d->d_rows, n, st));
     return MWW_OK;
 }
 

@@ -163,6 +163,15 @@ cudaError_t launch_detector_update_cutoffs(const DetectorArgs &a, const double *
 cudaError_t launch_detector_models_update_cutoffs(const DetectModelsArgsT<DetectModelRows> &a, cudaStream_t st);
 }  // namespace mww
 
+#include "mww_detector_records.h"
+namespace mww {
+// detector records (mww_detector_records.cu, layout and per-word bodies in mww_detector_records.h; companion library
+// libmww_detector_records.so): every used model's slot of the n records [n][J.words] of ids[0, n) (device memory, in range),
+// one launch each way
+cudaError_t launch_pack_detector_rows(const DetRecJob &J, void *records, const int32_t *ids, int n, cudaStream_t st);
+cudaError_t launch_unpack_detector_rows(const DetRecJob &J, const void *records, const int32_t *ids, int n, cudaStream_t st);
+}  // namespace mww
+
 namespace mww {
 // audio history (mww_history.cu, ring layout and index math in mww_history.h; companion library libmww_history.so)
 // the last min(n16, C) of a call's n16 16 kHz samples of streams [0, n_streams) of `audio` (pcm16 of T on load) -> their

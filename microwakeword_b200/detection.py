@@ -18,6 +18,7 @@ Live, the same rule runs per stream with its state carried across calls:
     MultiModelDetector(engine, cutoffs, windows, cooldown_slices, vad)   the same for every model of a MultiModelEngine in
                                                                        one launch, wake words gated by a VAD model
     set_cutoffs(...)                                                   either one: each stream's own sensitivity
+    export_rows / import_rows, export_streams / import_streams         either one: rows moved as packed device records
 """
 
 from __future__ import annotations
@@ -260,8 +261,57 @@ class _DeviceArray:
         self.__cuda_array_interface__ = dict(shape=(n,), typestr=typestr, data=(ptr, False), version=2, strides=None)
 
 
+def _record_ids(ids, what: str) -> np.ndarray:
+    """a list, NumPy array or CPU tensor of ids -> contiguous int32 array, or ValueError"""
+    if hasattr(ids, "is_cuda"):
+        if ids.is_cuda:
+            raise ValueError("%s must be in host memory" % what)
+        ids = ids.numpy()
+    a = np.asarray(ids)
+    if a.ndim != 1 or (a.size and (a.dtype == bool or not np.issubdtype(a.dtype, np.integer))):
+        raise ValueError("%s must be a 1-D sequence of integers" % what)
+    if a.size and (a.min() < np.iinfo(np.int32).min or a.max() > np.iinfo(np.int32).max):
+        raise ValueError("%s must fit in int32" % what)
+    return np.ascontiguousarray(a, np.int32)
+
+
+class DetectorRecords:
+    """Detector rows exported from a StreamDetector (export_rows) or a MultiModelDetector (export_streams): `data`,
+    torch.uint8 [n, record_bytes] on the detector's device, one packed record per listed id (include/mww.h), and `layout`,
+    the _lib.MwwDetectorLayout an importing detector must share.  `cutoffs` is each exported id's cutoff: float64 [n] for a
+    plain detector, a list of one float64 [n] per model for a models detector (NaN where the stream is not a member and
+    for an OFF model).  The records carry no events and no stream map."""
+
+    _SCALARS = ("record_bytes", "multi", "n_models")
+    _ARRAYS = ("role", "window", "cooldown_slices")
+
+    def __init__(self, data, layout, cutoffs):
+        self.data, self.layout, self.cutoffs = data, layout, cutoffs
+
+    def save(self, path) -> None:
+        """np.savez of the records, the layout's fields and the cutoffs: a checkpoint of some streams' detector rows"""
+        fields = {k: np.asarray(getattr(self.layout, k)) for k in self._SCALARS}
+        fields.update({k: np.ctypeslib.as_array(getattr(self.layout, k)).copy() for k in self._ARRAYS})
+        cut = np.stack(self.cutoffs) if self.layout.multi else np.asarray(self.cutoffs)
+        np.savez(path, data=self.data.cpu().numpy(), cutoffs=cut.astype(np.float64), **fields)
+
+    @classmethod
+    def load(cls, path, device) -> "DetectorRecords":
+        import torch
+        layout = _lib.MwwDetectorLayout()
+        with np.load(path) as z:
+            for k in cls._SCALARS:
+                setattr(layout, k, int(z[k]))
+            for k in cls._ARRAYS:
+                np.ctypeslib.as_array(getattr(layout, k))[:] = z[k]
+            data = torch.from_numpy(z["data"]).to(device)
+            cut = np.asarray(z["cutoffs"], np.float64)
+        return cls(data, layout, [c.copy() for c in cut] if layout.multi else cut.copy())
+
+
 class _Detector:
-    """what both detectors share: ownership of one mww_detector_t, its device views, drain and the reset dispatch"""
+    """what both detectors share: ownership of one mww_detector_t, its device views, drain, the reset dispatch and the
+    record calls"""
 
     def _own(self, rc: int, d, device: int, capacity: int) -> None:
         """take the detector a create call returned (rc, d) and make the views of its event buffers"""
@@ -301,6 +351,36 @@ class _Detector:
         self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
         ev = buf[:min(n.value, self.capacity)]
         return ev[np.lexsort(tuple(ev[k] for k in reversed(keys)))], max(n.value - self.capacity, 0)
+
+    def layout(self) -> "_lib.MwwDetectorLayout":
+        """record size, kind and each model's role, window and cooldown (mww_get_detector_layout; no device work)"""
+        out = _lib.MwwDetectorLayout()
+        self._check(self._L.mww_get_detector_layout(self._d, ctypes.byref(out)))
+        return out
+
+    def _export(self, ids, what: str):
+        """(records [n, record_bytes] of the listed ids, their layout), ordered on the current CUDA stream"""
+        import torch
+        ids = _record_ids(ids, what)
+        data = torch.empty((ids.size, int(self.layout().record_bytes)), dtype=torch.uint8, device=torch.device("cuda", self.device))
+        layout = _lib.MwwDetectorLayout()
+        self._check(self._L.mww_export_detector_rows(self._d, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
+                                                     self._cuda_stream()))
+        return ids, data, layout
+
+    def _import(self, ids, records: "DetectorRecords", what: str) -> np.ndarray:
+        """the listed ids take the records' state (the cutoffs are the caller's part); -> the ids as int32"""
+        import torch
+        ids = _record_ids(ids, what)
+        data = records.data
+        if (not isinstance(data, torch.Tensor) or data.dtype != torch.uint8 or data.dim() != 2 or data.shape[0] != ids.size
+                or data.shape[1] != records.layout.record_bytes or not data.is_contiguous() or not data.is_cuda
+                or data.device.index != self.device):
+            raise ValueError("records.data must be a contiguous uint8 tensor [len(%s)=%d, record_bytes=%d] on cuda:%d"
+                             % (what, ids.size, records.layout.record_bytes, self.device))
+        self._check(self._L.mww_import_detector_rows(self._d, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(records.layout),
+                                                     self._cuda_stream()))
+        return ids
 
     def _reset(self, ids, what: str) -> None:
         """reset all rows (None), or the ids of a contiguous 1-D CUDA int32 tensor or of a host sequence"""
@@ -403,6 +483,29 @@ class StreamDetector(_Detector):
         self._check(self._L.mww_get_detector_cutoffs(self._d, out.ctypes.data))
         return out
 
+    def export_rows(self, rows) -> DetectorRecords:
+        """The state of the listed ROW indices (hist, seen, cooldown) as packed records on this detector's device, ordered on
+        the current CUDA stream in one launch (mww_export_detector_rows), with each row's cutoff beside them.  A row may be
+        listed twice.  The detector does not change; events stay where they are (drain before moving)."""
+        ids, data, layout = self._export(rows, "rows")
+        return DetectorRecords(data, layout, self.cutoffs[ids])
+
+    def import_rows(self, rows, records: DetectorRecords) -> None:
+        """Row rows[i] takes the state of records.data[i] (mww_import_detector_rows) and continues bit for bit as the exported
+        row would have, its events reporting this detector's stream map.  Every other row is untouched.  Rows whose
+        exported cutoff differs from theirs get it (one set_cutoffs call, on the same CUDA stream), so two uniform detectors
+        with the same cutoff stay uniform.  Records of another kind, window or cooldown, out-of-range or duplicate rows:
+        MwwError with nothing changed; a malformed row list or records on another device: ValueError."""
+        if records.layout.multi == 0:
+            c = np.asarray(records.cutoffs, np.float64)
+            if c.shape != (records.data.shape[0],):
+                raise ValueError("records.cutoffs must hold one cutoff per record")
+        ids = self._import(rows, records, "rows")
+        c = np.asarray(records.cutoffs, np.float64)
+        diff = np.flatnonzero(c != self.cutoffs[ids])
+        if diff.size:
+            self.set_cutoffs(ids[diff], c[diff])
+
 
 def _cutoff_list(ids, cutoffs, name):
     """(int32 ids, float64 cutoffs) of one set-cutoffs call, or ValueError: ids a 1-D integer sequence, cutoffs one finite
@@ -451,7 +554,12 @@ class MultiModelDetector(_Detector):
     `cutoffs[k] = None` makes model k OFF; `windows` and `cooldown_slices` are one value or one per model (the VAD's
     cooldown is not used).  The detector copies the engine's strides and stream sets at creation and reads its pending rows
     then and after every update: it must see every call the engine makes, and after `engine.reset()` it needs `reset()`;
-    after `engine.set_streams` make a new one."""
+    after `engine.set_streams` make a new one and import every stream from the old one, so that the streams that stay
+    keep their rows and cutoffs:
+
+        new = MultiModelDetector(eng, ...)     # the same rules
+        all_ids = np.arange(eng.n_streams)
+        new.import_streams(all_ids, det.export_streams(all_ids))"""
 
     def __init__(self, engine, cutoffs, windows=5, cooldown_slices: int = 25, vad=None, capacity: int = 65536):
         K = engine.n_models
@@ -549,6 +657,54 @@ class MultiModelDetector(_Detector):
         out = np.empty(max(self.streams[k].size, 1), np.float64)
         self._check(self._L.mww_get_multi_detector_cutoffs(self._d, k, out.ctypes.data))
         return out[:self.streams[k].size]
+
+    def _lookup(self, k) -> np.ndarray:
+        """[n_streams]: the row of each global stream id in model k's list, -1 for a non-member (the lists are fixed)"""
+        if not hasattr(self, "_inv"):
+            self._inv = {}
+        if k not in self._inv:
+            inv = np.full(self.engine.n_streams, -1, np.int64)
+            inv[self.streams[k]] = np.arange(self.streams[k].size)
+            self._inv[k] = inv
+        return self._inv[k]
+
+    def export_streams(self, stream_ids) -> DetectorRecords:
+        """Every model's row of the listed GLOBAL streams (hist, seen, cooldown or active) as packed records on this
+        detector's device, ordered on the current CUDA stream in one launch (mww_export_detector_rows), with each stream's
+        cutoff per model beside them (NaN where it is not a member).  A stream may be listed twice.  The detector does not
+        change; events stay where they are (drain before moving)."""
+        ids, data, layout = self._export(stream_ids, "stream_ids")
+        cutoffs = []
+        for k in range(self.n_models):
+            c = np.full(ids.size, np.nan)
+            if self.roles[k] != _lib.MWW_DETECT_OFF:
+                row = self._lookup(k)[ids]
+                c[row >= 0] = self.get_cutoffs(k)[row[row >= 0]]
+            cutoffs.append(c)
+        return DetectorRecords(data, layout, cutoffs)
+
+    def import_streams(self, stream_ids, records: DetectorRecords) -> None:
+        """Stream stream_ids[i] takes the rows records.data[i] holds (mww_import_detector_rows).  Per model: a stream that is
+        not a member here ignores the record's slot; a member takes the slot's state, or fresh state (what reset gives) when
+        the exported stream was not a member; every other stream is untouched.  A member whose exported cutoff differs from
+        its own gets it (one set_cutoffs call per model, on the same CUDA stream).  After `engine.set_streams` this is how
+        the stayers keep their rows: make a new detector and import every stream from the old one.  Records of another
+        kind or rules, out-of-range or duplicate ids: MwwError with nothing changed; a malformed id list or records on
+        another device: ValueError."""
+        n = len(records.data)
+        if records.layout.multi == 1 and records.layout.n_models == self.n_models:
+            if len(records.cutoffs) != self.n_models or any(np.shape(c) != (n,) for c in records.cutoffs):
+                raise ValueError("records.cutoffs must hold one cutoff per record for each of the %d models" % self.n_models)
+        ids = self._import(stream_ids, records, "stream_ids")
+        for k in range(self.n_models):
+            if self.roles[k] == _lib.MWW_DETECT_OFF:
+                continue
+            row = self._lookup(k)[ids]
+            c = np.asarray(records.cutoffs[k], np.float64)
+            take = np.flatnonzero((row >= 0) & ~np.isnan(c))
+            take = take[c[take] != self.get_cutoffs(k)[row[take]]]
+            if take.size:
+                self.set_cutoffs(k, ids[take], c[take])
 
     def _flag_name(self, k):
         return "active" if self.roles[k] == _lib.MWW_DETECT_VAD else "cooldown"
