@@ -773,6 +773,65 @@ int mww_export_detector_rows(mww_detector_t *d, const int32_t *h_ids, int n, voi
 int mww_import_detector_rows(mww_detector_t *d, const int32_t *h_ids, int n, const void *d_records,
                              const mww_detector_layout *layout, void *cu_stream);
 
+/* ---- second-stage verification: re-score the streams a detector fired on, with a second model, from their audio history ----
+ * A small streaming model on every stream, and a larger one only on the few streams that just fired, over their last second
+ * or two of audio: the usual cascade against false wakes.  A VERIFIER owns one model (any container mww_create accepts:
+ * fp32 or int8 okay_nabu, any run-time geometry, hybrid), a fixed rule (n_samples, window, ignore_steps, cutoff) and `slots`
+ * scratch streams.  A verify call takes a source handle `src` that keeps an audio history and n <= slots stream ids.  For
+ * each index i:
+ *   - id in [0, src.n_streams): a = the last n_samples entries of that stream's audio history at this point in stream order,
+ *     what mww_read_audio_history returns.  p[0, m) = the probabilities a FRESH handle of the verifier's container (after
+ *     create or mww_reset(NULL)) gives from one mww_predict_clip of a, with m = frames / stride and frames = (n_samples -
+ *     480) / 160 + 1.  score[i] = mww_positive_scores of p with (window, ignore_steps): the max over j of the float32 mean of
+ *     p[ignore_steps + j, ignore_steps + j + window), NaN when fewer than window values remain -- the positive-sample score
+ *     of the reference's streaming ROC (test.py:364-373), on a fresh frontend per clip as the reference makes its positive
+ *     spectrograms.  confirmed[i] = the id when (double)score[i] > cutoff, else -1; NaN never confirms.
+ *   - any other id (the -1 slots of d_fired included): score[i] = NaN, confirmed[i] = -1.
+ * The scores are those of that definition bit for bit, because a call runs exactly those paths: the history read kernel on
+ * src, mww_reset(NULL) on the verifier's own handle, mww_predict_clip on it and mww_positive_scores.  A full reset leaves the
+ * handle as create does, so a verifier reused over many calls gives what a new one gives.
+ *
+ * Which ids:
+ *   - mww_verify_streams: d_ids [n], any int32 list in device memory (for example a plain detector's d_fired).
+ *   - mww_verify_detections: a detector's event slots [0, capacity), capacity <= slots.  Slot i is events[i].stream when
+ *     i < min(*d_count, capacity) and (model < 0 || events[i].reserved == model), else -1.  *d_count is read on the device,
+ *     in stream order.  Events of a models detector carry global stream ids, so they are src's ids; verify each wake word
+ *     with its own verifier through model = k.  Outputs are per slot: score i belongs to the drained event i, before any sort.
+ *
+ * Ordering and side effects:
+ *   - Both calls are asynchronous on cu_stream, never synchronise the host and never allocate: every buffer, the verifier
+ *     handle's clip scratch included, is sized at create.  A call issues a number of launches that depends neither on n nor
+ *     on how many events fired; n == 0 in mww_verify_streams does nothing.
+ *   - src and det are read, not changed: state, counters, audio history and events stay as they were.  The history read
+ *     is src's own kernel on src's ring, so it counts as one launch in mww_launch_count(src), as a direct read would.
+ *   - The verifier's handle is scratch, and calls on one verifier must be ordered by the caller.
+ *   - The read is "now": the last n_samples when the call runs, not the samples that end at the event.  A caller that
+ *     verifies at each drain, every D live calls of 480 samples, needs n_samples to cover what the verifier must hear plus
+ *     D x 480 samples.  Verify BEFORE mww_reset_device_ids(src, d_fired, ...): a reset zeroes the history.
+ *
+ * Refusals are MWW_EINVAL with a message in mww_last_error(NULL), and leave every object unchanged.
+ *   - create: slots < 1; n_samples outside [480, 2^22]; window outside [1, 32]; ignore_steps < 0; a non-finite cutoff; a
+ *     rule with m < ignore_steps + window (every score would be NaN); a frontend-only (NULL) blob.  Without a CUDA device
+ *     MWW_ECUDA ("no CUDA device"); a model that fails to load returns its mww_create error.
+ *   - verify: a NULL verifier or src; src without an audio history or with capacity < n_samples; src, det and the verifier
+ *     not on one device; n < 0 or n > slots; a detector capacity > slots; model >= K of the detector (a plain detector has
+ *     K = 1); d_ids NULL with n > 0; a poisoned src.  Either output pointer may be NULL.
+ *   - mww_verifier_info fills mww_verifier_desc: slots, steps (= m), device, the rule, and launches = mww_launch_count of the
+ *     verifier's handle. */
+typedef struct mww_verifier mww_verifier_t;
+typedef struct mww_verify_rule { int32_t n_samples, window, ignore_steps, pad; double cutoff; } mww_verify_rule;
+typedef struct mww_verifier_desc {
+    int32_t slots, steps, device, pad;
+    mww_verify_rule rule;
+    int64_t launches;
+} mww_verifier_desc;
+int mww_verifier_create(const void *model_blob, size_t n_bytes, int device, int slots, const mww_verify_rule *rule, mww_verifier_t **out);
+int mww_verifier_destroy(mww_verifier_t *v);
+int mww_verifier_info(const mww_verifier_t *v, mww_verifier_desc *out);
+int mww_verify_streams(mww_verifier_t *v, mww_t *src, const int32_t *d_ids, int n, float *d_scores, int32_t *d_confirmed, void *cu_stream);
+int mww_verify_detections(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, float *d_scores, int32_t *d_confirmed,
+                          void *cu_stream);
+
 #ifdef __cplusplus
 }
 #endif

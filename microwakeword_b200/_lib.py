@@ -41,6 +41,7 @@ EXPORTS = (
     "mww_predict_clip_multi_g711", "mww_predict_clip_host_multi_g711", "mww_predict_clip_remote_multi_g711",
     "mww_set_audio_history", "mww_get_audio_history", "mww_read_audio_history", "mww_read_audio_history_device_ids",
     "mww_get_detector_layout", "mww_export_detector_rows", "mww_import_detector_rows",
+    "mww_verifier_create", "mww_verifier_destroy", "mww_verifier_info", "mww_verify_streams", "mww_verify_detections",
 )
 
 
@@ -86,6 +87,18 @@ class MwwDetectorLayout(ctypes.Structure):
         ("record_bytes", ctypes.c_int64), ("multi", ctypes.c_int32), ("n_models", ctypes.c_int32),
         ("role", ctypes.c_int32 * 64), ("window", ctypes.c_int32 * 64), ("cooldown_slices", ctypes.c_int32 * 64),
     ]
+
+
+class MwwVerifyRule(ctypes.Structure):
+    """mww_verify_rule of include/mww.h: what a verifier reads, and how it scores and confirms"""
+    _fields_ = [("n_samples", ctypes.c_int32), ("window", ctypes.c_int32), ("ignore_steps", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("cutoff", ctypes.c_double)]
+
+
+class MwwVerifierDesc(ctypes.Structure):
+    """mww_verifier_desc of include/mww.h (mww_verifier_info)"""
+    _fields_ = [("slots", ctypes.c_int32), ("steps", ctypes.c_int32), ("device", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("rule", MwwVerifyRule), ("launches", ctypes.c_int64)]
 
 
 class MwwError(RuntimeError):
@@ -277,6 +290,16 @@ def lib() -> ctypes.CDLL:
     for name in ("mww_export_detector_rows", "mww_import_detector_rows"):
         getattr(L, name).restype = i32
         getattr(L, name).argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwDetectorLayout), vp]
+    L.mww_verifier_create.restype = i32
+    L.mww_verifier_create.argtypes = [vp, sz, i32, i32, ctypes.POINTER(MwwVerifyRule), ctypes.POINTER(vp)]
+    L.mww_verifier_destroy.restype = i32
+    L.mww_verifier_destroy.argtypes = [vp]
+    L.mww_verifier_info.restype = i32
+    L.mww_verifier_info.argtypes = [vp, ctypes.POINTER(MwwVerifierDesc)]
+    L.mww_verify_streams.restype = i32
+    L.mww_verify_streams.argtypes = [vp, vp, vp, i32, vp, vp, vp]
+    L.mww_verify_detections.restype = i32
+    L.mww_verify_detections.argtypes = [vp, vp, vp, i32, vp, vp, vp]
     _lib = L
     return L
 

@@ -183,3 +183,14 @@ cudaError_t launch_history_append(int16_t *ring, int C, long long seen, const T 
 cudaError_t launch_history_read(const int16_t *ring, int C, long long seen, const int32_t *ids, int n, int n_streams, int n_samples, int16_t *out,
                                 long long out_stride, int sm_count, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_verify.h"
+namespace mww {
+// second-stage verification (mww_verify.cu, per-element bodies in mww_verify.h; companion library libmww_verify.so)
+// ids [capacity]: the stream of each of a detector's event slots that holds an event of `model` (< 0: any), -1 elsewhere;
+// *count is read on the device
+cudaError_t launch_verify_slots(const long long *count, const mww_event *events, int capacity, int model, int32_t *ids, cudaStream_t st);
+// out_scores / out_confirmed [n] (either may be nullptr) from the ids [n] and the verifier's scores [n]
+cudaError_t launch_verify_confirm(const int32_t *ids, int n, int n_streams, const float *scores, double cutoff, float *out_scores,
+                                  int32_t *out_confirmed, cudaStream_t st);
+}  // namespace mww

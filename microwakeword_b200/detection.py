@@ -344,13 +344,17 @@ class _Detector:
         """free the detector now; fired_ids and event_count must not be used afterwards"""
         self._handle.close()
 
-    def _drain(self, dtype, keys):
-        """(events since the last drain as `dtype`, sorted by `keys`, most significant first; events dropped)"""
+    def _drain_slots(self, dtype):
+        """(events since the last drain as `dtype` in slot order, events that fired)"""
         buf = np.empty(self.capacity, dtype)
         n = ctypes.c_longlong(0)
         self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
-        ev = buf[:min(n.value, self.capacity)]
-        return ev[np.lexsort(tuple(ev[k] for k in reversed(keys)))], max(n.value - self.capacity, 0)
+        return buf[:min(n.value, self.capacity)], n.value
+
+    def _drain(self, dtype, keys):
+        """(events since the last drain as `dtype`, sorted by `keys`, most significant first; events dropped)"""
+        ev, n = self._drain_slots(dtype)
+        return ev[np.lexsort(tuple(ev[k] for k in reversed(keys)))], max(n - self.capacity, 0)
 
     def layout(self) -> "_lib.MwwDetectorLayout":
         """record size, kind and each model's role, window and cooldown (mww_get_detector_layout; no device work)"""
