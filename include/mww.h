@@ -832,6 +832,146 @@ int mww_verify_streams(mww_verifier_t *v, mww_t *src, const int32_t *d_ids, int 
 int mww_verify_detections(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, float *d_scores, int32_t *d_confirmed,
                           void *cu_stream);
 
+/* ---- endpointing: where the spoken command after a wake word ends, and its clip from the audio history ----------------------
+ * After a wake word a voice assistant sends the command that follows to speech-to-text and stops when the speaker stops.  An
+ * ENDPOINTER finds that end on the GPU, per stream, from a VAD model's probabilities, and cuts each command's clip from the
+ * audio history, with no host round trip.
+ *
+ * What it is bound to.  An endpointer is created from a handle h that keeps an audio history and a model index k, whose
+ * probabilities it reads as speech probabilities (any model works).  At create it copies, host side only, the model's
+ * stride s, its stream set S_k (all streams when it has none) and hop_samples.  Each member of S_k has one row, in list
+ * order, as the model's probabilities do (the VAD role of a models detector follows the same convention).
+ *
+ * Time axis.  Every position is on the audio history's axis (samples_seen of mww_get_audio_history), so a position reads
+ * back from the ring directly.  An update describes the handle call made just before it.  Right after that call the
+ * endpointer reads h's host-side counters: S = samples_seen, b = frontend_buffered - (480 - hop) and g = model k's pending
+ * rows.  The call's n steps end at
+ *     pos(j) = S - b - hop (g + (n - 1 - j) s),   j = 0 .. n - 1,
+ * the last 16 kHz sample of the newest feature window of step j.  Derivation: the frontend emits a row when it holds 480
+ * samples and then drops hop of them, so a call of n16 samples that emits R rows leaves buffered' = buffered + n16 - R hop,
+ * and after any row the carry holds the last 480 - hop samples of the newest window plus the b samples that came after it:
+ * buffered = (480 - hop) + b, so the newest row's window ends at S - b (before the first row, b < 0 and S - b is where a row
+ * before it would have ended, one hop before the first).  Model k runs a step on every s rows and holds the g newest, so
+ * its newest step ends g rows, hop g samples, before the newest row, and each earlier step s rows before the next.  In
+ * 480-sample live calls b = 0.  The endpointer keeps the counters of the previous update (S', b', g'); the rows emitted
+ * since then are R = ((S - b) - (S' - b')) / hop, and an update is refused (MWW_EINVAL, before any launch) unless R is a
+ * whole number >= 0 and n s = g' + R - g, as the models detector refuses inconsistent updates: this catches a skipped
+ * update.  After a full reset of the handle (mww_reset(NULL), mww_reset_frontend) or mww_set_audio_history, reset the whole
+ * endpointer, which takes the handle's counters as its new baseline.
+ *
+ * Speech flag.  Every member row runs the VAD rule of the models detector on every step, armed or not: float32 window_mean
+ * over vad_window (1 .. 32) probabilities, and speech = seen >= vad_window && (double)avg > vad_cutoff, with seen counting
+ * this step.  So a row's flag is the `active` flag of a models detector's VAD row with the same window and cutoff, fed the
+ * same probabilities, bit for bit.  Each row keeps its last 64 flags in a uint64 (bit i: i steps before the newest); a flag
+ * from before a reset, or from before the row had a full window, is 0.
+ *
+ * Segmenter.  It runs on armed rows only.  State: elapsed, run, silence, heard, start_sample, speech_end_sample.  For each
+ * step in order, with flag f at position p (the first step after arming sets start_sample = speech_end_sample = p - s hop):
+ *     elapsed += 1
+ *     if f:  run += 1; silence = 0; if run >= speech_steps: heard = 1;  if heard: speech_end_sample = p
+ *     else:  run = 0;  silence += 1
+ *     end with END_OF_SPEECH if heard && silence >= silence_steps
+ *     else NO_SPEECH         if !heard && elapsed >= timeout_steps
+ *     else MAX_LENGTH        if elapsed >= max_steps
+ * A row that ends emits one event and disarms; a row that is not armed holds zero segmenter state.
+ *
+ * Arming.  arm(ids) takes GLOBAL stream ids from the host (ids outside [0, n_streams) are MWW_EINVAL) or the device (ids
+ * outside the set and -1 are ignored, so a verifier's d_confirmed or a detector's d_fired is passed in directly).  A host id
+ * in range that is not a member of S_k is ignored, and an id listed twice arms once.  Arming a row gives it fresh segmenter
+ * state (re-arming an armed row restarts it), then replays its last L = min(lookback_steps, steps consumed since create or
+ * the last whole reset) flags, oldest first, at their recorded positions (lookback_steps in 0 .. 64).  So arming with
+ * lookback L is the same as having armed L steps earlier, which covers the detector -> verifier -> arm latency: a drain
+ * every 33 live calls is about 1 s, and 64 steps are 1.92 s at stride 3.  A replay that reaches an end condition emits its
+ * event during the arm call.  A replay that reaches back over the wake word hears it as speech: the segment then starts
+ * before the wake word, and a pause of silence_steps after it ends the command with END_OF_SPEECH before the command is
+ * spoken.  Choose lookback_steps (the latency to cover) and silence_steps (longer than the pause a speaker makes after the
+ * wake word) together.  disarm(ids) cancels without an event.  reset(ids) gives those rows fresh VAD and segmenter state:
+ * call it when the handle's streams are reset.  A whole reset (ids NULL) does that for every row, takes the handle's
+ * counters as the new baseline and forgets the steps consumed and their positions, so no replay reaches across it (the
+ * axis may have restarted: mww_set_audio_history sets samples_seen back to 0).
+ *
+ * Outputs, as the detectors keep them:
+ *   - events through a device counter into `capacity` slots; the count keeps going past capacity, and drain reports the
+ *     true count.  end_sample is the position of the ending step; speech_end_sample is start_sample if speech was never
+ *     heard; steps is elapsed at the end.
+ *   - d_ended [capacity]: the stream of each used slot, -1 elsewhere.  It feeds mww_reset_device_ids and
+ *     mww_read_audio_history_device_ids.
+ *   - d_armed [n_rows]: the global id of every armed row, -1 elsewhere.  With the history read it lets a server stream the
+ *     new audio of commands in progress to a streaming STT at each poll.
+ *   - drain synchronises cu_stream, copies min(count, capacity, max_events) events to h_events, *n_events = the events since
+ *     the last drain, then clears the counter and refills d_ended with -1.
+ *
+ * Command read.  mww_endpointer_read_commands writes, for each used event slot i, samples [a, e) of the stream's history,
+ * oldest first, into row i of d_out [capacity][out_stride] int16: a = start_sample - pre, e = min(speech_end_sample + post,
+ * end_sample) for END_OF_SPEECH and end_sample otherwise, the length capped at max_samples keeping the beginning.  Entries
+ * outside the ring are zeros: those older than samples_seen - C and those from before a reset, as the history rule already
+ * defines them, and those at or after samples_seen.  d_lengths[i] (int32) is the length, 0 for unused slots; row entries
+ * past the length are zeros.  The event count is read on the device.  One launch, no host synchronisation; read BEFORE the
+ * drain, and BEFORE any reset of those streams: a reset zeroes their history.
+ *
+ * Calls.  Update, arm, disarm, reset and read are asynchronous on cu_stream, never allocate and issue one launch each,
+ * whatever n is and however many rows are armed or ended; a host id list is copied into a buffer the endpointer owns, so
+ * calls on one endpointer from different CUDA streams must be ordered by the caller.  None of them launches work on h, and
+ * mww_endpointer_info reports the endpointer's own launches.  Events and state do not depend on how the audio was split into
+ * calls, as long as every call's probabilities are passed.
+ *   - update: d_probs [n_rows][pitch] (pitch >= n), the model's probabilities of the call just made on h.
+ *   - get_state / set_state: host buffers, synchronous, NULL pointers skipped; per row hist [n_rows][vad_window - 1] oldest
+ *     first, seen, flags, armed, elapsed, run, silence, heard, start_sample, speech_end_sample; and the endpointer's
+ *     baseline (samples_seen, buffered, pending), steps consumed since create or the last whole reset and positions[i], the position of the step i
+ *     steps before the newest (0 where there is none).  set refuses a negative seen or count, heard outside {0, 1}, an armed
+ *     value that is neither -1 nor the row's stream, and a baseline outside the handle's ranges.
+ *
+ * Refusals are MWW_EINVAL with a message in mww_last_error(NULL), before any device work.
+ *   - create: a handle without history; a frontend-only handle or k out of range; vad_window outside [1, 32] or a
+ *     non-finite vad_cutoff; speech_steps, silence_steps, timeout_steps or max_steps below 1; lookback_steps outside
+ *     [0, 64]; capacity < 1.  Without a CUDA device MWW_ECUDA ("no CUDA device").
+ *   - update: n < 0, pitch < n, NULL probabilities with n > 0, and the consistency check above.
+ *   - read: a different handle than the endpointer's, pre < 0, post < 0, max_samples outside [0, 2^22], out_stride <
+ *     max_samples, NULL buffers, or a handle that no longer keeps a history. */
+#define MWW_ENDPOINT_END_OF_SPEECH 1
+#define MWW_ENDPOINT_NO_SPEECH 2
+#define MWW_ENDPOINT_MAX_LENGTH 3
+typedef struct mww_endpointer mww_endpointer_t;
+typedef struct mww_endpoint_rule {
+    int32_t vad_window, speech_steps, silence_steps, timeout_steps, max_steps, lookback_steps;
+    double vad_cutoff;
+} mww_endpoint_rule;
+typedef struct mww_endpoint_event {
+    int32_t stream, reason;
+    int64_t start_sample, end_sample, speech_end_sample;
+    int32_t steps, pad;
+} mww_endpoint_event;
+typedef struct mww_endpointer_desc {
+    int32_t n_rows, model, stride, hop_samples, capacity, device;
+    mww_endpoint_rule rule;
+    int64_t steps, launches;
+} mww_endpointer_desc;
+typedef struct mww_endpoint_state {
+    float *hist;
+    int64_t *seen;
+    uint64_t *flags;
+    int32_t *armed, *elapsed, *run, *silence, *heard;
+    int64_t *start_sample, *speech_end_sample;
+    int64_t samples_seen, buffered, pending, steps;
+    int64_t positions[64];
+} mww_endpoint_state;
+int mww_endpointer_create(const mww_t *h, int model, const mww_endpoint_rule *rule, int capacity, mww_endpointer_t **out);
+int mww_endpointer_destroy(mww_endpointer_t *ep);
+int mww_endpointer_info(const mww_endpointer_t *ep, mww_endpointer_desc *out);
+int mww_endpointer_update(mww_endpointer_t *ep, const float *d_probs, int n, long long pitch, void *cu_stream);
+int mww_endpointer_arm(mww_endpointer_t *ep, const int32_t *h_ids, int n, void *cu_stream);
+int mww_endpointer_arm_device(mww_endpointer_t *ep, const int32_t *d_ids, int n, void *cu_stream);
+int mww_endpointer_disarm(mww_endpointer_t *ep, const int32_t *h_ids, int n, void *cu_stream);
+int mww_endpointer_reset(mww_endpointer_t *ep, const int32_t *h_ids, int n, void *cu_stream);
+int mww_endpointer_reset_device(mww_endpointer_t *ep, const int32_t *d_ids, int n, void *cu_stream);
+int mww_endpointer_drain(mww_endpointer_t *ep, mww_endpoint_event *h_events, int max_events, long long *n_events, void *cu_stream);
+int mww_endpointer_buffers(mww_endpointer_t *ep, const long long **d_count, const mww_endpoint_event **d_events, const int32_t **d_ended,
+                           const int32_t **d_armed, int *capacity);
+int mww_endpointer_get_state(mww_endpointer_t *ep, mww_endpoint_state *out);
+int mww_endpointer_set_state(mww_endpointer_t *ep, const mww_endpoint_state *in);
+int mww_endpointer_read_commands(mww_endpointer_t *ep, mww_t *h, long long pre, long long post, int max_samples, int16_t *d_out,
+                                 long long out_stride, int32_t *d_lengths, void *cu_stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -42,6 +42,10 @@ EXPORTS = (
     "mww_set_audio_history", "mww_get_audio_history", "mww_read_audio_history", "mww_read_audio_history_device_ids",
     "mww_get_detector_layout", "mww_export_detector_rows", "mww_import_detector_rows",
     "mww_verifier_create", "mww_verifier_destroy", "mww_verifier_info", "mww_verify_streams", "mww_verify_detections",
+    "mww_endpointer_create", "mww_endpointer_destroy", "mww_endpointer_info", "mww_endpointer_update", "mww_endpointer_arm",
+    "mww_endpointer_arm_device", "mww_endpointer_disarm", "mww_endpointer_reset", "mww_endpointer_reset_device",
+    "mww_endpointer_drain", "mww_endpointer_buffers", "mww_endpointer_get_state", "mww_endpointer_set_state",
+    "mww_endpointer_read_commands",
 )
 
 
@@ -99,6 +103,38 @@ class MwwVerifierDesc(ctypes.Structure):
     """mww_verifier_desc of include/mww.h (mww_verifier_info)"""
     _fields_ = [("slots", ctypes.c_int32), ("steps", ctypes.c_int32), ("device", ctypes.c_int32), ("pad", ctypes.c_int32),
                 ("rule", MwwVerifyRule), ("launches", ctypes.c_int64)]
+
+
+MWW_ENDPOINT_END_OF_SPEECH, MWW_ENDPOINT_NO_SPEECH, MWW_ENDPOINT_MAX_LENGTH = 1, 2, 3
+
+
+class MwwEndpointRule(ctypes.Structure):
+    """mww_endpoint_rule of include/mww.h: an endpointer's VAD rule and segmenter limits, in model steps"""
+    _fields_ = [("vad_window", ctypes.c_int32), ("speech_steps", ctypes.c_int32), ("silence_steps", ctypes.c_int32),
+                ("timeout_steps", ctypes.c_int32), ("max_steps", ctypes.c_int32), ("lookback_steps", ctypes.c_int32),
+                ("vad_cutoff", ctypes.c_double)]
+
+
+class MwwEndpointEvent(ctypes.Structure):
+    """mww_endpoint_event of include/mww.h: one command that ended"""
+    _fields_ = [("stream", ctypes.c_int32), ("reason", ctypes.c_int32), ("start_sample", ctypes.c_int64), ("end_sample", ctypes.c_int64),
+                ("speech_end_sample", ctypes.c_int64), ("steps", ctypes.c_int32), ("pad", ctypes.c_int32)]
+
+
+class MwwEndpointerDesc(ctypes.Structure):
+    """mww_endpointer_desc of include/mww.h (mww_endpointer_info)"""
+    _fields_ = [("n_rows", ctypes.c_int32), ("model", ctypes.c_int32), ("stride", ctypes.c_int32), ("hop_samples", ctypes.c_int32),
+                ("capacity", ctypes.c_int32), ("device", ctypes.c_int32), ("rule", MwwEndpointRule), ("steps", ctypes.c_int64),
+                ("launches", ctypes.c_int64)]
+
+
+class MwwEndpointState(ctypes.Structure):
+    """mww_endpoint_state of include/mww.h (mww_endpointer_get_state / _set_state): host pointers to the row arrays, the
+    baseline counters, the steps consumed and the last 64 step positions"""
+    _fields_ = [("hist", ctypes.c_void_p), ("seen", ctypes.c_void_p), ("flags", ctypes.c_void_p), ("armed", ctypes.c_void_p),
+                ("elapsed", ctypes.c_void_p), ("run", ctypes.c_void_p), ("silence", ctypes.c_void_p), ("heard", ctypes.c_void_p),
+                ("start_sample", ctypes.c_void_p), ("speech_end_sample", ctypes.c_void_p), ("samples_seen", ctypes.c_int64),
+                ("buffered", ctypes.c_int64), ("pending", ctypes.c_int64), ("steps", ctypes.c_int64), ("positions", ctypes.c_int64 * 64)]
 
 
 class MwwError(RuntimeError):
@@ -300,6 +336,28 @@ def lib() -> ctypes.CDLL:
     L.mww_verify_streams.argtypes = [vp, vp, vp, i32, vp, vp, vp]
     L.mww_verify_detections.restype = i32
     L.mww_verify_detections.argtypes = [vp, vp, vp, i32, vp, vp, vp]
+    L.mww_endpointer_create.restype = i32
+    L.mww_endpointer_create.argtypes = [vp, i32, ctypes.POINTER(MwwEndpointRule), i32, ctypes.POINTER(vp)]
+    L.mww_endpointer_destroy.restype = i32
+    L.mww_endpointer_destroy.argtypes = [vp]
+    L.mww_endpointer_info.restype = i32
+    L.mww_endpointer_info.argtypes = [vp, ctypes.POINTER(MwwEndpointerDesc)]
+    L.mww_endpointer_update.restype = i32
+    L.mww_endpointer_update.argtypes = [vp, vp, i32, ll, vp]
+    for name in ("mww_endpointer_arm", "mww_endpointer_arm_device", "mww_endpointer_disarm", "mww_endpointer_reset",
+                 "mww_endpointer_reset_device"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, vp]
+    L.mww_endpointer_drain.restype = i32
+    L.mww_endpointer_drain.argtypes = [vp, vp, i32, ctypes.POINTER(ll), vp]
+    L.mww_endpointer_buffers.restype = i32
+    L.mww_endpointer_buffers.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(vp), pi]
+    L.mww_endpointer_get_state.restype = i32
+    L.mww_endpointer_get_state.argtypes = [vp, ctypes.POINTER(MwwEndpointState)]
+    L.mww_endpointer_set_state.restype = i32
+    L.mww_endpointer_set_state.argtypes = [vp, ctypes.POINTER(MwwEndpointState)]
+    L.mww_endpointer_read_commands.restype = i32
+    L.mww_endpointer_read_commands.argtypes = [vp, vp, ll, ll, i32, vp, ll, vp, vp]
     _lib = L
     return L
 

@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmww_b200.so")
-SOURCES = ["mww_capi.cu", "mww_detector_capi.cu", "mww_verify_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_streams.cu", "mww_records.cu", "mww_detect.cu", "mww_tables.cc", "mww_container.cc"]
+SOURCES = ["mww_capi.cu", "mww_detector_capi.cu", "mww_verify_capi.cu", "mww_endpoint_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_streams.cu", "mww_records.cu", "mww_detect.cu", "mww_tables.cc", "mww_container.cc"]
 # the input-rate resampler kernel (mww_set_input_rate) is a companion library that libmww_b200.so links (rpath $ORIGIN): the
 # main library's own kernel set stays the one the SASS fixtures under tests/golden/ record
 RS_OUT = os.path.join(HERE, "libmww_resample.so")
@@ -44,6 +44,9 @@ DR_SOURCES = ["mww_detector_records.cu"]
 # exactly the kernels it had
 VER_OUT = os.path.join(HERE, "libmww_verify.so")
 VER_SOURCES = ["mww_verify.cu"]
+# and the endpointer's four kernels (mww_endpointer_*), likewise
+EP_OUT = os.path.join(HERE, "libmww_endpoint.so")
+EP_SOURCES = ["mww_endpoint.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -66,7 +69,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -87,9 +90,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
         for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (RR_OUT, RR_SOURCES, []), (DET_OUT, DET_SOURCES, []),
                                     (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []), (G711_OUT, G711_SOURCES, []),
                                     (HIST_OUT, HIST_SOURCES, []), (DR_OUT, DR_SOURCES, []), (VER_OUT, VER_SOURCES, []),
+                                    (EP_OUT, EP_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
                                                     "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711", "-lmww_history",
-                                                    "-lmww_detector_records", "-lmww_verify",
+                                                    "-lmww_detector_records", "-lmww_verify", "-lmww_endpoint",
                                                     "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra

@@ -2145,6 +2145,14 @@ int mww_set_audio_history(mww_t *h, int capacity, void *cu_stream) {
     return MWW_OK;
 }
 
+}  // extern "C"
+
+namespace mww {
+HistoryRing history_ring(const mww_t *h) { return HistoryRing{h->d_hist, h->hist_cap, h->hist_seen, h->n_streams, h->sm_count, h->poisoned}; }
+}  // namespace mww
+
+extern "C" {
+
 int mww_get_audio_history(const mww_t *h, int *capacity, long long *samples_seen) {
     if (!h) return MWW_EINVAL;
     if (capacity) *capacity = h->hist_cap;

@@ -1,5 +1,5 @@
-// mww_capi.h -- what the two C-ABI translation units share: mww_capi.cu (the handle) and mww_detector_capi.cu (the
-// streaming detectors).  Host code only.
+// mww_capi.h -- what the C-ABI translation units share: mww_capi.cu (the handle), mww_detector_capi.cu (the streaming
+// detectors) and mww_endpoint_capi.cu (the endpointer).  Host code only.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -26,5 +26,13 @@ struct DeviceGuard {
     }
     ~DeviceGuard() { if (switched) cudaSetDevice(prev); }
 };
+
+// a handle's audio history as a kernel of another object reads it in stream order (the endpointer's command read): ring
+// [n_streams][capacity] and samples_seen as of the calls issued so far.  ring is nullptr when the handle keeps no history;
+// poisoned is set when a staged call failed half-way.
+struct HistoryRing {
+    const int16_t *ring; int capacity; long long seen; int n_streams, sm_count; bool poisoned;
+};
+HistoryRing history_ring(const mww_t *h);
 
 }  // namespace mww

@@ -194,3 +194,19 @@ cudaError_t launch_verify_slots(const long long *count, const mww_event *events,
 cudaError_t launch_verify_confirm(const int32_t *ids, int n, int n_streams, const float *scores, double cutoff, float *out_scores,
                                   int32_t *out_confirmed, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_endpoint.h"
+namespace mww {
+// endpointing (mww_endpoint.cu, rule and per-row bodies in mww_endpoint.h; companion library libmww_endpoint.so), one launch
+// each.  update: n steps of every row, step j at position pos0 + j * a.step_samples
+cudaError_t launch_endpoint_update(const EndpointArgs &a, const float *probs, long long pitch, int n, long long pos0, cudaStream_t st);
+// arm the n listed global ids (device memory; ids outside the set ignored) with the replay R
+cudaError_t launch_endpoint_arm(const EndpointArgs &a, const EndpointReplay &R, const int32_t *ids, int n, cudaStream_t st);
+// disarm (reset 0) or reset (reset 1) the n listed global ids, or, ids == nullptr, rows [0, n)
+cudaError_t launch_endpoint_clear(const EndpointArgs &a, const int32_t *ids, int n, int reset, cudaStream_t st);
+// out [capacity][out_stride] and lengths [capacity]: the command of each used event slot from ring [n_streams][C], `seen`
+// samples appended; *count is read on the device
+cudaError_t launch_endpoint_read(const int16_t *ring, int C, long long seen, const unsigned long long *count, const mww_endpoint_event *events,
+                                 int capacity, long long pre, long long post, int max_samples, int16_t *out, long long out_stride,
+                                 int32_t *lengths, int sm_count, cudaStream_t st);
+}  // namespace mww

@@ -1,0 +1,268 @@
+"""Endpointing on the GPU (mww_endpointer_* of include/mww.h): after a wake word, find where each stream's spoken command
+ends from a VAD model's probabilities, and cut the command's clip from the engine's audio history.  Nothing leaves the GPU
+until the clips are wanted:
+
+    eng.set_audio_history(16000 * 12)
+    ep = Endpointer(eng, model=vad)                      # vad: the model index whose probabilities mean speech
+    probs = eng.step(chunk)
+    det.update(probs); ep.update(probs[vad])
+    scores, confirmed = ver.verify(eng, det)
+    ep.arm(confirmed)                                    # replays the last lookback_steps, so the command's start is kept
+    ...
+    clips, lengths = ep.commands(pre=1600, post=3200, max_samples=16000 * 10)     # before the drain and the reset
+    eng.reset(ep.ended_ids); det.reset(ep.ended_ids)
+    events, dropped = ep.drain()
+
+Every position is a sample index on the audio history's axis (engine.audio_samples_seen).  Steps are model steps: 30 ms at
+stride 3 and a 10 ms hop, which is what the defaults are written for.
+"""
+
+from __future__ import annotations
+
+import ctypes
+import math
+
+import numpy as np
+
+from . import _lib
+from .detection import _DeviceArray, _DetectorHandle, _record_ids
+from .engine import MAX_AUDIO_HISTORY
+
+END_OF_SPEECH, NO_SPEECH, MAX_LENGTH = _lib.MWW_ENDPOINT_END_OF_SPEECH, _lib.MWW_ENDPOINT_NO_SPEECH, _lib.MWW_ENDPOINT_MAX_LENGTH
+ENDPOINT_EVENT_DTYPE = np.dtype([("stream", np.int32), ("reason", np.int32), ("start_sample", np.int64), ("end_sample", np.int64),
+                                 ("speech_end_sample", np.int64), ("steps", np.int32), ("pad", np.int32)])
+
+
+def _int(value, name: str) -> int:
+    if isinstance(value, bool) or not isinstance(value, (int, np.integer)):
+        raise ValueError("%s must be an integer (got %r)" % (name, value))
+    return int(value)
+
+
+class _EndpointerHandle(_DetectorHandle):
+    """owner of one mww_endpointer_t: destroyed when the endpointer and every tensor over its buffers are gone"""
+
+    def close(self):
+        if self.ptr:
+            self.L.mww_endpointer_destroy(self.ptr)
+            self.ptr = None
+
+
+class Endpointer:
+    """Per-stream VAD endpointing of model `model` (None: 0) of `engine`, a StreamEngine or MultiModelEngine that keeps an
+    audio history.  Each member stream of the model's stream set has a row.  Every row runs the models detector's VAD rule
+    (moving average of `vad_window` probabilities above `vad_cutoff`) on every step; an armed row also runs the segmenter
+    and ends with one event:
+
+    - END_OF_SPEECH once speech was heard (`speech_steps` speech flags in a row; default 3 steps = 90 ms at 30 ms steps)
+      and then `silence_steps` steps without speech (default 25 = 0.75 s);
+    - NO_SPEECH when nothing was heard within `timeout_steps` (default 100 = 3 s);
+    - MAX_LENGTH after `max_steps` (default 334, about 10 s).
+
+    `lookback_steps` (0 .. 64, default 64 = 1.92 s) are replayed at arm, so arming late by the detector -> verifier
+    latency changes nothing.  The replay reaches back over the wake word itself, which the VAD hears as speech: the segment
+    (and the clip) starts before the wake word, and if the speaker pauses longer than `silence_steps` after it, the command
+    ends with END_OF_SPEECH before it is spoken.  Set lookback_steps to the latency to cover, not more, and silence_steps
+    above the pause speakers make after the wake word.  A whole reset() forgets the steps before it: no replay crosses it.
+    `capacity` events are kept between drains; more are counted and dropped."""
+
+    def __init__(self, engine, model=None, vad_window: int = 5, vad_cutoff: float = 0.5, speech_steps: int = 3, silence_steps: int = 25,
+                 timeout_steps: int = 100, max_steps: int = 334, lookback_steps: int = 64, capacity: int = 4096):
+        model = 0 if model is None else _int(model, "model")
+        vad_window, capacity = _int(vad_window, "vad_window"), _int(capacity, "capacity")
+        steps = {k: _int(v, k) for k, v in (("speech_steps", speech_steps), ("silence_steps", silence_steps),
+                                            ("timeout_steps", timeout_steps), ("max_steps", max_steps))}
+        lookback_steps = _int(lookback_steps, "lookback_steps")
+        if not 1 <= vad_window <= 32:
+            raise ValueError("vad_window must be in [1, 32] (got %d)" % vad_window)
+        if isinstance(vad_cutoff, bool) or not isinstance(vad_cutoff, (int, float, np.integer, np.floating)) or not math.isfinite(vad_cutoff):
+            raise ValueError("vad_cutoff must be a finite number (got %r)" % (vad_cutoff,))
+        for k, v in steps.items():
+            if v < 1:
+                raise ValueError("%s must be at least 1 (got %d)" % (k, v))
+        if not 0 <= lookback_steps <= 64:
+            raise ValueError("lookback_steps must be in [0, 64] (got %d)" % lookback_steps)
+        if capacity < 1:
+            raise ValueError("capacity must be at least 1 (got %d)" % capacity)
+        if getattr(engine, "_h", None) is None:
+            raise ValueError("engine must be a StreamEngine or MultiModelEngine")
+        if engine.audio_history_capacity == 0:
+            raise ValueError("the engine keeps no audio history (set_audio_history)")
+        n_models = getattr(engine, "n_models", 1)
+        if not 0 <= model < n_models:
+            raise ValueError("model must be in [0, %d) (got %d)" % (n_models, model))
+        self._L = _lib.lib()
+        rule = _lib.MwwEndpointRule(vad_window, steps["speech_steps"], steps["silence_steps"], steps["timeout_steps"], steps["max_steps"],
+                                    lookback_steps, float(vad_cutoff))
+        ep = ctypes.c_void_p()
+        self._check(self._L.mww_endpointer_create(engine._h, model, ctypes.byref(rule), capacity, ctypes.byref(ep)))
+        self._handle = _EndpointerHandle(self._L, ep.value)
+        self.engine, self.model, self.device, self.capacity = engine, model, int(engine.device), capacity
+        self.vad_window, self.vad_cutoff, self.lookback_steps = vad_window, float(vad_cutoff), lookback_steps
+        self.speech_steps, self.silence_steps = steps["speech_steps"], steps["silence_steps"]
+        self.timeout_steps, self.max_steps = steps["timeout_steps"], steps["max_steps"]
+        desc = self._desc()
+        self.n_rows, self.stride, self.hop = int(desc.n_rows), int(desc.stride), int(desc.hop_samples)
+        count, ended, armed = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+        self._check(self._L.mww_endpointer_buffers(self._ep, ctypes.byref(count), None, ctypes.byref(ended), ctypes.byref(armed), None))
+        import torch
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(dev):
+            # device views: the stream of each used event slot (-1 elsewhere), every row's stream while armed (-1 elsewhere),
+            # and how many commands ended since the last drain
+            self.ended_ids = torch.as_tensor(_DeviceArray(self._handle, ended.value, capacity, "<i4"), device=dev)
+            self.armed_ids = torch.as_tensor(_DeviceArray(self._handle, armed.value, max(self.n_rows, 1), "<i4"), device=dev)[:self.n_rows]
+            self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
+
+    @property
+    def _ep(self):
+        return self._handle.ptr
+
+    def _check(self, rc: int) -> None:
+        if rc != 0:
+            msg = self._L.mww_last_error(None)
+            raise _lib.MwwError(rc, msg.decode() if msg else "endpointer call failed")
+
+    def _desc(self) -> "_lib.MwwEndpointerDesc":
+        out = _lib.MwwEndpointerDesc()
+        self._check(self._L.mww_endpointer_info(self._ep, ctypes.byref(out)))
+        return out
+
+    @property
+    def launch_count(self) -> int:
+        """kernel launches of this endpointer since create: one per update, arm, disarm, reset and commands call"""
+        return int(self._desc().launches)
+
+    def _stream(self):
+        import torch
+        return ctypes.c_void_p(torch.cuda.current_stream(torch.device("cuda", self.device)).cuda_stream)
+
+    def close(self) -> None:
+        """free the endpointer now; armed_ids, ended_ids and event_count must not be used afterwards"""
+        self._handle.close()
+
+    def update(self, probs) -> None:
+        """The model's probabilities of the engine call just made: a StreamEngine result, or probs[model] of a MultiModelEngine
+        result (CUDA float32 [n_rows, steps], any row pitch).  Call it after every engine call, steps or none: the endpointer
+        places the steps on the history axis from the engine's counters and refuses an update that does not match them.
+        Asynchronous on the current CUDA stream."""
+        import torch
+        if (not isinstance(probs, torch.Tensor) or not probs.is_cuda or probs.dtype != torch.float32 or probs.dim() != 2
+                or probs.shape[0] != self.n_rows or probs.device.index != self.device):
+            raise ValueError("probs must be a CUDA float32 tensor [n_rows=%d, steps] on cuda:%d" % (self.n_rows, self.device))
+        n = probs.shape[1]
+        if n and ((n > 1 and probs.stride(1) != 1) or (self.n_rows > 1 and probs.stride(0) < n)):
+            probs = probs.contiguous()
+        pitch = probs.stride(0) if self.n_rows > 1 else n
+        self._check(self._L.mww_endpointer_update(self._ep, probs.data_ptr() if n and self.n_rows else None, n, pitch, self._stream()))
+
+    def _ids_call(self, ids, host_fn: str, device_fn, allow_all: bool = False) -> None:
+        """the host call `host_fn` or the device call `device_fn` (names; None: host ids only) on a checked id list"""
+        import torch
+        if ids is None and allow_all:
+            self._check(getattr(self._L, host_fn)(self._ep, None, 0, self._stream()))
+        elif isinstance(ids, torch.Tensor) and ids.is_cuda:
+            if device_fn is None:
+                raise ValueError("this call takes host stream ids")
+            if ids.dtype != torch.int32 or ids.dim() != 1 or not ids.is_contiguous() or ids.device.index != self.device:
+                raise ValueError("device stream ids must be a contiguous 1-D CUDA int32 tensor on cuda:%d" % self.device)
+            self._check(getattr(self._L, device_fn)(self._ep, ids.data_ptr(), ids.numel(), self._stream()))
+        else:
+            a = _record_ids(ids, "stream ids")
+            if a.size and (a.min() < 0 or a.max() >= self.engine.n_streams):
+                raise ValueError("stream ids must be in [0, %d)" % self.engine.n_streams)
+            self._check(getattr(self._L, host_fn)(self._ep, a.ctypes.data, a.size, self._stream()))
+
+    def arm(self, ids) -> None:
+        """Start a command on the listed GLOBAL stream ids: a host sequence, or a contiguous 1-D CUDA int32 tensor such as a
+        verifier's confirmed ids or a detector's fired_ids, whose -1 slots (and ids outside the model's stream set) are
+        ignored.  Re-arming restarts a row; the last lookback_steps flags are replayed."""
+        self._ids_call(ids, "mww_endpointer_arm", "mww_endpointer_arm_device")
+
+    def disarm(self, ids) -> None:
+        """Cancel the listed streams' commands without an event (host ids)"""
+        self._ids_call(ids, "mww_endpointer_disarm", None)
+
+    def reset(self, ids=None) -> None:
+        """Fresh VAD and segmenter state for all rows (None: also takes the engine's counters as the new baseline, the call to
+        make after engine.reset() or reset_frontend()) or the listed GLOBAL stream ids (host, or CUDA int32 such as
+        ended_ids): call it with the ids the engine resets."""
+        self._ids_call(ids, "mww_endpointer_reset", "mww_endpointer_reset_device", allow_all=True)
+
+    def commands(self, pre: int = 0, post: int = 0, max_samples: int = 160000, out=None, lengths=None):
+        """-> (clips, lengths): CUDA int16 [capacity, max_samples] and int32 [capacity].  Row i is event slot i's command,
+        samples [start_sample - pre, end) of its stream's history with end = min(speech_end_sample + post, end_sample) for
+        END_OF_SPEECH and end_sample otherwise, capped at max_samples; zeros outside the ring and past the length, and
+        length 0 in unused slots.  Call it before drain() and before the streams are reset.  Ordered on the current CUDA
+        stream, one launch, no host synchronisation."""
+        import torch
+        pre, post, max_samples = _int(pre, "pre"), _int(post, "post"), _int(max_samples, "max_samples")
+        if pre < 0 or post < 0:
+            raise ValueError("pre and post must not be negative")
+        if not 0 <= max_samples <= MAX_AUDIO_HISTORY:
+            raise ValueError("max_samples must be in [0, %d] (got %d)" % (MAX_AUDIO_HISTORY, max_samples))
+        dev = torch.device("cuda", self.device)
+        if out is None:
+            out = torch.empty((self.capacity, max_samples), dtype=torch.int16, device=dev)
+        elif (not isinstance(out, torch.Tensor) or out.dtype != torch.int16 or out.device != dev or out.dim() != 2
+              or out.shape[0] != self.capacity or out.shape[1] < max_samples or (out.shape[1] > 1 and out.stride(1) != 1)):
+            raise ValueError("out must be a CUDA int16 tensor [capacity=%d, >= %d] with contiguous rows on %s" % (self.capacity, max_samples, dev))
+        if lengths is None:
+            lengths = torch.empty(self.capacity, dtype=torch.int32, device=dev)
+        elif (not isinstance(lengths, torch.Tensor) or lengths.dtype != torch.int32 or lengths.device != dev
+              or lengths.shape != (self.capacity,) or not lengths.is_contiguous()):
+            raise ValueError("lengths must be a contiguous CUDA int32 tensor [capacity=%d] on %s" % (self.capacity, dev))
+        stride = out.stride(0) if self.capacity > 1 else max(out.shape[1], max_samples)
+        self._check(self._L.mww_endpointer_read_commands(self._ep, self.engine._h, pre, post, max_samples, out.data_ptr(), stride,
+                                                         lengths.data_ptr(), self._stream()))
+        return out[:, :max_samples], lengths
+
+    def _drain_slots(self):
+        buf = np.zeros(self.capacity, ENDPOINT_EVENT_DTYPE)
+        n = ctypes.c_longlong(0)
+        self._check(self._L.mww_endpointer_drain(self._ep, buf.ctypes.data, self.capacity, ctypes.byref(n), self._stream()))
+        return buf[:min(n.value, self.capacity)], n.value
+
+    def drain(self):
+        """-> (events, dropped): the commands that ended since the last drain (ENDPOINT_EVENT_DTYPE) sorted by (end_sample,
+        stream), and how many more ended than `capacity` could hold.  Waits for the current CUDA stream; clears the event
+        buffer and ended_ids."""
+        ev, n = self._drain_slots()
+        return ev[np.lexsort((ev["stream"], ev["end_sample"]))], max(n - self.capacity, 0)
+
+    _ROW_FIELDS = (("seen", np.int64), ("flags", np.uint64), ("armed", np.int32), ("elapsed", np.int32), ("run", np.int32),
+                   ("silence", np.int32), ("heard", np.int32), ("start_sample", np.int64), ("speech_end_sample", np.int64))
+
+    def state_dict(self) -> dict:
+        """every row's state (hist [n_rows, vad_window - 1] oldest first, seen, flags, armed, elapsed, run, silence, heard,
+        start_sample, speech_end_sample) and the baseline (samples_seen, buffered, pending), steps and positions [64].
+        Synchronous."""
+        d = {"hist": np.zeros((self.n_rows, self.vad_window - 1), np.float32)}
+        d.update({k: np.zeros(self.n_rows, t) for k, t in self._ROW_FIELDS})
+        st = _lib.MwwEndpointState()
+        st.hist = d["hist"].ctypes.data if d["hist"].size else None
+        for k, _ in self._ROW_FIELDS:
+            setattr(st, k, d[k].ctypes.data if self.n_rows else None)
+        self._check(self._L.mww_endpointer_get_state(self._ep, ctypes.byref(st)))
+        for k in ("samples_seen", "buffered", "pending", "steps"):
+            d[k] = int(getattr(st, k))
+        d["positions"] = np.ctypeslib.as_array(st.positions).copy()
+        return d
+
+    def load_state_dict(self, d: dict) -> None:
+        """the inverse of state_dict (synchronous); refusals as mww_endpointer_set_state"""
+        hist = np.ascontiguousarray(d["hist"], np.float32)
+        rows = {k: np.ascontiguousarray(d[k], t) for k, t in self._ROW_FIELDS}
+        if hist.shape != (self.n_rows, self.vad_window - 1) or any(a.shape != (self.n_rows,) for a in rows.values()):
+            raise ValueError("state arrays must have the endpointer's shapes")
+        pos = np.ascontiguousarray(d["positions"], np.int64)
+        if pos.shape != (64,):
+            raise ValueError("positions must hold 64 entries")
+        st = _lib.MwwEndpointState()
+        st.hist = hist.ctypes.data if hist.size else None
+        for k, a in rows.items():
+            setattr(st, k, a.ctypes.data if a.size else None)
+        for k in ("samples_seen", "buffered", "pending", "steps"):
+            setattr(st, k, int(d[k]))
+        np.ctypeslib.as_array(st.positions)[:] = pos
+        self._check(self._L.mww_endpointer_set_state(self._ep, ctypes.byref(st)))
