@@ -477,7 +477,8 @@ int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_reco
  *     _f32, _g711).  mww_infer_features takes rows, not audio, and appends nothing.
  *   - Every call that zeroes a stream's window carry zeroes its history too: mww_reset (all or by id),
  *     mww_reset_device_ids and mww_reset_frontend.  mww_import_streams zeroes the history of the streams it writes (records
- *     do not carry it; their layout is unchanged).  mww_set_audio_history zeroes every stream.  Nothing else touches it:
+ *     do not carry it; their layout is unchanged; mww_write_audio_history after the import carries it).
+ *     mww_set_audio_history zeroes every stream.  Nothing else touches it:
  *     not mww_set_state, mww_set_stream_rates, mww_set_model_streams or mww_set_window_step.
  *   - So after audio calls alone since the last zeroing, a stream's last frontend_buffered history samples equal
  *     carry[0, frontend_buffered) of mww_get_state whenever C >= frontend_buffered.
@@ -494,12 +495,27 @@ int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_reco
  * ids out of range are MWW_EINVAL (as mww_reset); device ids that are negative or >= n_streams give a zero row, which covers
  * the -1 slots of a detector's d_fired.  MWW_EINVAL before any device work when the handle keeps no history, n < 0,
  * n_samples is outside [0, C], out_stride < n_samples, or a buffer is NULL with work to do.  A poisoned handle refuses
- * set and read. */
+ * set and read.
+ * mww_write_audio_history: the inverse of the read, to carry a stream's history when it moves to another handle (read it on
+ * the source, import the stream records, then write it on the destination).  After the call, stream ids[i]'s history is an
+ * endless run of zeros followed by row i of d_in, n_samples long, oldest first: as if the history had been zeroed and those
+ * samples appended, with samples_seen unchanged.  So sample t of the row sits at axis position samples_seen - n_samples + t,
+ * in slot pos mod C of the ring, and only the last min(n_samples, C) samples can be read back.  Every other stream keeps
+ * every byte.  mww_import_streams zeroes the history of the streams it writes, so write AFTER the import.  d_in is
+ * [n][in_stride] int16 in memory the handle's GPU can address (peer memory from mww_ipc_open included); ids come from host
+ * memory.  Asynchronous on cu_stream, one launch counted in mww_launch_count whatever n is; n == 0 launches nothing.
+ * MWW_EINVAL before any device work when the handle keeps no history, n < 0, n_samples is outside [0, 2^22], in_stride <
+ * n_samples, a buffer is NULL with work to do (ids with n > 0, d_in with n > 0 and n_samples > 0), or an id is out of range
+ * or listed twice.  A poisoned handle refuses the call.  At 12 s of history a stream carries 384 kB: move many streams in
+ * batches of ids, or carry only the samples still needed (what a verifier hears, the endpointer's lookback and the commands
+ * in progress). */
 int mww_set_audio_history(mww_t *h, int capacity, void *cu_stream);
 int mww_get_audio_history(const mww_t *h, int *capacity, long long *samples_seen);
 int mww_read_audio_history(mww_t *h, const int32_t *h_ids, int n, int n_samples, int16_t *d_out, long long out_stride, void *cu_stream);
 int mww_read_audio_history_device_ids(mww_t *h, const int32_t *d_ids, int n, int n_samples, int16_t *d_out, long long out_stride,
                                       void *cu_stream);
+int mww_write_audio_history(mww_t *h, const int32_t *h_ids, int n, int n_samples, const int16_t *d_in, long long in_stride,
+                            void *cu_stream);
 
 /* ---- detection post-processing (microwakeword/test.py:337-341, :94-137, :364-373) -------------------------
  * Tracks are ragged: track i is d_probs[d_offsets[i] .. d_offsets[i] + d_lengths[i]) (float32 probabilities as
@@ -971,6 +987,59 @@ int mww_endpointer_get_state(mww_endpointer_t *ep, mww_endpoint_state *out);
 int mww_endpointer_set_state(mww_endpointer_t *ep, const mww_endpoint_state *in);
 int mww_endpointer_read_commands(mww_endpointer_t *ep, mww_t *h, long long pre, long long post, int max_samples, int16_t *d_out,
                                  long long out_stride, int32_t *d_lengths, void *cu_stream);
+
+/* ---- moving endpointer rows: export and import as packed records ----------------------------------------------------------
+ * When a server moves streams to another handle (mww_export_streams, mww_export_detector_rows, mww_write_audio_history), a
+ * stream that is speaking a command keeps it: its endpointer row moves as a packed device record, and the command ends with
+ * the same event and the same clip as if the stream had stayed, with positions on the destination's axis.
+ *   - Ids.  Both calls take GLOBAL stream ids of the endpointer's handle from host memory, as arm and reset do.  ids[i] on
+ *     import may differ from the id record i was exported from, so streams can be renumbered.
+ *   - One record, record_bytes long, every part padded to 16 bytes:
+ *         int32   member, armed, 0, 0                   member of the stream set; armed (the segmenter state follows)
+ *         int32   elapsed, run, silence, heard          zero unless armed
+ *         int64   seen; uint64 flags                    VAD count and the last 64 speech flags
+ *         int64   start_age, speech_end_age             S' - start_sample, S' - speech_end_sample; zero unless armed
+ *         float32 hist[vad_window - 1]                  oldest first (no bytes when vad_window = 1)
+ *     with S' the exporter's baseline samples_seen (its handle's counter at the endpointer's last update or whole reset).  A
+ *     rule of vad_window 5 has 80-byte records: 16 + 16 + 16 + 16 + 16 (4 floats).
+ *   - mww_endpointer_layout: record_bytes, vad_window, stride, hop_samples and the baseline buffered and pending rows that
+ *     import checks, and the exporter's baseline samples_seen and steps, for information.  mww_get_endpointer_layout fills
+ *     it without device work; export fills it too (out may be NULL).
+ *   - export writes one record per listed id (an id may appear twice): an id that is not a member of the model's stream set
+ *     gets a zero record (member = 0), an unarmed row a zero segmenter.  The endpointer does not change.
+ *   - import, per listed id: a non-member of the destination's set ignores the record; a member whose record has member = 0
+ *     gets what reset(ids) gives; a member whose record has member = 1 takes the record, with armed = the destination's
+ *     global id when the record is armed, and positions rebased to S'_dst - age.  arm_tag is not carried (each row keeps its
+ *     own).  Rows that are not listed keep every byte.  Events and d_ended do not move: drain the source first.
+ *   - Time axis.  Export and import are refused unless the endpointer is up to date with its handle: the handle's
+ *     samples_seen, frontend_buffered and model k's pending rows equal the endpointer's baseline (update the endpointer after
+ *     the handle's last call).  Import is refused when the records' vad_window, stride, hop_samples, buffered, pending or
+ *     record_bytes differ from the destination's; the message names the field.  Equal buffered and pending rows make a
+ *     step's age the same on both axes; two handles serving 480-sample live calls always meet it.  Other rule fields may
+ *     differ, and the row continues under the destination's rule.
+ *   - Positions after the move may be negative, when the destination's axis is younger than the moved command.  The command
+ *     read already handles that: it writes zeros only outside [samples_seen - C, samples_seen), and a history written with
+ *     mww_write_audio_history puts the moved samples at the matching positions.
+ *   - Replay limit.  A moved row's flags carry verbatim, but an arm after the move replays at most min(lookback_steps, steps
+ *     the DESTINATION endpointer consumed since create or its last whole reset), as for every row there.  For a full-depth
+ *     replay of a stream moved between its detection and its arm, update the destination endpointer for at least
+ *     lookback_steps calls before the move (it can run on the destination handle's idle streams).
+ *   - Both calls are asynchronous and ordered on cu_stream, with records [n][record_bytes] in memory the endpointer's GPU
+ *     can address, 16-byte aligned.  One launch each whatever n is; n == 0 launches nothing and still fills / checks the
+ *     layout.  The id list is staged in a buffer the endpointer owns, so calls on one endpointer from different CUDA streams
+ *     must be ordered by the caller.
+ *   - MWW_EINVAL before any device work, with the endpointer unchanged: a NULL endpointer, the conditions above, n < 0, NULL
+ *     or misaligned records with n > 0, a NULL layout on import, an id out of range, an id listed twice on import. */
+typedef struct mww_endpointer_layout {
+    int64_t record_bytes;
+    int32_t vad_window, stride, hop_samples, buffered, pending, pad;
+    int64_t samples_seen, steps;      /* the exporter's baseline, for information */
+} mww_endpointer_layout;
+int mww_get_endpointer_layout(const mww_endpointer_t *ep, mww_endpointer_layout *out);
+int mww_export_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n, void *d_records, mww_endpointer_layout *out,
+                               void *cu_stream);
+int mww_import_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n, const void *d_records,
+                               const mww_endpointer_layout *layout, void *cu_stream);
 
 #ifdef __cplusplus
 }

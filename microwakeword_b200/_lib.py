@@ -46,6 +46,7 @@ EXPORTS = (
     "mww_endpointer_arm_device", "mww_endpointer_disarm", "mww_endpointer_reset", "mww_endpointer_reset_device",
     "mww_endpointer_drain", "mww_endpointer_buffers", "mww_endpointer_get_state", "mww_endpointer_set_state",
     "mww_endpointer_read_commands",
+    "mww_write_audio_history", "mww_get_endpointer_layout", "mww_export_endpointer_rows", "mww_import_endpointer_rows",
 )
 
 
@@ -135,6 +136,13 @@ class MwwEndpointState(ctypes.Structure):
                 ("elapsed", ctypes.c_void_p), ("run", ctypes.c_void_p), ("silence", ctypes.c_void_p), ("heard", ctypes.c_void_p),
                 ("start_sample", ctypes.c_void_p), ("speech_end_sample", ctypes.c_void_p), ("samples_seen", ctypes.c_int64),
                 ("buffered", ctypes.c_int64), ("pending", ctypes.c_int64), ("steps", ctypes.c_int64), ("positions", ctypes.c_int64 * 64)]
+
+
+class MwwEndpointerLayout(ctypes.Structure):
+    """mww_endpointer_layout of include/mww.h: what travels beside exported endpointer records"""
+    _fields_ = [("record_bytes", ctypes.c_int64), ("vad_window", ctypes.c_int32), ("stride", ctypes.c_int32),
+                ("hop_samples", ctypes.c_int32), ("buffered", ctypes.c_int32), ("pending", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("samples_seen", ctypes.c_int64), ("steps", ctypes.c_int64)]
 
 
 class MwwError(RuntimeError):
@@ -358,6 +366,13 @@ def lib() -> ctypes.CDLL:
     L.mww_endpointer_set_state.argtypes = [vp, ctypes.POINTER(MwwEndpointState)]
     L.mww_endpointer_read_commands.restype = i32
     L.mww_endpointer_read_commands.argtypes = [vp, vp, ll, ll, i32, vp, ll, vp, vp]
+    L.mww_write_audio_history.restype = i32
+    L.mww_write_audio_history.argtypes = [vp, vp, i32, i32, vp, ll, vp]
+    L.mww_get_endpointer_layout.restype = i32
+    L.mww_get_endpointer_layout.argtypes = [vp, ctypes.POINTER(MwwEndpointerLayout)]
+    for name in ("mww_export_endpointer_rows", "mww_import_endpointer_rows"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwEndpointerLayout), vp]
     _lib = L
     return L
 

@@ -47,6 +47,11 @@ VER_SOURCES = ["mww_verify.cu"]
 # and the endpointer's four kernels (mww_endpointer_*), likewise
 EP_OUT = os.path.join(HERE, "libmww_endpoint.so")
 EP_SOURCES = ["mww_endpoint.cu"]
+# and the kernels that move a stream's serving state between handles: the audio history write (mww_write_audio_history) and
+# the endpointer records (mww_export_endpointer_rows / mww_import_endpointer_rows), so that libmww_history.so and
+# libmww_endpoint.so keep exactly the kernels they had
+SR_OUT = os.path.join(HERE, "libmww_serving_records.so")
+SR_SOURCES = ["mww_serving_records.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -69,7 +74,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -90,10 +95,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
         for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (RR_OUT, RR_SOURCES, []), (DET_OUT, DET_SOURCES, []),
                                     (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []), (G711_OUT, G711_SOURCES, []),
                                     (HIST_OUT, HIST_SOURCES, []), (DR_OUT, DR_SOURCES, []), (VER_OUT, VER_SOURCES, []),
-                                    (EP_OUT, EP_SOURCES, []),
+                                    (EP_OUT, EP_SOURCES, []), (SR_OUT, SR_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
                                                     "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711", "-lmww_history",
-                                                    "-lmww_detector_records", "-lmww_verify", "-lmww_endpoint",
+                                                    "-lmww_detector_records", "-lmww_verify", "-lmww_endpoint", "-lmww_serving_records",
                                                     "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra

@@ -2196,4 +2196,26 @@ int mww_read_audio_history_device_ids(mww_t *h, const int32_t *d_ids, int n, int
     return read_history(h, d_ids, n, n_samples, d_out, out_stride, static_cast<cudaStream_t>(cu_stream));
 }
 
+int mww_write_audio_history(mww_t *h, const int32_t *h_ids, int n, int n_samples, const int16_t *d_in, long long in_stride, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    const char *who = "mww_write_audio_history";
+    if (!h->d_hist) return fail(h, MWW_EINVAL, std::string(who) + ": the handle keeps no audio history (mww_set_audio_history)");
+    if (n < 0 || n_samples < 0 || n_samples > kHistoryMaxCapacity || in_stride < n_samples)
+        return fail(h, MWW_EINVAL, std::string(who) + ": needs n >= 0, 0 <= n_samples <= 2^22 and in_stride >= n_samples");
+    if (n > 0 && (!h_ids || (n_samples > 0 && !d_in))) return fail(h, MWW_EINVAL, std::string(who) + ": NULL ids or input");
+    std::vector<uint8_t> listed((size_t)h->n_streams, 0);
+    for (int i = 0; i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= h->n_streams) return fail(h, MWW_EINVAL, std::string(who) + ": stream id out of range");
+        if (listed[(size_t)h_ids[i]]) return fail(h, MWW_EINVAL, std::string(who) + ": a stream id is listed twice");
+        listed[(size_t)h_ids[i]] = 1;
+    }
+    ENTER_STATEFUL(h);
+    if (n == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+    CU(h, launch_history_write(h->d_hist, h->hist_cap, h->hist_seen, h->d_ids, n, n_samples, d_in, in_stride, h->sm_count, st));
+    h->launches += 1;
+    return MWW_OK;
+}
+
 }  // extern "C"

@@ -19,6 +19,8 @@ struct mww_endpointer {
     std::vector<int32_t> members;         // row -> global id
     std::vector<int32_t> row_of;          // global id -> row, -1 for a non-member
     int32_t *d_ids = nullptr;             // [n_rows] a host id list, filtered to members without repeats
+    int32_t *d_rec_ids = nullptr;         // [rec_ids_cap] the id list of a record call, as given
+    size_t rec_ids_cap = 0;
     long long launches = 0;
     int tag = 0;                          // arm calls so far
     // the handle's counters after the last update or whole reset, the steps consumed since then and their last positions
@@ -37,7 +39,7 @@ void endpointer_free(mww_endpointer_t *ep) {
     EndpointArgs &a = ep->a;
     cudaFree(a.hist); cudaFree(a.seen); cudaFree(a.flags); cudaFree(a.armed); cudaFree(a.elapsed); cudaFree(a.run); cudaFree(a.silence);
     cudaFree(a.heard); cudaFree(a.start); cudaFree(a.speech_end); cudaFree(a.arm_tag); cudaFree((void *)a.row_of); cudaFree(a.count);
-    cudaFree(a.events); cudaFree(a.ended); cudaFree(ep->d_ids);
+    cudaFree(a.events); cudaFree(a.ended); cudaFree(ep->d_ids); cudaFree(ep->d_rec_ids);
     delete ep;
 }
 
@@ -124,6 +126,54 @@ int clear(mww_endpointer_t *ep, const int32_t *d_ids, int n, int reset, cudaStre
     ECU(launch_endpoint_clear(ep->a, d_ids, n, reset, st));
     ep->launches += 1;
     return MWW_OK;
+}
+
+// ---- endpointer records (layout and per-row bodies: mww_serving_records.h) ----
+void fill_layout(const mww_endpointer_t *ep, mww_endpointer_layout *out) {
+    *out = mww_endpointer_layout{};
+    out->record_bytes = endpoint_record_layout(ep->a.rule.vad_window).record_bytes;
+    out->vad_window = ep->a.rule.vad_window; out->stride = ep->stride; out->hop_samples = ep->hop;
+    out->buffered = ep->base_buffered; out->pending = ep->base_pending;
+    out->samples_seen = ep->base_seen; out->steps = ep->steps;
+}
+
+// the checks export and import share, before any device work: arguments, ids in range (and, on import, listed once) and an
+// endpointer that is up to date with its handle
+int check_record_call(mww_endpointer_t *ep, const std::string &call, const int32_t *h_ids, int n, const void *d_records, bool once) {
+    if (n < 0 || (n > 0 && (!h_ids || !d_records))) return refuse(call + "needs n >= 0, and ids and records with n > 0");
+    if (reinterpret_cast<uintptr_t>(d_records) % 16 != 0) return refuse(call + "the records must be 16-byte aligned");
+    std::vector<uint8_t> listed(once ? (size_t)ep->n_streams : 0, 0);
+    for (int i = 0; i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= ep->n_streams)
+            return refuse(call + "stream id " + std::to_string(h_ids[i]) + " out of range [0, " + std::to_string(ep->n_streams) + ")");
+        if (once && listed[(size_t)h_ids[i]]++) return refuse(call + "stream id " + std::to_string(h_ids[i]) + " is listed twice");
+    }
+    long long S = 0;
+    int buffered = 0, pending = 0;
+    if (int rc = read_counters(ep, &S, &buffered, &pending)) return rc;
+    if (S != ep->base_seen || buffered != ep->base_buffered || pending != ep->base_pending)
+        return refuse(call + "the endpointer is behind its handle's counters: update the endpointer after the handle's last call");
+    return MWW_OK;
+}
+
+// a host id list -> d_rec_ids, on st; growing the buffer first waits for the call that may still read it
+int stage_record_ids(mww_endpointer_t *ep, const int32_t *h_ids, int n, cudaStream_t st) {
+    if ((size_t)n > ep->rec_ids_cap) {
+        if (ep->d_rec_ids) { ECU(cudaStreamSynchronize(st)); cudaFree(ep->d_rec_ids); ep->d_rec_ids = nullptr; ep->rec_ids_cap = 0; }
+        const size_t want = std::max<size_t>((size_t)n, 1024);
+        ECU(cudaMalloc(&ep->d_rec_ids, want * sizeof(int32_t)));
+        ep->rec_ids_cap = want;
+    }
+    ECU(cudaMemcpyAsync(ep->d_rec_ids, h_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return MWW_OK;
+}
+
+EpRecJob record_job(const mww_endpointer_t *ep) {
+    EpRecJob J;
+    J.a = ep->a;
+    J.base = ep->base_seen;
+    J.L = endpoint_record_layout(ep->a.rule.vad_window);
+    return J;
 }
 
 }  // namespace
@@ -371,6 +421,47 @@ int mww_endpointer_read_commands(mww_endpointer_t *ep, mww_t *h, long long pre, 
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
     ECU(launch_endpoint_read(ring.ring, ring.capacity, ring.seen, ep->a.count, ep->a.events, ep->capacity, pre, post, max_samples, d_out,
                              out_stride, d_lengths, ring.sm_count, static_cast<cudaStream_t>(cu_stream)));
+    ep->launches += 1;
+    return MWW_OK;
+}
+
+int mww_get_endpointer_layout(const mww_endpointer_t *ep, mww_endpointer_layout *out) {
+    if (!ep || !out) return refuse("mww_get_endpointer_layout: needs an endpointer and out");
+    fill_layout(ep, out);
+    return MWW_OK;
+}
+
+int mww_export_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n, void *d_records, mww_endpointer_layout *out, void *cu_stream) {
+    const std::string call = "mww_export_endpointer_rows: ";
+    if (!ep) return refuse(call + "endpointer is NULL");
+    if (int rc = check_record_call(ep, call, h_ids, n, d_records, false)) return rc;
+    if (out) fill_layout(ep, out);
+    if (n == 0) return MWW_OK;
+    DeviceGuard guard(ep->device);
+    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = stage_record_ids(ep, h_ids, n, st)) return rc;
+    ECU(launch_pack_endpointer_rows(record_job(ep), d_records, ep->d_rec_ids, n, st));
+    ep->launches += 1;
+    return MWW_OK;
+}
+
+int mww_import_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n, const void *d_records, const mww_endpointer_layout *layout,
+                               void *cu_stream) {
+    const std::string call = "mww_import_endpointer_rows: ";
+    if (!ep) return refuse(call + "endpointer is NULL");
+    if (!layout) return refuse(call + "layout is NULL");
+    if (int rc = check_record_call(ep, call, h_ids, n, d_records, true)) return rc;
+    mww_endpointer_layout mine;
+    fill_layout(ep, &mine);
+    if (const char *field = endpoint_layout_mismatch(*layout, mine))
+        return refuse(call + "the records' " + field + " differs from the endpointer's");
+    if (n == 0) return MWW_OK;
+    DeviceGuard guard(ep->device);
+    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = stage_record_ids(ep, h_ids, n, st)) return rc;
+    ECU(launch_unpack_endpointer_rows(record_job(ep), d_records, ep->d_rec_ids, n, st));
     ep->launches += 1;
     return MWW_OK;
 }

@@ -1,5 +1,6 @@
 // mww_history.h -- the audio history of a handle (mww_set_audio_history, rule in include/mww.h): a ring of the last C 16 kHz
-// int16 samples of every stream, and the index math of the two kernels that fill and read it (mww_history.cu).
+// int16 samples of every stream, and the index math of the two kernels that fill and read it (mww_history.cu) and of the
+// kernel that writes whole rows (mww_write_audio_history, mww_serving_records.cu).
 //
 // All streams advance in lockstep, so one counter, `seen` (16 kHz samples appended since the history was enabled), places
 // every stream's ring: sample t of the run since enabling lives in slot t mod C of its stream's row.  A zeroed row reads as
@@ -68,6 +69,32 @@ MWW_HD void history_append_one(int16_t *ring_row, const T *audio_row, const Hist
 MWW_HD int16_t history_read_one(const int16_t *ring, int C, int id, int n_streams, int slot0, int k) {
     if (id < 0 || id >= n_streams) return 0;
     return ring[(long long)id * C + history_slot(slot0, k, C)];
+}
+
+// ---- the write (mww_write_audio_history; kernel in mww_serving_records.cu) ------------------------------------------------------
+// A row of n samples written after `seen`: the stream's history becomes zeros followed by the row, so sample t of the row sits
+// at axis position seen - n + t.  The ring holds positions [seen - C, seen); entry e (oldest first) of that window is
+// position seen - C + e in slot history_slot(slot0, e, C), and holds row sample e - lead when that is >= 0, else zero.
+// lead = C - n is negative when n > C: only the row's last C samples land.  Every entry of the row is written.
+struct HistoryWrite {
+    long long lead;
+    int slot0;          // seen mod C
+};
+MWW_HD HistoryWrite history_write_plan(long long seen, int n, int C) {
+    HistoryWrite p;
+    p.lead = (long long)C - n;
+    p.slot0 = history_mod(seen, C);
+    return p;
+}
+// 8-entry units when every unit starts on a multiple of 8 in the ring and in the caller's row, so a unit is all zeros or all
+// row samples; the launcher adds the 16-byte alignment of the caller's buffer
+MWW_HD bool history_write_vec_shape(const HistoryWrite &p, long long in_stride) {
+    return p.slot0 % 8 == 0 && p.lead % 8 == 0 && in_stride % 8 == 0;
+}
+// write: entry e of one stream's ring row from its row of the caller's samples
+MWW_HD void history_write_one(int16_t *ring_row, const int16_t *in_row, const HistoryWrite &p, int e, int C) {
+    const long long t = (long long)e - p.lead;
+    ring_row[history_slot(p.slot0, e, C)] = t >= 0 ? in_row[t] : (int16_t)0;
 }
 
 }  // namespace mww

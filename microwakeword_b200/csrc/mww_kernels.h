@@ -210,3 +210,16 @@ cudaError_t launch_endpoint_read(const int16_t *ring, int C, long long seen, con
                                  int capacity, long long pre, long long post, int max_samples, int16_t *out, long long out_stride,
                                  int32_t *lengths, int sm_count, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_serving_records.h"
+namespace mww {
+// moving a stream's serving state (mww_serving_records.cu, index math in mww_history.h, record layout and per-row bodies in
+// mww_serving_records.h; companion library libmww_serving_records.so), one launch each.
+// ring rows ids[i] (device memory, in range, distinct) of ring [n_streams][C] <- zeros followed by the n_samples of row i of
+// in [n][in_stride], `seen` samples appended
+cudaError_t launch_history_write(int16_t *ring, int C, long long seen, const int32_t *ids, int n, int n_samples, const int16_t *in,
+                                 long long in_stride, int sm_count, cudaStream_t st);
+// the records [n][J.L.record_bytes] of the n listed global ids (device memory, in range) out of and into the endpointer J
+cudaError_t launch_pack_endpointer_rows(const EpRecJob &J, void *records, const int32_t *ids, int n, cudaStream_t st);
+cudaError_t launch_unpack_endpointer_rows(const EpRecJob &J, const void *records, const int32_t *ids, int n, cudaStream_t st);
+}  // namespace mww

@@ -39,6 +39,32 @@ def _int(value, name: str) -> int:
     return int(value)
 
 
+class EndpointerRecords:
+    """Endpointer rows exported from an Endpointer (export_streams): `data`, torch.uint8 [n, record_bytes] on the
+    endpointer's device, one packed record per listed stream (include/mww.h, "moving endpointer rows"), and `layout`, the
+    _lib.MwwEndpointerLayout an importing endpointer must share.  Positions travel as ages from the exporter's baseline, so
+    they land on the importer's axis.  The records carry no events."""
+
+    _FIELDS = ("record_bytes", "vad_window", "stride", "hop_samples", "buffered", "pending", "pad", "samples_seen", "steps")
+
+    def __init__(self, data, layout):
+        self.data, self.layout = data, layout
+
+    def save(self, path) -> None:
+        """np.savez of the records and the layout's fields: a checkpoint of some streams' endpointer rows"""
+        np.savez(path, data=self.data.cpu().numpy(), **{k: np.asarray(getattr(self.layout, k)) for k in self._FIELDS})
+
+    @classmethod
+    def load(cls, path, device) -> "EndpointerRecords":
+        import torch
+        layout = _lib.MwwEndpointerLayout()
+        with np.load(path) as z:
+            for k in cls._FIELDS:
+                setattr(layout, k, int(z[k]))
+            data = torch.from_numpy(z["data"]).to(device)
+        return cls(data, layout)
+
+
 class _EndpointerHandle(_DetectorHandle):
     """owner of one mww_endpointer_t: destroyed when the endpointer and every tensor over its buffers are gone"""
 
@@ -229,6 +255,52 @@ class Endpointer:
         buffer and ended_ids."""
         ev, n = self._drain_slots()
         return ev[np.lexsort((ev["stream"], ev["end_sample"]))], max(n - self.capacity, 0)
+
+    def layout(self) -> "_lib.MwwEndpointerLayout":
+        """record size, rule window, stride, hop and baseline (mww_get_endpointer_layout; no device work)"""
+        out = _lib.MwwEndpointerLayout()
+        self._check(self._L.mww_get_endpointer_layout(self._ep, ctypes.byref(out)))
+        return out
+
+    def _record_ids(self, stream_ids) -> np.ndarray:
+        a = _record_ids(stream_ids, "stream ids")
+        if a.size and (a.min() < 0 or a.max() >= self.engine.n_streams):
+            raise ValueError("stream ids must be in [0, %d)" % self.engine.n_streams)
+        return a
+
+    def export_streams(self, stream_ids) -> EndpointerRecords:
+        """The rows of the listed GLOBAL stream ids (host; an id may appear twice) as packed records on this endpointer's
+        device, ordered on the current CUDA stream in one launch (mww_export_endpointer_rows).  A stream outside the model's
+        stream set exports a zero record.  The endpointer must be up to date with its engine (update() after the engine's
+        last call) and does not change; drain() first, since events do not move."""
+        import torch
+        ids = self._record_ids(stream_ids)
+        data = torch.empty((ids.size, int(self.layout().record_bytes)), dtype=torch.uint8, device=torch.device("cuda", self.device))
+        layout = _lib.MwwEndpointerLayout()
+        self._check(self._L.mww_export_endpointer_rows(self._ep, ids.ctypes.data, ids.size, data.data_ptr() if ids.size else None,
+                                                       ctypes.byref(layout), self._stream()))
+        return EndpointerRecords(data, layout)
+
+    def import_streams(self, stream_ids, records: EndpointerRecords) -> None:
+        """Stream stream_ids[i] (GLOBAL, host, each at most once) takes records.data[i] (mww_import_endpointer_rows): a member
+        takes the row, armed under its new id with its positions rebased onto this endpointer's axis (a record of a
+        non-member resets it); a non-member ignores the record; unlisted rows keep every byte.  The records' vad_window,
+        stride, hop and baseline buffered / pending rows must equal this endpointer's, and it must be up to date with its
+        engine.  An arm after the move replays at most min(lookback_steps, steps this endpointer consumed since create or
+        its last whole reset): update it for lookback_steps calls before a move for a full-depth replay."""
+        import torch
+        ids = self._record_ids(stream_ids)
+        if np.unique(ids).size != ids.size:
+            raise ValueError("a stream id is listed twice")
+        data, layout = records.data, records.layout
+        if not isinstance(layout, _lib.MwwEndpointerLayout):
+            raise ValueError("records.layout must be a MwwEndpointerLayout")
+        if (not isinstance(data, torch.Tensor) or data.dtype != torch.uint8 or data.dim() != 2 or data.shape[0] != ids.size
+                or data.shape[1] != layout.record_bytes or not data.is_contiguous() or data.device != torch.device("cuda", self.device)):
+            raise ValueError("records.data must be a contiguous uint8 tensor [len(ids)=%d, record_bytes=%d] on cuda:%d"
+                             % (ids.size, layout.record_bytes, self.device))
+        self._check(self._L.mww_import_endpointer_rows(self._ep, ids.ctypes.data, ids.size, data.data_ptr() if ids.size else None,
+                                                       ctypes.byref(layout), self._stream()))
 
     _ROW_FIELDS = (("seen", np.int64), ("flags", np.uint64), ("armed", np.int32), ("elapsed", np.int32), ("run", np.int32),
                    ("silence", np.int32), ("heard", np.int32), ("start_sample", np.int64), ("speech_end_sample", np.int64))

@@ -169,18 +169,21 @@ def call_plan(buffered: int, n_samples: int, hop: int, pending_rows, strides, in
 class StreamRecords:
     """Streams exported from an engine (mww_export_streams): `data`, torch.uint8 [n, record_bytes] on the exporting
     engine's device, one packed record per stream (include/mww.h), and `layout`, the _lib.MwwStreamLayout that travels with
-    them: the sizes, models and lockstep counters an importing engine must share."""
+    them: the sizes, models and lockstep counters an importing engine must share.  `history` is None, or the last m samples
+    of each stream's audio history, oldest first: a CUDA int16 tensor [n, m] that import writes back after the records."""
 
     _SCALARS = ("record_bytes", "n_models", "frontend_buffered", "hop_samples")
     _ARRAYS = ("pending_rows", "model_hash", "rows_are_features")
 
-    def __init__(self, data, layout):
-        self.data, self.layout = data, layout
+    def __init__(self, data, layout, history=None):
+        self.data, self.layout, self.history = data, layout, history
 
     def save(self, path) -> None:
-        """np.savez of the records and the layout's fields: a checkpoint of some streams"""
+        """np.savez of the records, the layout's fields and the history when there is one: a checkpoint of some streams"""
         fields = {k: np.asarray(getattr(self.layout, k)) for k in self._SCALARS}
         fields.update({k: np.ctypeslib.as_array(getattr(self.layout, k)).copy() for k in self._ARRAYS})
+        if self.history is not None:
+            fields["audio_history"] = self.history.cpu().numpy()
         np.savez(path, data=self.data.cpu().numpy(), **fields)
 
     @classmethod
@@ -193,7 +196,8 @@ class StreamRecords:
             for k in cls._ARRAYS:
                 np.ctypeslib.as_array(getattr(layout, k))[:] = z[k]
             data = torch.from_numpy(z["data"]).to(device)
-        return cls(data, layout)
+            history = torch.from_numpy(z["audio_history"]).to(device) if "audio_history" in z.files else None
+        return cls(data, layout, history)
 
 
 class _Engine:
@@ -533,22 +537,32 @@ class _Engine:
         _lib.check(self._h, self._L.mww_stream_layout_get(self._h, ctypes.byref(layout)))
         return layout
 
-    def export_streams(self, ids) -> StreamRecords:
+    def export_streams(self, ids, history: int = 0) -> StreamRecords:
         """The whole state (frontend and every model) of streams `ids` as packed records on this engine's device, ordered on
-        the current CUDA stream in a constant number of launches (mww_export_streams).  The engine is not changed."""
+        the current CUDA stream in a constant number of launches (mww_export_streams).  The engine is not changed.
+        `history` > 0 (at most audio_history_capacity) also reads the last `history` samples of each stream's audio history
+        into records.history, on the same CUDA stream, so that the streams keep it when they move.  At 12 s a stream's
+        history is 384 kB: move many streams in batches of ids, or carry only the samples still needed (what a verifier
+        hears, an endpointer's lookback and the commands in progress)."""
         torch = _torch()
         ids = self._ids(ids)
+        if isinstance(history, bool) or not isinstance(history, (int, np.integer)) or history < 0:
+            raise ValueError("history must be a non-negative integer (got %r)" % (history,))
+        if history and not history <= self.audio_history_capacity:
+            raise ValueError("history must be at most the audio history capacity %d (got %d)" % (self.audio_history_capacity, history))
         data = torch.empty((ids.size, int(self.stream_layout().record_bytes)), dtype=torch.uint8, device=self._dev())
         layout = _lib.MwwStreamLayout()
         _lib.check(self._h, self._L.mww_export_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
                                                        self._cu_stream()))
-        return StreamRecords(data, layout)
+        return StreamRecords(data, layout, self.audio_history(ids, int(history)) if history else None)
 
     def import_streams(self, ids, records: StreamRecords) -> None:
         """Stream ids[i] of this engine takes the state of records.data[i] (mww_import_streams): it continues bit for bit as
         the exported stream would have.  Every other stream is untouched.  The records must be a contiguous uint8 tensor
         [len(ids), record_bytes] on this engine's device (ValueError otherwise); records that do not fit this engine's
-        models or lockstep counters, duplicate or out-of-range ids: MwwError, nothing changed."""
+        models or lockstep counters, duplicate or out-of-range ids: MwwError, nothing changed.  When records.history is
+        not None (a CUDA int16 tensor [len(ids), m] on this engine's device, and this engine keeps a history), each
+        stream's history becomes zeros followed by its row, written after the import (mww_write_audio_history)."""
         torch = _torch()
         ids = self._ids(ids)
         data = records.data
@@ -556,8 +570,21 @@ class _Engine:
                 or data.shape[1] != records.layout.record_bytes or not data.is_contiguous() or data.device != self._dev()):
             raise ValueError("records.data must be a contiguous uint8 tensor [len(ids)=%d, record_bytes=%d] on %s"
                              % (ids.size, records.layout.record_bytes, self._dev()))
+        hist = getattr(records, "history", None)
+        if hist is not None:
+            if (not isinstance(hist, torch.Tensor) or hist.dtype != torch.int16 or hist.dim() != 2 or hist.shape[0] != ids.size
+                    or hist.shape[1] > MAX_AUDIO_HISTORY or hist.device != self._dev()):
+                raise ValueError("records.history must be an int16 tensor [len(ids)=%d, <= %d] on %s" % (ids.size, MAX_AUDIO_HISTORY, self._dev()))
+            if self.audio_history_capacity == 0:
+                raise ValueError("records carry audio history but the engine keeps none (set_audio_history)")
+            if hist.shape[1] > 1 and hist.stride(1) != 1 or ids.size > 1 and hist.stride(0) < hist.shape[1]:
+                hist = hist.contiguous()
         _lib.check(self._h, self._L.mww_import_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(records.layout),
                                                        self._cu_stream()))
+        if hist is not None:
+            stride = hist.stride(0) if ids.size > 1 else hist.shape[1]
+            _lib.check(self._h, self._L.mww_write_audio_history(self._h, ids.ctypes.data, ids.size, hist.shape[1],
+                                                                hist.data_ptr() if hist.numel() else None, stride, self._cu_stream()))
 
     # ------------------------------------------------------------------ pinned host buffers next to the GPU
     def host_buffer(self, shape, dtype=np.int16, write_combined: bool = False) -> np.ndarray:
