@@ -141,8 +141,9 @@ int mww_set_window_step(mww_t *h, int hop_samples);
  *
  * mww_reset(NULL) and mww_reset_frontend zero the history and the counter; mww_reset(ids) / mww_reset_device_ids zero
  * those streams' history.  mww_export_streams / mww_import_streams return MWW_EUNSUPPORTED on a handle whose rate is not
- * 16000 (the records have no room for the history).  The staged paths tile input-rate audio; the 16 kHz tile scratch
- * counts against MWW_SCRATCH_MB. */
+ * 16000 (the records have no room for the history); mww_export_resampled_streams / mww_import_resampled_streams carry it
+ * (see "moving resampled streams" below).  The staged paths tile input-rate audio; the 16 kHz tile scratch counts against
+ * MWW_SCRATCH_MB. */
 /* Allowed when mww_set_window_step is (no buffered samples) and the counter is 0; any hop.  A rate outside the list:
  * MWW_EUNSUPPORTED; buffered samples: MWW_EINVAL.  Either way the handle is unchanged. */
 int mww_set_input_rate(mww_t *h, int rate);
@@ -182,8 +183,9 @@ int mww_resample_taps(int rate, int32_t *out, int max_taps, int *n_taps, int *L,
  * int16 [n_streams][H_max] and t, H_max = 243 (the largest H of any rate; 52, 111, 122, 163, 222 and 243 at 8, 22.05, 24,
  * 32, 44.1 and 48 kHz): each stream uses the first H of its own rate, and set refuses an odd t.  mww_reset(NULL) and
  * mww_reset_frontend zero every history and t and keep the rates; mww_reset(ids) zeroes those streams' histories.
- * mww_export_streams / mww_import_streams return MWW_EUNSUPPORTED.  mww_set_input_rate(h, r), allowed at t = 0, returns
- * the handle to one rate for every stream. */
+ * mww_export_streams / mww_import_streams return MWW_EUNSUPPORTED; mww_export_resampled_streams and
+ * mww_import_resampled_streams move these streams.  mww_set_input_rate(h, r), allowed at t = 0, returns the handle to one
+ * rate for every stream. */
 #define MWW_RATE_PER_STREAM 0
 /* Rate h_rates[i] for stream h_ids[i].  The first call puts the handle into per-stream-rate mode, with every stream not
  * listed at 16000; it is allowed only where mww_set_input_rate is (no buffered samples, counter 0) and on a 16 kHz handle
@@ -461,6 +463,66 @@ int mww_stream_layout_get(const mww_t *h, mww_stream_layout *out);
 int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out, void *cu_stream);
 int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout,
                        void *cu_stream);
+
+/* ---- moving resampled streams: records that carry the resampler history ----------------------------------------------
+ * A stream at an input rate other than 16000 (mww_set_input_rate, mww_set_stream_rates) carries one more piece of state:
+ * its resampler history.  mww_export_resampled_streams / mww_import_resampled_streams move streams with it, on any handle
+ * (a plain 16 kHz one included), in either mode and across modes.
+ *
+ * The continuation condition.  Take a stream at rate r, L / M = 16000 / r in lowest terms, that has been given N input
+ * samples.  It has emitted n0 = ceil(N L / M) outputs, and output n0 + q sits t0 + q M upsampled samples past its next
+ * input, t0 = n0 M - N L = (-N L) mod M.  That output reads the inputs k - i, k = floor((t0 + q M) / L), i < H (input 0
+ * being the next one): the last H inputs given and those still to come.  So every 16 kHz sample the stream emits from
+ * then on depends only on its last H inputs and on t0.  As gcd(L, M) = 1, L is invertible mod M and t0 determines
+ * N mod M.  A stream therefore continues bit for bit in another handle when that handle gives it the same rate and its
+ * input count N' for the stream satisfies
+ *     N' = N (mod M),
+ * and at any other N' every later output sits at another phase of the filter.  N is the counter of mww_get_input_rate on
+ * a single-rate handle, and N(t, r) = floor(t M / L) of the counter t with per-stream rates.  There the condition is the
+ * same as t' = t (mod L): write t M = N L + rho with 0 <= rho < L, so t0 = (rho - t M) mod M = rho mod M.  At 8 kHz M = 1
+ * and every N matches; at every other rate rho < L <= M, so t0 = rho = t M mod L, which fixes t mod L since M is
+ * invertible mod L.
+ *
+ * At the 30 ms cadence (calls of 480 16 kHz samples) handles almost always match: t is a multiple of 480, and L = 2, 2, 1,
+ * 160 and 1 at 8, 24, 32, 44.1 and 48 kHz all divide 480 (a single-rate handle's N is then a multiple of M as well).
+ * Only 22.05 kHz (L = 320) can differ: t mod 320 is 0 after an even number of calls and 160 after an odd one (N mod 441 is
+ * 0 or 220 on a single-rate handle, after 661 + 662 inputs per pair of calls), so two handles whose call counts differ in
+ * parity are half a cycle apart.  Advancing the destination by one call fixes it.
+ *
+ *   - One record is the stream record of mww_export_streams, byte for byte at the same offsets, then one 496-byte part at
+ *     resampler_off (== the stream layout's record_bytes): int16 hist[244], the stream's first H history samples in the
+ *     handle's order (H = 52, 111, 122, 163, 222 or 243 at 8, 22.05, 24, 32, 44.1 or 48 kHz, 0 at 16000), then zeros.
+ *     The resampler writes only the first H samples of a history row, and every call that sets a rate or resets a row
+ *     zeroes the whole row, so the rest of a row stays zero (unless mww_set_resampler_state wrote there; the resampler
+ *     never reads it).  On a 16 kHz handle the part is all zeros.
+ *   - The handle's counters travel beside the records in mww_resampler_layout, and the streams' rates in h_rates_out /
+ *     h_rates (int32, host memory; h_rates_out may be NULL): every check is on the host, before any device work.
+ *   - Import refuses with MWW_EINVAL, before any device work and with the handle unchanged, and names the field or id: the
+ *     stream layout does not fit (the fields and rules of mww_import_streams); record_bytes or resampler_off differs; a
+ *     listed stream's rate in h_rates is not the destination's rate for it (or, from a single-rate handle, not the
+ *     records' rate); or a listed stream fails the phase condition (the message names the rate and both phases N mod M).
+ *     Ids out of range or listed twice, n < 0, NULL or misaligned buffers with n > 0 and a poisoned handle are refused as
+ *     by mww_import_streams.
+ *   - Import writes the listed streams' resampler history and everything mww_import_streams writes, and zeroes their audio
+ *     history as it does (mww_write_audio_history comes after).  It never changes the counters or a stream's rate: set the
+ *     destination's rates first with mww_set_stream_rates.
+ *   - Export makes the launches of mww_export_streams plus one, import those of mww_import_streams plus one, whatever n
+ *     is; n == 0 launches nothing.  Export does not change the handle. */
+typedef struct mww_resampler_layout {
+    int64_t record_bytes;       /* the stream record plus the resampler part */
+    int64_t resampler_off;      /* == the stream layout's record_bytes */
+    int32_t rate;               /* the handle's input rate, or MWW_RATE_PER_STREAM */
+    int32_t reserved;
+    int64_t inputs_seen;        /* the counter of mww_get_input_rate: N on a single-rate handle (t with per-stream rates) */
+    int64_t samples16_seen;     /* t of mww_get_stream_rates */
+} mww_resampler_layout;
+/* this handle's resampled record layout and current counters, without device work */
+int mww_get_resampler_layout(const mww_t *h, mww_resampler_layout *out);
+int mww_export_resampled_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out,
+                                 mww_resampler_layout *rs_out, int32_t *h_rates_out, void *cu_stream);
+int mww_import_resampled_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records,
+                                 const mww_stream_layout *layout, const mww_resampler_layout *rs_layout,
+                                 const int32_t *h_rates, void *cu_stream);
 
 /* ---- audio history: the last seconds of each stream's 16 kHz audio, kept on the GPU -----------------------------------
  * What a stream said around a detection (for a second-stage verifier, the pre-roll of an STT request, or false-accept audio

@@ -47,6 +47,7 @@ EXPORTS = (
     "mww_endpointer_drain", "mww_endpointer_buffers", "mww_endpointer_get_state", "mww_endpointer_set_state",
     "mww_endpointer_read_commands",
     "mww_write_audio_history", "mww_get_endpointer_layout", "mww_export_endpointer_rows", "mww_import_endpointer_rows",
+    "mww_get_resampler_layout", "mww_export_resampled_streams", "mww_import_resampled_streams",
 )
 
 
@@ -68,6 +69,14 @@ class MwwStreamLayout(ctypes.Structure):
         ("record_bytes", ctypes.c_int64), ("n_models", ctypes.c_int32), ("frontend_buffered", ctypes.c_int32),
         ("hop_samples", ctypes.c_int32), ("pending_rows", ctypes.c_int32 * 64), ("model_hash", ctypes.c_uint64 * 64),
         ("rows_are_features", ctypes.c_uint8 * 64),
+    ]
+
+
+class MwwResamplerLayout(ctypes.Structure):
+    """mww_resampler_layout of include/mww.h: what travels beside resampled stream records, with the streams' rates"""
+    _fields_ = [
+        ("record_bytes", ctypes.c_int64), ("resampler_off", ctypes.c_int64), ("rate", ctypes.c_int32), ("reserved", ctypes.c_int32),
+        ("inputs_seen", ctypes.c_int64), ("samples16_seen", ctypes.c_int64),
     ]
 
 
@@ -269,6 +278,12 @@ def lib() -> ctypes.CDLL:
     L.mww_export_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), vp]
     L.mww_import_streams.restype = i32
     L.mww_import_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), vp]
+    L.mww_get_resampler_layout.restype = i32
+    L.mww_get_resampler_layout.argtypes = [vp, ctypes.POINTER(MwwResamplerLayout)]
+    L.mww_export_resampled_streams.restype = i32
+    L.mww_export_resampled_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), ctypes.POINTER(MwwResamplerLayout), vp, vp]
+    L.mww_import_resampled_streams.restype = i32
+    L.mww_import_resampled_streams.argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwStreamLayout), ctypes.POINTER(MwwResamplerLayout), vp, vp]
     L.mww_set_input_rate.restype = i32
     L.mww_set_input_rate.argtypes = [vp, i32]
     L.mww_get_input_rate.restype = i32

@@ -2051,52 +2051,46 @@ int mww_stream_layout_get(const mww_t *h, mww_stream_layout *out) {
     return MWW_OK;
 }
 
-int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out, void *cu_stream) {
-    if (!h) return MWW_EINVAL;
-    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_export_streams: stream records do not carry resampler history (input rate != 16000, or per-stream rates)");
-    if (int rc = check_record_args(h, "mww_export_streams", h_ids, n, d_records)) return rc;
-    ENTER_STATEFUL(h);
-    if (out) fill_stream_layout(h, out);
-    if (n == 0) return MWW_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+namespace {
+// the device work of mww_export_streams, into records `pitch` bytes apart (h->d_ids holds the n ids)
+int pack_stream_records(mww_t *h, int n, void *d_records, long long pitch, cudaStream_t st) {
     const RecordLayout L = handle_record_layout(h);
     const void *fe[kRecordMaxParts] = {nullptr, h->d_carry, h->d_estimate};
-    CU(h, launch_pack_streams(record_job_frontend(L), d_records, L.record_bytes, h->d_ids, n, fe, nullptr, h->sm_count, st));
+    CU(h, launch_pack_streams(record_job_frontend(L), d_records, pitch, h->d_ids, n, fe, nullptr, h->sm_count, st));
     h->launches += 1;
     for (size_t k = 0; k < h->models.size(); ++k) {
         const Model &m = h->models[k];
         const void *nn[kRecordMaxParts] = {m.d_nn_state, m.d_pend, nullptr};
-        CU(h, launch_pack_streams(model_record_job(L, (int)k, m), d_records, L.record_bytes, h->d_ids, n, nn, m.mem.d_inv, h->sm_count, st));
+        CU(h, launch_pack_streams(model_record_job(L, (int)k, m), d_records, pitch, h->d_ids, n, nn, m.mem.d_inv, h->sm_count, st));
         h->launches += 1;
     }
     return MWW_OK;
 }
 
-int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout, void *cu_stream) {
-    if (!h) return MWW_EINVAL;
-    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_import_streams: stream records do not carry resampler history (input rate != 16000, or per-stream rates)");
-    if (!layout) return fail(h, MWW_EINVAL, "mww_import_streams: bad arguments");
-    if (int rc = check_record_args(h, "mww_import_streams", h_ids, n, d_records)) return rc;
+// the host checks of mww_import_streams after the arguments: no id twice, and the records' layout fits the handle
+int check_import_layout(mww_t *h, const char *who, const int32_t *h_ids, int n, const mww_stream_layout *layout) {
     std::vector<uint8_t> listed((size_t)h->n_streams, 0);
     for (int i = 0; i < n; ++i) {
-        if (listed[(size_t)h_ids[i]]) return fail(h, MWW_EINVAL, "mww_import_streams: a stream id is listed twice");
+        if (listed[(size_t)h_ids[i]]) return fail(h, MWW_EINVAL, std::string(who) + ": a stream id is listed twice");
         listed[(size_t)h_ids[i]] = 1;
     }
     mww_stream_layout mine;
     fill_stream_layout(h, &mine);
     int which = -1;
     if (const char *field = stream_layout_mismatch(*layout, mine, &which))
-        return fail(h, MWW_EINVAL, std::string("mww_import_streams: the records' ") + field +
+        return fail(h, MWW_EINVAL, std::string(who) + ": the records' " + field +
                                        (which >= 0 ? " of model " + std::to_string(which) : std::string()) + " differs from the handle's");
-    ENTER_STATEFUL(h);
-    if (n == 0) return MWW_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    return MWW_OK;
+}
+
+// the device work of mww_import_streams, from records `pitch` bytes apart; uploads the n ids to h->d_ids
+int unpack_stream_records(mww_t *h, const int32_t *h_ids, int n, const void *d_records, long long pitch, const mww_stream_layout *layout,
+                          cudaStream_t st) {
     if (int rc = ensure_ids(h, &h->d_cids, &h->cids_cap, n, st)) return rc;
     if (int rc = upload_ids(h, h_ids, n, st)) return rc;
     const RecordLayout L = handle_record_layout(h);
     void *fe[kRecordMaxParts] = {nullptr, h->d_carry, h->d_estimate};
-    CU(h, launch_unpack_streams(record_job_frontend(L), d_records, L.record_bytes, h->d_ids, n, fe, nullptr, nullptr, h->sm_count, st));
+    CU(h, launch_unpack_streams(record_job_frontend(L), d_records, pitch, h->d_ids, n, fe, nullptr, nullptr, h->sm_count, st));
     h->launches += 1;
     // records carry no audio history: the streams written start theirs afresh
     if (h->d_hist)
@@ -2108,12 +2102,132 @@ int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_reco
         // members the records hold no state for start fresh, as the joiners of mww_set_model_streams do: zeros (fp32, hybrid)
         // are written by the unpack kernel, zero points (int8) by the model's fill kernel over the list it leaves in d_cids
         const RecordJob J = model_record_job(L, (int)k, m);
-        CU(h, launch_unpack_streams(J, d_records, L.record_bytes, h->d_ids, n, nn, m.mem.d_inv, J.zero_fresh ? nullptr : h->d_cids, h->sm_count, st));
+        CU(h, launch_unpack_streams(J, d_records, pitch, h->d_ids, n, nn, m.mem.d_inv, J.zero_fresh ? nullptr : h->d_cids, h->sm_count, st));
         h->launches += 1;
         if (!J.zero_fresh)
             if (int rc = reset_nn_by_id(h, m, m.d_nn_state, m.d_pend, h->d_cids, n, m.members(), st)) return rc;
         m.tc_rows_bounded = m.tc_rows_bounded && layout->rows_are_features[k];
     }
+    return MWW_OK;
+}
+}  // namespace
+
+int mww_export_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_export_streams: stream records do not carry resampler history (input rate != 16000, or per-stream rates)");
+    if (int rc = check_record_args(h, "mww_export_streams", h_ids, n, d_records)) return rc;
+    ENTER_STATEFUL(h);
+    if (out) fill_stream_layout(h, out);
+    if (n == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+    return pack_stream_records(h, n, d_records, handle_record_layout(h).record_bytes, st);
+}
+
+int mww_import_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (resampling(h)) return fail(h, MWW_EUNSUPPORTED, "mww_import_streams: stream records do not carry resampler history (input rate != 16000, or per-stream rates)");
+    if (!layout) return fail(h, MWW_EINVAL, "mww_import_streams: bad arguments");
+    if (int rc = check_record_args(h, "mww_import_streams", h_ids, n, d_records)) return rc;
+    if (int rc = check_import_layout(h, "mww_import_streams", h_ids, n, layout)) return rc;
+    ENTER_STATEFUL(h);
+    if (n == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    return unpack_stream_records(h, h_ids, n, d_records, handle_record_layout(h).record_bytes, layout, st);
+}
+
+// ---- resampled stream records: stream records plus the resampler history (rule: include/mww.h) -------------------------
+namespace {
+void fill_resampler_layout(const mww_t *h, mww_resampler_layout *o) {
+    memset(o, 0, sizeof *o);
+    o->resampler_off = handle_record_layout(h).record_bytes;
+    o->record_bytes = o->resampler_off + kRecordResamplerPart;
+    o->rate = h->per_rate ? MWW_RATE_PER_STREAM : h->rs.rate;
+    o->inputs_seen = h->rs_seen;
+    o->samples16_seen = h->per_rate ? h->rs_seen : resample_outputs(h->rs_seen, h->rs.L, h->rs.M);
+}
+
+int stream_rate_of(const mww_t *h, int id) { return h->per_rate ? h->stream_rate[(size_t)id] : h->rs.rate; }
+
+// N mod M of a stream at plan P on the counters of a resampler layout: N = inputs_seen on a single-rate handle,
+// floor(t M / L) with per-stream rates
+long long rate_phase(const mww_resampler_layout &r, const ResamplePlan &P) {
+    const long long N = r.rate == MWW_RATE_PER_STREAM ? resample_inputs(r.samples16_seen, P.L, P.M) : r.inputs_seen;
+    return N % P.M;
+}
+}  // namespace
+
+int mww_get_resampler_layout(const mww_t *h, mww_resampler_layout *out) {
+    if (!h || !out) return MWW_EINVAL;
+    fill_resampler_layout(h, out);
+    return MWW_OK;
+}
+
+int mww_export_resampled_streams(mww_t *h, const int32_t *h_ids, int n, void *d_records, mww_stream_layout *out,
+                                 mww_resampler_layout *rs_out, int32_t *h_rates_out, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (int rc = check_record_args(h, "mww_export_resampled_streams", h_ids, n, d_records)) return rc;
+    ENTER_STATEFUL(h);
+    if (out) fill_stream_layout(h, out);
+    mww_resampler_layout R;
+    fill_resampler_layout(h, &R);
+    if (rs_out) *rs_out = R;
+    if (h_rates_out)
+        for (int i = 0; i < n; ++i) h_rates_out[i] = stream_rate_of(h, h_ids[i]);
+    if (n == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = upload_ids(h, h_ids, n, st)) return rc;
+    if (int rc = pack_stream_records(h, n, d_records, R.record_bytes, st)) return rc;
+    const void *rs[kRecordMaxParts] = {h->d_rs_hist, nullptr, nullptr};
+    CU(h, launch_pack_streams(record_job_resampler(R.resampler_off, h->rs_hist_stride), d_records, R.record_bytes, h->d_ids, n, rs, nullptr,
+                              h->sm_count, st));
+    h->launches += 1;
+    return MWW_OK;
+}
+
+int mww_import_resampled_streams(mww_t *h, const int32_t *h_ids, int n, const void *d_records, const mww_stream_layout *layout,
+                                 const mww_resampler_layout *rs_layout, const int32_t *h_rates, void *cu_stream) {
+    static const char *who = "mww_import_resampled_streams";
+    if (!h) return MWW_EINVAL;
+    if (!layout || !rs_layout || (n > 0 && !h_rates)) return fail(h, MWW_EINVAL, std::string(who) + ": bad arguments");
+    if (int rc = check_record_args(h, who, h_ids, n, d_records)) return rc;
+    if (int rc = check_import_layout(h, who, h_ids, n, layout)) return rc;
+    mww_resampler_layout mine;
+    fill_resampler_layout(h, &mine);
+    const mww_resampler_layout &src = *rs_layout;
+    const auto refuse = [&](const std::string &why) { return fail(h, MWW_EINVAL, std::string(who) + ": " + why); };
+    if (src.record_bytes != mine.record_bytes) return refuse("the records' record_bytes differs from the handle's");
+    if (src.resampler_off != mine.resampler_off) return refuse("the records' resampler_off differs from the handle's");
+    ResamplePlan Psrc;
+    if (src.rate != MWW_RATE_PER_STREAM && !resample_plan(src.rate, &Psrc)) return refuse("the records' rate is not an input rate");
+    if (src.inputs_seen < 0 || src.samples16_seen < 0 || src.samples16_seen > (1ll << 50))
+        return refuse("the records' counters are out of range");
+    // each rate's phase in the records and in the handle, once per rate; the message is built only for a refusal
+    long long phase[kNumRates][2];
+    ResamplePlan plan[kNumRates];
+    for (int i = 0; i < kNumRates; ++i) {
+        resample_plan(kResampleRates[i], &plan[i]);
+        phase[i][0] = rate_phase(src, plan[i]);
+        phase[i][1] = rate_phase(mine, plan[i]);
+    }
+    for (int i = 0; i < n; ++i) {
+        const int id = h_ids[i], r = h_rates[i], dst_rate = stream_rate_of(h, id), slot = rate_slot(r);
+        if ((src.rate == MWW_RATE_PER_STREAM || r == src.rate) && r == dst_rate && phase[slot][0] == phase[slot][1]) continue;
+        const std::string stream = "stream " + std::to_string(id) + " (h_rates[" + std::to_string(i) + "] = " + std::to_string(r) + ")";
+        if (src.rate != MWW_RATE_PER_STREAM && r != src.rate)
+            return refuse(stream + ": the rate is not the records' rate " + std::to_string(src.rate));
+        if (r != dst_rate) return refuse(stream + ": the rate is not the handle's rate " + std::to_string(dst_rate) + " for it");
+        return refuse(stream + ": phase mismatch at " + std::to_string(r) + " Hz: the records' N mod " + std::to_string(plan[slot].M) + " = " +
+                      std::to_string(phase[slot][0]) + ", the handle's " + std::to_string(phase[slot][1]));
+    }
+    ENTER_STATEFUL(h);
+    if (n == 0) return MWW_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = unpack_stream_records(h, h_ids, n, d_records, mine.record_bytes, layout, st)) return rc;
+    void *rs[kRecordMaxParts] = {h->d_rs_hist, nullptr, nullptr};
+    CU(h, launch_unpack_streams(record_job_resampler(mine.resampler_off, h->rs_hist_stride), d_records, mine.record_bytes, h->d_ids, n, rs,
+                                nullptr, nullptr, h->sm_count, st));
+    h->launches += 1;
     return MWW_OK;
 }
 

@@ -97,6 +97,20 @@ inline RecordJob record_job_model(const RecordLayout &L, int k, const RecordMode
     return J;
 }
 
+// The resampler part of a resampled record (mww_export_resampled_streams), at rec_off = the stream record's record_bytes:
+// int16 hist[kRecordResamplerSamples], the first hist_stride samples of the stream's history row, zeros after them.  One
+// plain span per stream at the handle's row pitch (0 at 16 kHz: the whole part is padding, written as zero).
+constexpr int kRecordResamplerSamples = 244;        // the per-stream-rate row: H_max = 243 rounded up to even
+constexpr int kRecordResamplerBytes = kRecordResamplerSamples * 2;
+constexpr int kRecordResamplerPart = 496;           // kRecordResamplerBytes padded to 16
+
+inline RecordJob record_job_resampler(long long rec_off, int hist_stride) {
+    RecordJob J;
+    record_add_part(&J, rec_off, (long long)hist_stride * 2);
+    J.padded[0] = kRecordResamplerPart;
+    return J;
+}
+
 // widest word (16, 8, 4 or 1 bytes) that divides every part and every ring's offset and row, so that no word straddles a
 // part, a stream or a ring row: 16 for the frontend and for okay_nabu, fp32 (rows of 128 / 256 bytes) and int8 (32 / 64)
 // alike; whatever the span allows for a run-time geometry

@@ -170,26 +170,36 @@ class StreamRecords:
     """Streams exported from an engine (mww_export_streams): `data`, torch.uint8 [n, record_bytes] on the exporting
     engine's device, one packed record per stream (include/mww.h), and `layout`, the _lib.MwwStreamLayout that travels with
     them: the sizes, models and lockstep counters an importing engine must share.  `history` is None, or the last m samples
-    of each stream's audio history, oldest first: a CUDA int16 tensor [n, m] that import writes back after the records."""
+    of each stream's audio history, oldest first: a CUDA int16 tensor [n, m] that import writes back after the records.
+    Records exported with resampler=True (mww_export_resampled_streams) also carry each stream's resampler history:
+    `resampler` is then the _lib.MwwResamplerLayout (record size and the exporter's input-rate counters) and `rates` the
+    streams' input rates, np.int32 [n]; both are None otherwise."""
 
     _SCALARS = ("record_bytes", "n_models", "frontend_buffered", "hop_samples")
     _ARRAYS = ("pending_rows", "model_hash", "rows_are_features")
+    _RESAMPLER = ("record_bytes", "resampler_off", "rate", "inputs_seen", "samples16_seen")
 
-    def __init__(self, data, layout, history=None):
+    def __init__(self, data, layout, history=None, resampler=None, rates=None):
         self.data, self.layout, self.history = data, layout, history
+        self.resampler, self.rates = resampler, rates
 
     def save(self, path) -> None:
-        """np.savez of the records, the layout's fields and the history when there is one: a checkpoint of some streams"""
+        """np.savez of the records, the layout's fields, the history when there is one and the resampler layout and rates
+        when there are: a checkpoint of some streams"""
         fields = {k: np.asarray(getattr(self.layout, k)) for k in self._SCALARS}
         fields.update({k: np.ctypeslib.as_array(getattr(self.layout, k)).copy() for k in self._ARRAYS})
         if self.history is not None:
             fields["audio_history"] = self.history.cpu().numpy()
+        if self.resampler is not None:
+            fields.update({"resampler_" + k: np.asarray(getattr(self.resampler, k)) for k in self._RESAMPLER})
+            fields["rates"] = np.asarray(self.rates, np.int32)
         np.savez(path, data=self.data.cpu().numpy(), **fields)
 
     @classmethod
     def load(cls, path, device) -> "StreamRecords":
         torch = _torch()
         layout = _lib.MwwStreamLayout()
+        resampler = rates = None
         with np.load(path) as z:
             for k in cls._SCALARS:
                 setattr(layout, k, int(z[k]))
@@ -197,7 +207,12 @@ class StreamRecords:
                 np.ctypeslib.as_array(getattr(layout, k))[:] = z[k]
             data = torch.from_numpy(z["data"]).to(device)
             history = torch.from_numpy(z["audio_history"]).to(device) if "audio_history" in z.files else None
-        return cls(data, layout, history)
+            if "rates" in z.files:
+                resampler = _lib.MwwResamplerLayout()
+                for k in cls._RESAMPLER:
+                    setattr(resampler, k, int(z["resampler_" + k]))
+                rates = np.ascontiguousarray(z["rates"], np.int32)
+        return cls(data, layout, history, resampler, rates)
 
 
 class _Engine:
@@ -537,24 +552,41 @@ class _Engine:
         _lib.check(self._h, self._L.mww_stream_layout_get(self._h, ctypes.byref(layout)))
         return layout
 
-    def export_streams(self, ids, history: int = 0) -> StreamRecords:
+    def resampler_layout(self) -> "_lib.MwwResamplerLayout":
+        """record size of resampled records and the current input-rate counters (mww_get_resampler_layout; no device work)"""
+        layout = _lib.MwwResamplerLayout()
+        _lib.check(self._h, self._L.mww_get_resampler_layout(self._h, ctypes.byref(layout)))
+        return layout
+
+    def export_streams(self, ids, history: int = 0, resampler: bool = False) -> StreamRecords:
         """The whole state (frontend and every model) of streams `ids` as packed records on this engine's device, ordered on
         the current CUDA stream in a constant number of launches (mww_export_streams).  The engine is not changed.
         `history` > 0 (at most audio_history_capacity) also reads the last `history` samples of each stream's audio history
         into records.history, on the same CUDA stream, so that the streams keep it when they move.  At 12 s a stream's
         history is 384 kB: move many streams in batches of ids, or carry only the samples still needed (what a verifier
-        hears, an endpointer's lookback and the commands in progress)."""
+        hears, an endpointer's lookback and the commands in progress).
+        resampler=True exports records that also carry each stream's resampler history (mww_export_resampled_streams), on an
+        engine at any input rate or with per-stream rates; records.resampler and records.rates say what the importer must
+        match.  Without it an engine that resamples refuses (MwwError, MWW_EUNSUPPORTED)."""
         torch = _torch()
         ids = self._ids(ids)
         if isinstance(history, bool) or not isinstance(history, (int, np.integer)) or history < 0:
             raise ValueError("history must be a non-negative integer (got %r)" % (history,))
         if history and not history <= self.audio_history_capacity:
             raise ValueError("history must be at most the audio history capacity %d (got %d)" % (self.audio_history_capacity, history))
-        data = torch.empty((ids.size, int(self.stream_layout().record_bytes)), dtype=torch.uint8, device=self._dev())
         layout = _lib.MwwStreamLayout()
-        _lib.check(self._h, self._L.mww_export_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
-                                                       self._cu_stream()))
-        return StreamRecords(data, layout, self.audio_history(ids, int(history)) if history else None)
+        if resampler:
+            rs = _lib.MwwResamplerLayout()
+            rates = np.zeros(ids.size, np.int32)
+            data = torch.empty((ids.size, int(self.resampler_layout().record_bytes)), dtype=torch.uint8, device=self._dev())
+            _lib.check(self._h, self._L.mww_export_resampled_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
+                                                                     ctypes.byref(rs), rates.ctypes.data, self._cu_stream()))
+        else:
+            rs = rates = None
+            data = torch.empty((ids.size, int(self.stream_layout().record_bytes)), dtype=torch.uint8, device=self._dev())
+            _lib.check(self._h, self._L.mww_export_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
+                                                           self._cu_stream()))
+        return StreamRecords(data, layout, self.audio_history(ids, int(history)) if history else None, rs, rates)
 
     def import_streams(self, ids, records: StreamRecords) -> None:
         """Stream ids[i] of this engine takes the state of records.data[i] (mww_import_streams): it continues bit for bit as
@@ -562,14 +594,28 @@ class _Engine:
         [len(ids), record_bytes] on this engine's device (ValueError otherwise); records that do not fit this engine's
         models or lockstep counters, duplicate or out-of-range ids: MwwError, nothing changed.  When records.history is
         not None (a CUDA int16 tensor [len(ids), m] on this engine's device, and this engine keeps a history), each
-        stream's history becomes zeros followed by its row, written after the import (mww_write_audio_history)."""
+        stream's history becomes zeros followed by its row, written after the import (mww_write_audio_history).
+        Records with a resampler layout (export_streams(..., resampler=True)) take mww_import_resampled_streams: stream
+        ids[i] must already be at records.rates[i] here, and at the same phase of its resampler (include/mww.h), else
+        MwwError naming the stream.  On an engine with per-stream rates, set them first:
+
+            recs = src.export_streams(src_ids, history=m, resampler=True)
+            dst.set_stream_rates(dst_ids, recs.rates)
+            dst.import_streams(dst_ids, recs)"""
         torch = _torch()
         ids = self._ids(ids)
+        rs = getattr(records, "resampler", None)
+        record_bytes = records.layout.record_bytes if rs is None else rs.record_bytes
+        if rs is not None:
+            rates = records.rates
+            if not isinstance(rates, np.ndarray) or rates.dtype != np.int32 or rates.shape != (ids.size,):
+                raise ValueError("records.rates must be an np.int32 array [len(ids)=%d]" % ids.size)
+            rates = np.ascontiguousarray(rates)
         data = records.data
         if (not isinstance(data, torch.Tensor) or data.dtype != torch.uint8 or data.dim() != 2 or data.shape[0] != ids.size
-                or data.shape[1] != records.layout.record_bytes or not data.is_contiguous() or data.device != self._dev()):
+                or data.shape[1] != record_bytes or not data.is_contiguous() or data.device != self._dev()):
             raise ValueError("records.data must be a contiguous uint8 tensor [len(ids)=%d, record_bytes=%d] on %s"
-                             % (ids.size, records.layout.record_bytes, self._dev()))
+                             % (ids.size, record_bytes, self._dev()))
         hist = getattr(records, "history", None)
         if hist is not None:
             if (not isinstance(hist, torch.Tensor) or hist.dtype != torch.int16 or hist.dim() != 2 or hist.shape[0] != ids.size
@@ -579,8 +625,13 @@ class _Engine:
                 raise ValueError("records carry audio history but the engine keeps none (set_audio_history)")
             if hist.shape[1] > 1 and hist.stride(1) != 1 or ids.size > 1 and hist.stride(0) < hist.shape[1]:
                 hist = hist.contiguous()
-        _lib.check(self._h, self._L.mww_import_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(records.layout),
-                                                       self._cu_stream()))
+        if rs is None:
+            _lib.check(self._h, self._L.mww_import_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(records.layout),
+                                                           self._cu_stream()))
+        else:
+            _lib.check(self._h, self._L.mww_import_resampled_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(),
+                                                                     ctypes.byref(records.layout), ctypes.byref(rs), rates.ctypes.data,
+                                                                     self._cu_stream()))
         if hist is not None:
             stride = hist.stride(0) if ids.size > 1 else hist.shape[1]
             _lib.check(self._h, self._L.mww_write_audio_history(self._h, ids.ctypes.data, ids.size, hist.shape[1],
