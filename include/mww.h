@@ -910,6 +910,71 @@ int mww_verify_streams(mww_verifier_t *v, mww_t *src, const int32_t *d_ids, int 
 int mww_verify_detections(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, float *d_scores, int32_t *d_confirmed,
                           void *cu_stream);
 
+/* ---- event positions: where on the audio history's axis each detection happened ---------------------------------------------
+ * An event's `step` counts its row's probabilities since the row's last reset, and rows are reset from the device, so the
+ * host cannot place a step in the audio.  A TIMED detector stores one more value per event: its position on the axis of the
+ * audio history (mww_set_audio_history), whose sample t is the t-th 16 kHz sample appended since the history was enabled, the
+ * axis samples_seen counts and the endpointer's positions use.
+ *
+ * Definition.  An event's position is the history-axis position of the last 16 kHz sample of the newest feature window of
+ * the model step whose probability is the newest one in the firing window -- the endpointer's pos(j) of that step.
+ *   - Plain detector.  An update describes its n_steps steps by a clock (last_end, step_samples): step t of the call ends at
+ *     last_end - (n_steps - 1 - t) step_samples.  For an engine call, last_end = S - (buffered - (480 - hop)) - hop g and
+ *     step_samples = hop stride, with S = samples_seen, buffered = frontend_buffered and g the model's pending rows, all read
+ *     right after the call, as the endpointer reads them.
+ *   - Models detector.  The detector copies the handle's hop at create.  An update passes row_end = S - b (b = buffered -
+ *     (480 - hop), read right after the call) and each model's pending rows after the call, g_k, beside the n_k and p_k of
+ *     mww_multi_detector_update.  The call produced R = n_k s_k - p_k + g_k feature rows, the same R for every non-OFF model
+ *     (the step counts and p_k alone fix R only up to the strides).  WAKE step j of model k ends at
+ *     row_end - hop (R - 1 - e_k(j)), with e_k(j) = (j + 1) s_k - p_k - 1, which is row_end - hop (g_k + (n_k - 1 - j) s_k):
+ *     the endpointer's position formula.
+ *   - Events, state, d_fired, cutoffs and records are bit for bit what an untimed detector gives from the same
+ *     probabilities: the position is an extra output, not a change to the rule.
+ *
+ * Mode and calls (messages in mww_last_error(NULL); every refusal is MWW_EINVAL before any device work, detector unchanged):
+ *   - mww_time_detector_events: makes the detector timed, for good, and allocates int64 positions[capacity], -1 in every slot.
+ *     Only while its event buffer is empty: after create or a drain, with no update since; otherwise refused.  Timing a timed
+ *     detector does nothing.
+ *   - mww_update_detector_at / mww_update_multi_detector_at: the timed updates, one launch each as the untimed ones, which they
+ *     replace: a timed detector refuses mww_detector_update and mww_multi_detector_update, an untimed one refuses these two.
+ *     Refused also: step_samples < 1; NULL pending_after; pending rows after the call that give no common R; and every
+ *     refusal of the untimed call.  Untimed detectors change in nothing.
+ *   - mww_get_detector_positions: the device view, slot i the position of event slot i, as d_fired; -1 in unused slots (the
+ *     drain refills the used ones).
+ *   - mww_drain_detector_at: mww_detector_drain plus the positions of the same events into h_positions.  mww_detector_drain
+ *     on a timed detector drains without them.
+ *   - Orderings: update the detector right after each engine call, before the next one changes the counters; drain before
+ *     mww_set_audio_history, which restarts the axis.
+ *
+ * Reads that end at given positions.  mww_read_audio_history_at: row i of d_out [n][out_stride] holds the n_samples samples
+ * [d_ends[i] - n_samples, d_ends[i]) of stream d_ids[i], oldest first.  Entries outside [samples_seen - C, samples_seen)
+ * are zeros, as are ids outside [0, n_streams): the endpointer's command-read rule.  d_ids and d_ends are in device memory,
+ * so a detector's d_fired and positions go in as they are; a -1 position is an end far outside the ring.  One launch,
+ * counted in mww_launch_count, no host synchronisation, and the refusals of mww_read_audio_history_device_ids plus NULL
+ * d_ends with work to do.
+ *
+ * Verification anchored at the event.  mww_verify_detections_at, on a timed detector: slot i is verify_detections' slot id
+ * plus its position P.  Its clip is [e - n_samples, e) with e = min(P + post, S), S = src's samples_seen when the call is
+ * enqueued.  When the whole clip is still in the ring (e - n_samples >= S - C) the slot is scored as mww_verify_detections
+ * scores it: history read, fresh verifier handle, mww_predict_clip, mww_positive_scores, confirm.  Otherwise -- an unused
+ * slot, another model's event, an event whose clip has left the ring -- score NaN and confirmed -1.  An event younger than
+ * post samples at verify time is heard with a shorter post-roll: its clip still has n_samples samples and ends at S.  So
+ * n_samples is what the verifier hears, whatever the poll interval, and a verifier cutoff chosen offline on clips that end
+ * post samples after the wake word holds in serving.  post is in [0, 2^22]; an untimed detector is refused.  The launches
+ * are those of mww_verify_detections, whatever the number of events; src and det are not changed. */
+int mww_time_detector_events(mww_detector_t *d);
+int mww_update_detector_at(mww_detector_t *d, const float *d_probs, int n_steps, long long pitch, long long last_end, long long step_samples,
+                           void *cu_stream);
+int mww_update_multi_detector_at(mww_detector_t *d, const float *const *d_probs, const long long *pitch, const int *n_steps,
+                                 const int *pending_before, const int *pending_after, long long row_end, void *cu_stream);
+int mww_get_detector_positions(mww_detector_t *d, const int64_t **d_positions);
+int mww_drain_detector_at(mww_detector_t *d, mww_event *h_events, int64_t *h_positions, int max_events, long long *n_events,
+                          void *cu_stream);
+int mww_read_audio_history_at(mww_t *h, const int32_t *d_ids, const long long *d_ends, int n, int n_samples, int16_t *d_out,
+                              long long out_stride, void *cu_stream);
+int mww_verify_detections_at(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, long long post, float *d_scores,
+                             int32_t *d_confirmed, void *cu_stream);
+
 /* ---- endpointing: where the spoken command after a wake word ends, and its clip from the audio history ----------------------
  * After a wake word a voice assistant sends the command that follows to speech-to-text and stops when the speaker stops.  An
  * ENDPOINTER finds that end on the GPU, per stream, from a VAD model's probabilities, and cuts each command's clip from the

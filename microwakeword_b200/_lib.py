@@ -48,6 +48,8 @@ EXPORTS = (
     "mww_endpointer_read_commands",
     "mww_write_audio_history", "mww_get_endpointer_layout", "mww_export_endpointer_rows", "mww_import_endpointer_rows",
     "mww_get_resampler_layout", "mww_export_resampled_streams", "mww_import_resampled_streams",
+    "mww_time_detector_events", "mww_update_detector_at", "mww_update_multi_detector_at", "mww_get_detector_positions",
+    "mww_drain_detector_at", "mww_read_audio_history_at", "mww_verify_detections_at",
 )
 
 
@@ -388,6 +390,20 @@ def lib() -> ctypes.CDLL:
     for name in ("mww_export_endpointer_rows", "mww_import_endpointer_rows"):
         getattr(L, name).restype = i32
         getattr(L, name).argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwEndpointerLayout), vp]
+    L.mww_time_detector_events.restype = i32
+    L.mww_time_detector_events.argtypes = [vp]
+    L.mww_update_detector_at.restype = i32
+    L.mww_update_detector_at.argtypes = [vp, vp, i32, ll, ll, ll, vp]
+    L.mww_update_multi_detector_at.restype = i32
+    L.mww_update_multi_detector_at.argtypes = [vp, vp, vp, vp, vp, vp, ll, vp]
+    L.mww_get_detector_positions.restype = i32
+    L.mww_get_detector_positions.argtypes = [vp, ctypes.POINTER(vp)]
+    L.mww_drain_detector_at.restype = i32
+    L.mww_drain_detector_at.argtypes = [vp, vp, vp, i32, ctypes.POINTER(ll), vp]
+    L.mww_read_audio_history_at.restype = i32
+    L.mww_read_audio_history_at.argtypes = [vp, vp, vp, i32, i32, vp, ll, vp]
+    L.mww_verify_detections_at.restype = i32
+    L.mww_verify_detections_at.argtypes = [vp, vp, vp, i32, ll, vp, vp, vp]
     _lib = L
     return L
 

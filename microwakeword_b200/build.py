@@ -52,6 +52,11 @@ EP_SOURCES = ["mww_endpoint.cu"]
 # libmww_endpoint.so keep exactly the kernels they had
 SR_OUT = os.path.join(HERE, "libmww_serving_records.so")
 SR_SOURCES = ["mww_serving_records.cu"]
+# and the kernels of event positions: the timed detectors' updates, the history read that ends at given positions
+# (mww_read_audio_history_at) and the verifier slots that end at their events (mww_verify_detections_at), so that the detector,
+# history, endpoint and verify libraries keep exactly the kernels they had
+EVP_OUT = os.path.join(HERE, "libmww_event_positions.so")
+EVP_SOURCES = ["mww_event_positions.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -74,7 +79,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, EVP_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -95,10 +100,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
         for out, sources, extra in ((RS_OUT, RS_SOURCES, []), (RR_OUT, RR_SOURCES, []), (DET_OUT, DET_SOURCES, []),
                                     (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []), (G711_OUT, G711_SOURCES, []),
                                     (HIST_OUT, HIST_SOURCES, []), (DR_OUT, DR_SOURCES, []), (VER_OUT, VER_SOURCES, []),
-                                    (EP_OUT, EP_SOURCES, []), (SR_OUT, SR_SOURCES, []),
+                                    (EP_OUT, EP_SOURCES, []), (SR_OUT, SR_SOURCES, []), (EVP_OUT, EVP_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
                                                     "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711", "-lmww_history",
                                                     "-lmww_detector_records", "-lmww_verify", "-lmww_endpoint", "-lmww_serving_records",
+                                                    "-lmww_event_positions",
                                                     "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra

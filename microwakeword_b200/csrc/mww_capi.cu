@@ -2310,6 +2310,20 @@ int mww_read_audio_history_device_ids(mww_t *h, const int32_t *d_ids, int n, int
     return read_history(h, d_ids, n, n_samples, d_out, out_stride, static_cast<cudaStream_t>(cu_stream));
 }
 
+int mww_read_audio_history_at(mww_t *h, const int32_t *d_ids, const long long *d_ends, int n, int n_samples, int16_t *d_out, long long out_stride,
+                              void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    const char *who = "mww_read_audio_history_at";
+    if (int rc = check_history_read(h, who, d_ids, n, n_samples, d_out, out_stride)) return rc;
+    if (n > 0 && n_samples > 0 && !d_ends) return fail(h, MWW_EINVAL, std::string(who) + ": NULL ends");
+    ENTER_STATEFUL(h);
+    if (n == 0 || n_samples == 0) return MWW_OK;
+    CU(h, launch_history_read_at(h->d_hist, h->hist_cap, h->hist_seen, d_ids, d_ends, n, h->n_streams, n_samples, d_out, out_stride, h->sm_count,
+                                 static_cast<cudaStream_t>(cu_stream)));
+    h->launches += 1;
+    return MWW_OK;
+}
+
 int mww_write_audio_history(mww_t *h, const int32_t *h_ids, int n, int n_samples, const int16_t *d_in, long long in_stride, void *cu_stream) {
     if (!h) return MWW_EINVAL;
     const char *who = "mww_write_audio_history";

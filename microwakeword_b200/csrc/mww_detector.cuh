@@ -1,5 +1,6 @@
 // mww_detector.cuh -- the streaming detector's update kernel (rule and both forms: mww_detector.h), included by
-// mww_detector.cu (uniform cutoff) and mww_detector_cutoffs.cu (per-row cutoffs, mww_set_detector_cutoffs).
+// mww_detector.cu (uniform cutoff), mww_detector_cutoffs.cu (per-row cutoffs, mww_set_detector_cutoffs) and
+// mww_event_positions.cu (the timed kernels, which run the same body and also store each event's position).
 //
 // detector_update_kernel<false, *>, thread per row: the live shape, one or a few steps for very many rows.  State is
 // struct-of-arrays and the history [window - 1][n_rows], so every access of a warp is one coalesced line; a one-step call
@@ -41,8 +42,15 @@ struct PassWindow {
     }
 };
 
-// the warp's lanes whose `fire` is set append one event each: one atomicAdd for all of them.  Called by whole warps.
-MWW_D void append_events(const DetectorArgs &a, bool fire, int row, long long step, float score) {
+// no positions: the untimed detector stores nothing beside the event
+struct NoPositions {
+    MWW_D void put(unsigned long long, int) const {}
+};
+
+// the warp's lanes whose `fire` is set append one event each: one atomicAdd for all of them.  Called by whole warps.  t: the
+// step's index in the call, which a timed detector turns into the event's position (pos.put)
+template <typename P>
+MWW_D void append_events(const DetectorArgs &a, bool fire, int row, long long step, float score, const P &pos, int t) {
     const unsigned mask = __ballot_sync(kFull, fire);
     if (mask == 0) return;
     const int lane = threadIdx.x & 31;
@@ -56,14 +64,17 @@ MWW_D void append_events(const DetectorArgs &a, bool fire, int row, long long st
     e.stream = stream; e.reserved = 0; e.step = step; e.score = score; e.pad = 0;
     a.events[slot] = e;
     a.fired[slot] = stream;
+    pos.put(slot, t);
 }
 
 }  // namespace
 
-// kRowCutoff: the cutoff of row r is row_cutoff[r] (per-row mode); otherwise a.rule.cutoff and row_cutoff is not read
-template <bool kWarpPerRow, bool kRowCutoff>
-__global__ void __launch_bounds__(kThreads) detector_update_kernel(DetectorArgs a, const float *__restrict__ probs, int n_steps, long long pitch,
-                                                                   const double *__restrict__ row_cutoff) {
+// The update of one thread (thread form) or one warp (warp form), shared by detector_update_kernel and the timed kernel
+// (mww_event_positions.cu), which differ only in P.  kRowCutoff: the cutoff of row r is row_cutoff[r] (per-row mode);
+// otherwise a.rule.cutoff and row_cutoff is not read.
+template <bool kWarpPerRow, bool kRowCutoff, typename P>
+MWW_D void detector_update_rows(const DetectorArgs &a, const float *__restrict__ probs, int n_steps, long long pitch,
+                                const double *__restrict__ row_cutoff, const P &pos) {
     const DetectorRule &r = a.rule;
     if (!kWarpPerRow) {
         const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -83,7 +94,7 @@ __global__ void __launch_bounds__(kThreads) detector_update_kernel(DetectorArgs 
                 fire = detector_step_at(hist, r, cutoff, seen, cooldown, probs[row * pitch + t], &score);
                 ++seen;
             }
-            append_events(a, fire, (int)row, seen - 1, score);
+            append_events(a, fire, (int)row, seen - 1, score, pos, t);
         }
         if (active) { a.seen[row] = seen; a.cooldown[row] = cooldown; }
     } else {
@@ -105,7 +116,7 @@ __global__ void __launch_bounds__(kThreads) detector_update_kernel(DetectorArgs 
             const int first = detector_first_full(seen + base, w, n);
             const unsigned candidates = __ballot_sync(kFull, lane >= first && lane < n && (double)avg > cutoff);
             const unsigned fired = detector_chain_pass(r, candidates, first, n, cooldown);
-            append_events(a, (fired >> lane) & 1u, (int)row, seen + base + lane, avg);
+            append_events(a, (fired >> lane) & 1u, (int)row, seen + base + lane, avg, pos, base + lane);
             if (base + 32 < n_steps) x.prev = x.cur;
         }
         // new history: the last w - 1 of (old history, this call's steps), i.e. steps n - (w - 1) .. n - 1 of the last pass
@@ -115,16 +126,26 @@ __global__ void __launch_bounds__(kThreads) detector_update_kernel(DetectorArgs 
     }
 }
 
+template <bool kWarpPerRow, bool kRowCutoff>
+__global__ void __launch_bounds__(kThreads) detector_update_kernel(DetectorArgs a, const float *__restrict__ probs, int n_steps, long long pitch,
+                                                                   const double *__restrict__ row_cutoff) {
+    detector_update_rows<kWarpPerRow, kRowCutoff>(a, probs, n_steps, pitch, row_cutoff, NoPositions{});
+}
+
+// the grid of the form: a thread per row, or a warp per row from kDetectorWarpMinSteps steps on
+inline unsigned update_form_blocks(const DetectorArgs &a, int n_steps) {
+    const long long threads = (long long)a.n_rows * (n_steps >= kDetectorWarpMinSteps ? 32 : 1);
+    return (unsigned)((threads + kThreads - 1) / kThreads);
+}
+
 // the form for a call of n_steps: thread per row below kDetectorWarpMinSteps steps, warp per row from there on
 template <bool kRowCutoff>
 cudaError_t launch_update_form(const DetectorArgs &a, const double *row_cutoff, const float *probs, int n_steps, long long pitch, cudaStream_t st) {
     if (n_steps <= 0 || a.n_rows <= 0) return cudaSuccess;
-    if (n_steps >= kDetectorWarpMinSteps) {
-        const long long blocks = ((long long)a.n_rows * 32 + kThreads - 1) / kThreads;
-        detector_update_kernel<true, kRowCutoff><<<(unsigned)blocks, kThreads, 0, st>>>(a, probs, n_steps, pitch, row_cutoff);
-    } else {
-        detector_update_kernel<false, kRowCutoff><<<(unsigned)((a.n_rows + kThreads - 1) / kThreads), kThreads, 0, st>>>(a, probs, n_steps, pitch, row_cutoff);
-    }
+    if (n_steps >= kDetectorWarpMinSteps)
+        detector_update_kernel<true, kRowCutoff><<<update_form_blocks(a, n_steps), kThreads, 0, st>>>(a, probs, n_steps, pitch, row_cutoff);
+    else
+        detector_update_kernel<false, kRowCutoff><<<update_form_blocks(a, n_steps), kThreads, 0, st>>>(a, probs, n_steps, pitch, row_cutoff);
     return cudaGetLastError();
 }
 

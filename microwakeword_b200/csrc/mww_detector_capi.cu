@@ -40,6 +40,12 @@ struct mww_detector {
     std::vector<DetectModel> models;
     DetectModel *d_models = nullptr;
     DetectModelRows *d_models_rows = nullptr;
+    // event positions (mww_time_detector_events): positions [capacity] beside the events once timed; `updated` is set by every
+    // update that launched and cleared by a drain, so that a detector with buffered events cannot be timed; `hop` is a models
+    // detector's handle's hop at create
+    bool timed = false, updated = false;
+    long long *positions = nullptr;
+    int hop = kHop;
 };
 
 namespace {
@@ -54,7 +60,7 @@ void detector_free(mww_detector_t *d) {
         cudaFree(s.hist); cudaFree(s.seen); cudaFree(s.flag); cudaFree(const_cast<int32_t *>(s.inv)); cudaFree(s.d_cutoffs);
     }
     cudaFree(d->count); cudaFree(d->events); cudaFree(d->fired); cudaFree(d->d_stream_ids); cudaFree(d->d_rows);
-    cudaFree(d->d_models); cudaFree(d->d_models_rows);
+    cudaFree(d->d_models); cudaFree(d->d_models_rows); cudaFree(d->positions);
     delete d;
 }
 
@@ -256,6 +262,28 @@ int stage_ids(mww_detector_t *d, const int32_t *h_ids, int n, cudaStream_t st) {
     return MWW_OK;
 }
 
+// one models update call's description, checked as mww_multi_detector_update checks it; *any: some model has work
+int models_call(const mww_detector_t *d, const std::string &name, const float *const *d_probs, const long long *pitch, const int *n_steps,
+                const int *pending_before, DetectCall *call, bool *any) {
+    if (!d_probs || !pitch || !n_steps || !pending_before) return refuse(name + ": d_probs, pitch, n_steps and pending_before must not be NULL");
+    *any = false;
+    for (int k = 0; k < d->m.n_models; ++k) {
+        const DetectModel &M = d->models[k];
+        if (M.role == MWW_DETECT_OFF) continue;
+        DetectCall &c = call[k];
+        c.probs = d_probs[k]; c.pitch = pitch[k]; c.n_steps = n_steps[k]; c.pending = pending_before[k];
+        if (c.n_steps > 0 && M.n_rows > 0) {
+            if (!c.probs || c.pitch < c.n_steps)
+                return refuse(name + ": model " + std::to_string(k) + " needs d_probs and n_steps columns within the row pitch");
+            *any = true;
+        }
+    }
+    if (!detect_call_fits(d->models.data(), call, d->m.n_models))
+        return refuse(name + ": the step counts and pending rows do not describe one call "
+                      "(n_k = (p_k + R) div s_k with 0 <= p_k < s_k for one R >= 0)");
+    return MWW_OK;
+}
+
 // ---- detector records: each row set is one model of the record (the plain detector's one WAKE model, row = id)
 void fill_layout(const mww_detector_t *d, mww_detector_layout *o) {
     *o = mww_detector_layout{};
@@ -297,6 +325,38 @@ int check_rows(const mww_detector_t *d, const std::string &call, const int32_t *
     return MWW_OK;
 }
 
+// Both drains: the events (and, h_positions != nullptr, their positions) to the host; the counter cleared, d_fired and a timed
+// detector's positions refilled with -1
+int drain(mww_detector_t *d, mww_event *h_events, long long *h_positions, int max_events, long long *n_events, cudaStream_t st) {
+    DENTER(d);
+    unsigned long long count = 0;
+    DCU(cudaMemcpyAsync(&count, d->count, sizeof(count), cudaMemcpyDeviceToHost, st));
+    DCU(cudaStreamSynchronize(st));
+    const size_t stored = (size_t)std::min<unsigned long long>(count, (unsigned long long)d->capacity);
+    const size_t n = std::min(stored, (size_t)max_events);
+    if (n) DCU(cudaMemcpyAsync(h_events, d->events, n * sizeof(mww_event), cudaMemcpyDeviceToHost, st));
+    if (n && h_positions) DCU(cudaMemcpyAsync(h_positions, d->positions, n * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    if (stored) {
+        DCU(cudaMemsetAsync(d->count, 0, sizeof(count), st));
+        DCU(cudaMemsetAsync(d->fired, 0xFF, stored * sizeof(int32_t), st));
+        if (d->timed) DCU(cudaMemsetAsync(d->positions, 0xFF, stored * sizeof(long long), st));
+    }
+    if (n) DCU(cudaStreamSynchronize(st));
+    *n_events = (long long)count;
+    d->updated = false;
+    return MWW_OK;
+}
+
+// the untimed update calls refuse a timed detector, the timed ones an untimed detector
+int untimed_arg(const mww_detector_t *d, const char *call, const char *timed_call) {
+    if (d->timed) return refuse(std::string(call) + ": the detector is timed (mww_time_detector_events): it takes " + timed_call);
+    return MWW_OK;
+}
+int timed_arg(const mww_detector_t *d, const char *call) {
+    if (!d->timed) return refuse(std::string(call) + ": the detector is not timed: call mww_time_detector_events after create or a drain");
+    return MWW_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -313,21 +373,7 @@ int mww_detector_destroy(mww_detector_t *d) {
 int mww_detector_drain(mww_detector_t *d, mww_event *h_events, int max_events, long long *n_events, void *cu_stream) {
     if (!d || !n_events || max_events < 0 || (max_events > 0 && !h_events))
         return refuse("mww_detector_drain: needs a detector, n_events and room for max_events >= 0 events");
-    DENTER(d);
-    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    unsigned long long count = 0;
-    DCU(cudaMemcpyAsync(&count, d->count, sizeof(count), cudaMemcpyDeviceToHost, st));
-    DCU(cudaStreamSynchronize(st));
-    const size_t stored = (size_t)std::min<unsigned long long>(count, (unsigned long long)d->capacity);
-    const size_t n = std::min(stored, (size_t)max_events);
-    if (n) DCU(cudaMemcpyAsync(h_events, d->events, n * sizeof(mww_event), cudaMemcpyDeviceToHost, st));
-    if (stored) {
-        DCU(cudaMemsetAsync(d->count, 0, sizeof(count), st));
-        DCU(cudaMemsetAsync(d->fired, 0xFF, stored * sizeof(int32_t), st));
-    }
-    if (n) DCU(cudaStreamSynchronize(st));
-    *n_events = (long long)count;
-    return MWW_OK;
+    return drain(d, h_events, nullptr, max_events, n_events, static_cast<cudaStream_t>(cu_stream));
 }
 
 int mww_detector_buffers(mww_detector_t *d, const long long **d_count, const mww_event **d_events, const int32_t **d_fired, int *capacity) {
@@ -427,12 +473,14 @@ int mww_detector_create(int device, int n_rows, int window, double cutoff, int c
 
 int mww_detector_update(mww_detector_t *d, const float *d_probs, int n_steps, long long pitch, void *cu_stream) {
     if (int rc = plain_arg(d, "mww_detector_update", "mww_multi_detector_update")) return rc;
+    if (int rc = untimed_arg(d, "mww_detector_update", "mww_update_detector_at")) return rc;
     if (n_steps < 0 || (n_steps > 0 && (!d_probs || pitch < n_steps)))
         return refuse("mww_detector_update: needs d_probs and n_steps >= 0 columns within the row pitch");
     if (n_steps == 0) return MWW_OK;
     DENTER(d);
     if (d->per_row) DCU(launch_detector_update_cutoffs(d->a, d->sets[0].d_cutoffs, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
     else DCU(launch_detector_update(d->a, d_probs, n_steps, pitch, static_cast<cudaStream_t>(cu_stream)));
+    d->updated = true;
     return MWW_OK;
 }
 
@@ -495,6 +543,7 @@ int mww_multi_detector_create(const mww_t *h, const mww_detect_rule *rules, int 
     d->device = info.device;
     d->multi = true;
     d->capacity = capacity;
+    d->hop = info.hop_samples;
     d->sets.resize(K);
     DetectModelsArgs &m = d->m;
     m.n_streams = info.n_streams; m.n_models = K; m.vad = vad;
@@ -528,30 +577,17 @@ int mww_multi_detector_create(const mww_t *h, const mww_detect_rule *rules, int 
 int mww_multi_detector_update(mww_detector_t *d, const float *const *d_probs, const long long *pitch, const int *n_steps,
                                const int *pending_before, void *cu_stream) {
     if (int rc = models_arg(d, "mww_multi_detector_update")) return rc;
-    if (!d_probs || !pitch || !n_steps || !pending_before)
-        return refuse("mww_multi_detector_update: d_probs, pitch, n_steps and pending_before must not be NULL");
+    if (int rc = untimed_arg(d, "mww_multi_detector_update", "mww_update_multi_detector_at")) return rc;
     DetectModelsArgs &m = d->m;
     DetectCall call[kDetectMaxModels];
     bool any = false;
-    for (int k = 0; k < m.n_models; ++k) {
-        const DetectModel &M = d->models[k];
-        if (M.role == MWW_DETECT_OFF) continue;
-        DetectCall &c = call[k];
-        c.probs = d_probs[k]; c.pitch = pitch[k]; c.n_steps = n_steps[k]; c.pending = pending_before[k];
-        if (c.n_steps > 0 && M.n_rows > 0) {
-            if (!c.probs || c.pitch < c.n_steps)
-                return refuse("mww_multi_detector_update: model " + std::to_string(k) + " needs d_probs and n_steps columns within the row pitch");
-            any = true;
-        }
-    }
-    if (!detect_call_fits(d->models.data(), call, m.n_models))
-        return refuse("mww_multi_detector_update: the step counts and pending rows do not describe one call "
-                      "(n_k = (p_k + R) div s_k with 0 <= p_k < s_k for one R >= 0)");
+    if (int rc = models_call(d, "mww_multi_detector_update", d_probs, pitch, n_steps, pending_before, call, &any)) return rc;
     if (!any) return MWW_OK;
     DENTER(d);
     for (int k = 0; k < m.n_models; ++k) m.call[k] = call[k];
     if (d->per_row) DCU(launch_detector_models_update_cutoffs(detect_args_rows(m, d->d_models_rows), static_cast<cudaStream_t>(cu_stream)));
     else DCU(launch_detector_models_update(m, static_cast<cudaStream_t>(cu_stream)));
+    d->updated = true;
     return MWW_OK;
 }
 
@@ -579,6 +615,76 @@ int mww_get_multi_detector_cutoffs(mww_detector_t *d, int k, double *h_cutoffs) 
     if (!h_cutoffs && s->n_rows > 0) return refuse("mww_get_multi_detector_cutoffs: h_cutoffs is NULL");
     get_cutoffs(d, *s, h_cutoffs);
     return MWW_OK;
+}
+
+// ---- event positions (both kinds)
+int mww_time_detector_events(mww_detector_t *d) {
+    const std::string call = "mww_time_detector_events";
+    if (!d) return refuse(call + ": detector is NULL");
+    if (d->timed) return MWW_OK;
+    if (d->updated) return refuse(call + ": the detector may hold events: time it after create or a drain, before any update");
+    DENTER(d);
+    long long *p = nullptr;
+    DCU(cudaMalloc(&p, (size_t)d->capacity * sizeof(long long)));
+    if (cudaError_t e = cudaMemset(p, 0xFF, (size_t)d->capacity * sizeof(long long))) { cudaFree(p); return cuda_fail(nullptr, e, "cudaMemset"); }
+    d->positions = p;
+    d->timed = true;
+    return MWW_OK;
+}
+
+int mww_update_detector_at(mww_detector_t *d, const float *d_probs, int n_steps, long long pitch, long long last_end, long long step_samples,
+                           void *cu_stream) {
+    const char *call = "mww_update_detector_at";
+    if (int rc = plain_arg(d, call, "mww_update_multi_detector_at")) return rc;
+    if (int rc = timed_arg(d, call)) return rc;
+    if (n_steps < 0 || (n_steps > 0 && (!d_probs || pitch < n_steps)))
+        return refuse(std::string(call) + ": needs d_probs and n_steps >= 0 columns within the row pitch");
+    if (step_samples < 1) return refuse(std::string(call) + ": step_samples must be at least 1");
+    if (n_steps == 0) return MWW_OK;
+    DENTER(d);
+    DCU(launch_detector_update_at(d->a, d->per_row ? d->sets[0].d_cutoffs : nullptr, d_probs, n_steps, pitch, d->positions, last_end, step_samples,
+                                  static_cast<cudaStream_t>(cu_stream)));
+    d->updated = true;
+    return MWW_OK;
+}
+
+int mww_update_multi_detector_at(mww_detector_t *d, const float *const *d_probs, const long long *pitch, const int *n_steps,
+                                 const int *pending_before, const int *pending_after, long long row_end, void *cu_stream) {
+    const std::string call = "mww_update_multi_detector_at";
+    if (int rc = models_arg(d, call.c_str())) return rc;
+    if (int rc = timed_arg(d, call.c_str())) return rc;
+    DetectModelsArgs &m = d->m;
+    DetectCall c[kDetectMaxModels];
+    bool any = false;
+    if (int rc = models_call(d, call, d_probs, pitch, n_steps, pending_before, c, &any)) return rc;
+    if (!pending_after) return refuse(call + ": pending_after must not be NULL");
+    const long long R = event_call_rows(d->models.data(), c, pending_after, m.n_models);
+    if (R < 0)
+        return refuse(call + ": the step counts and pending rows before and after do not describe one call "
+                      "(R = n_k s_k - p_k + g_k with 0 <= p_k, g_k < s_k, the same R >= 0 for every model)");
+    if (!any) return MWW_OK;
+    DENTER(d);
+    for (int k = 0; k < m.n_models; ++k) m.call[k] = c[k];
+    const long long row0 = event_row0_end(row_end, d->hop, R);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (d->per_row) DCU(launch_detector_models_update_at(detect_args_rows(m, d->d_models_rows), d->positions, row0, d->hop, st));
+    else DCU(launch_detector_models_update_at(m, d->positions, row0, d->hop, st));
+    d->updated = true;
+    return MWW_OK;
+}
+
+int mww_get_detector_positions(mww_detector_t *d, const int64_t **d_positions) {
+    if (!d || !d_positions) return refuse("mww_get_detector_positions: needs a detector and d_positions");
+    if (int rc = timed_arg(d, "mww_get_detector_positions")) return rc;
+    *d_positions = reinterpret_cast<const int64_t *>(d->positions);
+    return MWW_OK;
+}
+
+int mww_drain_detector_at(mww_detector_t *d, mww_event *h_events, int64_t *h_positions, int max_events, long long *n_events, void *cu_stream) {
+    if (!d || !n_events || max_events < 0 || (max_events > 0 && (!h_events || !h_positions)))
+        return refuse("mww_drain_detector_at: needs a detector, n_events and room for max_events >= 0 events and positions");
+    if (int rc = timed_arg(d, "mww_drain_detector_at")) return rc;
+    return drain(d, h_events, reinterpret_cast<long long *>(h_positions), max_events, n_events, static_cast<cudaStream_t>(cu_stream));
 }
 
 }  // extern "C"

@@ -1,6 +1,6 @@
 // mww_detector_models.cuh -- the multi-model streaming detector's update kernel (rule and per-stream body:
-// mww_detector_models.h), included by mww_detector_models.cu (uniform mode) and mww_detector_cutoffs.cu (per-row mode,
-// mww_set_multi_detector_cutoffs).
+// mww_detector_models.h), included by mww_detector_models.cu (uniform mode), mww_detector_cutoffs.cu (per-row mode,
+// mww_set_multi_detector_cutoffs) and mww_event_positions.cu (the timed kernel, whose emit also stores each event's position).
 //
 // detector_models_update_kernel: a thread per global stream walks the call's steps of the VAD and of every WAKE model it
 // belongs to (detect_models_stream).  Each model's state is struct-of-arrays over its members, so for a model on all
@@ -23,22 +23,24 @@ constexpr unsigned kModelsFull = 0xffffffffu;
 constexpr int kModelsThreads = 256;
 
 // the warp's lanes whose `fire` is set append one event each: one atomicAdd for all of them.  Called by whole warps.
+// -> the slot of a stored event, -1 otherwise.
 template <typename M>
 struct WarpEmit {
     const DetectModelsArgsT<M> &a;
-    MWW_D void operator()(bool fire, int k, int stream, long long step, float score) const {
+    MWW_D long long operator()(bool fire, int k, int stream, long long step, float score) const {
         const unsigned mask = __ballot_sync(kModelsFull, fire);
-        if (mask == 0) return;
+        if (mask == 0) return -1;
         const int lane = threadIdx.x & 31;
         unsigned long long base = 0;
         if (lane == 0) base = atomicAdd(a.count, (unsigned long long)__popc(mask));
         base = __shfl_sync(kModelsFull, base, 0);
         const unsigned long long slot = base + __popc(mask & ((1u << lane) - 1));
-        if (!fire || slot >= (unsigned long long)a.capacity) return;      // past capacity: counted, not stored
+        if (!fire || slot >= (unsigned long long)a.capacity) return -1;   // past capacity: counted, not stored
         mww_event e;
         e.stream = stream; e.reserved = k; e.step = step; e.score = score; e.pad = 0;
         a.events[slot] = e;
         a.fired[slot] = stream;
+        return (long long)slot;
     }
 };
 

@@ -14,6 +14,8 @@
 
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "mww_detector.h"
 
 namespace mww {
@@ -134,7 +136,15 @@ inline bool detect_call_fits(const DetectModel *models, const DetectCall *call, 
     return any && lo <= hi;
 }
 
-// One call for one stream.  emit(fire, k, stream, step, score) is called for every WAKE step of every WAKE model in the
+// emit(fire, k, stream, step, score, j), j the step's index in the call, where Emit takes it (the timed kernel places the
+// event with it); emit(fire, k, stream, step, score) otherwise
+template <typename Emit>
+MWW_HD void detect_emit(Emit &emit, bool fire, int k, int stream, long long step, float score, int j) {
+    if constexpr (std::is_invocable_v<Emit &, bool, int, int, long long, float, int>) emit(fire, k, stream, step, score, j);
+    else emit(fire, k, stream, step, score);
+}
+
+// One call for one stream.  emit(fire, k, stream, step, score[, j]) is called for every WAKE step of every WAKE model in the
 // same order on every stream, member or not (fire false for a non-member), so that the kernel's warps can ballot on it.
 template <typename M, typename Emit>
 MWW_HD void detect_models_stream(const DetectModelsArgsT<M> &a, int stream, Emit &emit) {
@@ -175,7 +185,7 @@ MWW_HD void detect_models_stream(const DetectModelsArgsT<M> &a, int stream, Emit
                     }
                     ++seen;
                 }
-                emit(fire, k, stream, seen - 1, avg);
+                detect_emit(emit, fire, k, stream, seen - 1, avg, j);
             }
             if (row >= 0) { W.seen[row] = seen; W.flag[row] = cooldown; }
         }

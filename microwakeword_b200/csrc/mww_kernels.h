@@ -223,3 +223,24 @@ cudaError_t launch_history_write(int16_t *ring, int C, long long seen, const int
 cudaError_t launch_pack_endpointer_rows(const EpRecJob &J, void *records, const int32_t *ids, int n, cudaStream_t st);
 cudaError_t launch_unpack_endpointer_rows(const EpRecJob &J, const void *records, const int32_t *ids, int n, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_event_positions.h"
+namespace mww {
+// event positions (mww_event_positions.cu, positions and bodies in mww_event_positions.h; companion library
+// libmww_event_positions.so), one launch each.
+// the plain detector's update (row_cutoff == nullptr: uniform mode) that also writes positions[slot] for every stored event,
+// step t of the call ending at last_end - (n_steps - 1 - t) step_samples
+cudaError_t launch_detector_update_at(const DetectorArgs &a, const double *row_cutoff, const float *probs, int n_steps, long long pitch,
+                                      long long *positions, long long last_end, long long step_samples, cudaStream_t st);
+// the models detector's update that also writes positions[slot], WAKE step j of model k ending at row0_end + hop e_k(j)
+cudaError_t launch_detector_models_update_at(const DetectModelsArgs &a, long long *positions, long long row0_end, int hop, cudaStream_t st);
+cudaError_t launch_detector_models_update_at(const DetectModelsArgsT<DetectModelRows> &a, long long *positions, long long row0_end, int hop,
+                                             cudaStream_t st);
+// out [n][out_stride]: row i = samples [ends[i] - n_samples, ends[i]) of stream ids[i] from ring [n_streams][C], `seen` samples
+// appended (ids and ends in device memory; zeros outside the ring and for ids outside [0, n_streams))
+cudaError_t launch_history_read_at(const int16_t *ring, int C, long long seen, const int32_t *ids, const long long *ends, int n, int n_streams,
+                                   int n_samples, int16_t *out, long long out_stride, int sm_count, cudaStream_t st);
+// ids [capacity] and ends [capacity]: verify_slot_at of every slot of a timed detector; *count is read on the device
+cudaError_t launch_verify_slots_at(const long long *count, const mww_event *events, const long long *positions, int capacity, int model,
+                                   long long post, long long seen, int C, int n_samples, int32_t *ids, long long *ends, cudaStream_t st);
+}  // namespace mww

@@ -21,6 +21,7 @@ struct mww_verifier {
     int *d_lengths = nullptr;           // [slots] steps
     float *d_scores = nullptr;          // [slots] the positive scores of the first n tracks
     int32_t *d_ids = nullptr;           // [slots] a detector's slots as stream ids (mww_verify_detections)
+    long long *d_ends = nullptr;        // [slots] the end of each slot's clip (mww_verify_detections_at)
 };
 
 namespace {
@@ -39,7 +40,7 @@ int pass_on(int rc, const mww_t *h, const std::string &what) {
 
 void verifier_free(mww_verifier_t *v) {
     if (v->h) mww_destroy(v->h);
-    cudaFree(v->d_audio); cudaFree(v->d_probs); cudaFree(v->d_offsets); cudaFree(v->d_lengths); cudaFree(v->d_scores); cudaFree(v->d_ids);
+    cudaFree(v->d_audio); cudaFree(v->d_probs); cudaFree(v->d_offsets); cudaFree(v->d_lengths); cudaFree(v->d_scores); cudaFree(v->d_ids); cudaFree(v->d_ends);
     delete v;
 }
 
@@ -53,6 +54,7 @@ int verifier_alloc(mww_verifier_t *v) {
     VCU(cudaMalloc(&v->d_lengths, S * sizeof(int)));
     VCU(cudaMalloc(&v->d_scores, S * sizeof(float)));
     VCU(cudaMalloc(&v->d_ids, S * sizeof(int32_t)));
+    VCU(cudaMalloc(&v->d_ends, S * sizeof(long long)));
     std::vector<long long> offsets(S);
     for (size_t i = 0; i < S; ++i) offsets[i] = (long long)(i * M);
     const std::vector<int> lengths(S, v->steps);
@@ -86,18 +88,42 @@ int check_source(const mww_verifier_t *v, mww_t *src, const std::string &call, i
     return MWW_OK;
 }
 
-// The pass over n ids in device memory: src's history of each, a fresh verifier handle's clip probabilities, their positive
-// scores, and the confirm kernel.  A constant number of launches for n >= 1.
-int run(mww_verifier_t *v, mww_t *src, int src_streams, const int32_t *d_ids, int n, float *d_scores, int32_t *d_confirmed, cudaStream_t st,
-        const std::string &call) {
+// The pass over n ids in device memory: src's history of each (the last n_samples, or with d_ends the n_samples before
+// d_ends[i]), a fresh verifier handle's clip probabilities, their positive scores, and the confirm kernel.  A constant number
+// of launches for n >= 1.
+int run(mww_verifier_t *v, mww_t *src, int src_streams, const int32_t *d_ids, const long long *d_ends, int n, float *d_scores,
+        int32_t *d_confirmed, cudaStream_t st, const std::string &call) {
     const int N = v->rule.n_samples;
-    if (int rc = mww_read_audio_history_device_ids(src, d_ids, n, N, v->d_audio, N, st)) return pass_on(rc, src, call + ": history read");
+    const int rc = d_ends ? mww_read_audio_history_at(src, d_ids, d_ends, n, N, v->d_audio, N, st)
+                          : mww_read_audio_history_device_ids(src, d_ids, n, N, v->d_audio, N, st);
+    if (rc) return pass_on(rc, src, call + ": history read");
     if (int rc = mww_reset(v->h, nullptr, 0, st)) return pass_on(rc, v->h, call + ": verifier reset");
     int got = 0;
     if (int rc = mww_predict_clip(v->h, v->d_audio, N, N, v->d_probs, v->steps, &got, st)) return pass_on(rc, v->h, call + ": verifier clip");
     if (int rc = mww_positive_scores(v->d_probs, v->d_offsets, v->d_lengths, n, v->rule.window, v->rule.ignore_steps, v->d_scores, st))
         return fail(nullptr, rc, call + ": mww_positive_scores failed");
     VCU(launch_verify_confirm(d_ids, n, src_streams, v->d_scores, v->rule.cutoff, d_scores, d_confirmed, st));
+    return MWW_OK;
+}
+
+// The checks both detector calls share, before any device work: the detector's buffers, its size against the slots, the
+// source, the detector's device and the model index
+int check_detections(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, const std::string &call, const long long **d_count,
+                     const mww_event **d_events, int *capacity, int *src_streams, cudaStream_t st) {
+    if (!det) return refuse(call + ": detector is NULL");
+    mww_detector_buffers(det, d_count, d_events, nullptr, capacity);
+    if (v && *capacity > v->slots)
+        return refuse(call + ": the detector keeps " + std::to_string(*capacity) + " events; the verifier has " + std::to_string(v->slots) + " slots");
+    if (int rc = check_source(v, src, call, *capacity, src_streams, st)) return rc;
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, *d_count) != cudaSuccess || attr.device != v->device) {
+        cudaGetLastError();
+        return refuse(call + ": the detector is on another device than the verifier");
+    }
+    mww_detector_layout layout;
+    mww_get_detector_layout(det, &layout);
+    if (model >= layout.n_models)
+        return refuse(call + ": model " + std::to_string(model) + " of a detector of " + std::to_string(layout.n_models) + " model(s)");
     return MWW_OK;
 }
 
@@ -164,35 +190,43 @@ int mww_verify_streams(mww_verifier_t *v, mww_t *src, const int32_t *d_ids, int 
     if (n == 0) return MWW_OK;
     DeviceGuard guard(v->device);
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
-    return run(v, src, src_streams, d_ids, n, d_scores, d_confirmed, st, call);
+    return run(v, src, src_streams, d_ids, nullptr, n, d_scores, d_confirmed, st, call);
 }
 
 int mww_verify_detections(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, float *d_scores, int32_t *d_confirmed,
                           void *cu_stream) {
     const std::string call = "mww_verify_detections";
-    if (!det) return refuse(call + ": detector is NULL");
     const long long *d_count = nullptr;
     const mww_event *d_events = nullptr;
-    int capacity = 0;
-    mww_detector_buffers(det, &d_count, &d_events, nullptr, &capacity);
+    int capacity = 0, src_streams = 0;
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    int src_streams = 0;
-    if (v && capacity > v->slots)
-        return refuse(call + ": the detector keeps " + std::to_string(capacity) + " events; the verifier has " + std::to_string(v->slots) + " slots");
-    if (int rc = check_source(v, src, call, capacity, &src_streams, st)) return rc;
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, d_count) != cudaSuccess || attr.device != v->device) {
-        cudaGetLastError();
-        return refuse(call + ": the detector is on another device than the verifier");
-    }
-    mww_detector_layout layout;
-    mww_get_detector_layout(det, &layout);
-    if (model >= layout.n_models)
-        return refuse(call + ": model " + std::to_string(model) + " of a detector of " + std::to_string(layout.n_models) + " model(s)");
+    if (int rc = check_detections(v, src, det, model, call, &d_count, &d_events, &capacity, &src_streams, st)) return rc;
     DeviceGuard guard(v->device);
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
     VCU(launch_verify_slots(d_count, d_events, capacity, model, v->d_ids, st));
-    return run(v, src, src_streams, v->d_ids, capacity, d_scores, d_confirmed, st, call);
+    return run(v, src, src_streams, v->d_ids, nullptr, capacity, d_scores, d_confirmed, st, call);
+}
+
+int mww_verify_detections_at(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, long long post, float *d_scores, int32_t *d_confirmed,
+                             void *cu_stream) {
+    const std::string call = "mww_verify_detections_at";
+    if (post < 0 || post > kVerifyMaxSamples) return refuse(call + ": post must be in [0, 2^22]");
+    const int64_t *d_positions = nullptr;
+    if (det && mww_get_detector_positions(det, &d_positions) != MWW_OK)
+        return refuse(call + ": the detector is not timed (mww_time_detector_events): its events carry no positions");
+    const long long *d_count = nullptr;
+    const mww_event *d_events = nullptr;
+    int capacity = 0, src_streams = 0;
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (int rc = check_detections(v, src, det, model, call, &d_count, &d_events, &capacity, &src_streams, st)) return rc;
+    int C = 0;
+    long long S = 0;
+    mww_get_audio_history(src, &C, &S);
+    DeviceGuard guard(v->device);
+    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+    VCU(launch_verify_slots_at(d_count, d_events, reinterpret_cast<const long long *>(d_positions), capacity, model, post, S, C, v->rule.n_samples,
+                               v->d_ids, v->d_ends, st));
+    return run(v, src, src_streams, v->d_ids, v->d_ends, capacity, d_scores, d_confirmed, st, call);
 }
 
 }  // extern "C"

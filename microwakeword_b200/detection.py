@@ -28,6 +28,7 @@ import ctypes
 import numpy as np
 
 from . import _lib
+from .engine import WINDOW
 
 
 class _Packed:
@@ -309,6 +310,22 @@ class DetectorRecords:
         return cls(data, layout, [c.copy() for c in cut] if layout.multi else cut.copy())
 
 
+def timed_dtype(dtype) -> np.dtype:
+    """the drain dtype of a timed detector: `dtype` and the int64 `sample`, each event's position on the audio history's axis"""
+    return np.dtype(dtype.descr + [("sample", np.int64)])
+
+
+def _history_clock(engine, model):
+    """(samples_seen S, b, hop) of an engine with an audio history, read now: its newest feature row's window ends at history
+    sample S - b (include/mww.h, "event positions"); ValueError without a history, on which positions mean nothing"""
+    cap, S = engine._audio_history()
+    if cap == 0:
+        raise ValueError("a timed detector places events on the engine's audio history axis: the engine keeps no audio history "
+                         "(set_audio_history)")
+    hop = int(engine.hop)
+    return S, engine.frontend_buffered - (WINDOW - hop), hop
+
+
 class _Detector:
     """what both detectors share: ownership of one mww_detector_t, its device views, drain, the reset dispatch and the
     record calls"""
@@ -326,6 +343,21 @@ class _Detector:
             # device views: the stream of every event since the last drain (-1 in unused slots), and how many fired
             self.fired_ids = torch.as_tensor(_DeviceArray(self._handle, fired.value, self.capacity, "<i4"), device=dev)
             self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
+        self.timed = False
+        self.event_samples = None
+
+    def _time(self) -> None:
+        """make the detector timed (mww_time_detector_events) and make event_samples, the device view of the positions"""
+        self._check(self._L.mww_time_detector_events(self._d))
+        ptr = ctypes.c_void_p()
+        self._check(self._L.mww_get_detector_positions(self._d, ctypes.byref(ptr)))
+        import torch
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(dev):
+            # the position of every event since the last drain on the audio history's axis, slot by slot as fired_ids (-1 in
+            # unused slots)
+            self.event_samples = torch.as_tensor(_DeviceArray(self._handle, ptr.value, self.capacity, "<i8"), device=dev)
+        self.timed = True
 
     def _check(self, rc: int) -> None:
         if rc != 0:
@@ -345,11 +377,22 @@ class _Detector:
         self._handle.close()
 
     def _drain_slots(self, dtype):
-        """(events since the last drain as `dtype` in slot order, events that fired)"""
+        """(events since the last drain as `dtype` in slot order, events that fired); a timed detector's events carry `sample`
+        too (timed_dtype)"""
         buf = np.empty(self.capacity, dtype)
         n = ctypes.c_longlong(0)
-        self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
-        return buf[:min(n.value, self.capacity)], n.value
+        if not self.timed:
+            self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
+            return buf[:min(n.value, self.capacity)], n.value
+        pos = np.empty(self.capacity, np.int64)
+        self._check(self._L.mww_drain_detector_at(self._d, buf.ctypes.data, pos.ctypes.data, self.capacity, ctypes.byref(n),
+                                                  self._cuda_stream()))
+        m = min(n.value, self.capacity)
+        out = np.empty(m, timed_dtype(dtype))
+        for name in dtype.names:
+            out[name] = buf[name][:m]
+        out["sample"] = pos[:m]
+        return out, n.value
 
     def _drain(self, dtype, keys):
         """(events since the last drain as `dtype`, sorted by `keys`, most significant first; events dropped)"""
@@ -415,10 +458,20 @@ class StreamDetector(_Detector):
 
     `stream_ids`: event.stream of each row when it is not the row index (model k of an engine with stream sets scores its
     members in list order: pass MultiModelEngine.streams[k]).  `capacity`: events kept between drains; more are
-    counted and dropped."""
+    counted and dropped.
+
+    `timed=True` places every event on the engine's audio history axis (include/mww.h, "event positions"): update takes the
+    engine whose call made the probabilities, drain adds an int64 `sample` field, and event_samples is a device view beside
+    fired_ids.  Update right after each engine call, before the next changes its counters, and drain before
+    engine.set_audio_history, which restarts the axis:
+
+        eng.set_audio_history(48000)
+        det = StreamDetector(eng.n_streams, cutoff=0.9, timed=True)
+        det.update(eng.step(chunk), eng)
+        clips = eng.audio_history(det.fired_ids, 24000, end=det.event_samples)   # the 1.5 s before each detection"""
 
     def __init__(self, n_rows: int, cutoff: float, window: int = 5, cooldown_slices: int = 25, capacity: int = 65536,
-                 stream_ids=None, device: int = 0):
+                 stream_ids=None, device: int = 0, timed: bool = False):
         self._L = _lib.lib()
         d = ctypes.c_void_p()
         ids = None
@@ -430,11 +483,29 @@ class StreamDetector(_Detector):
                                          ids.ctypes.data if ids is not None else None, ctypes.byref(d))
         self._own(rc, d, device, capacity)
         self.n_rows, self.window, self.cutoff, self.cooldown_slices = int(n_rows), int(window), float(cutoff), int(cooldown_slices)
+        if timed:
+            self._time()
 
-    def update(self, probs) -> None:
+    def update(self, probs, engine=None, model=None) -> None:
         """CUDA float32 [n_rows, steps], any row pitch (a slice of a wider buffer is read in place); zero columns: nothing
-        happens.  Asynchronous on the current CUDA stream."""
+        happens.  Asynchronous on the current CUDA stream.  A timed detector takes the engine whose call just returned
+        `probs` (with `model` = k for probs[k] of a MultiModelEngine) and reads the clock of its steps from the engine's
+        counters now; an untimed detector takes neither."""
         import torch
+        if not self.timed:
+            if engine is not None or model is not None:
+                raise ValueError("only a timed detector (timed=True) takes the engine and model")
+        else:
+            if engine is None:
+                raise ValueError("a timed detector needs the engine whose call made the probabilities")
+            multi = hasattr(engine, "n_models")
+            if multi and (isinstance(model, bool) or not isinstance(model, (int, np.integer)) or not 0 <= model < engine.n_models):
+                raise ValueError("model must be a model index in [0, %d) for a MultiModelEngine (got %r)" % (engine.n_models, model))
+            if not multi and model is not None:
+                raise ValueError("model selects a model of a MultiModelEngine; a StreamEngine has one")
+            S, b, hop = _history_clock(engine, model)
+            stride = engine.stride[int(model)] if multi else engine.stride
+            g = engine.pending_rows[int(model)] if multi else engine.pending_rows
         if (not isinstance(probs, torch.Tensor) or not probs.is_cuda or probs.dtype != torch.float32 or probs.dim() != 2
                 or probs.shape[0] != self.n_rows or probs.device.index != self.device):
             raise ValueError("probs must be a CUDA float32 tensor [n_rows=%d, steps] on device %d" % (self.n_rows, self.device))
@@ -444,12 +515,15 @@ class StreamDetector(_Detector):
         if (n > 1 and probs.stride(1) != 1) or (self.n_rows > 1 and probs.stride(0) < n):
             probs = probs.contiguous()
         pitch = probs.stride(0) if self.n_rows > 1 else n
-        self._check(self._L.mww_detector_update(self._d, probs.data_ptr(), n, pitch, _stream(probs.device)))
+        if self.timed:
+            self._check(self._L.mww_update_detector_at(self._d, probs.data_ptr(), n, pitch, S - b - hop * g, hop * stride, _stream(probs.device)))
+        else:
+            self._check(self._L.mww_detector_update(self._d, probs.data_ptr(), n, pitch, _stream(probs.device)))
 
     def drain(self):
-        """-> (events, dropped): the events since the last drain as a structured array (EVENT_DTYPE) sorted by (step, stream),
-        and how many more fired than `capacity` could hold.  Waits for the current CUDA stream; clears the event buffer and
-        fired_ids."""
+        """-> (events, dropped): the events since the last drain as a structured array (EVENT_DTYPE, and `sample` for a timed
+        detector) sorted by (step, stream), and how many more fired than `capacity` could hold.  Waits for the current CUDA
+        stream; clears the event buffer and fired_ids."""
         return self._drain(EVENT_DTYPE, ("step", "stream"))
 
     def reset(self, rows=None) -> None:
@@ -563,9 +637,12 @@ class MultiModelDetector(_Detector):
 
         new = MultiModelDetector(eng, ...)     # the same rules
         all_ids = np.arange(eng.n_streams)
-        new.import_streams(all_ids, det.export_streams(all_ids))"""
+        new.import_streams(all_ids, det.export_streams(all_ids))
 
-    def __init__(self, engine, cutoffs, windows=5, cooldown_slices: int = 25, vad=None, capacity: int = 65536):
+    `timed=True` places every event on the engine's audio history axis, as StreamDetector's does: update reads the clock from
+    the engine, which must keep an audio history, drain adds `sample` and event_samples is the device view."""
+
+    def __init__(self, engine, cutoffs, windows=5, cooldown_slices: int = 25, vad=None, capacity: int = 65536, timed: bool = False):
         K = engine.n_models
         cutoffs = _per_model(cutoffs, K, "cutoffs")
         windows = _per_model(windows, K, "windows")
@@ -590,6 +667,9 @@ class MultiModelDetector(_Detector):
         self.cooldown_slices = [int(c) for c in cooldowns]
         self.streams = [s.copy() for s in engine.streams]
         self._pending = list(engine.pending_rows)
+        self._hop = int(engine.hop)
+        if timed:
+            self._time()
 
     @property
     def pending_rows(self) -> list:
@@ -622,8 +702,16 @@ class MultiModelDetector(_Detector):
             pitch[k] = p.stride(0) if rows > 1 else n
             steps[k] = n
         pend = (ctypes.c_int * K)(*self._pending)
-        self._check(self._L.mww_multi_detector_update(self._d, ptrs, pitch, steps, pend, self._cuda_stream()))
-        self._pending = list(self.engine.pending_rows)
+        after = list(self.engine.pending_rows)
+        if self.timed:
+            S, b, hop = _history_clock(self.engine, None)
+            if hop != self._hop:
+                raise ValueError("the engine's hop changed since this detector was made (%d, was %d): make a new detector" % (hop, self._hop))
+            self._check(self._L.mww_update_multi_detector_at(self._d, ptrs, pitch, steps, pend, (ctypes.c_int * K)(*after), S - b,
+                                                             self._cuda_stream()))
+        else:
+            self._check(self._L.mww_multi_detector_update(self._d, ptrs, pitch, steps, pend, self._cuda_stream()))
+        self._pending = after
 
     def drain(self):
         """-> (events, dropped): the events since the last drain (MODEL_EVENT_DTYPE, global stream ids) sorted by (model, step,

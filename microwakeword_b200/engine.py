@@ -478,12 +478,15 @@ class _Engine:
         """16 kHz samples every stream has appended since set_audio_history (resets do not clear it)"""
         return self._audio_history()[1]
 
-    def audio_history(self, stream_ids, n_samples: int, out=None):
+    def audio_history(self, stream_ids, n_samples: int, out=None, end=None):
         """The last n_samples (<= audio_history_capacity) 16 kHz samples of each listed stream, oldest first, zero-padded on
         the left: a CUDA int16 tensor [len(ids), n_samples], ordered on the current CUDA stream (mww_read_audio_history).
         `stream_ids`: a host sequence (ids in [0, n_streams)) or a contiguous 1-D CUDA int32 tensor such as a detector's
         fired_ids, read with no host round trip (ids outside [0, n_streams), the -1 slots, give zero rows).  Read before
-        reset(ids): a reset zeroes the history.  `out`: a CUDA int16 tensor [len(ids), >= n_samples] with contiguous rows."""
+        reset(ids): a reset zeroes the history.  `out`: a CUDA int16 tensor [len(ids), >= n_samples] with contiguous rows.
+        `end`: row i holds the samples [end[i] - n_samples, end[i]) of the history axis instead, zeros where they are not in
+        the ring [audio_samples_seen - capacity, audio_samples_seen) (mww_read_audio_history_at); a host sequence or a
+        contiguous 1-D CUDA int64 tensor aligned with the ids, such as a timed detector's event_samples."""
         torch = _torch()
         cap = self.audio_history_capacity
         if cap == 0:
@@ -507,12 +510,32 @@ class _Engine:
               or out.shape[1] < n_samples or (out.stride(1) != 1 and out.shape[1] > 1) or (n > 1 and out.stride(0) < n_samples)):
             raise ValueError("out must be a CUDA int16 tensor [len(ids)=%d, >= %d] with contiguous rows on %s" % (n, n_samples, self._dev()))
         stride = out.stride(0) if n > 1 else max(out.shape[1], n_samples)
+        if end is not None:
+            ends = self._history_ends(end, n)
+            dids = stream_ids if device_ids else torch.from_numpy(ids).to(self._dev())
+            _lib.check(self._h, self._L.mww_read_audio_history_at(self._h, dids.data_ptr(), ends.data_ptr(), n, n_samples, out.data_ptr(), stride,
+                                                                  self._cu_stream()))
+            return out[:, :n_samples]
         if device_ids:
             rc = self._L.mww_read_audio_history_device_ids(self._h, stream_ids.data_ptr(), n, n_samples, out.data_ptr(), stride, self._cu_stream())
         else:
             rc = self._L.mww_read_audio_history(self._h, ids.ctypes.data, n, n_samples, out.data_ptr(), stride, self._cu_stream())
         _lib.check(self._h, rc)
         return out[:, :n_samples]
+
+    def _history_ends(self, end, n: int):
+        """the ends of a read at positions as a CUDA int64 tensor [n] on this engine's device, or ValueError"""
+        torch = _torch()
+        if isinstance(end, torch.Tensor) and end.is_cuda:
+            if end.dtype != torch.int64 or end.dim() != 1 or not end.is_contiguous() or end.device != self._dev() or end.numel() != n:
+                raise ValueError("device ends must be a contiguous 1-D CUDA int64 tensor [len(ids)=%d] on %s" % (n, self._dev()))
+            return end
+        if hasattr(end, "is_cuda"):
+            end = end.numpy()
+        e = np.asarray(end)
+        if e.shape != (n,) or (e.size and (e.dtype == bool or not np.issubdtype(e.dtype, np.integer))):
+            raise ValueError("end must be one integer position per id (%d)" % n)
+        return torch.from_numpy(np.ascontiguousarray(e, np.int64)).to(self._dev())
 
     def features(self, audio, out=None, samples16=None, law=None):
         """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer.

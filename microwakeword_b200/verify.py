@@ -9,6 +9,9 @@ whose score is above its cutoff.  The audio never leaves the GPU and the host is
     eng.reset(confirmed)                           # restart only the confirmed streams
     events, dropped = ver.drain(det)               # now and then: events with their verifier_score
 
+With a timed detector the clip can end at the event instead of "now" (at_event=True): the verifier then hears the same
+n_samples around the wake word whatever the poll interval, post samples of them after the detection.
+
 The score is the positive-sample score of the reference's streaming ROC (test.py:364-373): the verifier model on a fresh
 frontend and fresh state over the clip, as the reference makes the spectrograms of its positive clips, then
 detection.positive_scores with (window, ignore_steps).  So detection.streaming_model_roc picks a verifier cutoff by the rule
@@ -41,9 +44,10 @@ class Verifier:
     `ignore_steps` probabilities.  A stream is confirmed when its score (as float64) is above `cutoff`.  `model`: what
     StreamEngine accepts (a container path or bytes, or a streaming .tflite; fp32, int8, any geometry, hybrid).
 
-    The read is "now", not the samples that end at the event: a caller that verifies at each drain, every D live calls of
-    480 samples, needs n_samples to cover what the verifier must hear plus D * 480 samples.  Calls on one verifier are
-    ordered on the current CUDA stream; the verifier's own model state is scratch."""
+    By default the read is "now", not the samples that end at the event: a caller that verifies at each drain, every D live
+    calls of 480 samples, needs n_samples to cover what the verifier must hear plus D * 480 samples.  verify(..., at_event=True)
+    on a timed detector reads the clip that ends `post` samples after each event instead, so n_samples is only what the
+    verifier hears.  Calls on one verifier are ordered on the current CUDA stream; the verifier's own model state is scratch."""
 
     def __init__(self, model, slots: int, n_samples: int, cutoff: float, window: int = 5, ignore_steps: int = 25, device: int = 0):
         slots, n_samples = _int(slots, "slots"), _int(n_samples, "n_samples")
@@ -98,13 +102,24 @@ class Verifier:
         except Exception:
             pass
 
-    def verify(self, engine, ids_or_detector, model=None):
+    def verify(self, engine, ids_or_detector, model=None, at_event: bool = False, post: int = 0):
         """-> (scores, confirmed): CUDA float32 and int32 tensors, ordered on the current CUDA stream.
         `ids_or_detector`: stream ids of `engine` (a host sequence, or a contiguous 1-D CUDA int32 tensor such as a
         StreamDetector's fired_ids, whose -1 slots give NaN / -1), one result per id; or a detector, one result per event
         slot [capacity] (slot i is drained event i), with `model` = k verifying only model k's events of a
-        MultiModelDetector.  An id outside [0, n_streams) scores NaN; confirmed[i] is the id or -1."""
+        MultiModelDetector.  An id outside [0, n_streams) scores NaN; confirmed[i] is the id or -1.
+        `at_event=True` (a timed detector only): each slot's clip is the n_samples that end at e = min(sample + post,
+        audio_samples_seen), `post` in [0, 2**22] samples after the event (mww_verify_detections_at).  An event younger than
+        `post` is heard with a shorter post-roll; a slot whose clip has left the history ring scores NaN / -1."""
         import torch
+        if at_event:
+            if not isinstance(ids_or_detector, _Detector) or not ids_or_detector.timed:
+                raise ValueError("at_event=True needs a timed detector (timed=True): its events carry their positions")
+            post = _int(post, "post")
+            if not 0 <= post <= MAX_AUDIO_HISTORY:
+                raise ValueError("post must be in [0, %d] (got %d)" % (MAX_AUDIO_HISTORY, post))
+        elif post != 0:
+            raise ValueError("post applies to verify(..., at_event=True) only")
         dev = torch.device("cuda", self.device)
         if getattr(engine, "device", None) != self.device:
             raise ValueError("the engine must be on cuda:%d, the verifier's device" % self.device)
@@ -138,8 +153,11 @@ class Verifier:
         scores = torch.empty(n, dtype=torch.float32, device=dev)
         confirmed = torch.empty(n, dtype=torch.int32, device=dev)
         if isinstance(ids_or_detector, _Detector):
-            self._check(self._L.mww_verify_detections(self._v, engine._h, det._d, -1 if model is None else int(model), scores.data_ptr(),
-                                                      confirmed.data_ptr(), st))
+            k = -1 if model is None else int(model)
+            if at_event:
+                self._check(self._L.mww_verify_detections_at(self._v, engine._h, det._d, k, post, scores.data_ptr(), confirmed.data_ptr(), st))
+            else:
+                self._check(self._L.mww_verify_detections(self._v, engine._h, det._d, k, scores.data_ptr(), confirmed.data_ptr(), st))
             self._last[det] = scores
         else:
             self._check(self._L.mww_verify_streams(self._v, engine._h, ids.data_ptr(), n, scores.data_ptr(), confirmed.data_ptr(), st))
@@ -148,14 +166,14 @@ class Verifier:
     def drain(self, detector):
         """detector.drain() with one more field, `verifier_score`: each event's score from the last verify(engine, detector)
         since the detector's last drain through this verifier, paired by slot; NaN for an event that fired after that verify,
-        for another model's event, and when there was none.  Waits for the current CUDA stream, and clears the detector's
-        events and fired_ids as its drain does."""
+        for another model's event, and when there was none.  A timed detector's events keep their `sample`.  Waits for the
+        current CUDA stream, and clears the detector's events and fired_ids as its drain does."""
         multi = isinstance(detector, MultiModelDetector)
         base, keys = (MODEL_EVENT_DTYPE, ("model", "step", "stream")) if multi else (EVENT_DTYPE, ("step", "stream"))
         ev, n = detector._drain_slots(base)
         scores = self._last.pop(detector, None)
-        out = np.empty(ev.size, np.dtype(base.descr + [("verifier_score", np.float32)]))
-        for name in base.names:
+        out = np.empty(ev.size, np.dtype(ev.dtype.descr + [("verifier_score", np.float32)]))
+        for name in ev.dtype.names:
             out[name] = ev[name]
         out["verifier_score"] = scores[:ev.size].cpu().numpy() if scores is not None else np.nan
         return out[np.lexsort(tuple(out[k] for k in reversed(keys)))], max(n - detector.capacity, 0)
