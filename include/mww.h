@@ -975,6 +975,78 @@ int mww_read_audio_history_at(mww_t *h, const int32_t *d_ids, const long long *d
 int mww_verify_detections_at(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int model, long long post, float *d_scores,
                              int32_t *d_confirmed, void *cu_stream);
 
+/* ---- grouped detection: one detection per household and window ---------------------------------------------------------------
+ * A household with several satellites hears one wake word on several streams at once.  A GROUPED detector gives each row (plain
+ * detector) or global stream (models detector) a group, an id in [0, n_groups) or -1 for none, and stores only the best event
+ * of each group and window, so everything that reads the event buffer (d_fired, positions, anchored verification, endpointer
+ * arming) does the work of one detection.  Rows of group -1 behave exactly as in the ungrouped timed detector.  A models
+ * detector merges per (group, WAKE model): two wake words in one household are two answers; a VAD row never has events.
+ *
+ * Rule.  An update u is one mww_update_detector_at or mww_update_multi_detector_at call, taken per WAKE model k for the models
+ * detector.  It has three positions on the history axis (event positions):
+ *   a_u  where its first step ends: last_end - (n_steps - 1) step_samples (plain), the end of model k's step 0 (models);
+ *   b_u  where its last step ends;
+ *   E_u  the earliest position at which a step of any later update can end: last_end + step_samples (plain), row_end + hop
+ *        (models).
+ * A CANDIDATE is an event the ungrouped timed detector would store for a row of group g.  Each group (each (group, model) of a
+ * models detector) is closed, or open with a deadline D_g and a best candidate.  At every update, for every group:
+ *   1. If g is open and a_u >= D_g, emit its best candidate and close g.  (A models update in which model k ran no step has no
+ *      a_u: step 1 is skipped, which gives what step 3 gives.)
+ *   2. Take g's candidates of this update, if any: if g is open, merge them into the window; if g is closed, open it with
+ *      D_g = p_min + W, p_min the smallest candidate position of this update, and merge them.  The best candidate has the
+ *      highest score; ties go to the earliest position, then to the lowest stream id (then to the lowest row, where a plain
+ *      detector's stream map repeats an id).  The result does not depend on thread scheduling.
+ *   3. If g is open and E_u >= D_g, emit its best candidate and close g.
+ * W (window_samples) is in [0, 2^22].  W = 0 is "at most one event per group per update".  Candidates of an update at or past
+ * D_g still join the window when a_u < D_g: a window closes between updates, never inside one.  A clip call is one update
+ * like any other; the rule is written for live calls, where a window of W samples spans about W / step_samples updates.
+ *
+ * Emit appends the event through the detector's own path: one slot, d_fired and its position, counted past capacity as
+ * every event is.  The event keeps the winner's own stream, step, score and position, so an anchored verify hears the clip
+ * around the winning detection; it is emitted up to W + step_samples after it fired, so a verify `post` of up to about W is
+ * heard in full at the poll, and an endpointer armed from it must replay that far back (lookback_steps).  A grouped event also
+ * records its group and `candidates`, the number of candidates merged into it; an event of a row of group -1 has group -1 and
+ * candidates 1.  Per-row state (moving averages, seen, cooldowns, cutoffs) is bit for bit the ungrouped timed detector's: a
+ * row that lost has still fired as far as its own cooldown is concerned.  Resets do not touch windows.
+ *
+ * Calls (messages in mww_last_error(NULL); refusals are MWW_EINVAL before any device work, detector unchanged):
+ *   - mww_group_detector_events: makes a TIMED detector grouped, for good, every row in group -1 and every group closed.
+ *     n_groups in [1, n_rows] (plain) or [1, n_streams] (models).  Refused while the detector may hold events, as
+ *     mww_time_detector_events is; grouping a grouped detector is refused.
+ *   - mww_set_detector_groups (rows) / mww_set_multi_detector_groups (global stream ids, one group per stream, shared by all
+ *     its WAKE models): the listed ids' groups, ordered on cu_stream.  Ids out of range or listed twice, and groups outside
+ *     [-1, n_groups), are refused.  Groups may change between any two calls; an open window keeps its candidates.
+ *     mww_get_detector_groups / mww_get_multi_detector_groups: every row's or stream's group.
+ *   - The timed updates run the grouped kernels on a grouped detector: two launches (the update, then the close of every
+ *     group), whatever the number of events.  Ungrouped and untimed detectors run exactly the kernels they ran before.
+ *   - mww_flush_detector_groups: emits every open window now (one launch).
+ *   - mww_drain_detector_groups: mww_drain_detector_at plus each event's group and candidates.
+ *   - mww_get_detector_group_windows / mww_set_detector_group_windows: every group slot's window, n_groups x n_wake entries
+ *     (n_wake 1 for a plain detector, its WAKE models for a models detector): slot g n_wake + w, w the index of the WAKE model
+ *     among the WAKE models in model order.  Both wait for the device.  Set refuses open not in {0, 1} and an open window with
+ *     candidates < 1.  With the groups, they are a grouped detector's checkpoint.
+ *   - Moves: detector records carry no windows and no groups (a destination keeps its own groups); export_rows and
+ *     import_rows leave the windows alone.  Drain before a move as always, and flush the source too, or accept that its open
+ *     windows are lost for the streams that leave. */
+typedef struct {
+    int64_t deadline;         /* D_g, when open */
+    int64_t sample, step;     /* the best candidate's position and step */
+    int32_t stream;           /* its stream (global stream id for a models detector) */
+    float score;              /* its score */
+    int32_t candidates;       /* candidates merged into the window */
+    int32_t open;             /* 1: open, 0: closed */
+} mww_group_window;
+int mww_group_detector_events(mww_detector_t *d, int n_groups, long long window_samples);
+int mww_set_detector_groups(mww_detector_t *d, const int32_t *h_rows, const int32_t *h_groups, int n, void *cu_stream);
+int mww_get_detector_groups(mww_detector_t *d, int32_t *h_groups);
+int mww_set_multi_detector_groups(mww_detector_t *d, const int32_t *h_stream_ids, const int32_t *h_groups, int n, void *cu_stream);
+int mww_get_multi_detector_groups(mww_detector_t *d, int32_t *h_groups);
+int mww_flush_detector_groups(mww_detector_t *d, void *cu_stream);
+int mww_drain_detector_groups(mww_detector_t *d, mww_event *h_events, int64_t *h_positions, int32_t *h_groups, int32_t *h_candidates,
+                              int max_events, long long *n_events, void *cu_stream);
+int mww_get_detector_group_windows(mww_detector_t *d, mww_group_window *h_windows);
+int mww_set_detector_group_windows(mww_detector_t *d, const mww_group_window *h_windows);
+
 /* ---- endpointing: where the spoken command after a wake word ends, and its clip from the audio history ----------------------
  * After a wake word a voice assistant sends the command that follows to speech-to-text and stops when the speaker stops.  An
  * ENDPOINTER finds that end on the GPU, per stream, from a VAD model's probabilities, and cuts each command's clip from the

@@ -50,6 +50,9 @@ EXPORTS = (
     "mww_get_resampler_layout", "mww_export_resampled_streams", "mww_import_resampled_streams",
     "mww_time_detector_events", "mww_update_detector_at", "mww_update_multi_detector_at", "mww_get_detector_positions",
     "mww_drain_detector_at", "mww_read_audio_history_at", "mww_verify_detections_at",
+    "mww_group_detector_events", "mww_set_detector_groups", "mww_get_detector_groups", "mww_set_multi_detector_groups",
+    "mww_get_multi_detector_groups", "mww_flush_detector_groups", "mww_drain_detector_groups", "mww_get_detector_group_windows",
+    "mww_set_detector_group_windows",
 )
 
 
@@ -404,6 +407,18 @@ def lib() -> ctypes.CDLL:
     L.mww_read_audio_history_at.argtypes = [vp, vp, vp, i32, i32, vp, ll, vp]
     L.mww_verify_detections_at.restype = i32
     L.mww_verify_detections_at.argtypes = [vp, vp, vp, i32, ll, vp, vp, vp]
+    L.mww_group_detector_events.restype = i32
+    L.mww_group_detector_events.argtypes = [vp, i32, ll]
+    for name in ("mww_set_detector_groups", "mww_set_multi_detector_groups"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, vp, i32, vp]
+    for name in ("mww_get_detector_groups", "mww_get_multi_detector_groups", "mww_get_detector_group_windows", "mww_set_detector_group_windows"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp]
+    L.mww_flush_detector_groups.restype = i32
+    L.mww_flush_detector_groups.argtypes = [vp, vp]
+    L.mww_drain_detector_groups.restype = i32
+    L.mww_drain_detector_groups.argtypes = [vp, vp, vp, vp, vp, i32, ctypes.POINTER(ll), vp]
     _lib = L
     return L
 

@@ -57,6 +57,10 @@ SR_SOURCES = ["mww_serving_records.cu"]
 # history, endpoint and verify libraries keep exactly the kernels they had
 EVP_OUT = os.path.join(HERE, "libmww_event_positions.so")
 EVP_SOURCES = ["mww_event_positions.cu"]
+# and the kernels of grouped detection: the grouped timed updates and the close of every group (mww_group_detector_events), so
+# that every library above keeps exactly the kernels it had
+GRP_OUT = os.path.join(HERE, "libmww_detector_groups.so")
+GRP_SOURCES = ["mww_detector_groups.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -79,7 +83,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, EVP_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, EVP_OUT, GRP_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -101,10 +105,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
                                     (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []), (G711_OUT, G711_SOURCES, []),
                                     (HIST_OUT, HIST_SOURCES, []), (DR_OUT, DR_SOURCES, []), (VER_OUT, VER_SOURCES, []),
                                     (EP_OUT, EP_SOURCES, []), (SR_OUT, SR_SOURCES, []), (EVP_OUT, EVP_SOURCES, []),
+                                    (GRP_OUT, GRP_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
                                                     "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711", "-lmww_history",
                                                     "-lmww_detector_records", "-lmww_verify", "-lmww_endpoint", "-lmww_serving_records",
-                                                    "-lmww_event_positions",
+                                                    "-lmww_event_positions", "-lmww_detector_groups",
                                                     "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra

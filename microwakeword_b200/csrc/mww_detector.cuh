@@ -1,6 +1,7 @@
 // mww_detector.cuh -- the streaming detector's update kernel (rule and both forms: mww_detector.h), included by
 // mww_detector.cu (uniform cutoff), mww_detector_cutoffs.cu (per-row cutoffs, mww_set_detector_cutoffs) and
-// mww_event_positions.cu (the timed kernels, which run the same body and also store each event's position).
+// mww_event_positions.cu (the timed kernels, which run the same body and also store each event's position) and
+// mww_detector_groups.cu (the grouped kernels, which offer a grouped row's events to its group).
 //
 // detector_update_kernel<false, *>, thread per row: the live shape, one or a few steps for very many rows.  State is
 // struct-of-arrays and the history [window - 1][n_rows], so every access of a warp is one coalesced line; a one-step call
@@ -42,15 +43,18 @@ struct PassWindow {
     }
 };
 
-// no positions: the untimed detector stores nothing beside the event
+// no positions: the untimed detector stores nothing beside the event, and every row's events go to the buffer
 struct NoPositions {
+    static constexpr bool kOffers = false;
     MWW_D void put(unsigned long long, int) const {}
 };
 
 // the warp's lanes whose `fire` is set append one event each: one atomicAdd for all of them.  Called by whole warps.  t: the
-// step's index in the call, which a timed detector turns into the event's position (pos.put)
+// step's index in the call, which a timed detector turns into the event's position (pos.put).  Where P::kOffers, pos.keep
+// first decides whether the event goes to the buffer at all (a grouped detector offers a grouped row's event to its group)
 template <typename P>
 MWW_D void append_events(const DetectorArgs &a, bool fire, int row, long long step, float score, const P &pos, int t) {
+    if constexpr (P::kOffers) fire = pos.keep(a, fire, row, score, t);
     const unsigned mask = __ballot_sync(kFull, fire);
     if (mask == 0) return;
     const int lane = threadIdx.x & 31;
@@ -69,9 +73,9 @@ MWW_D void append_events(const DetectorArgs &a, bool fire, int row, long long st
 
 }  // namespace
 
-// The update of one thread (thread form) or one warp (warp form), shared by detector_update_kernel and the timed kernel
-// (mww_event_positions.cu), which differ only in P.  kRowCutoff: the cutoff of row r is row_cutoff[r] (per-row mode);
-// otherwise a.rule.cutoff and row_cutoff is not read.
+// The update of one thread (thread form) or one warp (warp form), shared by detector_update_kernel, the timed kernel
+// (mww_event_positions.cu) and the grouped one (mww_detector_groups.cu), which differ only in P.  kRowCutoff: the cutoff of
+// row r is row_cutoff[r] (per-row mode); otherwise a.rule.cutoff and row_cutoff is not read.
 template <bool kWarpPerRow, bool kRowCutoff, typename P>
 MWW_D void detector_update_rows(const DetectorArgs &a, const float *__restrict__ probs, int n_steps, long long pitch,
                                 const double *__restrict__ row_cutoff, const P &pos) {

@@ -46,6 +46,12 @@ struct mww_detector {
     bool timed = false, updated = false;
     long long *positions = nullptr;
     int hop = kHop;
+    // grouped detection (mww_group_detector_events): the kernels' group arguments (g.positions is `positions`), n_groups, and the
+    // host copy of every row's (plain) or stream's (models) group
+    bool grouped = false;
+    int n_groups = 0;
+    GroupArgs g;
+    std::vector<int32_t> groups;
 };
 
 namespace {
@@ -61,6 +67,7 @@ void detector_free(mww_detector_t *d) {
     }
     cudaFree(d->count); cudaFree(d->events); cudaFree(d->fired); cudaFree(d->d_stream_ids); cudaFree(d->d_rows);
     cudaFree(d->d_models); cudaFree(d->d_models_rows); cudaFree(d->positions);
+    cudaFree(const_cast<int32_t *>(d->g.groups)); cudaFree(d->g.pending); cudaFree(d->g.windows); cudaFree(d->g.ev_group); cudaFree(d->g.ev_candidates);
     delete d;
 }
 
@@ -325,9 +332,10 @@ int check_rows(const mww_detector_t *d, const std::string &call, const int32_t *
     return MWW_OK;
 }
 
-// Both drains: the events (and, h_positions != nullptr, their positions) to the host; the counter cleared, d_fired and a timed
-// detector's positions refilled with -1
-int drain(mww_detector_t *d, mww_event *h_events, long long *h_positions, int max_events, long long *n_events, cudaStream_t st) {
+// The drains: the events (and, h_positions != nullptr, their positions; h_groups != nullptr, their groups and candidates) to the
+// host; the counter cleared, d_fired and a timed detector's positions refilled with -1
+int drain(mww_detector_t *d, mww_event *h_events, long long *h_positions, int max_events, long long *n_events, cudaStream_t st,
+          int32_t *h_groups = nullptr, int32_t *h_candidates = nullptr) {
     DENTER(d);
     unsigned long long count = 0;
     DCU(cudaMemcpyAsync(&count, d->count, sizeof(count), cudaMemcpyDeviceToHost, st));
@@ -336,6 +344,10 @@ int drain(mww_detector_t *d, mww_event *h_events, long long *h_positions, int ma
     const size_t n = std::min(stored, (size_t)max_events);
     if (n) DCU(cudaMemcpyAsync(h_events, d->events, n * sizeof(mww_event), cudaMemcpyDeviceToHost, st));
     if (n && h_positions) DCU(cudaMemcpyAsync(h_positions, d->positions, n * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    if (n && h_groups) {
+        DCU(cudaMemcpyAsync(h_groups, d->g.ev_group, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        DCU(cudaMemcpyAsync(h_candidates, d->g.ev_candidates, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    }
     if (stored) {
         DCU(cudaMemsetAsync(d->count, 0, sizeof(count), st));
         DCU(cudaMemsetAsync(d->fired, 0xFF, stored * sizeof(int32_t), st));
@@ -354,6 +366,43 @@ int untimed_arg(const mww_detector_t *d, const char *call, const char *timed_cal
 }
 int timed_arg(const mww_detector_t *d, const char *call) {
     if (!d->timed) return refuse(std::string(call) + ": the detector is not timed: call mww_time_detector_events after create or a drain");
+    return MWW_OK;
+}
+
+// ---- grouped detection
+int grouped_arg(const mww_detector_t *d, const std::string &call) {
+    if (!d) return refuse(call + ": detector is NULL");
+    if (!d->grouped) return refuse(call + ": the detector is not grouped (mww_group_detector_events)");
+    return MWW_OK;
+}
+
+// ids a grouped detector keys groups by: rows (plain) or global stream ids (models); its group slots
+int group_ids(const mww_detector_t *d) { return d->multi ? d->m.n_streams : d->sets[0].n_rows; }
+int group_slots(const mww_detector_t *d) { return d->g.n_slots; }
+
+// the listed ids' groups, checked before anything changes: ids in range and listed once, groups in [-1, n_groups); then the
+// span of ids the call touched is copied on cu_stream
+int set_groups(mww_detector_t *d, const std::string &call, const int32_t *h_ids, const int32_t *h_groups, int n, void *cu_stream) {
+    if (int rc = grouped_arg(d, call)) return rc;
+    if (n < 0) return refuse(call + ": n must not be negative");
+    if (n == 0) return MWW_OK;
+    if (!h_ids || !h_groups) return refuse(call + ": ids and h_groups must not be NULL");
+    const int n_ids = group_ids(d);
+    std::vector<char> listed((size_t)n_ids, 0);
+    int lo = n_ids, hi = -1;
+    for (int i = 0; i < n; ++i) {
+        const int32_t id = h_ids[i], grp = h_groups[i];
+        if (id < 0 || id >= n_ids) return refuse(call + ": id " + std::to_string(id) + " out of range");
+        if (listed[id]) return refuse(call + ": id " + std::to_string(id) + " listed twice");
+        if (grp < -1 || grp >= d->n_groups) return refuse(call + ": group " + std::to_string(grp) + " outside [-1, n_groups)");
+        listed[id] = 1;
+        lo = std::min(lo, (int)id); hi = std::max(hi, (int)id);
+    }
+    DENTER(d);
+    for (int i = 0; i < n; ++i) d->groups[h_ids[i]] = h_groups[i];
+    // from pageable memory: the call returns once the span is staged
+    DCU(cudaMemcpyAsync(const_cast<int32_t *>(d->g.groups) + lo, d->groups.data() + lo, (size_t)(hi - lo + 1) * sizeof(int32_t), cudaMemcpyHostToDevice,
+                        static_cast<cudaStream_t>(cu_stream)));
     return MWW_OK;
 }
 
@@ -642,8 +691,9 @@ int mww_update_detector_at(mww_detector_t *d, const float *d_probs, int n_steps,
     if (step_samples < 1) return refuse(std::string(call) + ": step_samples must be at least 1");
     if (n_steps == 0) return MWW_OK;
     DENTER(d);
-    DCU(launch_detector_update_at(d->a, d->per_row ? d->sets[0].d_cutoffs : nullptr, d_probs, n_steps, pitch, d->positions, last_end, step_samples,
-                                  static_cast<cudaStream_t>(cu_stream)));
+    const double *cut = d->per_row ? d->sets[0].d_cutoffs : nullptr;
+    if (d->grouped) DCU(launch_detector_update_grouped(d->a, cut, d_probs, n_steps, pitch, d->g, last_end, step_samples, static_cast<cudaStream_t>(cu_stream)));
+    else DCU(launch_detector_update_at(d->a, cut, d_probs, n_steps, pitch, d->positions, last_end, step_samples, static_cast<cudaStream_t>(cu_stream)));
     d->updated = true;
     return MWW_OK;
 }
@@ -662,13 +712,20 @@ int mww_update_multi_detector_at(mww_detector_t *d, const float *const *d_probs,
     if (R < 0)
         return refuse(call + ": the step counts and pending rows before and after do not describe one call "
                       "(R = n_k s_k - p_k + g_k with 0 <= p_k, g_k < s_k, the same R >= 0 for every model)");
-    if (!any) return MWW_OK;
+    // a grouped detector closes its windows at every call that moved the clock, even one in which no model ran a step
+    if (!any && !(d->grouped && R > 0)) return MWW_OK;
     DENTER(d);
     for (int k = 0; k < m.n_models; ++k) m.call[k] = c[k];
     const long long row0 = event_row0_end(row_end, d->hop, R);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    if (d->per_row) DCU(launch_detector_models_update_at(detect_args_rows(m, d->d_models_rows), d->positions, row0, d->hop, st));
-    else DCU(launch_detector_models_update_at(m, d->positions, row0, d->hop, st));
+    if (d->grouped) {
+        if (d->per_row) DCU(launch_detector_models_update_grouped(detect_args_rows(m, d->d_models_rows), m, d->g, row0, row_end, d->hop, st));
+        else DCU(launch_detector_models_update_grouped(m, d->g, row0, row_end, d->hop, st));
+    } else if (d->per_row) {
+        DCU(launch_detector_models_update_at(detect_args_rows(m, d->d_models_rows), d->positions, row0, d->hop, st));
+    } else {
+        DCU(launch_detector_models_update_at(m, d->positions, row0, d->hop, st));
+    }
     d->updated = true;
     return MWW_OK;
 }
@@ -685,6 +742,117 @@ int mww_drain_detector_at(mww_detector_t *d, mww_event *h_events, int64_t *h_pos
         return refuse("mww_drain_detector_at: needs a detector, n_events and room for max_events >= 0 events and positions");
     if (int rc = timed_arg(d, "mww_drain_detector_at")) return rc;
     return drain(d, h_events, reinterpret_cast<long long *>(h_positions), max_events, n_events, static_cast<cudaStream_t>(cu_stream));
+}
+
+// ---- grouped detection (both kinds)
+int mww_group_detector_events(mww_detector_t *d, int n_groups, long long window_samples) {
+    const std::string call = "mww_group_detector_events";
+    if (!d) return refuse(call + ": detector is NULL");
+    if (!d->timed) return refuse(call + ": only a timed detector can be grouped (mww_time_detector_events)");
+    if (d->grouped) return refuse(call + ": the detector is already grouped");
+    if (d->updated) return refuse(call + ": the detector may hold events: group it after create or a drain, before any update");
+    const int n_ids = group_ids(d);
+    if (n_groups < 1 || n_groups > n_ids)
+        return refuse(call + ": n_groups must be in [1, " + std::to_string(n_ids) + (d->multi ? "] (n_streams)" : "] (n_rows)"));
+    if (window_samples < 0 || window_samples > (1LL << 22)) return refuse(call + ": window_samples must be in [0, 2^22]");
+    DENTER(d);
+    GroupArgs g;
+    g.positions = d->positions;
+    g.window = window_samples;
+    g.n_wake = d->multi ? d->m.n_wake : 1;
+    g.n_slots = n_groups * g.n_wake;
+    for (int w = 0; w < g.n_wake && d->multi; ++w) g.wake_of[d->m.wake[w]] = (int8_t)w;
+    auto undo = [&](cudaError_t e, const char *what) {
+        cudaFree(const_cast<int32_t *>(g.groups)); cudaFree(g.pending); cudaFree(g.windows); cudaFree(g.ev_group); cudaFree(g.ev_candidates);
+        return cuda_fail(nullptr, e, what);
+    };
+    const size_t S = (size_t)g.n_slots, C = (size_t)d->capacity;
+    int32_t *groups = nullptr;
+    if (cudaError_t e = cudaMalloc(&groups, (size_t)n_ids * sizeof(int32_t))) return undo(e, "cudaMalloc");
+    g.groups = groups;
+    if (cudaError_t e = cudaMalloc(&g.pending, S * sizeof(GroupPending))) return undo(e, "cudaMalloc");
+    if (cudaError_t e = cudaMalloc(&g.windows, S * sizeof(mww_group_window))) return undo(e, "cudaMalloc");
+    if (cudaError_t e = cudaMalloc(&g.ev_group, C * sizeof(int32_t))) return undo(e, "cudaMalloc");
+    if (cudaError_t e = cudaMalloc(&g.ev_candidates, C * sizeof(int32_t))) return undo(e, "cudaMalloc");
+    const std::vector<GroupPending> pending(S);
+    if (cudaError_t e = cudaMemset(groups, 0xFF, (size_t)n_ids * sizeof(int32_t))) return undo(e, "cudaMemset");
+    if (cudaError_t e = cudaMemcpy(g.pending, pending.data(), S * sizeof(GroupPending), cudaMemcpyHostToDevice)) return undo(e, "cudaMemcpy");
+    if (cudaError_t e = cudaMemset(g.windows, 0, S * sizeof(mww_group_window))) return undo(e, "cudaMemset");
+    d->g = g;
+    d->groups.assign((size_t)n_ids, -1);
+    d->n_groups = n_groups;
+    d->grouped = true;
+    return MWW_OK;
+}
+
+int mww_set_detector_groups(mww_detector_t *d, const int32_t *h_rows, const int32_t *h_groups, int n, void *cu_stream) {
+    if (int rc = plain_arg(d, "mww_set_detector_groups", "mww_set_multi_detector_groups")) return rc;
+    return set_groups(d, "mww_set_detector_groups", h_rows, h_groups, n, cu_stream);
+}
+
+int mww_set_multi_detector_groups(mww_detector_t *d, const int32_t *h_stream_ids, const int32_t *h_groups, int n, void *cu_stream) {
+    if (int rc = models_arg(d, "mww_set_multi_detector_groups")) return rc;
+    return set_groups(d, "mww_set_multi_detector_groups", h_stream_ids, h_groups, n, cu_stream);
+}
+
+int mww_get_detector_groups(mww_detector_t *d, int32_t *h_groups) {
+    if (int rc = plain_arg(d, "mww_get_detector_groups", "mww_get_multi_detector_groups")) return rc;
+    if (int rc = grouped_arg(d, "mww_get_detector_groups")) return rc;
+    if (!h_groups) return refuse("mww_get_detector_groups: h_groups is NULL");
+    std::copy(d->groups.begin(), d->groups.end(), h_groups);
+    return MWW_OK;
+}
+
+int mww_get_multi_detector_groups(mww_detector_t *d, int32_t *h_groups) {
+    if (int rc = models_arg(d, "mww_get_multi_detector_groups")) return rc;
+    if (int rc = grouped_arg(d, "mww_get_multi_detector_groups")) return rc;
+    if (!h_groups) return refuse("mww_get_multi_detector_groups: h_groups is NULL");
+    std::copy(d->groups.begin(), d->groups.end(), h_groups);
+    return MWW_OK;
+}
+
+int mww_flush_detector_groups(mww_detector_t *d, void *cu_stream) {
+    if (int rc = grouped_arg(d, "mww_flush_detector_groups")) return rc;
+    DENTER(d);
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    if (d->multi) DCU(launch_detector_models_groups_flush(d->m, d->g, st));
+    else DCU(launch_detector_groups_flush(d->a, d->g, st));
+    d->updated = true;
+    return MWW_OK;
+}
+
+int mww_drain_detector_groups(mww_detector_t *d, mww_event *h_events, int64_t *h_positions, int32_t *h_groups, int32_t *h_candidates,
+                              int max_events, long long *n_events, void *cu_stream) {
+    if (!d || !n_events || max_events < 0 || (max_events > 0 && (!h_events || !h_positions || !h_groups || !h_candidates)))
+        return refuse("mww_drain_detector_groups: needs a detector, n_events and room for max_events >= 0 events, positions, groups and "
+                      "candidates");
+    if (int rc = grouped_arg(d, "mww_drain_detector_groups")) return rc;
+    return drain(d, h_events, reinterpret_cast<long long *>(h_positions), max_events, n_events, static_cast<cudaStream_t>(cu_stream), h_groups,
+                 h_candidates);
+}
+
+int mww_get_detector_group_windows(mww_detector_t *d, mww_group_window *h_windows) {
+    if (int rc = grouped_arg(d, "mww_get_detector_group_windows")) return rc;
+    if (!h_windows) return refuse("mww_get_detector_group_windows: h_windows is NULL");
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    DCU(cudaMemcpy(h_windows, d->g.windows, (size_t)group_slots(d) * sizeof(mww_group_window), cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+
+int mww_set_detector_group_windows(mww_detector_t *d, const mww_group_window *h_windows) {
+    const std::string call = "mww_set_detector_group_windows";
+    if (int rc = grouped_arg(d, call)) return rc;
+    if (!h_windows) return refuse(call + ": h_windows is NULL");
+    for (int s = 0; s < group_slots(d); ++s) {
+        const mww_group_window &w = h_windows[s];
+        if (w.open != 0 && w.open != 1) return refuse(call + ": slot " + std::to_string(s) + ": open must be 0 or 1");
+        if (w.open && w.candidates < 1) return refuse(call + ": slot " + std::to_string(s) + ": an open window needs candidates >= 1");
+    }
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    DCU(cudaMemcpy(d->g.windows, h_windows, (size_t)group_slots(d) * sizeof(mww_group_window), cudaMemcpyHostToDevice));
+    return MWW_OK;
 }
 
 }  // extern "C"

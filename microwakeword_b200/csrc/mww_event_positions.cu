@@ -19,6 +19,7 @@ struct StepPositions {
     long long *out;
     long long last_end, step_samples;
     int n;
+    static constexpr bool kOffers = false;
     MWW_D void put(unsigned long long slot, int t) const { out[slot] = event_step_end(last_end, step_samples, n, t); }
 };
 

@@ -244,3 +244,19 @@ cudaError_t launch_history_read_at(const int16_t *ring, int C, long long seen, c
 cudaError_t launch_verify_slots_at(const long long *count, const mww_event *events, const long long *positions, int capacity, int model,
                                    long long post, long long seen, int C, int n_samples, int32_t *ids, long long *ends, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_detector_groups.h"
+namespace mww {
+// grouped detection (mww_detector_groups.cu, key, offer and close in mww_detector_groups.h; companion library
+// libmww_detector_groups.so).  An update is two launches, the timed update whose grouped rows offer their events to their
+// group slots and the close of every slot; a flush is the close alone.
+cudaError_t launch_detector_update_grouped(const DetectorArgs &a, const double *row_cutoff, const float *probs, int n_steps, long long pitch,
+                                           const GroupArgs &g, long long last_end, long long step_samples, cudaStream_t st);
+cudaError_t launch_detector_models_update_grouped(const DetectModelsArgs &a, const GroupArgs &g, long long row0_end, long long row_end, int hop,
+                                                  cudaStream_t st);
+// per-row mode: the update over per-row descriptors, the close over `base` (the uniform descriptors, for seen and stride)
+cudaError_t launch_detector_models_update_grouped(const DetectModelsArgsT<DetectModelRows> &a, const DetectModelsArgs &base, const GroupArgs &g,
+                                                  long long row0_end, long long row_end, int hop, cudaStream_t st);
+cudaError_t launch_detector_groups_flush(const DetectorArgs &a, const GroupArgs &g, cudaStream_t st);
+cudaError_t launch_detector_models_groups_flush(const DetectModelsArgs &a, const GroupArgs &g, cudaStream_t st);
+}  // namespace mww

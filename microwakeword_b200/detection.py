@@ -315,6 +315,32 @@ def timed_dtype(dtype) -> np.dtype:
     return np.dtype(dtype.descr + [("sample", np.int64)])
 
 
+def grouped_dtype(dtype) -> np.dtype:
+    """the drain dtype of a grouped detector: timed_dtype(dtype) and the int32 `group` and `candidates` of each event (group -1
+    and candidates 1 for an event of an ungrouped row)"""
+    return np.dtype(timed_dtype(dtype).descr + [("group", np.int32), ("candidates", np.int32)])
+
+
+# mww_group_window of include/mww.h: one group slot's window
+GROUP_WINDOW_DTYPE = np.dtype([("deadline", np.int64), ("sample", np.int64), ("step", np.int64), ("stream", np.int32), ("score", np.float32),
+                               ("candidates", np.int32), ("open", np.int32)])
+
+
+def _group_list(ids, groups, name):
+    """(int32 ids, int32 groups) of one set-groups call, or ValueError: ids a 1-D integer sequence, groups one integer or one per id"""
+    i = _record_ids(ids, name)
+    g = np.asarray(groups)
+    if g.dtype == bool or not (np.issubdtype(g.dtype, np.integer) or g.size == 0):
+        raise ValueError("groups must be integers")
+    if g.ndim == 0:
+        g = np.full(i.size, g, np.int64)
+    if g.shape != i.shape:
+        raise ValueError("groups must be one value or one per entry of %s (%d)" % (name, i.size))
+    if g.size and (g.min() < np.iinfo(np.int32).min or g.max() > np.iinfo(np.int32).max):
+        raise ValueError("groups must fit in int32")
+    return i, np.ascontiguousarray(g, np.int32)
+
+
 def _history_clock(engine, model):
     """(samples_seen S, b, hop) of an engine with an audio history, read now: its newest feature row's window ends at history
     sample S - b (include/mww.h, "event positions"); ValueError without a history, on which positions mean nothing"""
@@ -345,6 +371,7 @@ class _Detector:
             self.event_count = torch.as_tensor(_DeviceArray(self._handle, count.value, 1, "<i8"), device=dev)
         self.timed = False
         self.event_samples = None
+        self.n_groups, self.group_window = 0, 0
 
     def _time(self) -> None:
         """make the detector timed (mww_time_detector_events) and make event_samples, the device view of the positions"""
@@ -358,6 +385,76 @@ class _Detector:
             # unused slots)
             self.event_samples = torch.as_tensor(_DeviceArray(self._handle, ptr.value, self.capacity, "<i8"), device=dev)
         self.timed = True
+
+    @staticmethod
+    def _group_args(timed: bool, groups, group_window) -> None:
+        """ValueError unless groups is None, or an integer with timed and an integer group_window"""
+        if groups is None:
+            return
+        if not timed:
+            raise ValueError("groups need a timed detector (timed=True): the rule places every detection on the audio history's axis")
+        for v, name in ((groups, "groups"), (group_window, "group_window")):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise ValueError("%s must be an integer (got %r)" % (name, v))
+
+    def _group(self, groups, group_window) -> None:
+        """make a timed detector grouped (mww_group_detector_events): `groups` groups, windows of `group_window` samples"""
+        if groups is None:
+            return
+        self._check(self._L.mww_group_detector_events(self._d, int(groups), int(group_window)))
+        self.n_groups, self.group_window = int(groups), int(group_window)
+
+    @property
+    def grouped(self) -> bool:
+        return self.n_groups > 0
+
+    def _n_group_slots(self) -> int:
+        return self.n_groups * (sum(r == _lib.MWW_DETECT_WAKE for r in self.roles) if hasattr(self, "roles") else 1)
+
+    def flush(self) -> None:
+        """Emit every open group window now (mww_flush_detector_groups): before a final drain, or before moving streams out
+        of this detector.  Ordered on the current CUDA stream; one launch."""
+        self._check(self._L.mww_flush_detector_groups(self._d, self._cuda_stream()))
+
+    def group_windows(self) -> np.ndarray:
+        """GROUP_WINDOW_DTYPE [group slots]: each group's open window (slot g n_wake + w of a models detector, w the WAKE model's
+        index among the WAKE models); waits for the device"""
+        out = np.zeros(self._n_group_slots(), GROUP_WINDOW_DTYPE)
+        self._check(self._L.mww_get_detector_group_windows(self._d, out.ctypes.data))
+        return out
+
+    def _group_state(self, d: dict) -> dict:
+        if self.grouped:
+            d["groups"] = self.groups
+            d["group_windows"] = self.group_windows()
+        return d
+
+    def _load_group_state(self, d: dict):
+        """the checked (groups, windows) of a state dict, to apply with _apply_group_state once every other part is checked"""
+        if not self.grouped:
+            if "groups" in d:
+                raise ValueError("the state holds groups; this detector is not grouped")
+            return None
+        if "groups" not in d or "group_windows" not in d:
+            raise ValueError("a grouped detector's state holds groups and group_windows")
+        g = np.ascontiguousarray(d["groups"], np.int32)
+        w = np.ascontiguousarray(d["group_windows"], GROUP_WINDOW_DTYPE)
+        if g.shape != self.groups.shape or w.shape != (self._n_group_slots(),):
+            raise ValueError("groups must be [%d] and group_windows [%d]" % (self.groups.size, self._n_group_slots()))
+        if g.size and (g.min() < -1 or g.max() >= self.n_groups):
+            raise ValueError("groups must be in [-1, %d)" % self.n_groups)
+        if not np.isin(w["open"], (0, 1)).all() or (w["candidates"][w["open"] == 1] < 1).any():
+            raise ValueError("group_windows: open must be 0 or 1, and an open window needs candidates >= 1")
+        return g, w
+
+    def _apply_group_state(self, gw) -> None:
+        if gw is None:
+            return
+        g, w = gw
+        ids = np.arange(g.size, dtype=np.int32)
+        fn = self._L.mww_set_multi_detector_groups if hasattr(self, "roles") else self._L.mww_set_detector_groups
+        self._check(fn(self._d, ids.ctypes.data, g.ctypes.data, g.size, self._cuda_stream()))
+        self._check(self._L.mww_set_detector_group_windows(self._d, w.ctypes.data))
 
     def _check(self, rc: int) -> None:
         if rc != 0:
@@ -385,13 +482,20 @@ class _Detector:
             self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
             return buf[:min(n.value, self.capacity)], n.value
         pos = np.empty(self.capacity, np.int64)
-        self._check(self._L.mww_drain_detector_at(self._d, buf.ctypes.data, pos.ctypes.data, self.capacity, ctypes.byref(n),
-                                                  self._cuda_stream()))
+        if self.grouped:
+            grp, cand = np.empty(self.capacity, np.int32), np.empty(self.capacity, np.int32)
+            self._check(self._L.mww_drain_detector_groups(self._d, buf.ctypes.data, pos.ctypes.data, grp.ctypes.data, cand.ctypes.data,
+                                                          self.capacity, ctypes.byref(n), self._cuda_stream()))
+        else:
+            self._check(self._L.mww_drain_detector_at(self._d, buf.ctypes.data, pos.ctypes.data, self.capacity, ctypes.byref(n),
+                                                      self._cuda_stream()))
         m = min(n.value, self.capacity)
-        out = np.empty(m, timed_dtype(dtype))
+        out = np.empty(m, grouped_dtype(dtype) if self.grouped else timed_dtype(dtype))
         for name in dtype.names:
             out[name] = buf[name][:m]
         out["sample"] = pos[:m]
+        if self.grouped:
+            out["group"], out["candidates"] = grp[:m], cand[:m]
         return out, n.value
 
     def _drain(self, dtype, keys):
@@ -468,10 +572,16 @@ class StreamDetector(_Detector):
         eng.set_audio_history(48000)
         det = StreamDetector(eng.n_streams, cutoff=0.9, timed=True)
         det.update(eng.step(chunk), eng)
-        clips = eng.audio_history(det.fired_ids, 24000, end=det.event_samples)   # the 1.5 s before each detection"""
+        clips = eng.audio_history(det.fired_ids, 24000, end=det.event_samples)   # the 1.5 s before each detection
+
+    `groups=n` (timed only) answers a wake word once per household (include/mww.h, "grouped detection"): set_groups puts rows
+    in groups [0, n) (-1: none, the default), and of the detections of one group that start within `group_window` samples
+    only the best is stored, up to group_window + one step after it fired; drain adds `group` and `candidates`, and flush()
+    stores the windows still open.  Every row's state, cooldown included, is what the ungrouped detector's would be."""
 
     def __init__(self, n_rows: int, cutoff: float, window: int = 5, cooldown_slices: int = 25, capacity: int = 65536,
-                 stream_ids=None, device: int = 0, timed: bool = False):
+                 stream_ids=None, device: int = 0, timed: bool = False, groups=None, group_window: int = 0):
+        self._group_args(timed, groups, group_window)
         self._L = _lib.lib()
         d = ctypes.c_void_p()
         ids = None
@@ -485,6 +595,7 @@ class StreamDetector(_Detector):
         self.n_rows, self.window, self.cutoff, self.cooldown_slices = int(n_rows), int(window), float(cutoff), int(cooldown_slices)
         if timed:
             self._time()
+        self._group(groups, group_window)
 
     def update(self, probs, engine=None, model=None) -> None:
         """CUDA float32 [n_rows, steps], any row pitch (a slice of a wider buffer is read in place); zero columns: nothing
@@ -521,8 +632,8 @@ class StreamDetector(_Detector):
             self._check(self._L.mww_detector_update(self._d, probs.data_ptr(), n, pitch, _stream(probs.device)))
 
     def drain(self):
-        """-> (events, dropped): the events since the last drain as a structured array (EVENT_DTYPE, and `sample` for a timed
-        detector) sorted by (step, stream), and how many more fired than `capacity` could hold.  Waits for the current CUDA
+        """-> (events, dropped): the events since the last drain as a structured array (EVENT_DTYPE, `sample` for a timed
+        detector, `group` and `candidates` for a grouped one) sorted by (step, stream), and how many more fired than `capacity` could hold.  Waits for the current CUDA
         stream; clears the event buffer and fired_ids."""
         return self._drain(EVENT_DTYPE, ("step", "stream"))
 
@@ -532,10 +643,12 @@ class StreamDetector(_Detector):
         self._reset(rows, "row indices")
 
     def state_dict(self) -> dict:
+        """{hist [n_rows, window - 1], seen [n_rows], cooldown [n_rows]}, and a grouped detector's groups [n_rows] and
+        group_windows (GROUP_WINDOW_DTYPE [groups])"""
         d = dict(hist=np.zeros((self.n_rows, self.window - 1), np.float32), seen=np.zeros(self.n_rows, np.int64),
                  cooldown=np.zeros(self.n_rows, np.int32))
         self._check(self._L.mww_detector_get_state(self._d, d["hist"].ctypes.data, d["seen"].ctypes.data, d["cooldown"].ctypes.data))
-        return d
+        return self._group_state(d)
 
     def load_state_dict(self, d: dict) -> None:
         hist = np.ascontiguousarray(d["hist"], np.float32)
@@ -543,7 +656,22 @@ class StreamDetector(_Detector):
         cooldown = np.ascontiguousarray(d["cooldown"], np.int32)
         if hist.shape != (self.n_rows, self.window - 1) or seen.shape != (self.n_rows,) or cooldown.shape != (self.n_rows,):
             raise ValueError("state must be hist [n_rows, window - 1], seen [n_rows], cooldown [n_rows]")
+        gw = self._load_group_state(d)
         self._check(self._L.mww_detector_set_state(self._d, hist.ctypes.data, seen.ctypes.data, cooldown.ctypes.data))
+        self._apply_group_state(gw)
+
+    def set_groups(self, rows, groups) -> None:
+        """Put the listed ROW indices in `groups` (one value or one per row; -1: no group) (mww_set_detector_groups).  Ordered
+        on the current CUDA stream: updates after it use the new groups.  An open window keeps its candidates."""
+        r, g = _group_list(rows, groups, "rows")
+        self._check(self._L.mww_set_detector_groups(self._d, r.ctypes.data, g.ctypes.data, r.size, self._cuda_stream()))
+
+    @property
+    def groups(self) -> np.ndarray:
+        """int32 [n_rows]: every row's group, -1 for none"""
+        out = np.empty(self.n_rows, np.int32)
+        self._check(self._L.mww_get_detector_groups(self._d, out.ctypes.data))
+        return out
 
 
     def set_cutoffs(self, rows, cutoffs) -> None:
@@ -640,9 +768,14 @@ class MultiModelDetector(_Detector):
         new.import_streams(all_ids, det.export_streams(all_ids))
 
     `timed=True` places every event on the engine's audio history axis, as StreamDetector's does: update reads the clock from
-    the engine, which must keep an audio history, drain adds `sample` and event_samples is the device view."""
+    the engine, which must keep an audio history, drain adds `sample` and event_samples is the device view.
 
-    def __init__(self, engine, cutoffs, windows=5, cooldown_slices: int = 25, vad=None, capacity: int = 65536, timed: bool = False):
+    `groups=n` (timed only) groups streams as StreamDetector's does, per (group, WAKE model): set_groups takes global stream
+    ids, one group per stream for all its wake words."""
+
+    def __init__(self, engine, cutoffs, windows=5, cooldown_slices: int = 25, vad=None, capacity: int = 65536, timed: bool = False,
+                 groups=None, group_window: int = 0):
+        self._group_args(timed, groups, group_window)
         K = engine.n_models
         cutoffs = _per_model(cutoffs, K, "cutoffs")
         windows = _per_model(windows, K, "windows")
@@ -670,6 +803,20 @@ class MultiModelDetector(_Detector):
         self._hop = int(engine.hop)
         if timed:
             self._time()
+        self._group(groups, group_window)
+
+    def set_groups(self, stream_ids, groups) -> None:
+        """Put the listed GLOBAL streams in `groups` (one value or one per stream; -1: no group), for every WAKE model
+        (mww_set_multi_detector_groups).  Ordered on the current CUDA stream; an open window keeps its candidates."""
+        i, g = _group_list(stream_ids, groups, "stream_ids")
+        self._check(self._L.mww_set_multi_detector_groups(self._d, i.ctypes.data, g.ctypes.data, i.size, self._cuda_stream()))
+
+    @property
+    def groups(self) -> np.ndarray:
+        """int32 [n_streams]: every stream's group, -1 for none"""
+        out = np.empty(self.engine.n_streams, np.int32)
+        self._check(self._L.mww_get_multi_detector_groups(self._d, out.ctypes.data))
+        return out
 
     @property
     def pending_rows(self) -> list:
@@ -802,7 +949,8 @@ class MultiModelDetector(_Detector):
         return "active" if self.roles[k] == _lib.MWW_DETECT_VAD else "cooldown"
 
     def state_dict(self) -> dict:
-        """{pending_rows: [p_k], models: [None for an OFF model, else {hist [n_k, window - 1], seen [n_k], cooldown or active [n_k]}]}"""
+        """{pending_rows: [p_k], models: [None for an OFF model, else {hist [n_k, window - 1], seen [n_k], cooldown or active [n_k]}]},
+        and a grouped detector's groups [n_streams] and group_windows (GROUP_WINDOW_DTYPE [groups x WAKE models])"""
         models = []
         for k in range(self.n_models):
             if self.roles[k] == _lib.MWW_DETECT_OFF:
@@ -812,7 +960,7 @@ class MultiModelDetector(_Detector):
             m = {"hist": np.zeros((n, self.windows[k] - 1), np.float32), "seen": np.zeros(n, np.int64), self._flag_name(k): np.zeros(n, np.int32)}
             self._check(self._L.mww_multi_detector_get_state(self._d, k, m["hist"].ctypes.data, m["seen"].ctypes.data, m[self._flag_name(k)].ctypes.data))
             models.append(m)
-        return dict(pending_rows=list(self._pending), models=models)
+        return self._group_state(dict(pending_rows=list(self._pending), models=models))
 
     def load_state_dict(self, d: dict) -> None:
         if len(d["models"]) != self.n_models or len(d["pending_rows"]) != self.n_models:
@@ -834,7 +982,9 @@ class MultiModelDetector(_Detector):
             if (seen < 0).any() or (f < 0).any() or (f > hi).any():       # checked for every model before any is written
                 raise ValueError("model %d: seen must not be negative and %s must be in [0, %d]" % (k, flag, hi))
             arrays.append((hist, seen, f))
+        gw = self._load_group_state(d)
         for k, a in enumerate(arrays):
             if a is not None:
                 self._check(self._L.mww_multi_detector_set_state(self._d, k, a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data))
+        self._apply_group_state(gw)
         self._pending = [int(p) for p in d["pending_rows"]]
