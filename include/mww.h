@@ -1047,6 +1047,100 @@ int mww_drain_detector_groups(mww_detector_t *d, mww_event *h_events, int64_t *h
 int mww_get_detector_group_windows(mww_detector_t *d, mww_group_window *h_windows);
 int mww_set_detector_group_windows(mww_detector_t *d, const mww_group_window *h_windows);
 
+/* ---- media guard: suppress the detections that many households, or a registered media clip, heard alike ---------------------
+ * A TV advert, a podcast or a broadcast that says the wake word makes thousands of households fire within a second, and every
+ * one of those detections is a true positive for the wake model and the verifier.  A broadcast is the same audio heard in many
+ * homes at once; a MEDIA GUARD fingerprints each detection's clip and takes the ones that match other households' recent
+ * detections, or a registered media clip, out of what gets armed.  Like a verifier it works on slots.  Slot i has a stream id,
+ * an end position e_i, a position P_i on the history axis (event positions) and a household h_i.
+ *
+ * Clip.  The n_samples 16 kHz samples [e_i - n_samples, e_i) of that stream's audio history, what mww_read_audio_history_at
+ * returns.  A slot is INVALID when its id is -1 or outside [0, src.n_streams), when it holds another model's event, or when its
+ * clip has partly left the ring: e_i - n_samples < S - C (S = src's samples_seen when the call is enqueued, C its capacity).
+ *   - mww_media_check_streams: d_ids[i], e_i = P_i = d_ends[i], h_i = d_households[i] (-1 for every slot when d_households is
+ *     NULL).
+ *   - mww_media_check_detections_at: event slot i of a timed detector, as mww_verify_detections_at takes it: the event's stream,
+ *     P_i its position, e_i = min(P_i + post, S); h_i the event's group on a grouped detector, -1 on an ungrouped one (so every
+ *     stream is its own household).
+ * Features.  F = the rows a fresh frontend (the guard's own frontend-only handle after mww_reset(NULL)) emits from one
+ * mww_features call over the clip: T = (n_samples - 480) / 160 + 1 rows of 40 uint16 values, the verifier's fresh frontend
+ * per clip.
+ * Fingerprint.  One uint64 word per frame t in [1, T): bit c, c in [0, 39), is set when the int32 value
+ *     (F[t][c] - F[t][c+1]) - (F[t-1][c] - F[t-1][c+1]) > 0
+ * (the Haitsma-Kalker energy-difference sign); bits 39..63 are zero.  A clip has W = T - 1 words.
+ * Distance.  For fingerprints x (n_x words) and y (n_y words) at lag l, the overlap O(l) = #{t : 0 <= t < n_x, 0 <= t + l < n_y}
+ * and the mismatches m(l) = sum over it of popcount(x[t] XOR y[t + l]).  x and y MATCH when some allowed l has O(l) >=
+ * min_overlap and m(l) 1000 <= max_ber_milli 39 O(l): integers, so the result is exact.  Between two detections the allowed
+ * lags are |l| <= max_lag frames (the jitter between where different households' detectors fire on the same content);
+ * against a registered clip every l with O(l) >= min_overlap is allowed, so the clip may sit anywhere in a long advert.
+ * Rule of one check call.  For each valid slot i:
+ *   - matches[i] = the number of candidates j that are (1) one of this call's other valid slots or one of the ring's entries,
+ *     (2) in another household -- two events are in one household when h_i == h_j >= 0, or h_i == h_j == -1 on one stream --,
+ *     (3) within |P_j - P_i| <= window_samples, and (4) match i;
+ *   - media[i] = bit 0 when i matches any registered clip | bit 1 when matches[i] >= min_matches;
+ *   - passed[i] = -1 when media[i] != 0, else d_confirmed[i], or the slot's stream id when d_confirmed is NULL: it goes
+ *     straight into mww_endpointer_arm_device.
+ * An invalid slot gives matches -1, media 0, and passed its confirmed id: the guard never blocks what it cannot hear.  A slot's
+ * stream id is d_ids[i], or the event's stream (-1 for an unused slot or another model's event).
+ * Ring.  After matching, every valid slot is appended to a ring of `ring` entries in slot order, flagged or not: its
+ * fingerprint, stream, household and P.  When the ring is full the oldest entry is overwritten.  So a detection is matched
+ * against the ones of earlier checks within the window, however the polls cut the wave.
+ *
+ * Rule fields (mww_media_rule; fixed at create):  n_samples in [640, 160000]; max_lag in [0, 64]; min_overlap in [1, W] with
+ * max_lag <= W - min_overlap; max_ber_milli in [0, 500]; min_matches >= 1; ring in [0, 2^20]; window_samples in [0, 2^40];
+ * max_media (registered clips) in [0, 4096]; max_media_samples in [0, 2^24], and when max_media > 0 at least 640 and with
+ * (max_media_samples - 480) / 160 >= min_overlap; max_media times that word count at most 2^27.
+ *
+ * Calls (refusals are MWW_EINVAL with a message in mww_last_error(NULL), before any device work, every object unchanged):
+ *   - mww_media_guard_create: slots >= 1 and the rule above; MWW_ECUDA without a device.  _destroy waits for the device.
+ *     mww_media_guard_info fills mww_media_guard_desc: slots, frames (T), device, n_media (registered clips), the rule,
+ *     ring_count (slots appended since the last clear), ring_fill = min(ring_count, ring), and launches: the kernel launches
+ *     of the guard and its frontend handles since create.  It waits for the device.
+ *   - mww_media_check_streams / mww_media_check_detections_at: outputs [n] (capacity for a detector), each may be NULL;
+ *     d_confirmed [n] may be NULL.  Refused: a NULL guard or src; src without an audio history or with capacity < n_samples; src,
+ *     det and the guard not on one device; n < 0 or n > slots; a detector capacity > slots; d_ids or d_ends NULL with n > 0;
+ *     a poisoned src; an untimed detector; model >= the detector's model count (model < 0: every model; model = k: one wake word
+ *     of a models detector); post outside [0, 2^22].  n == 0 does nothing.
+ *   - Ordering and side effects, as for the verifier: asynchronous on cu_stream, no host synchronisation and no allocation after
+ *     create; src and det are read, not changed (the history read is src's own kernel, one launch of mww_launch_count(src));
+ *     check BEFORE mww_reset_device_ids(src, ...), which zeroes the history.  A call launches the same kernels whatever n and
+ *     however many events fired.  Calls on one guard are ordered by the caller on one stream.
+ *   - mww_media_register: fingerprints n_samples 16 kHz int16 samples in device memory through the same frontend path (a fresh
+ *     frontend, W_k = (n_samples - 480) / 160 words) and appends them as registered clip *index.  Refused: a NULL guard or audio,
+ *     a full list, n_samples above max_media_samples or with W_k < min_overlap.  Asynchronous on cu_stream.
+ *     mww_media_clear_registered empties the list.
+ *   - mww_media_clear_ring empties the ring; use it after mww_set_audio_history, which restarts the axis.  It waits for the
+ *     device.
+ *   - mww_media_get_state / mww_media_set_state: the ring and the registered clips as one host blob, for checkpoints.  Get with
+ *     h_state NULL writes the blob's size to *n_bytes; otherwise *n_bytes must be at least that size.  Both wait for the device.
+ *     Layout: int64 ring_count; int32 words (W), ring, n_media, pad; int64 media_words; then uint64 ring_fp[ring][W], int64
+ *     ring_pos[ring], int32 ring_stream[ring], int32 ring_household[ring]; then int64 clip_words[n_media] and the uint64
+ *     words of every clip, in order.  Set refuses a blob of another size, W or ring, more clips than max_media, a clip length
+ *     outside [min_overlap, the longest registrable] or a sum that is not media_words. */
+typedef struct mww_media_guard mww_media_guard_t;
+typedef struct mww_media_rule {
+    int32_t n_samples, max_lag, min_overlap, max_ber_milli;
+    int32_t min_matches, ring, max_media, max_media_samples;
+    int64_t window_samples;
+} mww_media_rule;
+typedef struct mww_media_guard_desc {
+    int32_t slots, frames, device, n_media;
+    mww_media_rule rule;
+    int64_t ring_fill, ring_count, launches;
+} mww_media_guard_desc;
+int mww_media_guard_create(int device, int slots, const mww_media_rule *rule, mww_media_guard_t **out);
+int mww_media_guard_destroy(mww_media_guard_t *g);
+int mww_media_guard_info(const mww_media_guard_t *g, mww_media_guard_desc *out);
+int mww_media_check_streams(mww_media_guard_t *g, mww_t *src, const int32_t *d_ids, const long long *d_ends, const int32_t *d_households, int n,
+                            const int32_t *d_confirmed, int32_t *d_matches, int32_t *d_media, int32_t *d_passed, void *cu_stream);
+int mww_media_check_detections_at(mww_media_guard_t *g, mww_t *src, mww_detector_t *det, int model, long long post, const int32_t *d_confirmed,
+                                  int32_t *d_matches, int32_t *d_media, int32_t *d_passed, void *cu_stream);
+int mww_media_register(mww_media_guard_t *g, const int16_t *d_audio, int n_samples, int *index, void *cu_stream);
+int mww_media_clear_registered(mww_media_guard_t *g);
+int mww_media_clear_ring(mww_media_guard_t *g);
+int mww_media_get_state(mww_media_guard_t *g, void *h_state, long long *n_bytes);
+int mww_media_set_state(mww_media_guard_t *g, const void *h_state, long long n_bytes);
+
 /* ---- endpointing: where the spoken command after a wake word ends, and its clip from the audio history ----------------------
  * After a wake word a voice assistant sends the command that follows to speech-to-text and stops when the speaker stops.  An
  * ENDPOINTER finds that end on the GPU, per stream, from a VAD model's probabilities, and cuts each command's clip from the

@@ -53,6 +53,9 @@ EXPORTS = (
     "mww_group_detector_events", "mww_set_detector_groups", "mww_get_detector_groups", "mww_set_multi_detector_groups",
     "mww_get_multi_detector_groups", "mww_flush_detector_groups", "mww_drain_detector_groups", "mww_get_detector_group_windows",
     "mww_set_detector_group_windows",
+    "mww_media_guard_create", "mww_media_guard_destroy", "mww_media_guard_info", "mww_media_check_streams",
+    "mww_media_check_detections_at", "mww_media_register", "mww_media_clear_registered", "mww_media_clear_ring",
+    "mww_media_get_state", "mww_media_set_state",
 )
 
 
@@ -118,6 +121,19 @@ class MwwVerifierDesc(ctypes.Structure):
     """mww_verifier_desc of include/mww.h (mww_verifier_info)"""
     _fields_ = [("slots", ctypes.c_int32), ("steps", ctypes.c_int32), ("device", ctypes.c_int32), ("pad", ctypes.c_int32),
                 ("rule", MwwVerifyRule), ("launches", ctypes.c_int64)]
+
+
+class MwwMediaRule(ctypes.Structure):
+    """mww_media_rule of include/mww.h: what a media guard hears and when two fingerprints match"""
+    _fields_ = [("n_samples", ctypes.c_int32), ("max_lag", ctypes.c_int32), ("min_overlap", ctypes.c_int32), ("max_ber_milli", ctypes.c_int32),
+                ("min_matches", ctypes.c_int32), ("ring", ctypes.c_int32), ("max_media", ctypes.c_int32), ("max_media_samples", ctypes.c_int32),
+                ("window_samples", ctypes.c_int64)]
+
+
+class MwwMediaGuardDesc(ctypes.Structure):
+    """mww_media_guard_desc of include/mww.h (mww_media_guard_info)"""
+    _fields_ = [("slots", ctypes.c_int32), ("frames", ctypes.c_int32), ("device", ctypes.c_int32), ("n_media", ctypes.c_int32),
+                ("rule", MwwMediaRule), ("ring_fill", ctypes.c_int64), ("ring_count", ctypes.c_int64), ("launches", ctypes.c_int64)]
 
 
 MWW_ENDPOINT_END_OF_SPEECH, MWW_ENDPOINT_NO_SPEECH, MWW_ENDPOINT_MAX_LENGTH = 1, 2, 3
@@ -419,6 +435,25 @@ def lib() -> ctypes.CDLL:
     L.mww_flush_detector_groups.argtypes = [vp, vp]
     L.mww_drain_detector_groups.restype = i32
     L.mww_drain_detector_groups.argtypes = [vp, vp, vp, vp, vp, i32, ctypes.POINTER(ll), vp]
+    L.mww_media_guard_create.restype = i32
+    L.mww_media_guard_create.argtypes = [i32, i32, ctypes.POINTER(MwwMediaRule), ctypes.POINTER(vp)]
+    L.mww_media_guard_destroy.restype = i32
+    L.mww_media_guard_destroy.argtypes = [vp]
+    L.mww_media_guard_info.restype = i32
+    L.mww_media_guard_info.argtypes = [vp, ctypes.POINTER(MwwMediaGuardDesc)]
+    L.mww_media_check_streams.restype = i32
+    L.mww_media_check_streams.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp]
+    L.mww_media_check_detections_at.restype = i32
+    L.mww_media_check_detections_at.argtypes = [vp, vp, vp, i32, ll, vp, vp, vp, vp, vp]
+    L.mww_media_register.restype = i32
+    L.mww_media_register.argtypes = [vp, vp, i32, pi, vp]
+    for name in ("mww_media_clear_registered", "mww_media_clear_ring"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp]
+    L.mww_media_get_state.restype = i32
+    L.mww_media_get_state.argtypes = [vp, vp, ctypes.POINTER(ll)]
+    L.mww_media_set_state.restype = i32
+    L.mww_media_set_state.argtypes = [vp, vp, ll]
     _lib = L
     return L
 

@@ -1,5 +1,5 @@
 // mww_capi.h -- what the C-ABI translation units share: mww_capi.cu (the handle), mww_detector_capi.cu (the streaming
-// detectors) and mww_endpoint_capi.cu (the endpointer).  Host code only.
+// detectors), mww_endpoint_capi.cu (the endpointer) and mww_media_guard_capi.cu (the media guard).  Host code only.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -34,5 +34,9 @@ struct HistoryRing {
     const int16_t *ring; int capacity; long long seen; int n_streams, sm_count; bool poisoned;
 };
 HistoryRing history_ring(const mww_t *h);
+
+// a detector's per-event-slot groups [capacity] (mww_drain_detector_groups' source) as the media guard's kernels read them;
+// nullptr for a detector that is not grouped
+const int32_t *detector_event_groups(const mww_detector_t *d);
 
 }  // namespace mww

@@ -54,6 +54,10 @@ struct mww_detector {
     std::vector<int32_t> groups;
 };
 
+namespace mww {
+const int32_t *detector_event_groups(const mww_detector_t *d) { return d->grouped ? d->g.ev_group : nullptr; }
+}  // namespace mww
+
 namespace {
 
 #define DCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(nullptr, e_, #call); } while (0)

@@ -260,3 +260,48 @@ cudaError_t launch_detector_models_update_grouped(const DetectModelsArgsT<Detect
 cudaError_t launch_detector_groups_flush(const DetectorArgs &a, const GroupArgs &g, cudaStream_t st);
 cudaError_t launch_detector_models_groups_flush(const DetectModelsArgs &a, const GroupArgs &g, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_media_guard.h"
+namespace mww {
+// media guard (mww_media_guard.cu, bodies in mww_media_guard.h; companion library libmww_media_guard.so), one launch each.
+// The slots of a check: a detector's event slots [0, n) when events is set (count, events, positions and ev_group its
+// buffers, ev_group nullptr when ungrouped), else the n listed ids ending at ends (households may be nullptr)
+struct MediaSlotsArgs {
+    int n, n_streams, C, n_samples;
+    long long seen;
+    const int32_t *ids; const long long *ends; const int32_t *households;
+    const long long *count; const mww_event *events; const long long *positions; const int32_t *ev_group;
+    int capacity, model; long long post;
+};
+// [n] each: the slots, each valid slot's rank among them, and the counters the match adds to; state: the guard's ring state
+struct MediaSlotsOut {
+    int32_t *sid, *rid, *hh, *rank, *count, *clip_hit;
+    long long *end, *pos;
+    MediaRingState *state;
+};
+cudaError_t launch_media_slots(const MediaSlotsArgs &a, const MediaSlotsOut &o, cudaStream_t st);
+// fp [n][fp_stride]: words [0, words) of each of the n clips whose feature rows are feat [n][rows][40]
+cudaError_t launch_media_fingerprint(const uint16_t *feat, long long rows, int n, int words, uint64_t *fp, long long fp_stride, cudaStream_t st);
+// the lag search of every valid slot against this check's other valid slots, the ring's entries and the registered clips
+struct MediaMatchArgs {
+    const uint64_t *fp; int words, n;
+    const int32_t *rid, *hh; const long long *pos;
+    const uint64_t *ring_fp; const int32_t *ring_stream, *ring_hh; const long long *ring_pos; int ring;
+    const MediaRingState *state;
+    const uint64_t *clip_fp; const long long *clip_off; const int32_t *clip_len, *clip_task0; int n_clips; long long clip_tasks;
+    int max_lag, min_overlap, max_ber_milli; long long window;
+    int32_t *count, *clip_hit;
+    int tasks_per_cta;
+};
+size_t media_match_smem(int words);
+cudaError_t launch_media_match(const MediaMatchArgs &a, cudaStream_t st);
+// matches, media and passed [n] (each may be nullptr) and the ring append
+struct MediaDecideArgs {
+    int n, words, ring, min_matches;
+    const uint64_t *fp; const int32_t *sid, *rid, *hh, *rank, *count, *clip_hit, *confirmed; const long long *pos;
+    const MediaRingState *state;
+    int32_t *matches, *media, *passed;
+    uint64_t *ring_fp; int32_t *ring_stream, *ring_hh; long long *ring_pos;
+};
+cudaError_t launch_media_decide(const MediaDecideArgs &a, cudaStream_t st);
+}  // namespace mww
