@@ -1141,6 +1141,97 @@ int mww_media_clear_ring(mww_media_guard_t *g);
 int mww_media_get_state(mww_media_guard_t *g, void *h_state, long long *n_bytes);
 int mww_media_set_state(mww_media_guard_t *g, const void *h_state, long long n_bytes);
 
+/* ---- playback guard: suppress the detections a device's own playback said ---------------------------------------------------
+ * A satellite plays what the server sends it -- replies, music -- and its microphone hears that playback.  A reply that says
+ * the wake word, or a word close to it, fires the stream, and for the wake model and the verifier that is a true positive.
+ * The server knows what it sent to each stream, so a PLAYBACK GUARD keeps that playback on the GPU and asks, at each detection:
+ * did the device itself say the wake word in the delay window before it?  A wake model answers that on the clean playback.
+ *
+ * Binding and axis.  A guard is bound at create to a handle h that keeps an audio history, as an endpointer is, and uses h's
+ * history axis: position t is the t-th 16 kHz sample appended since the history was enabled (samples_seen).  The guard reads
+ * h's counters on the host only and never launches work on h.
+ * Playback.  For each stream s, pb_s maps axis positions to int16, 0 everywhere until written.
+ * Rows.  The guard owns `rows` ring rows of C int16 samples (C a multiple of 8 in [8, 2^22]).  A stream that is playing holds
+ * one row with a head w, the end of its latest write; the row holds positions [w - C, w).  Reading position p gives pb_s(p)
+ * when w - C <= p < w, else 0; a stream without a row reads 0 everywhere.
+ * Write (s, a, x[0, n)).  If s has no row it takes the lowest-numbered free row (ids in list order), which counts as holding
+ * zeros with head a - C.  Then, with w' = max(w, a + n): positions [max(a, w' - C), a + n) get x; when a > w the gap
+ * [max(w, w' - C), a) gets zeros; every other held position keeps its value; the head becomes w'.  So a write into the past
+ * (a + n <= w) overwrites only what the ring still holds, and writes ahead of samples_seen are allowed.
+ * Release.  At the start of every write call every row whose head w <= S - C is freed (S = h's samples_seen at the call).  No
+ * check can see it: a heard clip starts at r0 >= S - C, and everything such a row holds lies before w <= S - C.  A write that
+ * needs more rows than are free after the release is refused with MWW_ENOMEM, and nothing is written or freed.  Reset(ids)
+ * frees those streams' rows; a whole reset (NULL) frees every row -- use it after mww_set_audio_history, which restarts the axis.
+ * Slots.  As the verifier's: slot i has a stream id and a clip end e_i.
+ *   - mww_playback_check_streams: d_ids[i] and d_ends[i].
+ *   - mww_playback_check_detections_at: event slot i of a timed detector under mww_verify_detections_at's slot rule: the event's
+ *     stream (-1 for an unused slot or another model's event), its position P, e_i = min(P + post, S); model < 0: every model,
+ *     k: one wake word of a models detector.
+ * Reference clip.  L_ref = n_samples + max_delay - min_delay.  Slot i's reference clip is pb_s over [r0, r1), r1 = e_i -
+ * min_delay, r0 = r1 - L_ref: the union of the playback windows [e - n_samples - d, e - d) of every delay d in [min_delay,
+ * max_delay], d being the samples between a playback position and where the microphone hears it.
+ * Heard.  A slot is heard when its id is in [0, n_streams), the stream holds a row, r0 >= S - C, r0 >= w - C and r0 < w: the row
+ * still holds the whole window, and the window starts before the head, so some of it has been written.
+ * Score and decision.  For a heard slot, score = exactly what a verifier of the guard's container with rule (L_ref, window,
+ * ignore_steps, cutoff) gives on the reference clip (a fresh handle, one mww_predict_clip, mww_positive_scores with (window,
+ * ignore_steps)); flagged = (double)score > cutoff, which NaN never is; passed = -1 when flagged, else d_confirmed[i], or the
+ * slot's stream id when d_confirmed is NULL.  An unheard slot gets score NaN, flagged 0 and passed its confirmed id: the guard
+ * never blocks what it cannot hear.  passed goes straight into mww_endpointer_arm_device, after the media guard's passed.
+ * What it cannot know:
+ *   - The rule never looks at the microphone audio.  A detection is suppressed because the device itself said something the
+ *     model scores above cutoff in the delay window.  So a user who says the wake word over music passes, and one who says it
+ *     over the device saying it is suppressed.
+ *   - Playback that fires the detector only after the room has coloured it is missed; a guard cutoff below the detector's
+ *     widens the net.
+ *   - C must cover the longest write made ahead of time plus L_ref.  Real-time writes need only L_ref plus the poll latency.
+ *
+ * Calls (refusals are MWW_EINVAL with a message in mww_last_error(NULL), before any device work, the guard unchanged; the one
+ * other code is MWW_ENOMEM for a write that runs out of rows):
+ *   - mww_playback_guard_create: refused for a handle without an audio history or frontend-only; a NULL blob; slots < 1; rows
+ *     outside [1, n_streams]; a bad capacity C; n_samples < 480; delays outside 0 <= min_delay <= max_delay <= 2^22; L_ref >
+ *     min(C, 2^22); and the verifier's refusals of window, ignore_steps and cutoff, "every score would be NaN" included.
+ *     MWW_ECUDA without a device.  _destroy waits for the device.  mww_playback_guard_info fills mww_playback_guard_desc: slots,
+ *     steps (the verifier's m), rows, rows_used, capacity (C), l_ref, device, the rule and launches (the guard's kernel launches
+ *     and its verifier handle's).
+ *   - mww_playback_write: n distinct ids in [0, n_streams) with starts in [-2^50, 2^50] (host memory), each writing row i of
+ *     d_audio [n][audio_stride] (n_samples in [0, 2^22], audio_stride >= n_samples).  One host-to-device copy of the call's
+ *     (row, start, old head) list and one launch, whatever n.
+ *   - mww_playback_read: d_out [n][out_stride] row i = pb of stream d_ids[i] over [d_ends[i] - n_samples, d_ends[i]) by the read
+ *     rule (0 for an id outside [0, n_streams)); ids and ends in device memory.
+ *   - mww_playback_reset: frees the rows of the n listed ids (host memory), or of every stream when h_ids is NULL.
+ *   - mww_playback_get_heads: h_rows [n_streams] (-1: no row) and h_heads [n_streams] (0 without a row), either may be NULL;
+ *     the host's copy, so it needs no device synchronisation.  With mww_playback_read and mww_playback_write it moves a stream's
+ *     playback to another guard.
+ *   - mww_playback_check_streams / mww_playback_check_detections_at: outputs [n] (capacity for a detector), each may be NULL;
+ *     d_confirmed may be NULL.  Refused as the verifier's checks are, with the bound handle in place of src: a NULL guard; the
+ *     bound handle without an audio history, or poisoned; n < 0 or n > slots; d_ids or d_ends NULL with n > 0; a detector
+ *     capacity > slots or on another device; model >= the detector's model count; an untimed detector; post outside [0, 2^22].
+ *     A check makes a constant number of launches whatever the number of events: the slots and reference read, the model's
+ *     reset and clip, the positive scores, the decision.  n == 0 does nothing.
+ *   - Nothing allocates after create; every call is asynchronous on cu_stream, and calls on one guard are ordered by the caller. */
+typedef struct mww_playback_guard mww_playback_guard_t;
+typedef struct mww_playback_rule { int32_t n_samples, window, ignore_steps, pad; int64_t min_delay, max_delay; double cutoff; } mww_playback_rule;
+typedef struct mww_playback_guard_desc {
+    int32_t slots, steps, rows, rows_used;
+    int32_t capacity, l_ref, device, pad;
+    mww_playback_rule rule;
+    int64_t launches;
+} mww_playback_guard_desc;
+int mww_playback_guard_create(const mww_t *h, const void *model_blob, size_t n_bytes, int slots, int rows, int capacity,
+                              const mww_playback_rule *rule, mww_playback_guard_t **out);
+int mww_playback_guard_destroy(mww_playback_guard_t *g);
+int mww_playback_guard_info(const mww_playback_guard_t *g, mww_playback_guard_desc *out);
+int mww_playback_write(mww_playback_guard_t *g, const int32_t *h_ids, const long long *h_starts, int n,
+                       const int16_t *d_audio, int n_samples, long long audio_stride, void *cu_stream);
+int mww_playback_read(mww_playback_guard_t *g, const int32_t *d_ids, const long long *d_ends, int n, int n_samples,
+                      int16_t *d_out, long long out_stride, void *cu_stream);
+int mww_playback_reset(mww_playback_guard_t *g, const int32_t *h_ids, int n, void *cu_stream);
+int mww_playback_get_heads(const mww_playback_guard_t *g, int32_t *h_rows, int64_t *h_heads);
+int mww_playback_check_streams(mww_playback_guard_t *g, const int32_t *d_ids, const long long *d_ends, int n, const int32_t *d_confirmed,
+                               float *d_scores, int32_t *d_flagged, int32_t *d_passed, void *cu_stream);
+int mww_playback_check_detections_at(mww_playback_guard_t *g, mww_detector_t *det, int model, long long post, const int32_t *d_confirmed,
+                                     float *d_scores, int32_t *d_flagged, int32_t *d_passed, void *cu_stream);
+
 /* ---- endpointing: where the spoken command after a wake word ends, and its clip from the audio history ----------------------
  * After a wake word a voice assistant sends the command that follows to speech-to-text and stops when the speaker stops.  An
  * ENDPOINTER finds that end on the GPU, per stream, from a VAD model's probabilities, and cuts each command's clip from the

@@ -56,6 +56,8 @@ EXPORTS = (
     "mww_media_guard_create", "mww_media_guard_destroy", "mww_media_guard_info", "mww_media_check_streams",
     "mww_media_check_detections_at", "mww_media_register", "mww_media_clear_registered", "mww_media_clear_ring",
     "mww_media_get_state", "mww_media_set_state",
+    "mww_playback_guard_create", "mww_playback_guard_destroy", "mww_playback_guard_info", "mww_playback_write", "mww_playback_read",
+    "mww_playback_reset", "mww_playback_get_heads", "mww_playback_check_streams", "mww_playback_check_detections_at",
 )
 
 
@@ -134,6 +136,19 @@ class MwwMediaGuardDesc(ctypes.Structure):
     """mww_media_guard_desc of include/mww.h (mww_media_guard_info)"""
     _fields_ = [("slots", ctypes.c_int32), ("frames", ctypes.c_int32), ("device", ctypes.c_int32), ("n_media", ctypes.c_int32),
                 ("rule", MwwMediaRule), ("ring_fill", ctypes.c_int64), ("ring_count", ctypes.c_int64), ("launches", ctypes.c_int64)]
+
+
+class MwwPlaybackRule(ctypes.Structure):
+    """mww_playback_rule of include/mww.h: the reference clip a playback guard scores, and its cutoff"""
+    _fields_ = [("n_samples", ctypes.c_int32), ("window", ctypes.c_int32), ("ignore_steps", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("min_delay", ctypes.c_int64), ("max_delay", ctypes.c_int64), ("cutoff", ctypes.c_double)]
+
+
+class MwwPlaybackGuardDesc(ctypes.Structure):
+    """mww_playback_guard_desc of include/mww.h (mww_playback_guard_info)"""
+    _fields_ = [("slots", ctypes.c_int32), ("steps", ctypes.c_int32), ("rows", ctypes.c_int32), ("rows_used", ctypes.c_int32),
+                ("capacity", ctypes.c_int32), ("l_ref", ctypes.c_int32), ("device", ctypes.c_int32), ("pad", ctypes.c_int32),
+                ("rule", MwwPlaybackRule), ("launches", ctypes.c_int64)]
 
 
 MWW_ENDPOINT_END_OF_SPEECH, MWW_ENDPOINT_NO_SPEECH, MWW_ENDPOINT_MAX_LENGTH = 1, 2, 3
@@ -454,6 +469,24 @@ def lib() -> ctypes.CDLL:
     L.mww_media_get_state.argtypes = [vp, vp, ctypes.POINTER(ll)]
     L.mww_media_set_state.restype = i32
     L.mww_media_set_state.argtypes = [vp, vp, ll]
+    L.mww_playback_guard_create.restype = i32
+    L.mww_playback_guard_create.argtypes = [vp, vp, sz, i32, i32, i32, ctypes.POINTER(MwwPlaybackRule), ctypes.POINTER(vp)]
+    L.mww_playback_guard_destroy.restype = i32
+    L.mww_playback_guard_destroy.argtypes = [vp]
+    L.mww_playback_guard_info.restype = i32
+    L.mww_playback_guard_info.argtypes = [vp, ctypes.POINTER(MwwPlaybackGuardDesc)]
+    L.mww_playback_write.restype = i32
+    L.mww_playback_write.argtypes = [vp, vp, vp, i32, vp, i32, ll, vp]
+    L.mww_playback_read.restype = i32
+    L.mww_playback_read.argtypes = [vp, vp, vp, i32, i32, vp, ll, vp]
+    L.mww_playback_reset.restype = i32
+    L.mww_playback_reset.argtypes = [vp, vp, i32, vp]
+    L.mww_playback_get_heads.restype = i32
+    L.mww_playback_get_heads.argtypes = [vp, vp, vp]
+    L.mww_playback_check_streams.restype = i32
+    L.mww_playback_check_streams.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp]
+    L.mww_playback_check_detections_at.restype = i32
+    L.mww_playback_check_detections_at.argtypes = [vp, vp, i32, ll, vp, vp, vp, vp, vp]
     _lib = L
     return L
 

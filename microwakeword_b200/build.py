@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmww_b200.so")
-SOURCES = ["mww_capi.cu", "mww_detector_capi.cu", "mww_verify_capi.cu", "mww_endpoint_capi.cu", "mww_media_guard_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_streams.cu", "mww_records.cu", "mww_detect.cu", "mww_tables.cc", "mww_container.cc"]
+SOURCES = ["mww_capi.cu", "mww_detector_capi.cu", "mww_verify_capi.cu", "mww_endpoint_capi.cu", "mww_media_guard_capi.cu", "mww_playback_capi.cu", "mww_frontend.cu", "mww_nn.cu", "mww_nn_int8.cu", "mww_nn_live.cu", "mww_nn_i8_live.cu", "mww_nn_generic.cu", "mww_nn_tc.cu", "mww_streams.cu", "mww_records.cu", "mww_detect.cu", "mww_tables.cc", "mww_container.cc"]
 # the input-rate resampler kernel (mww_set_input_rate) is a companion library that libmww_b200.so links (rpath $ORIGIN): the
 # main library's own kernel set stays the one the SASS fixtures under tests/golden/ record
 RS_OUT = os.path.join(HERE, "libmww_resample.so")
@@ -64,6 +64,9 @@ GRP_SOURCES = ["mww_detector_groups.cu"]
 # and the media guard's four kernels (mww_media_guard_create and the checks), likewise
 MG_OUT = os.path.join(HERE, "libmww_media_guard.so")
 MG_SOURCES = ["mww_media_guard.cu"]
+# and the playback guard's three kernels (mww_playback_guard_create and the writes, reads and checks), likewise
+PB_OUT = os.path.join(HERE, "libmww_playback.so")
+PB_SOURCES = ["mww_playback.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -86,7 +89,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, EVP_OUT, GRP_OUT, MG_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, EVP_OUT, GRP_OUT, MG_OUT, PB_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -108,11 +111,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
                                     (MD_OUT, MD_SOURCES, []), (DC_OUT, DC_SOURCES, []), (G711_OUT, G711_SOURCES, []),
                                     (HIST_OUT, HIST_SOURCES, []), (DR_OUT, DR_SOURCES, []), (VER_OUT, VER_SOURCES, []),
                                     (EP_OUT, EP_SOURCES, []), (SR_OUT, SR_SOURCES, []), (EVP_OUT, EVP_SOURCES, []),
-                                    (GRP_OUT, GRP_SOURCES, []), (MG_OUT, MG_SOURCES, []),
+                                    (GRP_OUT, GRP_SOURCES, []), (MG_OUT, MG_SOURCES, []), (PB_OUT, PB_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
                                                     "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711", "-lmww_history",
                                                     "-lmww_detector_records", "-lmww_verify", "-lmww_endpoint", "-lmww_serving_records",
-                                                    "-lmww_event_positions", "-lmww_detector_groups", "-lmww_media_guard",
+                                                    "-lmww_event_positions", "-lmww_detector_groups", "-lmww_media_guard", "-lmww_playback",
                                                     "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra

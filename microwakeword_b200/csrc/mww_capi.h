@@ -1,5 +1,6 @@
 // mww_capi.h -- what the C-ABI translation units share: mww_capi.cu (the handle), mww_detector_capi.cu (the streaming
-// detectors), mww_endpoint_capi.cu (the endpointer) and mww_media_guard_capi.cu (the media guard).  Host code only.
+// detectors), mww_endpoint_capi.cu (the endpointer), mww_media_guard_capi.cu (the media guard), mww_verify_capi.cu (the
+// verifier) and mww_playback_capi.cu (the playback guard).  Host code only.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -38,5 +39,12 @@ HistoryRing history_ring(const mww_t *h);
 // a detector's per-event-slot groups [capacity] (mww_drain_detector_groups' source) as the media guard's kernels read them;
 // nullptr for a detector that is not grouped
 const int32_t *detector_event_groups(const mww_detector_t *d);
+
+// A verifier's scoring pass over the clips already in its clip buffer [slots][n_samples] (mww_verify_capi.cu):
+// mww_reset(NULL) of its model handle, one mww_predict_clip over every slot and mww_positive_scores of the first n tracks into
+// verifier_scores(v).  The verifier calls it after its history read; the playback guard after its reference read.
+int16_t *verifier_clips(mww_verifier_t *v);
+const float *verifier_scores(const mww_verifier_t *v);
+int verifier_score_clips(mww_verifier_t *v, int n, cudaStream_t st, const std::string &call);
 
 }  // namespace mww

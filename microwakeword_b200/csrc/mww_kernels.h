@@ -305,3 +305,30 @@ struct MediaDecideArgs {
 };
 cudaError_t launch_media_decide(const MediaDecideArgs &a, cudaStream_t st);
 }  // namespace mww
+
+#include "mww_playback.h"
+namespace mww {
+// playback guard (mww_playback.cu, bodies in mww_playback.h; companion library libmww_playback.so), one launch each.
+// the n_jobs jobs (device memory) of a write call: job j with a row writes row j of audio [.][audio_stride], n_samples each, into
+// ring [rows][C] and sets row_of[stream] and head[row]; a job with row -1 sets row_of[stream] = -1
+cudaError_t launch_playback_write(const PlaybackJob *jobs, int n_jobs, const int16_t *audio, long long audio_stride, int n_samples,
+                                  int16_t *ring, int C, int32_t *row_of, long long *head, cudaStream_t st);
+// The slots of a check or a read: a detector's event slots [0, n) when events is set (count, events and positions its buffers),
+// else the n listed ids ending at ends.  out [n][out_stride]: row i = pb over [e_i - min_delay - L, e_i - min_delay) of slot i's
+// stream; with sid set (a check) also sid and heard [n].  vec is set by the launcher.
+struct PlaybackSlotsArgs {
+    int n, n_streams, C, L;
+    long long seen, min_delay;
+    const int32_t *ids; const long long *ends;
+    const long long *count; const mww_event *events; const long long *positions;
+    int capacity, model; long long post;
+    const int16_t *ring; const int32_t *row_of; const long long *head;
+    int16_t *out; long long out_stride;
+    int32_t *sid, *heard;
+    int vec;
+};
+cudaError_t launch_playback_slots(const PlaybackSlotsArgs &a, cudaStream_t st);
+// out_scores, out_flagged and out_passed [n] (each may be nullptr): playback_decide of every slot from the verifier's scores
+cudaError_t launch_playback_decide(int n, const int32_t *sid, const int32_t *heard, const float *scores, double cutoff, const int32_t *confirmed,
+                                   float *out_scores, int32_t *out_flagged, int32_t *out_passed, cudaStream_t st);
+}  // namespace mww

@@ -89,19 +89,14 @@ int check_source(const mww_verifier_t *v, mww_t *src, const std::string &call, i
 }
 
 // The pass over n ids in device memory: src's history of each (the last n_samples, or with d_ends the n_samples before
-// d_ends[i]), a fresh verifier handle's clip probabilities, their positive scores, and the confirm kernel.  A constant number
-// of launches for n >= 1.
+// d_ends[i]), their scores (verifier_score_clips), and the confirm kernel.  A constant number of launches for n >= 1.
 int run(mww_verifier_t *v, mww_t *src, int src_streams, const int32_t *d_ids, const long long *d_ends, int n, float *d_scores,
         int32_t *d_confirmed, cudaStream_t st, const std::string &call) {
     const int N = v->rule.n_samples;
     const int rc = d_ends ? mww_read_audio_history_at(src, d_ids, d_ends, n, N, v->d_audio, N, st)
                           : mww_read_audio_history_device_ids(src, d_ids, n, N, v->d_audio, N, st);
     if (rc) return pass_on(rc, src, call + ": history read");
-    if (int rc = mww_reset(v->h, nullptr, 0, st)) return pass_on(rc, v->h, call + ": verifier reset");
-    int got = 0;
-    if (int rc = mww_predict_clip(v->h, v->d_audio, N, N, v->d_probs, v->steps, &got, st)) return pass_on(rc, v->h, call + ": verifier clip");
-    if (int rc = mww_positive_scores(v->d_probs, v->d_offsets, v->d_lengths, n, v->rule.window, v->rule.ignore_steps, v->d_scores, st))
-        return fail(nullptr, rc, call + ": mww_positive_scores failed");
+    if (int rc = verifier_score_clips(v, n, st, call)) return rc;
     VCU(launch_verify_confirm(d_ids, n, src_streams, v->d_scores, v->rule.cutoff, d_scores, d_confirmed, st));
     return MWW_OK;
 }
@@ -128,6 +123,23 @@ int check_detections(mww_verifier_t *v, mww_t *src, mww_detector_t *det, int mod
 }
 
 }  // namespace
+
+namespace mww {
+
+int16_t *verifier_clips(mww_verifier_t *v) { return v->d_audio; }
+const float *verifier_scores(const mww_verifier_t *v) { return v->d_scores; }
+
+int verifier_score_clips(mww_verifier_t *v, int n, cudaStream_t st, const std::string &call) {
+    const int N = v->rule.n_samples;
+    if (int rc = mww_reset(v->h, nullptr, 0, st)) return pass_on(rc, v->h, call + ": verifier reset");
+    int got = 0;
+    if (int rc = mww_predict_clip(v->h, v->d_audio, N, N, v->d_probs, v->steps, &got, st)) return pass_on(rc, v->h, call + ": verifier clip");
+    if (int rc = mww_positive_scores(v->d_probs, v->d_offsets, v->d_lengths, n, v->rule.window, v->rule.ignore_steps, v->d_scores, st))
+        return fail(nullptr, rc, call + ": mww_positive_scores failed");
+    return MWW_OK;
+}
+
+}  // namespace mww
 
 extern "C" {
 
