@@ -1047,6 +1047,49 @@ int mww_drain_detector_groups(mww_detector_t *d, mww_event *h_events, int64_t *h
 int mww_get_detector_group_windows(mww_detector_t *d, mww_group_window *h_windows);
 int mww_set_detector_group_windows(mww_detector_t *d, const mww_group_window *h_windows);
 
+/* ---- group arbitration: the satellite that heard the wake word best answers ----------------------------------------------------
+ * Grouped detection picks a window's winner by score.  Every satellite that hears the word clearly saturates an int8 model's
+ * score (multiples of 1/256), and all streams of a handle step in lockstep, so the score and position tie and the lowest stream
+ * id answers.  An ARBITRATED detector picks the candidate that heard the word loudest over its own background instead: the
+ * device next to the speaker, not the one across the room.  It is opt-in; a detector that is not arbitrated is unchanged.
+ *
+ * Rule.  A grouped, timed detector is bound to a handle src with (speech_samples Ls, noise_samples Ln), both in [480, 2^20],
+ * Ls + Ln at most src's history capacity.  For a candidate (grouped detection) of stream s at position P:
+ *   - Spans: speech [P - Ls, P), noise [P - Ls - Ln, P - Ls), read from src's history ring with the read-at rule: a position
+ *     outside [S - C, S) reads as zero, S src's samples_seen at the update (the update runs right after the engine call).
+ *   - Energy of a span of L int16 samples x: q = (double)sum x^2 (exact: below 2^53 for L <= 2^22), r = (double)sum x,
+ *     e = (q - r r / L) / L, every operation a separately rounded IEEE double operation (no fused multiply-add): the
+ *     mean-removed power, so that a microphone's DC offset does not make a satellite look loud.
+ *   - level = (float)((e_speech + 1) / (e_noise + 1)), rounded to nearest.  The + 1 is a floor of one LSB^2, so an all-zero
+ *     (noise-gated) span divides by 1.  10 log10(level) is the level in dB.
+ *   - Order: the best candidate of a group and window has the highest level, then the highest score, then the earliest
+ *     position, then the lowest row (plain detector) or lowest global stream (models detector).  Steps 1 to 3 of grouped
+ *     detection are unchanged; when an update's best joins an open window, "better" is this order and an exact tie keeps the
+ *     earlier candidate.
+ *   - Per-row state is bit for bit the ungrouped timed detector's, and rows of group -1 store their events as before.  Each
+ *     emitted winner carries its level; an event of a row of group -1 carries NaN.
+ * What the level cannot know: how far each device's microphone gain, enclosure and placement differ; a satellite with a hotter
+ * microphone looks closer.  The level compares each device with its own background, which cancels a fixed gain only where
+ * both spans see it alike.
+ *
+ * Calls (messages in mww_last_error(NULL); refusals are MWW_EINVAL before any device work, detector unchanged):
+ *   - mww_arbitrate_detector_groups: makes a grouped detector arbitrated, for good, every window level 0.  Refused when the
+ *     detector is not grouped, is already arbitrated or may hold events; when src is NULL, poisoned or on another device;
+ *     when a row's stream (plain: its stream_ids entry or row; models: every global stream) is outside src; when Ls or Ln is
+ *     out of range or Ls + Ln exceeds src's history capacity.  src must outlive the detector.
+ *   - The timed updates and mww_flush_detector_groups then run the arbitrated kernels: the same two launches per update (one
+ *     per flush) whatever the number of events.  An update is refused while src's history holds fewer than Ls + Ln samples
+ *     (mww_set_audio_history), lacks a stream a row reads, or is poisoned.
+ *   - mww_drain_detector_arbitrated: mww_drain_detector_groups plus each event's level.
+ *   - mww_get_detector_group_levels / mww_set_detector_group_levels: every group slot's window level (slots as the windows'),
+ *     part of the checkpoint with the windows and groups.  Both wait for the device; set refuses a level that is NaN,
+ *     infinite or negative.  Detector records carry no levels, as they carry no windows. */
+int mww_arbitrate_detector_groups(mww_detector_t *d, mww_t *src, int speech_samples, int noise_samples);
+int mww_drain_detector_arbitrated(mww_detector_t *d, mww_event *h_events, int64_t *h_positions, int32_t *h_groups, int32_t *h_candidates,
+                                  float *h_levels, int max_events, long long *n_events, void *cu_stream);
+int mww_get_detector_group_levels(mww_detector_t *d, float *h_levels);
+int mww_set_detector_group_levels(mww_detector_t *d, const float *h_levels);
+
 /* ---- media guard: suppress the detections that many households, or a registered media clip, heard alike ---------------------
  * A TV advert, a podcast or a broadcast that says the wake word makes thousands of households fire within a second, and every
  * one of those detections is a true positive for the wake model and the verifier.  A broadcast is the same audio heard in many

@@ -58,6 +58,7 @@ EXPORTS = (
     "mww_media_get_state", "mww_media_set_state",
     "mww_playback_guard_create", "mww_playback_guard_destroy", "mww_playback_guard_info", "mww_playback_write", "mww_playback_read",
     "mww_playback_reset", "mww_playback_get_heads", "mww_playback_check_streams", "mww_playback_check_detections_at",
+    "mww_arbitrate_detector_groups", "mww_drain_detector_arbitrated", "mww_get_detector_group_levels", "mww_set_detector_group_levels",
 )
 
 
@@ -487,6 +488,13 @@ def lib() -> ctypes.CDLL:
     L.mww_playback_check_streams.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp]
     L.mww_playback_check_detections_at.restype = i32
     L.mww_playback_check_detections_at.argtypes = [vp, vp, i32, ll, vp, vp, vp, vp, vp]
+    L.mww_arbitrate_detector_groups.restype = i32
+    L.mww_arbitrate_detector_groups.argtypes = [vp, vp, i32, i32]
+    L.mww_drain_detector_arbitrated.restype = i32
+    L.mww_drain_detector_arbitrated.argtypes = [vp, vp, vp, vp, vp, vp, i32, ctypes.POINTER(ll), vp]
+    for name in ("mww_get_detector_group_levels", "mww_set_detector_group_levels"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp]
     _lib = L
     return L
 

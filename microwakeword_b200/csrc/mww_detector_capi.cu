@@ -52,6 +52,13 @@ struct mww_detector {
     int n_groups = 0;
     GroupArgs g;
     std::vector<int32_t> groups;
+    // the plain detector's row -> stream map as given at create (empty: stream = row)
+    std::vector<int32_t> stream_ids;
+    // group arbitration (mww_arbitrate_detector_groups): the source handle whose history every update measures, and the kernels'
+    // arguments (ring, seen and capacity are read from src at each update); the largest stream id a row reads
+    mww_t *arb_src = nullptr;
+    ArbitrationArgs r;
+    int arb_max_stream = -1;
 };
 
 namespace mww {
@@ -72,6 +79,7 @@ void detector_free(mww_detector_t *d) {
     cudaFree(d->count); cudaFree(d->events); cudaFree(d->fired); cudaFree(d->d_stream_ids); cudaFree(d->d_rows);
     cudaFree(d->d_models); cudaFree(d->d_models_rows); cudaFree(d->positions);
     cudaFree(const_cast<int32_t *>(d->g.groups)); cudaFree(d->g.pending); cudaFree(d->g.windows); cudaFree(d->g.ev_group); cudaFree(d->g.ev_candidates);
+    cudaFree(d->r.levels); cudaFree(d->r.ev_level);
     delete d;
 }
 
@@ -339,7 +347,7 @@ int check_rows(const mww_detector_t *d, const std::string &call, const int32_t *
 // The drains: the events (and, h_positions != nullptr, their positions; h_groups != nullptr, their groups and candidates) to the
 // host; the counter cleared, d_fired and a timed detector's positions refilled with -1
 int drain(mww_detector_t *d, mww_event *h_events, long long *h_positions, int max_events, long long *n_events, cudaStream_t st,
-          int32_t *h_groups = nullptr, int32_t *h_candidates = nullptr) {
+          int32_t *h_groups = nullptr, int32_t *h_candidates = nullptr, float *h_levels = nullptr) {
     DENTER(d);
     unsigned long long count = 0;
     DCU(cudaMemcpyAsync(&count, d->count, sizeof(count), cudaMemcpyDeviceToHost, st));
@@ -352,6 +360,7 @@ int drain(mww_detector_t *d, mww_event *h_events, long long *h_positions, int ma
         DCU(cudaMemcpyAsync(h_groups, d->g.ev_group, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         DCU(cudaMemcpyAsync(h_candidates, d->g.ev_candidates, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     }
+    if (n && h_levels) DCU(cudaMemcpyAsync(h_levels, d->r.ev_level, n * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (stored) {
         DCU(cudaMemsetAsync(d->count, 0, sizeof(count), st));
         DCU(cudaMemsetAsync(d->fired, 0xFF, stored * sizeof(int32_t), st));
@@ -407,6 +416,26 @@ int set_groups(mww_detector_t *d, const std::string &call, const int32_t *h_ids,
     // from pageable memory: the call returns once the span is staged
     DCU(cudaMemcpyAsync(const_cast<int32_t *>(d->g.groups) + lo, d->groups.data() + lo, (size_t)(hi - lo + 1) * sizeof(int32_t), cudaMemcpyHostToDevice,
                         static_cast<cudaStream_t>(cu_stream)));
+    return MWW_OK;
+}
+
+// ---- group arbitration
+int arbitrated_arg(const mww_detector_t *d, const std::string &call) {
+    if (int rc = grouped_arg(d, call)) return rc;
+    if (!d->arb_src) return refuse(call + ": the detector is not arbitrated (mww_arbitrate_detector_groups)");
+    return MWW_OK;
+}
+
+// an arbitrated update's source history, read now and checked: src healthy, still holding Ls + Ln samples and every stream a
+// row reads
+int arbitration_clock(mww_detector_t *d, const std::string &call) {
+    const HistoryRing h = history_ring(d->arb_src);
+    if (h.poisoned) return refuse(call + ": the arbitration source handle failed a staged call and cannot be read");
+    if (h.capacity < d->r.speech + d->r.noise)
+        return refuse(call + ": the arbitration source keeps " + std::to_string(h.capacity) + " samples of audio history; the detector reads " +
+                      std::to_string(d->r.speech + d->r.noise) + " (speech_samples + noise_samples)");
+    if (d->arb_max_stream >= h.n_streams) return refuse(call + ": a row reads a stream the arbitration source no longer has");
+    d->r.ring = h.ring; d->r.capacity = h.capacity; d->r.seen = h.seen;
     return MWW_OK;
 }
 
@@ -519,6 +548,7 @@ int mww_detector_create(int device, int n_rows, int window, double cutoff, int c
     s.role = MWW_DETECT_WAKE;
     s.rule.window = window; s.rule.cutoff = cutoff; s.rule.cooldown_slices = cooldown_slices;
     s.n_rows = n_rows;
+    if (h_stream_ids) d->stream_ids.assign(h_stream_ids, h_stream_ids + n_rows);
     if (int rc = detector_alloc(d, h_stream_ids)) { detector_free(d); return rc; }
     *out = d;
     return MWW_OK;
@@ -696,7 +726,10 @@ int mww_update_detector_at(mww_detector_t *d, const float *d_probs, int n_steps,
     if (n_steps == 0) return MWW_OK;
     DENTER(d);
     const double *cut = d->per_row ? d->sets[0].d_cutoffs : nullptr;
-    if (d->grouped) DCU(launch_detector_update_grouped(d->a, cut, d_probs, n_steps, pitch, d->g, last_end, step_samples, static_cast<cudaStream_t>(cu_stream)));
+    if (d->arb_src) {
+        if (int rc = arbitration_clock(d, call)) return rc;
+        DCU(launch_detector_update_arbitrated(d->a, cut, d_probs, n_steps, pitch, d->g, d->r, last_end, step_samples, static_cast<cudaStream_t>(cu_stream)));
+    } else if (d->grouped) DCU(launch_detector_update_grouped(d->a, cut, d_probs, n_steps, pitch, d->g, last_end, step_samples, static_cast<cudaStream_t>(cu_stream)));
     else DCU(launch_detector_update_at(d->a, cut, d_probs, n_steps, pitch, d->positions, last_end, step_samples, static_cast<cudaStream_t>(cu_stream)));
     d->updated = true;
     return MWW_OK;
@@ -718,11 +751,16 @@ int mww_update_multi_detector_at(mww_detector_t *d, const float *const *d_probs,
                       "(R = n_k s_k - p_k + g_k with 0 <= p_k, g_k < s_k, the same R >= 0 for every model)");
     // a grouped detector closes its windows at every call that moved the clock, even one in which no model ran a step
     if (!any && !(d->grouped && R > 0)) return MWW_OK;
+    if (d->arb_src)
+        if (int rc = arbitration_clock(d, call)) return rc;
     DENTER(d);
     for (int k = 0; k < m.n_models; ++k) m.call[k] = c[k];
     const long long row0 = event_row0_end(row_end, d->hop, R);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    if (d->grouped) {
+    if (d->arb_src) {
+        if (d->per_row) DCU(launch_detector_models_update_arbitrated(detect_args_rows(m, d->d_models_rows), m, d->g, d->r, row0, row_end, d->hop, st));
+        else DCU(launch_detector_models_update_arbitrated(m, d->g, d->r, row0, row_end, d->hop, st));
+    } else if (d->grouped) {
         if (d->per_row) DCU(launch_detector_models_update_grouped(detect_args_rows(m, d->d_models_rows), m, d->g, row0, row_end, d->hop, st));
         else DCU(launch_detector_models_update_grouped(m, d->g, row0, row_end, d->hop, st));
     } else if (d->per_row) {
@@ -819,7 +857,9 @@ int mww_flush_detector_groups(mww_detector_t *d, void *cu_stream) {
     if (int rc = grouped_arg(d, "mww_flush_detector_groups")) return rc;
     DENTER(d);
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
-    if (d->multi) DCU(launch_detector_models_groups_flush(d->m, d->g, st));
+    if (d->arb_src && d->multi) DCU(launch_detector_models_arbitrated_flush(d->m, d->g, d->r, st));
+    else if (d->arb_src) DCU(launch_detector_arbitrated_flush(d->a, d->g, d->r, st));
+    else if (d->multi) DCU(launch_detector_models_groups_flush(d->m, d->g, st));
     else DCU(launch_detector_groups_flush(d->a, d->g, st));
     d->updated = true;
     return MWW_OK;
@@ -856,6 +896,82 @@ int mww_set_detector_group_windows(mww_detector_t *d, const mww_group_window *h_
     DENTER(d);
     DCU(cudaDeviceSynchronize());
     DCU(cudaMemcpy(d->g.windows, h_windows, (size_t)group_slots(d) * sizeof(mww_group_window), cudaMemcpyHostToDevice));
+    return MWW_OK;
+}
+
+// ---- group arbitration (both kinds)
+int mww_arbitrate_detector_groups(mww_detector_t *d, mww_t *src, int speech_samples, int noise_samples) {
+    const std::string call = "mww_arbitrate_detector_groups";
+    if (int rc = grouped_arg(d, call)) return rc;
+    if (d->arb_src) return refuse(call + ": the detector is already arbitrated");
+    if (d->updated) return refuse(call + ": the detector may hold events: arbitrate it after grouping or a drain, before any update");
+    if (!src) return refuse(call + ": src is NULL");
+    mww_info info;
+    if (mww_get_info(src, &info) != MWW_OK) return refuse(call + ": cannot read the source handle");
+    if (info.device != d->device) return refuse(call + ": the source handle is on another device than the detector");
+    const HistoryRing h = history_ring(src);
+    if (h.poisoned) return refuse(call + ": the source handle failed a staged call and cannot be read");
+    const std::string range = "[" + std::to_string(kArbitrationMinSamples) + ", 2^20]";
+    if (speech_samples < kArbitrationMinSamples || speech_samples > kArbitrationMaxSamples) return refuse(call + ": speech_samples must be in " + range);
+    if (noise_samples < kArbitrationMinSamples || noise_samples > kArbitrationMaxSamples) return refuse(call + ": noise_samples must be in " + range);
+    if ((long long)speech_samples + noise_samples > h.capacity)
+        return refuse(call + ": speech_samples + noise_samples (" + std::to_string((long long)speech_samples + noise_samples) +
+                      ") exceed the source's audio history (" + std::to_string(h.capacity) + " samples)");
+    int lo = 0, hi = 0;
+    if (d->multi) {
+        hi = d->m.n_streams - 1;
+    } else if (!d->stream_ids.empty()) {
+        lo = *std::min_element(d->stream_ids.begin(), d->stream_ids.end());
+        hi = *std::max_element(d->stream_ids.begin(), d->stream_ids.end());
+    } else {
+        hi = d->sets[0].n_rows - 1;
+    }
+    if (lo < 0 || hi >= info.n_streams)
+        return refuse(call + ": the rows read streams in [" + std::to_string(lo) + ", " + std::to_string(hi) + "]; the source has " +
+                      std::to_string(info.n_streams));
+    DENTER(d);
+    ArbitrationArgs r;
+    r.speech = speech_samples; r.noise = noise_samples;
+    const size_t S = (size_t)group_slots(d), C = (size_t)d->capacity;
+    auto undo = [&](cudaError_t e, const char *what) { cudaFree(r.levels); cudaFree(r.ev_level); return cuda_fail(nullptr, e, what); };
+    if (cudaError_t e = cudaMalloc(&r.levels, S * sizeof(float))) return undo(e, "cudaMalloc");
+    if (cudaError_t e = cudaMalloc(&r.ev_level, C * sizeof(float))) return undo(e, "cudaMalloc");
+    if (cudaError_t e = cudaMemset(r.levels, 0, S * sizeof(float))) return undo(e, "cudaMemset");
+    d->r = r;
+    d->arb_src = src;
+    d->arb_max_stream = hi;
+    return MWW_OK;
+}
+
+int mww_drain_detector_arbitrated(mww_detector_t *d, mww_event *h_events, int64_t *h_positions, int32_t *h_groups, int32_t *h_candidates,
+                                  float *h_levels, int max_events, long long *n_events, void *cu_stream) {
+    if (!d || !n_events || max_events < 0 || (max_events > 0 && (!h_events || !h_positions || !h_groups || !h_candidates || !h_levels)))
+        return refuse("mww_drain_detector_arbitrated: needs a detector, n_events and room for max_events >= 0 events, positions, groups, "
+                      "candidates and levels");
+    if (int rc = arbitrated_arg(d, "mww_drain_detector_arbitrated")) return rc;
+    return drain(d, h_events, reinterpret_cast<long long *>(h_positions), max_events, n_events, static_cast<cudaStream_t>(cu_stream), h_groups,
+                 h_candidates, h_levels);
+}
+
+int mww_get_detector_group_levels(mww_detector_t *d, float *h_levels) {
+    if (int rc = arbitrated_arg(d, "mww_get_detector_group_levels")) return rc;
+    if (!h_levels) return refuse("mww_get_detector_group_levels: h_levels is NULL");
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    DCU(cudaMemcpy(h_levels, d->r.levels, (size_t)group_slots(d) * sizeof(float), cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+
+int mww_set_detector_group_levels(mww_detector_t *d, const float *h_levels) {
+    const std::string call = "mww_set_detector_group_levels";
+    if (int rc = arbitrated_arg(d, call)) return rc;
+    if (!h_levels) return refuse(call + ": h_levels is NULL");
+    for (int s = 0; s < group_slots(d); ++s)
+        if (!(h_levels[s] >= 0.f && h_levels[s] <= 3.4028234663852886e38f))
+            return refuse(call + ": slot " + std::to_string(s) + ": a level must be finite and not negative");
+    DENTER(d);
+    DCU(cudaDeviceSynchronize());
+    DCU(cudaMemcpy(d->r.levels, h_levels, (size_t)group_slots(d) * sizeof(float), cudaMemcpyHostToDevice));
     return MWW_OK;
 }
 

@@ -120,6 +120,7 @@ struct GroupEvent {
     long long sample = 0, step = 0;
     int32_t stream = 0, candidates = 0;
     float score = 0.f;
+    float level = 0.f;                       // an arbitrated detector's (mww_group_arbitration.h); not read otherwise
 };
 
 MWW_HD GroupEvent group_window_event(const mww_group_window &w) {
@@ -134,21 +135,42 @@ struct GroupClosed {
     GroupEvent e1, e2;
 };
 
+// whether an update's best replaces the window's: always into a closed window; into an open one when it is better, a tie keeping
+// the earlier candidate -- a higher score, or (kLevel, group arbitration) a higher level, then a higher score
+template <bool kLevel>
+MWW_HD bool group_takes(const mww_group_window &w, const GroupEvent &best, float w_level) {
+    if constexpr (kLevel) {
+        const uint32_t b = group_ordered(best.level), o = group_ordered(w_level);
+        return !w.open || b > o || (b == o && group_ordered(best.score) > group_ordered(w.score));
+    } else {
+        return !w.open || group_ordered(best.score) > group_ordered(w.score);
+    }
+}
+
 // The rule's steps 1 to 3 for one group at the end of an update.  n: the candidates of this update (best: the best of them,
 // with its position and step; p_min: their smallest position).  has_first: the update had a step (a models update in which
 // this model ran no step has none, and step 1 is skipped: step 3 decides alone).  a, E: the update's a_u and E_u; W: the
-// window.  A flush is E = the largest value, has_first false, n 0.
+// window.  A flush is E = the largest value, has_first false, n 0.  kLevel (group arbitration): *w_level is the open window's
+// level, compared first and carried into the emitted events.
+template <bool kLevel = false>
 MWW_HD GroupClosed group_close(mww_group_window &w, uint32_t n, const GroupEvent &best, long long p_min, bool has_first, long long a,
-                               long long E, long long W) {
+                               long long E, long long W, float *w_level = nullptr) {
     GroupClosed c;
-    if (w.open && has_first && a >= w.deadline) { c.first = true; c.e1 = group_window_event(w); w.open = 0; }
+    if (w.open && has_first && a >= w.deadline) {
+        c.first = true; c.e1 = group_window_event(w); w.open = 0;
+        if constexpr (kLevel) c.e1.level = *w_level;
+    }
     if (n) {
-        const bool take = !w.open || group_ordered(best.score) > group_ordered(w.score);   // a tie keeps the earlier candidate
+        const bool take = group_takes<kLevel>(w, best, kLevel ? *w_level : 0.f);
         if (!w.open) { w.open = 1; w.deadline = p_min + W; w.candidates = 0; }
         if (take) { w.sample = best.sample; w.step = best.step; w.stream = best.stream; w.score = best.score; }
+        if constexpr (kLevel) { if (take) *w_level = best.level; }
         w.candidates += (int32_t)n;
     }
-    if (w.open && E >= w.deadline) { c.second = true; c.e2 = group_window_event(w); w.open = 0; }
+    if (w.open && E >= w.deadline) {
+        c.second = true; c.e2 = group_window_event(w); w.open = 0;
+        if constexpr (kLevel) c.e2.level = *w_level;
+    }
     return c;
 }
 

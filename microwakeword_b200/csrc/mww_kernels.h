@@ -261,6 +261,22 @@ cudaError_t launch_detector_groups_flush(const DetectorArgs &a, const GroupArgs 
 cudaError_t launch_detector_models_groups_flush(const DetectModelsArgs &a, const GroupArgs &g, cudaStream_t st);
 }  // namespace mww
 
+#include "mww_group_arbitration.h"
+namespace mww {
+// group arbitration (mww_group_arbitration.cu, spans, level, key and close in mww_group_arbitration.h; companion library
+// libmww_group_arbitration.so): the grouped launches above with each candidate's level measured at its offer and compared
+// first at the close.  The same two launches per update, one per flush.
+cudaError_t launch_detector_update_arbitrated(const DetectorArgs &a, const double *row_cutoff, const float *probs, int n_steps, long long pitch,
+                                              const GroupArgs &g, const ArbitrationArgs &r, long long last_end, long long step_samples,
+                                              cudaStream_t st);
+cudaError_t launch_detector_models_update_arbitrated(const DetectModelsArgs &a, const GroupArgs &g, const ArbitrationArgs &r, long long row0_end,
+                                                     long long row_end, int hop, cudaStream_t st);
+cudaError_t launch_detector_models_update_arbitrated(const DetectModelsArgsT<DetectModelRows> &a, const DetectModelsArgs &base, const GroupArgs &g,
+                                                     const ArbitrationArgs &r, long long row0_end, long long row_end, int hop, cudaStream_t st);
+cudaError_t launch_detector_arbitrated_flush(const DetectorArgs &a, const GroupArgs &g, const ArbitrationArgs &r, cudaStream_t st);
+cudaError_t launch_detector_models_arbitrated_flush(const DetectModelsArgs &a, const GroupArgs &g, const ArbitrationArgs &r, cudaStream_t st);
+}  // namespace mww
+
 #include "mww_media_guard.h"
 namespace mww {
 // media guard (mww_media_guard.cu, bodies in mww_media_guard.h; companion library libmww_media_guard.so), one launch each.

@@ -321,6 +321,12 @@ def grouped_dtype(dtype) -> np.dtype:
     return np.dtype(timed_dtype(dtype).descr + [("group", np.int32), ("candidates", np.int32)])
 
 
+def arbitrated_dtype(dtype) -> np.dtype:
+    """the drain dtype of an arbitrated detector: grouped_dtype(dtype) and the float32 `level` of each event (NaN for an event
+    of an ungrouped row); 10 log10(level) is the level in dB"""
+    return np.dtype(grouped_dtype(dtype).descr + [("level", np.float32)])
+
+
 # mww_group_window of include/mww.h: one group slot's window
 GROUP_WINDOW_DTYPE = np.dtype([("deadline", np.int64), ("sample", np.int64), ("step", np.int64), ("stream", np.int32), ("score", np.float32),
                                ("candidates", np.int32), ("open", np.int32)])
@@ -372,6 +378,7 @@ class _Detector:
         self.timed = False
         self.event_samples = None
         self.n_groups, self.group_window = 0, 0
+        self.arbitrated, self._arb_engine = False, None
 
     def _time(self) -> None:
         """make the detector timed (mww_time_detector_events) and make event_samples, the device view of the positions"""
@@ -411,6 +418,24 @@ class _Detector:
     def _n_group_slots(self) -> int:
         return self.n_groups * (sum(r == _lib.MWW_DETECT_WAKE for r in self.roles) if hasattr(self, "roles") else 1)
 
+    def _arbitrate(self, engine, speech_samples, noise_samples) -> None:
+        """bind a grouped detector's arbitration to `engine`'s audio history (mww_arbitrate_detector_groups)"""
+        for v, name in ((speech_samples, "speech_samples"), (noise_samples, "noise_samples")):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise ValueError("%s must be an integer (got %r)" % (name, v))
+        if not self.grouped:
+            raise ValueError("arbitration picks the winner of a group: make the detector with groups=n first")
+        self._check(self._L.mww_arbitrate_detector_groups(self._d, engine._h, int(speech_samples), int(noise_samples)))
+        self.arbitrated, self._arb_engine = True, engine
+        self.speech_samples, self.noise_samples = int(speech_samples), int(noise_samples)
+
+    def group_levels(self) -> np.ndarray:
+        """float32 [group slots]: the level of each open window's best candidate (slots as group_windows'); waits for the
+        device"""
+        out = np.zeros(self._n_group_slots(), np.float32)
+        self._check(self._L.mww_get_detector_group_levels(self._d, out.ctypes.data))
+        return out
+
     def flush(self) -> None:
         """Emit every open group window now (mww_flush_detector_groups): before a final drain, or before moving streams out
         of this detector.  Ordered on the current CUDA stream; one launch."""
@@ -427,6 +452,8 @@ class _Detector:
         if self.grouped:
             d["groups"] = self.groups
             d["group_windows"] = self.group_windows()
+        if self.arbitrated:
+            d["group_levels"] = self.group_levels()
         return d
 
     def _load_group_state(self, d: dict):
@@ -445,16 +472,29 @@ class _Detector:
             raise ValueError("groups must be in [-1, %d)" % self.n_groups)
         if not np.isin(w["open"], (0, 1)).all() or (w["candidates"][w["open"] == 1] < 1).any():
             raise ValueError("group_windows: open must be 0 or 1, and an open window needs candidates >= 1")
-        return g, w
+        if not self.arbitrated:
+            if "group_levels" in d:
+                raise ValueError("the state holds group_levels; this detector is not arbitrated")
+            return g, w, None
+        if "group_levels" not in d:
+            raise ValueError("an arbitrated detector's state holds group_levels")
+        lv = np.ascontiguousarray(d["group_levels"], np.float32)
+        if lv.shape != (self._n_group_slots(),):
+            raise ValueError("group_levels must be [%d]" % self._n_group_slots())
+        if not (np.isfinite(lv).all() and (lv >= 0).all()):
+            raise ValueError("group_levels must be finite and not negative")
+        return g, w, lv
 
     def _apply_group_state(self, gw) -> None:
         if gw is None:
             return
-        g, w = gw
+        g, w, lv = gw
         ids = np.arange(g.size, dtype=np.int32)
         fn = self._L.mww_set_multi_detector_groups if hasattr(self, "roles") else self._L.mww_set_detector_groups
         self._check(fn(self._d, ids.ctypes.data, g.ctypes.data, g.size, self._cuda_stream()))
         self._check(self._L.mww_set_detector_group_windows(self._d, w.ctypes.data))
+        if lv is not None:
+            self._check(self._L.mww_set_detector_group_levels(self._d, lv.ctypes.data))
 
     def _check(self, rc: int) -> None:
         if rc != 0:
@@ -482,7 +522,11 @@ class _Detector:
             self._check(self._L.mww_detector_drain(self._d, buf.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
             return buf[:min(n.value, self.capacity)], n.value
         pos = np.empty(self.capacity, np.int64)
-        if self.grouped:
+        if self.arbitrated:
+            grp, cand, lev = np.empty(self.capacity, np.int32), np.empty(self.capacity, np.int32), np.empty(self.capacity, np.float32)
+            self._check(self._L.mww_drain_detector_arbitrated(self._d, buf.ctypes.data, pos.ctypes.data, grp.ctypes.data, cand.ctypes.data,
+                                                              lev.ctypes.data, self.capacity, ctypes.byref(n), self._cuda_stream()))
+        elif self.grouped:
             grp, cand = np.empty(self.capacity, np.int32), np.empty(self.capacity, np.int32)
             self._check(self._L.mww_drain_detector_groups(self._d, buf.ctypes.data, pos.ctypes.data, grp.ctypes.data, cand.ctypes.data,
                                                           self.capacity, ctypes.byref(n), self._cuda_stream()))
@@ -490,12 +534,14 @@ class _Detector:
             self._check(self._L.mww_drain_detector_at(self._d, buf.ctypes.data, pos.ctypes.data, self.capacity, ctypes.byref(n),
                                                       self._cuda_stream()))
         m = min(n.value, self.capacity)
-        out = np.empty(m, grouped_dtype(dtype) if self.grouped else timed_dtype(dtype))
+        out = np.empty(m, arbitrated_dtype(dtype) if self.arbitrated else grouped_dtype(dtype) if self.grouped else timed_dtype(dtype))
         for name in dtype.names:
             out[name] = buf[name][:m]
         out["sample"] = pos[:m]
         if self.grouped:
             out["group"], out["candidates"] = grp[:m], cand[:m]
+        if self.arbitrated:
+            out["level"] = lev[:m]
         return out, n.value
 
     def _drain(self, dtype, keys):
@@ -577,7 +623,11 @@ class StreamDetector(_Detector):
     `groups=n` (timed only) answers a wake word once per household (include/mww.h, "grouped detection"): set_groups puts rows
     in groups [0, n) (-1: none, the default), and of the detections of one group that start within `group_window` samples
     only the best is stored, up to group_window + one step after it fired; drain adds `group` and `candidates`, and flush()
-    stores the windows still open.  Every row's state, cooldown included, is what the ungrouped detector's would be."""
+    stores the windows still open.  Every row's state, cooldown included, is what the ungrouped detector's would be.
+
+    arbitrate(engine) makes the household's answer come from the satellite that heard the wake word loudest over its own
+    background (include/mww.h, "group arbitration"): each candidate's level is measured from the engine's audio history and
+    compared before the score, and drain adds a float32 `level` (NaN for rows of group -1)."""
 
     def __init__(self, n_rows: int, cutoff: float, window: int = 5, cooldown_slices: int = 25, capacity: int = 65536,
                  stream_ids=None, device: int = 0, timed: bool = False, groups=None, group_window: int = 0):
@@ -614,6 +664,8 @@ class StreamDetector(_Detector):
                 raise ValueError("model must be a model index in [0, %d) for a MultiModelEngine (got %r)" % (engine.n_models, model))
             if not multi and model is not None:
                 raise ValueError("model selects a model of a MultiModelEngine; a StreamEngine has one")
+            if self.arbitrated and engine is not self._arb_engine:
+                raise ValueError("an arbitrated detector measures the engine it was bound to (arbitrate): update it with that engine")
             S, b, hop = _history_clock(engine, model)
             stride = engine.stride[int(model)] if multi else engine.stride
             g = engine.pending_rows[int(model)] if multi else engine.pending_rows
@@ -644,7 +696,7 @@ class StreamDetector(_Detector):
 
     def state_dict(self) -> dict:
         """{hist [n_rows, window - 1], seen [n_rows], cooldown [n_rows]}, and a grouped detector's groups [n_rows] and
-        group_windows (GROUP_WINDOW_DTYPE [groups])"""
+        group_windows (GROUP_WINDOW_DTYPE [groups]), and an arbitrated one's group_levels (float32 [groups])"""
         d = dict(hist=np.zeros((self.n_rows, self.window - 1), np.float32), seen=np.zeros(self.n_rows, np.int64),
                  cooldown=np.zeros(self.n_rows, np.int32))
         self._check(self._L.mww_detector_get_state(self._d, d["hist"].ctypes.data, d["seen"].ctypes.data, d["cooldown"].ctypes.data))
@@ -659,6 +711,15 @@ class StreamDetector(_Detector):
         gw = self._load_group_state(d)
         self._check(self._L.mww_detector_set_state(self._d, hist.ctypes.data, seen.ctypes.data, cooldown.ctypes.data))
         self._apply_group_state(gw)
+
+    def arbitrate(self, engine, speech_samples: int = 12000, noise_samples: int = 8000) -> None:
+        """Pick each group window's winner by level, then score (mww_arbitrate_detector_groups), for good: a candidate at
+        position P is measured over the speech span [P - speech_samples, P) and the noise span of noise_samples before it, both
+        read from `engine`'s audio history (the engine every update takes; the rows' streams are its streams), and its level
+        is (mean-removed power of speech + 1) / (that of noise + 1).  10 log10(level) is the level in dB.  The defaults, 0.75 s
+        of speech after 0.5 s of noise, are guesses: nobody has measured which spans pick the nearest device best in real
+        rooms.  Only on a grouped detector that holds no events (after create, or a drain before any update)."""
+        self._arbitrate(engine, speech_samples, noise_samples)
 
     def set_groups(self, rows, groups) -> None:
         """Put the listed ROW indices in `groups` (one value or one per row; -1: no group) (mww_set_detector_groups).  Ordered
@@ -771,7 +832,8 @@ class MultiModelDetector(_Detector):
     the engine, which must keep an audio history, drain adds `sample` and event_samples is the device view.
 
     `groups=n` (timed only) groups streams as StreamDetector's does, per (group, WAKE model): set_groups takes global stream
-    ids, one group per stream for all its wake words."""
+    ids, one group per stream for all its wake words.  arbitrate(engine) picks each window's winner by level, as
+    StreamDetector.arbitrate does."""
 
     def __init__(self, engine, cutoffs, windows=5, cooldown_slices: int = 25, vad=None, capacity: int = 65536, timed: bool = False,
                  groups=None, group_window: int = 0):
@@ -804,6 +866,13 @@ class MultiModelDetector(_Detector):
         if timed:
             self._time()
         self._group(groups, group_window)
+
+    def arbitrate(self, multi, speech_samples: int = 12000, noise_samples: int = 8000) -> None:
+        """StreamDetector.arbitrate for this detector: `multi` must be the engine it was made with, whose history the updates
+        already read their clock from; ties below the level go to the lowest global stream.  The defaults are guesses."""
+        if multi is not self.engine:
+            raise ValueError("a models detector is arbitrated with the engine it was made with")
+        self._arbitrate(multi, speech_samples, noise_samples)
 
     def set_groups(self, stream_ids, groups) -> None:
         """Put the listed GLOBAL streams in `groups` (one value or one per stream; -1: no group), for every WAKE model
@@ -950,7 +1019,8 @@ class MultiModelDetector(_Detector):
 
     def state_dict(self) -> dict:
         """{pending_rows: [p_k], models: [None for an OFF model, else {hist [n_k, window - 1], seen [n_k], cooldown or active [n_k]}]},
-        and a grouped detector's groups [n_streams] and group_windows (GROUP_WINDOW_DTYPE [groups x WAKE models])"""
+        and a grouped detector's groups [n_streams] and group_windows (GROUP_WINDOW_DTYPE [groups x WAKE models]), and an
+        arbitrated one's group_levels (float32 [groups x WAKE models])"""
         models = []
         for k in range(self.n_models):
             if self.roles[k] == _lib.MWW_DETECT_OFF:
