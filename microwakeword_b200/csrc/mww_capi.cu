@@ -322,10 +322,16 @@ int run_frontend_tile(mww_t *h, int first, int n, const T *d_audio, long long au
     }
     if (clip_fuses(h, n_frames)) {
         // long call, one CTA per stream: K1 and the temporal chain in one launch, features written directly (whatever the
-        // size of this particular tile -- the scratch was sized for the fused form)
+        // size of this particular tile -- the scratch was sized for the fused form).  k1_clip_kernel, with half-warp barriers;
+        // MWW_K1_OCC=3 (read once per process) selects the 3-CTA-per-SM kernel with its lane twiddles in registers.
+        static const bool occ3 = getenv("MWW_K1_OCC") != nullptr && atoi(getenv("MWW_K1_OCC")) == 3;
         ProfScope p(h, 0, st);
-        CU(h, launch_frontend_clip_fused(h->P, h->d_carry + (size_t)first * kWindow, h->used, d_audio, audio_stride, n_samples, n, n_frames,
-                                         h->d_estimate + (size_t)first * kNumChannels, d_feat, feat_stream_stride, st));
+        if (occ3)
+            CU(h, launch_frontend_clip_fused(h->P, h->d_carry + (size_t)first * kWindow, h->used, d_audio, audio_stride, n_samples, n, n_frames,
+                                             h->d_estimate + (size_t)first * kNumChannels, d_feat, feat_stream_stride, st));
+        else
+            CU(h, launch_frontend_clip(h->P, h->d_carry + (size_t)first * kWindow, h->used, d_audio, audio_stride, n_samples, n, n_frames,
+                                       h->d_estimate + (size_t)first * kNumChannels, d_feat, feat_stream_stride, st));
         h->launches += 1;
         return MWW_OK;
     }

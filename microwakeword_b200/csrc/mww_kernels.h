@@ -33,6 +33,13 @@ template <typename T>
 cudaError_t launch_frontend_clip_fused(const FrontendParams &P, const int16_t *carry, int used, const T *audio, long long audio_stride,
                                        int n_samples, int n_streams, int n_frames, uint32_t *estimate, uint16_t *feat, long long feat_stream_stride,
                                        cudaStream_t st);
+// the same features from k1_clip_kernel (mww_frontend_clip.cu, companion library libmww_frontend_clip.so): half-warp barriers
+// between the per-frame phases.  The C-ABI layer runs it for every fused clip call except under MWW_K1_OCC=3, which selects
+// launch_frontend_clip_fused's 3-CTA instantiation.
+template <typename T>
+cudaError_t launch_frontend_clip(const FrontendParams &P, const int16_t *carry, int used, const T *audio, long long audio_stride,
+                                 int n_samples, int n_streams, int n_frames, uint32_t *estimate, uint16_t *feat, long long feat_stream_stride,
+                                 cudaStream_t st);
 // any even hop <= 480 samples (window_step != 10 ms): K1 + temporal chain, one CTA per stream, features written directly
 template <typename T>
 cudaError_t launch_frontend_hop(const FrontendParams &P, const int16_t *carry, int used, const T *audio, long long audio_stride,
