@@ -200,6 +200,53 @@ int mww_get_stream_rates(const mww_t *h, int32_t *h_rates, long long *samples16_
  * MWW_EUNSUPPORTED; samples16 outside [0, 2^50] or inputs NULL: MWW_EINVAL. */
 int mww_rate_inputs(int rate, long long samples16, long long *inputs);
 
+/* ---- Per-stream sample formats -----------------------------------------------------------------------------------------
+ * A handle with per-stream rates also gives each stream s a sample format f_s, so that telephony (G.711 bytes at 8 kHz) and
+ * WebRTC or satellites (int16 or float32) feed one handle in one call.  Four formats, one code each (the G.711 codes are
+ * those of MWW_G711_ULAW / MWW_G711_ALAW below):
+ *     MWW_FORMAT_S16 (0) int16 PCM, 2 bytes;   MWW_FORMAT_ULAW (1) mu-law, 1 byte;   MWW_FORMAT_ALAW (2) A-law, 1 byte;
+ *     MWW_FORMAT_F32 (3) float32 in [-1, 1], 4 bytes, converted as mww_features_f32 converts it.
+ * Every stream starts as MWW_FORMAT_S16.  The _mixed entry points (mww_features_mixed, mww_predict_clip_mixed and the
+ * _multi, _host, _host_multi, _remote and _remote_multi forms) take the arguments of their _f32 counterparts with the audio
+ * as bytes.  Row s of the audio starts at audio + s * audio_stride, audio_stride in BYTES, and holds the stream's
+ *     D_s * bytes(f_s)   bytes   (D_s as above: the call's input samples of stream s at its rate),
+ * its samples in its own format; the bytes after them, up to the next row, are never read.  audio_stride must be at least the
+ * largest such row of any (rate, format) pair present on the handle, and the base address and audio_stride must both be
+ * multiples of 4 (float rows aligned); n_samples is n16 as in every call of this mode.  Anything else is MWW_EINVAL before
+ * any work, and a handle without per-stream rates is MWW_EUNSUPPORTED; either way the handle is unchanged.
+ * Stream s is bit-identical to the same stream given its samples decoded to int16 (the G.711 rule below, or the float32
+ * conversion) in an int16 call: features, every model's probabilities and state, resampler history and audio history.  The
+ * resampler decodes each row on load, one launch per rate with streams in the tile as for int16 rows (16 kHz streams on its
+ * identity plan), and every later kernel reads its 16 kHz int16 output.  The staged paths copy each tile's rows as wide as
+ * the tile's widest row, rounded up to 4 bytes: a caller that gives neighbouring streams like sources moves one byte per
+ * G.711 sample.  Their two staging tiles count against MWW_SCRATCH_MB.  A single-rate handle has no per-stream formats; its
+ * calls take one sample type for every row (int16, _f32, _g711). */
+#define MWW_FORMAT_S16 0
+#define MWW_FORMAT_ULAW 1
+#define MWW_FORMAT_ALAW 2
+#define MWW_FORMAT_F32 3
+/* Format h_formats[i] for stream h_ids[i], ordered on cu_stream.  A format changes no state: decoding is memoryless and the
+ * resampler history holds decoded int16 samples.  A handle without per-stream rates: MWW_EUNSUPPORTED; an unknown code, an id
+ * out of range or listed twice, or n < 0: MWW_EINVAL.  Every refusal leaves the handle unchanged.  mww_set_input_rate (back
+ * to one rate) forgets the formats; mww_set_stream_rates and resets keep them. */
+int mww_set_stream_formats(mww_t *h, const int32_t *h_ids, const int32_t *h_formats, int n, void *cu_stream);
+/* h_formats [n_streams]: each stream's format (MWW_FORMAT_S16 for every stream of a single-rate handle) */
+int mww_get_stream_formats(const mww_t *h, int32_t *h_formats);
+int mww_features_mixed(mww_t *h, const uint8_t *d_audio, int n_samples, long long audio_stride,
+                       uint16_t *d_feat, int max_rows, int *h_rows_out, void *cu_stream);
+int mww_predict_clip_mixed(mww_t *h, const uint8_t *d_audio, int n_samples, long long audio_stride,
+                           float *d_probs, int max_probs, int *h_probs_out, void *cu_stream);
+int mww_predict_clip_multi_mixed(mww_t *h, const uint8_t *d_audio, int n_samples, long long audio_stride,
+                                 float *const *d_probs, const int *max_probs, int *h_probs_out, void *cu_stream);
+int mww_predict_clip_host_mixed(mww_t *h, const uint8_t *h_audio, int n_samples, long long audio_stride,
+                                float *h_probs, int max_probs, int *h_probs_out);
+int mww_predict_clip_host_multi_mixed(mww_t *h, const uint8_t *h_audio, int n_samples, long long audio_stride,
+                                      float *const *h_probs, const int *max_probs, int *h_probs_out);
+int mww_predict_clip_remote_mixed(mww_t *h, const uint8_t *src_audio, int n_samples, long long audio_stride,
+                                  float *d_probs, int max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
+int mww_predict_clip_remote_multi_mixed(mww_t *h, const uint8_t *src_audio, int n_samples, long long audio_stride,
+                                        float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream);
+
 /* Frontend only.  d_audio: int16 [n_streams][n_samples] with row pitch `audio_stride` samples.
  * Appends the samples to every stream's window buffer and emits one uint16[40] row per completed
  * 10 ms hop into d_feat [n_streams][max_rows][40].  *h_rows_out = rows emitted per stream

@@ -16,6 +16,7 @@ SO_PATH = os.path.join(_HERE, "libmww_b200.so")
 MWW_ROWS_U16, MWW_ROWS_F32, MWW_ROWS_I8 = 0, 1, 2
 MWW_RATE_PER_STREAM = 0
 MWW_G711_ULAW, MWW_G711_ALAW = 1, 2
+MWW_FORMAT_S16, MWW_FORMAT_ULAW, MWW_FORMAT_ALAW, MWW_FORMAT_F32 = 0, 1, 2, 3
 
 # every symbol include/mww.h declares (checked by tests/test_capi_symbols.py)
 EXPORTS = (
@@ -33,6 +34,9 @@ EXPORTS = (
     "mww_stream_layout_get", "mww_export_streams", "mww_import_streams",
     "mww_set_input_rate", "mww_get_input_rate", "mww_get_resampler_state", "mww_set_resampler_state", "mww_resample_taps",
     "mww_set_stream_rates", "mww_get_stream_rates", "mww_rate_inputs",
+    "mww_set_stream_formats", "mww_get_stream_formats", "mww_features_mixed", "mww_predict_clip_mixed", "mww_predict_clip_multi_mixed",
+    "mww_predict_clip_host_mixed", "mww_predict_clip_host_multi_mixed", "mww_predict_clip_remote_mixed",
+    "mww_predict_clip_remote_multi_mixed",
     "mww_detector_create", "mww_detector_destroy", "mww_detector_update", "mww_detector_drain", "mww_detector_buffers",
     "mww_detector_reset", "mww_detector_reset_device", "mww_detector_get_state", "mww_detector_set_state",
     "mww_multi_detector_create", "mww_multi_detector_update", "mww_multi_detector_get_state", "mww_multi_detector_set_state",
@@ -374,6 +378,13 @@ def lib() -> ctypes.CDLL:
         args = getattr(L, name).argtypes
         getattr(L, name + "_g711").restype = i32
         getattr(L, name + "_g711").argtypes = args[:2] + [i32] + args[2:]
+        # mixed rows (a format per stream): the int16 counterpart's arguments, the audio as bytes with a stride in bytes
+        getattr(L, name + "_mixed").restype = i32
+        getattr(L, name + "_mixed").argtypes = list(args)
+    L.mww_set_stream_formats.restype = i32
+    L.mww_set_stream_formats.argtypes = [vp, vp, vp, i32, vp]
+    L.mww_get_stream_formats.restype = i32
+    L.mww_get_stream_formats.argtypes = [vp, vp]
     L.mww_set_audio_history.restype = i32
     L.mww_set_audio_history.argtypes = [vp, i32, vp]
     L.mww_get_audio_history.restype = i32

@@ -14,6 +14,7 @@
 
 #include <algorithm>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/mww.h"
@@ -103,6 +104,11 @@ struct mww_handle {
     RateGroup groups[kNumRates];
     std::vector<int32_t> rate_ids;                      // every group's members, group after group
     int32_t *d_rate_ids = nullptr;                      // device copy of rate_ids
+    // per-stream sample formats (mww_set_stream_formats) of the _mixed entry points: each stream's kFormat* code, its device
+    // copy, and per rate the formats (bit f for code f) of that rate's members
+    std::vector<uint8_t> stream_format;                 // [n_streams]
+    uint8_t *d_stream_format = nullptr;
+    unsigned rate_formats[kNumRates] = {};
     // audio history (mww_set_audio_history; mww_history.h): the last hist_cap 16 kHz samples of every stream, a ring row per
     // stream; hist_seen counts the samples appended since it was enabled (resets zero rows, not the counter)
     int16_t *d_hist = nullptr;                          // [n_streams][hist_cap]
@@ -216,6 +222,37 @@ bool resample_call_fits(const mww_t *h, int n) {
 bool bad_audio(const mww_t *h, int n_samples, const void *audio, long long audio_stride) {
     return n_samples < 0 || (h->per_rate && (n_samples & 1)) || (n_samples > 0 && !audio) || audio_stride < input_width(h, n_samples);
 }
+// Mixed byte rows (the _mixed entry points, per-stream rates only): row s holds D_s samples of stream s's format.  The call's
+// widest row over the (rate, format) pairs present, in bytes.
+long long mixed_width(const mww_t *h, int n16) {
+    long long w = 0;
+    for (int i = 0; i < kNumRates; ++i)
+        for (int f = 0; f < kNumFormats; ++f)
+            if (h->groups[i].n > 0 && (h->rate_formats[i] >> f & 1)) w = std::max(w, rate_inputs(h, h->groups[i], n16) * format_bytes(f));
+    return w;
+}
+// the same over streams [first, first + n) only: the bytes the staged paths copy per row of that tile
+long long mixed_tile_width(const mww_t *h, int first, int n, int n16) {
+    if (first == 0 && n == h->n_streams) return mixed_width(h, n16);
+    return mixed_rows_width(h->stream_rate.data(), h->stream_format.data(), first, n, h->rs_seen, n16);
+}
+// the audio arguments of a mixed call: n16 as bad_audio, and the base and the byte stride multiples of 4 (float rows
+// aligned), the stride at least the widest row.  The caller has checked that the handle has per-stream rates.
+bool bad_audio(const mww_t *h, int n_samples, const Mixed8 *audio, long long audio_stride) {
+    return n_samples < 0 || (n_samples & 1) || (n_samples > 0 && !audio) || audio_stride < mixed_width(h, n_samples) || (audio_stride & 3) ||
+           (reinterpret_cast<uintptr_t>(audio) & 3);
+}
+// Mixed rows reach only the resampler: the _mixed entry points refuse a handle without per-stream rates before anything
+// else, and on a handle with them every kernel after the resampler reads the 16 kHz scratch.  The call bodies name the
+// direct paths of a single-rate handle for every sample type; with mixed rows they are never taken.
+int mixed_direct(mww_t *h) { return fail(h, MWW_EUNSUPPORTED, "mixed rows need per-stream rates"); }
+// the samples (for mixed rows the bytes) a row of the caller's audio holds for a call of n
+template <typename T>
+long long row_width(const mww_t *h, int n) {
+    if constexpr (std::is_same<T, Mixed8>::value) return mixed_width(h, n);
+    else return input_width(h, n);
+}
+
 // samples of the resampler history a stream keeps (the row length of mww_get_resampler_state)
 int hist_len(const mww_t *h) { return h->per_rate ? resample_max_history() : h->rs.H; }
 
@@ -244,7 +281,10 @@ int run_rates_tile(mww_t *h, int first, int n, const T *d_audio, long long audio
         r.audio_stride = audio_stride; r.out_stride = n16;
         r.L = g.P.L; r.M = g.P.M; r.T = g.P.T; r.H = g.P.H; r.pitch = g.P.pitch;
         r.t0 = resample_t0(resample_inputs(h->rs_seen, g.P.L, g.P.M), g.P.L, g.P.M); r.n_in = n_in; r.n_out = n16; r.n_streams = b - a;
-        CU(h, launch_resample_members(r, h->d_rate_ids + g.off + a, first, d_audio, h->d_rs_out, h->sm_count, st));
+        if constexpr (std::is_same<T, Mixed8>::value)
+            CU(h, launch_resample_mixed(r, h->d_rate_ids + g.off + a, first, h->d_stream_format, d_audio, h->d_rs_out, h->sm_count, st));
+        else
+            CU(h, launch_resample_members(r, h->d_rate_ids + g.off + a, first, d_audio, h->d_rs_out, h->sm_count, st));
         h->launches += 1;
     }
     return MWW_OK;
@@ -253,15 +293,19 @@ int run_rates_tile(mww_t *h, int first, int n, const T *d_audio, long long audio
 template <typename T>
 int run_resample_tile(mww_t *h, int first, int n, const T *d_audio, long long audio_stride, int n_in, int n16, cudaStream_t st) {
     if (h->per_rate) return run_rates_tile(h, first, n, d_audio, audio_stride, n16, st);
-    if (n_in <= 0) return MWW_OK;
-    ResampleArgs a;
-    a.table = h->d_rs_table; a.hist = h->d_rs_hist + (size_t)first * h->rs_hist_stride; a.hist_stride = h->rs_hist_stride;
-    a.audio_stride = audio_stride; a.out_stride = n16;
-    a.L = h->rs.L; a.M = h->rs.M; a.T = h->rs.T; a.H = h->rs.H; a.pitch = h->rs.pitch;
-    a.t0 = resample_t0(h->rs_seen, h->rs.L, h->rs.M); a.n_in = n_in; a.n_out = n16; a.n_streams = n;
-    CU(h, launch_resample(a, d_audio, h->d_rs_out, h->sm_count, st));
-    h->launches += 1;
-    return MWW_OK;
+    if constexpr (std::is_same<T, Mixed8>::value) {
+        return mixed_direct(h);
+    } else {
+        if (n_in <= 0) return MWW_OK;
+        ResampleArgs a;
+        a.table = h->d_rs_table; a.hist = h->d_rs_hist + (size_t)first * h->rs_hist_stride; a.hist_stride = h->rs_hist_stride;
+        a.audio_stride = audio_stride; a.out_stride = n16;
+        a.L = h->rs.L; a.M = h->rs.M; a.T = h->rs.T; a.H = h->rs.H; a.pitch = h->rs.pitch;
+        a.t0 = resample_t0(h->rs_seen, h->rs.L, h->rs.M); a.n_in = n_in; a.n_out = n16; a.n_streams = n;
+        CU(h, launch_resample(a, d_audio, h->d_rs_out, h->sm_count, st));
+        h->launches += 1;
+        return MWW_OK;
+    }
 }
 
 int frames_for(const mww_t *h, int n_samples) {
@@ -369,6 +413,11 @@ int run_history_tile(mww_t *h, int first, int n, const T *d_audio, long long aud
     h->launches += 1;
     return MWW_OK;
 }
+// the direct paths with mixed rows: never taken (mixed_direct)
+int run_frontend_tile(mww_t *h, int, int, const Mixed8 *, long long, int, int, uint16_t *, long long, cudaStream_t) { return mixed_direct(h); }
+int run_carry_tile(mww_t *h, int, int, const Mixed8 *, long long, int, int, cudaStream_t) { return mixed_direct(h); }
+int run_history_tile(mww_t *h, int, int, const Mixed8 *, long long, int, cudaStream_t) { return mixed_direct(h); }
+
 // once per call, where the frontend's counters move on
 void end_history_call(mww_t *h, int n16) {
     if (h->d_hist) h->hist_seen += n16;
@@ -603,6 +652,7 @@ void destroy_impl(mww_t *h) {
     cudaFree(h->d_v); cudaFree(h->d_feat); cudaFree(h->d_ids);
     cudaFree(h->d_gather); cudaFree(h->d_cids);
     cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist); cudaFree(h->d_rs_out); cudaFree(h->d_rate_ids); cudaFree(h->d_hist);
+    cudaFree(h->d_stream_format);
     for (RateGroup &g : h->groups) cudaFree(g.d_table);
     for (int b = 0; b < 2; ++b) {
         cudaFree(h->d_audio_tile[b]); cudaFree(h->d_probs_tile[b]);
@@ -1189,10 +1239,11 @@ int mww_set_input_rate(mww_t *h, int rate) {
     cudaFree(h->d_rs_table); cudaFree(h->d_rs_hist);
     if (h->per_rate) {                 // back to one rate for every stream
         for (RateGroup &g : h->groups) cudaFree(g.d_table);
-        cudaFree(h->d_rate_ids);
+        cudaFree(h->d_rate_ids); cudaFree(h->d_stream_format);
         for (RateGroup &g : h->groups) g = RateGroup{};
-        h->d_rate_ids = nullptr;
-        h->rate_ids.clear(); h->stream_rate.clear();
+        h->d_rate_ids = nullptr; h->d_stream_format = nullptr;
+        h->rate_ids.clear(); h->stream_rate.clear(); h->stream_format.clear();
+        for (unsigned &m : h->rate_formats) m = 0;
         h->per_rate = false;
     }
     h->d_rs_table = table; h->d_rs_hist = hist;
@@ -1252,6 +1303,14 @@ void plan_rate_groups(mww_t *h) {
         g.n = (int)h->rate_ids.size() - g.off;
     }
 }
+// the formats present at each rate, from stream_rate and stream_format
+void plan_rate_formats(mww_t *h) {
+    for (int i = 0; i < kNumRates; ++i) {
+        const RateGroup &g = h->groups[i];
+        h->rate_formats[i] = 0;
+        for (int k = g.off; k < g.off + g.n; ++k) h->rate_formats[i] |= 1u << h->stream_format[(size_t)h->rate_ids[(size_t)k]];
+    }
+}
 
 // the first mww_set_stream_rates: every rate's table, the [n_streams][H_max] history (zero) and the member list, all streams
 // at 16 kHz.  Nothing of the handle changes unless all of it could be allocated.
@@ -1260,10 +1319,13 @@ int enter_per_rate(mww_t *h) {
     const int stride = (resample_max_history() + 1) / 2 * 2;
     int16_t *hist = nullptr;
     int32_t *ids = nullptr;
+    uint8_t *formats = nullptr;
     const size_t S = (size_t)h->n_streams;
     cudaError_t e = cudaMalloc(&hist, S * stride * sizeof(int16_t));
     if (e == cudaSuccess) e = cudaMemset(hist, 0, S * stride * sizeof(int16_t));
     if (e == cudaSuccess) e = cudaMalloc(&ids, S * sizeof(int32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&formats, S);                  // every stream starts as int16 (kFormatS16 = 0)
+    if (e == cudaSuccess) e = cudaMemset(formats, 0, S);
     bool bound = true;
     for (int i = 0; i < kNumRates && e == cudaSuccess && bound; ++i) {
         resample_plan(kResampleRates[i], &g[i].P);
@@ -1276,23 +1338,27 @@ int enter_per_rate(mww_t *h) {
         if (e == cudaSuccess) e = cudaMemcpy(g[i].d_table, host.data(), host.size() * sizeof(int16_t), cudaMemcpyHostToDevice);
     }
     if (e != cudaSuccess || !bound) {
-        cudaFree(hist); cudaFree(ids);
+        cudaFree(hist); cudaFree(ids); cudaFree(formats);
         for (RateGroup &r : g) cudaFree(r.d_table);
         if (!bound) return fail(h, MWW_EINVAL, "mww_set_stream_rates: a phase breaks the partial-sum bound");
         return fail(h, e == cudaErrorMemoryAllocation ? MWW_ENOMEM : MWW_ECUDA, std::string("mww_set_stream_rates: ") + cudaGetErrorString(e));
     }
     h->stream_rate.assign(S, 16000);
+    h->stream_format.assign(S, kFormatS16);
     for (int i = 0; i < kNumRates; ++i) h->groups[i] = g[i];
     plan_rate_groups(h);
+    plan_rate_formats(h);
     if ((e = cudaMemcpy(ids, h->rate_ids.data(), S * sizeof(int32_t), cudaMemcpyHostToDevice)) != cudaSuccess) {
-        cudaFree(hist); cudaFree(ids);
+        cudaFree(hist); cudaFree(ids); cudaFree(formats);
         for (RateGroup &r : h->groups) { cudaFree(r.d_table); r = RateGroup{}; }
-        h->stream_rate.clear(); h->rate_ids.clear();
+        h->stream_rate.clear(); h->rate_ids.clear(); h->stream_format.clear();
+        for (unsigned &m : h->rate_formats) m = 0;
         return cuda_fail(h, e, "mww_set_stream_rates");
     }
     h->d_rs_hist = hist;
     h->rs_hist_stride = stride;
     h->d_rate_ids = ids;
+    h->d_stream_format = formats;
     h->per_rate = true;
     return MWW_OK;
 }
@@ -1323,6 +1389,7 @@ int mww_set_stream_rates(mww_t *h, const int32_t *h_ids, const int32_t *h_rates,
     if (int rc = fill_by_id(h, h->d_rs_hist, (size_t)h->rs_hist_stride * sizeof(int16_t), h->d_ids, n, h->n_streams, st)) return rc;
     for (int i = 0; i < n; ++i) h->stream_rate[(size_t)h_ids[i]] = h_rates[i];
     plan_rate_groups(h);
+    plan_rate_formats(h);
     CU(h, cudaMemcpyAsync(h->d_rate_ids, h->rate_ids.data(), (size_t)h->n_streams * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     return MWW_OK;
 }
@@ -1340,6 +1407,39 @@ int mww_rate_inputs(int rate, long long samples16, long long *inputs) {
     if (!resample_plan(rate, &P)) { g_create_error = "mww_rate_inputs: unsupported input rate"; return MWW_EUNSUPPORTED; }
     if (samples16 < 0 || samples16 > (1ll << 50) || !inputs) { g_create_error = "mww_rate_inputs: bad arguments"; return MWW_EINVAL; }
     *inputs = resample_inputs(samples16, P.L, P.M);
+    return MWW_OK;
+}
+
+static_assert(kFormatS16 == MWW_FORMAT_S16 && kFormatUlaw == MWW_FORMAT_ULAW && kFormatAlaw == MWW_FORMAT_ALAW && kFormatF32 == MWW_FORMAT_F32 &&
+              MWW_FORMAT_ULAW == MWW_G711_ULAW && MWW_FORMAT_ALAW == MWW_G711_ALAW, "format codes");
+
+int mww_set_stream_formats(mww_t *h, const int32_t *h_ids, const int32_t *h_formats, int n, void *cu_stream) {
+    if (!h) return MWW_EINVAL;
+    if (!h->per_rate)
+        return fail(h, MWW_EUNSUPPORTED, "mww_set_stream_formats: sample formats per stream need per-stream rates (mww_set_stream_rates)");
+    if (n < 0 || (n > 0 && (!h_ids || !h_formats))) return fail(h, MWW_EINVAL, "mww_set_stream_formats: bad arguments");
+    std::vector<char> listed((size_t)h->n_streams, 0);
+    for (int i = 0; i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= h->n_streams) return fail(h, MWW_EINVAL, "mww_set_stream_formats: stream id out of range");
+        if (listed[(size_t)h_ids[i]]) return fail(h, MWW_EINVAL, "mww_set_stream_formats: duplicate stream id");
+        listed[(size_t)h_ids[i]] = 1;
+        if (h_formats[i] < 0 || h_formats[i] >= kNumFormats)
+            return fail(h, MWW_EINVAL, "mww_set_stream_formats: a format must be MWW_FORMAT_S16, _ULAW, _ALAW or _F32, not " + std::to_string(h_formats[i]));
+    }
+    ENTER_STATEFUL(h);
+    if (n == 0) return MWW_OK;
+    std::vector<uint8_t> next = h->stream_format;
+    for (int i = 0; i < n; ++i) next[(size_t)h_ids[i]] = (uint8_t)h_formats[i];
+    // pageable source: the copy has taken the bytes when it returns
+    CU(h, cudaMemcpyAsync(h->d_stream_format, next.data(), next.size(), cudaMemcpyHostToDevice, static_cast<cudaStream_t>(cu_stream)));
+    h->stream_format.swap(next);
+    plan_rate_formats(h);
+    return MWW_OK;
+}
+
+int mww_get_stream_formats(const mww_t *h, int32_t *h_formats) {
+    if (!h || !h_formats) return MWW_EINVAL;
+    for (int s = 0; s < h->n_streams; ++s) h_formats[s] = h->per_rate ? h->stream_format[(size_t)s] : kFormatS16;
     return MWW_OK;
 }
 
@@ -1428,13 +1528,14 @@ size_t probs_tile_offset(const mww_t *h, const NnOuts &o, int tile, size_t k) {
 }
 
 // T = int16_t, float, Ulaw8 or Alaw8: the staging buffers hold the caller's samples as they are, and the frontend and carry
-// kernels of that sample type convert them (as on the device path)
+// kernels of that sample type convert them (as on the device path); Mixed8: the bytes of mixed rows, which the resampler
+// decodes
 template <typename T>
 int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, const NnOuts &o, bool dst_is_host,
                  int tile, int n_frames, int n16) {
     const size_t K = h->models.size();
     const T *audio_tile[2] = {static_cast<const T *>(h->d_audio_tile[0]), static_cast<const T *>(h->d_audio_tile[1])};
-    const long long width = input_width(h, n_samples);      // samples per staged row
+    const long long call_width = row_width<T>(h, n_samples);      // samples per staged row
     float *tile_probs[kMaxModels];
     long long tile_probs_stride[kMaxModels];
     TileSpan span[kMaxModels];
@@ -1443,6 +1544,9 @@ int staged_tiles(mww_t *h, const T *src, int n_samples, long long audio_stride, 
     for (int first = 0; first < h->n_streams; first += tile, ++it) {
         const int n = std::min(tile, h->n_streams - first);
         const int b = it & 1;
+        // mixed rows: as many bytes as the tile's widest row, rounded up to 4 so that its float rows stay aligned
+        long long width = call_width;
+        if constexpr (std::is_same<T, Mixed8>::value) width = (mixed_tile_width(h, first, n, n_samples) + 3) / 4 * 4;
         // the staging buffer is free once the kernels of the tile that used it two iterations ago are done
         if (it >= 2) CU(h, cudaStreamWaitEvent(h->st_h2d, h->ev_compute[b], 0));
         cudaEvent_t tl[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1520,9 +1624,12 @@ int predict_clip_staged(mww_t *h, const char *who, const T *src, int n_samples, 
     if (want_tiles <= 0) want_tiles = 16;
     // float32 samples double the staging buffers, so their two tiles count against the scratch budget (MWW_SCRATCH_MB) with
     // the scratch; int16 tiles keep the sizing they have always had, from the scratch alone, and G.711 tiles (half an int16
-    // tile) need nothing beyond that either.  A resampling handle adds its 16 kHz tile scratch.
-    const long long width = input_width(h, n_samples);      // per-stream rates: the call's largest D_s
-    const size_t staged_bytes = sizeof(T) <= sizeof(int16_t) ? 0 : 2 * (size_t)std::max<long long>(width, 1) * sizeof(T);
+    // tile) need nothing beyond that either.  A resampling handle adds its 16 kHz tile scratch.  Mixed rows count their two
+    // tiles at the call's widest row in bytes, rounded up to 4 as each tile's rows are.
+    constexpr bool mixed = std::is_same<T, Mixed8>::value;
+    long long width = row_width<T>(h, n_samples);      // per-stream rates: the call's largest D_s (mixed rows: bytes)
+    if (mixed) width = (width + 3) / 4 * 4;
+    const size_t staged_bytes = sizeof(T) <= sizeof(int16_t) && !mixed ? 0 : 2 * (size_t)std::max<long long>(width, 1) * sizeof(T);
     const size_t gather = gather_bytes_per_stream(h, n_frames);
     int tile = tile_streams(h, n_frames, true, staged_bytes + gather + (resampling(h) ? (size_t)n16 * 2 : 0));
     tile = std::max(1, std::min(tile, std::max((h->n_streams + want_tiles - 1) / want_tiles, std::min(h->n_streams, h->min_tile_streams))));
@@ -1676,6 +1783,14 @@ int with_law(mww_t *h, const char *who, int law, const uint8_t *audio, F run) {
     return fail(h, MWW_EINVAL, std::string(who) + ": law must be MWW_G711_ULAW (1) or MWW_G711_ALAW (2), not " + std::to_string(law));
 }
 
+// run(audio as mixed rows); a handle without per-stream rates is refused before anything else looks at its state
+template <typename F>
+int with_mixed(mww_t *h, const char *who, const uint8_t *audio, F run) {
+    if (!h) return MWW_EINVAL;
+    if (!h->per_rate) return fail(h, MWW_EUNSUPPORTED, std::string(who) + ": mixed rows need per-stream rates (mww_set_stream_rates)");
+    return run(reinterpret_cast<const Mixed8 *>(audio));
+}
+
 }  // namespace
 }  // extern "C++"
 
@@ -1723,6 +1838,55 @@ int mww_predict_clip_remote_multi_g711(mww_t *h, const uint8_t *src_audio, int l
                                        float *const *d_probs, const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
     return with_law(h, "mww_predict_clip_remote_multi_g711", law, src_audio, [&](auto a) {
         return predict_clip_remote_impl(h, "mww_predict_clip_remote_multi_g711", a, n_samples, audio_stride, d_probs, max_probs,
+                                        h_probs_out, n_tiles, cu_stream);
+    });
+}
+
+// ---- mixed rows: the bodies above with a sample format per stream (Mixed8 bytes, decoded by the resampler) --------------
+int mww_features_mixed(mww_t *h, const uint8_t *d_audio, int n_samples, long long audio_stride, uint16_t *d_feat, int max_rows,
+                       int *h_rows_out, void *cu_stream) {
+    return with_mixed(h, "mww_features_mixed", d_audio, [&](auto a) {
+        return features_impl(h, "mww_features_mixed", a, n_samples, audio_stride, d_feat, max_rows, h_rows_out, cu_stream);
+    });
+}
+int mww_predict_clip_mixed(mww_t *h, const uint8_t *d_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                           int *h_probs_out, void *cu_stream) {
+    return with_mixed(h, "mww_predict_clip_mixed", d_audio, [&](auto a) {
+        if (int rc = refuse_multi(h, "mww_predict_clip_mixed", "mww_predict_clip_multi_mixed")) return rc;
+        return predict_clip_impl(h, "mww_predict_clip_mixed", a, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out, cu_stream);
+    });
+}
+int mww_predict_clip_multi_mixed(mww_t *h, const uint8_t *d_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                                 const int *max_probs, int *h_probs_out, void *cu_stream) {
+    return with_mixed(h, "mww_predict_clip_multi_mixed", d_audio, [&](auto a) {
+        return predict_clip_impl(h, "mww_predict_clip_multi_mixed", a, n_samples, audio_stride, d_probs, max_probs, h_probs_out, cu_stream);
+    });
+}
+int mww_predict_clip_host_mixed(mww_t *h, const uint8_t *h_audio, int n_samples, long long audio_stride, float *h_probs, int max_probs,
+                                int *h_probs_out) {
+    return with_mixed(h, "mww_predict_clip_host_mixed", h_audio, [&](auto a) {
+        if (int rc = refuse_multi(h, "mww_predict_clip_host_mixed", "mww_predict_clip_host_multi_mixed")) return rc;
+        return predict_clip_host_impl(h, "mww_predict_clip_host_mixed", a, n_samples, audio_stride, &h_probs, &max_probs, h_probs_out);
+    });
+}
+int mww_predict_clip_host_multi_mixed(mww_t *h, const uint8_t *h_audio, int n_samples, long long audio_stride, float *const *h_probs,
+                                      const int *max_probs, int *h_probs_out) {
+    return with_mixed(h, "mww_predict_clip_host_multi_mixed", h_audio, [&](auto a) {
+        return predict_clip_host_impl(h, "mww_predict_clip_host_multi_mixed", a, n_samples, audio_stride, h_probs, max_probs, h_probs_out);
+    });
+}
+int mww_predict_clip_remote_mixed(mww_t *h, const uint8_t *src_audio, int n_samples, long long audio_stride, float *d_probs, int max_probs,
+                                  int *h_probs_out, int n_tiles, void *cu_stream) {
+    return with_mixed(h, "mww_predict_clip_remote_mixed", src_audio, [&](auto a) {
+        if (int rc = refuse_multi(h, "mww_predict_clip_remote_mixed", "mww_predict_clip_remote_multi_mixed")) return rc;
+        return predict_clip_remote_impl(h, "mww_predict_clip_remote_mixed", a, n_samples, audio_stride, &d_probs, &max_probs, h_probs_out,
+                                        n_tiles, cu_stream);
+    });
+}
+int mww_predict_clip_remote_multi_mixed(mww_t *h, const uint8_t *src_audio, int n_samples, long long audio_stride, float *const *d_probs,
+                                        const int *max_probs, int *h_probs_out, int n_tiles, void *cu_stream) {
+    return with_mixed(h, "mww_predict_clip_remote_multi_mixed", src_audio, [&](auto a) {
+        return predict_clip_remote_impl(h, "mww_predict_clip_remote_multi_mixed", a, n_samples, audio_stride, d_probs, max_probs,
                                         h_probs_out, n_tiles, cu_stream);
     });
 }

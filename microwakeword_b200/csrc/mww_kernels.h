@@ -131,6 +131,11 @@ cudaError_t launch_resample(const ResampleArgs &a, const T *audio, int16_t *out,
 template <typename T>
 cudaError_t launch_resample_members(const ResampleArgs &a, const int32_t *ids, int first, const T *audio, int16_t *out, int sm_count,
                                     cudaStream_t st);
+// the same with a sample format per stream (MixedRows, mww_resample.h): audio is bytes, a.audio_stride counts bytes, and
+// member ids[i] reads its row in format formats[ids[i]] (device memory [n_streams]); base and stride multiples of 4.
+// Instantiated in libmww_resample_mixed.so.
+cudaError_t launch_resample_mixed(const ResampleArgs &a, const int32_t *ids, int first, const uint8_t *formats, const Mixed8 *audio,
+                                  int16_t *out, int sm_count, cudaStream_t st);
 }  // namespace mww
 
 #include "mww_records.h"

@@ -1,7 +1,7 @@
 // mww_resample.cuh -- the input-rate resampler kernel (definition and index math: mww_resample.h) and its launchers, included
 // by the translation units that instantiate them: mww_resample.cu (the tile's streams in order, a handle with one input
 // rate) and mww_resample_rates.cu (one rate's members in the tile, per-stream rates), each in a companion library of its own,
-// and mww_frontend_g711.cu (both, for G.711 audio).
+// mww_frontend_g711.cu (both, for G.711 audio) and mww_resample_mixed.cu (members with a sample format per stream).
 //
 // One launch per stream tile (per rate in the tile with per-stream rates) turns input-rate samples (int16, or float32
 // converted by pcm16_from_f32, or G.711 decoded, on load) into 16 kHz int16 samples in scratch, which the frontend kernels then read as any
@@ -36,6 +36,41 @@ struct SmemWindow {
 };
 }  // namespace
 
+// one stream of a launch, its rows x (input, samples of type T), hist and y (16 kHz output); the whole CTA runs it
+template <bool kGathered, typename T>
+MWW_D void resample_stream(const ResampleArgs &a, const int16_t *table, int32_t *xs, const T *x, int16_t *hist, int16_t *y) {
+    if constexpr (kGathered) {
+        if (a.T == 0) {                                // the identity plan (16 kHz members): no window, no history
+            for (int q = threadIdx.x; q < a.n_out; q += blockDim.x) y[q] = pcm16(x[q]);
+            return;
+        }
+    }
+    for (int q0 = 0; q0 < a.n_out; q0 += kChunk) {
+        const int nq = min(kChunk, a.n_out - q0);
+        const int k_first = (a.t0 + q0 * a.M) / a.L;
+        const int k_last = (a.t0 + (q0 + nq - 1) * a.M) / a.L;
+        const int lo = k_first - (a.T - 1);
+        __syncthreads();                               // the previous chunk (or stream) is done with xs
+        for (int j = lo + (int)threadIdx.x; j <= k_last; j += blockDim.x)
+            xs[j - lo] = j >= 0 ? (int32_t)pcm16(x[j]) : (int32_t)hist[a.H + j];
+        __syncthreads();
+        const SmemWindow w{xs, lo};
+        for (int q = q0 + threadIdx.x; q < q0 + nq; q += blockDim.x)
+            y[q] = resample_output(table, a.pitch, a.T, a.L, a.M, a.t0, q, w);
+    }
+    // history: the last H samples of (history, this call's input)
+    __syncthreads();
+    for (int j = threadIdx.x; j < a.H; j += blockDim.x) {
+        const int src = a.n_in - a.H + j;
+        xs[j] = src >= 0 ? (int32_t)pcm16(x[src]) : (int32_t)hist[a.H + src];
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < a.H; j += blockDim.x) hist[j] = (int16_t)xs[j];
+}
+
+// Rows::kMixed (MixedRows): `audio` is bytes and a.audio_stride counts bytes; each stream's row holds samples of its own
+// format, which the CTA reads once and dispatches on -- a branch per stream, uniform over the CTA, none per sample.  The
+// caller keeps the base and the stride multiples of 4, so float rows are aligned.
 template <typename T, typename Rows>
 __global__ void __launch_bounds__(kResampleThreads) resample_kernel(ResampleArgs a, const T *__restrict__ audio, int16_t *__restrict__ out, Rows rows) {
     extern __shared__ __align__(16) unsigned char smem[];
@@ -48,33 +83,16 @@ __global__ void __launch_bounds__(kResampleThreads) resample_kernel(ResampleArgs
         const T *x = audio + (size_t)rows.io(s) * a.audio_stride;
         int16_t *hist = a.hist + (size_t)rows.hist(s) * a.hist_stride;
         int16_t *y = out + (size_t)rows.io(s) * a.out_stride;
-        if constexpr (Rows::kGathered) {
-            if (a.T == 0) {                            // the identity plan (16 kHz members): no window, no history
-                for (int q = threadIdx.x; q < a.n_out; q += blockDim.x) y[q] = pcm16(x[q]);
-                continue;
+        if constexpr (Rows::kMixed) {
+            switch (rows.format(s)) {
+            case kFormatUlaw: resample_stream<true>(a, table, xs, reinterpret_cast<const Ulaw8 *>(x), hist, y); break;
+            case kFormatAlaw: resample_stream<true>(a, table, xs, reinterpret_cast<const Alaw8 *>(x), hist, y); break;
+            case kFormatF32: resample_stream<true>(a, table, xs, reinterpret_cast<const float *>(x), hist, y); break;
+            default: resample_stream<true>(a, table, xs, reinterpret_cast<const int16_t *>(x), hist, y); break;
             }
+        } else {
+            resample_stream<Rows::kGathered>(a, table, xs, x, hist, y);
         }
-        for (int q0 = 0; q0 < a.n_out; q0 += kChunk) {
-            const int nq = min(kChunk, a.n_out - q0);
-            const int k_first = (a.t0 + q0 * a.M) / a.L;
-            const int k_last = (a.t0 + (q0 + nq - 1) * a.M) / a.L;
-            const int lo = k_first - (a.T - 1);
-            __syncthreads();                           // the previous chunk (or stream) is done with xs
-            for (int j = lo + (int)threadIdx.x; j <= k_last; j += blockDim.x)
-                xs[j - lo] = j >= 0 ? (int32_t)pcm16(x[j]) : (int32_t)hist[a.H + j];
-            __syncthreads();
-            const SmemWindow w{xs, lo};
-            for (int q = q0 + threadIdx.x; q < q0 + nq; q += blockDim.x)
-                y[q] = resample_output(table, a.pitch, a.T, a.L, a.M, a.t0, q, w);
-        }
-        // history: the last H samples of (history, this call's input)
-        __syncthreads();
-        for (int j = threadIdx.x; j < a.H; j += blockDim.x) {
-            const int src = a.n_in - a.H + j;
-            xs[j] = src >= 0 ? (int32_t)pcm16(x[src]) : (int32_t)hist[a.H + src];
-        }
-        __syncthreads();
-        for (int j = threadIdx.x; j < a.H; j += blockDim.x) hist[j] = (int16_t)xs[j];
     }
 }
 

@@ -162,18 +162,53 @@ inline int resample_max_history() {
 // Which rows stream index s of a resample_kernel launch reads and writes.  TileRows: the tile's streams in order (a handle
 // with one input rate).  MemberRows: the members of one rate in the tile, ids[0, n) sorted global ids (per-stream rates):
 // input and output rows ids[s] - first of the tile, history row ids[s] of the handle.  A plan without taps (16 kHz) is the
-// identity there: output q = pcm16(input q), no history.
+// identity there: output q = pcm16(input q), no history.  MixedRows (below): MemberRows with a sample format per stream.
 struct TileRows {
-    static constexpr bool kGathered = false;
+    static constexpr bool kGathered = false, kMixed = false;
     MWW_HD int io(int s) const { return s; }
     MWW_HD int hist(int s) const { return s; }
 };
 struct MemberRows {
-    static constexpr bool kGathered = true;
+    static constexpr bool kGathered = true, kMixed = false;
     const int32_t *ids; int first;
     MWW_HD int io(int s) const { return ids[s] - first; }
     MWW_HD int hist(int s) const { return ids[s]; }
 };
+
+// Per-stream sample formats (mww_set_stream_formats): the codes of include/mww.h, and the bytes one sample of each takes.
+// A row of mixed audio (the _mixed entry points) is bytes: row s holds D_s samples of stream s's own format, with the row
+// pitch in bytes; Mixed8 is one such byte, the sample type the call bodies of mww_capi.cu carry for these rows.
+constexpr int kFormatS16 = 0, kFormatUlaw = 1, kFormatAlaw = 2, kFormatF32 = 3, kNumFormats = 4;
+MWW_HD int format_bytes(int f) { return f == kFormatF32 ? 4 : (f == kFormatS16 ? 2 : 1); }
+struct Mixed8 { uint8_t v; };
+// MemberRows whose rows are bytes in each member's own format, fmt [n_streams] by global id (the resampler reads it once per
+// stream and runs that format's body)
+struct MixedRows {
+    static constexpr bool kGathered = true, kMixed = true;
+    const int32_t *ids; int first; const uint8_t *fmt;
+    MWW_HD int io(int s) const { return ids[s] - first; }
+    MWW_HD int hist(int s) const { return ids[s]; }
+    MWW_HD int format(int s) const { return fmt[ids[s]]; }
+};
+
+// Mixed rows of a call of n16 at counter t16 (per-stream rates): the bytes the widest row of streams [first, first + n)
+// holds, D_s * format_bytes(f_s), rates[s] one of kResampleRates.  The staged paths copy each tile's rows this wide.
+inline long long mixed_rows_width(const int32_t *rates, const uint8_t *formats, int first, int n, long long t16, int n16) {
+    constexpr int kRates = (int)(sizeof kResampleRates / sizeof kResampleRates[0]);
+    long long D[kRates];
+    for (int i = 0; i < kRates; ++i) {
+        const int g = resample_gcd(16000, kResampleRates[i]), L = 16000 / g, M = kResampleRates[i] / g;
+        D[i] = resample_inputs(t16 + n16, L, M) - resample_inputs(t16, L, M);
+    }
+    long long w = 0;
+    for (int s = first; s < first + n; ++s) {
+        int i = 0;
+        while (i + 1 < kRates && kResampleRates[i] != rates[s]) ++i;
+        const long long b = D[i] * format_bytes(formats[s]);
+        w = b > w ? b : w;
+    }
+    return w;
+}
 
 // Output q of a call: t = t0 + q M upsampled samples past the call's first input, newest input k = floor(t / L), phase
 // p = t mod L, and y = sat16((sum_i table[p][i] x(k - i) + 2^14) >> 15) over i < T.  x(j) is the call's input j for j >= 0 and

@@ -105,6 +105,34 @@ def _law_code(law, is_uint8: bool):
     return None if law is None else G711_LAWS[law]
 
 
+# sample formats per stream (set_stream_formats, include/mww.h): name -> code, and the bytes one sample of each code takes
+SAMPLE_FORMATS = {"s16": _lib.MWW_FORMAT_S16, "ulaw": _lib.MWW_FORMAT_ULAW, "alaw": _lib.MWW_FORMAT_ALAW, "f32": _lib.MWW_FORMAT_F32}
+FORMAT_BYTES = np.array([2, 1, 1, 4], np.int32)
+
+
+def format_codes(formats, n: int) -> np.ndarray:
+    """formats (one name of SAMPLE_FORMATS or code, or one per stream) -> np.int32 [n] codes; ValueError for anything else"""
+    f = np.asarray(formats, dtype=object)
+    if f.ndim == 0:
+        f = np.full(n, f.item(), dtype=object)
+    if f.shape != (n,):
+        raise ValueError("formats must be one format per id (%d), not shape %s" % (n, f.shape))
+    out = np.zeros(n, np.int32)
+    for i, v in enumerate(f):
+        if isinstance(v, str) and v in SAMPLE_FORMATS:
+            out[i] = SAMPLE_FORMATS[v]
+        elif isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_)) and int(v) in SAMPLE_FORMATS.values():
+            out[i] = int(v)
+        else:
+            raise ValueError("a sample format must be one of %s or its code 0..3, not %r" % (sorted(SAMPLE_FORMATS), v))
+    return out
+
+
+def bytes_for_formats(rates, formats, samples16_seen: int, n16: int) -> np.ndarray:
+    """int32 [len(rates)]: the bytes row s of a mixed call of n16 holds, D_s (inputs_for_rates) times its format's sample size"""
+    return inputs_for_rates(rates, samples16_seen, n16) * FORMAT_BYTES[np.asarray(formats, np.int64)]
+
+
 def _kind(dtype) -> str:
     """numpy or torch sample dtype -> "int16", "float32", "uint8", ..."""
     return str(dtype).replace("torch.", "")
@@ -173,15 +201,16 @@ class StreamRecords:
     of each stream's audio history, oldest first: a CUDA int16 tensor [n, m] that import writes back after the records.
     Records exported with resampler=True (mww_export_resampled_streams) also carry each stream's resampler history:
     `resampler` is then the _lib.MwwResamplerLayout (record size and the exporter's input-rate counters) and `rates` the
-    streams' input rates, np.int32 [n]; both are None otherwise."""
+    streams' input rates, np.int32 [n]; both are None otherwise.  `formats` is None, or (records of an engine with per-stream
+    rates) the streams' sample formats, np.int32 [n] codes, which import_streams gives the streams it writes."""
 
     _SCALARS = ("record_bytes", "n_models", "frontend_buffered", "hop_samples")
     _ARRAYS = ("pending_rows", "model_hash", "rows_are_features")
     _RESAMPLER = ("record_bytes", "resampler_off", "rate", "inputs_seen", "samples16_seen")
 
-    def __init__(self, data, layout, history=None, resampler=None, rates=None):
+    def __init__(self, data, layout, history=None, resampler=None, rates=None, formats=None):
         self.data, self.layout, self.history = data, layout, history
-        self.resampler, self.rates = resampler, rates
+        self.resampler, self.rates, self.formats = resampler, rates, formats
 
     def save(self, path) -> None:
         """np.savez of the records, the layout's fields, the history when there is one and the resampler layout and rates
@@ -193,13 +222,15 @@ class StreamRecords:
         if self.resampler is not None:
             fields.update({"resampler_" + k: np.asarray(getattr(self.resampler, k)) for k in self._RESAMPLER})
             fields["rates"] = np.asarray(self.rates, np.int32)
+        if self.formats is not None:
+            fields["formats"] = np.asarray(self.formats, np.int32)
         np.savez(path, data=self.data.cpu().numpy(), **fields)
 
     @classmethod
     def load(cls, path, device) -> "StreamRecords":
         torch = _torch()
         layout = _lib.MwwStreamLayout()
-        resampler = rates = None
+        resampler = rates = formats = None
         with np.load(path) as z:
             for k in cls._SCALARS:
                 setattr(layout, k, int(z[k]))
@@ -212,7 +243,9 @@ class StreamRecords:
                 for k in cls._RESAMPLER:
                     setattr(resampler, k, int(z["resampler_" + k]))
                 rates = np.ascontiguousarray(z["rates"], np.int32)
-        return cls(data, layout, history, resampler, rates)
+            if "formats" in z.files:
+                formats = np.ascontiguousarray(z["formats"], np.int32)
+        return cls(data, layout, history, resampler, rates, formats)
 
 
 class _Engine:
@@ -267,7 +300,7 @@ class _Engine:
         while no samples are buffered (after create / reset / reset_frontend).  On an engine with per-stream rates it returns
         every stream to this one rate."""
         _lib.check(self._h, self._L.mww_set_input_rate(self._h, int(rate)))
-        self._rate_set = None
+        self._rate_set = self._pair_set = None
 
     # ------------------------------------------------------------------ per-stream input rates
     @property
@@ -294,7 +327,7 @@ class _Engine:
         if r.shape != ids.shape or (r.size and not np.issubdtype(r.dtype, np.integer)):
             raise ValueError("rates must be one integer rate per id")
         r = np.ascontiguousarray(r, np.int32)
-        self._rate_set = None
+        self._rate_set = self._pair_set = None
         _lib.check(self._h, self._L.mww_set_stream_rates(self._h, ids.ctypes.data, r.ctypes.data, ids.size, self._cu_stream()))
 
     def _rates_present(self) -> tuple:
@@ -302,6 +335,52 @@ class _Engine:
         if getattr(self, "_rate_set", None) is None:
             self._rate_set = tuple(int(r) for r in np.unique(self.stream_rates))
         return self._rate_set
+
+    # ------------------------------------------------------------------ per-stream sample formats
+    @property
+    def stream_formats(self) -> np.ndarray:
+        """int32 [n_streams]: each stream's sample format code (SAMPLE_FORMATS; "s16" for every stream unless
+        per_stream_rates)"""
+        out = np.zeros(self.n_streams, np.int32)
+        _lib.check(self._h, self._L.mww_get_stream_formats(self._h, out.ctypes.data))
+        return out
+
+    def set_stream_formats(self, ids, formats) -> None:
+        """Stream ids[i] sends its audio in formats[i] from the next call on ("s16", "f32", "ulaw", "alaw" or their codes; one
+        format applies to every listed id), ordered on the current CUDA stream (mww_set_stream_formats).  Only on an engine
+        with per-stream rates (MwwError MWW_EUNSUPPORTED otherwise).  No state changes: a stream may switch formats between
+        any two calls.  The mixed=True calls then take uint8 rows, row s holding bytes_for(samples16)[s] bytes."""
+        ids = self._ids(ids)
+        f = format_codes(formats, ids.size)
+        self._pair_set = None
+        _lib.check(self._h, self._L.mww_set_stream_formats(self._h, ids.ctypes.data, f.ctypes.data, ids.size, self._cu_stream()))
+
+    def _pairs_present(self) -> tuple:
+        """the distinct (rate, format) pairs of the streams, kept until rates or formats change"""
+        if getattr(self, "_pair_set", None) is None:
+            pairs = np.unique(np.stack([self.stream_rates, self.stream_formats], 1), axis=0)
+            self._pair_set = tuple((int(r), int(f)) for r, f in pairs)
+        return self._pair_set
+
+    def bytes_for(self, samples16: int) -> np.ndarray:
+        """int32 [n_streams]: the bytes each stream's row holds in the next mixed=True call of samples16 (per_stream_rates
+        only): inputs_for(samples16) times the sample size of the stream's format (2, 4 or 1 for s16, f32 and G.711).  The
+        rows' pitch is at least the largest of these and, like the buffer's address, a multiple of 4."""
+        return self.inputs_for(samples16) * FORMAT_BYTES[self.stream_formats]
+
+    def _mixed_len(self, width: int, stride: int, ptr: int, samples16) -> int:
+        """-> n_samples (n16) of a mixed=True call whose rows hold `width` bytes at pitch `stride` from address `ptr`, or
+        ValueError before the library is called"""
+        rate, t = self._rate()
+        if rate != RATE_PER_STREAM:
+            raise ValueError("mixed=True is for an engine with per-stream rates (set_stream_rates)")
+        n16 = self._check_samples16(samples16)
+        need = max((int(bytes_for_formats([r], [f], t, n16)[0]) for r, f in self._pairs_present()), default=0) if n16 else 0
+        if width < need:
+            raise ValueError("mixed rows hold %d bytes; this call of %d 16 kHz samples needs %d (bytes_for)" % (width, n16, need))
+        if stride % 4 or ptr % 4:
+            raise ValueError("mixed rows need an address and a row pitch that are multiples of 4 bytes (pitch %d)" % stride)
+        return n16
 
     def inputs_for(self, samples16: int) -> np.ndarray:
         """int32 [n_streams]: the samples each stream's row holds in the next call of samples16 (per_stream_rates only):
@@ -347,6 +426,7 @@ class _Engine:
         d.update(input_rate=self.input_rate, resampler_history=hist, inputs_seen=seen.value)
         if self.input_rate == RATE_PER_STREAM:
             d["stream_rates"] = self.stream_rates
+            d["stream_formats"] = self.stream_formats
 
     def _set_resampler(self, d: dict) -> None:
         rate = int(d.get("input_rate", 16000))
@@ -363,13 +443,26 @@ class _Engine:
             if rates.shape != (self.n_streams,):
                 raise ValueError("stream_rates must be int32 [n_streams]")
             self.set_stream_rates(np.arange(self.n_streams, dtype=np.int32), rates)
+            if "stream_formats" in d:
+                self.set_stream_formats(np.arange(self.n_streams, dtype=np.int32), np.ascontiguousarray(d["stream_formats"], np.int32))
         _lib.check(self._h, self._L.mww_set_resampler_state(self._h, hist.ctypes.data, int(d["inputs_seen"])))
 
     @property
     def launch_count(self) -> int:
         return int(self._L.mww_launch_count(self._h))
 
-    def _check_audio(self, audio, law=None):
+    @staticmethod
+    def _check_mixed(law, mixed: bool, is_uint8: bool) -> bool:
+        """mixed=True: the audio is uint8 rows of bytes in each stream's format, and law= has no meaning"""
+        if not mixed:
+            return False
+        if law is not None:
+            raise ValueError("law= is for uint8 audio of one G.711 law; with mixed=True each stream's format says how to read it")
+        if not is_uint8:
+            raise ValueError("mixed=True takes uint8 rows of bytes (bytes_for), not another dtype")
+        return True
+
+    def _check_audio(self, audio, law=None, mixed=False):
         """-> (n_samples, row pitch in samples, is_float32).  float32 audio is converted to int16 inside the frontend kernels,
         exactly as audio_utils.to_int16 converts it on the host; other float dtypes are refused (float64 keeps its exact host
         conversion: rounding it to float32 first could move a sample across an integer boundary after the x 32768).  uint8
@@ -379,12 +472,13 @@ class _Engine:
                 or not audio.is_cuda):
             raise ValueError("audio must be a CUDA int16 or float32 tensor (uint8 with law=) of shape [n_streams=%d, n_samples]"
                              % self.n_streams)
-        _law_code(law, audio.dtype == torch.uint8)
+        if not self._check_mixed(law, mixed, audio.dtype == torch.uint8):
+            _law_code(law, audio.dtype == torch.uint8)
         if audio.stride(1) != 1 and audio.shape[1] > 1:
             raise ValueError("audio samples must be contiguous along the last dimension")
         return audio.shape[1], (audio.stride(0) if audio.shape[1] > 0 else 0), audio.dtype == torch.float32
 
-    def _check_host_audio(self, audio: np.ndarray, law=None):
+    def _check_host_audio(self, audio: np.ndarray, law=None, mixed=False):
         """int16 or float32 host audio [S, N] -> (the array with contiguous samples, its row pitch in samples, is_float32).
         An array whose samples are not contiguous, or whose row stride is not a whole number of samples >= N (a view made
         with as_strided or an explicit strides= argument, a broadcast, reversed rows), is copied first.  float32 goes through
@@ -395,15 +489,18 @@ class _Engine:
                 or audio.shape[0] != self.n_streams):
             raise ValueError("audio must be an int16 or float32 array (uint8 with law=) of shape [n_streams=%d, n_samples]"
                              % self.n_streams)
-        _law_code(law, audio.dtype == np.uint8)
+        if not self._check_mixed(law, mixed, audio.dtype == np.uint8):
+            _law_code(law, audio.dtype == np.uint8)
         n, size = audio.shape[1], audio.itemsize
         if n > 0 and ((audio.strides[1] != size and n > 1) or audio.strides[0] % size or audio.strides[0] < n * size):
             audio = np.ascontiguousarray(audio)
         return audio, (audio.strides[0] // audio.itemsize if n else 0), audio.dtype == np.float32
 
-    def _remote_fn(self, dtype, name: str, law=None):
+    def _remote_fn(self, dtype, name: str, law=None, mixed=False):
         """the int16, float32 or G.711 (uint8 with `law`) form of the raw-pointer entry point `name`, from a numpy (or torch)
-        sample dtype"""
+        sample dtype; None is int16, or uint8 with mixed=True (the _mixed form)"""
+        if dtype is None:
+            dtype = np.uint8 if mixed else np.int16
         if str(dtype) in ("torch.int16", "torch.float32", "torch.uint8"):
             dtype = _kind(dtype)
         try:
@@ -412,11 +509,13 @@ class _Engine:
             dt = None
         if dt not in (np.dtype(np.int16), np.dtype(np.float32), np.dtype(np.uint8)):
             raise ValueError("dtype must be int16 or float32 (uint8 with law=), not %r" % (dtype,))
-        return self._audio_fn(name, dt.name, law)
+        return self._audio_fn(name, dt.name, law, mixed)
 
-    def _audio_fn(self, name: str, kind: str, law=None):
-        """the entry point `name` for audio of `kind` ("int16", "float32" or "uint8"): `name`, its _f32 form, or its _g711 form
-        with the law's code passed after the audio pointer"""
+    def _audio_fn(self, name: str, kind: str, law=None, mixed=False):
+        """the entry point `name` for audio of `kind` ("int16", "float32" or "uint8"): `name`, its _f32 form, its _g711 form
+        with the law's code passed after the audio pointer, or with mixed=True its _mixed form"""
+        if self._check_mixed(law, mixed, kind == "uint8"):
+            return getattr(self._L, name + "_mixed")
         code = _law_code(law, kind == "uint8")
         if code is None:
             return getattr(self._L, name + "_f32" if kind == "float32" else name)
@@ -537,13 +636,14 @@ class _Engine:
             raise ValueError("end must be one integer position per id (%d)" % n)
         return torch.from_numpy(np.ascontiguousarray(e, np.int64)).to(self._dev())
 
-    def features(self, audio, out=None, samples16=None, law=None):
+    def features(self, audio, out=None, samples16=None, law=None, mixed=False):
         """int16 or float32 CUDA tensor [S, N] -> uint16 CUDA tensor [S, rows, 40] (rows may be 0); `out` reuses a caller buffer.
         With per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16).  G.711 audio: a uint8 tensor
-        of codes and law='ulaw' or 'alaw', decoded inside the kernels (include/mww.h gives the rule)."""
+        of codes and law='ulaw' or 'alaw', decoded inside the kernels (include/mww.h gives the rule).  mixed=True (per-stream
+        rates): a uint8 tensor of bytes, row s in stream s's format (set_stream_formats), N >= every bytes_for(samples16)."""
         torch = _torch()
-        width, stride, _ = self._check_audio(audio, law)
-        n = self._call_len(width, samples16)
+        width, stride, _ = self._check_audio(audio, law, mixed)
+        n = self._mixed_len(width, max(stride, width), audio.data_ptr(), samples16) if mixed else self._call_len(width, samples16)
         stride = max(stride, width)
         rows = rows_for(self.frontend_buffered, self._samples16(n), self.hop)
         if out is None:
@@ -552,7 +652,7 @@ class _Engine:
               or out.shape[1] < max(rows, 1) or out.shape[2] != NUM_FEATURES):
             raise ValueError("out must be a contiguous CUDA uint16 tensor [n_streams, >= rows, 40]")
         got = ctypes.c_int(0)
-        fn = self._audio_fn("mww_features", _kind(audio.dtype), law)
+        fn = self._audio_fn("mww_features", _kind(audio.dtype), law, mixed)
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, stride, out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
@@ -590,7 +690,8 @@ class _Engine:
         hears, an endpointer's lookback and the commands in progress).
         resampler=True exports records that also carry each stream's resampler history (mww_export_resampled_streams), on an
         engine at any input rate or with per-stream rates; records.resampler and records.rates say what the importer must
-        match.  Without it an engine that resamples refuses (MwwError, MWW_EUNSUPPORTED)."""
+        match, and on an engine with per-stream rates records.formats holds the streams' sample formats.  Without it an engine
+        that resamples refuses (MwwError, MWW_EUNSUPPORTED)."""
         torch = _torch()
         ids = self._ids(ids)
         if isinstance(history, bool) or not isinstance(history, (int, np.integer)) or history < 0:
@@ -604,12 +705,13 @@ class _Engine:
             data = torch.empty((ids.size, int(self.resampler_layout().record_bytes)), dtype=torch.uint8, device=self._dev())
             _lib.check(self._h, self._L.mww_export_resampled_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
                                                                      ctypes.byref(rs), rates.ctypes.data, self._cu_stream()))
+            formats = self.stream_formats[ids] if self.per_stream_rates else None
         else:
-            rs = rates = None
+            rs = rates = formats = None
             data = torch.empty((ids.size, int(self.stream_layout().record_bytes)), dtype=torch.uint8, device=self._dev())
             _lib.check(self._h, self._L.mww_export_streams(self._h, ids.ctypes.data, ids.size, data.data_ptr(), ctypes.byref(layout),
                                                            self._cu_stream()))
-        return StreamRecords(data, layout, self.audio_history(ids, int(history)) if history else None, rs, rates)
+        return StreamRecords(data, layout, self.audio_history(ids, int(history)) if history else None, rs, rates, formats)
 
     def import_streams(self, ids, records: StreamRecords) -> None:
         """Stream ids[i] of this engine takes the state of records.data[i] (mww_import_streams): it continues bit for bit as
@@ -624,7 +726,11 @@ class _Engine:
 
             recs = src.export_streams(src_ids, history=m, resampler=True)
             dst.set_stream_rates(dst_ids, recs.rates)
-            dst.import_streams(dst_ids, recs)"""
+            dst.import_streams(dst_ids, recs)
+
+        Records that carry formats (records.formats) give them to the streams with set_stream_formats once the import is
+        done, so that a stream that sent mu-law keeps being read as mu-law; formats other than "s16" need an engine with
+        per-stream rates (ValueError before anything is imported otherwise)."""
         torch = _torch()
         ids = self._ids(ids)
         rs = getattr(records, "resampler", None)
@@ -634,6 +740,11 @@ class _Engine:
             if not isinstance(rates, np.ndarray) or rates.dtype != np.int32 or rates.shape != (ids.size,):
                 raise ValueError("records.rates must be an np.int32 array [len(ids)=%d]" % ids.size)
             rates = np.ascontiguousarray(rates)
+        formats = getattr(records, "formats", None)
+        if formats is not None:
+            formats = format_codes(formats, ids.size)
+            if formats.any() and not self.per_stream_rates:
+                raise ValueError("records.formats holds formats other than 's16'; they need an engine with per-stream rates")
         data = records.data
         if (not isinstance(data, torch.Tensor) or data.dtype != torch.uint8 or data.dim() != 2 or data.shape[0] != ids.size
                 or data.shape[1] != record_bytes or not data.is_contiguous() or data.device != self._dev()):
@@ -659,6 +770,8 @@ class _Engine:
             stride = hist.stride(0) if ids.size > 1 else hist.shape[1]
             _lib.check(self._h, self._L.mww_write_audio_history(self._h, ids.ctypes.data, ids.size, hist.shape[1],
                                                                 hist.data_ptr() if hist.numel() else None, stride, self._cu_stream()))
+        if formats is not None and self.per_stream_rates:
+            self.set_stream_formats(ids, formats)
 
     # ------------------------------------------------------------------ pinned host buffers next to the GPU
     def host_buffer(self, shape, dtype=np.int16, write_combined: bool = False) -> np.ndarray:
@@ -692,9 +805,12 @@ class StreamEngine(_Engine):
     """`model`: path to (or bytes of) an MWW container or a streaming ``.tflite`` flatbuffer (recognised and converted by
     ``tflite_file``, inference.py:36-45), or None for a frontend-only engine."""
 
-    def __init__(self, model, n_streams: int = 1, device: int = 0, input_rate: int = 16000, stream_rates=None):
+    def __init__(self, model, n_streams: int = 1, device: int = 0, input_rate: int = 16000, stream_rates=None,
+                 stream_formats=None):
         if stream_rates is not None and input_rate != 16000:
             raise ValueError("give input_rate= or stream_rates=, not both")
+        if stream_formats is not None and stream_rates is None:
+            raise ValueError("stream_formats= needs stream_rates= (sample formats per stream need per-stream rates)")
         blob = load_model_blob(model)
         self._L = _lib.lib()
         self._h = ctypes.c_void_p()
@@ -715,6 +831,8 @@ class StreamEngine(_Engine):
             self.set_input_rate(input_rate)
         if stream_rates is not None:
             self.set_stream_rates(np.arange(self.n_streams, dtype=np.int32), stream_rates)
+        if stream_formats is not None:
+            self.set_stream_formats(np.arange(self.n_streams, dtype=np.int32), stream_formats)
 
     @property
     def pending_rows(self) -> int:
@@ -756,46 +874,47 @@ class StreamEngine(_Engine):
             raise ValueError("dst_ids and src_ids must have the same length")
         _lib.check(self._h, self._L.mww_copy_nn_state(self._h, d.ctypes.data, src._h, s.ctypes.data, d.size, self._cu_stream()))
 
-    def predict_clip(self, audio, out=None, samples16=None, law=None):
+    def predict_clip(self, audio, out=None, samples16=None, law=None, mixed=False):
         """int16 or float32 CUDA tensor [S, N] -> float32 probabilities [S, steps]; state carries over between calls.  float32
         samples are converted to int16 inside the frontend kernels (x * 32768, clipped, as audio_utils.to_int16).  With
         per-stream rates: samples16= (even), and N >= every stream's inputs_for(samples16).  G.711: uint8 codes with
-        law='ulaw' or 'alaw' (as features)."""
+        law='ulaw' or 'alaw' (as features).  mixed=True: uint8 rows in each stream's own format (as features)."""
         torch = _torch()
-        width, stride, _ = self._check_audio(audio, law)
-        n = self._call_len(width, samples16)
+        width, stride, _ = self._check_audio(audio, law, mixed)
+        n = self._mixed_len(width, max(stride, width), audio.data_ptr(), samples16) if mixed else self._call_len(width, samples16)
         stride = max(stride, width)
         steps = self._steps(n)
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
         got = ctypes.c_int(0)
-        fn = self._audio_fn("mww_predict_clip", _kind(audio.dtype), law)
+        fn = self._audio_fn("mww_predict_clip", _kind(audio.dtype), law, mixed)
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, stride, out.data_ptr(), out.shape[1], ctypes.byref(got), self._cu_stream()))
         return out[:, :got.value]
 
-    def step(self, audio, out=None, law=None):
+    def step(self, audio, out=None, law=None, mixed=False):
         """the live "one chunk of new audio per call" surface (north_star step()): predict_clip; with per-stream rates a
         30 ms call (samples16 = 480)"""
-        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None, law=law)
+        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None, law=law, mixed=mixed)
 
-    def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None, samples16=None, law=None) -> np.ndarray:
+    def predict_clip_host(self, audio: np.ndarray, out: np.ndarray | None = None, samples16=None, law=None, mixed=False) -> np.ndarray:
         """int16 or float32 HOST array [S, N] -> float32 HOST array [S, steps]; copies are pipelined inside the library.
         float32 samples cross PCIe as they are and are converted in the frontend kernels (as predict_clip converts them), and
-        so do uint8 G.711 codes with law='ulaw' or 'alaw' (one byte per sample).  Other dtypes (float64 included) and wrong
-        shapes: ValueError; a too-small `out`: MwwError."""
-        audio, stride, _ = self._check_host_audio(audio, law)
-        n = self._call_len(audio.shape[1], samples16)
+        so do uint8 G.711 codes with law='ulaw' or 'alaw' (one byte per sample), and with mixed=True uint8 rows in each
+        stream's own format.  Other dtypes (float64 included) and wrong shapes: ValueError; a too-small `out`: MwwError."""
+        audio, stride, _ = self._check_host_audio(audio, law, mixed)
+        n = self._mixed_len(audio.shape[1], stride, audio.ctypes.data, samples16) if mixed else self._call_len(audio.shape[1], samples16)
         steps = self._steps(n)
         if out is None:
             out = np.empty((self.n_streams, max(steps, 1)), np.float32)
         got = ctypes.c_int(0)
-        fn = self._audio_fn("mww_predict_clip_host", _kind(audio.dtype), law)
+        fn = self._audio_fn("mww_predict_clip_host", _kind(audio.dtype), law, mixed)
         _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, out.ctypes.data, out.shape[1], ctypes.byref(got)))
         return out[:, :got.value]
 
-    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None, dtype=np.int16,
-                            samples16=None, law=None):
-        """Audio [S, n_samples] of `dtype` (int16, float32, or uint8 G.711 codes with law='ulaw' or 'alaw'; stride in samples)
+    def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None, dtype=None,
+                            samples16=None, law=None, mixed=False):
+        """Audio [S, n_samples] of `dtype` (int16 by default, float32, or uint8 G.711 codes with law='ulaw' or 'alaw'; stride
+        in samples; with mixed=True uint8 rows of n_samples bytes in each stream's own format, stride in bytes)
         at address `src_ptr` -- device memory of a PEER
         GPU mapped into this process (sharding.IngestBuffer.block_ptr) or host memory (mww_predict_clip_remote[_f32]).
         tiles = 0: a peer-mapped (or local) buffer is read in place by the frontend kernel, over NVLink; host memory is staged
@@ -803,10 +922,10 @@ class StreamEngine(_Engine):
         CUDA probabilities [S, steps]; stream-ordered like predict_clip.  With per-stream rates n_samples is the samples each
         row holds (>= every inputs_for(samples16)) and samples16= the call."""
         torch = _torch()
-        fn = self._remote_fn(dtype, "mww_predict_clip_remote", law)
+        fn = self._remote_fn(dtype, "mww_predict_clip_remote", law, mixed)
         width = int(n_samples)
-        n = self._call_len(width, samples16)
         stride = int(stride) if stride else width
+        n = self._mixed_len(width, stride, int(src_ptr), samples16) if mixed else self._call_len(width, samples16)
         steps = self._steps(n)
         if out is None:
             out = torch.empty((self.n_streams, max(steps, 1)), dtype=torch.float32, device=self._dev())
@@ -859,9 +978,12 @@ class MultiModelEngine(_Engine):
     them only, and its results have one row per id, in that order (row j belongs to stream streams[k][j]).  Unsorted,
     duplicate or out-of-range ids raise ValueError.  `engine.streams[k]` is model k's set (int32), `set_streams` changes it."""
 
-    def __init__(self, models, n_streams: int = 1, device: int = 0, streams=None, input_rate: int = 16000, stream_rates=None):
+    def __init__(self, models, n_streams: int = 1, device: int = 0, streams=None, input_rate: int = 16000, stream_rates=None,
+                 stream_formats=None):
         if stream_rates is not None and input_rate != 16000:
             raise ValueError("give input_rate= or stream_rates=, not both")
+        if stream_formats is not None and stream_rates is None:
+            raise ValueError("stream_formats= needs stream_rates= (sample formats per stream need per-stream rates)")
         blobs = [load_model_blob(m) for m in models]
         if any(b is None for b in blobs):
             raise ValueError("every model must be a path or the bytes of a model file")
@@ -897,6 +1019,8 @@ class MultiModelEngine(_Engine):
             self.set_input_rate(input_rate)
         if stream_rates is not None:
             self.set_stream_rates(np.arange(self.n_streams, dtype=np.int32), stream_rates)
+        if stream_formats is not None:
+            self.set_stream_formats(np.arange(self.n_streams, dtype=np.int32), stream_formats)
 
     @staticmethod
     def _stream_set(ids, n_streams: int) -> np.ndarray:
@@ -961,37 +1085,37 @@ class MultiModelEngine(_Engine):
         maxp = (ctypes.c_int * K)(*[o.shape[1] for o in out])
         return out, ptrs, maxp, (ctypes.c_int * K)()
 
-    def predict_clip(self, audio, out=None, samples16=None, law=None) -> list:
+    def predict_clip(self, audio, out=None, samples16=None, law=None, mixed=False) -> list:
         """int16 or float32 CUDA tensor [S, N] -> [float32 probabilities [S, steps_k] for each model k]; state carries over
-        between calls.  `out`: one CUDA float32 buffer [S, >= steps_k] per model to write into.  samples16= and law=: as
-        StreamEngine.predict_clip."""
-        width, stride, _ = self._check_audio(audio, law)
-        n = self._call_len(width, samples16)
+        between calls.  `out`: one CUDA float32 buffer [S, >= steps_k] per model to write into.  samples16=, law= and
+        mixed=: as StreamEngine.predict_clip."""
+        width, stride, _ = self._check_audio(audio, law, mixed)
+        n = self._mixed_len(width, max(stride, width), audio.data_ptr(), samples16) if mixed else self._call_len(width, samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
-        fn = self._audio_fn("mww_predict_clip_multi", _kind(audio.dtype), law)
+        fn = self._audio_fn("mww_predict_clip_multi", _kind(audio.dtype), law, mixed)
         _lib.check(self._h, fn(self._h, audio.data_ptr(), n, max(stride, width), ptrs, maxp, got, self._cu_stream()))
         return [o[:, :g] for o, g in zip(out, got)]
 
-    def step(self, audio, out=None, law=None) -> list:
+    def step(self, audio, out=None, law=None, mixed=False) -> list:
         """predict_clip; with per-stream rates a 30 ms call (samples16 = 480)"""
-        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None, law=law)
+        return self.predict_clip(audio, out, LIVE_SAMPLES16 if self.per_stream_rates else None, law=law, mixed=mixed)
 
-    def predict_clip_host(self, audio: np.ndarray, out=None, samples16=None, law=None) -> list:
-        """int16 or float32 HOST array (uint8 with law=) [S, N] -> [float32 HOST array [S, steps_k] for each model k]; each
-        audio tile is copied once."""
-        audio, stride, _ = self._check_host_audio(audio, law)
-        n = self._call_len(audio.shape[1], samples16)
+    def predict_clip_host(self, audio: np.ndarray, out=None, samples16=None, law=None, mixed=False) -> list:
+        """int16 or float32 HOST array (uint8 with law= or mixed=True) [S, N] -> [float32 HOST array [S, steps_k] for each
+        model k]; each audio tile is copied once."""
+        audio, stride, _ = self._check_host_audio(audio, law, mixed)
+        n = self._mixed_len(audio.shape[1], stride, audio.ctypes.data, samples16) if mixed else self._call_len(audio.shape[1], samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, True)
-        fn = self._audio_fn("mww_predict_clip_host_multi", _kind(audio.dtype), law)
+        fn = self._audio_fn("mww_predict_clip_host_multi", _kind(audio.dtype), law, mixed)
         _lib.check(self._h, fn(self._h, audio.ctypes.data, n, stride, ptrs, maxp, got))
         return [o[:, :g] for o, g in zip(out, got)]
 
     def predict_clip_remote(self, src_ptr: int, n_samples: int, stride: int | None = None, tiles: int = 0, out=None,
-                            dtype=np.int16, samples16=None, law=None) -> list:
+                            dtype=None, samples16=None, law=None, mixed=False) -> list:
         """StreamEngine.predict_clip_remote for every model: one result per model, each audio tile pulled once."""
-        fn = self._remote_fn(dtype, "mww_predict_clip_remote_multi", law)
+        fn = self._remote_fn(dtype, "mww_predict_clip_remote_multi", law, mixed)
         width = int(n_samples)
-        n = self._call_len(width, samples16)
+        n = self._mixed_len(width, int(stride) if stride else width, int(src_ptr), samples16) if mixed else self._call_len(width, samples16)
         out, ptrs, maxp, got = self._outs(self._steps(n), out, False)
         _lib.check(self._h, fn(self._h, ctypes.c_void_p(int(src_ptr)), n, int(stride) if stride else width, ptrs, maxp, got, int(tiles),
                                self._cu_stream()))
