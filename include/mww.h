@@ -1375,7 +1375,7 @@ int mww_playback_check_detections_at(mww_playback_guard_t *g, mww_detector_t *de
  * event during the arm call.  A replay that reaches back over the wake word hears it as speech: the segment then starts
  * before the wake word, and a pause of silence_steps after it ends the command with END_OF_SPEECH before the command is
  * spoken.  Choose lookback_steps (the latency to cover) and silence_steps (longer than the pause a speaker makes after the
- * wake word) together.  disarm(ids) cancels without an event.  reset(ids) gives those rows fresh VAD and segmenter state:
+ * wake word) together, or arm at the detection's position instead ("positioned arm" below).  disarm(ids) cancels without an event.  reset(ids) gives those rows fresh VAD and segmenter state:
  * call it when the handle's streams are reset.  A whole reset (ids NULL) does that for every row, takes the handle's
  * counters as the new baseline and forgets the steps consumed and their positions, so no replay reaches across it (the
  * axis may have restarted: mww_set_audio_history sets samples_seen back to 0).
@@ -1469,7 +1469,8 @@ int mww_endpointer_read_commands(mww_endpointer_t *ep, mww_t *h, long long pre, 
  *   - Ids.  Both calls take GLOBAL stream ids of the endpointer's handle from host memory, as arm and reset do.  ids[i] on
  *     import may differ from the id record i was exported from, so streams can be renumbered.
  *   - One record, record_bytes long, every part padded to 16 bytes:
- *         int32   member, armed, 0, 0                   member of the stream set; armed (the segmenter state follows)
+ *         int32   member, armed, mute, 0                member of the stream set; armed (the segmenter state follows);
+ *                                                       the row's mute word from a positioned exporter, else 0
  *         int32   elapsed, run, silence, heard          zero unless armed
  *         int64   seen; uint64 flags                    VAD count and the last 64 speech flags
  *         int64   start_age, speech_end_age             S' - start_sample, S' - speech_end_sample; zero unless armed
@@ -1477,7 +1478,8 @@ int mww_endpointer_read_commands(mww_endpointer_t *ep, mww_t *h, long long pre, 
  *     with S' the exporter's baseline samples_seen (its handle's counter at the endpointer's last update or whole reset).  A
  *     rule of vad_window 5 has 80-byte records: 16 + 16 + 16 + 16 + 16 (4 floats).
  *   - mww_endpointer_layout: record_bytes, vad_window, stride, hop_samples and the baseline buffered and pending rows that
- *     import checks, and the exporter's baseline samples_seen and steps, for information.  mww_get_endpointer_layout fills
+ *     import checks, and the exporter's baseline samples_seen and steps, for information.  pad is 1 when the exporter is
+ *     positioned (its records carry mute words) and 0 otherwise; import refuses any other value.  mww_get_endpointer_layout fills
  *     it without device work; export fills it too (out may be NULL).
  *   - export writes one record per listed id (an id may appear twice): an id that is not a member of the model's stream set
  *     gets a zero record (member = 0), an unarmed row a zero segmenter.  The endpointer does not change.
@@ -1514,6 +1516,61 @@ int mww_export_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n
                                void *cu_stream);
 int mww_import_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n, const void *d_records,
                                const mww_endpointer_layout *layout, void *cu_stream);
+
+/* ---- positioned arm: the command starts at the detection, after the wake word ----------------------------------------------
+ * arm replays the row's last lookback_steps flags, which reach back over the wake word: the VAD hears it as speech, so the
+ * command's clip holds the wake word, and a pause after it longer than silence_steps ends the command before it is spoken.
+ * A timed detector knows where the wake word ended (its event positions, "event positions"), on the axis the endpointer's
+ * steps use.  arm_at starts the command there.
+ *
+ * Rule.  arm_at(ids, positions, skip), for each listed id whose row r is a member; P is the id's position and skip >= 0 is in
+ * samples.
+ *   - Newest position.  q = S' - b' - hop g', from the endpointer's baseline (S' samples_seen, b' = buffered' - (480 - hop),
+ *     g' the model's pending rows): the position of the newest step consumed, or, with no step since a whole reset, where it
+ *     would have been.  Future steps fall at q + k stride hop, k >= 1.  P' = min(P, q): a position in the future counts as now.
+ *   - Fresh segment.  The row gets fresh segmenter state with start_sample = speech_end_sample = P'.  The plain rule's "the
+ *     first step sets start_sample" does not apply to it.
+ *   - Replay.  Of arm's replay steps (L = min(lookback_steps, steps consumed)), those at p > P' run, oldest first, each with
+ *     flag f' = f && p > P' + skip.  The stored flags do not change.  elapsed counts the steps replayed only: steps after P'
+ *     older than the replay are not counted.  A replay that reaches an end emits its event during the call, as arm's does.
+ *   - Mute.  The row keeps mute = max(0, floor((P' + skip - q) / (stride hop))): the future steps that still fall within the
+ *     skip.  While the row is armed, each update step with mute > 0 takes f' = 0, then mute -= 1.
+ *   - Clearing.  Every call that gives a row fresh segmenter state sets its mute to 0: arm, disarm, reset, an end, and an
+ *     import of a record without a mute.
+ *   - Repeated ids.  An id listed twice in one call arms once, at the latest P (equal positions give equal results): a
+ *     detector may hold two slots for one stream, two fires between polls or two wake words of a models detector.
+ *   - Ids.  Host ids outside [0, n_streams) are MWW_EINVAL.  Device ids that are -1, out of range or not members are ignored,
+ *     as arm_device ignores them, so a verifier's d_confirmed, a guard's d_passed or a detector's d_fired go in slot for slot
+ *     with the detector's d_positions (mww_get_detector_positions).
+ *   - Properties.  (1) With P = (the oldest replayed position - stride hop) and skip = 0, arm_at is arm, bit for bit.  (2)
+ *     Results do not depend on when arm_at is called, as long as P <= q and the replay still reaches P (its oldest step is at
+ *     most P + stride hop).  (3) With every mute at 0, the positioned forms below give exactly what the plain ones give.
+ *   - Command read, unchanged: a = start_sample - pre.  With pre = 0 the clip starts at the detection and leaves the wake word
+ *     out; pre > 0 takes it back in.
+ *
+ * The mute word.  mww_endpointer_get_mutes / _set_mutes read and write every row's int32 mute word, [n_rows], synchronously,
+ * beside get_state / set_state for checkpoints.  Bits 0 .. 29 hold the mute count (at most 2^22); bit 30 (placed) is set
+ * while a row that arm_at armed with no step replayed has taken no step since: its start_sample is fixed, and its first step
+ * leaves it.  The first step clears the bit.  set refuses a negative word or a count above 2^22.
+ *
+ * Mode.  An endpointer runs the plain kernels (libmww_endpoint.so, libmww_serving_records.so) and issues exactly the launches
+ * it issued before this section existed, until its first arm_at, set_mutes or import of records whose layout has pad = 1.
+ * From then on, for good, update, arm, disarm, reset, export and import run the positioned forms (libmww_endpoint_at.so),
+ * one launch each as before; arm_at is two launches whatever n is, a reduction of each row's latest position and the arm.
+ * A positioned exporter writes each armed row's mute word into its record head's third word and sets the layout's pad to 1;
+ * a plain endpointer's records are byte for byte what they were.  Importing records of either kind into a positioned
+ * endpointer takes the word (0 from plain records); importing positioned records into a plain endpointer makes it positioned,
+ * so a mute is never dropped.
+ *
+ * Calls.  Asynchronous on cu_stream, no allocation: the mute words, the reduction's keys and the staging of a host list are
+ * allocated at create.  A host list is copied into buffers the endpointer owns, so calls on one endpointer from different
+ * CUDA streams must be ordered by the caller.  Refusals, MWW_EINVAL before any device work: a NULL endpointer, n < 0, NULL
+ * ids or positions with n > 0, skip_samples outside [0, 2^22], and a host id out of range. */
+int mww_endpointer_arm_at(mww_endpointer_t *ep, const int32_t *h_ids, const int64_t *h_positions, int n, long long skip_samples, void *cu_stream);
+int mww_endpointer_arm_at_device(mww_endpointer_t *ep, const int32_t *d_ids, const int64_t *d_positions, int n, long long skip_samples,
+                                 void *cu_stream);
+int mww_endpointer_get_mutes(mww_endpointer_t *ep, int32_t *h_mutes);
+int mww_endpointer_set_mutes(mww_endpointer_t *ep, const int32_t *h_mutes);
 
 #ifdef __cplusplus
 }

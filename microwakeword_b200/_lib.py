@@ -63,6 +63,7 @@ EXPORTS = (
     "mww_playback_guard_create", "mww_playback_guard_destroy", "mww_playback_guard_info", "mww_playback_write", "mww_playback_read",
     "mww_playback_reset", "mww_playback_get_heads", "mww_playback_check_streams", "mww_playback_check_detections_at",
     "mww_arbitrate_detector_groups", "mww_drain_detector_arbitrated", "mww_get_detector_group_levels", "mww_set_detector_group_levels",
+    "mww_endpointer_arm_at", "mww_endpointer_arm_at_device", "mww_endpointer_get_mutes", "mww_endpointer_set_mutes",
 )
 
 
@@ -436,6 +437,12 @@ def lib() -> ctypes.CDLL:
     for name in ("mww_export_endpointer_rows", "mww_import_endpointer_rows"):
         getattr(L, name).restype = i32
         getattr(L, name).argtypes = [vp, vp, i32, vp, ctypes.POINTER(MwwEndpointerLayout), vp]
+    for name in ("mww_endpointer_arm_at", "mww_endpointer_arm_at_device"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp, vp, i32, ll, vp]
+    for name in ("mww_endpointer_get_mutes", "mww_endpointer_set_mutes"):
+        getattr(L, name).restype = i32
+        getattr(L, name).argtypes = [vp, vp]
     L.mww_time_detector_events.restype = i32
     L.mww_time_detector_events.argtypes = [vp]
     L.mww_update_detector_at.restype = i32

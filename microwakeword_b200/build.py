@@ -78,6 +78,10 @@ FC_SOURCES = ["mww_frontend_clip.cu"]
 # so that libmww_resample_rates.so and libmww_g711.so keep exactly the kernels they had
 RM_OUT = os.path.join(HERE, "libmww_resample_mixed.so")
 RM_SOURCES = ["mww_resample_mixed.cu"]
+# and the positioned endpointer's kernels (mww_endpointer_arm_at and the forms that keep each row's mute word), so that
+# libmww_endpoint.so and libmww_serving_records.so keep exactly the kernels they had
+EPA_OUT = os.path.join(HERE, "libmww_endpoint_at.so")
+EPA_SOURCES = ["mww_endpoint_at.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
          "-Xcompiler", "-fPIC", "-cudart", "static"]
@@ -100,7 +104,7 @@ def source_hash() -> str:
 
 
 def _stale() -> bool:
-    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, EVP_OUT, GRP_OUT, MG_OUT, PB_OUT, ARB_OUT, FC_OUT, RM_OUT, STAMP)):
+    if not all(os.path.exists(p) for p in (OUT, RS_OUT, RR_OUT, DET_OUT, MD_OUT, DC_OUT, G711_OUT, HIST_OUT, DR_OUT, VER_OUT, EP_OUT, SR_OUT, EVP_OUT, GRP_OUT, MG_OUT, PB_OUT, ARB_OUT, FC_OUT, RM_OUT, EPA_OUT, STAMP)):
         return True
     try:
         return open(STAMP).read().strip() != source_hash()
@@ -124,11 +128,12 @@ def build(force: bool = False, verbose: bool = False) -> str:
                                     (EP_OUT, EP_SOURCES, []), (SR_OUT, SR_SOURCES, []), (EVP_OUT, EVP_SOURCES, []),
                                     (GRP_OUT, GRP_SOURCES, []), (MG_OUT, MG_SOURCES, []), (PB_OUT, PB_SOURCES, []),
                                     (ARB_OUT, ARB_SOURCES, []), (FC_OUT, FC_SOURCES, []), (RM_OUT, RM_SOURCES, []),
+                                    (EPA_OUT, EPA_SOURCES, []),
                                     (OUT, SOURCES, ["-L" + HERE, "-lmww_resample", "-lmww_resample_rates", "-lmww_detector",
                                                     "-lmww_detector_models", "-lmww_detector_cutoffs", "-lmww_g711", "-lmww_history",
                                                     "-lmww_detector_records", "-lmww_verify", "-lmww_endpoint", "-lmww_serving_records",
                                                     "-lmww_event_positions", "-lmww_detector_groups", "-lmww_media_guard", "-lmww_playback",
-                                                    "-lmww_group_arbitration", "-lmww_frontend_clip", "-lmww_resample_mixed",
+                                                    "-lmww_group_arbitration", "-lmww_frontend_clip", "-lmww_resample_mixed", "-lmww_endpoint_at",
                                                     "-Xlinker", "-rpath,$ORIGIN"])):
             tmp = out + ".tmp.%d" % os.getpid()
             cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + [os.path.join(CSRC, s) for s in sources] + extra

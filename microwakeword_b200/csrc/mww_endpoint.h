@@ -107,10 +107,9 @@ struct EndpointSeg {
 };
 MWW_HD EndpointSeg endpoint_fresh_seg() { return EndpointSeg{0, 0, 0, 0, 0, 0}; }
 
-// one step with flag f at position p; the first step after arming places start_sample.  -> the end reason, 0 while the row
-// goes on.  Ties on one step go to the first condition that holds.
-MWW_HD int endpoint_segment(const mww_endpoint_rule &r, long long step_samples, EndpointSeg &g, bool f, long long p) {
-    if (g.elapsed == 0) g.start = g.speech_end = p - step_samples;
+// one step with flag f at position p, start_sample already placed.  -> the end reason, 0 while the row goes on.  Ties on one
+// step go to the first condition that holds.
+MWW_HD int endpoint_segment_step(const mww_endpoint_rule &r, EndpointSeg &g, bool f, long long p) {
     g.elapsed += 1;
     if (f) {
         g.run += 1;
@@ -125,6 +124,11 @@ MWW_HD int endpoint_segment(const mww_endpoint_rule &r, long long step_samples, 
     if (!g.heard && g.elapsed >= r.timeout_steps) return MWW_ENDPOINT_NO_SPEECH;
     if (g.elapsed >= r.max_steps) return MWW_ENDPOINT_MAX_LENGTH;
     return 0;
+}
+// one step with flag f at position p; the first step after arming places start_sample
+MWW_HD int endpoint_segment(const mww_endpoint_rule &r, long long step_samples, EndpointSeg &g, bool f, long long p) {
+    if (g.elapsed == 0) g.start = g.speech_end = p - step_samples;
+    return endpoint_segment_step(r, g, f, p);
 }
 
 MWW_HD EndpointSeg endpoint_load_seg(const EndpointArgs &a, int r) {
@@ -147,9 +151,17 @@ MWW_HD void endpoint_emit(const EndpointArgs &a, int32_t id, int reason, const E
 }
 
 // ---- the four kernels' bodies ---------------------------------------------------------------------------------------------------
+// The positioned forms (kAt, libmww_endpoint_at.so; include/mww.h, "positioned arm") also keep each row's mute word,
+// mute[r]: the low bits count the update steps that still take flag 0, and kEndpointPlaced marks a row whose start_sample
+// an arm_at fixed and which has taken no step since.  Every form that gives a row fresh segmenter state sets the word to 0.
+// The plain forms (kAt = false) neither read nor write it.
+constexpr int32_t kEndpointPlaced = 1 << 30;
+constexpr int32_t kEndpointMuteSteps = kEndpointPlaced - 1;
+
 // update, row r: n steps of probs[r * pitch + j], step j at position pos0 + j * step_samples, in order.  Every row takes the
 // flag; an armed row then runs the segmenter, and disarms when it ends.  A row that is not armed keeps fresh segmenter state.
-MWW_HD void endpoint_update_row(const EndpointArgs &a, int r, const float *probs, long long pitch, int n, long long pos0) {
+template <bool kAt>
+MWW_HD void endpoint_update_row_t(const EndpointArgs &a, int32_t *mute, int r, const float *probs, long long pitch, int n, long long pos0) {
     const EndpointHist hist{a.hist, a.n_rows, r};
     const int w = a.rule.vad_window;
     long long seen = a.seen[r];
@@ -157,6 +169,8 @@ MWW_HD void endpoint_update_row(const EndpointArgs &a, int r, const float *probs
     int32_t id = a.armed[r];
     const bool was_armed = id >= 0;
     EndpointSeg g = was_armed ? endpoint_load_seg(a, r) : endpoint_fresh_seg();
+    int32_t m = 0;
+    if constexpr (kAt) m = was_armed ? mute[r] : 0;
     const float *row = probs + (long long)r * pitch;
     for (int j = 0; j < n; ++j) {
         const bool f = endpoint_speech(hist, w, a.rule.vad_cutoff, seen, row[j]);
@@ -164,10 +178,21 @@ MWW_HD void endpoint_update_row(const EndpointArgs &a, int r, const float *probs
         flags = flags << 1 | (f ? 1ull : 0ull);
         if (id < 0) continue;
         const long long p = pos0 + (long long)j * a.step_samples;
-        if (const int reason = endpoint_segment(a.rule, a.step_samples, g, f, p)) {
+        int reason;
+        if constexpr (kAt) {
+            // a muted step takes flag 0 (the stored flag keeps f); a placed row's first step leaves start_sample where it is
+            const bool muted = (m & kEndpointMuteSteps) != 0;
+            const bool placed = (m & kEndpointPlaced) != 0;
+            m = (m & kEndpointMuteSteps) - (muted ? 1 : 0);
+            reason = placed ? endpoint_segment_step(a.rule, g, f && !muted, p) : endpoint_segment(a.rule, a.step_samples, g, f && !muted, p);
+        } else {
+            reason = endpoint_segment(a.rule, a.step_samples, g, f, p);
+        }
+        if (reason) {
             endpoint_emit(a, id, reason, g, p);
             id = -1;
             g = endpoint_fresh_seg();
+            m = 0;
         }
     }
     a.seen[r] = seen;
@@ -175,12 +200,17 @@ MWW_HD void endpoint_update_row(const EndpointArgs &a, int r, const float *probs
     if (was_armed) {
         a.armed[r] = id;
         endpoint_store_seg(a, r, g);
+        if constexpr (kAt) mute[r] = m;
     }
+}
+MWW_HD void endpoint_update_row(const EndpointArgs &a, int r, const float *probs, long long pitch, int n, long long pos0) {
+    endpoint_update_row_t<false>(a, nullptr, r, probs, pitch, n, pos0);
 }
 
 // arm, one listed global id: a member row not yet taken by this call gets fresh segmenter state and replays its last
 // R.steps flags, oldest first, at their positions.  Ids outside the set (-1 included) are ignored.
-MWW_HD void endpoint_arm_one(const EndpointArgs &a, const EndpointReplay &R, int32_t id) {
+template <bool kAt>
+MWW_HD void endpoint_arm_one_t(const EndpointArgs &a, int32_t *mute, const EndpointReplay &R, int32_t id) {
     if (id < 0 || id >= a.n_streams) return;
     const int r = a.row_of[id];
     if (r < 0 || endpoint_take(&a.arm_tag[r], R.tag) == R.tag) return;
@@ -198,20 +228,85 @@ MWW_HD void endpoint_arm_one(const EndpointArgs &a, const EndpointReplay &R, int
     }
     a.armed[r] = armed;
     endpoint_store_seg(a, r, g);
+    if constexpr (kAt) mute[r] = 0;
 }
+MWW_HD void endpoint_arm_one(const EndpointArgs &a, const EndpointReplay &R, int32_t id) { endpoint_arm_one_t<false>(a, nullptr, R, id); }
 
 // disarm (reset = 0) or reset (reset = 1) of row r: disarming drops the segment without an event; a reset also gives fresh
 // VAD state (zero history, seen 0, every flag 0)
-MWW_HD void endpoint_clear_row(const EndpointArgs &a, int r, int reset) {
+template <bool kAt>
+MWW_HD void endpoint_clear_row_t(const EndpointArgs &a, int32_t *mute, int r, int reset) {
     a.armed[r] = -1;
     endpoint_store_seg(a, r, endpoint_fresh_seg());
+    if constexpr (kAt) mute[r] = 0;
     if (!reset) return;
     for (int j = 0; j < a.rule.vad_window - 1; ++j) a.hist[(long long)j * a.n_rows + r] = 0.0f;
     a.seen[r] = 0;
     a.flags[r] = 0;
 }
+MWW_HD void endpoint_clear_row(const EndpointArgs &a, int r, int reset) { endpoint_clear_row_t<false>(a, nullptr, r, reset); }
 // the row of a listed global id, -1 for an id outside the set
 MWW_HD int endpoint_row(const EndpointArgs &a, int32_t id) { return id >= 0 && id < a.n_streams ? a.row_of[id] : -1; }
+
+// ---- positioned arm (mww_endpointer_arm_at): two launches, a reduction of each row's latest position, then the arm --------------
+// what both passes take beside EndpointArgs: the replay of arm, q (the position of the newest step consumed: endpoint_position
+// of the baseline with n = 1), the skip in samples, the rows' mute words and the reduction's keys
+struct EndpointAt {
+    EndpointReplay R;
+    long long q, skip;
+    int32_t *mute;
+    unsigned long long *key;               // [n_rows] the latest P' of the call as an ordered key; 0 (none) between calls
+};
+// a position as an unsigned key in the same order, 0 for the smallest
+MWW_HD unsigned long long endpoint_at_key(long long P) { return (unsigned long long)P ^ 0x8000000000000000ull; }
+MWW_HD long long endpoint_at_clamp(long long P, long long q) { return P < q ? P : q; }
+
+// pass 1, one listed (id, P): the row's key becomes the largest P' = min(P, q) listed for it
+MWW_HD void endpoint_at_reduce_one(const EndpointArgs &a, const EndpointAt &A, int32_t id, long long P) {
+    const int r = endpoint_row(a, id);
+    if (r < 0) return;
+    const unsigned long long k = endpoint_at_key(endpoint_at_clamp(P, A.q));
+#if defined(__CUDA_ARCH__)
+    atomicMax(&A.key[r], k);
+#else
+    if (k > A.key[r]) A.key[r] = k;
+#endif
+}
+
+// pass 2, one listed (id, P): the slot whose P' is the row's latest takes the row (one take per call; equal positions arm
+// alike) and puts its key back to 0.  The row gets fresh segmenter state with start_sample = speech_end_sample = P', replays the
+// steps of R after P', each with flag f && p > P' + skip, and keeps the mute word of the steps still within the skip.  A slot
+// that reads the key after the taker cleared it reads 0, the key of no position a later slot could still take with.
+MWW_HD void endpoint_arm_at_one(const EndpointArgs &a, const EndpointAt &A, int32_t id, long long P) {
+    const int r = endpoint_row(a, id);
+    if (r < 0) return;
+    const long long Pc = endpoint_at_clamp(P, A.q);
+    if (endpoint_at_key(Pc) != A.key[r] || endpoint_take(&a.arm_tag[r], A.R.tag) == A.R.tag) return;
+    A.key[r] = 0;
+    EndpointSeg g = endpoint_fresh_seg();
+    g.start = g.speech_end = Pc;
+    const unsigned long long flags = a.flags[r];
+    int32_t armed = id;
+    for (int i = A.R.steps - 1; i >= 0; --i) {
+        const long long p = A.R.pos[i];
+        if (p <= Pc) continue;
+        if (const int reason = endpoint_segment_step(a.rule, g, ((flags >> i) & 1ull) && p > Pc + A.skip, p)) {
+            endpoint_emit(a, id, reason, g, p);
+            armed = -1;
+            g = endpoint_fresh_seg();
+            break;
+        }
+    }
+    int32_t m = 0;
+    if (armed >= 0) {
+        const long long d = Pc + A.skip - A.q;                  // future steps q + k stride hop with k >= 1 that are <= P' + skip
+        m = d > 0 ? (int32_t)(d / a.step_samples) : 0;
+        if (g.elapsed == 0) m |= kEndpointPlaced;
+    }
+    a.armed[r] = armed;
+    endpoint_store_seg(a, r, g);
+    A.mute[r] = m;
+}
 
 // ---- command read ---------------------------------------------------------------------------------------------------------------
 // event slot i's samples [a, a + len) on the history axis: a = start - pre; the end is min(speech_end + post, end) for

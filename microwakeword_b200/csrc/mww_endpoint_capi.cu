@@ -27,6 +27,13 @@ struct mww_endpointer {
     long long base_seen = 0, steps = 0;
     int base_buffered = 0, base_pending = 0;
     long long pos[kEndpointMaxLookback] = {};   // pos[i]: the step i steps before the newest
+    // the positioned forms (include/mww.h, "positioned arm"): each row's mute word, the reduction keys of arm_at and the
+    // staging buffer of a host position list, all [n_rows]; positioned switches on for good at the first arm_at, set_mutes or
+    // import of positioned records, and selects the kernels of libmww_endpoint_at.so from then on
+    int32_t *d_mute = nullptr;
+    unsigned long long *d_at_key = nullptr;
+    long long *d_positions = nullptr;
+    bool positioned = false;
 };
 
 namespace {
@@ -40,6 +47,7 @@ void endpointer_free(mww_endpointer_t *ep) {
     cudaFree(a.hist); cudaFree(a.seen); cudaFree(a.flags); cudaFree(a.armed); cudaFree(a.elapsed); cudaFree(a.run); cudaFree(a.silence);
     cudaFree(a.heard); cudaFree(a.start); cudaFree(a.speech_end); cudaFree(a.arm_tag); cudaFree((void *)a.row_of); cudaFree(a.count);
     cudaFree(a.events); cudaFree(a.ended); cudaFree(ep->d_ids); cudaFree(ep->d_rec_ids);
+    cudaFree(ep->d_mute); cudaFree(ep->d_at_key); cudaFree(ep->d_positions);
     delete ep;
 }
 
@@ -71,6 +79,9 @@ int endpointer_alloc(mww_endpointer_t *ep) {
     ECU(alloc_fill(&a.events, (size_t)a.capacity, 0));
     ECU(alloc_fill(&a.ended, (size_t)a.capacity, 0xFF));
     ECU(alloc_fill(&ep->d_ids, R, 0));
+    ECU(alloc_fill(&ep->d_mute, R, 0));
+    ECU(alloc_fill(&ep->d_at_key, R, 0));
+    ECU(alloc_fill(&ep->d_positions, R, 0));
     ECU(cudaDeviceSynchronize());
     return MWW_OK;
 }
@@ -115,15 +126,43 @@ EndpointReplay replay_of(mww_endpointer_t *ep) {
 int arm(mww_endpointer_t *ep, const int32_t *d_ids, int n, cudaStream_t st) {
     DeviceGuard guard(ep->device);
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
-    ECU(launch_endpoint_arm(ep->a, replay_of(ep), d_ids, n, st));
+    if (ep->positioned) ECU(launch_endpoint_arm_muted(ep->a, replay_of(ep), ep->d_mute, d_ids, n, st));
+    else ECU(launch_endpoint_arm(ep->a, replay_of(ep), d_ids, n, st));
     ep->launches += 1;
+    return MWW_OK;
+}
+
+// the position of the newest step consumed (or of where it would have been, with none since a whole reset)
+long long newest_position(const mww_endpointer_t *ep) {
+    return endpoint_position(ep->base_seen, ep->base_buffered, ep->hop, ep->base_pending, ep->stride, 1, 0);
+}
+
+// arm_at: two launches, the reduction of each row's latest position and the arm; the endpointer is positioned from here on
+int arm_at(mww_endpointer_t *ep, const int32_t *d_ids, const long long *d_positions, int n, long long skip, cudaStream_t st) {
+    DeviceGuard guard(ep->device);
+    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+    ep->positioned = true;
+    EndpointAt A{};
+    A.R = replay_of(ep);
+    A.q = newest_position(ep);
+    A.skip = skip;
+    A.mute = ep->d_mute;
+    A.key = ep->d_at_key;
+    ECU(launch_endpoint_arm_at(ep->a, A, d_ids, d_positions, n, st));
+    ep->launches += 2;
+    return MWW_OK;
+}
+
+int check_skip(const std::string &call, long long skip) {
+    if (skip < 0 || skip > kHistoryMaxCapacity) return refuse(call + ": skip_samples must be in [0, 2^22]");
     return MWW_OK;
 }
 
 int clear(mww_endpointer_t *ep, const int32_t *d_ids, int n, int reset, cudaStream_t st) {
     DeviceGuard guard(ep->device);
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
-    ECU(launch_endpoint_clear(ep->a, d_ids, n, reset, st));
+    if (ep->positioned) ECU(launch_endpoint_clear_muted(ep->a, ep->d_mute, d_ids, n, reset, st));
+    else ECU(launch_endpoint_clear(ep->a, d_ids, n, reset, st));
     ep->launches += 1;
     return MWW_OK;
 }
@@ -135,6 +174,7 @@ void fill_layout(const mww_endpointer_t *ep, mww_endpointer_layout *out) {
     out->vad_window = ep->a.rule.vad_window; out->stride = ep->stride; out->hop_samples = ep->hop;
     out->buffered = ep->base_buffered; out->pending = ep->base_pending;
     out->samples_seen = ep->base_seen; out->steps = ep->steps;
+    out->pad = ep->positioned ? 1 : 0;
 }
 
 // the checks export and import share, before any device work: arguments, ids in range (and, on import, listed once) and an
@@ -255,7 +295,8 @@ int mww_endpointer_update(mww_endpointer_t *ep, const float *d_probs, int n, lon
     DeviceGuard guard(ep->device);
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
     const long long pos0 = endpoint_position(S, buffered, ep->hop, pending, ep->stride, n, 0);
-    ECU(launch_endpoint_update(ep->a, d_probs, pitch, n, pos0, static_cast<cudaStream_t>(cu_stream)));
+    if (ep->positioned) ECU(launch_endpoint_update_muted(ep->a, ep->d_mute, d_probs, pitch, n, pos0, static_cast<cudaStream_t>(cu_stream)));
+    else ECU(launch_endpoint_update(ep->a, d_probs, pitch, n, pos0, static_cast<cudaStream_t>(cu_stream)));
     ep->launches += 1;
     ep->base_seen = S; ep->base_buffered = buffered; ep->base_pending = pending;
     const int keep = std::min(n, kEndpointMaxLookback);
@@ -405,6 +446,64 @@ int mww_endpointer_set_state(mww_endpointer_t *ep, const mww_endpoint_state *in)
     return MWW_OK;
 }
 
+int mww_endpointer_arm_at(mww_endpointer_t *ep, const int32_t *h_ids, const int64_t *h_positions, int n, long long skip_samples, void *cu_stream) {
+    const std::string call = "mww_endpointer_arm_at";
+    if (!ep) return refuse(call + ": endpointer is NULL");
+    if (n < 0 || (n > 0 && (!h_ids || !h_positions))) return refuse(call + ": needs n >= 0, and ids and positions with n > 0");
+    if (int rc = check_skip(call, skip_samples)) return rc;
+    // the list filtered to members, each row once at its latest position, staged in d_ids / d_positions
+    std::vector<int32_t> ids;
+    std::vector<long long> pos;
+    std::vector<int> slot(ep->members.size(), -1);
+    for (int i = 0; i < n; ++i) {
+        if (h_ids[i] < 0 || h_ids[i] >= ep->n_streams)
+            return refuse(call + ": stream id " + std::to_string(h_ids[i]) + " out of range [0, " + std::to_string(ep->n_streams) + ")");
+        const int r = ep->row_of[h_ids[i]];
+        if (r < 0) continue;
+        if (slot[r] < 0) { slot[r] = (int)ids.size(); ids.push_back(h_ids[i]); pos.push_back(h_positions[i]); }
+        else pos[slot[r]] = std::max<long long>(pos[slot[r]], h_positions[i]);
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
+    DeviceGuard guard(ep->device);
+    if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
+    // from pageable memory, as stage_ids: the copies have taken the bytes when cudaMemcpyAsync returns
+    if (!ids.empty()) {
+        ECU(cudaMemcpyAsync(ep->d_ids, ids.data(), ids.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        ECU(cudaMemcpyAsync(ep->d_positions, pos.data(), pos.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+    }
+    return arm_at(ep, ep->d_ids, ep->d_positions, (int)ids.size(), skip_samples, st);
+}
+
+int mww_endpointer_arm_at_device(mww_endpointer_t *ep, const int32_t *d_ids, const int64_t *d_positions, int n, long long skip_samples,
+                                 void *cu_stream) {
+    const std::string call = "mww_endpointer_arm_at_device";
+    if (!ep) return refuse(call + ": endpointer is NULL");
+    if (n < 0 || (n > 0 && (!d_ids || !d_positions))) return refuse(call + ": needs n >= 0, and ids and positions with n > 0");
+    if (int rc = check_skip(call, skip_samples)) return rc;
+    return arm_at(ep, d_ids, reinterpret_cast<const long long *>(d_positions), n, skip_samples, static_cast<cudaStream_t>(cu_stream));
+}
+
+int mww_endpointer_get_mutes(mww_endpointer_t *ep, int32_t *h_mutes) {
+    if (!ep || (!h_mutes && ep->a.n_rows > 0)) return refuse("mww_endpointer_get_mutes: needs an endpointer and a buffer");
+    DeviceGuard guard(ep->device);
+    ECU(cudaDeviceSynchronize());
+    if (ep->a.n_rows > 0) ECU(cudaMemcpy(h_mutes, ep->d_mute, (size_t)ep->a.n_rows * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return MWW_OK;
+}
+
+int mww_endpointer_set_mutes(mww_endpointer_t *ep, const int32_t *h_mutes) {
+    const std::string call = "mww_endpointer_set_mutes: ";
+    if (!ep || (!h_mutes && ep->a.n_rows > 0)) return refuse(call + "needs an endpointer and the mute words");
+    for (int r = 0; r < ep->a.n_rows; ++r)
+        if (h_mutes[r] < 0 || (h_mutes[r] & kEndpointMuteSteps) > kHistoryMaxCapacity)
+            return refuse(call + "a mute word holds a count in [0, 2^22] and the placed bit 2^30");
+    DeviceGuard guard(ep->device);
+    ECU(cudaDeviceSynchronize());
+    if (ep->a.n_rows > 0) ECU(cudaMemcpy(ep->d_mute, h_mutes, (size_t)ep->a.n_rows * sizeof(int32_t), cudaMemcpyHostToDevice));
+    ep->positioned = true;
+    return MWW_OK;
+}
+
 int mww_endpointer_read_commands(mww_endpointer_t *ep, mww_t *h, long long pre, long long post, int max_samples, int16_t *d_out,
                                  long long out_stride, int32_t *d_lengths, void *cu_stream) {
     const std::string call = "mww_endpointer_read_commands: ";
@@ -441,7 +540,8 @@ int mww_export_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
     if (int rc = stage_record_ids(ep, h_ids, n, st)) return rc;
-    ECU(launch_pack_endpointer_rows(record_job(ep), d_records, ep->d_rec_ids, n, st));
+    if (ep->positioned) ECU(launch_pack_endpointer_rows_muted(record_job(ep), ep->d_mute, d_records, ep->d_rec_ids, n, st));
+    else ECU(launch_pack_endpointer_rows(record_job(ep), d_records, ep->d_rec_ids, n, st));
     ep->launches += 1;
     return MWW_OK;
 }
@@ -456,12 +556,15 @@ int mww_import_endpointer_rows(mww_endpointer_t *ep, const int32_t *h_ids, int n
     fill_layout(ep, &mine);
     if (const char *field = endpoint_layout_mismatch(*layout, mine))
         return refuse(call + "the records' " + field + " differs from the endpointer's");
+    if (layout->pad != 0 && layout->pad != 1) return refuse(call + "the layout's pad (the positioned flag) must be 0 or 1");
+    if (layout->pad == 1) ep->positioned = true;          // the records carry mute words: keep them
     if (n == 0) return MWW_OK;
     DeviceGuard guard(ep->device);
     if (guard.err != cudaSuccess) return cuda_fail(nullptr, guard.err, "cudaSetDevice");
     cudaStream_t st = static_cast<cudaStream_t>(cu_stream);
     if (int rc = stage_record_ids(ep, h_ids, n, st)) return rc;
-    ECU(launch_unpack_endpointer_rows(record_job(ep), d_records, ep->d_rec_ids, n, st));
+    if (ep->positioned) ECU(launch_unpack_endpointer_rows_muted(record_job(ep), ep->d_mute, d_records, ep->d_rec_ids, n, st));
+    else ECU(launch_unpack_endpointer_rows(record_job(ep), d_records, ep->d_rec_ids, n, st));
     ep->launches += 1;
     return MWW_OK;
 }

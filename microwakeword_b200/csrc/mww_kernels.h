@@ -234,6 +234,19 @@ cudaError_t launch_history_write(int16_t *ring, int C, long long seen, const int
 // the records [n][J.L.record_bytes] of the n listed global ids (device memory, in range) out of and into the endpointer J
 cudaError_t launch_pack_endpointer_rows(const EpRecJob &J, void *records, const int32_t *ids, int n, cudaStream_t st);
 cudaError_t launch_unpack_endpointer_rows(const EpRecJob &J, const void *records, const int32_t *ids, int n, cudaStream_t st);
+
+// the positioned endpointer (mww_endpoint_at.cu, bodies in mww_endpoint.h and mww_serving_records.h; companion library
+// libmww_endpoint_at.so): the forms above that also keep each row's mute word mute [n_rows], one launch each, and arm_at, two
+// launches (the reduction of each row's latest position, then the arm) of the n listed global ids and positions (device memory)
+cudaError_t launch_endpoint_update_muted(const EndpointArgs &a, int32_t *mute, const float *probs, long long pitch, int n, long long pos0,
+                                         cudaStream_t st);
+cudaError_t launch_endpoint_arm_muted(const EndpointArgs &a, const EndpointReplay &R, int32_t *mute, const int32_t *ids, int n, cudaStream_t st);
+cudaError_t launch_endpoint_clear_muted(const EndpointArgs &a, int32_t *mute, const int32_t *ids, int n, int reset, cudaStream_t st);
+cudaError_t launch_endpoint_arm_at(const EndpointArgs &a, const EndpointAt &A, const int32_t *ids, const long long *positions, int n,
+                                   cudaStream_t st);
+cudaError_t launch_pack_endpointer_rows_muted(const EpRecJob &J, const int32_t *mute, void *records, const int32_t *ids, int n, cudaStream_t st);
+cudaError_t launch_unpack_endpointer_rows_muted(const EpRecJob &J, int32_t *mute, const void *records, const int32_t *ids, int n,
+                                                cudaStream_t st);
 }  // namespace mww
 
 #include "mww_event_positions.h"

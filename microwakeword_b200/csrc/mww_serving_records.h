@@ -2,7 +2,8 @@
 // include/mww.h, "moving endpointer rows") and the per-row bodies of the two kernels that fill and read it
 // (mww_serving_records.cu).  One record holds one stream's row:
 //
-//     int32  member, armed, 0, 0                                    member of the stream set; armed (segmenter state follows)
+//     int32  member, armed, mute, 0                                 member of the stream set; armed (segmenter state follows);
+//                                                                   the mute word of a positioned exporter, else 0
 //     int32  elapsed, run, silence, heard                           zero unless armed
 //     int64  seen; uint64 flags                                     the VAD count and the last 64 speech flags
 //     int64  start_age, speech_end_age                              S' - start_sample, S' - speech_end_sample; zero unless armed
@@ -67,12 +68,15 @@ MWW_HD uint32_t endpoint_hi(long long v) { return (uint32_t)((unsigned long long
 MWW_HD long long endpoint_join(uint32_t lo, uint32_t hi) { return (long long)(((unsigned long long)hi << 32) | lo); }
 
 // endpointer -> the record of global id `id` (in range).  A non-member gets a zero record; an unarmed row zero segmenter
-// state.  Reads only.
-MWW_HD void endpoint_record_pack(const EpRecJob &J, int id, uint32_t *rec) {
+// state.  kAt: an armed row's mute word goes into the head's third word.  Reads only.
+template <bool kAt>
+MWW_HD void endpoint_record_pack_t(const EpRecJob &J, const int32_t *mute, int id, uint32_t *rec) {
     const EndpointArgs &a = J.a;
     const int r = endpoint_row(a, id);
     const bool member = r >= 0, armed = member && a.armed[r] >= 0;
-    endpoint_record_put(rec + J.L.head / 4, EpRecPart{{member ? 1u : 0u, armed ? 1u : 0u, 0u, 0u}});
+    uint32_t m = 0u;
+    if constexpr (kAt) m = armed ? (uint32_t)mute[r] : 0u;
+    endpoint_record_put(rec + J.L.head / 4, EpRecPart{{member ? 1u : 0u, armed ? 1u : 0u, m, 0u}});
     EpRecPart seg{{0u, 0u, 0u, 0u}}, ages{{0u, 0u, 0u, 0u}}, vad{{0u, 0u, 0u, 0u}};
     if (armed) {
         seg = EpRecPart{{(uint32_t)a.elapsed[r], (uint32_t)a.run[r], (uint32_t)a.silence[r], (uint32_t)a.heard[r]}};
@@ -98,17 +102,20 @@ MWW_HD void endpoint_record_pack(const EpRecJob &J, int id, uint32_t *rec) {
         endpoint_record_put(rec + J.L.hist / 4 + 4 * c, p);
     }
 }
+MWW_HD void endpoint_record_pack(const EpRecJob &J, int id, uint32_t *rec) { endpoint_record_pack_t<false>(J, nullptr, id, rec); }
 
 // record -> endpointer, global id `id` (in range).  A non-member ignores the record; a member whose record has member = 0
 // gets what reset(ids) gives; a member whose record has member = 1 takes the VAD state, and, when the record is armed, the
-// segmenter with armed = id and positions S' - age.  arm_tag is not written.
-MWW_HD void endpoint_record_unpack(const EpRecJob &J, int id, const uint32_t *rec) {
+// segmenter with armed = id and positions S' - age.  arm_tag is not written.  kAt: the row's mute word is the head's third
+// word when the record is armed (0 in a plain exporter's records) and 0 otherwise.
+template <bool kAt>
+MWW_HD void endpoint_record_unpack_t(const EpRecJob &J, int32_t *mute, int id, const uint32_t *rec) {
     const EndpointArgs &a = J.a;
     const int r = endpoint_row(a, id);
     if (r < 0) return;
     const EpRecPart head = endpoint_record_get(rec + J.L.head / 4);
     if (!head.w[0]) {
-        endpoint_clear_row(a, r, 1);
+        endpoint_clear_row_t<kAt>(a, mute, r, 1);
         return;
     }
     const EpRecPart vad = endpoint_record_get(rec + J.L.vad / 4);
@@ -125,6 +132,7 @@ MWW_HD void endpoint_record_unpack(const EpRecJob &J, int id, const uint32_t *re
     if (!head.w[1]) {
         a.armed[r] = -1;
         endpoint_store_seg(a, r, endpoint_fresh_seg());
+        if constexpr (kAt) mute[r] = 0;
         return;
     }
     const EpRecPart seg = endpoint_record_get(rec + J.L.seg / 4);
@@ -132,7 +140,9 @@ MWW_HD void endpoint_record_unpack(const EpRecJob &J, int id, const uint32_t *re
     a.armed[r] = id;
     endpoint_store_seg(a, r, EndpointSeg{(int)seg.w[0], (int)seg.w[1], (int)seg.w[2], (int)seg.w[3],
                                          J.base - endpoint_join(ages.w[0], ages.w[1]), J.base - endpoint_join(ages.w[2], ages.w[3])});
+    if constexpr (kAt) mute[r] = (int32_t)head.w[2];
 }
+MWW_HD void endpoint_record_unpack(const EpRecJob &J, int id, const uint32_t *rec) { endpoint_record_unpack_t<false>(J, nullptr, id, rec); }
 
 // The first field in which the layout the records were exported with differs from the importing endpointer's own, nullptr
 // when the records fit.  The baselines (samples_seen, steps) are for information and not compared.

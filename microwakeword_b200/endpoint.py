@@ -8,6 +8,7 @@ until the clips are wanted:
     det.update(probs); ep.update(probs[vad])
     scores, confirmed = ver.verify(eng, det)
     ep.arm(confirmed)                                    # replays the last lookback_steps, so the command's start is kept
+    ep.arm(passed, at=det)                               # or: start at each detection's position, after the wake word
     ...
     clips, lengths = ep.commands(pre=1600, post=3200, max_samples=16000 * 10)     # before the drain and the reset
     eng.reset(ep.ended_ids); det.reset(ep.ended_ids)
@@ -28,6 +29,9 @@ from . import _lib
 from .detection import _DeviceArray, _DetectorHandle, _record_ids
 from .engine import MAX_AUDIO_HISTORY
 
+MAX_SKIP = 1 << 22
+MUTE_PLACED = 1 << 30              # the mute word's bit of a row armed at a position that has taken no step since
+
 END_OF_SPEECH, NO_SPEECH, MAX_LENGTH = _lib.MWW_ENDPOINT_END_OF_SPEECH, _lib.MWW_ENDPOINT_NO_SPEECH, _lib.MWW_ENDPOINT_MAX_LENGTH
 ENDPOINT_EVENT_DTYPE = np.dtype([("stream", np.int32), ("reason", np.int32), ("start_sample", np.int64), ("end_sample", np.int64),
                                  ("speech_end_sample", np.int64), ("steps", np.int32), ("pad", np.int32)])
@@ -43,7 +47,8 @@ class EndpointerRecords:
     """Endpointer rows exported from an Endpointer (export_streams): `data`, torch.uint8 [n, record_bytes] on the
     endpointer's device, one packed record per listed stream (include/mww.h, "moving endpointer rows"), and `layout`, the
     _lib.MwwEndpointerLayout an importing endpointer must share.  Positions travel as ages from the exporter's baseline, so
-    they land on the importer's axis.  The records carry no events."""
+    they land on the importer's axis.  The records carry no events.  layout.pad is 1 when the exporter was positioned
+    (its records carry each armed row's mute word) and 0 otherwise."""
 
     _FIELDS = ("record_bytes", "vad_window", "stride", "hop_samples", "buffered", "pending", "pad", "samples_seen", "steps")
 
@@ -89,7 +94,8 @@ class Endpointer:
     latency changes nothing.  The replay reaches back over the wake word itself, which the VAD hears as speech: the segment
     (and the clip) starts before the wake word, and if the speaker pauses longer than `silence_steps` after it, the command
     ends with END_OF_SPEECH before it is spoken.  Set lookback_steps to the latency to cover, not more, and silence_steps
-    above the pause speakers make after the wake word.  A whole reset() forgets the steps before it: no replay crosses it.
+    above the pause speakers make after the wake word -- or arm at the detection's position, arm(ids, at=det), which starts
+    the command after the wake word.  A whole reset() forgets the steps before it: no replay crosses it.
     `capacity` events are kept between drains; more are counted and dropped."""
 
     def __init__(self, engine, model=None, vad_window: int = 5, vad_cutoff: float = 0.5, speech_steps: int = 3, silence_steps: int = 25,
@@ -199,11 +205,77 @@ class Endpointer:
                 raise ValueError("stream ids must be in [0, %d)" % self.engine.n_streams)
             self._check(getattr(self._L, host_fn)(self._ep, a.ctypes.data, a.size, self._stream()))
 
-    def arm(self, ids) -> None:
+    def arm(self, ids, at=None, skip=None) -> None:
         """Start a command on the listed GLOBAL stream ids: a host sequence, or a contiguous 1-D CUDA int32 tensor such as a
         verifier's confirmed ids or a detector's fired_ids, whose -1 slots (and ids outside the model's stream set) are
-        ignored.  Re-arming restarts a row; the last lookback_steps flags are replayed."""
-        self._ids_call(ids, "mww_endpointer_arm", "mww_endpointer_arm_device")
+        ignored.  Re-arming restarts a row; the last lookback_steps flags are replayed.
+
+        at: each id's position on the audio history's axis (include/mww.h, "positioned arm"): the command starts there, not
+        lookback_steps before the arm, so it leaves the wake word out.  It is one of
+          - a timed StreamDetector or MultiModelDetector of this engine and device: its event_samples, slot for slot with
+            ids, which must then be a CUDA int32 tensor of its capacity (passed, confirmed or fired_ids);
+          - a CUDA int64 tensor beside CUDA ids;
+          - a host sequence beside host ids.
+        The steps within `skip` samples after a position take no speech (default vad_window * stride * hop, which covers the
+        VAD average's lag behind the end of the wake word; a guess, not measured on real speech), so the wake word's tail
+        does not count as the command.  A stream listed twice arms at its latest position.  The first positioned arm makes
+        the endpointer positioned for good: every later call runs the positioned kernels, which give the same results while
+        no row is muted."""
+        if at is None:
+            if skip is not None:
+                raise ValueError("skip applies to a positioned arm (at=...)")
+            self._ids_call(ids, "mww_endpointer_arm", "mww_endpointer_arm_device")
+            return
+        skip = self.vad_window * self.stride * self.hop if skip is None else _int(skip, "skip")
+        if not 0 <= skip <= MAX_SKIP:
+            raise ValueError("skip must be in [0, %d] samples (got %d)" % (MAX_SKIP, skip))
+        import torch
+        ids_dev = isinstance(ids, torch.Tensor) and ids.is_cuda
+        if hasattr(at, "event_samples") and hasattr(at, "fired_ids"):
+            if not at.timed:
+                raise ValueError("at= needs a timed detector (timed=True): an untimed one has no positions")
+            if int(at.device) != self.device:
+                raise ValueError("the detector is on cuda:%d, the endpointer on cuda:%d" % (at.device, self.device))
+            bound = [e for e in (getattr(at, "engine", None), getattr(at, "_arb_engine", None)) if e is not None]
+            if any(e is not self.engine for e in bound):
+                raise ValueError("the detector serves another engine than this endpointer's")
+            if not ids_dev or ids.numel() != at.capacity:
+                raise ValueError("with a detector, ids must be a CUDA int32 tensor of its %d slots (passed, confirmed or fired_ids)"
+                                 % at.capacity)
+            at = at.event_samples
+        if isinstance(at, torch.Tensor) and at.is_cuda:
+            if not ids_dev:
+                raise ValueError("ids and positions must both be host sequences or both CUDA tensors")
+            if (ids.dtype != torch.int32 or ids.dim() != 1 or not ids.is_contiguous() or ids.device.index != self.device
+                    or at.dtype != torch.int64 or at.dim() != 1 or not at.is_contiguous() or at.device.index != self.device):
+                raise ValueError("device ids and positions must be contiguous 1-D CUDA int32 and int64 tensors on cuda:%d" % self.device)
+            if at.numel() != ids.numel():
+                raise ValueError("ids and positions differ in length (%d, %d)" % (ids.numel(), at.numel()))
+            self._check(self._L.mww_endpointer_arm_at_device(self._ep, ids.data_ptr(), at.data_ptr(), ids.numel(), skip, self._stream()))
+            return
+        if ids_dev or isinstance(at, torch.Tensor):
+            raise ValueError("ids and positions must both be host sequences or both CUDA tensors")
+        a = _record_ids(ids, "stream ids")
+        if a.size and (a.min() < 0 or a.max() >= self.engine.n_streams):
+            raise ValueError("stream ids must be in [0, %d)" % self.engine.n_streams)
+        p = np.asarray(at)
+        if p.ndim != 1 or (p.size and p.dtype.kind not in "iu") or p.size != a.size:
+            raise ValueError("positions must be a 1-D integer sequence beside the ids")
+        p = np.ascontiguousarray(p, np.int64)
+        self._check(self._L.mww_endpointer_arm_at(self._ep, a.ctypes.data, p.ctypes.data, a.size, skip, self._stream()))
+
+    @property
+    def positioned(self) -> bool:
+        """whether the endpointer runs the positioned kernels: after its first arm(at=...), a loaded mute or an import of
+        positioned records"""
+        return bool(self.layout().pad)
+
+    def mutes(self) -> np.ndarray:
+        """every row's mute word (include/mww.h, "positioned arm"): bits 0 .. 29 the steps still muted, bit 30 set while a
+        row armed at a position with nothing replayed has taken no step.  Synchronous."""
+        out = np.zeros(self.n_rows, np.int32)
+        self._check(self._L.mww_endpointer_get_mutes(self._ep, out.ctypes.data if self.n_rows else None))
+        return out
 
     def disarm(self, ids) -> None:
         """Cancel the listed streams' commands without an event (host ids)"""
@@ -307,7 +379,7 @@ class Endpointer:
 
     def state_dict(self) -> dict:
         """every row's state (hist [n_rows, vad_window - 1] oldest first, seen, flags, armed, elapsed, run, silence, heard,
-        start_sample, speech_end_sample) and the baseline (samples_seen, buffered, pending), steps and positions [64].
+        start_sample, speech_end_sample, mute) and the baseline (samples_seen, buffered, pending), steps and positions [64].
         Synchronous."""
         d = {"hist": np.zeros((self.n_rows, self.vad_window - 1), np.float32)}
         d.update({k: np.zeros(self.n_rows, t) for k, t in self._ROW_FIELDS})
@@ -319,11 +391,16 @@ class Endpointer:
         for k in ("samples_seen", "buffered", "pending", "steps"):
             d[k] = int(getattr(st, k))
         d["positions"] = np.ctypeslib.as_array(st.positions).copy()
+        d["mute"] = self.mutes()
         return d
 
     def load_state_dict(self, d: dict) -> None:
-        """the inverse of state_dict (synchronous); refusals as mww_endpointer_set_state"""
+        """the inverse of state_dict (synchronous); refusals as mww_endpointer_set_state.  A dict without `mute` loads zero
+        mutes.  Nonzero mutes make the endpointer positioned; zero mutes leave a plain endpointer plain."""
         hist = np.ascontiguousarray(d["hist"], np.float32)
+        mute = np.ascontiguousarray(d.get("mute", np.zeros(self.n_rows, np.int32)), np.int32)
+        if mute.shape != (self.n_rows,) or (mute < 0).any() or ((mute & (MUTE_PLACED - 1)) > MAX_SKIP).any():
+            raise ValueError("mute must hold one word per row: a count in [0, 2^22], and bit 30")
         rows = {k: np.ascontiguousarray(d[k], t) for k, t in self._ROW_FIELDS}
         if hist.shape != (self.n_rows, self.vad_window - 1) or any(a.shape != (self.n_rows,) for a in rows.values()):
             raise ValueError("state arrays must have the endpointer's shapes")
@@ -338,3 +415,5 @@ class Endpointer:
             setattr(st, k, int(d[k]))
         np.ctypeslib.as_array(st.positions)[:] = pos
         self._check(self._L.mww_endpointer_set_state(self._ep, ctypes.byref(st)))
+        if mute.any() or self.positioned:
+            self._check(self._L.mww_endpointer_set_mutes(self._ep, mute.ctypes.data if mute.size else None))
